@@ -83,7 +83,8 @@ enum vb_agg {
     VB_AGG_MAX = 3,
     VB_AGG_COUNT = 4,
     VB_AGG_COGROUP = 5,
-    VB_AGG_SORT = 6
+    VB_AGG_SORT = 6,
+    VB_AGG_MEAN = 7     /* vb_agg_col only */
 };
 
 /* VB_PART_HASH_METRO64: MetroHash64_1(key LE bytes, seed 0) % n_reduce (src/partitioner.rs:21-25,
@@ -235,6 +236,38 @@ VB_API int32_t vb_shuffle_is_sealed(vb_shuf *s);
 VB_API int32_t vb_shuffle_reduce_size(vb_shuf *s, uint32_t reduce_id, uint64_t *n_keys, uint64_t *n_vals);
 VB_API int32_t vb_shuffle_reduce(vb_shuf *s, uint32_t reduce_id, void *out_keys, void *out_combined,
                                  uint64_t *out_offsets, void *out_vals, int32_t dst_loc);
+
+/* ---- combine_by_key: several named aggregates per key in one shuffle (PairRdd::combine_by_key,
+ *      src/rdd/pair_rdd.rs:20-33, with a combiner of up to VB_MAX_AGGS named fields) --------------------------
+ * Rows are a key column plus n_val_cols value columns (SoA only) of dtypes val_dtypes[].  Aggregate a is op
+ * aggs[a].agg folded over input column aggs[a].src, independently for every key:
+ *   SUM / MIN / MAX follow the vb_agg rules of that column's dtype (wrapping integer sums, unsigned / signed
+ *         compares, f64 MIN/MAX as f64::min / f64::max with NaN ignored); output dtype = the column's dtype.
+ *   COUNT rows of the key (src ignored); output u64.
+ *   MEAN  f64: for u64 / i64 columns (double)S / (double)n, S = the 64-bit wrapping sum read with the column's
+ *         signedness, so it is exact only while the key's sum does not wrap; for f64 columns the f64 SUM / n.
+ * A MEAN keeps a SUM accumulator and shares one COUNT accumulator (the spec's own COUNT if it has one, else an
+ * internal one); that internal COUNT counts against VB_MAX_AGGS.  Keys are placed by MetroHash64_1(k) % n_reduce,
+ * the same partition as any single-column shuffle of the same keys; vb_shuffle_set_key_width / set_hint apply.
+ * VB_ERR_INVALID: more than VB_MAX_VAL_COLS columns or VB_MAX_AGGS aggregates, src out of range, or a GROUP /
+ * COGROUP / SORT op.  Not supported (VB_ERR_UNSUPPORTED): world > 1 (vb_shuffle_set_dist, export / import /
+ * exchange), the bincode blob calls, AoS rows (vb_shuffle_map_aos).  vb_shuffle_map_soa returns VB_ERR_INVALID;
+ * vb_shuffle_reduce returns the keys only (VB_ERR_INVALID with out_combined != NULL); the join calls return
+ * VB_ERR_INVALID; vb_shuffle_reduce_size / seal / stats / kernel_time / free work as for any reduce shuffle.   */
+#define VB_MAX_VAL_COLS 4
+#define VB_MAX_AGGS 8
+typedef struct vb_agg_col {
+    int32_t agg; /* VB_AGG_SUM / MIN / MAX / COUNT / MEAN */
+    int32_t src; /* input value column (ignored by COUNT) */
+} vb_agg_col;
+VB_API int32_t vb_shuffle_create_multi(vb_ctx *ctx, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce, int32_t key_dtype,
+                                       uint32_t n_val_cols, const int32_t *val_dtypes, uint32_t n_aggs, const vb_agg_col *aggs,
+                                       vb_shuf **out);
+/* one map partition: keys[n_rows] and vals[c][n_rows] for c < n_val_cols (a column no aggregate reads may be NULL) */
+VB_API int32_t vb_shuffle_map_cols(vb_shuf *s, uint32_t map_id, const void *keys, const void *const *vals, uint64_t n_rows,
+                                   int32_t src_loc);
+/* one reduce partition: out_keys[n_keys] and out_aggs[a][n_keys] per aggregate (NULL entries are skipped) */
+VB_API int32_t vb_shuffle_reduce_cols(vb_shuf *s, uint32_t reduce_id, void *out_keys, void *const *out_aggs, int32_t dst_loc);
 
 /* Inner join of two sealed GROUP/COGROUP shuffles with equal n_reduce, for one partition:
  * per key `for v in left { for w in right }` (src/rdd/pair_rdd.rs:109-115).                  */

@@ -156,6 +156,47 @@ public:
         return out;
     }
 
+    // combine_by_key with named aggregates of the value column (VB_AGG_SUM / MIN / MAX / COUNT / MEAN), one shuffle:
+    // per key one result per aggregate, as 64-bit patterns (COUNT: uint64_t, MEAN: double, others: V; read them with
+    // detail::from_bits<T>)
+    std::vector<std::pair<K, std::vector<uint64_t>>> combine_by_key(const std::vector<int32_t> &aggs, size_t num_splits) const
+    {
+        if (num_slices_ < 1) throw Error(VB_ERR_INVALID, "Number of slices should be greater than or equal to 1");
+        const uint64_t n = keys_.size();
+        std::vector<uint64_t> starts(std::min<uint64_t>(n, num_slices_) + 2);
+        const uint64_t n_map = vb_slice(n, num_slices_, starts.data());
+        std::vector<vb_agg_col> spec;
+        for (int32_t a : aggs) spec.push_back(vb_agg_col{a, 0});
+        const int32_t vcode = detail::dtype<V>::code;
+        vb_shuf *raw = nullptr;
+        check(vb_shuffle_create_multi(sc_->raw(), sc_->new_shuffle_id(), (uint32_t)n_map, (uint32_t)num_splits, detail::dtype<K>::code, 1,
+                                      &vcode, (uint32_t)spec.size(), spec.data(), &raw));
+        detail::ShufPtr s(raw);
+        if (detail::dtype<K>::width == 4) check(vb_shuffle_set_key_width(raw, 4));
+        for (uint64_t m = 0; m < n_map; ++m) {
+            const uint64_t lo = starts[m], cnt = starts[m + 1] - lo;
+            const void *col = cnt ? vals_.data() + lo : nullptr;
+            check(vb_shuffle_map_cols(raw, (uint32_t)m, cnt ? keys_.data() + lo : nullptr, &col, cnt, VB_HOST));
+        }
+        check(vb_shuffle_seal(raw));
+        std::vector<std::pair<K, std::vector<uint64_t>>> out;
+        for (uint32_t r = 0; r < num_splits; ++r) {
+            uint64_t nk = 0, nv = 0;
+            check(vb_shuffle_reduce_size(raw, r, &nk, &nv));
+            std::vector<uint64_t> k(nk);
+            std::vector<std::vector<uint64_t>> cols(aggs.size(), std::vector<uint64_t>(nk));
+            std::vector<void *> ptrs;
+            for (auto &c : cols) ptrs.push_back(c.data());
+            check(vb_shuffle_reduce_cols(raw, r, k.data(), ptrs.data(), VB_HOST));
+            for (uint64_t i = 0; i < nk; ++i) {
+                std::vector<uint64_t> row;
+                for (auto &c : cols) row.push_back(c[i]);
+                out.emplace_back(detail::from_bits<K>(k[i]), std::move(row));
+            }
+        }
+        return out;
+    }
+
     // self.join(other, num_splits).collect()  →  Vec<(K, (V, W))>, inner join
     template <typename W>
     std::vector<std::pair<K, std::pair<V, W>>> join(const PairRddT<K, W> &other, size_t num_splits) const

@@ -8,11 +8,14 @@ use std::os::raw::{c_char, c_void};
 
 #[repr(C)] pub struct vb_ctx { _p: [u8; 0] }
 #[repr(C)] pub struct vb_shuf { _p: [u8; 0] }
+/// include/vega_b200.h `vb_agg_col`: aggregate `agg` (VB_AGG_SUM / MIN / MAX / COUNT / MEAN) over value column `src`
+#[repr(C)] pub struct vb_agg_col { pub agg: i32, pub src: i32 }
 
 pub const VB_OK: i32 = 0;
 pub const VB_U64: i32 = 0; pub const VB_I64: i32 = 1; pub const VB_F64: i32 = 2;
 pub const VB_AGG_GROUP: i32 = 0; pub const VB_AGG_SUM: i32 = 1; pub const VB_AGG_MIN: i32 = 2;
 pub const VB_AGG_MAX: i32 = 3; pub const VB_AGG_COUNT: i32 = 4; pub const VB_AGG_COGROUP: i32 = 5;
+pub const VB_AGG_MEAN: i32 = 7;   // vb_agg_col only
 pub const VB_PART_HASH_METRO64: i32 = 0;
 pub const VB_HOST: i32 = 0;
 
@@ -57,6 +60,11 @@ extern "C" {
     // device-resident source (Context::range)
     pub fn vb_range_len(start: u64, end: u64, step: u64) -> u64;
     pub fn vb_range(ctx: *mut vb_ctx, out_dev: *mut c_void, start: u64, end: u64, step: u64) -> i32;
+    // combine_by_key: several named aggregates per key in one shuffle (SoA columns)
+    pub fn vb_shuffle_create_multi(ctx: *mut vb_ctx, shuffle_id: u64, n_map: u32, n_reduce: u32, key_dtype: i32, n_val_cols: u32,
+                                   val_dtypes: *const i32, n_aggs: u32, aggs: *const vb_agg_col, out: *mut *mut vb_shuf) -> i32;
+    pub fn vb_shuffle_map_cols(s: *mut vb_shuf, map_id: u32, keys: *const c_void, vals: *const *const c_void, n_rows: u64, src_loc: i32) -> i32;
+    pub fn vb_shuffle_reduce_cols(s: *mut vb_shuf, reduce_id: u32, out_keys: *mut c_void, out_aggs: *const *mut c_void, dst_loc: i32) -> i32;
     pub fn vb_shuffle_free(s: *mut vb_shuf) -> i32;
     pub fn vb_last_error() -> *const c_char;
     pub fn vb_get_partition(key: u64, key_width: u32, n_reduce: u32) -> u32;

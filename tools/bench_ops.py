@@ -17,7 +17,7 @@ from vega_b200 import _lib as L
 ap = argparse.ArgumentParser()
 ap.add_argument("--rows", type=float, default=1e9)
 ap.add_argument("--distinct", type=float, default=1e6)
-ap.add_argument("--ops", default="reduce,group,sort,sortkv,join,count")
+ap.add_argument("--ops", default="reduce,group,sort,sortkv,join,count")   # also: zipf, zipfgroup, combine, combinezipf
 ap.add_argument("--reps", type=int, default=3)
 args = ap.parse_args()
 N, D = int(args.rows), int(args.distinct)
@@ -132,4 +132,68 @@ if "join" in ops:
     res = timed(join, max(1, args.reps - 1))
     assert res[-1][1]["join_rows"] == shared, (res[-1][1]["join_rows"], shared)
     report("join", 2 * n_side, 32.0 * n_side + 24.0 * shared, res, {"join_rows": shared})
+if "combine" in ops or "combinezipf" in ops:
+    # combine_by_key: sum(v0), min(v1), max(v1), mean(v2), count in one shuffle (5 accumulators) against the baseline a
+    # user has without it, one single-column shuffle per aggregate (the mean from a sum and the count).  v0 is gen_pairs'
+    # value column (< 2^20), v1 = 7 v0 - 3e6 (i64), v2 = v0 / 2 (f64), all on the device.
+    from bench import gpu_info
+    card = gpu_info(0)
+    for zipf in ([False] if "combinezipf" not in ops else [False, True] if "combine" in ops else [True]):
+        keys = torch.empty(N, dtype=torch.int64, device="cuda")
+        v0 = torch.empty(N, dtype=torch.int64, device="cuda")
+        sc.gen_pairs(out_keys=keys, out_vals=v0, first=0, n=N, mode="zipf" if zipf else "uniform", n_distinct=D,
+                     seed_k=5 if zipf else 1, zipf_s=1.1 if zipf else 0.0)
+        v1 = v0 * 7 - 3_000_000
+        v2 = v0.to(torch.float64) * 0.5
+        torch.cuda.synchronize()
+        K = vb.rdd._Col(keys)
+        K.code = L.VB_U64
+        cols = (vb.rdd._Col(v0), vb.rdd._Col(v1), vb.rdd._Col(v2))
+        cols[0].code = L.VB_U64
+        spec = [(L.VB_AGG_SUM, 0), (L.VB_AGG_MIN, 1), (L.VB_AGG_MAX, 1), (L.VB_AGG_MEAN, 2), (L.VB_AGG_COUNT, 0)]
+        M, R = 8, 8
+        starts = vb.slice_starts(N, M)
+
+        def fused():
+            sh = vb.Shuffle(sc, M, R, L.VB_U64, L.VB_U64, L.VB_AGG_SUM, hint=0 if zipf else D, multi=([c.code for c in cols], spec))
+            for m in range(M):
+                sh.map_cols(m, K, cols, int(starts[m]), int(starts[m + 1]))
+            sh.seal()
+            st = sh.stats()
+            sh.free()
+            return st
+
+        singles = [(L.VB_AGG_SUM, cols[0]), (L.VB_AGG_MIN, cols[1]), (L.VB_AGG_MAX, cols[1]), (L.VB_AGG_SUM, cols[2]),
+                   (L.VB_AGG_COUNT, None)]
+
+        def per_aggregate():
+            tot = None
+            for agg, col in singles:
+                sh = vb.Shuffle(sc, M, R, L.VB_U64, col.code if col is not None else L.VB_U64, agg, hint=0 if zipf else D)
+                for m in range(M):
+                    sh.map(m, K, col, int(starts[m]), int(starts[m + 1]))
+                sh.seal()
+                st = sh.stats()
+                sh.free()
+                if tot is None:
+                    tot = st
+                else:
+                    for kk in st["kernels"]:
+                        tot["kernels"][kk]["ms"] += st["kernels"][kk]["ms"]
+                        tot["kernels"][kk]["launches"] += st["kernels"][kk]["launches"]
+                    for kk in ("kernel_launches", "table_restarts"):
+                        tot[kk] += st[kk]
+                    tot["table_slots"] = max(tot["table_slots"], st["table_slots"])
+            return tot
+
+        tag = " zipf(1.1)" if zipf else ""
+        alg = 8.0 * (1 + 3) * N + 8.0 * (1 + 5) * D
+        rf = timed(fused, args.reps)
+        rb = timed(per_aggregate, args.reps)
+        med = lambda r: sorted(x[0] for x in r)[len(r) // 2]
+        extra = {"gpu": card["name"], "power_limit_w": card["power_limit_w"], "aggregates": 5, "accumulators": 5}
+        report("combine_by_key 5 aggs" + tag, N, alg, rf, dict(extra, per_aggregate_ms=round(med(rb), 3)))
+        report("5 x reduce_by_key" + tag, N, alg, rb, dict(extra, fused_ms=round(med(rf), 3)))
+        del keys, v0, v1, v2, K, cols
+        torch.cuda.empty_cache()
 sc.close()

@@ -12,7 +12,8 @@ LIB_PATH = os.environ.get("VEGA_B200_LIB") or os.path.join(_PKG, "libvega_b200.s
 
 VB_OK, VB_ERR_INVALID, VB_ERR_CUDA, VB_ERR_OOM, VB_ERR_STATE, VB_ERR_UNSUPPORTED, VB_ERR_TOO_LARGE = 0, -1, -2, -3, -4, -5, -6
 VB_U64, VB_I64, VB_F64 = 0, 1, 2
-VB_AGG_GROUP, VB_AGG_SUM, VB_AGG_MIN, VB_AGG_MAX, VB_AGG_COUNT, VB_AGG_COGROUP, VB_AGG_SORT = range(7)
+VB_AGG_GROUP, VB_AGG_SUM, VB_AGG_MIN, VB_AGG_MAX, VB_AGG_COUNT, VB_AGG_COGROUP, VB_AGG_SORT, VB_AGG_MEAN = range(8)
+VB_MAX_VAL_COLS, VB_MAX_AGGS = 4, 8
 VB_PART_HASH_METRO64, VB_PART_RANGE = 0, 1
 VB_HOST, VB_DEVICE, VB_DEVICE_BORROWED = 0, 1, 2
 VB_GEN_UNIFORM, VB_GEN_ZIPF, VB_GEN_UNIQUE = 0, 1, 2
@@ -42,6 +43,10 @@ class vb_xstats(ctypes.Structure):
     _fields_ = [("sent_rows", ctypes.c_uint64), ("recv_rows", ctypes.c_uint64), ("exchanges", ctypes.c_uint64),
                 ("exchange_ms", ctypes.c_double), ("kind", ctypes.c_int32), ("pad", ctypes.c_int32),
                 ("prepare_wall_ms", ctypes.c_double), ("counts_wall_ms", ctypes.c_double), ("post_wall_ms", ctypes.c_double)]
+
+
+class vb_agg_col(ctypes.Structure):
+    _fields_ = [("agg", ctypes.c_int32), ("src", ctypes.c_int32)]
 
 
 # name -> (restype, argtypes); also the list of symbols include/vega_b200.h declares
@@ -81,6 +86,9 @@ SYMBOLS = {
     "vb_shuffle_is_sealed": (_i32, [_vp]),
     "vb_shuffle_reduce_size": (_i32, [_vp, _u32, _pu64, _pu64]),
     "vb_shuffle_reduce": (_i32, [_vp, _u32, _vp, _vp, _vp, _vp, _i32]),
+    "vb_shuffle_create_multi": (_i32, [_vp, _u64, _u32, _u32, _i32, _u32, _vp, _u32, ctypes.POINTER(vb_agg_col), _pvp]),
+    "vb_shuffle_map_cols": (_i32, [_vp, _u32, _vp, _pvp, _u64, _i32]),
+    "vb_shuffle_reduce_cols": (_i32, [_vp, _u32, _vp, _pvp, _i32]),
     "vb_join_size": (_i32, [_vp, _vp, _u32, _pu64]),
     "vb_join": (_i32, [_vp, _vp, _u32, _vp, _vp, _vp, _i32]),
     "vb_shuffle_reduce_blob_size": (_i32, [_vp, _u32, _pu64]),

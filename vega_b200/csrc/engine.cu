@@ -262,6 +262,7 @@ struct MapOut {
     const u64 *rows = nullptr;
     const u64 *keys = nullptr;
     const u64 *vals = nullptr;
+    const u64 *cols[MA_MAX_COLS] = {};   // multi-aggregate shuffles: borrowed value columns (shared-table rebuilds)
     bool owned = false;
     bool in_shared = false;   // reduce ops, borrowed device input: combined straight into the shuffle's shared table
 };
@@ -284,6 +285,13 @@ struct vb_shuf {
     u64 id = 0;
     u32 n_map = 0, n_reduce = 0;
     int kdt = 0, vdt = 0, agg = 0, part = 0;
+    // multi-aggregate shuffle (vb_shuffle_create_multi): agg is VB_AGG_SUM for the reduce-op plumbing, the
+    // accumulators are described by the specs below and the results live in res_cols
+    bool multi = false;
+    u32 n_cols = 0;
+    AccSpec acc_map{}, acc_merge{};   // map-side combine / table merge (COUNT merges as ADD, no order transform)
+    OutSpec outs{};                   // one output column per vb_agg_col
+    u64 *res_cols = nullptr;          // [outs.n][n_keys], partition-major like res_keys
     u32 key_width = 8;
     u64 hint = 0;
     u64 learned_distinct = 0;      // distinct keys seen by the previous table build of this shuffle
@@ -441,6 +449,7 @@ struct AggInput {
     u64 n;           // rows (IN_TABLE: slots incl. the special one)
     int loc;         // VB_HOST or device
     u64 items = 0;   // IN_TABLE: upper bound on the occupied slots (n_inserted + 1); 0 = n
+    const u64 *cols[MA_MAX_COLS] = {};   // multi-aggregate IN_SOA: value columns (b unused); IN_TABLE: b = first accumulator column
 };
 
 template <int IN, int OPK, int TX>
@@ -508,6 +517,71 @@ static int launch_hash_agg(vb_shuf *s, int klass, int in, int opk, int tx, const
     case IN_TABLE: return launch_hash_agg_in<IN_TABLE>(s, klass, opk, tx, a, b, n, tab, log_cap, ctl, mi, so);
     }
     return set_err(VB_ERR_INVALID, "hash_agg: bad input mode %d", in);
+}
+
+// Multi-aggregate combine: keys + NV value columns (IN_SOA), or a source table of the same spec (IN_TABLE).
+template <int IN, int NV>
+static int launch_hash_agg_multi_t(vb_shuf *s, int klass, const AccSpec &sp, const u64 *keys, const MaCols &cols, u64 n, void *tab,
+                                   u32 log_cap, TableCtl *ctl, u64 max_inserts)
+{
+    vb_ctx *c = s->ctx;
+    const Table t = table_at(tab, log_cap);
+    if constexpr (IN == IN_SOA) {
+        static const bool no_bulk = getenv("VEGA_B200_NO_BULK") != nullptr;
+        uintptr_t addr = (uintptr_t)keys;
+        for (int i = 0; i < NV; ++i) addr |= (uintptr_t)cols.c[i];
+        constexpr u64 tile = (u64)HA_THREADS * ma_rows<NV>();
+        if (!no_bulk && (addr & 15u) == 0 && n >= tile * 64) {
+            auto kb = hash_agg_multi_bulk_kernel<NV>;
+            const size_t smem = ma_bulk_smem<NV>(MA_MAX_ACCS);     // sized for the widest spec: one occupancy for every spec
+            if (c->occ_cache.find((const void *)kb) == c->occ_cache.end())
+                CU(cudaFuncSetAttribute(kb, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            const int occ = occupancy(c, kb, HB_THREADS, smem);
+            const u64 grid = std::min<u64>(n / tile, (u64)c->sm_count * occ);
+            KLaunch kl(s, klass, n);
+            if (klass == K_HASH_AGG) s->st.hot_kernel_variant = 1;
+            kb<<<(unsigned)grid, HB_THREADS, smem, c->stream>>>(keys, cols, n, t, sp, ctl, max_inserts);
+            return kl.done("hash_agg_multi_bulk_kernel");
+        }
+    }
+    auto kern = hash_agg_multi_kernel<IN, NV>;
+    const size_t smem = IN == IN_SOA ? ma_cache_bytes(MA_MAX_ACCS) : 0;
+    const int occ = occupancy(c, kern, HA_THREADS, smem);
+    const u64 tile = (u64)HA_THREADS * ma_rows<NV>();
+    const u64 grid = std::min<u64>((n + tile - 1) / tile, (u64)c->sm_count * occ);
+    if (grid == 0) return VB_OK;
+    KLaunch kl(s, klass, n);
+    kern<<<(unsigned)grid, HA_THREADS, smem, c->stream>>>(keys, cols, n, t, sp, ctl, max_inserts);
+    return kl.done("hash_agg_multi_kernel");
+}
+
+static int launch_hash_agg_multi(vb_shuf *s, int klass, const AccSpec &sp, const AggInput &in, const u64 *keys, const u64 *const *vcols,
+                                 u64 n, void *tab, u32 log_cap, TableCtl *ctl, u64 mi)
+{
+    MaCols mc{};
+    if (in.in == IN_TABLE) {
+        mc.c[0] = in.b;
+        mc.stride = (in.n - 1) + BUCKET;                    // the source has in.n - 1 regular slots
+        return launch_hash_agg_multi_t<IN_TABLE, 1>(s, klass, sp, keys, mc, n, tab, log_cap, ctl, mi);
+    }
+    for (u32 i = 0; i < s->n_cols; ++i) mc.c[i] = vcols[i];
+    switch (s->n_cols) {
+    case 1: return launch_hash_agg_multi_t<IN_SOA, 1>(s, klass, sp, keys, mc, n, tab, log_cap, ctl, mi);
+    case 2: return launch_hash_agg_multi_t<IN_SOA, 2>(s, klass, sp, keys, mc, n, tab, log_cap, ctl, mi);
+    case 3: return launch_hash_agg_multi_t<IN_SOA, 3>(s, klass, sp, keys, mc, n, tab, log_cap, ctl, mi);
+    case 4: return launch_hash_agg_multi_t<IN_SOA, 4>(s, klass, sp, keys, mc, n, tab, log_cap, ctl, mi);
+    }
+    return set_err(VB_ERR_INVALID, "hash_agg_multi: %u value columns", s->n_cols);
+}
+
+static int init_table(vb_shuf *s, void *tab, u32 log_cap, int opk, const AccSpec *ms)
+{
+    vb_ctx *c = s->ctx;
+    KLaunch kl(s, K_MISC);
+    const u64 blocks = std::min<u64>((acc_stride(log_cap) + 255) / 256, (u64)c->sm_count * 8);
+    if (ms) table_init_multi_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(table_at(tab, log_cap), *ms);
+    else table_init_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(table_at(tab, log_cap), op_identity(opk));
+    return kl.done(ms ? "table_init_multi_kernel" : "table_init_kernel");
 }
 
 constexpr u64 HOST_CHUNK_ROWS = 8ull << 20;    // host inputs stream through two 128 MiB staging halves (double-buffered)
@@ -606,15 +680,16 @@ static int estimate_distinct(vb_shuf *s, const std::vector<AggInput> &inputs, u6
 // When the load-0.4 table would spill out of L2 (2/3 of it is the budget: the input stream passes through the rest)
 // but a table at load <= 0.5 of an *estimated* key count fits, the fuller L2-resident table is taken (the estimate
 // already carries a 1.25x margin, so the real load stays under the 0.6 restart threshold).  VEGA_B200_NO_L2_FIT=1
-// disables that.
-static u32 choose_log_cap(u64 total, u64 hint_distinct, bool estimated, u32 max_log, u64 l2_bytes)
+// disables that.  slot_bytes: 16 for a single accumulator, 8 * (1 + n_acc) for a multi-aggregate table.
+static u32 choose_log_cap(u64 total, u64 hint_distinct, bool estimated, u32 max_log, u64 l2_bytes, u32 slot_bytes = 16)
 {
     u64 target = hint_distinct ? (hint_distinct * 5) / 2 : std::min<u64>(2 * std::max<u64>(total, 1), 1ull << 21);
     if (hint_distinct && target > (1ull << 22)) target = 2 * hint_distinct;
     static const bool no_l2_fit = getenv("VEGA_B200_NO_L2_FIT") != nullptr;
     const u64 budget = l2_bytes / 3 * 2;
-    if (estimated && !no_l2_fit && table_bytes(ceil_log2_u64(target)) > budget &&
-        table_bytes(ceil_log2_u64(hint_distinct * 8 / 5)) <= budget)
+    auto bytes = [&](u32 lc) { return (((u64)1 << lc) + BUCKET) * slot_bytes; };
+    if (estimated && !no_l2_fit && bytes(ceil_log2_u64(target)) > budget &&
+        bytes(ceil_log2_u64(hint_distinct * 8 / 5)) <= budget)
         target = hint_distinct * 8 / 5;
     // an estimate from a sample is a lower bound under skew: never start a large input below 2^21 slots (32 MB)
     if (estimated) target = std::max<u64>(target, 1ull << 21);
@@ -645,8 +720,9 @@ static int launch_hash_agg_partitioned(vb_shuf *s, int klass, int in, int opk, i
 
 // Feed every input into one fresh table; on overflow (abort flag) start again 4x larger.
 // slot_out (OPK_DICT): one u32 per row over the concatenation of the inputs.
+// ms != nullptr: a multi-aggregate table with these accumulators (opk / tx unused); inputs carry value columns.
 static int build_table(vb_shuf *s, int klass, const std::vector<AggInput> &inputs, int opk, int tx, u64 hint_distinct,
-                       void **out_tab, u32 *out_log_cap, u64 *out_inserted, u32 *slot_out)
+                       void **out_tab, u32 *out_log_cap, u64 *out_inserted, u32 *slot_out, const AccSpec *ms = nullptr)
 {
     vb_ctx *c = s->ctx;
     u64 total = 0;          // items that can each bring a new key (table inputs: occupied slots, not capacity)
@@ -662,15 +738,18 @@ static int build_table(vb_shuf *s, int klass, const std::vector<AggInput> &input
     const u32 max_log = std::min<u32>(MAX_LOG_CAP, std::max<u32>(4, ceil_log2_u64(2 * std::max<u64>(total, 1))));
     bool estimated = false;
     if (!hint_distinct && total > (1ull << 20)) { TRY(estimate_distinct(s, inputs, total, &hint_distinct)); estimated = true; }
-    u32 log_cap = choose_log_cap(total, hint_distinct, estimated, max_log, c->l2_bytes);
+    const u32 slot_bytes = ms ? 8 * (1 + ms->n) : 16;
+    u32 log_cap = choose_log_cap(total, hint_distinct, estimated, max_log, c->l2_bytes, slot_bytes);
 
     DevBuf ctl(c), stage_a(c), stage_b(c);
     TRY(ctl.alloc(sizeof(TableCtl)));
     const u64 stage_rows = std::min(max_host, HOST_CHUNK_ROWS);
+    const u64 row_bytes = ms ? 8 * (1 + s->n_cols) : 16;
     bool half_used[2] = {false, false};
     if (any_host) {
-        TRY(stage_a.alloc(stage_rows * 16));   // per half: AoS rows, or SoA keys in the first 8 B/row / vals in the second
-        TRY(stage_b.alloc(stage_rows * 16));
+        // per half: AoS rows, or SoA keys in the first 8 B/row / vals (multi: each value column) in the next
+        TRY(stage_a.alloc(stage_rows * row_bytes));
+        TRY(stage_b.alloc(stage_rows * row_bytes));
         CU(cudaEventRecord(c->ev_ready, c->stream));               // the pool hands the halves out in stream order
         CU(cudaStreamWaitEvent(c->copy_stream, c->ev_ready, 0));
     }
@@ -679,19 +758,16 @@ static int build_table(vb_shuf *s, int klass, const std::vector<AggInput> &input
     for (;;) {
         const u64 cap = 1ull << log_cap;
         DevBuf tab(c);
-        TRY(tab.alloc(table_bytes(log_cap)));
-        {
-            KLaunch kl(s, K_MISC);
-            u64 blocks = std::min<u64>((cap + BUCKET + 255) / 256, (u64)c->sm_count * 8);
-            table_init_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(table_at(tab.p, log_cap), op_identity(opk));
-            TRY(kl.done("table_init_kernel"));
-        }
+        TRY(tab.alloc(ms ? table_bytes_multi(log_cap, ms->n) : table_bytes(log_cap)));
+        TRY(init_table(s, tab.p, log_cap, opk, ms));
         CU(cudaMemsetAsync(ctl.p, 0, sizeof(TableCtl), c->stream));
         const u64 max_inserts = (log_cap == max_log) ? ~0ull : (cap / 10) * 6;
         u64 row_base = 0;
         for (auto &in : inputs) {
             if (in.n == 0) continue;
-            if (in.loc != VB_HOST && !slot_out && want_partition(in.in, opk, log_cap, in.n)) {
+            if (ms && in.loc != VB_HOST) {             // partition-first building moves one value column: not for multi tables
+                TRY(launch_hash_agg_multi(s, klass, *ms, in, in.a, in.cols, in.n, tab.p, log_cap, ctl.as<TableCtl>(), max_inserts));
+            } else if (in.loc != VB_HOST && !slot_out && want_partition(in.in, opk, log_cap, in.n)) {
                 TRY(launch_hash_agg_partitioned(s, klass, in.in, opk, tx, in.a, in.b, in.n, tab.p, log_cap, ctl.as<TableCtl>(), max_inserts));
             } else if (in.loc != VB_HOST) {
                 TRY(launch_hash_agg(s, klass, in.in, opk, tx, in.a, in.b, in.n, tab.p, log_cap, ctl.as<TableCtl>(),
@@ -706,7 +782,17 @@ static int build_table(vb_shuf *s, int klass, const std::vector<AggInput> &input
                     u64 *half = hb ? stage_b.as<u64>() : stage_a.as<u64>();
                     const u64 *da = half, *db = nullptr;
                     if (half_used[hb]) CU(cudaStreamWaitEvent(c->copy_stream, c->ev_kernel[hb], 0));   // its last reader is done
-                    if (in.in == IN_AOS) {
+                    const u64 *vc[MA_MAX_COLS] = {};
+                    if (ms) {
+                        CU(cudaMemcpyAsync(half, in.a + off, m * 8, cudaMemcpyHostToDevice, c->copy_stream));
+                        s->st.h2d_bytes += m * 8;
+                        for (u32 col = 0; col < s->n_cols; ++col) {
+                            if (!in.cols[col]) continue;
+                            vc[col] = half + (u64)(1 + col) * chunk;
+                            CU(cudaMemcpyAsync((void *)vc[col], in.cols[col] + off, m * 8, cudaMemcpyHostToDevice, c->copy_stream));
+                            s->st.h2d_bytes += m * 8;
+                        }
+                    } else if (in.in == IN_AOS) {
                         CU(cudaMemcpyAsync(half, in.a + 2 * off, m * 16, cudaMemcpyHostToDevice, c->copy_stream));
                         s->st.h2d_bytes += m * 16;
                     } else {
@@ -720,8 +806,8 @@ static int build_table(vb_shuf *s, int klass, const std::vector<AggInput> &input
                     }
                     CU(cudaEventRecord(c->ev_copied[hb], c->copy_stream));
                     CU(cudaStreamWaitEvent(c->stream, c->ev_copied[hb], 0));
-                    TRY(launch_hash_agg(s, klass, in.in, opk, tx, da, db, m, tab.p, log_cap, ctl.as<TableCtl>(),
-                                        max_inserts, nullptr));
+                    if (ms) TRY(launch_hash_agg_multi(s, klass, *ms, in, da, vc, m, tab.p, log_cap, ctl.as<TableCtl>(), max_inserts));
+                    else TRY(launch_hash_agg(s, klass, in.in, opk, tx, da, db, m, tab.p, log_cap, ctl.as<TableCtl>(), max_inserts, nullptr));
                     CU(cudaEventRecord(c->ev_kernel[hb], c->stream));
                     half_used[hb] = true;
                 }
@@ -1342,6 +1428,68 @@ extern "C" int32_t vb_shuffle_create(vb_ctx *c, uint64_t shuffle_id, uint32_t n_
     return VB_OK;
 }
 
+// Accumulators of a multi-aggregate shuffle: aggregate a owns accumulator a; a MEAN's is its SUM, and every MEAN
+// divides by the spec's first COUNT accumulator, or by one appended after the aggregates when the spec has none.
+extern "C" int32_t vb_shuffle_create_multi(vb_ctx *c, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce, int32_t kdt,
+                                           uint32_t n_val_cols, const int32_t *val_dtypes, uint32_t n_aggs, const vb_agg_col *aggs,
+                                           vb_shuf **out)
+{
+    if (!c || !out || !val_dtypes || !aggs) return set_err(VB_ERR_INVALID, "vb_shuffle_create_multi: NULL argument");
+    *out = nullptr;
+    if (n_val_cols < 1 || n_val_cols > VB_MAX_VAL_COLS) return set_err(VB_ERR_INVALID, "%u value columns (1..%d)", n_val_cols, VB_MAX_VAL_COLS);
+    if (n_aggs < 1 || n_aggs > VB_MAX_AGGS) return set_err(VB_ERR_INVALID, "%u aggregates (1..%d)", n_aggs, VB_MAX_AGGS);
+    for (u32 i = 0; i < n_val_cols; ++i)
+        if (val_dtypes[i] < VB_U64 || val_dtypes[i] > VB_F64) return set_err(VB_ERR_INVALID, "bad dtype %d of value column %u", val_dtypes[i], i);
+    int count_acc = -1;
+    bool any_mean = false;
+    for (u32 a = 0; a < n_aggs; ++a) {
+        const int op = aggs[a].agg;
+        if (op != VB_AGG_SUM && op != VB_AGG_MIN && op != VB_AGG_MAX && op != VB_AGG_COUNT && op != VB_AGG_MEAN)
+            return set_err(VB_ERR_INVALID, "aggregate %u: op %d is not SUM / MIN / MAX / COUNT / MEAN", a, op);
+        if (op != VB_AGG_COUNT && (aggs[a].src < 0 || (u32)aggs[a].src >= n_val_cols))
+            return set_err(VB_ERR_INVALID, "aggregate %u reads column %d of %u", a, aggs[a].src, n_val_cols);
+        if (op == VB_AGG_COUNT && count_acc < 0) count_acc = (int)a;
+        any_mean |= op == VB_AGG_MEAN;
+    }
+    const u32 n_acc = n_aggs + ((any_mean && count_acc < 0) ? 1 : 0);
+    if (n_acc > VB_MAX_AGGS) return set_err(VB_ERR_INVALID, "%u aggregates plus the COUNT a MEAN needs exceed %d", n_aggs, VB_MAX_AGGS);
+    if (count_acc < 0) count_acc = (int)n_aggs;
+    TRY(vb_shuffle_create(c, shuffle_id, n_map, n_reduce, kdt, VB_U64, VB_AGG_SUM, VB_PART_HASH_METRO64, out));
+    vb_shuf *s = *out;
+    s->multi = true;
+    s->n_cols = n_val_cols;
+    AccSpec &mp = s->acc_map, &mg = s->acc_merge;
+    OutSpec &os = s->outs;
+    mp.n = mg.n = n_acc;
+    os.n = n_aggs;
+    for (u32 a = 0; a < n_acc; ++a) {
+        const int op = a < n_aggs ? aggs[a].agg : VB_AGG_COUNT;
+        const int src = op == VB_AGG_COUNT ? 0 : aggs[a].src;
+        const int dt = val_dtypes[src];
+        int opk = OPK_COUNT, tx = TX_NONE;
+        if (op == VB_AGG_SUM || op == VB_AGG_MEAN) opk = dt == VB_F64 ? OPK_ADD_F64 : OPK_ADD_U64;
+        else if (op == VB_AGG_MIN || op == VB_AGG_MAX) {
+            opk = op == VB_AGG_MIN ? OPK_MIN_U64 : OPK_MAX_U64;
+            tx = dt == VB_I64 ? TX_I64 : dt == VB_F64 ? TX_F64 : TX_NONE;
+        }
+        spec_set(mp.op, a, opk); spec_set(mp.tx, a, tx); spec_set(mp.src, a, src);
+        spec_set(mg.op, a, merge_op(opk)); spec_set(mg.src, a, a);
+        if (a >= n_aggs) continue;
+        os.acc[a] = (unsigned char)a;
+        os.cnt[a] = (unsigned char)count_acc;
+        os.tx[a] = (unsigned char)tx;
+        os.kind[a] = op != VB_AGG_MEAN ? MO_COPY : dt == VB_U64 ? MO_MEAN_U64 : dt == VB_I64 ? MO_MEAN_I64 : MO_MEAN_F64;
+    }
+    return VB_OK;
+}
+
+static_assert(MA_MAX_COLS == VB_MAX_VAL_COLS && MA_MAX_ACCS == VB_MAX_AGGS, "kernel limits = ABI limits");
+
+static int reject_multi(const vb_shuf *s, const char *what)
+{
+    return set_err(VB_ERR_UNSUPPORTED, "shuffle %llu has several aggregates per key: %s is not supported for it yet", (unsigned long long)s->id, what);
+}
+
 extern "C" int32_t vb_shuffle_set_key_width(vb_shuf *s, uint32_t bytes)
 {
     if (!s || (bytes != 4 && bytes != 8)) return set_err(VB_ERR_INVALID, "key width must be 4 or 8");
@@ -1359,6 +1507,7 @@ extern "C" int32_t vb_shuffle_set_hint(vb_shuf *s, uint64_t d)
 extern "C" int32_t vb_shuffle_set_dist(vb_shuf *s, uint32_t rank, uint32_t world)
 {
     if (!s || world < 1 || rank >= world || world > 256) return set_err(VB_ERR_INVALID, "bad rank/world");
+    if (s->multi && world > 1) return reject_multi(s, "multi-rank use (the exchange moves one value column)");
     s->rank = rank;
     s->world = world;
     return VB_OK;
@@ -1372,7 +1521,11 @@ static void free_map(vb_shuf *s, MapOut &m)
     m = MapOut();
 }
 
-static int shuffle_map(vb_shuf *s, u32 map_id, const u64 *rows, const u64 *keys, const u64 *vals, u64 n, int loc, bool combined = false)
+static const AccSpec *map_spec(const vb_shuf *s) { return s->multi ? &s->acc_map : nullptr; }
+
+// cols: the value columns of a multi-aggregate shuffle (keys + cols, vals unused)
+static int shuffle_map(vb_shuf *s, u32 map_id, const u64 *rows, const u64 *keys, const u64 *vals, u64 n, int loc, bool combined = false,
+                       const u64 *const *cols = nullptr)
 {
     if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
     if (map_id >= s->n_map) return set_err(VB_ERR_INVALID, "map_id %u >= n_map %u", map_id, s->n_map);
@@ -1395,35 +1548,33 @@ static int shuffle_map(vb_shuf *s, u32 map_id, const u64 *rows, const u64 *keys,
         free_map(s, m);
     }
     m.n_rows = n;
+    const AccSpec *ms = map_spec(s);
     if (is_reduce_op(s->agg) && loc == VB_DEVICE_BORROWED && !combined) {
-        if (!rows && !vals && s->agg != VB_AGG_COUNT && n) return set_err(VB_ERR_INVALID, "values required for this aggregator");
+        if (!ms && !rows && !vals && s->agg != VB_AGG_COUNT && n) return set_err(VB_ERR_INVALID, "values required for this aggregator");
         std::vector<AggInput> in(1);
         in[0] = AggInput{rows ? IN_AOS : IN_SOA, rows ? rows : keys, vals, n, VB_DEVICE};
+        if (ms) for (u32 i = 0; i < s->n_cols; ++i) in[0].cols[i] = m.cols[i] = cols[i];
         if (!s->sh_tab && !s->sh_dirty && n) {       // first borrowed map task: size and create the shared table
             u64 hint = s->hint;
             bool estimated = false;
             const u64 total_guess = n * std::max<u64>(1, s->n_map / std::max<u32>(1, s->world));
             if (!hint && n > (1ull << 20)) { TRY(estimate_distinct(s, in, total_guess, &hint)); estimated = true; }
             const u32 max_log = std::min<u32>(MAX_LOG_CAP, std::max<u32>(4, ceil_log2_u64(2 * std::max<u64>(total_guess, 1))));
-            s->sh_log_cap = choose_log_cap(total_guess, hint, estimated, max_log, c->l2_bytes);
+            s->sh_log_cap = choose_log_cap(total_guess, hint, estimated, max_log, c->l2_bytes, ms ? 8 * (1 + ms->n) : 16);
             DevBuf tab(c), ctl(c);
-            TRY(tab.alloc(table_bytes(s->sh_log_cap)));
+            TRY(tab.alloc(ms ? table_bytes_multi(s->sh_log_cap, ms->n) : table_bytes(s->sh_log_cap)));
             TRY(ctl.alloc(sizeof(TableCtl)));
             CU(cudaMemsetAsync(ctl.p, 0, sizeof(TableCtl), c->stream));
-            {
-                KLaunch kl(s, K_MISC);
-                const u64 cap = 1ull << s->sh_log_cap;
-                u64 blocks = std::min<u64>((cap + BUCKET + 255) / 256, (u64)c->sm_count * 8);
-                table_init_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(table_at(tab.p, s->sh_log_cap), op_identity(map_opk(s)));
-                TRY(kl.done("table_init_kernel"));
-            }
+            TRY(init_table(s, tab.p, s->sh_log_cap, map_opk(s), ms));
             s->sh_max_inserts = (s->sh_log_cap >= max_log) ? ~0ull : ((1ull << s->sh_log_cap) / 10) * 6;
             s->sh_tab = tab.release();
             s->sh_ctl = (TableCtl *)ctl.release();
             s->st.table_slots = std::max<u64>(s->st.table_slots, 1ull << s->sh_log_cap);
         }
         if (s->sh_tab && !s->sh_dirty && n) {         // asynchronous: checked at seal
-            if (want_partition(in[0].in, map_opk(s), s->sh_log_cap, n))
+            if (ms)
+                TRY(launch_hash_agg_multi(s, K_HASH_AGG, *ms, in[0], keys, cols, n, s->sh_tab, s->sh_log_cap, s->sh_ctl, s->sh_max_inserts));
+            else if (want_partition(in[0].in, map_opk(s), s->sh_log_cap, n))
                 TRY(launch_hash_agg_partitioned(s, K_HASH_AGG, in[0].in, map_opk(s), val_tx(s), in[0].a, in[0].b, n, s->sh_tab, s->sh_log_cap,
                                                 s->sh_ctl, s->sh_max_inserts));
             else
@@ -1432,12 +1583,14 @@ static int shuffle_map(vb_shuf *s, u32 map_id, const u64 *rows, const u64 *keys,
         }
         m.rows = rows; m.keys = keys; m.vals = vals; m.owned = false; m.in_shared = true;
     } else if (is_reduce_op(s->agg)) {
-        if (!rows && !vals && s->agg != VB_AGG_COUNT && n) return set_err(VB_ERR_INVALID, "values required for this aggregator");
+        if (!ms && !rows && !vals && s->agg != VB_AGG_COUNT && n) return set_err(VB_ERR_INVALID, "values required for this aggregator");
         std::vector<AggInput> in(1);
         in[0] = AggInput{rows ? IN_AOS : IN_SOA, rows ? rows : keys, vals, n, loc == VB_HOST ? VB_HOST : VB_DEVICE};
+        if (ms) for (u32 i = 0; i < s->n_cols; ++i) in[0].cols[i] = cols[i];
         const u64 hint = s->hint ? s->hint : (s->learned_distinct ? s->learned_distinct + s->learned_distinct / 4 : 0);
         // a map-side-combined bucket carries combiners, merged with merge_combiners (partial counts are summed)
-        TRY(build_table(s, K_HASH_AGG, in, combined ? merge_opk(s) : map_opk(s), val_tx(s), hint, &m.table, &m.log_cap, &m.n_inserted, nullptr));
+        TRY(build_table(s, K_HASH_AGG, in, combined ? merge_opk(s) : map_opk(s), val_tx(s), hint, &m.table, &m.log_cap, &m.n_inserted, nullptr,
+                        ms));
         s->learned_distinct = std::max<u64>(m.n_inserted, 1);
     } else if (n) {
         if (loc == VB_DEVICE_BORROWED) {
@@ -1486,11 +1639,25 @@ static int shuffle_map(vb_shuf *s, u32 map_id, const u64 *rows, const u64 *keys,
 
 extern "C" int32_t vb_shuffle_map_aos(vb_shuf *s, uint32_t map_id, const void *rows, uint64_t n, int32_t loc)
 {
+    if (s && s->multi) return reject_multi(s, "AoS rows");
     return shuffle_map(s, map_id, (const u64 *)rows, nullptr, nullptr, n, loc);
 }
 extern "C" int32_t vb_shuffle_map_soa(vb_shuf *s, uint32_t map_id, const void *keys, const void *vals, uint64_t n, int32_t loc)
 {
+    if (s && s->multi) return set_err(VB_ERR_INVALID, "shuffle %llu has several aggregates per key: map it with vb_shuffle_map_cols", (unsigned long long)s->id);
     return shuffle_map(s, map_id, nullptr, (const u64 *)keys, (const u64 *)vals, n, loc);
+}
+extern "C" int32_t vb_shuffle_map_cols(vb_shuf *s, uint32_t map_id, const void *keys, const void *const *vals, uint64_t n, int32_t loc)
+{
+    if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
+    if (!s->multi) return set_err(VB_ERR_INVALID, "vb_shuffle_map_cols needs a shuffle from vb_shuffle_create_multi");
+    const u64 *cols[MA_MAX_COLS] = {};
+    for (u32 i = 0; vals && i < s->n_cols; ++i) cols[i] = (const u64 *)vals[i];
+    for (u32 a = 0; a < s->acc_map.n; ++a)
+        if (n && spec_at(s->acc_map.op, a) != OPK_COUNT && !cols[spec_at(s->acc_map.src, a)])
+            return set_err(VB_ERR_INVALID, "value column %d is read by an aggregate but NULL", spec_at(s->acc_map.src, a));
+    if (n && !keys) return set_err(VB_ERR_INVALID, "NULL keys with n_rows > 0");
+    return shuffle_map(s, map_id, nullptr, (const u64 *)keys, nullptr, n, loc, false, cols);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1667,9 +1834,12 @@ static int settle_shared_table(vb_shuf *s, u64 *n_ins)
         if (any) {
             std::vector<AggInput> in;
             for (auto &m : s->maps)
-                if (m.present && m.in_shared && m.n_rows)
+                if (m.present && m.in_shared && m.n_rows) {
                     in.push_back(AggInput{m.rows ? IN_AOS : IN_SOA, m.rows ? m.rows : m.keys, m.vals, m.n_rows, VB_DEVICE});
-            TRY(build_table(s, K_HASH_AGG, in, map_opk(s), val_tx(s), std::max<u64>(s->hint, 2 * (*n_ins)), &s->sh_tab, &s->sh_log_cap, n_ins, nullptr));
+                    std::copy(m.cols, m.cols + MA_MAX_COLS, in.back().cols);
+                }
+            TRY(build_table(s, K_HASH_AGG, in, map_opk(s), val_tx(s), std::max<u64>(s->hint, 2 * (*n_ins)), &s->sh_tab, &s->sh_log_cap, n_ins, nullptr,
+                            map_spec(s)));
         }
     }
     return VB_OK;
@@ -1701,7 +1871,8 @@ static int merge_map_tables(vb_shuf *s, void **tab, u32 *log_cap, u64 *n_ins)
         in.push_back(AggInput{IN_TABLE, mt.keys, mt.accs, (1ull << t.log_cap) + 1, VB_DEVICE, t.ins + 1});
         max_ins = std::max(max_ins, t.ins);
     }
-    TRY(build_table(s, K_MERGE, in, merge_opk(s), TX_NONE, std::max<u64>(max_ins, s->hint), tab, log_cap, n_ins, nullptr));
+    TRY(build_table(s, K_MERGE, in, merge_opk(s), TX_NONE, std::max<u64>(max_ins, s->hint), tab, log_cap, n_ins, nullptr,
+                    s->multi ? &s->acc_merge : nullptr));
     for (auto &t : ts) dev_free(s->ctx, t.tab);
     disown();
     return VB_OK;
@@ -1717,6 +1888,27 @@ static int finalize_reduce(vb_shuf *s, void *tab, u32 log_cap, u64 n_ins)
     if (!tab) return VB_OK;
     const u64 cap = 1ull << log_cap;
     const u64 max_d = n_ins + 1;
+    if (s->multi) {
+        // keys and slot indices grouped by reduce partition, then one gather per output column
+        DevBuf k(c), sl(c), out(c);
+        TRY(k.alloc(max_d * 8));
+        TRY(sl.alloc(max_d * 8));
+        const Table ft = table_at(tab, log_cap);
+        TRY(multisplit(s, Loader{LD_TABLE_KI, ft.keys, nullptr, cap}, cap + 1, DG_BUCKET, R, max_d, k.as<u64>(), sl.as<u64>(), s->bucket_off));
+        const u64 D = s->bucket_off[R];
+        if (D) {
+            TRY(out.alloc(D * 8 * s->outs.n));
+            KLaunch kl(s, K_MISC);
+            const u64 blocks = std::min<u64>((D + 255) / 256, (u64)c->sm_count * 8);
+            multi_finalize_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(ft.accs, acc_stride(log_cap), sl.as<u64>(), D, s->outs, out.as<u64>());
+            TRY(kl.done("multi_finalize_kernel"));
+        }
+        s->n_keys = D;
+        s->res_keys = (u64 *)k.release();
+        s->res_cols = (u64 *)out.release();
+        s->st.rows_out = D;
+        return VB_OK;
+    }
     DevBuf k(c), v(c);
     TRY(k.alloc(max_d * 8));
     TRY(v.alloc(max_d * 8));
@@ -1921,6 +2113,7 @@ static int export_prepare_locked(vb_shuf *s, uint64_t *counts)
 extern "C" int32_t vb_shuffle_export_prepare(vb_shuf *s, uint64_t *counts)
 {
     if (!s || !counts) return set_err(VB_ERR_INVALID, "NULL argument");
+    if (s->multi) return reject_multi(s, "multi-rank exchange");
     if (s->world < 2) return set_err(VB_ERR_STATE, "vb_shuffle_export_prepare needs vb_shuffle_set_dist(world > 1)");
     vb_ctx *c = s->ctx;
     std::lock_guard<std::mutex> lk(c->mu);
@@ -2034,6 +2227,7 @@ static int export_counts_locked(vb_shuf *s, uint64_t *counts)
 extern "C" int32_t vb_shuffle_export_counts(vb_shuf *s, uint64_t *counts)
 {
     if (!s || !counts) return set_err(VB_ERR_INVALID, "NULL argument");
+    if (s->multi) return reject_multi(s, "multi-rank exchange");
     if (s->world < 2) return set_err(VB_ERR_STATE, "vb_shuffle_export_counts needs vb_shuffle_set_dist(world > 1)");
     std::lock_guard<std::mutex> lk(s->ctx->mu);
     CU(cudaSetDevice(s->ctx->device));
@@ -2098,6 +2292,7 @@ static int export_direct_locked(vb_shuf *s, const uint64_t *dst_row_offset, cons
 extern "C" int32_t vb_shuffle_export_direct(vb_shuf *s, const uint64_t *dst_row_offset, const uint64_t *dst_total_rows)
 {
     if (!s || !dst_row_offset || !dst_total_rows) return set_err(VB_ERR_INVALID, "NULL argument");
+    if (s->multi) return reject_multi(s, "multi-rank exchange");
     std::lock_guard<std::mutex> lk(s->ctx->mu);
     CU(cudaSetDevice(s->ctx->device));
     return export_direct_locked(s, dst_row_offset, dst_total_rows, true);
@@ -2108,6 +2303,7 @@ extern "C" int32_t vb_shuffle_export_direct(vb_shuf *s, const uint64_t *dst_row_
 extern "C" int32_t vb_shuffle_import_arena(vb_shuf *s, const uint64_t *counts)
 {
     if (!s || !counts) return set_err(VB_ERR_INVALID, "NULL argument");
+    if (s->multi) return reject_multi(s, "multi-rank exchange");
     if (!s->exported || s->sealed) return set_err(VB_ERR_STATE, "import needs the export first and no seal yet");
     u64 n = 0;
     for (u32 r = 0; r < s->world; ++r) n += counts[r];
@@ -2123,6 +2319,7 @@ extern "C" int32_t vb_shuffle_import_arena(vb_shuf *s, const uint64_t *counts)
 extern "C" int32_t vb_shuffle_export_buffers(vb_shuf *s, void **keys_dev, void **vals_dev)
 {
     if (!s || !keys_dev || !vals_dev) return set_err(VB_ERR_INVALID, "NULL argument");
+    if (s->multi) return reject_multi(s, "multi-rank exchange");
     if (!s->exported) return set_err(VB_ERR_STATE, "vb_shuffle_export_buffers before vb_shuffle_export_prepare");
     *keys_dev = s->exp_keys;
     *vals_dev = s->exp_vals;
@@ -2132,6 +2329,7 @@ extern "C" int32_t vb_shuffle_export_buffers(vb_shuf *s, void **keys_dev, void *
 extern "C" int32_t vb_shuffle_import(vb_shuf *s, const void *keys_dev, const void *vals_dev, const uint64_t *counts)
 {
     if (!s || !counts) return set_err(VB_ERR_INVALID, "NULL argument");
+    if (s->multi) return reject_multi(s, "multi-rank exchange");
     if (!s->exported || s->sealed) return set_err(VB_ERR_STATE, "import needs export_prepare first and no seal yet");
     u64 n = 0;
     for (u32 r = 0; r < s->world; ++r) n += counts[r];
@@ -2598,6 +2796,7 @@ static int exchange_sort_locked(vb_shuf *s)
 extern "C" int32_t vb_shuffle_exchange(vb_shuf *s, int32_t mode)
 {
     if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
+    if (s->multi) return reject_multi(s, "multi-rank exchange");
     vb_ctx *c = s->ctx;
     if (s->world < 2) return set_err(VB_ERR_STATE, "vb_shuffle_exchange needs vb_shuffle_set_dist(world > 1)");
     if (!c->comm) return set_err(VB_ERR_STATE, "vb_shuffle_exchange needs vb_ctx_comm_init");
@@ -3005,10 +3204,30 @@ extern "C" int32_t vb_shuffle_reduce(vb_shuf *s, uint32_t r, void *out_keys, voi
             }
         }
         TRY(copy_out(s, out_vals, s->res_vals ? s->res_vals + v0 : nullptr, nv * 8, dst_loc));
+    } else if (out_combined && s->multi) {
+        return set_err(VB_ERR_INVALID, "shuffle %llu has several aggregates per key: read them with vb_shuffle_reduce_cols", (unsigned long long)s->id);
     } else if (out_combined && nk) {
         if (!s->res_comb && s->agg == VB_AGG_SORT) return set_err(VB_ERR_INVALID, "key-only sort has no payload");
         TRY(copy_out(s, out_combined, s->res_comb + b0, nk * 8, dst_loc));
     }
+    CU(cudaStreamSynchronize(c->stream));
+    return VB_OK;
+}
+
+extern "C" int32_t vb_shuffle_reduce_cols(vb_shuf *s, uint32_t r, void *out_keys, void *const *out_aggs, int32_t dst_loc)
+{
+    if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
+    if (!s->multi) return set_err(VB_ERR_INVALID, "vb_shuffle_reduce_cols needs a shuffle from vb_shuffle_create_multi");
+    if (r >= s->n_reduce) return set_err(VB_ERR_INVALID, "reduce_id %u >= n_reduce %u", r, s->n_reduce);
+    if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
+    TRY(wait_sealed(s));
+    vb_ctx *c = s->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    const u64 b0 = s->bucket_off[r], nk = s->bucket_off[r + 1] - b0;
+    TRY(copy_out(s, out_keys, s->res_keys ? s->res_keys + b0 : nullptr, nk * 8, dst_loc));
+    for (u32 o = 0; out_aggs && o < s->outs.n; ++o)
+        TRY(copy_out(s, out_aggs[o], s->res_cols ? s->res_cols + (u64)o * s->n_keys + b0 : nullptr, nk * 8, dst_loc));
     CU(cudaStreamSynchronize(c->stream));
     return VB_OK;
 }
@@ -3026,6 +3245,7 @@ static u64 blob_bytes(const vb_shuf *s, u32 r)
 extern "C" int32_t vb_shuffle_reduce_blob_size(vb_shuf *s, uint32_t r, uint64_t *n_bytes)
 {
     if (!s || !n_bytes) return set_err(VB_ERR_INVALID, "NULL argument");
+    if (s->multi) return reject_multi(s, "bincode blobs");
     if (r >= s->n_reduce) return set_err(VB_ERR_INVALID, "reduce_id %u >= n_reduce %u", r, s->n_reduce);
     TRY(wait_sealed(s));
     if (s->lazy) {
@@ -3040,6 +3260,7 @@ extern "C" int32_t vb_shuffle_reduce_blob_size(vb_shuf *s, uint32_t r, uint64_t 
 extern "C" int32_t vb_shuffle_reduce_blob(vb_shuf *s, uint32_t r, void *out_blob, int32_t dst_loc)
 {
     if (!s || !out_blob) return set_err(VB_ERR_INVALID, "NULL argument");
+    if (s->multi) return reject_multi(s, "bincode blobs");
     if (r >= s->n_reduce) return set_err(VB_ERR_INVALID, "reduce_id %u >= n_reduce %u", r, s->n_reduce);
     if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
     TRY(wait_sealed(s));
@@ -3072,6 +3293,7 @@ extern "C" int32_t vb_shuffle_reduce_blob(vb_shuf *s, uint32_t r, void *out_blob
 extern "C" int32_t vb_shuffle_map_blob(vb_shuf *s, uint32_t map_id, const void *blob, uint64_t n_bytes, int32_t src_loc)
 {
     if (!s || !blob) return set_err(VB_ERR_INVALID, "NULL argument");
+    if (s->multi) return reject_multi(s, "bincode blobs");
     if (src_loc < VB_HOST || src_loc > VB_DEVICE_BORROWED) return set_err(VB_ERR_INVALID, "bad src_loc");
     if (s->agg == VB_AGG_SORT) return set_err(VB_ERR_UNSUPPORTED, "sort_by_key takes rows, not combined buckets");
     if (n_bytes < 8 || (n_bytes & 7)) return set_err(VB_ERR_INVALID, "corrupted blob: %llu bytes", (unsigned long long)n_bytes);
@@ -3268,7 +3490,7 @@ extern "C" int32_t vb_shuffle_free(vb_shuf *s)
         resolve_timers(s);
         for (auto &m : s->maps) free_map(s, m);
         release_inputs(s);
-        dev_free(c, s->res_keys); dev_free(c, s->res_comb); dev_free(c, s->res_offs); dev_free(c, s->res_vals);
+        dev_free(c, s->res_keys); dev_free(c, s->res_comb); dev_free(c, s->res_offs); dev_free(c, s->res_vals); dev_free(c, s->res_cols);
         dev_free(c, s->dict); dev_free(c, s->dense_of_slot);
         for (auto &kv : s->join_plans) { dev_free(c, kv.second.pos); dev_free(c, kv.second.match); }
         free_lazy_rows(s);

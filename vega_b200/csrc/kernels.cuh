@@ -146,8 +146,9 @@ VB_D u64 home_bucket(u64 key, u32 log_cap) { return slot_hash(key) >> (64 - (log
 // Resolve `key` starting from bucket `b` whose content `bk` is already loaded: find it, or claim the
 // first empty slot with a CAS, or move on to the next bucket.  Slots only ever go EMPTY → key and are
 // claimed first-empty-first, so a key can never end up in two slots (a stale view is an older view).
-template <int OPK>
-VB_D bool table_resolve(const Table &t, u64 b, Bucket4 bk, u64 key, u64 v, u32 &slot_idx, u32 &inserted)
+// on_hit(slot) combines into the slot's accumulator(s).
+template <class OnHit>
+VB_D bool table_resolve_with(const Table &t, u64 b, Bucket4 bk, u64 key, u32 &inserted, OnHit &&on_hit)
 {
     const u64 nb_mask = (1ull << (t.log_cap - 2)) - 1;
 #pragma unroll 1
@@ -164,14 +165,17 @@ VB_D bool table_resolve(const Table &t, u64 b, Bucket4 bk, u64 key, u64 v, u32 &
             }
         }
         if (hit >= 0) {
-            const u64 s = 4 * b + (u64)hit;
-            op_red<OPK>(&t.accs[s], v);
-            slot_idx = (u32)s;
+            on_hit(4 * b + (u64)hit);
             return true;
         }
         bk = ld_bucket(&t.keys[4 * b]);
     }
     return false;
+}
+template <int OPK>
+VB_D bool table_resolve(const Table &t, u64 b, Bucket4 bk, u64 key, u64 v, u32 &slot_idx, u32 &inserted)
+{
+    return table_resolve_with(t, b, bk, key, inserted, [&](u64 s) { op_red<OPK>(&t.accs[s], v); slot_idx = (u32)s; });
 }
 
 // ---- per-CTA hot-key cache (skewed keys) -------------------------------------------------------
@@ -197,24 +201,34 @@ VB_D void op_shared(u64 *acc, u64 v)
     else if (OPK == OPK_MAX_U64) atomicMax((unsigned long long *)acc, (unsigned long long)v);
 }
 
-// 0: not absorbed (row goes to the table); 1: hit an already cached key; 2: claimed an empty cache slot
-template <int OPK>
-VB_D int cache_combine(u64 *hc_keys, u64 *hc_acc, u64 h, u64 key, u64 v)
+// 0: not absorbed (row goes to the table); 1: hit an already cached key; 2: claimed an empty cache slot.
+// on_hit(i) combines the row into cache slot i.
+template <u32 SLOTS, class OnHit>
+VB_D int cache_combine_with(u64 *hc_keys, u64 h, u64 key, OnHit &&on_hit)
 {
-    const u32 i1 = (u32)h & (HC_SLOTS - 1), i2 = (u32)(h >> 10) & (HC_SLOTS - 1);
+    const u32 i1 = (u32)h & (SLOTS - 1), i2 = (u32)(h >> 10) & (SLOTS - 1);
     const u64 c1 = hc_keys[i1];
-    if (c1 == key) { op_shared<OPK>(&hc_acc[i1], v); return 1; }
+    if (c1 == key) { on_hit(i1); return 1; }
     const u64 c2 = hc_keys[i2];
-    if (c2 == key) { op_shared<OPK>(&hc_acc[i2], v); return 1; }
+    if (c2 == key) { on_hit(i2); return 1; }
     u32 slot;
     if (c1 == EMPTY_KEY) slot = i1;
     else if (c2 == EMPTY_KEY) slot = i2;
     else return 0;
     const u64 old = atomicCAS((unsigned long long *)&hc_keys[slot], (unsigned long long)EMPTY_KEY, (unsigned long long)key);
-    if (old == EMPTY_KEY) { op_shared<OPK>(&hc_acc[slot], v); return 2; }
-    if (old == key) { op_shared<OPK>(&hc_acc[slot], v); return 1; }
+    if (old == EMPTY_KEY) { on_hit(slot); return 2; }
+    if (old == key) { on_hit(slot); return 1; }
     return 0;
 }
+template <int OPK>
+VB_D int cache_combine(u64 *hc_keys, u64 *hc_acc, u64 h, u64 key, u64 v)
+{
+    return cache_combine_with<HC_SLOTS>(hc_keys, h, key, [&](u32 i) { op_shared<OPK>(&hc_acc[i], v); });
+}
+
+template <int ROWS, class OnHit>
+VB_D void ha_probe_rows(const Table &t, TableCtl *ctl, const u64 (&k)[ROWS], bool (&ok)[ROWS], const u64 (&h)[ROWS], u32 &my_inserts,
+                        OnHit &&on_hit);
 
 // The per-tile work shared by the register-staged and the bulk-staged kernels: thread-private rows
 // k/v/ok (HA_ROWS of them, row j of the thread is input row row0 + j * HA_THREADS) → special key,
@@ -225,7 +239,6 @@ VB_D void ha_process_rows(const Table &t, TableCtl *ctl, u64 (&k)[ROWS], u64 (&v
 {
     const u64 cap = 1ull << t.log_cap;
     const u64 tpol = table_policy();
-    const u32 hshift = 64 - (t.log_cap - 2);
     // f64 MIN/MAX fold like Rust's f64::min / f64::max: a NaN value is ignored (it becomes the op's identity, so the
     // key is still inserted), and a key whose values are all NaN finalises to tx_inv(identity), which is a NaN.
     constexpr bool NAN_IS_IDENTITY = (TX == TX_F64) && (OPK == OPK_MIN_U64 || OPK == OPK_MAX_U64);
@@ -250,6 +263,20 @@ VB_D void ha_process_rows(const Table &t, TableCtl *ctl, u64 (&k)[ROWS], u64 (&v
             if (c) { ok[j] = false; my_hits += (c == 1); }
         }
     }
+    ha_probe_rows(t, ctl, k, ok, h, my_inserts, [&](u64 sl, int j) {
+        op_red_hint<OPK>(&t.accs[sl], v[j], tpol);
+        if (OPK == OPK_DICT) st_stream_u32(slot_out + row0 + (u64)j * HA_THREADS, (u32)sl);
+    });
+}
+
+// Lockstep probe/insert of the pending rows (ok[j]) of one thread, with hashes h[j]; on_hit(slot, j) once per
+// resolved row.  A probe chain longer than HA_MAX_PROBE buckets raises the table's abort flag.
+template <int ROWS, class OnHit>
+VB_D void ha_probe_rows(const Table &t, TableCtl *ctl, const u64 (&k)[ROWS], bool (&ok)[ROWS], const u64 (&h)[ROWS], u32 &my_inserts,
+                        OnHit &&on_hit)
+{
+    const u64 tpol = table_policy();
+    const u32 hshift = 64 - (t.log_cap - 2);
     // Probe rounds run in lockstep over the ROWS rows of a thread: every round first consumes the
     // buckets loaded by the previous one, then issues the next probes of all unresolved rows together,
     // so a tile costs max-over-rows (not sum-over-rows) dependent L2 latencies.
@@ -281,9 +308,7 @@ VB_D void ha_process_rows(const Table &t, TableCtl *ctl, u64 (&k)[ROWS], u64 (&v
                 }
             }
             if (hit >= 0) {
-                const u64 sl = 4 * bidx[j] + (u64)hit;
-                op_red_hint<OPK>(&t.accs[sl], v[j], tpol);
-                if (OPK == OPK_DICT) st_stream_u32(slot_out + row0 + (u64)j * HA_THREADS, (u32)sl);
+                on_hit(4 * bidx[j] + (u64)hit, j);
                 ok[j] = false;
             } else {
                 pending = true;
@@ -546,6 +571,371 @@ hash_agg_bulk_kernel(const u64 *__restrict__ a, const u64 *__restrict__ b, u64 n
     if ((tid & 31u) == 0 && w) atomicAdd(&s_inserts, w);
     named_bar_sync(1, HA_THREADS);
     if (tid == 0 && s_inserts) atomicAdd(&ctl->n_inserted, (unsigned long long)s_inserts);
+}
+
+// ---- several aggregates per key (combine_by_key) -------------------------------------------------------
+// Table: keys[cap + 4], then n accumulator columns accs[a][cap + 4] (column a at t.accs + a * (cap + 4)), each
+// kept apart from the keys and from each other for the same reason the single-column table is not interleaved.
+// A row costs one probe/insert (ha_probe_rows, shared with the kernels above) and then one RED per accumulator.
+// Up to MA_MAX_COLS input value columns; the column count is a template parameter (register arrays are only
+// indexed by compile-time indices: an accumulator picks its column with an unrolled compare chain), the
+// accumulator list (op, order transform, input column) is a kernel argument read from parameter space.
+constexpr int MA_MAX_COLS = 4;
+constexpr int MA_MAX_ACCS = 8;
+// One byte per accumulator, packed into a u64 so a run-time accumulator index is a shift, not a local-memory array.
+struct AccSpec {
+    u32 n;      // accumulators
+    u64 op;     // OPK_ADD_U64 / OPK_ADD_F64 / OPK_MIN_U64 / OPK_MAX_U64 / OPK_COUNT
+    u64 tx;     // order transform on load (MIN/MAX over i64 / f64; NaN -> identity for f64)
+    u64 src;    // input value column (table merges: accumulator a reads source column a)
+};
+VB_HD int spec_at(u64 packed, int a) { return (int)(packed >> (8 * a)) & 0xFF; }
+VB_HD void spec_set(u64 &packed, int a, int v) { packed = (packed & ~(0xFFull << (8 * a))) | ((u64)(v & 0xFF) << (8 * a)); }
+struct MaCols {
+    const u64 *c[MA_MAX_COLS];           // value columns (IN_TABLE: c[0] = the source table's first accumulator column)
+    u64 stride;                          // IN_TABLE: distance between the source's accumulator columns
+};
+VB_HD size_t table_bytes_multi(u32 log_cap, u32 n_acc) { return (((size_t)1 << log_cap) + BUCKET) * 8 * (1 + n_acc); }
+VB_HD u64 acc_stride(u32 log_cap) { return (1ull << log_cap) + BUCKET; }
+
+// Hot-key cache of the multi kernels: 512 slots x (key + n partials) in dynamic shared memory (36 KB at 8
+// accumulators), so that stage + cache of the bulk variant still fit two CTAs per SM at 4 value columns.
+constexpr u32 MA_HC_SLOTS = 512;
+VB_HD size_t ma_cache_bytes(u32 n_acc) { return (size_t)MA_HC_SLOTS * 8 * (1 + n_acc); }
+// Rows per thread: 4 with one value column, 2 with more (the tile's values live in registers until the REDs; the
+// bulk kernel spilled at 2 columns x 4 rows under its 2-CTA register budget).
+template <int NV> constexpr int ma_rows() { return NV == 1 ? 4 : 2; }
+#ifndef VB_MA_STAGES
+#define VB_MA_STAGES 3
+#endif
+constexpr int MA_STAGES = VB_MA_STAGES;
+template <int NV> constexpr size_t ma_stage_bytes() { return (size_t)HA_THREADS * ma_rows<NV>() * 8 * (1 + NV); }
+template <int NV> constexpr size_t ma_bulk_smem(u32 n_acc) { return MA_STAGES * ma_stage_bytes<NV>() + ma_cache_bytes(n_acc); }
+
+// one RED with a run-time op (warp-uniform: every lane runs the same accumulator list); global or shared memory
+VB_D void op_red_rt(u64 *acc, int opk, u64 v)
+{
+    switch (opk) {
+    case OPK_ADD_U64: atomicAdd((unsigned long long *)acc, (unsigned long long)v); break;
+    case OPK_ADD_F64: atomicAdd((double *)acc, __longlong_as_double((long long)v)); break;
+    case OPK_MIN_U64: atomicMin((unsigned long long *)acc, (unsigned long long)v); break;
+    case OPK_MAX_U64: atomicMax((unsigned long long *)acc, (unsigned long long)v); break;
+    default: atomicAdd((unsigned long long *)acc, 1ull); break;       // OPK_COUNT
+    }
+}
+VB_HD int merge_op(int opk) { return opk == OPK_COUNT ? OPK_ADD_U64 : opk; }   // partial counts are summed
+
+template <int NV, int ROWS>
+VB_D u64 ma_pick(const u64 (&v)[NV][ROWS], int src, int j)
+{
+    u64 x = v[0][j];
+#pragma unroll
+    for (int c = 1; c < NV; ++c)
+        if (src == c) x = v[c][j];
+    return x;
+}
+// the value accumulator `a` folds: order transform, and a NaN becomes the identity of f64 MIN/MAX (tx is set only for MIN/MAX)
+VB_D u64 ma_prep(u64 x, int opk, int tx)
+{
+    if (tx == TX_F64 && (x & 0x7FFFFFFFFFFFFFFFull) > 0x7FF0000000000000ull) return op_identity(opk);
+    return tx_fwd(x, tx);
+}
+
+__global__ void table_init_multi_kernel(Table t, AccSpec sp)
+{
+    const u64 cap = 1ull << t.log_cap, stride = acc_stride(t.log_cap);
+    u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    const u64 step = (u64)gridDim.x * blockDim.x;
+    for (; i < stride; i += step) {
+        t.keys[i] = (i >= cap) ? 0ull : EMPTY_KEY;
+        for (int a = 0; a < (int)sp.n; ++a) t.accs[(u64)a * stride + i] = op_identity(spec_at(sp.op, a));
+    }
+}
+
+// Special key, hot-key cache, probe + one RED per accumulator for ROWS rows of a thread.  IN_SOA: v[c][j] is the
+// value of column c; IN_TABLE (merge): v[0][j] is the source slot, whose accumulators are read at the RED.
+template <int IN, int NV, int ROWS, bool CACHE>
+VB_D void ma_process_rows(const Table &t, TableCtl *ctl, const AccSpec &sp, const MaCols &src, u64 (&k)[ROWS], u64 (&v)[NV][ROWS],
+                          bool (&ok)[ROWS], u64 *hc_keys, u64 *hc_acc, bool use_cache, u32 &my_inserts, u32 &my_hits)
+{
+    const u64 cap = 1ull << t.log_cap, stride = acc_stride(t.log_cap);
+    const u64 ops = sp.op, txs = sp.tx, srcs = sp.src;
+    const int n_acc = (int)sp.n;
+    // not unrolled: 8 accumulators x ROWS rows x 3 call sites of an unrolled RED chain spilled
+    auto red_all = [&](u64 *base, u64 col_stride, int j) {
+#pragma unroll 1
+        for (int a = 0; a < n_acc; ++a) {
+            const int op = spec_at(ops, a);
+            const u64 x = IN == IN_TABLE ? ld_cg_u64(src.c[0] + (u64)a * src.stride + v[0][j])
+                                         : ma_prep(ma_pick<NV, ROWS>(v, spec_at(srcs, a), j), op, spec_at(txs, a));
+            op_red_rt(base + (u64)a * col_stride, op, x);
+        }
+    };
+    u64 h[ROWS];
+#pragma unroll
+    for (int j = 0; j < ROWS; ++j) {
+        h[j] = slot_hash(k[j]);
+        if (ok[j] && k[j] == EMPTY_KEY) {           // a real key equal to the empty marker: special slot
+            t.keys[cap] = 1ull;
+            red_all(t.accs + cap, stride, j);
+            ok[j] = false;
+        }
+    }
+    if (CACHE && use_cache) {
+#pragma unroll
+        for (int j = 0; j < ROWS; ++j) {
+            if (!ok[j]) continue;
+            const int c = cache_combine_with<MA_HC_SLOTS>(hc_keys, h[j], k[j], [&](u32 i) { red_all(hc_acc + i, MA_HC_SLOTS, j); });
+            if (c) { ok[j] = false; my_hits += (c == 1); }
+        }
+    }
+    ha_probe_rows(t, ctl, k, ok, h, my_inserts, [&](u64 sl, int j) { red_all(t.accs + sl, stride, j); });
+}
+
+template <u32 NT>
+VB_D void ma_cache_init(u64 *hc_keys, u64 *hc_acc, const AccSpec &sp, u32 tid)
+{
+    for (u32 i = tid; i < MA_HC_SLOTS; i += NT) {
+        hc_keys[i] = EMPTY_KEY;
+        for (int a = 0; a < (int)sp.n; ++a) hc_acc[a * MA_HC_SLOTS + i] = op_identity(spec_at(sp.op, a));
+    }
+}
+// flush the CTA's cached partials into the table, combined with each accumulator's merge op
+VB_D void ma_cache_flush(const Table &t, TableCtl *ctl, const AccSpec &sp, const u64 *hc_keys, const u64 *hc_acc, u32 tid, u32 &my_inserts)
+{
+    const u64 stride = acc_stride(t.log_cap);
+    for (u32 i = tid; i < MA_HC_SLOTS; i += HA_THREADS) {
+        const u64 key = hc_keys[i];
+        if (key == EMPTY_KEY) continue;
+        const u64 hb = home_bucket(key, t.log_cap);
+        if (!table_resolve_with(t, hb, ld_bucket(&t.keys[4 * hb]), key, my_inserts, [&](u64 s) {
+                for (int a = 0; a < (int)sp.n; ++a) op_red_rt(t.accs + (u64)a * stride + s, merge_op(spec_at(sp.op, a)), hc_acc[a * MA_HC_SLOTS + i]);
+            }))
+            atomicExch(&ctl->abort, 1u);
+    }
+}
+
+// Periodic load-factor check of the multi kernels (+ the cache verdict after the first 16 tiles), over the
+// HA_THREADS consumer threads (named barrier 1).  Returns true when the table overflowed (host restarts larger).
+template <bool CACHE>
+VB_D bool ma_check(TableCtl *ctl, u64 max_inserts, u32 iter, u32 tile_rows, u32 &my_inserts, u32 my_hits, bool &use_cache, u32 *s_inserts,
+                   u32 *s_hits, u32 *s_abort)
+{
+    const u32 tid = threadIdx.x;
+    u32 w = __reduce_add_sync(0xffffffffu, my_inserts);
+    my_inserts = 0;
+    if ((tid & 31u) == 0 && w) atomicAdd(s_inserts, w);
+    if (CACHE && iter == 15u) {
+        u32 hw = __reduce_add_sync(0xffffffffu, my_hits);
+        if ((tid & 31u) == 0 && hw) atomicAdd(s_hits, hw);
+    }
+    named_bar_sync(1, HA_THREADS);
+    if (tid == 0) {
+        u32 c = *s_inserts;
+        *s_inserts = 0;
+        u64 tot = atomicAdd(&ctl->n_inserted, (unsigned long long)c) + c;
+        u32 ab = ld_volatile_u32(&ctl->abort);
+        if (tot > max_inserts) { ab = 1; atomicExch(&ctl->abort, 1u); }
+        *s_abort = ab;
+    }
+    named_bar_sync(1, HA_THREADS);
+    if (CACHE && iter == 15u && *s_hits * 16u < 16u * tile_rows) use_cache = false;   // < 1/16 of the first 16 tiles
+    return *s_abort != 0;
+}
+
+// Register-staged multi-aggregate combine: IN_SOA (keys + NV value columns) or IN_TABLE (merge of a per-map
+// table of the same spec: NV = 1, sp = the merge spec).  Dynamic shared memory: the hot-key cache (IN_SOA).
+template <int IN, int NV>
+__global__ void __launch_bounds__(HA_THREADS, 2)
+hash_agg_multi_kernel(const u64 *__restrict__ keys, MaCols cols, u64 n, Table t, AccSpec sp, TableCtl *ctl, u64 max_inserts)
+{
+    static_assert(IN == IN_SOA || (IN == IN_TABLE && NV == 1), "SoA rows or a table merge");
+    constexpr bool CACHE = VB_HC_ENABLE && (IN != IN_TABLE);
+    constexpr int ROWS = ma_rows<NV>();
+    constexpr int TILE = HA_THREADS * ROWS;
+    extern __shared__ __align__(16) u64 ma_cache[];          // hc_keys[MA_HC_SLOTS], hc_acc[n][MA_HC_SLOTS]
+    __shared__ u32 s_inserts, s_abort, s_hits;
+    u64 *hc_keys = ma_cache, *hc_acc = ma_cache + MA_HC_SLOTS;
+    const u32 tid = threadIdx.x;
+    if (tid == 0) { s_inserts = 0; s_abort = 0; s_hits = 0; }
+    if (CACHE) ma_cache_init<HA_THREADS>(hc_keys, hc_acc, sp, tid);
+    __syncthreads();
+    const u64 pol = policy_evict_first();
+    const u64 n_tiles = (n + TILE - 1) / TILE;
+    u32 my_inserts = 0, my_hits = 0, iter = 0;
+    bool use_cache = CACHE;
+    for (u64 tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++iter) {
+        const u64 base = tile * TILE;
+        u64 k[ROWS], v[NV][ROWS];
+        bool ok[ROWS];
+#pragma unroll
+        for (int j = 0; j < ROWS; ++j) {
+            const u64 idx = base + (u64)j * HA_THREADS + tid;
+            ok[j] = idx < n;
+            k[j] = 0;
+#pragma unroll
+            for (int c = 0; c < NV; ++c) v[c][j] = 0;
+            if (ok[j]) {
+                k[j] = ld_stream_u64(keys + idx, pol);
+                if (IN == IN_SOA) {
+#pragma unroll
+                    for (int c = 0; c < NV; ++c)
+                        if (cols.c[c]) v[c][j] = ld_stream_u64(cols.c[c] + idx, pol);
+                } else {
+                    v[0][j] = idx;
+                    if (idx == n - 1) { ok[j] = (k[j] == 1ull); k[j] = EMPTY_KEY; }   // special slot
+                    else if (k[j] == EMPTY_KEY) ok[j] = false;                       // unoccupied
+                }
+            }
+        }
+        ma_process_rows<IN, NV, ROWS, CACHE>(t, ctl, sp, cols, k, v, ok, hc_keys, hc_acc, use_cache, my_inserts, my_hits);
+        if ((iter & 15u) == 15u && ma_check<CACHE>(ctl, max_inserts, iter, TILE, my_inserts, my_hits, use_cache, &s_inserts, &s_hits, &s_abort))
+            return;
+    }
+    if (CACHE) {
+        __syncthreads();
+        ma_cache_flush(t, ctl, sp, hc_keys, hc_acc, tid, my_inserts);
+    }
+    u32 w = __reduce_add_sync(0xffffffffu, my_inserts);
+    if ((tid & 31u) == 0 && w) atomicAdd(&s_inserts, w);
+    __syncthreads();
+    if (tid == 0 && s_inserts) atomicAdd(&ctl->n_inserted, (unsigned long long)s_inserts);
+}
+
+// Bulk-staged (copy engine) multi-aggregate combine over SoA keys + NV value columns: the producer warp stages
+// the keys and every value column of a tile with cp.async.bulk (MA_STAGES tiles in flight), the 8 consumer warps
+// probe and RED, as hash_agg_bulk_kernel.  Dynamic shared memory: [MA_STAGES][keys | col 0 | ... | col NV-1], then
+// the hot-key cache.  Full 16-byte aligned tiles only; the sub-tile tail is read with plain loads.
+template <int NV>
+__global__ void __launch_bounds__(HB_THREADS, 2)
+hash_agg_multi_bulk_kernel(const u64 *__restrict__ keys, MaCols cols, u64 n, Table t, AccSpec sp, TableCtl *ctl, u64 max_inserts)
+{
+    constexpr bool CACHE = VB_HC_ENABLE;
+    constexpr int ROWS = ma_rows<NV>();
+    constexpr int TILE = HA_THREADS * ROWS;
+    constexpr u32 STAGE_BYTES = (u32)ma_stage_bytes<NV>();
+    extern __shared__ __align__(128) unsigned char ma_stage[];
+    __shared__ __align__(8) u64 full_bar[MA_STAGES];
+    __shared__ __align__(8) u64 empty_bar[MA_STAGES];
+    __shared__ u32 s_inserts, s_abort, s_hits;
+    u64 *hc_keys = (u64 *)(ma_stage + (size_t)MA_STAGES * STAGE_BYTES), *hc_acc = hc_keys + MA_HC_SLOTS;
+    const u32 tid = threadIdx.x;
+    if (tid == 0) {
+        s_inserts = 0; s_abort = 0; s_hits = 0;
+#pragma unroll
+        for (int s = 0; s < MA_STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], HA_THREADS / 32); }
+        mbar_fence_init();
+    }
+    if (CACHE) ma_cache_init<HB_THREADS>(hc_keys, hc_acc, sp, tid);
+    __syncthreads();
+    const u64 n_full = n / TILE;
+
+    if (tid >= HA_THREADS) {                                // ===== producer warp =====
+        if (tid == HA_THREADS) {
+            const u64 pol = policy_evict_first();
+            u32 i = 0;
+            for (u64 tile = blockIdx.x; tile < n_full; tile += gridDim.x, ++i) {
+                const u32 s = i % MA_STAGES;
+                if (i >= MA_STAGES) mbar_wait(&empty_bar[s], ((i / MA_STAGES) & 1u) ^ 1u);
+                unsigned char *dst = ma_stage + (size_t)s * STAGE_BYTES;
+                u32 bytes = TILE * 8;
+#pragma unroll
+                for (int c = 0; c < NV; ++c) bytes += cols.c[c] ? TILE * 8 : 0;
+                mbar_arrive_expect_tx(&full_bar[s], bytes);
+                bulk_g2s(dst, keys + tile * TILE, TILE * 8, &full_bar[s], pol);
+#pragma unroll
+                for (int c = 0; c < NV; ++c)
+                    if (cols.c[c]) bulk_g2s(dst + (size_t)(1 + c) * TILE * 8, cols.c[c] + tile * TILE, TILE * 8, &full_bar[s], pol);
+            }
+        }
+        return;
+    }
+
+    // ===== consumer warps =====
+    u32 my_inserts = 0, my_hits = 0, iter = 0;
+    bool use_cache = CACHE;
+    bool drain = false;        // after an abort: keep the pipeline moving (copies in flight target this CTA's smem), skip the work
+    for (u64 tile = blockIdx.x; tile < n_full; tile += gridDim.x, ++iter) {
+        const u32 s = iter % MA_STAGES;
+        mbar_wait(&full_bar[s], (iter / MA_STAGES) & 1u);
+        const u64 *src = reinterpret_cast<const u64 *>(ma_stage + (size_t)s * STAGE_BYTES);
+        u64 k[ROWS], v[NV][ROWS];
+        bool ok[ROWS];
+#pragma unroll
+        for (int j = 0; j < ROWS; ++j) {
+            const u32 r = (u32)j * HA_THREADS + tid;
+            ok[j] = !drain;
+            k[j] = src[r];
+#pragma unroll
+            for (int c = 0; c < NV; ++c) v[c][j] = cols.c[c] ? src[(1 + c) * TILE + r] : 0ull;
+        }
+        fence_proxy_async();        // generic-proxy reads ordered before the slot is refilled by the async proxy
+        __syncwarp();
+        if ((tid & 31u) == 0) mbar_arrive(&empty_bar[s]);
+        if (!drain) ma_process_rows<IN_SOA, NV, ROWS, CACHE>(t, ctl, sp, cols, k, v, ok, hc_keys, hc_acc, use_cache, my_inserts, my_hits);
+        if ((iter & 15u) == 15u && ma_check<CACHE>(ctl, max_inserts, iter, TILE, my_inserts, my_hits, use_cache, &s_inserts, &s_hits, &s_abort))
+            drain = true;
+    }
+    if (!drain && (n % TILE) && blockIdx.x == (u32)(n_full % gridDim.x)) {   // tail: plain loads
+        const u64 pol = policy_evict_first();
+        const u64 base = n_full * TILE;
+        u64 k[ROWS], v[NV][ROWS];
+        bool ok[ROWS];
+#pragma unroll
+        for (int j = 0; j < ROWS; ++j) {
+            const u64 idx = base + (u64)j * HA_THREADS + tid;
+            ok[j] = idx < n;
+            k[j] = 0;
+#pragma unroll
+            for (int c = 0; c < NV; ++c) v[c][j] = 0;
+            if (ok[j]) {
+                k[j] = ld_stream_u64(keys + idx, pol);
+#pragma unroll
+                for (int c = 0; c < NV; ++c)
+                    if (cols.c[c]) v[c][j] = ld_stream_u64(cols.c[c] + idx, pol);
+            }
+        }
+        ma_process_rows<IN_SOA, NV, ROWS, CACHE>(t, ctl, sp, cols, k, v, ok, hc_keys, hc_acc, use_cache, my_inserts, my_hits);
+    }
+    if (CACHE) {
+        named_bar_sync(1, HA_THREADS);
+        if (!drain) ma_cache_flush(t, ctl, sp, hc_keys, hc_acc, tid, my_inserts);
+    }
+    u32 w = __reduce_add_sync(0xffffffffu, my_inserts);
+    if ((tid & 31u) == 0 && w) atomicAdd(&s_inserts, w);
+    named_bar_sync(1, HA_THREADS);
+    if (tid == 0 && s_inserts) atomicAdd(&ctl->n_inserted, (unsigned long long)s_inserts);
+}
+
+// Finalize: output column o of row i (key slot slots[i]) from the table.  kind 0: the accumulator with the inverse
+// order transform; MEAN: sum / count as f64, the sum read as u64 (1), i64 (2) or f64 (3).
+enum : int { MO_COPY = 0, MO_MEAN_U64 = 1, MO_MEAN_I64 = 2, MO_MEAN_F64 = 3 };
+struct OutSpec {
+    u32 n;
+    unsigned char acc[MA_MAX_ACCS], cnt[MA_MAX_ACCS], kind[MA_MAX_ACCS], tx[MA_MAX_ACCS];
+};
+__global__ void multi_finalize_kernel(const u64 *__restrict__ accs, u64 stride, const u64 *__restrict__ slots, u64 d, OutSpec os,
+                                      u64 *__restrict__ out)
+{
+    const u64 step = (u64)gridDim.x * blockDim.x;
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < d; i += step) {
+        const u64 sl = slots[i];
+#pragma unroll
+        for (int o = 0; o < MA_MAX_ACCS; ++o) {
+            if (o >= (int)os.n) break;
+            const u64 x = accs[(u64)os.acc[o] * stride + sl];
+            u64 r;
+            if (os.kind[o] == MO_COPY) {
+                r = tx_inv(x, os.tx[o]);
+            } else {
+                const double cnt = (double)accs[(u64)os.cnt[o] * stride + sl];
+                const double sum = os.kind[o] == MO_MEAN_U64 ? (double)x
+                                 : os.kind[o] == MO_MEAN_I64 ? (double)(long long)x : __longlong_as_double((long long)x);
+                r = (u64)__double_as_longlong(sum / cnt);
+            }
+            out[(u64)o * d + i] = r;
+        }
+    }
 }
 
 // Strided key sample for the distinct-count estimate that sizes the first table.

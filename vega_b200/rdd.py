@@ -23,6 +23,7 @@ from . import _lib as L
 _AGG = {"group": L.VB_AGG_GROUP, "sum": L.VB_AGG_SUM, "min": L.VB_AGG_MIN, "max": L.VB_AGG_MAX,
         "count": L.VB_AGG_COUNT, "cogroup": L.VB_AGG_COGROUP, "sort": L.VB_AGG_SORT}
 _NP_OF = {L.VB_U64: np.uint64, L.VB_I64: np.int64, L.VB_F64: np.float64}
+_COMBINE_OPS = {"sum": L.VB_AGG_SUM, "min": L.VB_AGG_MIN, "max": L.VB_AGG_MAX, "count": L.VB_AGG_COUNT, "mean": L.VB_AGG_MEAN}
 
 
 def _is_torch(x):
@@ -140,7 +141,12 @@ class Context:
 
     def parallelize(self, data, num_slices, values=None):
         """`sc.parallelize(vec, num_slices)`.  data: 1-D keys (→ Rdd), (n,2) rows or
-        (keys, values) (→ PairRdd)."""
+        (keys, values) (→ PairRdd).  values may also be a tuple of up to 4 value columns (combine_by_key)."""
+        if isinstance(values, tuple):                 # a list stays one value column, as before
+            if not 1 <= len(values) <= L.VB_MAX_VAL_COLS:
+                raise ValueError(f"{len(values)} value columns: 1 to {L.VB_MAX_VAL_COLS} are supported")
+            cols = tuple(_Col(v, role="value") for v in values)
+            return PairRdd(self, _Col(data), cols[0] if len(cols) == 1 else None, num_slices, cols=cols)
         if values is not None:
             return PairRdd(self, _Col(data), _Col(values, role="value"), num_slices)
         if isinstance(data, tuple) and len(data) == 2:
@@ -219,14 +225,22 @@ class Context:
 class Shuffle:
     """Thin RAII wrapper of one vb_shuf (== one ShuffleDependency / shuffle_id)."""
 
-    def __init__(self, sc, n_map, n_reduce, kcode, vcode, agg, key_width=8, hint=0, rank=0, world=1):
+    def __init__(self, sc, n_map, n_reduce, kcode, vcode, agg, key_width=8, hint=0, rank=0, world=1, multi=None):
+        """multi: (value column dtype codes, [(vb_agg, column), ...]) for a vb_shuffle_create_multi shuffle."""
         self.sc, self._lib = sc, sc._lib
         self.n_map, self.n_reduce, self.agg, self.vcode, self.kcode = n_map, n_reduce, agg, vcode, kcode
         self.has_payload = True
         self._keepalive = []      # owners of VB_DEVICE_BORROWED inputs: the library reads them until seal
         h = ctypes.c_void_p()
-        part = L.VB_PART_RANGE if agg == L.VB_AGG_SORT else L.VB_PART_HASH_METRO64
-        L.check(self._lib.vb_shuffle_create(sc._h, sc.new_shuffle_id(), n_map, n_reduce, kcode, vcode, agg, part, ctypes.byref(h)))
+        if multi is not None:
+            codes, aggs = multi
+            dts = (ctypes.c_int32 * len(codes))(*codes)
+            spec = (L.vb_agg_col * len(aggs))(*[L.vb_agg_col(a, c) for a, c in aggs])
+            L.check(self._lib.vb_shuffle_create_multi(sc._h, sc.new_shuffle_id(), n_map, n_reduce, kcode, len(codes), dts,
+                                                      len(aggs), spec, ctypes.byref(h)))
+        else:
+            part = L.VB_PART_RANGE if agg == L.VB_AGG_SORT else L.VB_PART_HASH_METRO64
+            L.check(self._lib.vb_shuffle_create(sc._h, sc.new_shuffle_id(), n_map, n_reduce, kcode, vcode, agg, part, ctypes.byref(h)))
         self._h = h
         sc._shuffles.add(self)
         if key_width != 8:
@@ -247,6 +261,31 @@ class Shuffle:
             if vals is not None and vals.loc != keys.loc:
                 raise ValueError("keys and values must live in the same memory space")
             L.check(self._lib.vb_shuffle_map_soa(self._h, map_id, keys.at(start), vals.at(start) if vals is not None else None, n, keys.loc))
+
+    def map_cols(self, map_id, keys, cols, start, stop):
+        """One map partition of a multi-aggregate shuffle: rows [start, stop) of keys and every value column."""
+        if any(c.loc != keys.loc for c in cols):
+            raise ValueError("keys and values must live in the same memory space")
+        if keys.loc == L.VB_DEVICE_BORROWED:
+            self._keepalive.append((keys.owner,) + tuple(c.owner for c in cols))
+        ptrs = (ctypes.c_void_p * len(cols))(*[c.at(start) for c in cols])
+        L.check(self._lib.vb_shuffle_map_cols(self._h, map_id, keys.at(start), ptrs, stop - start, keys.loc))
+
+    def reduce_cols(self, r, out_dtypes, dst_loc=L.VB_HOST, out_keys=None, out_aggs=None):
+        """Reduce partition r of a multi-aggregate shuffle → (keys, [one array per aggregate]) on the host, or into
+        caller-provided torch CUDA tensors with dst_loc=VB_DEVICE (any may be None)."""
+        if dst_loc == L.VB_DEVICE:
+            _sync_torch(out_keys, *(out_aggs or []))
+            p = lambda t: t.data_ptr() if t is not None else None
+            ptrs = (ctypes.c_void_p * len(out_aggs))(*[p(t) for t in out_aggs])
+            L.check(self._lib.vb_shuffle_reduce_cols(self._h, r, p(out_keys), ptrs, L.VB_DEVICE))
+            return out_keys, out_aggs
+        nk, _ = self.reduce_size(r)
+        keys = np.empty(nk, dtype=_NP_OF[self.kcode])
+        outs = [np.empty(nk, dtype=dt) for dt in out_dtypes]
+        ptrs = (ctypes.c_void_p * len(outs))(*[o.ctypes.data for o in outs])
+        L.check(self._lib.vb_shuffle_reduce_cols(self._h, r, keys.ctypes.data_as(ctypes.c_void_p), ptrs, L.VB_HOST))
+        return keys, outs
 
     def exchange(self, mode=L.VB_XCHG_AUTO):
         """The shuffle's exchange step inside the library (collective; needs Context.comm_init)."""
@@ -358,6 +397,8 @@ class ShuffledRdd(_Base):
     def __init__(self, parent, agg_name, num_splits, hint=0):
         if num_splits < 1:
             raise ValueError("num_splits must be >= 1")
+        if len(getattr(parent, "cols", ())) > 1:
+            raise TypeError("a PairRdd with several value columns supports combine_by_key only")
         self.parent, self.agg_name, self.num_slices, self.hint = parent, agg_name, num_splits, hint
         self.sc = parent.sc
         self._sh = None
@@ -448,15 +489,90 @@ class JoinedRdd(_Base):
         return out
 
 
+class CombinedRdd(_Base):
+    """`combine_by_key` with named aggregates (src/rdd/pair_rdd.rs:20-33): one shuffle, several aggregates per key.
+    `compute(r)` / `collect()` return (keys, {name: array}) with the aggregates in the order they were given."""
+
+    def __init__(self, parent, aggs, num_splits, hint=0):
+        if num_splits < 1:
+            raise ValueError("num_splits must be >= 1")
+        if not hasattr(aggs, "items") or not aggs:
+            raise ValueError("aggs must be a non-empty mapping name -> (op, column)")
+        cols = parent.cols
+        spec, names = [], []
+        for name, item in aggs.items():
+            if not isinstance(item, (tuple, list)) or len(item) != 2:
+                raise ValueError(f"aggregate {name!r}: expected (op, column), got {item!r}")
+            op, col = item
+            if op not in _COMBINE_OPS:
+                raise ValueError(f"aggregate {name!r}: op {op!r} is not one of {sorted(_COMBINE_OPS)}")
+            if op == "count":
+                col = 0
+            elif not isinstance(col, (int, np.integer)) or isinstance(col, bool) or not 0 <= col < len(cols):
+                raise ValueError(f"aggregate {name!r}: column {col!r} out of range for {len(cols)} value columns")
+            spec.append((_COMBINE_OPS[op], int(col)))
+            names.append(name)
+        ops = [op for op, _ in aggs.values()]
+        n_acc = len(ops) + (1 if "mean" in ops and "count" not in ops else 0)
+        if n_acc > L.VB_MAX_AGGS:
+            raise ValueError(f"{len(ops)} aggregates{' plus the count a mean needs' if n_acc > len(ops) else ''} "
+                             f"exceed {L.VB_MAX_AGGS}")
+        self.parent, self.num_slices, self.hint, self.sc = parent, num_splits, hint, parent.sc
+        self.spec, self.names = spec, names
+        self.out_dtypes = [np.uint64 if a == L.VB_AGG_COUNT else np.float64 if a == L.VB_AGG_MEAN else _NP_OF[cols[c].code]
+                           for a, c in spec]
+        self._sh = None
+
+    def _run(self):
+        if self._sh is not None:
+            return self._sh
+        p = self.parent
+        starts = slice_starts(p.n, p.num_slices)
+        sh = Shuffle(self.sc, len(starts) - 1, self.num_slices, p.keys.code, L.VB_U64, L.VB_AGG_SUM, key_width=p.keys.key_width,
+                     hint=self.hint, multi=([c.code for c in p.cols], self.spec))
+        for m in range(len(starts) - 1):
+            sh.map_cols(m, p.keys, p.cols, int(starts[m]), int(starts[m + 1]))
+        sh.seal()
+        self._sh = sh
+        return sh
+
+    def compute(self, split):
+        keys, outs = self._run().reduce_cols(split, self.out_dtypes)
+        return keys, dict(zip(self.names, outs))
+
+    def collect(self):
+        parts = [self.compute(r) for r in range(self.num_slices)]
+        return (np.concatenate([p[0] for p in parts]),
+                {name: np.concatenate([p[1][name] for p in parts]) for name in self.names})
+
+    def stats(self):
+        return self._run().stats()
+
+
 class PairRdd(_Base):
     """PairRdd<K,V> source (ParallelCollection of (K,V)); methods per src/rdd/pair_rdd.rs."""
 
-    def __init__(self, sc, keys, vals, num_slices):
+    def __init__(self, sc, keys, vals, num_slices, cols=None):
         if num_slices < 1:
             raise ValueError("Number of slices should be greater than or equal to 1")
         if vals is not None and vals.n != keys.n:
             raise ValueError("keys and values differ in length")
+        if cols is not None and any(c.n != keys.n for c in cols):
+            raise ValueError("keys and value columns differ in length")
+        if cols is not None and any(c.loc != keys.loc for c in cols):
+            raise ValueError("keys and values must live in the same memory space")
         self.sc, self.keys, self.vals, self.num_slices, self.n = sc, keys, vals, num_slices, keys.n
+        self.cols = cols if cols is not None else ((vals,) if vals is not None else ())
+
+    def combine_by_key(self, aggs, num_splits, hint=0):
+        """Several named aggregates per key in one shuffle.  aggs: ordered mapping name -> (op, column) with op in
+        "sum" | "min" | "max" | "count" | "mean" and column an index into the value columns (ignored by "count"), e.g.
+        {"n": ("count", None), "avg": ("mean", 0), "hi": ("max", 1)}."""
+        if not self.cols:
+            raise ValueError("combine_by_key needs value columns")
+        if self.keys.rows:
+            raise ValueError("combine_by_key takes keys and value columns, not (n,2) rows")
+        return CombinedRdd(self, aggs, num_splits, hint)
 
     def group_by_key(self, num_splits):
         return ShuffledRdd(self, "group", num_splits)
