@@ -17,6 +17,7 @@
  *                             + ShuffleFetcher::fetch             src/shuffle/shuffle_fetcher.rs:16-119
  *   vb_join*               <- CoGroupedRdd::compute               src/rdd/co_grouped_rdd.rs:206-249
  *                             + PairRdd::join cross product       src/rdd/pair_rdd.rs:104-121
+ *   vb_join_outer*         <- nothing: vega has no outer joins (Spark's left/right/full outer join, new)
  *   vb_shuffle_free        <- (the reference never evicts SHUFFLE_CACHE, src/env.rs:27)
  *   vb_slice               <- ParallelCollection::slice           src/rdd/parallel_collection_rdd.rs:116-145
  *   vb_shuffle_export_* / vb_shuffle_import
@@ -274,6 +275,23 @@ VB_API int32_t vb_shuffle_reduce_cols(vb_shuf *s, uint32_t reduce_id, void *out_
 VB_API int32_t vb_join_size(vb_shuf *left, vb_shuf *right, uint32_t reduce_id, uint64_t *n_out);
 VB_API int32_t vb_join(vb_shuf *left, vb_shuf *right, uint32_t reduce_id, void *out_k, void *out_v, void *out_w,
                        int32_t dst_loc);
+
+/* Outer joins (Spark's leftOuterJoin / rightOuterJoin / fullOuterJoin; the reference has none, so there is no
+ * reference output to compare against).  Same arguments and rules as vb_join, plus the kind (VB_ERR_INVALID for any
+ * other value: the inner join is vb_join).  For a key with left values vs and right values ws, each in cogroup order:
+ *   key on both sides     for v in vs { for w in ws } -> (k, v, w)          every kind
+ *   key only on the left  (k, v, None) for each v                           LEFT, FULL
+ *   key only on the right (k, None, w) for each w                           RIGHT, FULL
+ * so a key gives max(|vs|,1) * max(|ws|,1) rows on the kept sides.  A key's rows are contiguous, in that order; the
+ * order of keys within the partition is unspecified.  A None slot holds 0 and its validity byte is 0.
+ * out_v_valid / out_w_valid (one byte per row, same dst_loc) are optional: when given, they are written for every
+ * row, including the 1s of a side that is always present.  On a rank of a multi-rank shuffle only the partitions
+ * that rank owns have rows.                                                                                       */
+enum vb_join_kind { VB_JOIN_LEFT = 1, VB_JOIN_RIGHT = 2, VB_JOIN_FULL = 3 };
+VB_API int32_t vb_join_outer_size(vb_shuf *left, vb_shuf *right, uint32_t reduce_id, int32_t kind, uint64_t *n_out);
+VB_API int32_t vb_join_outer(vb_shuf *left, vb_shuf *right, uint32_t reduce_id, int32_t kind,
+                             void *out_k, void *out_v, void *out_w,
+                             uint8_t *out_v_valid, uint8_t *out_w_valid, int32_t dst_loc);
 
 /* ---- SURVEY §8(f) N1: bincode blobs — the payload format of SHUFFLE_CACHE ------------------------
  * The reference serialises every (map, reduce) bucket with bincode 1.2.1 defaults (src/dependency.rs:213-214:

@@ -12,6 +12,7 @@
 #pragma once
 #include <cstdint>
 #include <memory>
+#include <optional>
 #include <stdexcept>
 #include <string>
 #include <type_traits>
@@ -215,9 +216,52 @@ public:
         return out;
     }
 
+    // Outer joins (Spark's leftOuterJoin / rightOuterJoin / fullOuterJoin; vega has none): a key missing on the other
+    // side still gives rows, with std::nullopt on that side.  A key's rows are contiguous.
+    template <typename W>
+    std::vector<std::pair<K, std::pair<V, std::optional<W>>>> left_outer_join(const PairRddT<K, W> &other, size_t num_splits) const
+    {
+        std::vector<std::pair<K, std::pair<V, std::optional<W>>>> out;
+        outer_join_rows(other, num_splits, VB_JOIN_LEFT, [&](K k, std::optional<V> v, std::optional<W> w) { out.emplace_back(k, std::make_pair(*v, w)); });
+        return out;
+    }
+    template <typename W>
+    std::vector<std::pair<K, std::pair<std::optional<V>, W>>> right_outer_join(const PairRddT<K, W> &other, size_t num_splits) const
+    {
+        std::vector<std::pair<K, std::pair<std::optional<V>, W>>> out;
+        outer_join_rows(other, num_splits, VB_JOIN_RIGHT, [&](K k, std::optional<V> v, std::optional<W> w) { out.emplace_back(k, std::make_pair(v, *w)); });
+        return out;
+    }
+    template <typename W>
+    std::vector<std::pair<K, std::pair<std::optional<V>, std::optional<W>>>> full_outer_join(const PairRddT<K, W> &other, size_t num_splits) const
+    {
+        std::vector<std::pair<K, std::pair<std::optional<V>, std::optional<W>>>> out;
+        outer_join_rows(other, num_splits, VB_JOIN_FULL, [&](K k, std::optional<V> v, std::optional<W> w) { out.emplace_back(k, std::make_pair(v, w)); });
+        return out;
+    }
+
     std::shared_ptr<Context> sc_;
     size_t num_slices_;
     std::vector<uint64_t> keys_, vals_;
+
+private:
+    // every row of vb_join_outer, partition by partition, as emit(k, v or nullopt, w or nullopt)
+    template <typename W, typename Emit>
+    void outer_join_rows(const PairRddT<K, W> &other, size_t num_splits, int32_t kind, Emit emit) const
+    {
+        auto a = detail::run_shuffle<K>(*sc_, keys_, &vals_, num_slices_, num_splits, detail::dtype<V>::code, VB_AGG_COGROUP);
+        auto b = detail::run_shuffle<K>(*sc_, other.keys_, &other.vals_, other.num_slices_, num_splits, detail::dtype<W>::code, VB_AGG_COGROUP);
+        for (uint32_t r = 0; r < num_splits; ++r) {
+            uint64_t n = 0;
+            check(vb_join_outer_size(a.get(), b.get(), r, kind, &n));
+            std::vector<uint64_t> k(n), v(n), w(n);
+            std::vector<uint8_t> vv(n), wv(n);
+            check(vb_join_outer(a.get(), b.get(), r, kind, k.data(), v.data(), w.data(), vv.data(), wv.data(), VB_HOST));
+            for (uint64_t i = 0; i < n; ++i)
+                emit(detail::from_bits<K>(k[i]), vv[i] ? std::optional<V>(detail::from_bits<V>(v[i])) : std::nullopt,
+                     wv[i] ? std::optional<W>(detail::from_bits<W>(w[i])) : std::nullopt);
+        }
+    }
 };
 
 template <typename K>

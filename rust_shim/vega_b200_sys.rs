@@ -18,6 +18,8 @@ pub const VB_AGG_MAX: i32 = 3; pub const VB_AGG_COUNT: i32 = 4; pub const VB_AGG
 pub const VB_AGG_MEAN: i32 = 7;   // vb_agg_col only
 pub const VB_PART_HASH_METRO64: i32 = 0;
 pub const VB_HOST: i32 = 0;
+/// include/vega_b200.h `vb_join_kind` (vb_join_outer; the inner join is vb_join)
+pub const VB_JOIN_LEFT: i32 = 1; pub const VB_JOIN_RIGHT: i32 = 2; pub const VB_JOIN_FULL: i32 = 3;
 
 #[link(name = "vega_b200")]
 extern "C" {
@@ -36,6 +38,11 @@ extern "C" {
     pub fn vb_join_size(left: *mut vb_shuf, right: *mut vb_shuf, reduce_id: u32, n_out: *mut u64) -> i32;
     pub fn vb_join(left: *mut vb_shuf, right: *mut vb_shuf, reduce_id: u32, out_k: *mut c_void, out_v: *mut c_void,
                    out_w: *mut c_void, dst_loc: i32) -> i32;
+    // left / right / full outer joins: a None slot holds 0 and its validity byte (optional arrays) is 0
+    pub fn vb_join_outer_size(left: *mut vb_shuf, right: *mut vb_shuf, reduce_id: u32, kind: i32, n_out: *mut u64) -> i32;
+    pub fn vb_join_outer(left: *mut vb_shuf, right: *mut vb_shuf, reduce_id: u32, kind: i32, out_k: *mut c_void,
+                         out_v: *mut c_void, out_w: *mut c_void, out_v_valid: *mut u8, out_w_valid: *mut u8,
+                         dst_loc: i32) -> i32;
     // N1: bincode blobs (the payload format of SHUFFLE_CACHE)
     pub fn vb_shuffle_reduce_blob_size(s: *mut vb_shuf, reduce_id: u32, n_bytes: *mut u64) -> i32;
     pub fn vb_shuffle_reduce_blob(s: *mut vb_shuf, reduce_id: u32, out_blob: *mut c_void, dst_loc: i32) -> i32;

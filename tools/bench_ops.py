@@ -17,7 +17,8 @@ from vega_b200 import _lib as L
 ap = argparse.ArgumentParser()
 ap.add_argument("--rows", type=float, default=1e9)
 ap.add_argument("--distinct", type=float, default=1e6)
-ap.add_argument("--ops", default="reduce,group,sort,sortkv,join,count")   # also: zipf, zipfgroup, combine, combinezipf
+ap.add_argument("--ops", default="reduce,group,sort,sortkv,join,count")   # also: zipf, zipfgroup, combine, combinezipf,
+#                                                                             leftjoin, fulljoin
 ap.add_argument("--reps", type=int, default=3)
 args = ap.parse_args()
 N, D = int(args.rows), int(args.distinct)
@@ -92,9 +93,11 @@ if "sort" in ops:
     report("sort_by_key(keys only)", N, 16.0 * N, timed(lambda: run_shuffle(L.VB_AGG_SORT, keys=keys), max(1, args.reps - 1)))
     del keys
     torch.cuda.empty_cache()
-if "join" in ops:
+join_ops = [o for o in ("join", "leftjoin", "fulljoin") if o in ops]
+if join_ops:
     # BASELINE config 4, per-GPU share at 8 GPUs: 6.25e7 rows per side, each rank once per side,
     # 1.25e6 shared keys per GPU (1e7 / 8)
+    import ctypes
     n_side = int(min(N, 5e8) // 8)
     shared = n_side // 50
     a = torch.empty((n_side, 2), dtype=torch.int64, device="cuda")
@@ -102,7 +105,7 @@ if "join" in ops:
     sc.gen_pairs(out_rows=a, first=0, n=n_side, mode="unique", rank_base=0)
     sc.gen_pairs(out_rows=b, first=0, n=n_side, mode="unique", rank_base=n_side - shared)
 
-    def join():
+    def cogroup_pair():
         sa = vb.Shuffle(sc, 8, 8, L.VB_U64, L.VB_U64, L.VB_AGG_COGROUP)
         sb = vb.Shuffle(sc, 8, 8, L.VB_U64, L.VB_U64, L.VB_AGG_COGROUP)
         for s_, t in ((sa, a), (sb, b)):
@@ -111,7 +114,18 @@ if "join" in ops:
             for m in range(8):
                 s_.map(m, col, None, int(st[m]), int(st[m + 1]))
             s_.seal()
-        import ctypes
+        return sa, sb
+
+    def pair_stats(sa, sb):
+        st = sa.stats()
+        stb = sb.stats()
+        for kk in st["kernels"]:
+            st["kernels"][kk]["ms"] += stb["kernels"][kk]["ms"]; st["kernels"][kk]["launches"] += stb["kernels"][kk]["launches"]
+        st["kernel_launches"] += stb["kernel_launches"]
+        return st
+
+    def join():
+        sa, sb = cogroup_pair()
         tot = 0
         for r in range(8):
             nn = ctypes.c_uint64()
@@ -120,18 +134,65 @@ if "join" in ops:
             p = lambda t: ctypes.c_void_p(t.data_ptr()) if t.numel() else None
             L.check(sc._lib.vb_join(sa._h, sb._h, r, p(k), p(v), p(w), L.VB_DEVICE))
             tot += nn.value
-        st = sa.stats()
-        stb = sb.stats()
-        for kk in st["kernels"]:
-            st["kernels"][kk]["ms"] += stb["kernels"][kk]["ms"]; st["kernels"][kk]["launches"] += stb["kernels"][kk]["launches"]
-        st["kernel_launches"] += stb["kernel_launches"]
+        st = pair_stats(sa, sb)
         st["join_rows"] = tot
         sa.free(); sb.free()
         return st
 
+if "join" in ops:
     res = timed(join, max(1, args.reps - 1))
     assert res[-1][1]["join_rows"] == shared, (res[-1][1]["join_rows"], shared)
     report("join", 2 * n_side, 32.0 * n_side + 24.0 * shared, res, {"join_rows": shared})
+if "leftjoin" in ops or "fulljoin" in ops:
+    # Each outer join against the inner join of the same inputs and against the workaround without outer joins:
+    # materialising the cogroup of both sides (vb_shuffle_reduce of every partition, device output), which the
+    # caller then still has to expand.  All outputs stay on the device.
+    from bench import gpu_info
+    card = gpu_info(0)
+    p = lambda t: ctypes.c_void_p(t.data_ptr()) if t.numel() else None
+    dev = lambda n, dt=torch.int64: torch.empty(n, dtype=dt, device="cuda")
+
+    def outer(kind):
+        def run():
+            sa, sb = cogroup_pair()
+            tot = 0
+            for r in range(8):
+                nn = ctypes.c_uint64()
+                L.check(sc._lib.vb_join_outer_size(sa._h, sb._h, r, kind, ctypes.byref(nn)))
+                k, v, w = dev(nn.value), dev(nn.value), dev(nn.value)
+                vv, wv = dev(nn.value, torch.uint8), dev(nn.value, torch.uint8)
+                L.check(sc._lib.vb_join_outer(sa._h, sb._h, r, kind, p(k), p(v), p(w), p(vv), p(wv), L.VB_DEVICE))
+                tot += nn.value
+            st = pair_stats(sa, sb)
+            st["join_rows"] = tot
+            sa.free(); sb.free()
+            return st
+        return run
+
+    def cogroup_both():
+        sa, sb = cogroup_pair()
+        for r in range(8):
+            for s_ in (sa, sb):
+                nk, nv = ctypes.c_uint64(), ctypes.c_uint64()
+                L.check(sc._lib.vb_shuffle_reduce_size(s_._h, r, ctypes.byref(nk), ctypes.byref(nv)))
+                k, o, v = dev(nk.value), dev(nk.value + 1), dev(nv.value)
+                L.check(sc._lib.vb_shuffle_reduce(s_._h, r, p(k), None, p(o), p(v), L.VB_DEVICE))
+        st = pair_stats(sa, sb)
+        sa.free(); sb.free()
+        return st
+
+    med = lambda r: sorted(x[0] for x in r)[len(r) // 2]
+    reps = max(1, args.reps - 1)
+    r_inner = timed(join, reps)
+    r_cog = timed(cogroup_both, reps)
+    for op, kind, want in (("leftjoin", L.VB_JOIN_LEFT, n_side), ("fulljoin", L.VB_JOIN_FULL, 2 * n_side - shared)):
+        if op not in ops:
+            continue
+        res = timed(outer(kind), reps)
+        assert res[-1][1]["join_rows"] == want, (res[-1][1]["join_rows"], want)
+        extra = {"gpu": card["name"], "power_limit_w": card["power_limit_w"], "join_rows": want,
+                 "inner_join_ms": round(med(r_inner), 3), "cogroup_both_sides_ms": round(med(r_cog), 3)}
+        report({"leftjoin": "left_outer_join", "fulljoin": "full_outer_join"}[op], 2 * n_side, 32.0 * n_side + 26.0 * want, res, extra)
 if "combine" in ops or "combinezipf" in ops:
     # combine_by_key: sum(v0), min(v1), max(v1), mean(v2), count in one shuffle (5 accumulators) against the baseline a
     # user has without it, one single-column shuffle per aggregate (the mean from a sum and the count).  v0 is gen_pairs'

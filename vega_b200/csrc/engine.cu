@@ -12,6 +12,7 @@
 #include <map>
 #include <mutex>
 #include <string>
+#include <tuple>
 #include <vector>
 
 #include "../../include/vega_b200.h"
@@ -276,8 +277,10 @@ struct Timer {
 struct JoinPlan {
     u64 total = 0;
     u32 nl = 0;
-    u64 *pos = nullptr;
+    u64 *pos = nullptr;            // [nl + nr] exclusive: the left keys' rows first, then the right-only keys' rows
     u32 *match = nullptr;
+    u32 nr = 0;                    // RIGHT / FULL: right keys of the partition
+    u64 total_left = 0;            // rows of the left keys (pos[nl])
 };
 
 struct vb_shuf {
@@ -336,15 +339,17 @@ struct vb_shuf {
     void *dict = nullptr;          // group ops: key → slot table, kept for joins
     u32 dict_log_cap = 0;
     u32 *dense_of_slot = nullptr;
-    std::map<std::pair<const vb_shuf *, u32>, JoinPlan> join_plans;
+    std::map<std::tuple<const vb_shuf *, u32, int>, JoinPlan> join_plans;   // by (right side, partition, join kind)
     // COGROUP shuffles are grouped lazily: seal keeps the (owned) rows; the CSR is built by the first reduce call
-    // (cogroup materialisation), or — if a join comes first — only for the keys that occur on BOTH sides.
+    // (cogroup materialisation), or — if a join comes first — only for the rows the join kind needs: the keys on BOTH
+    // sides (inner), every row of the preserved side plus the matching rows of the other (LEFT / RIGHT), or all (FULL).
     u64 uid = 0;                                   // process-unique id (cache key that survives pointer reuse)
     bool lazy = false;                             // sealed, rows in lz_*, not grouped yet
     u64 *lz_keys = nullptr, *lz_vals = nullptr;
     u64 lz_n = 0;
     std::vector<vb_shuf *> trash;                  // internal shuffles of a failed filtered join
-    std::map<u64, std::pair<vb_shuf *, vb_shuf *>> filtered;   // by the right side's uid: internal (left, right) shuffles over the matching rows
+    // by (the right side's uid, join kind): internal (left, right) shuffles over the rows that join kind keeps
+    std::map<std::pair<u64, int>, std::pair<vb_shuf *, vb_shuf *>> filtered;
     // stats
     vb_stats st{};
     std::vector<Timer> timers;
@@ -2990,28 +2995,36 @@ static vb_shuf *make_internal_like(const vb_shuf *s)
 
 extern "C" int32_t vb_shuffle_free(vb_shuf *s);
 
-// both sides lazy: internal (left, right) shuffles grouped over the rows whose key occurs on both sides
-static int filtered_pair(vb_shuf *l, vb_shuf *r, vb_shuf **fl_out, vb_shuf **fr_out)
+// both sides lazy: internal (left, right) shuffles grouped over the rows the join kind needs.  A side the kind
+// preserves (LEFT: the left, RIGHT: the right, FULL: both) keeps every row; any other side keeps the rows whose key
+// occurs on both sides.
+static int filtered_pair(vb_shuf *l, vb_shuf *r, int kind, vb_shuf **fl_out, vb_shuf **fr_out)
 {
-    auto it = l->filtered.find(r->uid);
+    const auto cache_key = std::make_pair(r->uid, kind);
+    auto it = l->filtered.find(cache_key);
     if (it != l->filtered.end()) { *fl_out = it->second.first; *fr_out = it->second.second; return VB_OK; }
     vb_ctx *c = l->ctx;
     vb_shuf *fl = make_internal_like(l), *fr = make_internal_like(r);
     auto fail = [&](int rc) { delete fl; delete fr; return rc; };
     fl->bucket_off.assign((size_t)l->n_reduce + 1, 0); fl->val_off = fl->bucket_off;
     fr->bucket_off = fl->bucket_off; fr->val_off = fl->bucket_off;
-    if (l->lz_n && r->lz_n) {
+    const bool all_l = kind == JK_LEFT || kind == JK_FULL, all_r = kind == JK_RIGHT || kind == JK_FULL;
+    Gathered gl, gr;                                // the rows each internal shuffle groups
+    DevBuf lk(c), lv(c), rk(c), rv(c);
+    if (all_l) { gl.keys = l->lz_keys; gl.vals = l->lz_vals; gl.n = l->lz_n; }
+    if (all_r) { gr.keys = r->lz_keys; gr.vals = r->lz_vals; gr.n = r->lz_n; }
+    u64 cap = 0;
+    int rc = VB_OK;
+    if (l->lz_n && r->lz_n && !(all_l && all_r)) {
         // 1. dictionary of the right keys (slot per right row)
         DevBuf ids_r(c);
-        int rc = ids_r.alloc(r->lz_n * 4);
-        if (rc) return fail(rc);
+        if ((rc = ids_r.alloc(r->lz_n * 4))) return fail(rc);
         std::vector<AggInput> in(1);
         in[0] = AggInput{IN_SOA, r->lz_keys, nullptr, r->lz_n, VB_DEVICE};
         void *tab = nullptr; u32 log_cap = 0; u64 n_ins = 0;
-        rc = build_table(l, K_DICT, in, OPK_DICT, TX_NONE, r->hint, &tab, &log_cap, &n_ins, ids_r.as<u32>());
-        if (rc) return fail(rc);
+        if ((rc = build_table(l, K_DICT, in, OPK_DICT, TX_NONE, r->hint, &tab, &log_cap, &n_ins, ids_r.as<u32>()))) return fail(rc);
         DevBuf tab_guard(c); tab_guard.p = tab;
-        const u64 cap = 1ull << log_cap;
+        cap = 1ull << log_cap;
         // 2. probe with every left row; 3. mark the right rows whose key matched
         DevBuf slot_flag(c), ml(c), mr(c);
         if ((rc = slot_flag.alloc(cap + 1 + 16)) || (rc = ml.alloc(l->lz_n)) || (rc = mr.alloc(r->lz_n))) return fail(rc);
@@ -3022,33 +3035,34 @@ static int filtered_pair(vb_shuf *l, vb_shuf *r, vb_shuf **fl_out, vb_shuf **fr_
             semi_probe_kernel<<<g, 256, 0, c->stream>>>(l->lz_keys, l->lz_n, table_at(tab, log_cap), slot_flag.as<unsigned char>(), ml.as<unsigned char>());
             if ((rc = kl.done("semi_probe_kernel"))) return fail(rc);
         }
-        {
+        if (!all_r) {
             KLaunch kl(l, K_JOIN);
             const unsigned g = (unsigned)std::min<u64>((r->lz_n + 255) / 256, (u64)c->sm_count * 16);
             mark_rows_kernel<<<g, 256, 0, c->stream>>>(ids_r.as<u32>(), r->lz_n, slot_flag.as<unsigned char>(), mr.as<unsigned char>());
             if ((rc = kl.done("mark_rows_kernel"))) return fail(rc);
         }
-        // 4. stable compaction of both sides, then the ordinary cogroup of what is left
-        DevBuf lk(c), lv(c), rk(c), rv(c);
-        u64 m_l = 0, m_r = 0;
-        if ((rc = compact_rows(l, l->lz_keys, l->lz_vals, l->lz_n, ml.as<unsigned char>(), lk, lv, &m_l))) return fail(rc);
-        if ((rc = compact_rows(l, r->lz_keys, r->lz_vals, r->lz_n, mr.as<unsigned char>(), rk, rv, &m_r))) return fail(rc);
-        if (m_l && m_r) {
-            Gathered gl, gr;
-            gl.keys = lk.as<u64>(); gl.vals = lv.as<u64>(); gl.n = m_l;
-            gr.keys = rk.as<u64>(); gr.vals = rv.as<u64>(); gr.n = m_r;
-            if ((rc = seal_group(fl, gl)) || (rc = seal_group(fr, gr))) {
-                l->trash.push_back(fl); l->trash.push_back(fr);      // freed with l (vb_shuffle_free would re-lock the context here)
-                return rc;
-            }
-            // kernel counters of the internal shuffles belong to the caller's statistics
-            for (int k = 0; k < K_N; ++k) { l->klaunch[k] += fl->klaunch[k] + fr->klaunch[k]; }
-            l->st.kernel_launches += fl->st.kernel_launches + fr->st.kernel_launches;
-            l->st.table_slots = std::max<u64>(l->st.table_slots, std::max<u64>(cap, std::max(fl->st.table_slots, fr->st.table_slots)));
+        // 4. stable compaction of the side(s) the kind does not preserve, then the ordinary cogroup of what is left
+        if (!all_l) {
+            if ((rc = compact_rows(l, l->lz_keys, l->lz_vals, l->lz_n, ml.as<unsigned char>(), lk, lv, &gl.n))) return fail(rc);
+            gl.keys = lk.as<u64>(); gl.vals = lv.as<u64>();
         }
-        cudaStreamSynchronize(c->stream);
+        if (!all_r) {
+            if ((rc = compact_rows(l, r->lz_keys, r->lz_vals, r->lz_n, mr.as<unsigned char>(), rk, rv, &gr.n))) return fail(rc);
+            gr.keys = rk.as<u64>(); gr.vals = rv.as<u64>();
+        }
     }
-    l->filtered[r->uid] = std::make_pair(fl, fr);
+    if (gl.n || gr.n) {
+        if ((gl.n && (rc = seal_group(fl, gl))) || (gr.n && (rc = seal_group(fr, gr)))) {
+            l->trash.push_back(fl); l->trash.push_back(fr);      // freed with l (vb_shuffle_free would re-lock the context here)
+            return rc;
+        }
+        // kernel counters of the internal shuffles belong to the caller's statistics
+        for (int k = 0; k < K_N; ++k) { l->klaunch[k] += fl->klaunch[k] + fr->klaunch[k]; }
+        l->st.kernel_launches += fl->st.kernel_launches + fr->st.kernel_launches;
+        l->st.table_slots = std::max<u64>(l->st.table_slots, std::max<u64>(cap, std::max(fl->st.table_slots, fr->st.table_slots)));
+    }
+    cudaStreamSynchronize(c->stream);
+    l->filtered[cache_key] = std::make_pair(fl, fr);
     *fl_out = fl; *fr_out = fr;
     return VB_OK;
 }
@@ -3369,34 +3383,84 @@ static int join_check(vb_shuf *l, vb_shuf *r, u32 rid)
     return VB_OK;
 }
 
-static int join_plan(vb_shuf *l, vb_shuf *r, u32 rid, JoinPlan **out)
+static_assert(JK_LEFT == (int)VB_JOIN_LEFT && JK_RIGHT == (int)VB_JOIN_RIGHT && JK_FULL == (int)VB_JOIN_FULL, "join kinds");
+
+// Row counts and output positions of partition rid.  Left-driven rows first: per left key |vs| * |ws| when the right
+// side has the key, |vs| when it does not and the kind keeps the left side (LEFT / FULL), else 0.  RIGHT / FULL then
+// place the right-only keys (|ws| rows each, found by probing the left dictionary); one exclusive scan covers both.
+static int join_plan(vb_shuf *l, vb_shuf *r, u32 rid, int kind, JoinPlan **out)
 {
     vb_ctx *c = l->ctx;
-    auto key = std::make_pair((const vb_shuf *)r, rid);
+    auto key = std::make_tuple((const vb_shuf *)r, rid, kind);
     auto it = l->join_plans.find(key);
     if (it != l->join_plans.end()) { *out = &it->second; return VB_OK; }
     JoinPlan p;
     const u64 lb = l->bucket_off[rid], le = l->bucket_off[rid + 1];
     p.nl = (u32)(le - lb);
-    if (p.nl && r->n_keys && r->dict) {
-        DevBuf cnt(c), pos(c), match(c), tot(c);
-        TRY(cnt.alloc((u64)p.nl * 8));
-        TRY(pos.alloc((u64)p.nl * 8));
-        TRY(match.alloc((u64)p.nl * 4));
-        TRY(tot.alloc(8));
-        {
-            KLaunch kl(l, K_JOIN);
-            join_probe_kernel<<<(p.nl + 255) / 256, 256, 0, c->stream>>>(l->res_keys, l->res_offs, (u32)lb, (u32)le,
-                                                                         table_at(r->dict, r->dict_log_cap), r->dense_of_slot,
-                                                                         r->res_offs, cnt.as<u64>(), match.as<u32>());
-            TRY(kl.done("join_probe_kernel"));
+    if (kind == JK_INNER) {
+        if (p.nl && r->n_keys && r->dict) {
+            DevBuf cnt(c), pos(c), match(c), tot(c);
+            TRY(cnt.alloc((u64)p.nl * 8));
+            TRY(pos.alloc((u64)p.nl * 8));
+            TRY(match.alloc((u64)p.nl * 4));
+            TRY(tot.alloc(8));
+            {
+                KLaunch kl(l, K_JOIN);
+                join_probe_kernel<JK_INNER><<<(p.nl + 255) / 256, 256, 0, c->stream>>>(l->res_keys, l->res_offs, (u32)lb, (u32)le,
+                                                                                   table_at(r->dict, r->dict_log_cap), r->dense_of_slot,
+                                                                                   r->res_offs, cnt.as<u64>(), match.as<u32>());
+                TRY(kl.done("join_probe_kernel"));
+            }
+            TRY(exclusive_scan_u64(l, cnt.as<u64>(), pos.as<u64>(), p.nl, tot.as<u64>()));
+            CU(cudaMemcpyAsync(c->h_scratch, tot.p, 8, cudaMemcpyDeviceToHost, c->stream));
+            CU(cudaStreamSynchronize(c->stream));
+            p.total = *(u64 *)c->h_scratch;
+            p.pos = (u64 *)pos.release();
+            p.match = (u32 *)match.release();
         }
-        TRY(exclusive_scan_u64(l, cnt.as<u64>(), pos.as<u64>(), p.nl, tot.as<u64>()));
-        CU(cudaMemcpyAsync(c->h_scratch, tot.p, 8, cudaMemcpyDeviceToHost, c->stream));
-        CU(cudaStreamSynchronize(c->stream));
-        p.total = *(u64 *)c->h_scratch;
-        p.pos = (u64 *)pos.release();
-        p.match = (u32 *)match.release();
+    } else {
+        const u64 rb = r->bucket_off[rid], re = r->bucket_off[rid + 1];
+        p.nr = (kind == JK_LEFT) ? 0 : (u32)(re - rb);
+        const u64 n = (u64)p.nl + p.nr;
+        if (n) {
+            if ((r->n_keys && !r->dict) || (l->n_keys && !l->dict)) return set_err(VB_ERR_STATE, "join side without a key dictionary");
+            const Table rtab = table_at(r->n_keys ? r->dict : nullptr, r->dict_log_cap);   // keys NULL: that side is empty
+            const Table ltab = table_at(l->n_keys ? l->dict : nullptr, l->dict_log_cap);
+            DevBuf cnt(c), pos(c), match(c), tot(c);
+            TRY(cnt.alloc(n * 8));
+            TRY(pos.alloc(n * 8));
+            TRY(match.alloc(std::max<u64>(p.nl, 1) * 4));
+            TRY(tot.alloc(8));
+            if (p.nl) {
+                KLaunch kl(l, K_JOIN);
+                const unsigned g = (p.nl + 255) / 256;
+                if (kind == JK_LEFT)
+                    join_probe_kernel<JK_LEFT><<<g, 256, 0, c->stream>>>(l->res_keys, l->res_offs, (u32)lb, (u32)le, rtab, r->dense_of_slot,
+                                                                         r->res_offs, cnt.as<u64>(), match.as<u32>());
+                else if (kind == JK_RIGHT)
+                    join_probe_kernel<JK_RIGHT><<<g, 256, 0, c->stream>>>(l->res_keys, l->res_offs, (u32)lb, (u32)le, rtab, r->dense_of_slot,
+                                                                          r->res_offs, cnt.as<u64>(), match.as<u32>());
+                else
+                    join_probe_kernel<JK_FULL><<<g, 256, 0, c->stream>>>(l->res_keys, l->res_offs, (u32)lb, (u32)le, rtab, r->dense_of_slot,
+                                                                         r->res_offs, cnt.as<u64>(), match.as<u32>());
+                TRY(kl.done("join_probe_kernel"));
+            }
+            if (p.nr) {
+                KLaunch kl(l, K_JOIN);
+                join_probe_right_kernel<<<(p.nr + 255) / 256, 256, 0, c->stream>>>(r->res_keys, r->res_offs, (u32)rb, (u32)re, ltab,
+                                                                                   cnt.as<u64>() + p.nl);
+                TRY(kl.done("join_probe_right_kernel"));
+            }
+            TRY(exclusive_scan_u64(l, cnt.as<u64>(), pos.as<u64>(), n, tot.as<u64>()));
+            u64 *h = (u64 *)c->h_scratch;
+            CU(cudaMemcpyAsync(h, tot.p, 8, cudaMemcpyDeviceToHost, c->stream));
+            if (p.nr) CU(cudaMemcpyAsync(h + 1, pos.as<u64>() + p.nl, 8, cudaMemcpyDeviceToHost, c->stream));
+            CU(cudaStreamSynchronize(c->stream));
+            p.total = h[0];
+            p.total_left = p.nr ? h[1] : p.total;
+            p.pos = (u64 *)pos.release();
+            p.match = (u32 *)match.release();
+        }
     }
     auto ins = l->join_plans.emplace(key, p);
     *out = &ins.first->second;
@@ -3404,11 +3468,11 @@ static int join_plan(vb_shuf *l, vb_shuf *r, u32 rid, JoinPlan **out)
 }
 
 // the pair of shuffles whose CSR the join reads: the filtered internal pair while both sides are still lazy
-static int join_sides(vb_shuf *&l, vb_shuf *&r)
+static int join_sides(vb_shuf *&l, vb_shuf *&r, int kind)
 {
     if (l->lazy && r->lazy && l != r) {
         vb_shuf *fl = nullptr, *fr = nullptr;
-        TRY(filtered_pair(l, r, &fl, &fr));
+        TRY(filtered_pair(l, r, kind, &fl, &fr));
         l = fl; r = fr;
         return VB_OK;
     }
@@ -3417,58 +3481,104 @@ static int join_sides(vb_shuf *&l, vb_shuf *&r)
     return VB_OK;
 }
 
-extern "C" int32_t vb_join_size(vb_shuf *l, vb_shuf *r, uint32_t rid, uint64_t *n_out)
+static int join_size(vb_shuf *l, vb_shuf *r, uint32_t rid, int kind, uint64_t *n_out)
 {
     TRY(join_check(l, r, rid));
     if (!n_out) return set_err(VB_ERR_INVALID, "n_out is NULL");
     std::lock_guard<std::mutex> lk(l->ctx->mu);
     CU(cudaSetDevice(l->ctx->device));
-    TRY(join_sides(l, r));
+    TRY(join_sides(l, r, kind));
     JoinPlan *p = nullptr;
-    TRY(join_plan(l, r, rid, &p));
+    TRY(join_plan(l, r, rid, kind, &p));
     *n_out = p->total;
     return VB_OK;
 }
 
-extern "C" int32_t vb_join(vb_shuf *l, vb_shuf *r, uint32_t rid, void *out_k, void *out_v, void *out_w, int32_t dst_loc)
+static int join_rows(vb_shuf *l, vb_shuf *r, uint32_t rid, int kind, void *out_k, void *out_v, void *out_w,
+                     uint8_t *out_vv, uint8_t *out_wv, int32_t dst_loc)
 {
     TRY(join_check(l, r, rid));
     if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
     vb_ctx *c = l->ctx;
     std::lock_guard<std::mutex> lk(c->mu);
     CU(cudaSetDevice(c->device));
-    TRY(join_sides(l, r));
+    TRY(join_sides(l, r, kind));
     JoinPlan *p = nullptr;
-    TRY(join_plan(l, r, rid, &p));
+    TRY(join_plan(l, r, rid, kind, &p));
     const u64 total = p->total;
     int rc = VB_OK;
     if (total) {
         if (!out_k || !out_v || !out_w) return set_err(VB_ERR_INVALID, "NULL output with %llu rows to write", (unsigned long long)total);
-        DevBuf bk(c), bv(c), bw(c);
+        DevBuf bk(c), bv(c), bw(c), bvv(c), bwv(c);
         u64 *dk = (u64 *)out_k, *dv = (u64 *)out_v, *dw = (u64 *)out_w;
+        unsigned char *dvv = out_vv, *dwv = out_wv;
         if (dst_loc == VB_HOST) {
             TRY(bk.alloc(total * 8)); TRY(bv.alloc(total * 8)); TRY(bw.alloc(total * 8));
             dk = bk.as<u64>(); dv = bv.as<u64>(); dw = bw.as<u64>();
+            if (out_vv) { TRY(bvv.alloc(total)); dvv = bvv.as<unsigned char>(); }
+            if (out_wv) { TRY(bwv.alloc(total)); dwv = bwv.as<unsigned char>(); }
         }
-        {
+        const u64 lb = l->bucket_off[rid];
+        const u64 total_left = kind == JK_INNER ? total : p->total_left;
+        if (total_left) {
             KLaunch kl(l, K_JOIN);
-            u64 blocks = std::min<u64>((total + 255) / 256, (u64)c->sm_count * 8);
-            join_expand_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(p->pos, p->nl, total, l->res_keys, l->res_offs, l->res_vals,
-                                                                        (u32)l->bucket_off[rid], p->match, r->res_offs, r->res_vals,
-                                                                        dk, dv, dw);
+            u64 blocks = std::min<u64>((total_left + 255) / 256, (u64)c->sm_count * 8);
+#define VB_JOIN_EXPAND(KIND) join_expand_kernel<KIND><<<(unsigned)blocks, 256, 0, c->stream>>>(p->pos, p->nl, total_left, l->res_keys, \
+                                 l->res_offs, l->res_vals, (u32)lb, p->match, r->res_offs, r->res_vals, dk, dv, dw, dvv, dwv)
+            switch (kind) {
+            case JK_INNER: VB_JOIN_EXPAND(JK_INNER); break;
+            case JK_LEFT: VB_JOIN_EXPAND(JK_LEFT); break;
+            case JK_RIGHT: VB_JOIN_EXPAND(JK_RIGHT); break;
+            default: VB_JOIN_EXPAND(JK_FULL); break;
+            }
+#undef VB_JOIN_EXPAND
             rc = kl.done("join_expand_kernel");
+        }
+        if (rc == VB_OK && total > total_left) {
+            KLaunch kl(l, K_JOIN);
+            u64 blocks = std::min<u64>((total - total_left + 255) / 256, (u64)c->sm_count * 8);
+            join_expand_right_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(p->pos + p->nl, p->nr, total, r->res_keys, r->res_offs,
+                                                                              r->res_vals, (u32)r->bucket_off[rid], dk, dv, dw, dvv, dwv);
+            rc = kl.done("join_expand_right_kernel");
         }
         if (rc == VB_OK && dst_loc == VB_HOST) {
             rc = copy_out(l, out_k, dk, total * 8, VB_HOST);
             if (rc == VB_OK) rc = copy_out(l, out_v, dv, total * 8, VB_HOST);
             if (rc == VB_OK) rc = copy_out(l, out_w, dw, total * 8, VB_HOST);
+            if (rc == VB_OK) rc = copy_out(l, out_vv, dvv, total, VB_HOST);
+            if (rc == VB_OK) rc = copy_out(l, out_wv, dwv, total, VB_HOST);
         }
         cudaStreamSynchronize(c->stream);
     }
     dev_free(c, p->pos);
     dev_free(c, p->match);
-    l->join_plans.erase(std::make_pair((const vb_shuf *)r, rid));
+    l->join_plans.erase(std::make_tuple((const vb_shuf *)r, rid, kind));
     return rc;
+}
+
+extern "C" int32_t vb_join_size(vb_shuf *l, vb_shuf *r, uint32_t rid, uint64_t *n_out)
+{
+    return join_size(l, r, rid, JK_INNER, n_out);
+}
+
+extern "C" int32_t vb_join(vb_shuf *l, vb_shuf *r, uint32_t rid, void *out_k, void *out_v, void *out_w, int32_t dst_loc)
+{
+    return join_rows(l, r, rid, JK_INNER, out_k, out_v, out_w, nullptr, nullptr, dst_loc);
+}
+
+static bool outer_kind(int32_t kind) { return kind == VB_JOIN_LEFT || kind == VB_JOIN_RIGHT || kind == VB_JOIN_FULL; }
+
+extern "C" int32_t vb_join_outer_size(vb_shuf *l, vb_shuf *r, uint32_t rid, int32_t kind, uint64_t *n_out)
+{
+    if (!outer_kind(kind)) return set_err(VB_ERR_INVALID, "bad join kind %d", kind);
+    return join_size(l, r, rid, kind, n_out);
+}
+
+extern "C" int32_t vb_join_outer(vb_shuf *l, vb_shuf *r, uint32_t rid, int32_t kind, void *out_k, void *out_v, void *out_w,
+                                 uint8_t *out_v_valid, uint8_t *out_w_valid, int32_t dst_loc)
+{
+    if (!outer_kind(kind)) return set_err(VB_ERR_INVALID, "bad join kind %d", kind);
+    return join_rows(l, r, rid, kind, out_k, out_v, out_w, out_v_valid, out_w_valid, dst_loc);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -1588,7 +1588,13 @@ __global__ void aos_to_soa_kernel(const u64 *__restrict__ rows, u64 n, u64 *__re
 // ---------------------------------------------------------------------------------------------
 // join (CoGroupedRdd::compute + cross product)
 // ---------------------------------------------------------------------------------------------
-// For left keys [lb, le): find the key in the right shuffle's dictionary; cnt = lenL * lenR.
+// Join kinds: the inner join, and the outer joins with the values of vb_join_kind (include/vega_b200.h).
+enum : int { JK_INNER = 0, JK_LEFT = 1, JK_RIGHT = 2, JK_FULL = 3 };
+template <int KIND> constexpr bool jk_keeps_left() { return KIND == JK_LEFT || KIND == JK_FULL; }
+
+// For left keys [lb, le): find the key in the right shuffle's dictionary; cnt = lenL * lenR.  An unmatched key counts
+// lenL rows (k, v, None) when the kind keeps the left side.  The outer kinds accept an empty right side (rtab.keys NULL).
+template <int KIND>
 __global__ void join_probe_kernel(const u64 *__restrict__ lkeys, const u64 *__restrict__ loffs, u32 lb, u32 le,
                                   Table rtab, const u32 *__restrict__ r_dense,
                                   const u64 *__restrict__ roffs, u64 *__restrict__ cnt, u32 *__restrict__ match)
@@ -1596,23 +1602,38 @@ __global__ void join_probe_kernel(const u64 *__restrict__ lkeys, const u64 *__re
     u32 j = lb + blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= le) return;
     u64 key = lkeys[j];
-    u32 s = table_find(rtab, key);
+    u32 s = (KIND == JK_INNER || rtab.keys) ? table_find(rtab, key) : 0xFFFFFFFFu;
     u64 c = 0;
     u32 m = 0xFFFFFFFFu;
     if (s != 0xFFFFFFFFu) {
         m = r_dense[s];
         c = (loffs[j + 1] - loffs[j]) * (roffs[m + 1] - roffs[m]);
+    } else if (jk_keeps_left<KIND>()) {
+        c = loffs[j + 1] - loffs[j];
     }
     cnt[j - lb] = c;
     match[j - lb] = m;
 }
 
-// One thread per output row: binary-search the owning left key, then (v, w) = divmod.
+// For right keys [rb, re) of a RIGHT / FULL join: cnt = lenR for a key the left side lacks (rows (k, None, w)), else 0
+// (its rows come from the left-driven part).  ltab.keys is NULL when the left side has no rows.
+__global__ void join_probe_right_kernel(const u64 *__restrict__ rkeys, const u64 *__restrict__ roffs, u32 rb, u32 re,
+                                        Table ltab, u64 *__restrict__ cnt)
+{
+    const u32 j = rb + blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= re) return;
+    const bool in_left = ltab.keys && table_find(ltab, rkeys[j]) != 0xFFFFFFFFu;
+    cnt[j - rb] = in_left ? 0 : roffs[j + 1] - roffs[j];
+}
+
+// One thread per output row: binary-search the owning left key, then (v, w) = divmod.  The outer kinds also write the
+// rows of unmatched left keys as (k, v, 0), and the validity bytes when out_vv / out_wv are given.
+template <int KIND>
 __global__ void join_expand_kernel(const u64 *__restrict__ pos /*[nl] exclusive*/, u32 nl, u64 total,
                                    const u64 *__restrict__ lkeys, const u64 *__restrict__ loffs, const u64 *__restrict__ lvals,
                                    u32 lb, const u32 *__restrict__ match, const u64 *__restrict__ roffs,
                                    const u64 *__restrict__ rvals, u64 *__restrict__ out_k, u64 *__restrict__ out_v,
-                                   u64 *__restrict__ out_w)
+                                   u64 *__restrict__ out_w, unsigned char *__restrict__ out_vv, unsigned char *__restrict__ out_wv)
 {
     u64 o = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     const u64 stride = (u64)gridDim.x * blockDim.x;
@@ -1625,11 +1646,46 @@ __global__ void join_expand_kernel(const u64 *__restrict__ pos /*[nl] exclusive*
         const u32 j = lo;
         const u32 m = match[j];
         const u64 local = o - pos[j];
+        if (jk_keeps_left<KIND>() && m == 0xFFFFFFFFu) {
+            out_k[o] = lkeys[lb + j];
+            out_v[o] = lvals[loffs[lb + j] + local];
+            out_w[o] = 0;
+            if (out_vv) out_vv[o] = 1;
+            if (out_wv) out_wv[o] = 0;
+            continue;
+        }
         const u64 lenr = roffs[m + 1] - roffs[m];
         const u64 vi = local / lenr, wi = local - vi * lenr;
         out_k[o] = lkeys[lb + j];
         out_v[o] = lvals[loffs[lb + j] + vi];
         out_w[o] = rvals[roffs[m] + wi];
+        if (KIND != JK_INNER) {
+            if (out_vv) out_vv[o] = 1;
+            if (out_wv) out_wv[o] = 1;
+        }
+    }
+}
+
+// Rows [pos[0], total) of a RIGHT / FULL join: the right-only keys, (k, 0, w) with validity (0, 1).  pos[nr] holds the
+// exclusive positions of the partition's right keys, continuing after the left-driven rows.
+__global__ void join_expand_right_kernel(const u64 *__restrict__ pos, u32 nr, u64 total, const u64 *__restrict__ rkeys,
+                                         const u64 *__restrict__ roffs, const u64 *__restrict__ rvals, u32 rb,
+                                         u64 *__restrict__ out_k, u64 *__restrict__ out_v, u64 *__restrict__ out_w,
+                                         unsigned char *__restrict__ out_vv, unsigned char *__restrict__ out_wv)
+{
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 o = pos[0] + (u64)blockIdx.x * blockDim.x + threadIdx.x; o < total; o += stride) {
+        u32 lo = 0, hi = nr;
+        while (hi - lo > 1) {
+            u32 mid = (lo + hi) >> 1;
+            if (pos[mid] <= o) lo = mid; else hi = mid;
+        }
+        const u32 j = rb + lo;
+        out_k[o] = rkeys[j];
+        out_v[o] = 0;
+        out_w[o] = rvals[roffs[j] + (o - pos[lo])];
+        if (out_vv) out_vv[o] = 0;
+        if (out_wv) out_wv[o] = 1;
     }
 }
 

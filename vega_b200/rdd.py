@@ -440,12 +440,28 @@ class ShuffledRdd(_Base):
         return self._run().stats()
 
 
+_JOIN_KINDS = {"left": L.VB_JOIN_LEFT, "right": L.VB_JOIN_RIGHT, "full": L.VB_JOIN_FULL}
+
+
 class JoinedRdd(_Base):
     """`a.join(b, num_splits)` (src/rdd/pair_rdd.rs:104-121): cogroup of two Vec-append
-    shuffles + per-key cross product, inner join."""
+    shuffles + per-key cross product, inner join.
 
-    def __init__(self, left, right, num_splits):
+    kind "left" / "right" / "full": the outer joins (Spark's leftOuterJoin / rightOuterJoin / fullOuterJoin, which
+    vega lacks).  A key missing on the other side still gives rows, with None on that side.  compute(r) / collect()
+    return (k, v, w); a side that can be None is a numpy.ma.MaskedArray (masked = None, data 0), the other side a
+    plain array."""
+
+    def __init__(self, left, right, num_splits, kind=None):
+        if kind is not None:
+            if kind not in _JOIN_KINDS:
+                raise ValueError(f"join kind {kind!r} is not one of {sorted(_JOIN_KINDS)}")
+            if num_splits < 1:
+                raise ValueError("num_splits must be >= 1")
+            if left.keys.key_width != right.keys.key_width:
+                raise TypeError("join sides have different key types")
         self.left, self.right, self.num_slices, self.sc = left, right, num_splits, left.sc
+        self.kind = kind
         self._shs = None
 
     def _run(self):
@@ -461,17 +477,31 @@ class JoinedRdd(_Base):
         a, b = self._run()
         lib = self.sc._lib
         n = ctypes.c_uint64()
-        L.check(lib.vb_join_size(a._h, b._h, split, ctypes.byref(n)))
+        p = lambda x: x.ctypes.data_as(ctypes.c_void_p) if x is not None else None
+        if self.kind is not None:
+            kind = _JOIN_KINDS[self.kind]
+            L.check(lib.vb_join_outer_size(a._h, b._h, split, kind, ctypes.byref(n)))
+        else:
+            L.check(lib.vb_join_size(a._h, b._h, split, ctypes.byref(n)))
         k = np.empty(n.value, dtype=_NP_OF[a.kcode])
         v = np.empty(n.value, dtype=_NP_OF[a.vcode])
         w = np.empty(n.value, dtype=_NP_OF[b.vcode])
-        p = lambda x: x.ctypes.data_as(ctypes.c_void_p)
-        L.check(lib.vb_join(a._h, b._h, split, p(k), p(v), p(w), L.VB_HOST))
+        if self.kind is None:
+            L.check(lib.vb_join(a._h, b._h, split, p(k), p(v), p(w), L.VB_HOST))
+            return k, v, w
+        vv = np.empty(n.value, dtype=np.uint8) if self.kind != "left" else None     # validity of the side that can be None
+        wv = np.empty(n.value, dtype=np.uint8) if self.kind != "right" else None
+        L.check(lib.vb_join_outer(a._h, b._h, split, kind, p(k), p(v), p(w), p(vv), p(wv), L.VB_HOST))
+        if vv is not None:
+            v = np.ma.MaskedArray(v, mask=vv == 0)
+        if wv is not None:
+            w = np.ma.MaskedArray(w, mask=wv == 0)
         return k, v, w
 
     def collect(self):
         parts = [self.compute(r) for r in range(self.num_slices)]
-        return tuple(np.concatenate([p[i] for p in parts]) for i in range(3))
+        cat = lambda xs: np.ma.concatenate(xs) if isinstance(xs[0], np.ma.MaskedArray) else np.concatenate(xs)
+        return tuple(cat([p[i] for p in parts]) for i in range(3))
 
     def cogroup_collect(self):
         """cogroup(): per partition, the union of keys with both value lists (co_grouped_rdd.rs:206-249)."""
@@ -587,6 +617,18 @@ class PairRdd(_Base):
 
     def join(self, other, num_splits):
         return JoinedRdd(self, other, num_splits)
+
+    def left_outer_join(self, other, num_splits):
+        """(k, v, w) for every left row; w is None (masked) for a key the other side lacks."""
+        return JoinedRdd(self, other, num_splits, "left")
+
+    def right_outer_join(self, other, num_splits):
+        """(k, v, w) for every right row; v is None (masked) for a key this side lacks."""
+        return JoinedRdd(self, other, num_splits, "right")
+
+    def full_outer_join(self, other, num_splits):
+        """Rows of both sides; v or w is None (masked) for a key only the other side has."""
+        return JoinedRdd(self, other, num_splits, "full")
 
     def cogroup(self, other, num_splits):
         return JoinedRdd(self, other, num_splits)
