@@ -757,40 +757,6 @@ def test_range_source_is_generated_on_device(sc):
     assert sc.range(5, 4, 1, 2).n == 0
 
 
-def test_sweep_pass_opt_in_matches_oracle():
-    """The one-kernel radix pass (csrc/sweep.cuh: copy-engine staged tiles + decoupled look-back) is opt-in
-    (VEGA_B200_SWEEP=1, read once per process): run group_by_key, sort_by_key and a >L2 reduce through it in a
-    subprocess and diff against the oracle."""
-    import os
-    import subprocess
-    import sys
-    code = r'''
-import numpy as np, vega_b200 as vb
-from oracle import oracle as O
-from tests.util import gpu_group_parts, oracle_group, rand_pairs
-rng = np.random.default_rng(21)
-with vb.Context(0) as sc:
-    keys, vals = rand_pairs(rng, 300_000, 40_000)
-    assert gpu_group_parts(sc.parallelize((keys, vals), 5).group_by_key(6)) == oracle_group(keys, vals, 5, 6)
-    rows = np.stack([keys, vals], axis=1)
-    assert gpu_group_parts(sc.parallelize(rows, 3).group_by_key(4)) == oracle_group(keys, vals, 3, 4)
-    for kd, k in (("u64", rng.integers(0, 1 << 63, 200_001).astype(np.uint64)), ("i64", rng.integers(-(1 << 40), 1 << 40, 99_999).astype(np.int64))):
-        v = np.arange(len(k), dtype=np.uint64)
-        ok, ov, ps = O.sort_by_key(k, v, 4, kd)
-        gk, gv = sc.parallelize((k, v), 3).sort_by_key(4).collect()
-        assert np.array_equal(gk.view(np.uint64), ok.view(np.uint64)) and np.array_equal(gv.view(np.uint64), ov)
-        gk2, _ = sc.parallelize(k, 2).sort(3).collect()
-        assert np.array_equal(gk2.view(np.uint64), ok.view(np.uint64))
-    st = sc.parallelize((keys, vals), 2).group_by_key(2).stats()
-    assert st["kernels"]["rp_scan"]["launches"] >= 1
-print("sweep ok")
-'''
-    env = dict(os.environ, VEGA_B200_SWEEP="1")
-    out = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=600, env=env,
-                         cwd=os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-    assert out.returncode == 0 and "sweep ok" in out.stdout, out.stdout[-2000:] + out.stderr[-4000:]
-
-
 def test_zipf_hot_key_cache_over_many_tiles_matches_oracle(sc):
     """Enough rows per map task (> 16 tiles per CTA) for the CTAs to finish their learning tiles and keep using
     the hot-key cache and its flush at CTA exit over many tiles: sums, extrema, counts and f64 sums
@@ -846,10 +812,26 @@ def test_gather_sweep_full_and_partial_tiles_match_oracle(sc):
     st = sc.parallelize(np.arange(3_000_000, dtype=np.uint64)[::-1].copy(), 2).sort(2).stats()
     assert st["kernels"]["rp_scatter"]["launches"] >= 1
     _medium_sort_and_group_cases(sc)
+    # 1e5-3e5 rows (every part shorter than one gather-sweep tile): group_by_key from SoA columns and from AoS host rows,
+    # key-value and key-only sorts
+    rng = np.random.default_rng(21)
+    keys, vals = rand_pairs(rng, 300_000, 40_000)
+    assert gpu_group_parts(sc.parallelize((keys, vals), 5).group_by_key(6)) == oracle_group(keys, vals, 5, 6)
+    rows = np.stack([keys, vals], axis=1)
+    assert gpu_group_parts(sc.parallelize(rows, 3).group_by_key(4)) == oracle_group(keys, vals, 3, 4)
+    for kd, k in (("u64", rng.integers(0, 1 << 63, 200_001).astype(np.uint64)), ("i64", rng.integers(-(1 << 40), 1 << 40, 99_999).astype(np.int64))):
+        v = np.arange(len(k), dtype=np.uint64)
+        ok, ov, ps = O.sort_by_key(k, v, 4, kd)
+        gk, gv = sc.parallelize((k, v), 3).sort_by_key(4).collect()
+        assert np.array_equal(gk.view(np.uint64), ok.view(np.uint64)) and np.array_equal(gv.view(np.uint64), ov), kd
+        gk2, _ = sc.parallelize(k, 2).sort(3).collect()
+        assert np.array_equal(gk2.view(np.uint64), ok.view(np.uint64)), kd
+    st = sc.parallelize((keys, vals), 2).group_by_key(2).stats()
+    assert st["kernels"]["rp_scan"]["launches"] >= 1
 
 
 def test_sweep_static_fallback_matches_oracle():
-    """VEGA_B200_NO_GSWEEP=1 (read once per process) sends the LSD passes back through rp_sweep_kernel<STATIC>:
+    """VEGA_B200_NO_GSWEEP=1 (read once per process) sends the LSD passes back through rp_sweep_kernel:
     the same medium-size cases must still match the oracle."""
     import os
     import subprocess

@@ -707,7 +707,7 @@ static u32 choose_log_cap(u64 total, u64 hint_distinct, bool estimated, u32 max_
 // stays L2-resident while it is being filled.  Reduce ops on device-resident rows only (the dictionary of group ops
 // must keep row order, host inputs are PCIe-bound anyway).  VEGA_B200_NO_PARTITION=1 disables it.
 struct PassPlan;
-template <typename KeyT, bool HAS_VAL> static PassPlan plan_pass(vb_ctx *c, u64 n, int bits);
+template <typename KeyT, bool HAS_VAL> static PassPlan plan_pass(vb_ctx *c, u64 n);
 template <typename KeyT, bool HAS_VAL>
 static int radix_pass(vb_shuf *s, const Loader &ld, const Digit &dg, u64 n, KeyT *out_keys, u64 *out_vals, u32 *d_hist, const PassPlan &plan,
                       u64 *csr = nullptr, bool *csr_done = nullptr);
@@ -839,18 +839,15 @@ static int build_table(vb_shuf *s, int klass, const std::vector<AggInput> &input
 struct PassPlan {
     u32 num_parts = 0;
     u64 rows_per_part = 0;
-    u32 nb = RP_NB;     // bins of this pass
-    size_t hist_bytes() const { return ((size_t)nb * num_parts + 1) * sizeof(u32); }
+    size_t hist_bytes() const { return ((size_t)RP_NB * num_parts + 1) * sizeof(u32); }
 };
 
-// (LDM, DGM, BITS) combinations the engine uses; anything else is a programming error.
-// Multisplits (hash(K) % R, destination rank) use 8-bit digits, the LSD sorts 10-bit digits.
-#define RP_COMBOS(X)                                                                                           \
-    X(LD_SOA64, DG_BITS, RP_SORT_BITS) X(LD_AOS64, DG_BITS, RP_SORT_BITS)                                       \
-    X(LD_KEY32_VAL_SOA, DG_BITS, RP_SORT_BITS) X(LD_KEY32_VAL_AOS, DG_BITS, RP_SORT_BITS)                       \
-    X(LD_SOA64, DG_BUCKET, 8) X(LD_TABLE_KV, DG_BUCKET, 8) X(LD_TABLE_KI, DG_BUCKET, 8)                         \
-    X(LD_SOA64, DG_DEST, 8) X(LD_AOS64, DG_DEST, 8) X(LD_TABLE_KV, DG_DEST, 8)                                 \
-    X(LD_SOA64, DG_HASHTOP, 8) X(LD_AOS64, DG_HASHTOP, 8)
+// (LDM, DGM) combinations the engine uses; anything else is a programming error.
+#define RP_COMBOS(X)                                                                                 \
+    X(LD_SOA64, DG_BITS) X(LD_AOS64, DG_BITS) X(LD_KEY32_VAL_SOA, DG_BITS) X(LD_KEY32_VAL_AOS, DG_BITS) \
+    X(LD_SOA64, DG_BUCKET) X(LD_TABLE_KV, DG_BUCKET) X(LD_TABLE_KI, DG_BUCKET)                         \
+    X(LD_SOA64, DG_DEST) X(LD_AOS64, DG_DEST) X(LD_TABLE_KV, DG_DEST)                                 \
+    X(LD_SOA64, DG_HASHTOP) X(LD_AOS64, DG_HASHTOP)
 
 template <typename KeyT, int LDM> constexpr bool rp_key_ok()
 {
@@ -858,30 +855,24 @@ template <typename KeyT, int LDM> constexpr bool rp_key_ok()
 }
 
 template <typename KeyT, bool HAS_VAL>
-static const void *scatter_fn(int ldm, int dgm, int bits)
+static const void *scatter_fn(int ldm, int dgm)
 {
-#define X(L, D, B) if (ldm == L && dgm == D && bits == B) { if constexpr (rp_key_ok<KeyT, L>()) return (const void *)rp_scatter_kernel<KeyT, HAS_VAL, L, D, B>; }
+#define X(L, D) if (ldm == L && dgm == D) { if constexpr (rp_key_ok<KeyT, L>()) return (const void *)rp_scatter_kernel<KeyT, HAS_VAL, L, D>; }
     RP_COMBOS(X)
 #undef X
     return nullptr;
 }
 
 template <typename KeyT>
-static const void *hist_fn(int ldm, int dgm, int bits)
+static const void *hist_fn(int ldm, int dgm)
 {
-#define X(L, D, B) if (ldm == L && dgm == D && bits == B) { if constexpr (rp_key_ok<KeyT, L>()) return (const void *)rp_hist_kernel<KeyT, L, D, B>; }
+#define X(L, D) if (ldm == L && dgm == D) { if constexpr (rp_key_ok<KeyT, L>()) return (const void *)rp_hist_kernel<KeyT, L, D>; }
     RP_COMBOS(X)
 #undef X
     return nullptr;
 }
 
-template <typename KeyT, bool HAS_VAL>
-static size_t scatter_smem(int bits)
-{
-    return bits == 8 ? rp_scatter_smem<KeyT, HAS_VAL, 8>() : rp_scatter_smem<KeyT, HAS_VAL, RP_SORT_BITS>();
-}
-
-// The gather sweep (gsweep.cuh) is the scatter of the DG_BITS passes; VEGA_B200_NO_GSWEEP=1 falls back to rp_sweep_kernel<STATIC>.
+// The gather sweep (gsweep.cuh) is the scatter of the DG_BITS passes; VEGA_B200_NO_GSWEEP=1 falls back to rp_sweep_kernel.
 static bool gsweep_enabled()
 {
     static const bool on = getenv("VEGA_B200_NO_GSWEEP") == nullptr;
@@ -907,27 +898,29 @@ static bool gsweep_lookup(int ldm, const void **kern, size_t *smem, u32 *tile, u
 }
 
 template <typename KeyT, bool HAS_VAL>
-static PassPlan plan_pass(vb_ctx *c, u64 n, int bits)
+static PassPlan plan_pass(vb_ctx *c, u64 n)
 {
     PassPlan p;
-    p.nb = 1u << bits;
     if (n == 0) return p;
-    // occupancy is the same for every loader/digit instantiation to within a CTA; use a representative one
-    const void *kern = bits == 8 ? scatter_fn<KeyT, HAS_VAL>(LD_SOA64, DG_BUCKET, 8)
-                                 : (sizeof(KeyT) == 4 ? scatter_fn<KeyT, HAS_VAL>(LD_KEY32_VAL_SOA, DG_BITS, bits)
-                                                      : scatter_fn<KeyT, HAS_VAL>(LD_SOA64, DG_BITS, bits));
-    size_t smem = scatter_smem<KeyT, HAS_VAL>(bits);
-    int occ = 2;
-    if (kern) {
-        cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        occ = occupancy(c, kern, RPS_THREADS, smem);
+    // one part per resident CTA of the scatter that will run
+    int occ;
+    if (gsweep_enabled()) {
+        occ = GsPlan<KeyT, HAS_VAL, (sizeof(KeyT) == 4 ? LD_KEY32_VAL_SOA : LD_SOA64)>::CTAS;
+    } else {
+        // occupancy of rp_scatter_kernel is the same for every loader/digit instantiation to within a CTA; use a representative one
+        const void *kern = scatter_fn<KeyT, HAS_VAL>(LD_SOA64, DG_BUCKET);
+        const size_t smem = rp_scatter_smem<KeyT, HAS_VAL>();
+        occ = 2;
+        if (kern) {
+            cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            occ = occupancy(c, kern, RPS_THREADS, smem);
+        }
+        occ = std::max(occ, sw_ctas<KeyT, HAS_VAL>());
     }
-    if (bits == 8) occ = gsweep_enabled() ? GsPlan<KeyT, HAS_VAL, (sizeof(KeyT) == 4 ? LD_KEY32_VAL_SOA : LD_SOA64)>::CTAS
-                                          : std::max(occ, sw_ctas<KeyT, HAS_VAL>());   // one part per resident CTA of the scatter that will run
     u64 tiles = (n + RP_TILE - 1) / RP_TILE;
     u64 parts = std::min<u64>(tiles, (u64)c->sm_count * occ);
     u64 tiles_per_part = (tiles + parts - 1) / parts;
-    if (bits == 8 && tiles_per_part > 6) tiles_per_part = (tiles_per_part + 5) / 6 * 6;   // 24576-row units: a multiple of every sweep tile (3072 ... 8192 rows)
+    if (tiles_per_part > 6) tiles_per_part = (tiles_per_part + 5) / 6 * 6;   // 24576-row units: a multiple of every sweep tile (3072 ... 8192 rows)
     p.rows_per_part = tiles_per_part * RP_TILE;
     p.num_parts = (u32)((n + p.rows_per_part - 1) / p.rows_per_part);
     return p;
@@ -941,9 +934,8 @@ static int radix_hist_scan(vb_shuf *s, const Loader &ld, const Digit &dg, u64 n,
 {
     vb_ctx *c = s->ctx;
     if (n == 0 || plan.num_parts == 0) return VB_OK;
-    const int bits = plan.nb == 256 ? 8 : RP_SORT_BITS;
-    const void *hk = hist_fn<KeyT>(ld.mode, dg.mode, bits);
-    if (!hk) return set_err(VB_ERR_UNSUPPORTED, "radix pass: loader %d / digit %d / %d bits not instantiated", ld.mode, dg.mode, bits);
+    const void *hk = hist_fn<KeyT>(ld.mode, dg.mode);
+    if (!hk) return set_err(VB_ERR_UNSUPPORTED, "radix pass: loader %d / digit %d not instantiated", ld.mode, dg.mode);
     const u64 tiles_per_part = plan.rows_per_part / RP_TILE;
     u32 split = (u32)std::max<u64>(1, std::min<u64>(tiles_per_part, ((u64)c->sm_count * 6 + plan.num_parts - 1) / plan.num_parts));
     CU(cudaMemsetAsync(d_hist, 0, plan.hist_bytes(), c->stream));
@@ -954,21 +946,39 @@ static int radix_hist_scan(vb_shuf *s, const Loader &ld, const Digit &dg, u64 n,
     {
         KLaunch kl(s, K_RP_HIST, n);
         void *args[] = {&ldc, &dgc, &n, &rows_per_part, &d_hist, &num_parts, &split};
-        const size_t hsmem = rp_hist_smem(bits);
+        const size_t hsmem = rp_hist_smem();
         CU(cudaFuncSetAttribute(hk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hsmem));
         CU(cudaLaunchKernel(hk, dim3(plan.num_parts * split), dim3(RP_THREADS), args, hsmem, c->stream));
         TRY(kl.done("rp_hist_kernel"));
     }
     {
         KLaunch kl(s, K_RP_SCAN);
-        rp_scan_kernel<<<1, 1024, 0, c->stream>>>(d_hist, plan.nb * plan.num_parts);
+        rp_scan_kernel<<<1, 1024, 0, c->stream>>>(d_hist, RP_NB * plan.num_parts);
         TRY(kl.done("rp_scan_kernel"));
     }
     return VB_OK;
 }
 
+// Row-stream loader / digit pairs rp_sweep_kernel is instantiated for (sweep.cuh)
+#define SW_COMBOS_U64V(X) X(LD_SOA64, DG_BITS) X(LD_AOS64, DG_BITS) X(LD_SOA64, DG_DEST) X(LD_AOS64, DG_DEST) X(LD_SOA64, DG_HASHTOP) X(LD_AOS64, DG_HASHTOP) X(LD_SOA64, DG_BUCKET)
+#define SW_COMBOS_U64K(X) X(LD_SOA64, DG_BITS)
+#define SW_COMBOS_U32V(X) X(LD_KEY32_VAL_SOA, DG_BITS) X(LD_KEY32_VAL_AOS, DG_BITS)
+
 template <typename KeyT, bool HAS_VAL>
-static bool sweep_lookup(int ldm, int dgm, const void **kern, const void **hist, size_t *smem, const void **kern_static = nullptr);
+static bool sweep_lookup(int ldm, int dgm, const void **kern, size_t *smem)
+{
+#define X(L, D)                                                      \
+    if (ldm == L && dgm == D) {                                      \
+        *kern = (const void *)rp_sweep_kernel<KeyT, HAS_VAL, L, D>; \
+        *smem = SwSmem<KeyT, HAS_VAL, L>::total;                     \
+        return true;                                                 \
+    }
+    if constexpr (sizeof(KeyT) == 8 && HAS_VAL) { SW_COMBOS_U64V(X) }
+    if constexpr (sizeof(KeyT) == 8 && !HAS_VAL) { SW_COMBOS_U64K(X) }
+    if constexpr (sizeof(KeyT) == 4 && HAS_VAL) { SW_COMBOS_U32V(X) }
+#undef X
+    return false;
+}
 
 template <typename KeyT, bool HAS_VAL>
 static int radix_pass(vb_shuf *s, const Loader &ld, const Digit &dg, u64 n, KeyT *out_keys, u64 *out_vals, u32 *d_hist,
@@ -976,15 +986,14 @@ static int radix_pass(vb_shuf *s, const Loader &ld, const Digit &dg, u64 n, KeyT
 {
     vb_ctx *c = s->ctx;
     if (n == 0 || plan.num_parts == 0) return VB_OK;
-    const int bits = plan.nb == 256 ? 8 : RP_SORT_BITS;
-    const void *sk = scatter_fn<KeyT, HAS_VAL>(ld.mode, dg.mode, bits);
-    if (!sk) return set_err(VB_ERR_UNSUPPORTED, "radix pass: loader %d / digit %d / %d bits not instantiated", ld.mode, dg.mode, bits);
+    const void *sk = scatter_fn<KeyT, HAS_VAL>(ld.mode, dg.mode);
+    if (!sk) return set_err(VB_ERR_UNSUPPORTED, "radix pass: loader %d / digit %d not instantiated", ld.mode, dg.mode);
     TRY((radix_hist_scan<KeyT>(s, ld, dg, n, d_hist, plan)));
     {   // LSD digit passes over row streams: the gather sweep (two 512-thread CTAs per SM, rows stay where the copy engine put them)
         const void *gk = nullptr;
         size_t gsm = 0;
         u32 GT = 0, gthreads = 0;
-        if (gsweep_enabled() && bits == 8 && dg.mode == DG_BITS && n < SW_MAX_ROWS * 2 && plan.rows_per_part % 4096 == 0 &&
+        if (gsweep_enabled() && dg.mode == DG_BITS && n < SW_ROW_LIMIT && plan.rows_per_part % 4096 == 0 &&
             gsweep_lookup<KeyT, HAS_VAL>(ld.mode, &gk, &gsm, &GT, &gthreads) && n >= 4ull * GT &&
             !(((uintptr_t)ld.keys & 15u) || (ld.vals && ((uintptr_t)ld.vals & 15u))) && !(HAS_VAL && ld.mode != LD_AOS64 && !ld.vals)) {
             if (c->occ_cache.find(gk) == c->occ_cache.end()) CU(cudaFuncSetAttribute(gk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gsm));
@@ -1005,8 +1014,6 @@ static int radix_pass(vb_shuf *s, const Loader &ld, const Digit &dg, u64 n, KeyT
                     if (csr_done) *csr_done = true;
                 }
             }
-            static const u32 stagger = getenv("VEGA_B200_GS_STAGGER") ? (u32)atoi(getenv("VEGA_B200_GS_STAGGER")) : 0u;
-            a.stagger_ns = stagger;
             Digit dgs = dg;
             KLaunch kl(s, K_RP_SCATTER, n);
             void *args[] = {&a, &dgs};
@@ -1014,29 +1021,26 @@ static int radix_pass(vb_shuf *s, const Loader &ld, const Digit &dg, u64 n, KeyT
             return kl.done("rp_gsweep_kernel");
         }
     }
-    {   // row streams: the sweep tile pipeline fed by the per-part offsets (no look-back)
-        static const bool off = getenv("VEGA_B200_NO_SWEEP_STATIC") != nullptr;
-        const void *k0 = nullptr, *hk0 = nullptr, *kst = nullptr;
-        size_t sm0 = 0;
+    {   // other row streams: the sweep tile pipeline fed by the per-part offsets
+        const void *sw = nullptr;
+        size_t swsm = 0;
         const u32 T = sw_tile<KeyT, HAS_VAL>();
-        if (!off && bits == 8 && n < SW_MAX_ROWS * 2 && plan.rows_per_part % T == 0 && n >= 4ull * T &&
-            sweep_lookup<KeyT, HAS_VAL>(ld.mode, dg.mode, &k0, &hk0, &sm0, &kst) &&
+        if (n < SW_ROW_LIMIT && plan.rows_per_part % T == 0 && n >= 4ull * T && sweep_lookup<KeyT, HAS_VAL>(ld.mode, dg.mode, &sw, &swsm) &&
             !(((uintptr_t)ld.keys & 15u) || (ld.vals && ((uintptr_t)ld.vals & 15u))) && !(HAS_VAL && ld.mode != LD_AOS64 && !ld.vals)) {
-            if (c->occ_cache.find(kst) == c->occ_cache.end()) CU(cudaFuncSetAttribute(kst, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm0));
-            (void)occupancy(c, kst, sw_threads<KeyT, HAS_VAL>(), sm0);
+            if (c->occ_cache.find(sw) == c->occ_cache.end()) CU(cudaFuncSetAttribute(sw, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)swsm));
+            (void)occupancy(c, sw, sw_threads<KeyT, HAS_VAL>(), swsm);
             SweepArgs a{};
             a.keys = ld.keys; a.vals = ld.vals; a.n = n; a.n_tiles = (u32)((n + T - 1) / T);
-            a.tile_counter = nullptr; a.state = nullptr; a.digit_base = nullptr;
             a.out_keys = out_keys; a.out_vals = out_vals;
             a.part_off = d_hist; a.num_parts = plan.num_parts; a.rows_per_part = plan.rows_per_part;
             Digit dgs = dg;
             KLaunch kl(s, K_RP_SCATTER, n);
             void *args[] = {&a, &dgs};
-            CU(cudaLaunchKernel(kst, dim3(plan.num_parts), dim3(sw_threads<KeyT, HAS_VAL>()), args, sm0, c->stream));
-            return kl.done("rp_sweep_kernel<STATIC>");
+            CU(cudaLaunchKernel(sw, dim3(plan.num_parts), dim3(sw_threads<KeyT, HAS_VAL>()), args, swsm, c->stream));
+            return kl.done("rp_sweep_kernel");
         }
     }
-    const size_t smem = scatter_smem<KeyT, HAS_VAL>(bits);
+    const size_t smem = rp_scatter_smem<KeyT, HAS_VAL>();
     CU(cudaFuncSetAttribute(sk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     u64 rows_per_part = plan.rows_per_part;
     u32 num_parts = plan.num_parts;
@@ -1053,108 +1057,6 @@ static int radix_pass(vb_shuf *s, const Loader &ld, const Digit &dg, u64 n, KeyT
     return VB_OK;
 }
 
-// ---------------------------------------------------------------------------------------------
-// sweep pass (sweep.cuh): one kernel per pass, decoupled look-back, copy-engine staged input
-// ---------------------------------------------------------------------------------------------
-#define SW_COMBOS_U64V(X) X(LD_SOA64, DG_BITS) X(LD_AOS64, DG_BITS) X(LD_SOA64, DG_DEST) X(LD_AOS64, DG_DEST) X(LD_SOA64, DG_HASHTOP) X(LD_AOS64, DG_HASHTOP) X(LD_SOA64, DG_BUCKET)
-#define SW_COMBOS_U64K(X) X(LD_SOA64, DG_BITS)
-#define SW_COMBOS_U32V(X) X(LD_KEY32_VAL_SOA, DG_BITS) X(LD_KEY32_VAL_AOS, DG_BITS)
-
-template <typename KeyT, bool HAS_VAL>
-static bool sweep_lookup(int ldm, int dgm, const void **kern, const void **hist, size_t *smem, const void **kern_static)
-{
-#define X(L, D)                                                                                   \
-    if (ldm == L && dgm == D) {                                                                   \
-        *kern = (const void *)rp_sweep_kernel<KeyT, HAS_VAL, L, D>;                               \
-        if (kern_static) *kern_static = (const void *)rp_sweep_kernel<KeyT, HAS_VAL, L, D, true>; \
-        *hist = (const void *)sw_hist_all_kernel<KeyT, L, D>;                                     \
-        *smem = SwSmem<KeyT, HAS_VAL, L>::total;                                                  \
-        return true;                                                                              \
-    }
-    if constexpr (sizeof(KeyT) == 8 && HAS_VAL) { SW_COMBOS_U64V(X) }
-    if constexpr (sizeof(KeyT) == 8 && !HAS_VAL) { SW_COMBOS_U64K(X) }
-    if constexpr (sizeof(KeyT) == 4 && HAS_VAL) { SW_COMBOS_U32V(X) }
-#undef X
-    return false;
-}
-
-// The one-kernel (look-back) pass is OPT-IN (VEGA_B200_SWEEP=1): at the chip-wide tile rate the decoupled look-back needs
-// tens of predecessors per tile (windows of 16 status words, each an L2 round trip spent behind a barrier), which puts the
-// pass on par with histogram + scan + scatter, not ahead of it.  The same tile pipeline WITHOUT
-// the look-back (rp_sweep_kernel<STATIC>, fed by the per-part offsets) is the default scatter for row streams (radix_pass).
-static bool sweep_enabled()
-{
-    static const bool on = getenv("VEGA_B200_SWEEP") != nullptr && getenv("VEGA_B200_NO_SWEEP") == nullptr;
-    return on;
-}
-
-// rows of `ld` must be a plain row stream (every row valid) with 16-byte aligned column bases
-template <typename KeyT, bool HAS_VAL>
-static bool sweep_applicable(const Loader &ld, const Digit &dg, u64 n)
-{
-    const void *k, *h; size_t sm;
-    if (!sweep_enabled() || n == 0 || n >= SW_MAX_ROWS) return false;
-    if (!sweep_lookup<KeyT, HAS_VAL>(ld.mode, dg.mode, &k, &h, &sm)) return false;
-    if (((uintptr_t)ld.keys & 15u) || (ld.vals && ((uintptr_t)ld.vals & 15u))) return false;
-    if (HAS_VAL && ld.mode != LD_AOS64 && !ld.vals) return false;       // key-only rows in a (key, value) pass: the rp_* kernels fill zeros
-    return true;
-}
-
-// Global histogram of `n_pos` digit positions in one read of the keys, scanned in place: d_bases[p][256].
-template <typename KeyT, bool HAS_VAL>
-static int sweep_hist(vb_shuf *s, const Loader &ld, const Digit &dg, u64 n, const HistAllArgs &ha, u32 *d_bases)
-{
-    vb_ctx *c = s->ctx;
-    const void *kern, *hk; size_t smem;
-    if (!sweep_lookup<KeyT, HAS_VAL>(ld.mode, dg.mode, &kern, &hk, &smem)) return set_err(VB_ERR_UNSUPPORTED, "sweep: loader %d / digit %d not instantiated", ld.mode, dg.mode);
-    CU(cudaMemsetAsync(d_bases, 0, (size_t)ha.n_pos * SW_NB * 4, c->stream));
-    Loader ldc = ld; Digit dgc = dg; HistAllArgs hac = ha;
-    {
-        KLaunch kl(s, K_RP_HIST, n);
-        const unsigned grid = (unsigned)std::min<u64>((n + 2047) / 2048, (u64)c->sm_count * 4);
-        void *args[] = {&ldc, &dgc, &n, &hac, &d_bases};
-        CU(cudaLaunchKernel(hk, dim3(grid), dim3(512), args, 0, c->stream));
-        TRY(kl.done("sw_hist_all_kernel"));
-    }
-    {
-        KLaunch kl(s, K_RP_SCAN);
-        sw_scan_bases_kernel<<<ha.n_pos, SW_NB, 0, c->stream>>>(d_bases, ha.n_pos);
-        TRY(kl.done("sw_scan_bases_kernel"));
-    }
-    return VB_OK;
-}
-
-// One stable pass with the digit bases already on the device.  `scratch` (>= sweep_scratch_bytes) is reused across passes.
-template <typename KeyT, bool HAS_VAL>
-static size_t sweep_scratch_bytes(u64 n)
-{
-    const u64 tiles = (n + sw_tile<KeyT, HAS_VAL>() - 1) / sw_tile<KeyT, HAS_VAL>();
-    return (size_t)(tiles * SW_NB + 4) * 4;
-}
-
-template <typename KeyT, bool HAS_VAL>
-static int sweep_pass(vb_shuf *s, const Loader &ld, const Digit &dg, u64 n, KeyT *out_keys, u64 *out_vals, const u32 *d_base, u32 *scratch)
-{
-    vb_ctx *c = s->ctx;
-    const void *kern, *hk; size_t smem;
-    if (!sweep_lookup<KeyT, HAS_VAL>(ld.mode, dg.mode, &kern, &hk, &smem)) return set_err(VB_ERR_UNSUPPORTED, "sweep: loader %d / digit %d not instantiated", ld.mode, dg.mode);
-    const u32 T = sw_tile<KeyT, HAS_VAL>();
-    const u32 tiles = (u32)((n + T - 1) / T);
-    CU(cudaMemsetAsync(scratch, 0, sweep_scratch_bytes<KeyT, HAS_VAL>(n), c->stream));
-    if (c->occ_cache.find(kern) == c->occ_cache.end()) CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const int occ = occupancy(c, kern, sw_threads<KeyT, HAS_VAL>(), smem);
-    SweepArgs a;
-    a.keys = ld.keys; a.vals = ld.vals; a.n = n; a.n_tiles = tiles;
-    a.tile_counter = scratch; a.state = scratch + 4;
-    a.digit_base = d_base; a.out_keys = out_keys; a.out_vals = out_vals;
-    Digit dgc = dg;
-    KLaunch kl(s, K_RP_SCATTER, n);
-    const unsigned grid = (unsigned)std::min<u64>(tiles, (u64)c->sm_count * occ);
-    void *args[] = {&a, &dgc};
-    CU(cudaLaunchKernel(kern, dim3(grid), dim3(sw_threads<KeyT, HAS_VAL>()), args, smem, c->stream));
-    return kl.done("rp_sweep_kernel");
-}
-
 static int launch_hash_agg_partitioned(vb_shuf *s, int klass, int in, int opk, int tx, const u64 *a, const u64 *b, u64 n, void *tab,
                                        u32 log_cap, TableCtl *ctl, u64 mi)
 {
@@ -1163,22 +1065,13 @@ static int launch_hash_agg_partitioned(vb_shuf *s, int klass, int in, int opk, i
     DevBuf tk(c), tv(c), hist(c);
     TRY(tk.alloc(n * 8));
     TRY(tv.alloc(n * 8));
-    PassPlan plan = plan_pass<u64, true>(c, n, 8);
+    PassPlan plan = plan_pass<u64, true>(c, n);
     TRY(hist.alloc(plan.hist_bytes()));
     Loader ld = (in == IN_AOS) ? Loader{LD_AOS64, a, nullptr, 0} : Loader{LD_SOA64, a, b, 0};
     Digit dg{};
     dg.mode = DG_HASHTOP;
     dg.shift = 64 - pbits;
     dg.mask = (1u << pbits) - 1;
-    if (sweep_applicable<u64, true>(ld, dg, n)) {
-        DevBuf bases(c), scratch(c);
-        TRY(bases.alloc(SW_NB * 4));
-        TRY(scratch.alloc((sweep_scratch_bytes<u64, true>(n))));
-        HistAllArgs ha{}; ha.n_pos = 1;
-        TRY((sweep_hist<u64, true>(s, ld, dg, n, ha, bases.as<u32>())));
-        TRY((sweep_pass<u64, true>(s, ld, dg, n, tk.as<u64>(), tv.as<u64>(), bases.as<u32>(), scratch.as<u32>())));
-        return launch_hash_agg(s, klass, IN_SOA, opk, tx, tk.as<u64>(), tv.as<u64>(), n, tab, log_cap, ctl, mi, nullptr);
-    }
     TRY((radix_pass<u64, true>(s, ld, dg, n, tk.as<u64>(), tv.as<u64>(), hist.as<u32>(), plan)));
     // stream-ordered frees: the buffers outlive the kernels queued on c->stream
     return launch_hash_agg(s, klass, IN_SOA, opk, tx, tk.as<u64>(), tv.as<u64>(), n, tab, log_cap, ctl, mi, nullptr);
@@ -1258,24 +1151,7 @@ static int multisplit(vb_shuf *s, const Loader &ld, u64 n, int mode, u32 nbins, 
     vb_ctx *c = s->ctx;
     bin_off.assign((size_t)nbins + 1, 0);
     if (n == 0) return VB_OK;
-    if (nbins <= RP_NB) {
-        Digit dg = make_bucket_digit(s, mode, 0, 0xFFFFFFFFu);
-        if (sweep_applicable<u64, true>(ld, dg, n)) {          // row streams: one look-back pass + one histogram read
-            DevBuf bases(c), scratch(c);
-            TRY(bases.alloc(SW_NB * 4));
-            TRY(scratch.alloc((sweep_scratch_bytes<u64, true>(n))));
-            HistAllArgs ha{}; ha.n_pos = 1;
-            TRY((sweep_hist<u64, true>(s, ld, dg, n, ha, bases.as<u32>())));
-            TRY((sweep_pass<u64, true>(s, ld, dg, n, out_keys, out_vals, bases.as<u32>(), scratch.as<u32>())));
-            u32 *h = (u32 *)c->h_scratch;
-            CU(cudaMemcpyAsync(h, bases.p, SW_NB * 4, cudaMemcpyDeviceToHost, c->stream));
-            CU(cudaStreamSynchronize(c->stream));
-            for (u32 d = 0; d < nbins; ++d) bin_off[d] = h[d];
-            bin_off[nbins] = n;
-            return VB_OK;
-        }
-    }
-    PassPlan plan = plan_pass<u64, true>(c, n, 8);
+    PassPlan plan = plan_pass<u64, true>(c, n);
     DevBuf hist(c);
     TRY(hist.alloc(plan.hist_bytes()));
     if (nbins <= RP_NB) {
@@ -1295,7 +1171,7 @@ static int multisplit(vb_shuf *s, const Loader &ld, u64 n, int mode, u32 nbins, 
     TRY(fetch_offsets(c, hist.as<u32>(), plan, RP_NB, tmp.data()));
     const u64 nv = tmp[RP_NB];
     if (nv == 0) return VB_OK;
-    PassPlan plan2 = plan_pass<u64, true>(c, nv, 8);
+    PassPlan plan2 = plan_pass<u64, true>(c, nv);
     DevBuf hist2(c);
     TRY(hist2.alloc(plan2.hist_bytes()));
     Loader l2{LD_SOA64, tk.p, tv.p, 0};
@@ -1325,53 +1201,14 @@ static int sort_id_pairs(vb_shuf *s, u32 *ids_a, const Loader &first, u64 n, u32
                          u64 *csr = nullptr, bool *csr_done = nullptr)
 {
     vb_ctx *c = s->ctx;
-    const u32 passes = std::max<u32>(1, (bits + RP_SORT_BITS - 1) / RP_SORT_BITS);
+    const u32 passes = std::max<u32>(1, (bits + 7) / 8);
     if (xlat) {                               // slot ids -> dense ids, in place
         KLaunch kl(s, K_MISC);
         u64 blocks = std::min<u64>((n + 255) / 256, (u64)c->sm_count * 8);
         translate_ids_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(ids_a, n, xlat);
         TRY(kl.done("translate_ids_kernel"));
     }
-    {
-        Loader probe = first;
-        probe.keys = ids_a;
-        Digit dgp{};
-        dgp.mode = DG_BITS;
-        if (sweep_applicable<u32, true>(probe, dgp, n) && RP_SORT_BITS == 8) {
-            // sweep path: ONE histogram read for all digit positions, then one look-back kernel per pass
-            DevBuf bases(c), scratch(c), ids_b(c), vals_a(c), vals_b(c);
-            TRY(bases.alloc((size_t)passes * SW_NB * 4));
-            TRY(scratch.alloc((sweep_scratch_bytes<u32, true>(n))));
-            TRY(ids_b.alloc(n * 4));
-            TRY(vals_b.alloc(n * 8));
-            if (passes >= 2) TRY(vals_a.alloc(n * 8));
-            HistAllArgs ha{};
-            ha.n_pos = passes;
-            for (u32 p = 0; p < passes; ++p) ha.shifts[p] = 8 * p;
-            Loader lk{LD_KEY32_VAL_SOA, ids_a, nullptr, 0};
-            TRY((sweep_hist<u32, true>(s, lk, dgp, n, ha, bases.as<u32>())));
-            u32 *src_ids = ids_a, *dst_ids = ids_b.as<u32>();
-            u64 *src_vals = nullptr, *dst_vals = vals_b.as<u64>();
-            for (u32 p = 0; p < passes; ++p) {
-                Loader ld = first;
-                if (p == 0) ld.keys = src_ids;
-                else ld = Loader{LD_KEY32_VAL_SOA, src_ids, src_vals, 0};
-                Digit dg{};
-                dg.mode = DG_BITS; dg.shift = 8 * p; dg.mask = 0xFF; dg.tx = TX_NONE;
-                TRY((sweep_pass<u32, true>(s, ld, dg, n, dst_ids, dst_vals, bases.as<u32>() + (size_t)p * SW_NB, scratch.as<u32>())));
-                std::swap(src_ids, dst_ids);
-                u64 *nv = (src_vals == nullptr) ? vals_a.as<u64>() : src_vals;
-                src_vals = dst_vals;
-                dst_vals = nv;
-            }
-            *out_ids = src_ids;
-            *out_vals = src_vals;
-            if (src_ids == ids_b.as<u32>()) ids_b.release();
-            if (src_vals == vals_b.as<u64>()) vals_b.release(); else vals_a.release();
-            return VB_OK;
-        }
-    }
-    PassPlan plan = plan_pass<u32, true>(c, n, RP_SORT_BITS);
+    PassPlan plan = plan_pass<u32, true>(c, n);
     DevBuf hist(c), ids_b(c), vals_a(c), vals_b(c);
     TRY(hist.alloc(plan.hist_bytes()));
     TRY(ids_b.alloc(n * 4));
@@ -1385,8 +1222,8 @@ static int sort_id_pairs(vb_shuf *s, u32 *ids_a, const Loader &first, u64 n, u32
         else ld = Loader{LD_KEY32_VAL_SOA, src_ids, src_vals, 0};
         Digit dg{};
         dg.mode = DG_BITS;
-        dg.shift = RP_SORT_BITS * p;
-        dg.mask = (1u << RP_SORT_BITS) - 1;
+        dg.shift = 8 * p;
+        dg.mask = 0xFF;
         dg.tx = TX_NONE;
         const bool last = (p + 1 == passes);
         TRY((radix_pass<u32, true>(s, ld, dg, n, dst_ids, dst_vals, hist.as<u32>(), plan, last ? csr : nullptr, last ? csr_done : nullptr)));
@@ -1951,56 +1788,11 @@ static int seal_sort(vb_shuf *s, const Gathered &g)
     TRY(kb.alloc(n * 8));
     if (has_val) { TRY(va.alloc(n * 8)); TRY(vbuf.alloc(n * 8)); }
     u64 *src_k = nullptr, *src_v = nullptr, *dst_k = ka.as<u64>(), *dst_v = va.as<u64>();
-    constexpr u32 SORT_PASSES = (64 + RP_SORT_BITS - 1) / RP_SORT_BITS;
-    bool swept = false;
-    {
-        Loader l0 = g.rows ? Loader{LD_AOS64, g.rows, nullptr, 0} : Loader{LD_SOA64, g.keys, g.vals, 0};
-        Digit dgp{};
-        dgp.mode = DG_BITS; dgp.tx = tx;
-        const bool ok = RP_SORT_BITS == 8 && (has_val ? sweep_applicable<u64, true>(l0, dgp, n) : sweep_applicable<u64, false>(l0, dgp, n));
-        if (ok) {
-            // sweep path: all 8 digit histograms from ONE read of the keys; a digit on which every key agrees (one bin
-            // holds all n rows) needs no pass; then one look-back kernel per remaining digit
-            DevBuf bases(c), scratch(c);
-            TRY(bases.alloc((size_t)8 * SW_NB * 4));
-            TRY(scratch.alloc(std::max(sweep_scratch_bytes<u64, true>(n), sweep_scratch_bytes<u64, false>(n))));
-            HistAllArgs ha{};
-            ha.n_pos = 8;
-            for (u32 p = 0; p < 8; ++p) ha.shifts[p] = 8 * p;
-            if (has_val) TRY((sweep_hist<u64, true>(s, l0, dgp, n, ha, bases.as<u32>())));
-            else TRY((sweep_hist<u64, false>(s, l0, dgp, n, ha, bases.as<u32>())));
-            u32 *hb = (u32 *)c->h_scratch;
-            CU(cudaMemcpyAsync(hb, bases.p, 8 * SW_NB * 4, cudaMemcpyDeviceToHost, c->stream));
-            CU(cudaStreamSynchronize(c->stream));
-            bool vary[8];
-            u32 n_vary = 0;
-            for (u32 p = 0; p < 8; ++p) {          // exclusive scan of a one-bin histogram: every base is 0 or n
-                vary[p] = false;
-                for (u32 d = 0; d < SW_NB; ++d) { const u32 b = hb[p * SW_NB + d]; if (b != 0 && b != (u32)n) { vary[p] = true; break; } }
-                n_vary += vary[p];
-            }
-            if (n_vary == 0) vary[0] = true;      // at least one pass: it also copies the rows out
-            bool first = true;
-            for (u32 p = 0; p < 8; ++p) {
-                if (!vary[p]) continue;
-                Loader ld = first ? l0 : Loader{LD_SOA64, src_k, has_val ? src_v : nullptr, 0};
-                first = false;
-                Digit dg{};
-                dg.mode = DG_BITS; dg.shift = 8 * p; dg.mask = 0xFF; dg.tx = tx;
-                if (has_val) TRY((sweep_pass<u64, true>(s, ld, dg, n, dst_k, dst_v, bases.as<u32>() + (size_t)p * SW_NB, scratch.as<u32>())));
-                else TRY((sweep_pass<u64, false>(s, ld, dg, n, dst_k, nullptr, bases.as<u32>() + (size_t)p * SW_NB, scratch.as<u32>())));
-                u64 *nk = (src_k == nullptr) ? kb.as<u64>() : src_k;
-                u64 *nv = (src_v == nullptr) ? vbuf.as<u64>() : src_v;
-                src_k = dst_k; src_v = dst_v; dst_k = nk; dst_v = nv;
-            }
-            swept = true;
-        }
-    }
-    PassPlan plan = has_val ? plan_pass<u64, true>(c, n, RP_SORT_BITS) : plan_pass<u64, false>(c, n, RP_SORT_BITS);
-    if (!swept) TRY(hist.alloc(plan.hist_bytes()));
+    PassPlan plan = has_val ? plan_pass<u64, true>(c, n) : plan_pass<u64, false>(c, n);
+    TRY(hist.alloc(plan.hist_bytes()));
     // digits on which all keys agree are skipped (e.g. 32-bit-range keys take 4 passes, not 8)
-    u64 varying = ~0ull;
-    if (!swept) {
+    u64 varying;
+    {
         DevBuf bits(c);
         TRY(bits.alloc(16));
         const unsigned long long init[2] = {0ull, ~0ull};
@@ -2015,9 +1807,9 @@ static int seal_sort(vb_shuf *s, const Gathered &g)
     }
     bool first = true;
     u32 done = 0;
-    for (u32 p = 0; p < SORT_PASSES && !swept; ++p) {
-        const u64 dmask = (u64)((1u << RP_SORT_BITS) - 1) << (RP_SORT_BITS * p);
-        const bool last_chance = (p + 1 == SORT_PASSES) && done == 0;      // at least one pass: it also copies the rows out
+    for (u32 p = 0; p < 8; ++p) {
+        const u64 dmask = 0xFFull << (8 * p);
+        const bool last_chance = p == 7 && done == 0;      // at least one pass: it also copies the rows out
         if (!(varying & dmask) && !last_chance) continue;
         ++done;
         Loader ld;
@@ -2025,7 +1817,7 @@ static int seal_sort(vb_shuf *s, const Gathered &g)
         else ld = Loader{LD_SOA64, src_k, has_val ? src_v : nullptr, 0};
         first = false;
         Digit dg{};
-        dg.mode = DG_BITS; dg.shift = RP_SORT_BITS * p; dg.mask = (1u << RP_SORT_BITS) - 1; dg.tx = tx;
+        dg.mode = DG_BITS; dg.shift = 8 * p; dg.mask = 0xFF; dg.tx = tx;
         if (has_val) TRY((radix_pass<u64, true>(s, ld, dg, n, dst_k, dst_v, hist.as<u32>(), plan)));
         else TRY((radix_pass<u64, false>(s, ld, dg, n, dst_k, nullptr, hist.as<u32>(), plan)));
         u64 *nk = (src_k == nullptr) ? kb.as<u64>() : src_k;
@@ -2212,7 +2004,7 @@ static int export_counts_locked(vb_shuf *s, uint64_t *counts)
     s->exp_rows = g.rows; s->exp_k = g.keys; s->exp_v = g.vals; s->exp_n = g.n;
     s->exp_digit_start.assign((size_t)s->world + 1, 0);
     if (g.n) {
-        PassPlan plan = plan_pass<u64, true>(c, g.n, 8);
+        PassPlan plan = plan_pass<u64, true>(c, g.n);
         DevBuf hist(c);
         TRY(hist.alloc(plan.hist_bytes()));
         Loader ld = g.rows ? Loader{LD_AOS64, g.rows, nullptr, 0} : Loader{LD_SOA64, g.keys, g.vals, 0};
@@ -2272,9 +2064,9 @@ static int export_direct_locked(vb_shuf *s, const uint64_t *dst_row_offset, cons
         CU(cudaMemcpyAsync(da.p, hadj.data(), W * 4, cudaMemcpyHostToDevice, c->stream));
         Loader ld = s->exp_rows ? Loader{LD_AOS64, s->exp_rows, nullptr, 0} : Loader{LD_SOA64, s->exp_k, s->exp_v, 0};
         Digit dg = make_bucket_digit(s, DG_DEST, 0, 0xFFFFFFFFu);
-        const void *sk = s->exp_rows ? (const void *)rp_scatter_kernel<u64, true, LD_AOS64, DG_DEST, 8, true>
-                                     : (const void *)rp_scatter_kernel<u64, true, LD_SOA64, DG_DEST, 8, true>;
-        const size_t smem = scatter_smem<u64, true>(8);
+        const void *sk = s->exp_rows ? (const void *)rp_scatter_kernel<u64, true, LD_AOS64, DG_DEST, true>
+                                     : (const void *)rp_scatter_kernel<u64, true, LD_SOA64, DG_DEST, true>;
+        const size_t smem = rp_scatter_smem<u64, true>();
         CU(cudaFuncSetAttribute(sk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         u64 n = s->exp_n, rpp = s->exp_rows_per_part;
         u32 np = s->exp_parts;

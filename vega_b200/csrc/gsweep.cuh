@@ -1,6 +1,6 @@
 // gsweep.cuh — the scatter of the LSD sort passes (DG_BITS digits), third generation.
 //
-// rp_sweep_kernel<STATIC> spends half of a pass issue-bound in the ballot ranking and the other half bound by the
+// rp_sweep_kernel spends half of a pass issue-bound in the ballot ranking and the other half bound by the
 // shared-memory pipe while it permutes whole rows into a staging buffer (bank conflicts; mio_throttle + short_scoreboard
 // stalls) — one after the other, separated by CTA barriers, with nothing else resident on the SM to fill the idle unit.
 // This kernel changes three things:
@@ -151,7 +151,6 @@ rp_gsweep_kernel(SweepArgs a, Digit dg)
 
     for (u32 d = tid; d < SW_NB; d += THREADS) run_off[d] = a.part_off[(size_t)d * a.num_parts + blockIdx.x];
     for (u32 i = lane; i < SW_NB / 2; i += 32) ((u32 *)my_cnt)[i] = 0;
-    if (a.stagger_ns && blockIdx.x >= (gridDim.x + 1) / 2) __nanosleep(a.stagger_ns);   // timing experiments only
     if (tid == 0) {
         mbar_init(&bar_k[0], 1);
         mbar_init(&bar_k[1], 1);
@@ -197,7 +196,7 @@ rp_gsweep_kernel(SweepArgs a, Digit dg)
 #pragma unroll
         for (int i = 0; i < K; ++i) {
             const u32 d = dr[i];
-            const u32 peers = FULL ? match_digit8(d) : warp_match_digit<8>(d);
+            const u32 peers = FULL ? match_digit8(d) : warp_match_digit(d);
             const u32 lower = peers & lt;
             u32 base = 0;
             if (FULL || d < SW_NB) base = my_cnt[d];                      // every lane of the group reads the same counter

@@ -978,12 +978,12 @@ constexpr int RP_THREADS = 256;
 constexpr int RP_WARPS = RP_THREADS / 32;
 constexpr int RP_TILE = VB_RP_TILE;              // rows per tile
 constexpr int RP_ITEMS = RP_TILE / RP_THREADS;   // histogram kernel: items per thread per tile
-constexpr int RP_NB = 256;                       // bins of an 8-bit pass (multisplit); bin NB = "invalid, drop"
+constexpr int RP_NB = 256;                       // bins of a pass: 8-bit digits; bin RP_NB = "invalid, drop"
 constexpr int RPS_THREADS = VB_RPS_THREADS;      // scatter kernel: 16 warps x 8 items cover the same 4096-row tile with
 constexpr int RPS_WARPS = RPS_THREADS / 32;      // <= 64 registers/thread, so 2 CTAs = 32 warps stay resident per SM
 constexpr int RPS_ITEMS = RP_TILE / RPS_THREADS; // (256 x 16 needed 128 registers: 16 warps/SM, issue slots 32 % busy)
-constexpr int RP_SORT_BITS = 8;                  // digit width of the LSD sort passes; a 10-bit variant was slower per pass
-                                                 // (per-tile scan over 1025 bins + 4-row write runs)
+// Every pass, the LSD sort passes included, uses 8-bit digits: a 10-bit variant of the sort was slower per pass
+// (per-tile scan over 1025 bins + 4-row write runs).
 
 enum : int { LD_SOA64 = 0, LD_AOS64 = 1, LD_KEY32_VAL_SOA = 2, LD_KEY32_VAL_AOS = 3, LD_TABLE_KV = 4, LD_TABLE_KI = 5 };
 
@@ -1070,15 +1070,14 @@ VB_D u32 rp_digit(const Digit &dg, KeyT key)
     }
 }
 
-// Lanes of the warp whose (BITS+1)-bit digit equals mine.  Built from BITS+1 ballots instead of
-// MATCH.ANY: the hardware match iterates over the distinct values in the warp (~30 for random
+// Lanes of the warp whose 9-bit digit (8 digit bits + the "invalid" bit RP_NB) equals mine.  Built from 9 ballots
+// instead of MATCH.ANY: the hardware match iterates over the distinct values in the warp (~30 for random
 // digits) and dominated both radix kernels (short_scoreboard stalls).
-template <int BITS>
 VB_D u32 warp_match_digit(u32 d)
 {
     u32 peers = 0xffffffffu;
 #pragma unroll
-    for (int b = 0; b <= BITS; ++b) {          // BITS digit bits + the "invalid" bit
+    for (int b = 0; b <= 8; ++b) {
         const bool bit = (d >> b) & 1u;
         const u32 m = __ballot_sync(0xffffffffu, bit);
         peers &= bit ? m : ~m;
@@ -1095,13 +1094,13 @@ VB_D u32 warp_match_digit(u32 d)
 // pc[warp][digit][lane] in shared memory: an item is one LDS.U8 / IADD / STS.U8, no atomics, no votes.
 // A thread adds at most RP_ITEMS per tile, so the bytes are folded into the CTA's u32 histogram
 // every 255 / RP_ITEMS tiles (15 * 16 = 240 <= 255).
-constexpr size_t rp_hist_smem(int bits) { return (size_t)RP_WARPS * ((size_t)1 << bits) * 32; }
+constexpr size_t rp_hist_smem() { return (size_t)RP_WARPS * RP_NB * 32; }
 
-template <typename KeyT, int LDM, int DGM, int BITS>
+template <typename KeyT, int LDM, int DGM>
 __global__ void __launch_bounds__(RP_THREADS)
 rp_hist_kernel(Loader ld, Digit dg, u64 n, u64 rows_per_part, u32 *__restrict__ hist, u32 num_parts, u32 split)
 {
-    constexpr int NB = 1 << BITS;
+    constexpr int NB = RP_NB;
     extern __shared__ __align__(16) unsigned char pc_raw[];        // [RP_WARPS][NB][32] byte counters
     __shared__ u32 cta_hist[NB];
     const u32 tid = threadIdx.x, warp = tid >> 5, lane = tid & 31u;
@@ -1232,12 +1231,12 @@ struct RemoteDst {
 // destination rank locally and handing the buffers to an all-to-all, the staged runs are stored straight
 // into the destination GPUs' HBM (st.global on peer-mapped addresses), so the NVLink transfer overlaps
 // ranking/staging of the following tiles.
-template <typename KeyT, bool HAS_VAL, int LDM, int DGM, int BITS, bool REMOTE = false>
+template <typename KeyT, bool HAS_VAL, int LDM, int DGM, bool REMOTE = false>
 __global__ void __launch_bounds__(RPS_THREADS, (RPS_THREADS > 512 ? 1 : RPS_THREADS > 256 ? 2 : 4))
 rp_scatter_kernel(Loader ld, Digit dg, u64 n, u64 rows_per_part, const u32 *__restrict__ part_off, u32 num_parts,
                   KeyT *__restrict__ out_keys, u64 *__restrict__ out_vals, RemoteDst rd)
 {
-    constexpr int NB = 1 << BITS;
+    constexpr int NB = RP_NB;
     static_assert(NB <= RPS_THREADS, "one thread per digit in the tile scan");
     extern __shared__ __align__(16) unsigned char smem_raw[];
     u64 *stage_vals = (u64 *)smem_raw;                                       // [RP_TILE] if HAS_VAL
@@ -1292,7 +1291,7 @@ rp_scatter_kernel(Loader ld, Digit dg, u64 n, u64 rows_per_part, const u32 *__re
 #pragma unroll
         for (int i = 0; i < RPS_ITEMS; ++i) {
             const u32 d = dig[i];
-            const u32 peers = warp_match_digit<BITS>(d);
+            const u32 peers = warp_match_digit(d);
             const u32 leader = (u32)(__ffs(peers) - 1);
             u32 base = 0;
             if (lane == leader) { base = cnt[warp][d]; cnt[warp][d] = base + __popc(peers); }   // only the group leader touches smem
@@ -1365,7 +1364,7 @@ rp_scatter_kernel(Loader ld, Digit dg, u64 n, u64 rows_per_part, const u32 *__re
     }
 }
 
-template <typename KeyT, bool HAS_VAL, int BITS>
+template <typename KeyT, bool HAS_VAL>
 constexpr size_t rp_scatter_smem() { return (size_t)RP_TILE * ((HAS_VAL ? 8 : 0) + sizeof(KeyT) + ((sizeof(KeyT) == 8 && HAS_VAL) ? 1 : 4)); }
 
 // ---------------------------------------------------------------------------------------------

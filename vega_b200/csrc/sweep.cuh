@@ -1,14 +1,15 @@
-// sweep.cuh — the radix pass as ONE kernel per pass.
+// sweep.cuh — the scatter of a radix pass over row streams that the gather sweep (gsweep.cuh) does not take:
+// the multisplits (DG_BUCKET, DG_DEST, DG_HASHTOP digits) and, with VEGA_B200_NO_GSWEEP=1, the LSD sort passes.
 //
+//   * offsets come from the per-part histogram (rp_hist_kernel + rp_scan_kernel): CTA p walks its own contiguous
+//     part of the input and keeps running digit offsets in shared memory;
 //   * input tiles are staged global → shared by the copy engine (cp.async.bulk + mbarrier): no registers,
 //     no LSU instructions for the stream, and the next tile's copy is in flight while the current tile is
 //     scanned, staged and written out;
-//   * tiles are claimed in order from an atomic counter and chained with a decoupled look-back
-//     (per (tile, digit) status words), so there is no per-part histogram kernel and no scan kernel per pass —
-//     the only other kernel is ONE histogram pass that counts every digit position of the key at once;
-//   * 4 CTA barriers per tile (the old rp_scatter_kernel had 5): warp-private u16 counters are cleared by their
+//   * 4 CTA barriers per tile (rp_scatter_kernel has 5): warp-private u16 counters are cleared by their
 //     own warp, the staging buffer is only rewritten after the next tile's third barrier.
 //
+// With the CTA shape picked per row type (sw_threads) it is faster than rp_scatter_kernel on 1e9 rows.
 // Stable: rows keep their input order inside every digit (tile order → warp order → lane-striped item order),
 // which the LSD sort and the group value order (SURVEY §8a, tests/test_pair_rdd.rs:30-36) rely on.
 // Handles the row-stream loaders (all rows valid); table loaders and the REMOTE scatter stay on rp_scatter_kernel.
@@ -33,12 +34,7 @@ template <typename KeyT, bool HAS_VAL> constexpr int sw_threads() { return HAS_V
 template <typename KeyT, bool HAS_VAL> constexpr int sw_ctas() { return 1024 / sw_threads<KeyT, HAS_VAL>(); }
 constexpr int SW_MAX_CTAS = 4;
 constexpr int SW_NB = 256;
-constexpr u32 SW_FLAG_AGG = 1u << 30, SW_FLAG_INC = 2u << 30, SW_VAL_MASK = (1u << 30) - 1;   // look-back words
-#ifndef VB_SW_LB
-#define VB_SW_LB 16
-#endif
-constexpr int SW_LB = VB_SW_LB;            // look-back window: status words fetched per step
-constexpr u64 SW_MAX_ROWS = 1ull << 30;     // prefixes live in 30 bits; larger inputs use the rp_* kernels
+constexpr u64 SW_ROW_LIMIT = 1ull << 31;    // the sweeps take n < SW_ROW_LIMIT rows (u32 output positions); larger inputs use rp_scatter_kernel
 
 // items per thread by row width: the tile buffers (raw + staged) of the resident CTAs fit the 227 KB of an SM
 template <typename KeyT, bool HAS_VAL> constexpr int sw_items() { return (sizeof(KeyT) + (HAS_VAL ? 8 : 0)) >= 16 ? 6 : (sizeof(KeyT) + (HAS_VAL ? 8 : 0)) == 12 ? 8 : VB_SW_ITEMS_KEY; }
@@ -63,104 +59,20 @@ struct SweepArgs {
     const void *keys;         // u64* / u32* / AoS rows
     const void *vals;         // u64* or NULL; LD_KEY32_VAL_AOS: AoS rows whose .y is the value
     u64 n;
-    u32 n_tiles;
-    u32 *tile_counter;        // zeroed before the launch
-    u32 *state;               // [n_tiles][256] look-back words, zeroed before the launch
-    const u32 *digit_base;    // [256] exclusive scan of the global histogram of this pass's digit
+    u32 n_tiles;              // rp_sweep_kernel: tiles of the whole input
     void *out_keys;
     u64 *out_vals;
-    // STATIC variant (no look-back): CTA p owns the contiguous rows [p*rows_per_part, (p+1)*rows_per_part) and starts
-    // digit d at part_off[d*num_parts + p] (the scanned per-part histogram of rp_hist_kernel + rp_scan_kernel)
+    // CTA p owns the contiguous rows [p*rows_per_part, (p+1)*rows_per_part) and starts digit d at
+    // part_off[d*num_parts + p] (the scanned per-part histogram of rp_hist_kernel + rp_scan_kernel)
     const u32 *part_off;
     u32 num_parts;
     u64 rows_per_part;        // multiple of the tile size
-    u32 stagger_ns;           // rp_gsweep_kernel: start delay of the second half of the grid (timing experiments)
     u64 *csr;                 // rp_gsweep_kernel<CSR>: csr[id] = min(output position of a row that starts a run of id)
 };
 
-// ---------------------------------------------------------------------------------------------
-// One histogram pass for every digit position: hist[p][d] += 1 for the p-th 8-bit digit of each key.
-// (DG_BITS: positions of the order-transformed key listed in `shifts`; other digit modes: one position.)
-// ---------------------------------------------------------------------------------------------
-struct HistAllArgs {
-    u32 n_pos;
-    u32 shifts[8];
-};
-
-template <typename KeyT, int LDM, int DGM>
-__global__ void __launch_bounds__(512) sw_hist_all_kernel(Loader ld, Digit dg, u64 n, HistAllArgs ha, u32 *__restrict__ hist /*[n_pos][256]*/)
-{
-    __shared__ u32 sh[8 * SW_NB];
-    for (u32 i = threadIdx.x; i < ha.n_pos * SW_NB; i += blockDim.x) sh[i] = 0;
-    __syncthreads();
-    const u64 pol = policy_evict_first();
-    constexpr int B = 4;
-    const u64 stride = (u64)gridDim.x * blockDim.x * B;
-    for (u64 i0 = ((u64)blockIdx.x * blockDim.x) * B + threadIdx.x; i0 < n; i0 += stride) {
-        KeyT key[B];
-        bool ok[B];
-#pragma unroll
-        for (int j = 0; j < B; ++j) {
-            const u64 i = i0 + (u64)j * blockDim.x;
-            key[j] = 0;
-            ok[j] = i < n && rp_load_key<KeyT, LDM>(ld, i, key[j], pol);
-        }
-#pragma unroll
-        for (int j = 0; j < B; ++j) {
-            if (!ok[j]) continue;
-            if constexpr (DGM == DG_BITS) {
-                const u64 k = (sizeof(KeyT) == 8) ? tx_fwd((u64)key[j], dg.tx) : (u64)key[j];
-                for (u32 p = 0; p < ha.n_pos; ++p) atomicAdd(&sh[p * SW_NB + ((u32)(k >> ha.shifts[p]) & 0xFFu)], 1u);
-            } else {
-                atomicAdd(&sh[rp_digit<KeyT, DGM>(dg, key[j])], 1u);
-            }
-        }
-    }
-    __syncthreads();
-    for (u32 i = threadIdx.x; i < ha.n_pos * SW_NB; i += blockDim.x)
-        if (sh[i]) atomicAdd(&hist[i], sh[i]);
-}
-
-// exclusive scan of each 256-bin histogram in place; hist[p][256 + p_total?] not needed: total = n
-__global__ void __launch_bounds__(SW_NB) sw_scan_bases_kernel(u32 *__restrict__ hist /*[n_pos][256]*/, u32 n_pos)
-{
-    __shared__ u32 ws[8];
-    const u32 d = threadIdx.x, lane = d & 31u, warp = d >> 5;
-    for (u32 p = blockIdx.x; p < n_pos; p += gridDim.x) {
-        const u32 c = hist[p * SW_NB + d];
-        u32 incl = c;
-#pragma unroll
-        for (int off = 1; off < 32; off <<= 1) {
-            const u32 t = __shfl_up_sync(0xffffffffu, incl, off);
-            if (lane >= (u32)off) incl += t;
-        }
-        if (lane == 31) ws[warp] = incl;
-        __syncthreads();
-        u32 base = 0;
-        for (u32 w = 0; w < warp; ++w) base += ws[w];
-        hist[p * SW_NB + d] = base + incl - c;
-        __syncthreads();
-    }
-}
-
-// ---------------------------------------------------------------------------------------------
-// The pass
-// ---------------------------------------------------------------------------------------------
-VB_D u32 ld_relaxed_u32(const u32 *p)
-{
-    u32 v;
-    asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-VB_D void st_relaxed_u32(u32 *p, u32 v) { asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
-
-// STATIC = false: tiles claimed from an atomic counter, digit offsets by decoupled look-back (one kernel per pass).
-// STATIC = true : the same tile pipeline (copy-engine staging, warp-private u16 counters, 4 barriers, full-tile fast path)
-//                 fed by the per-part histogram of rp_hist/rp_scan: each CTA walks its own contiguous part and keeps
-//                 running digit offsets in shared memory — no status words, no polling.  This is the product's scatter
-//                 for row streams that the gather sweep does not take: with the CTA shape picked per row type (sw_threads)
-//                 faster than rp_scatter_kernel on 1e9 rows.
-template <typename KeyT, bool HAS_VAL, int LDM, int DGM, bool STATIC = false>
+// Each CTA walks its own contiguous part tile by tile (copy-engine staging, warp-private u16 counters, 4 barriers,
+// full-tile fast path) and keeps running digit offsets in shared memory.
+template <typename KeyT, bool HAS_VAL, int LDM, int DGM>
 __global__ void __launch_bounds__((sw_threads<KeyT, HAS_VAL>()), (sw_ctas<KeyT, HAS_VAL>()))
 rp_sweep_kernel(SweepArgs a, Digit dg)
 {
@@ -188,7 +100,7 @@ rp_sweep_kernel(SweepArgs a, Digit dg)
     __shared__ u32 wtot[SW_WARPS];
     __shared__ u32 dbase[SW_NB];              // tile-local start of digit d
     __shared__ u32 gbase[SW_NB];              // global offset of digit d's first row of this tile, minus dbase[d]
-    __shared__ u32 run_off[STATIC ? SW_NB : 1];   // STATIC: global offset of the next row of digit d of this part
+    __shared__ u32 run_off[SW_NB];            // global offset of the next row of digit d of this part
 
     const u32 tid = threadIdx.x, warp = tid >> 5, lane = tid & 31u;
     const u32 lt = lanemask_lt();
@@ -207,15 +119,14 @@ rp_sweep_kernel(SweepArgs a, Digit dg)
     };
     auto tile_is_full = [&](u32 t) { return (u64)(t + 1) * T <= n; };
 
-    // STATIC: this CTA's tiles are [part_first, part_last); a.n_tiles doubles as the "no more tiles" sentinel
-    const u32 part_first = STATIC ? (u32)(((u64)blockIdx.x * a.rows_per_part) / T) : 0u;
-    const u32 part_last = STATIC ? (u32)min((u64)a.n_tiles, (((u64)blockIdx.x + 1) * a.rows_per_part) / T) : 0u;
-    if (STATIC)
-        for (u32 d = tid; d < SW_NB; d += SW_THREADS) run_off[d] = a.part_off[(size_t)d * a.num_parts + blockIdx.x];
+    // this CTA's tiles are [part_first, part_last); a.n_tiles doubles as the "no more tiles" sentinel
+    const u32 part_first = (u32)(((u64)blockIdx.x * a.rows_per_part) / T);
+    const u32 part_last = (u32)min((u64)a.n_tiles, (((u64)blockIdx.x + 1) * a.rows_per_part) / T);
+    for (u32 d = tid; d < SW_NB; d += SW_THREADS) run_off[d] = a.part_off[(size_t)d * a.num_parts + blockIdx.x];
     if (tid == 0) {
         mbar_init(&full_bar, 1);
         mbar_fence_init();
-        const u32 t0 = STATIC ? (part_first < part_last ? part_first : a.n_tiles) : atomicAdd(a.tile_counter, 1u);
+        const u32 t0 = part_first < part_last ? part_first : a.n_tiles;
         s_tile[0] = t0;
         if (t0 < a.n_tiles && tile_is_full(t0)) issue_tile(t0);
     }
@@ -271,9 +182,6 @@ rp_sweep_kernel(SweepArgs a, Digit dg)
         for (int i = 0; i < K; ++i) {
             const u32 d = dr[i];
             u32 peers;
-#ifdef VB_SW_DEBUG_NORANK        // timing bisection only
-            if (full) { peers = 1u << lane; } else
-#endif
             if (full) {
                 peers = 0xffffffffu;
 #pragma unroll
@@ -283,7 +191,7 @@ rp_sweep_kernel(SweepArgs a, Digit dg)
                     peers &= bit ? m : ~m;
                 }
             } else {
-                peers = warp_match_digit<8>(d);
+                peers = warp_match_digit(d);
             }
             const u32 leader = (u32)(__ffs(peers) - 1);
             u32 base = 0;
@@ -293,21 +201,17 @@ rp_sweep_kernel(SweepArgs a, Digit dg)
             __syncwarp();
         }
         __syncthreads();                                                        // B1: counters complete, raw buffer consumed
-        if (tid == 0) {                                                          // claim + prefetch the next tile
-            const u32 nx = STATIC ? (tile + 1 < part_last ? tile + 1 : a.n_tiles) : atomicAdd(a.tile_counter, 1u);
+        if (tid == 0) {                                                          // prefetch the next tile of the part
+            const u32 nx = tile + 1 < part_last ? tile + 1 : a.n_tiles;
             s_tile[(it + 1) & 1u] = nx;
             if (nx < a.n_tiles && tile_is_full(nx)) issue_tile(nx);
         }
 
-        // ---- 3. thread d < 256: column scan over the warps, publish the tile aggregate, block scan over digits
+        // ---- 3. thread d < 256: column scan over the warps, block scan over digits
         u32 total = 0;
         if (tid < SW_NB) {
 #pragma unroll
             for (int w = 0; w < SW_WARPS; ++w) { const u32 c = cnt[w * SW_NB + tid]; cnt[w * SW_NB + tid] = (unsigned short)total; total += c; }
-            if (!STATIC) {
-                if (tile == 0) st_relaxed_u32(&a.state[tid], SW_FLAG_INC | total);
-                else st_relaxed_u32(&a.state[(size_t)tile * SW_NB + tid], SW_FLAG_AGG | total);
-            }
         }
         u32 incl = total;
 #pragma unroll
@@ -334,53 +238,12 @@ rp_sweep_kernel(SweepArgs a, Digit dg)
                 st_dig[pos] = (unsigned char)d;
             }
         }
-        // ---- 4. decoupled look-back, thread d < 256 for digit d.  It runs AFTER staging: the tile's registers are
-        // dead (room for a window of SW_LB status words in flight per thread) and the predecessors have had the whole
-        // staging phase to publish.  A serial one-tile-per-L2-round-trip walk cannot keep up with > 10 tiles/us
-        // chip-wide (measured: 3x slower than the two-kernel pass), so SW_LB predecessors are fetched per step.
-        if (STATIC) {
-            if (tid < SW_NB) { const u32 ro = run_off[tid]; gbase[tid] = ro - excl_local; run_off[tid] = ro + total; }
-        } else if (tid < SW_NB) {
-            u32 prefix = 0;
-#ifdef VB_SW_DEBUG_NOLB          // timing bisection only: results are wrong
-            if (false) {
-#else
-            if (tile > 0) {
-#endif
-                long long tt = (long long)tile - 1;
-                bool done = false;
-                while (!done) {
-                    u32 v[SW_LB];
-#pragma unroll
-                    for (int j = 0; j < SW_LB; ++j) {
-                        const long long idx = tt - j;
-                        v[j] = idx >= 0 ? ld_relaxed_u32(&a.state[(size_t)idx * SW_NB + tid]) : SW_FLAG_INC;   // before tile 0: prefix 0
-                    }
-                    int used = 0;
-#pragma unroll
-                    for (int j = 0; j < SW_LB; ++j) {
-                        if (!done && used == j) {                 // stop consuming at the first word not yet published
-                            const u32 x = v[j];
-                            if ((x >> 30) != 0u) {
-                                prefix += x & SW_VAL_MASK;
-                                ++used;
-                                if (x & SW_FLAG_INC) done = true;
-                            }
-                        }
-                    }
-                    tt -= used;
-                }
-                st_relaxed_u32(&a.state[(size_t)tile * SW_NB + tid], SW_FLAG_INC | (prefix + total));
-            }
-            gbase[tid] = a.digit_base[tid] + prefix - excl_local;
-        }
+        // ---- 4. global offsets of this tile's digits from the part's running offsets
+        if (tid < SW_NB) { const u32 ro = run_off[tid]; gbase[tid] = ro - excl_local; run_off[tid] = ro + total; }
         __syncthreads();                                                        // B4: tile staged
         for (u32 i = lane; i < SW_NB / 2; i += 32) ((u32 *)my_cnt)[i] = 0;      // own counters: next tile's ranking
         __syncwarp();
         KeyT *ok = (KeyT *)a.out_keys;
-#ifdef VB_SW_DEBUG_NOWRITE       // timing bisection only
-        if (tile == 0xFFFFFFFEu)
-#endif
         for (u32 p = tid; p < rows_here; p += SW_THREADS) {
             const u32 o = gbase[st_dig[p]] + p;
             ok[o] = st_keys[p];
