@@ -18,6 +18,7 @@
  *   vb_join*               <- CoGroupedRdd::compute               src/rdd/co_grouped_rdd.rs:206-249
  *                             + PairRdd::join cross product       src/rdd/pair_rdd.rs:104-121
  *   vb_join_outer*         <- nothing: vega has no outer joins (Spark's left/right/full outer join, new)
+ *   vb_cogroup*            <- CoGroupedRdd::compute for PairRdd::cogroup  src/rdd/co_grouped_rdd.rs:206-249
  *   vb_shuffle_free        <- (the reference never evicts SHUFFLE_CACHE, src/env.rs:27)
  *   vb_slice               <- ParallelCollection::slice           src/rdd/parallel_collection_rdd.rs:116-145
  *   vb_shuffle_export_* / vb_shuffle_import
@@ -292,6 +293,25 @@ VB_API int32_t vb_join_outer_size(vb_shuf *left, vb_shuf *right, uint32_t reduce
 VB_API int32_t vb_join_outer(vb_shuf *left, vb_shuf *right, uint32_t reduce_id, int32_t kind,
                              void *out_k, void *out_v, void *out_w,
                              uint8_t *out_v_valid, uint8_t *out_w_valid, int32_t dst_loc);
+
+/* CoGroupedRdd::compute for PairRdd::cogroup (src/rdd/pair_rdd.rs:123-155, src/rdd/co_grouped_rdd.rs:206-249):
+ * partition reduce_id of the cogroup of two sealed GROUP/COGROUP shuffles, as one key list with two CSR value lists.
+ *   keys     every key that occurs on either side in the partition, exactly once; the order of keys within the
+ *            partition is unspecified (as for vb_shuffle_reduce).
+ *   lists    a key's left list is exactly the value list vb_shuffle_reduce of the left shuffle gives for it (map-id
+ *            order, then encounter order), and the same holds for the right list.  A key a side lacks has an empty
+ *            list on that side.  left == right is allowed and gives two equal lists.
+ *   offsets  out_left_offsets / out_right_offsets [n_keys + 1] are relative to the partition and start at 0, as
+ *            vb_shuffle_reduce's do: key i's left values are out_left_vals[out_left_offsets[i] .. [i + 1]).
+ * The argument rules are vb_join's (two sealed GROUP/COGROUP shuffles with equal n_reduce and key width on the same
+ * context, reduce_id < n_reduce; anything else is VB_ERR_INVALID), and the call blocks until both sides are sealed.
+ * vb_cogroup_size gives the output sizes (NULL pointers skipped); vb_cogroup writes to dst_loc VB_HOST or VB_DEVICE
+ * and skips NULL outputs.  On a rank of a multi-rank shuffle only the partitions that rank owns have keys.         */
+VB_API int32_t vb_cogroup_size(vb_shuf *left, vb_shuf *right, uint32_t reduce_id,
+                               uint64_t *n_keys, uint64_t *n_left_vals, uint64_t *n_right_vals);
+VB_API int32_t vb_cogroup(vb_shuf *left, vb_shuf *right, uint32_t reduce_id, void *out_keys,
+                          uint64_t *out_left_offsets /*n_keys+1*/, void *out_left_vals,
+                          uint64_t *out_right_offsets /*n_keys+1*/, void *out_right_vals, int32_t dst_loc);
 
 /* ---- SURVEY §8(f) N1: bincode blobs — the payload format of SHUFFLE_CACHE ------------------------
  * The reference serialises every (map, reduce) bucket with bincode 1.2.1 defaults (src/dependency.rs:213-214:

@@ -216,6 +216,30 @@ public:
         return out;
     }
 
+    // self.cogroup(other, num_splits).collect()  →  Vec<(K, (Vec<V>, Vec<W>))> (src/rdd/pair_rdd.rs:123-155): every key
+    // of either side once, with both value lists in cogroup order; a side that lacks the key has an empty list.
+    template <typename W>
+    std::vector<std::pair<K, std::pair<std::vector<V>, std::vector<W>>>> cogroup(const PairRddT<K, W> &other, size_t num_splits) const
+    {
+        auto a = detail::run_shuffle<K>(*sc_, keys_, &vals_, num_slices_, num_splits, detail::dtype<V>::code, VB_AGG_COGROUP);
+        auto b = detail::run_shuffle<K>(*sc_, other.keys_, &other.vals_, other.num_slices_, num_splits, detail::dtype<W>::code, VB_AGG_COGROUP);
+        std::vector<std::pair<K, std::pair<std::vector<V>, std::vector<W>>>> out;
+        for (uint32_t r = 0; r < num_splits; ++r) {
+            uint64_t nk = 0, nv = 0, nw = 0;
+            check(vb_cogroup_size(a.get(), b.get(), r, &nk, &nv, &nw));
+            std::vector<uint64_t> k(nk), vo(nk + 1), v(nv), wo(nk + 1), w(nw);
+            check(vb_cogroup(a.get(), b.get(), r, k.data(), vo.data(), v.data(), wo.data(), w.data(), VB_HOST));
+            for (uint64_t i = 0; i < nk; ++i) {
+                std::vector<V> vs;
+                std::vector<W> ws;
+                for (uint64_t j = vo[i]; j < vo[i + 1]; ++j) vs.push_back(detail::from_bits<V>(v[j]));
+                for (uint64_t j = wo[i]; j < wo[i + 1]; ++j) ws.push_back(detail::from_bits<W>(w[j]));
+                out.emplace_back(detail::from_bits<K>(k[i]), std::make_pair(std::move(vs), std::move(ws)));
+            }
+        }
+        return out;
+    }
+
     // Outer joins (Spark's leftOuterJoin / rightOuterJoin / fullOuterJoin; vega has none): a key missing on the other
     // side still gives rows, with std::nullopt on that side.  A key's rows are contiguous.
     template <typename W>

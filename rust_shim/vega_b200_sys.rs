@@ -43,6 +43,12 @@ extern "C" {
     pub fn vb_join_outer(left: *mut vb_shuf, right: *mut vb_shuf, reduce_id: u32, kind: i32, out_k: *mut c_void,
                          out_v: *mut c_void, out_w: *mut c_void, out_v_valid: *mut u8, out_w_valid: *mut u8,
                          dst_loc: i32) -> i32;
+    // CoGroupedRdd::compute for PairRdd::cogroup: every key once, left and right value lists as two CSRs
+    pub fn vb_cogroup_size(left: *mut vb_shuf, right: *mut vb_shuf, reduce_id: u32, n_keys: *mut u64,
+                           n_left_vals: *mut u64, n_right_vals: *mut u64) -> i32;
+    pub fn vb_cogroup(left: *mut vb_shuf, right: *mut vb_shuf, reduce_id: u32, out_keys: *mut c_void,
+                      out_left_offsets: *mut u64, out_left_vals: *mut c_void, out_right_offsets: *mut u64,
+                      out_right_vals: *mut c_void, dst_loc: i32) -> i32;
     // N1: bincode blobs (the payload format of SHUFFLE_CACHE)
     pub fn vb_shuffle_reduce_blob_size(s: *mut vb_shuf, reduce_id: u32, n_bytes: *mut u64) -> i32;
     pub fn vb_shuffle_reduce_blob(s: *mut vb_shuf, reduce_id: u32, out_blob: *mut c_void, dst_loc: i32) -> i32;

@@ -18,7 +18,7 @@ ap = argparse.ArgumentParser()
 ap.add_argument("--rows", type=float, default=1e9)
 ap.add_argument("--distinct", type=float, default=1e6)
 ap.add_argument("--ops", default="reduce,group,sort,sortkv,join,count")   # also: zipf, zipfgroup, combine, combinezipf,
-#                                                                             leftjoin, fulljoin
+#                                                                             leftjoin, fulljoin, cogroup
 ap.add_argument("--reps", type=int, default=3)
 args = ap.parse_args()
 N, D = int(args.rows), int(args.distinct)
@@ -93,7 +93,7 @@ if "sort" in ops:
     report("sort_by_key(keys only)", N, 16.0 * N, timed(lambda: run_shuffle(L.VB_AGG_SORT, keys=keys), max(1, args.reps - 1)))
     del keys
     torch.cuda.empty_cache()
-join_ops = [o for o in ("join", "leftjoin", "fulljoin") if o in ops]
+join_ops = [o for o in ("join", "leftjoin", "fulljoin", "cogroup") if o in ops]
 if join_ops:
     # BASELINE config 4, per-GPU share at 8 GPUs: 6.25e7 rows per side, each rank once per side,
     # 1.25e6 shared keys per GPU (1e7 / 8)
@@ -143,7 +143,7 @@ if "join" in ops:
     res = timed(join, max(1, args.reps - 1))
     assert res[-1][1]["join_rows"] == shared, (res[-1][1]["join_rows"], shared)
     report("join", 2 * n_side, 32.0 * n_side + 24.0 * shared, res, {"join_rows": shared})
-if "leftjoin" in ops or "fulljoin" in ops:
+if "leftjoin" in ops or "fulljoin" in ops or "cogroup" in ops:
     # Each outer join against the inner join of the same inputs and against the workaround without outer joins:
     # materialising the cogroup of both sides (vb_shuffle_reduce of every partition, device output), which the
     # caller then still has to expand.  All outputs stay on the device.
@@ -181,9 +181,24 @@ if "leftjoin" in ops or "fulljoin" in ops:
         sa.free(); sb.free()
         return st
 
+    def cogroup():
+        # vb_cogroup of every partition: both sides grouped and aligned by key, device output
+        sa, sb = cogroup_pair()
+        tot = 0
+        for r in range(8):
+            nk, nl, nr = ctypes.c_uint64(), ctypes.c_uint64(), ctypes.c_uint64()
+            L.check(sc._lib.vb_cogroup_size(sa._h, sb._h, r, ctypes.byref(nk), ctypes.byref(nl), ctypes.byref(nr)))
+            k, lo, lv, ro, rv = dev(nk.value), dev(nk.value + 1), dev(nl.value), dev(nk.value + 1), dev(nr.value)
+            L.check(sc._lib.vb_cogroup(sa._h, sb._h, r, p(k), p(lo), p(lv), p(ro), p(rv), L.VB_DEVICE))
+            tot += nk.value
+        st = pair_stats(sa, sb)
+        st["cogroup_keys"] = tot
+        sa.free(); sb.free()
+        return st
+
     med = lambda r: sorted(x[0] for x in r)[len(r) // 2]
     reps = max(1, args.reps - 1)
-    r_inner = timed(join, reps)
+    r_inner = timed(join, reps) if "leftjoin" in ops or "fulljoin" in ops else None
     r_cog = timed(cogroup_both, reps)
     for op, kind, want in (("leftjoin", L.VB_JOIN_LEFT, n_side), ("fulljoin", L.VB_JOIN_FULL, 2 * n_side - shared)):
         if op not in ops:
@@ -193,6 +208,14 @@ if "leftjoin" in ops or "fulljoin" in ops:
         extra = {"gpu": card["name"], "power_limit_w": card["power_limit_w"], "join_rows": want,
                  "inner_join_ms": round(med(r_inner), 3), "cogroup_both_sides_ms": round(med(r_cog), 3)}
         report({"leftjoin": "left_outer_join", "fulljoin": "full_outer_join"}[op], 2 * n_side, 32.0 * n_side + 26.0 * want, res, extra)
+    if "cogroup" in ops:
+        # against cogroup_both (two vb_shuffle_reduce per partition): the grouping alone, without the alignment by key
+        res = timed(cogroup, reps)
+        want = 2 * n_side - shared
+        assert res[-1][1]["cogroup_keys"] == want, (res[-1][1]["cogroup_keys"], want)
+        extra = {"gpu": card["name"], "power_limit_w": card["power_limit_w"], "cogroup_keys": want,
+                 "cogroup_both_sides_ms": round(med(r_cog), 3)}
+        report("cogroup", 2 * n_side, 32.0 * n_side + 24.0 * want, res, extra)
 if "combine" in ops or "combinezipf" in ops:
     # combine_by_key: sum(v0), min(v1), max(v1), mean(v2), count in one shuffle (5 accumulators) against the baseline a
     # user has without it, one single-column shuffle per aggregate (the mean from a sum and the count).  v0 is gen_pairs'

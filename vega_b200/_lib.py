@@ -94,6 +94,8 @@ SYMBOLS = {
     "vb_join": (_i32, [_vp, _vp, _u32, _vp, _vp, _vp, _i32]),
     "vb_join_outer_size": (_i32, [_vp, _vp, _u32, _i32, _pu64]),
     "vb_join_outer": (_i32, [_vp, _vp, _u32, _i32, _vp, _vp, _vp, _vp, _vp, _i32]),
+    "vb_cogroup_size": (_i32, [_vp, _vp, _u32, _pu64, _pu64, _pu64]),
+    "vb_cogroup": (_i32, [_vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _i32]),
     "vb_shuffle_reduce_blob_size": (_i32, [_vp, _u32, _pu64]),
     "vb_shuffle_reduce_blob": (_i32, [_vp, _u32, _vp, _i32]),
     "vb_shuffle_map_blob": (_i32, [_vp, _u32, _vp, _u64, _i32]),

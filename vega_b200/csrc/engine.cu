@@ -283,6 +283,17 @@ struct JoinPlan {
     u64 total_left = 0;            // rows of the left keys (pos[nl])
 };
 
+// vb_cogroup_size's result for one (right side, partition), kept for vb_cogroup.  Output keys: the nl left keys in
+// the left CSR's order, then the n_ro right-only keys in the right CSR's order.
+struct CogroupPlan {
+    u32 nl = 0, nr = 0;            // left / right keys of the partition
+    u64 n_ro = 0;                  // right-only keys
+    u64 n_lv = 0, n_rv = 0;        // left / right values of the partition
+    u64 *pos = nullptr;            // [nl + nr + 1] exclusive right-value positions: the left keys', then the right keys'
+    u32 *match = nullptr;          // [nl] matched right key index, 0xFFFFFFFF if none
+    u64 *ro_keys = nullptr, *ro_pos = nullptr;   // [n_ro] the right-only keys and their right-value positions
+};
+
 struct vb_shuf {
     vb_ctx *ctx = nullptr;
     u64 id = 0;
@@ -340,6 +351,7 @@ struct vb_shuf {
     u32 dict_log_cap = 0;
     u32 *dense_of_slot = nullptr;
     std::map<std::tuple<const vb_shuf *, u32, int>, JoinPlan> join_plans;   // by (right side, partition, join kind)
+    std::map<std::pair<const vb_shuf *, u32>, CogroupPlan> cogroup_plans;   // by (right side, partition)
     // COGROUP shuffles are grouped lazily: seal keeps the (owned) rows; the CSR is built by the first reduce call
     // (cogroup materialisation), or — if a join comes first — only for the rows the join kind needs: the keys on BOTH
     // sides (inner), every row of the preserved side plus the matching rows of the other (LEFT / RIGHT), or all (FULL).
@@ -3374,6 +3386,149 @@ extern "C" int32_t vb_join_outer(vb_shuf *l, vb_shuf *r, uint32_t rid, int32_t k
 }
 
 // ---------------------------------------------------------------------------------------------
+// cogroup (CoGroupedRdd::compute for PairRdd::cogroup, co_grouped_rdd.rs:206-249)
+// Both sides are grouped completely (the FULL filtered pair while both are lazy, shared with full_outer_join), so the
+// result is the two CSRs aligned by key: the left keys in the left CSR's order, then the right-only keys in the right
+// CSR's order.  The left values are the left partition's value slice as it is; the right values are the right
+// partition's value segments permuted into output key order by cogroup_gather_right_kernel.
+// ---------------------------------------------------------------------------------------------
+static void free_cogroup_plan(vb_ctx *c, CogroupPlan &p)
+{
+    dev_free(c, p.pos); dev_free(c, p.match); dev_free(c, p.ro_keys); dev_free(c, p.ro_pos);
+}
+
+static int cogroup_plan(vb_shuf *l, vb_shuf *r, u32 rid, CogroupPlan **out)
+{
+    vb_ctx *c = l->ctx;
+    const auto key = std::make_pair((const vb_shuf *)r, rid);
+    auto it = l->cogroup_plans.find(key);
+    if (it != l->cogroup_plans.end()) { *out = &it->second; return VB_OK; }
+    CogroupPlan p;
+    const u64 lb = l->bucket_off[rid], le = l->bucket_off[rid + 1];
+    const u64 rb = r->bucket_off[rid], re = r->bucket_off[rid + 1];
+    p.nl = (u32)(le - lb);
+    p.nr = (u32)(re - rb);
+    p.n_lv = l->val_off[rid + 1] - l->val_off[rid];
+    const u64 n = (u64)p.nl + p.nr;
+    DevBuf pos(c), match(c), ro_keys(c), ro_pos(c);
+    TRY(pos.alloc((n + 1) * 8));
+    if (n == 0) {
+        CU(cudaMemsetAsync(pos.p, 0, 8, c->stream));
+    } else {
+        if ((r->n_keys && !r->dict) || (l->n_keys && !l->dict)) return set_err(VB_ERR_STATE, "cogroup side without a key dictionary");
+        const Table rtab = table_at(r->n_keys ? r->dict : nullptr, r->dict_log_cap);   // keys NULL: that side is empty
+        const Table ltab = table_at(l->n_keys ? l->dict : nullptr, l->dict_log_cap);
+        DevBuf cnt(c), flag(c);
+        TRY(cnt.alloc(n * 8));
+        TRY(match.alloc(std::max<u64>(p.nl, 1) * 4));
+        if (p.nl) {
+            KLaunch kl(l, K_JOIN);
+            cogroup_probe_kernel<<<(p.nl + 255) / 256, 256, 0, c->stream>>>(l->res_keys, (u32)lb, (u32)le, rtab, r->dense_of_slot,
+                                                                            r->res_offs, cnt.as<u64>(), match.as<u32>());
+            TRY(kl.done("cogroup_probe_kernel"));
+        }
+        if (p.nr) {
+            TRY(flag.alloc(p.nr));
+            {
+                KLaunch kl(l, K_JOIN);
+                join_probe_right_kernel<<<(p.nr + 255) / 256, 256, 0, c->stream>>>(r->res_keys, r->res_offs, (u32)rb, (u32)re, ltab,
+                                                                                   cnt.as<u64>() + p.nl);
+                TRY(kl.done("join_probe_right_kernel"));
+            }
+            KLaunch kl(l, K_JOIN);
+            cogroup_flag_kernel<<<(p.nr + 255) / 256, 256, 0, c->stream>>>(cnt.as<u64>() + p.nl, p.nr, flag.as<unsigned char>());
+            TRY(kl.done("cogroup_flag_kernel"));
+        }
+        TRY(exclusive_scan_u64(l, cnt.as<u64>(), pos.as<u64>(), n, pos.as<u64>() + n));
+        // the right-only keys and their positions, in the right CSR's order (stable compaction)
+        if (p.nr) TRY(compact_rows(l, r->res_keys + rb, pos.as<u64>() + p.nl, p.nr, flag.as<unsigned char>(), ro_keys, ro_pos, &p.n_ro));
+    }
+    CU(cudaMemcpyAsync(c->h_scratch, pos.as<u64>() + n, 8, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    p.n_rv = *(u64 *)c->h_scratch;
+    p.pos = (u64 *)pos.release();
+    p.match = (u32 *)match.release();
+    p.ro_keys = (u64 *)ro_keys.release();
+    p.ro_pos = (u64 *)ro_pos.release();
+    *out = &l->cogroup_plans.emplace(key, p).first->second;
+    return VB_OK;
+}
+
+extern "C" int32_t vb_cogroup_size(vb_shuf *l, vb_shuf *r, uint32_t rid, uint64_t *n_keys, uint64_t *n_left_vals,
+                                   uint64_t *n_right_vals)
+{
+    TRY(join_check(l, r, rid));
+    std::lock_guard<std::mutex> lk(l->ctx->mu);
+    CU(cudaSetDevice(l->ctx->device));
+    TRY(join_sides(l, r, JK_FULL));
+    CogroupPlan *p = nullptr;
+    TRY(cogroup_plan(l, r, rid, &p));
+    if (n_keys) *n_keys = p->nl + p->n_ro;
+    if (n_left_vals) *n_left_vals = p->n_lv;
+    if (n_right_vals) *n_right_vals = p->n_rv;
+    return VB_OK;
+}
+
+extern "C" int32_t vb_cogroup(vb_shuf *l, vb_shuf *r, uint32_t rid, void *out_keys, uint64_t *out_left_offsets,
+                              void *out_left_vals, uint64_t *out_right_offsets, void *out_right_vals, int32_t dst_loc)
+{
+    TRY(join_check(l, r, rid));
+    if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
+    vb_ctx *c = l->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    TRY(join_sides(l, r, JK_FULL));
+    CogroupPlan *p = nullptr;
+    TRY(cogroup_plan(l, r, rid, &p));
+    const u64 nl = p->nl, nk = nl + p->n_ro, n = nl + p->nr;
+    const u64 lb = l->bucket_off[rid], lv0 = l->val_off[rid];
+    int rc = [&]() -> int {
+        // keys: the left keys, then the right-only keys
+        TRY(copy_out(l, out_keys, l->res_keys ? l->res_keys + lb : nullptr, nl * 8, dst_loc));
+        TRY(copy_out(l, out_keys ? (u64 *)out_keys + nl : nullptr, p->ro_keys, p->n_ro * 8, dst_loc));
+        // left lists: the partition's value slice as it is; offsets rebased, then flat for the right-only keys
+        if (out_left_offsets) {
+            DevBuf tmp(c);
+            u64 *d = out_left_offsets;
+            if (dst_loc == VB_HOST) { TRY(tmp.alloc((nk + 1) * 8)); d = tmp.as<u64>(); }
+            {
+                KLaunch kl(l, K_JOIN);
+                cogroup_left_offsets_kernel<<<(unsigned)((nk + 1 + 255) / 256), 256, 0, c->stream>>>(l->res_offs, (u32)lb, (u32)nl, nk + 1,
+                                                                                                    lv0, p->n_lv, d);
+                TRY(kl.done("cogroup_left_offsets_kernel"));
+            }
+            if (dst_loc == VB_HOST) TRY(copy_out(l, out_left_offsets, d, (nk + 1) * 8, VB_HOST));
+        }
+        TRY(copy_out(l, out_left_vals, l->res_vals ? l->res_vals + lv0 : nullptr, p->n_lv * 8, dst_loc));
+        // right offsets: the left keys' positions, the right-only keys' positions, the total
+        if (out_right_offsets) {
+            TRY(copy_out(l, out_right_offsets, p->pos, nl * 8, dst_loc));
+            TRY(copy_out(l, out_right_offsets + nl, p->ro_pos, p->n_ro * 8, dst_loc));
+            TRY(copy_out(l, out_right_offsets + nk, p->pos + n, 8, dst_loc));
+        }
+        // right lists: each right key's value segment, gathered into output key order
+        if (out_right_vals && p->n_rv) {
+            DevBuf tmp(c);
+            u64 *d = (u64 *)out_right_vals;
+            if (dst_loc == VB_HOST) { TRY(tmp.alloc(p->n_rv * 8)); d = tmp.as<u64>(); }
+            {
+                KLaunch kl(l, K_JOIN);
+                const u64 blocks = std::min<u64>((p->n_rv + 255) / 256, (u64)c->sm_count * 8);
+                cogroup_gather_right_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(p->pos, (u32)n, p->n_rv, p->match, (u32)nl,
+                                                                                    (u32)r->bucket_off[rid], r->res_offs, r->res_vals, d);
+                TRY(kl.done("cogroup_gather_right_kernel"));
+            }
+            if (dst_loc == VB_HOST) TRY(copy_out(l, out_right_vals, d, p->n_rv * 8, VB_HOST));
+        }
+        return VB_OK;
+    }();
+    cudaStreamSynchronize(c->stream);
+    free_cogroup_plan(c, *p);
+    l->cogroup_plans.erase(std::make_pair((const vb_shuf *)r, rid));
+    return rc;
+}
+
+// ---------------------------------------------------------------------------------------------
 // free / stats
 // ---------------------------------------------------------------------------------------------
 extern "C" int32_t vb_shuffle_free(vb_shuf *s)
@@ -3395,6 +3550,7 @@ extern "C" int32_t vb_shuffle_free(vb_shuf *s)
         dev_free(c, s->res_keys); dev_free(c, s->res_comb); dev_free(c, s->res_offs); dev_free(c, s->res_vals); dev_free(c, s->res_cols);
         dev_free(c, s->dict); dev_free(c, s->dense_of_slot);
         for (auto &kv : s->join_plans) { dev_free(c, kv.second.pos); dev_free(c, kv.second.match); }
+        for (auto &kv : s->cogroup_plans) free_cogroup_plan(c, kv.second);
         free_lazy_rows(s);
         cudaStreamSynchronize(c->stream);
     }

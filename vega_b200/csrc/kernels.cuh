@@ -1689,6 +1689,58 @@ __global__ void join_expand_right_kernel(const u64 *__restrict__ pos, u32 nr, u6
 }
 
 // ---------------------------------------------------------------------------------------------
+// cogroup (CoGroupedRdd::compute): every key of a partition once, the left keys first, then the right-only keys
+// ---------------------------------------------------------------------------------------------
+// For left keys [lb, le): match = the right key's index (0xFFFFFFFF when the right side lacks the key) and
+// cnt = lenR, the number of right values the key's output list gets (0 when unmatched).  rtab.keys NULL: no right rows.
+__global__ void cogroup_probe_kernel(const u64 *__restrict__ lkeys, u32 lb, u32 le, Table rtab, const u32 *__restrict__ r_dense,
+                                     const u64 *__restrict__ roffs, u64 *__restrict__ cnt, u32 *__restrict__ match)
+{
+    const u32 j = lb + blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= le) return;
+    const u32 s = rtab.keys ? table_find(rtab, lkeys[j]) : 0xFFFFFFFFu;
+    const u32 m = s != 0xFFFFFFFFu ? r_dense[s] : 0xFFFFFFFFu;
+    cnt[j - lb] = m != 0xFFFFFFFFu ? roffs[m + 1] - roffs[m] : 0;
+    match[j - lb] = m;
+}
+
+// flag[i] = 1 for a right-only key: join_probe_right_kernel counted its values (a key always has at least one)
+__global__ void cogroup_flag_kernel(const u64 *__restrict__ cnt, u32 n, unsigned char *__restrict__ flag)
+{
+    const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) flag[i] = cnt[i] != 0;
+}
+
+// out[i] for i in [0, n): the left CSR's offsets of keys [lb, lb + nl) rebased to base, then n_lv (an empty left list)
+// for the right-only keys.
+__global__ void cogroup_left_offsets_kernel(const u64 *__restrict__ loffs, u32 lb, u32 nl, u64 n, u64 base, u64 n_lv,
+                                            u64 *__restrict__ out)
+{
+    const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) out[i] = i < nl ? loffs[lb + i] - base : n_lv;
+}
+
+// The right values in output key order, one thread per value (a key with 10^6 values spreads over 10^6 threads).
+// pos[n] holds the exclusive output positions of the partition's left keys (their matched right lists) followed by its
+// right keys (the right-only ones; 0 values for a key the left side has).  Output value o belongs to the largest j with
+// pos[j] <= o; its source segment is the right key match[j] (j < nl) or rb + j - nl.
+__global__ void cogroup_gather_right_kernel(const u64 *__restrict__ pos, u32 n, u64 total, const u32 *__restrict__ match,
+                                            u32 nl, u32 rb, const u64 *__restrict__ roffs, const u64 *__restrict__ rvals,
+                                            u64 *__restrict__ out)
+{
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 o = (u64)blockIdx.x * blockDim.x + threadIdx.x; o < total; o += stride) {
+        u32 lo = 0, hi = n;
+        while (hi - lo > 1) {
+            const u32 mid = (lo + hi) >> 1;
+            if (pos[mid] <= o) lo = mid; else hi = mid;
+        }
+        const u32 src = lo < nl ? match[lo] : rb + (lo - nl);
+        out[o] = rvals[roffs[src] + (o - pos[lo])];
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
 // bincode 1.2.1 blob codec (SURVEY §8(f) N1): pure byte shuffling, HBM-bound
 // ---------------------------------------------------------------------------------------------
 // Vec<(u64,u64)>: out = u64 n | n x (k, c)

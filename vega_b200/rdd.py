@@ -503,19 +503,30 @@ class JoinedRdd(_Base):
         cat = lambda xs: np.ma.concatenate(xs) if isinstance(xs[0], np.ma.MaskedArray) else np.concatenate(xs)
         return tuple(cat([p[i] for p in parts]) for i in range(3))
 
-    def cogroup_collect(self):
-        """cogroup(): per partition, the union of keys with both value lists (co_grouped_rdd.rs:206-249)."""
+    def cogroup_compute(self, split):
+        """Partition `split` of the cogroup (co_grouped_rdd.rs:206-249), aligned on the device by vb_cogroup:
+        (keys, (left_offsets, left_vals), (right_offsets, right_vals)).  Every key of either side appears once; key
+        i's lists are left_vals[left_offsets[i]:left_offsets[i + 1]] and the same on the right, empty where that
+        side lacks the key."""
         a, b = self._run()
+        lib = self.sc._lib
+        nk, nl, nr = ctypes.c_uint64(), ctypes.c_uint64(), ctypes.c_uint64()
+        L.check(lib.vb_cogroup_size(a._h, b._h, split, ctypes.byref(nk), ctypes.byref(nl), ctypes.byref(nr)))
+        keys = np.empty(nk.value, dtype=_NP_OF[a.kcode])
+        lo, ro = np.empty(nk.value + 1, dtype=np.uint64), np.empty(nk.value + 1, dtype=np.uint64)
+        lv, rv = np.empty(nl.value, dtype=_NP_OF[a.vcode]), np.empty(nr.value, dtype=_NP_OF[b.vcode])
+        p = lambda x: x.ctypes.data_as(ctypes.c_void_p)
+        L.check(lib.vb_cogroup(a._h, b._h, split, p(keys), p(lo), p(lv), p(ro), p(rv), L.VB_HOST))
+        return keys, (lo, lv), (ro, rv)
+
+    def cogroup_collect(self):
+        """cogroup(): per partition, the union of keys with both value lists (co_grouped_rdd.rs:206-249), as a list
+        of (k, (vs, ws)) with numpy arrays."""
         out = []
         for r in range(self.num_slices):
-            ka, oa, va = a.reduce(r)
-            kb, ob, vb = b.reduce(r)
-            g = {}
-            for i, k in enumerate(ka.tolist()):
-                g[k] = [va[int(oa[i]):int(oa[i + 1])], vb[:0]]
-            for i, k in enumerate(kb.tolist()):
-                g.setdefault(k, [va[:0], None])[1] = vb[int(ob[i]):int(ob[i + 1])]
-            out.extend((k, (x[0], x[1])) for k, x in g.items())
+            keys, (lo, lv), (ro, rv) = self.cogroup_compute(r)
+            lo, ro = lo.tolist(), ro.tolist()
+            out.extend((k, (lv[lo[i]:lo[i + 1]], rv[ro[i]:ro[i + 1]])) for i, k in enumerate(keys.tolist()))
         return out
 
 
