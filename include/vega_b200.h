@@ -313,6 +313,43 @@ VB_API int32_t vb_cogroup(vb_shuf *left, vb_shuf *right, uint32_t reduce_id, voi
                           uint64_t *out_left_offsets /*n_keys+1*/, void *out_left_vals,
                           uint64_t *out_right_offsets /*n_keys+1*/, void *out_right_vals, int32_t dst_loc);
 
+/* ---- string keys: byte-string keys that hash like Rust `String` (reduce_by_key / count_by_key / count_by_value /
+ *      distinct / group_by_key / partition_by_key over `String` keys, examples/group_by.rs, tests/test_pair_rdd.rs:8-37)
+ * Key i of a map partition is key_bytes[key_offsets[i] .. key_offsets[i+1]) (Arrow-style: key_offsets has n_rows + 1
+ * entries and need not start at 0, so a slice of a larger column is passed as is).  The bytes are not checked for
+ * UTF-8; equal keys are byte-equal keys; the empty key and keys containing NUL bytes are ordinary keys.
+ *   placement  MetroHash64_1(bytes ‖ 0xFF, seed 0) % n_reduce: `str::hash` (the bytes, then write_u8(0xff)) fed to
+ *              the buffering MetroHasher the integer keys already assume (vb_hash_str / vb_get_partition_str).
+ *   reduce ops per key, the results and rules of the integer-key shuffle with the same agg and val_dtype (wrapping
+ *              integer sums, unsigned / signed MIN and MAX, f64 MIN / MAX as f64::min / f64::max with NaN ignored,
+ *              COUNT as u64, vals may be NULL for COUNT).
+ *   GROUP      per key, the values in input order (map-id order, then encounter order).
+ * Re-submitting a map_id overwrites it: a key only the replaced submission had is not in the output.
+ * Limits: fewer than 2^32 - 2 rows per map partition and per shuffle, fewer than 2^31 distinct keys, every key shorter
+ * than 2^32 bytes (VB_ERR_TOO_LARGE beyond them).  Key offsets that decrease or exceed n_bytes are VB_ERR_INVALID,
+ * for device input too (checked on the device).  One process only: vb_shuffle_set_dist with world > 1, export /
+ * import / exchange and the blob calls return VB_ERR_UNSUPPORTED; vb_shuffle_set_key_width, the integer map and
+ * reduce calls and the join / cogroup calls return VB_ERR_INVALID on a string shuffle, and the string calls return
+ * VB_ERR_INVALID on any other shuffle.  seal / is_sealed / stats / kernel_time / set_hint / free work as for any
+ * shuffle (table_slots: largest dictionary index, table_restarts: index growths).
+ * vb_shuffle_reduce_str_size / vb_shuffle_reduce_str block until the shuffle is sealed and skip NULL outputs; the
+ * order of keys within a partition is unspecified.  out_key_offsets [n_keys + 1] start at 0 and index
+ * out_key_bytes [n_key_bytes]; out_combined [n_keys] for reduce ops; out_offsets [n_keys + 1] (from 0) and out_vals
+ * [n_vals] for GROUP.  dst_loc: VB_HOST or VB_DEVICE.                                                                */
+VB_API int32_t vb_shuffle_create_str(vb_ctx *ctx, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce,
+                                     int32_t val_dtype, int32_t agg, vb_shuf **out);
+VB_API int32_t vb_shuffle_map_str(vb_shuf *s, uint32_t map_id, const uint64_t *key_offsets /*n_rows+1*/,
+                                  const void *key_bytes, uint64_t n_bytes, const void *vals /*NULL for COUNT*/,
+                                  uint64_t n_rows, int32_t src_loc);
+VB_API int32_t vb_shuffle_reduce_str_size(vb_shuf *s, uint32_t reduce_id, uint64_t *n_keys, uint64_t *n_key_bytes,
+                                          uint64_t *n_vals);
+VB_API int32_t vb_shuffle_reduce_str(vb_shuf *s, uint32_t reduce_id, uint64_t *out_key_offsets /*n_keys+1*/,
+                                     void *out_key_bytes, void *out_combined, uint64_t *out_offsets /*n_keys+1*/,
+                                     void *out_vals, int32_t dst_loc);
+/* MetroHash64_1(bytes ‖ 0xFF, seed 0): the reference's hash of a `String` / `&str` key */
+VB_API uint64_t vb_hash_str(const void *bytes, uint64_t len);
+VB_API uint32_t vb_get_partition_str(const void *bytes, uint64_t len, uint32_t n_reduce);
+
 /* ---- SURVEY §8(f) N1: bincode blobs — the payload format of SHUFFLE_CACHE ------------------------
  * The reference serialises every (map, reduce) bucket with bincode 1.2.1 defaults (src/dependency.rs:213-214:
  * little-endian, fixed-width integers, u64 length prefixes) and decodes it in the fetcher

@@ -6,8 +6,9 @@
 //   PairRdd::group_by_key / reduce_by_key / join   src/rdd/pair_rdd.rs:35-52,54-80,104-121
 //   Rdd::count_by_value / distinct / collect       src/rdd/rdd.rs:450-459,502-522,420-434
 //   Rdd::intersection / subtract                   src/rdd/rdd.rs:838-946
-// Rows are Vec<(K,V)> with K in {u64,i64,i32,u32} and V in {u64,i64,f64}; reduce_by_key takes a
-// named Op (the reference's serde_closure cannot cross into CUDA).  Errors throw vega::Error
+// Rows are Vec<(K,V)> with K in {u64,i64,i32,u32,std::string} and V in {u64,i64,f64}; std::string keys are placed
+// like the reference's String keys and support group_by_key / reduce_by_key / count_by_key / count_by_value /
+// distinct.  reduce_by_key takes a named Op (the reference's serde_closure cannot cross into CUDA).  Errors throw vega::Error
 // (the reference returns Result<_> / panics).
 #pragma once
 #include <cstdint>
@@ -80,6 +81,15 @@ public:
     template <typename K, typename V>
     PairRddT<K, V> parallelize(const std::vector<std::pair<K, V>> &data, size_t num_slices) { return make_rdd(data, num_slices); }
     template <typename K> KeyRddT<K> parallelize(const std::vector<K> &data, size_t num_slices);
+
+    // std::string keys (Rust String): group_by_key / reduce_by_key / count_by_key, count_by_value / distinct
+    template <typename V> class StrPairRddT;
+    class StrKeyRddT;
+    template <typename V>
+    StrPairRddT<V> make_rdd(const std::vector<std::pair<std::string, V>> &data, size_t num_slices);
+    template <typename V>
+    StrPairRddT<V> parallelize(const std::vector<std::pair<std::string, V>> &data, size_t num_slices) { return make_rdd(data, num_slices); }
+    StrKeyRddT parallelize(const std::vector<std::string> &data, size_t num_slices);
 
 private:
     Context() = default;
@@ -360,6 +370,157 @@ private:
     size_t num_slices_;
     std::vector<uint64_t> keys_;
 };
+
+namespace detail {
+// A string key column, Arrow-style: key i is bytes[offs[i] .. offs[i + 1]).
+struct StrCol {
+    std::vector<uint64_t> offs{0};
+    std::string bytes;
+    void push(const std::string &k) { bytes += k; offs.push_back(bytes.size()); }
+    uint64_t size() const { return offs.size() - 1; }
+};
+
+inline ShufPtr run_str_shuffle(Context &sc, const StrCol &keys, const std::vector<uint64_t> *vals, size_t num_slices, size_t num_splits,
+                               int vcode, int agg)
+{
+    if (num_slices < 1) throw Error(VB_ERR_INVALID, "Number of slices should be greater than or equal to 1");
+    const uint64_t n = keys.size();
+    std::vector<uint64_t> starts(std::min<uint64_t>(n, num_slices) + 2);
+    const uint64_t n_map = vb_slice(n, num_slices, starts.data());
+    vb_shuf *raw = nullptr;
+    check(vb_shuffle_create_str(sc.raw(), sc.new_shuffle_id(), (uint32_t)n_map, (uint32_t)num_splits, vcode, agg, &raw));
+    ShufPtr s(raw);
+    for (uint64_t m = 0; m < n_map; ++m) {
+        const uint64_t lo = starts[m], cnt = starts[m + 1] - lo;
+        check(vb_shuffle_map_str(raw, (uint32_t)m, keys.offs.data() + lo, keys.bytes.data(), keys.bytes.size(),
+                                 (vals && cnt) ? vals->data() + lo : nullptr, cnt, VB_HOST));
+    }
+    check(vb_shuffle_seal(raw));
+    return s;
+}
+
+// partition r of a sealed string shuffle: its keys, and the combined values (reduce ops) or the CSR (GROUP)
+inline std::vector<std::string> read_str_part(vb_shuf *s, uint32_t r, std::vector<uint64_t> *comb, std::vector<uint64_t> *offs,
+                                              std::vector<uint64_t> *vals)
+{
+    uint64_t nk = 0, nb = 0, nv = 0;
+    check(vb_shuffle_reduce_str_size(s, r, &nk, &nb, &nv));
+    std::vector<uint64_t> ko(nk + 1);
+    std::string kb(nb, '\0');
+    if (comb) comb->resize(nk);
+    if (offs) offs->resize(nk + 1);
+    if (vals) vals->resize(nv);
+    check(vb_shuffle_reduce_str(s, r, ko.data(), kb.data(), comb ? comb->data() : nullptr, offs ? offs->data() : nullptr,
+                                vals ? vals->data() : nullptr, VB_HOST));
+    std::vector<std::string> keys;
+    for (uint64_t i = 0; i < nk; ++i) keys.emplace_back(kb, ko[i], ko[i + 1] - ko[i]);
+    return keys;
+}
+}  // namespace detail
+
+template <typename V>
+class Context::StrPairRddT {
+public:
+    StrPairRddT(std::shared_ptr<Context> sc, const std::vector<std::pair<std::string, V>> &data, size_t num_slices)
+        : sc_(std::move(sc)), num_slices_(num_slices)
+    {
+        for (auto &kv : data) { keys_.push(kv.first); vals_.push_back(detail::to_bits<V>(kv.second)); }
+    }
+    size_t number_of_splits() const { return num_slices_; }
+
+    // group_by_key(num_splits).collect()  →  Vec<(String, Vec<V>)>, values in input order
+    std::vector<std::pair<std::string, std::vector<V>>> group_by_key(size_t num_splits) const
+    {
+        auto s = detail::run_str_shuffle(*sc_, keys_, &vals_, num_slices_, num_splits, detail::dtype<V>::code, VB_AGG_GROUP);
+        std::vector<std::pair<std::string, std::vector<V>>> out;
+        for (uint32_t r = 0; r < num_splits; ++r) {
+            std::vector<uint64_t> o, v;
+            auto k = detail::read_str_part(s.get(), r, nullptr, &o, &v);
+            for (size_t i = 0; i < k.size(); ++i) {
+                std::vector<V> vs;
+                for (uint64_t j = o[i]; j < o[i + 1]; ++j) vs.push_back(detail::from_bits<V>(v[j]));
+                out.emplace_back(std::move(k[i]), std::move(vs));
+            }
+        }
+        return out;
+    }
+
+    // reduce_by_key(op, num_splits).collect()  →  Vec<(String, V)>
+    std::vector<std::pair<std::string, V>> reduce_by_key(Op op, size_t num_splits) const
+    {
+        auto s = detail::run_str_shuffle(*sc_, keys_, &vals_, num_slices_, num_splits, detail::dtype<V>::code, (int)op);
+        std::vector<std::pair<std::string, V>> out;
+        for (uint32_t r = 0; r < num_splits; ++r) {
+            std::vector<uint64_t> c;
+            auto k = detail::read_str_part(s.get(), r, &c, nullptr, nullptr);
+            for (size_t i = 0; i < k.size(); ++i) out.emplace_back(std::move(k[i]), detail::from_bits<V>(c[i]));
+        }
+        return out;
+    }
+
+    // count_by_key(num_splits).collect()  →  Vec<(String, u64)>
+    std::vector<std::pair<std::string, uint64_t>> count_by_key(size_t num_splits) const
+    {
+        auto s = detail::run_str_shuffle(*sc_, keys_, nullptr, num_slices_, num_splits, VB_U64, VB_AGG_COUNT);
+        std::vector<std::pair<std::string, uint64_t>> out;
+        for (uint32_t r = 0; r < num_splits; ++r) {
+            std::vector<uint64_t> c;
+            auto k = detail::read_str_part(s.get(), r, &c, nullptr, nullptr);
+            for (size_t i = 0; i < k.size(); ++i) out.emplace_back(std::move(k[i]), c[i]);
+        }
+        return out;
+    }
+
+private:
+    std::shared_ptr<Context> sc_;
+    size_t num_slices_;
+    detail::StrCol keys_;
+    std::vector<uint64_t> vals_;
+};
+
+class Context::StrKeyRddT {
+public:
+    StrKeyRddT(std::shared_ptr<Context> sc, const std::vector<std::string> &data, size_t num_slices) : sc_(std::move(sc)), num_slices_(num_slices)
+    {
+        for (auto &k : data) keys_.push(k);
+    }
+    // count_by_value().collect() → Vec<(String, u64)>   (src/rdd/rdd.rs:450-459)
+    std::vector<std::pair<std::string, uint64_t>> count_by_value() const
+    {
+        std::vector<uint64_t> starts(std::min<uint64_t>(keys_.size(), num_slices_) + 2);
+        const size_t n_splits = vb_slice(keys_.size(), num_slices_, starts.data());
+        auto s = detail::run_str_shuffle(*sc_, keys_, nullptr, num_slices_, n_splits, VB_U64, VB_AGG_COUNT);
+        std::vector<std::pair<std::string, uint64_t>> out;
+        for (uint32_t r = 0; r < n_splits; ++r) {
+            std::vector<uint64_t> c;
+            auto k = detail::read_str_part(s.get(), r, &c, nullptr, nullptr);
+            for (size_t i = 0; i < k.size(); ++i) out.emplace_back(std::move(k[i]), c[i]);
+        }
+        return out;
+    }
+    // distinct().collect()   (src/rdd/rdd.rs:502-522)
+    std::vector<std::string> distinct() const
+    {
+        std::vector<std::string> out;
+        for (auto &kv : count_by_value()) out.push_back(kv.first);
+        return out;
+    }
+
+private:
+    std::shared_ptr<Context> sc_;
+    size_t num_slices_;
+    detail::StrCol keys_;
+};
+
+template <typename V>
+Context::StrPairRddT<V> Context::make_rdd(const std::vector<std::pair<std::string, V>> &data, size_t num_slices)
+{
+    return StrPairRddT<V>(shared_from_this(), data, num_slices);
+}
+inline Context::StrKeyRddT Context::parallelize(const std::vector<std::string> &data, size_t num_slices)
+{
+    return StrKeyRddT(shared_from_this(), data, num_slices);
+}
 
 template <typename K, typename V>
 Context::PairRddT<K, V> Context::make_rdd(const std::vector<std::pair<K, V>> &data, size_t num_slices)

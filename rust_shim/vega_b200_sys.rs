@@ -78,6 +78,17 @@ extern "C" {
                                    val_dtypes: *const i32, n_aggs: u32, aggs: *const vb_agg_col, out: *mut *mut vb_shuf) -> i32;
     pub fn vb_shuffle_map_cols(s: *mut vb_shuf, map_id: u32, keys: *const c_void, vals: *const *const c_void, n_rows: u64, src_loc: i32) -> i32;
     pub fn vb_shuffle_reduce_cols(s: *mut vb_shuf, reduce_id: u32, out_keys: *mut c_void, out_aggs: *const *mut c_void, dst_loc: i32) -> i32;
+    // String keys (Arrow-style offsets + bytes; placed by MetroHash64_1(bytes ‖ 0xFF) like `str::hash`)
+    pub fn vb_shuffle_create_str(ctx: *mut vb_ctx, shuffle_id: u64, n_map: u32, n_reduce: u32, val_dtype: i32, agg: i32,
+                                 out: *mut *mut vb_shuf) -> i32;
+    pub fn vb_shuffle_map_str(s: *mut vb_shuf, map_id: u32, key_offsets: *const u64, key_bytes: *const c_void, n_bytes: u64,
+                              vals: *const c_void, n_rows: u64, src_loc: i32) -> i32;
+    pub fn vb_shuffle_reduce_str_size(s: *mut vb_shuf, reduce_id: u32, n_keys: *mut u64, n_key_bytes: *mut u64,
+                                      n_vals: *mut u64) -> i32;
+    pub fn vb_shuffle_reduce_str(s: *mut vb_shuf, reduce_id: u32, out_key_offsets: *mut u64, out_key_bytes: *mut c_void,
+                                 out_combined: *mut c_void, out_offsets: *mut u64, out_vals: *mut c_void, dst_loc: i32) -> i32;
+    pub fn vb_hash_str(bytes: *const c_void, len: u64) -> u64;
+    pub fn vb_get_partition_str(bytes: *const c_void, len: u64, n_reduce: u32) -> u32;
     pub fn vb_shuffle_free(s: *mut vb_shuf) -> i32;
     pub fn vb_last_error() -> *const c_char;
     pub fn vb_get_partition(key: u64, key_width: u32, n_reduce: u32) -> u32;

@@ -96,6 +96,12 @@ SYMBOLS = {
     "vb_join_outer": (_i32, [_vp, _vp, _u32, _i32, _vp, _vp, _vp, _vp, _vp, _i32]),
     "vb_cogroup_size": (_i32, [_vp, _vp, _u32, _pu64, _pu64, _pu64]),
     "vb_cogroup": (_i32, [_vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _i32]),
+    "vb_shuffle_create_str": (_i32, [_vp, _u64, _u32, _u32, _i32, _i32, _pvp]),
+    "vb_shuffle_map_str": (_i32, [_vp, _u32, _vp, _vp, _u64, _vp, _u64, _i32]),
+    "vb_shuffle_reduce_str_size": (_i32, [_vp, _u32, _pu64, _pu64, _pu64]),
+    "vb_shuffle_reduce_str": (_i32, [_vp, _u32, _vp, _vp, _vp, _vp, _vp, _i32]),
+    "vb_hash_str": (_u64, [_vp, _u64]),
+    "vb_get_partition_str": (_u32, [_vp, _u64, _u32]),
     "vb_shuffle_reduce_blob_size": (_i32, [_vp, _u32, _pu64]),
     "vb_shuffle_reduce_blob": (_i32, [_vp, _u32, _vp, _i32]),
     "vb_shuffle_map_blob": (_i32, [_vp, _u32, _vp, _u64, _i32]),

@@ -19,6 +19,7 @@
 #include "kernels.cuh"
 #include "sweep.cuh"
 #include "gsweep.cuh"
+#include "strkeys.cuh"
 #include <type_traits>
 
 using namespace vb;
@@ -360,6 +361,7 @@ struct vb_shuf {
     u64 *lz_keys = nullptr, *lz_vals = nullptr;
     u64 lz_n = 0;
     std::vector<vb_shuf *> trash;                  // internal shuffles of a failed filtered join
+    struct StrState *str = nullptr;                // string-key shuffle (vb_shuffle_create_str): dictionary, rows, results
     // by (the right side's uid, join kind): internal (left, right) shuffles over the rows that join kind keeps
     std::map<std::pair<u64, int>, std::pair<vb_shuf *, vb_shuf *>> filtered;
     // stats
@@ -368,6 +370,9 @@ struct vb_shuf {
     double kms[K_N] = {0};
     u64 klaunch[K_N] = {0};
 };
+
+static int seal_str(vb_shuf *s);
+static void free_str(vb_shuf *s);
 
 static bool is_reduce_op(int agg) { return agg == VB_AGG_SUM || agg == VB_AGG_MIN || agg == VB_AGG_MAX || agg == VB_AGG_COUNT; }
 static bool is_group_op(int agg) { return agg == VB_AGG_GROUP || agg == VB_AGG_COGROUP; }
@@ -1344,9 +1349,20 @@ static int reject_multi(const vb_shuf *s, const char *what)
     return set_err(VB_ERR_UNSUPPORTED, "shuffle %llu has several aggregates per key: %s is not supported for it yet", (unsigned long long)s->id, what);
 }
 
+// string-key shuffles: calls that do not apply (VB_ERR_INVALID) and calls not supported for them yet (VB_ERR_UNSUPPORTED)
+static int invalid_str(const vb_shuf *s, const char *what)
+{
+    return set_err(VB_ERR_INVALID, "shuffle %llu has string keys: %s does not apply to it", (unsigned long long)s->id, what);
+}
+static int reject_str(const vb_shuf *s, const char *what)
+{
+    return set_err(VB_ERR_UNSUPPORTED, "shuffle %llu has string keys: %s is not supported for it yet", (unsigned long long)s->id, what);
+}
+
 extern "C" int32_t vb_shuffle_set_key_width(vb_shuf *s, uint32_t bytes)
 {
     if (!s || (bytes != 4 && bytes != 8)) return set_err(VB_ERR_INVALID, "key width must be 4 or 8");
+    if (s->str) return invalid_str(s, "vb_shuffle_set_key_width");
     s->key_width = bytes;
     return VB_OK;
 }
@@ -1362,6 +1378,7 @@ extern "C" int32_t vb_shuffle_set_dist(vb_shuf *s, uint32_t rank, uint32_t world
 {
     if (!s || world < 1 || rank >= world || world > 256) return set_err(VB_ERR_INVALID, "bad rank/world");
     if (s->multi && world > 1) return reject_multi(s, "multi-rank use (the exchange moves one value column)");
+    if (s->str && world > 1) return reject_str(s, "multi-rank use");
     s->rank = rank;
     s->world = world;
     return VB_OK;
@@ -1382,6 +1399,7 @@ static int shuffle_map(vb_shuf *s, u32 map_id, const u64 *rows, const u64 *keys,
                        const u64 *const *cols = nullptr)
 {
     if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
+    if (s->str) return invalid_str(s, "an integer-key map call");
     if (map_id >= s->n_map) return set_err(VB_ERR_INVALID, "map_id %u >= n_map %u", map_id, s->n_map);
     if (loc < VB_HOST || loc > VB_DEVICE_BORROWED) return set_err(VB_ERR_INVALID, "bad src_loc %d", loc);
     if (n && !rows && !keys) return set_err(VB_ERR_INVALID, "NULL input with n_rows > 0");
@@ -1923,6 +1941,7 @@ extern "C" int32_t vb_shuffle_export_prepare(vb_shuf *s, uint64_t *counts)
 {
     if (!s || !counts) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "multi-rank exchange");
+    if (s->str) return reject_str(s, "multi-rank exchange");
     if (s->world < 2) return set_err(VB_ERR_STATE, "vb_shuffle_export_prepare needs vb_shuffle_set_dist(world > 1)");
     vb_ctx *c = s->ctx;
     std::lock_guard<std::mutex> lk(c->mu);
@@ -2037,6 +2056,7 @@ extern "C" int32_t vb_shuffle_export_counts(vb_shuf *s, uint64_t *counts)
 {
     if (!s || !counts) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "multi-rank exchange");
+    if (s->str) return reject_str(s, "multi-rank exchange");
     if (s->world < 2) return set_err(VB_ERR_STATE, "vb_shuffle_export_counts needs vb_shuffle_set_dist(world > 1)");
     std::lock_guard<std::mutex> lk(s->ctx->mu);
     CU(cudaSetDevice(s->ctx->device));
@@ -2102,6 +2122,7 @@ extern "C" int32_t vb_shuffle_export_direct(vb_shuf *s, const uint64_t *dst_row_
 {
     if (!s || !dst_row_offset || !dst_total_rows) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "multi-rank exchange");
+    if (s->str) return reject_str(s, "multi-rank exchange");
     std::lock_guard<std::mutex> lk(s->ctx->mu);
     CU(cudaSetDevice(s->ctx->device));
     return export_direct_locked(s, dst_row_offset, dst_total_rows, true);
@@ -2113,6 +2134,7 @@ extern "C" int32_t vb_shuffle_import_arena(vb_shuf *s, const uint64_t *counts)
 {
     if (!s || !counts) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "multi-rank exchange");
+    if (s->str) return reject_str(s, "multi-rank exchange");
     if (!s->exported || s->sealed) return set_err(VB_ERR_STATE, "import needs the export first and no seal yet");
     u64 n = 0;
     for (u32 r = 0; r < s->world; ++r) n += counts[r];
@@ -2129,6 +2151,7 @@ extern "C" int32_t vb_shuffle_export_buffers(vb_shuf *s, void **keys_dev, void *
 {
     if (!s || !keys_dev || !vals_dev) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "multi-rank exchange");
+    if (s->str) return reject_str(s, "multi-rank exchange");
     if (!s->exported) return set_err(VB_ERR_STATE, "vb_shuffle_export_buffers before vb_shuffle_export_prepare");
     *keys_dev = s->exp_keys;
     *vals_dev = s->exp_vals;
@@ -2139,6 +2162,7 @@ extern "C" int32_t vb_shuffle_import(vb_shuf *s, const void *keys_dev, const voi
 {
     if (!s || !counts) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "multi-rank exchange");
+    if (s->str) return reject_str(s, "multi-rank exchange");
     if (!s->exported || s->sealed) return set_err(VB_ERR_STATE, "import needs export_prepare first and no seal yet");
     u64 n = 0;
     for (u32 r = 0; r < s->world; ++r) n += counts[r];
@@ -2606,6 +2630,7 @@ extern "C" int32_t vb_shuffle_exchange(vb_shuf *s, int32_t mode)
 {
     if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
     if (s->multi) return reject_multi(s, "multi-rank exchange");
+    if (s->str) return reject_str(s, "multi-rank exchange");
     vb_ctx *c = s->ctx;
     if (s->world < 2) return set_err(VB_ERR_STATE, "vb_shuffle_exchange needs vb_shuffle_set_dist(world > 1)");
     if (!c->comm) return set_err(VB_ERR_STATE, "vb_shuffle_exchange needs vb_ctx_comm_init");
@@ -2902,7 +2927,9 @@ extern "C" int32_t vb_shuffle_seal(vb_shuf *s)
             if (s->world == 1) {
                 for (u32 m = 0; m < s->n_map; ++m)
                     if (!s->maps[m].present) return set_err(VB_ERR_STATE, "shuffle %llu sealed but map %u was never submitted", (unsigned long long)s->id, m);
-                if (is_reduce_op(s->agg)) {
+                if (s->str) {
+                    TRY(seal_str(s));
+                } else if (is_reduce_op(s->agg)) {
                     void *tab = nullptr; u32 log_cap = 0; u64 n_ins = 0;
                     TRY(merge_map_tables(s, &tab, &log_cap, &n_ins));
                     DevBuf guard(c); guard.p = tab;
@@ -2972,6 +2999,7 @@ static int wait_sealed(vb_shuf *s)
 extern "C" int32_t vb_shuffle_reduce_size(vb_shuf *s, uint32_t r, uint64_t *n_keys, uint64_t *n_vals)
 {
     if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
+    if (s->str) return invalid_str(s, "vb_shuffle_reduce_size (read it with vb_shuffle_reduce_str_size)");
     if (r >= s->n_reduce) return set_err(VB_ERR_INVALID, "reduce_id %u >= n_reduce %u", r, s->n_reduce);
     TRY(wait_sealed(s));
     if (s->lazy) {                                   // first cogroup materialisation: group all rows now
@@ -2997,6 +3025,7 @@ extern "C" int32_t vb_shuffle_reduce(vb_shuf *s, uint32_t r, void *out_keys, voi
                                      void *out_vals, int32_t dst_loc)
 {
     if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
+    if (s->str) return invalid_str(s, "vb_shuffle_reduce (read it with vb_shuffle_reduce_str)");
     if (r >= s->n_reduce) return set_err(VB_ERR_INVALID, "reduce_id %u >= n_reduce %u", r, s->n_reduce);
     if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
     TRY(wait_sealed(s));
@@ -3064,6 +3093,7 @@ extern "C" int32_t vb_shuffle_reduce_blob_size(vb_shuf *s, uint32_t r, uint64_t 
 {
     if (!s || !n_bytes) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "bincode blobs");
+    if (s->str) return reject_str(s, "bincode blobs");
     if (r >= s->n_reduce) return set_err(VB_ERR_INVALID, "reduce_id %u >= n_reduce %u", r, s->n_reduce);
     TRY(wait_sealed(s));
     if (s->lazy) {
@@ -3079,6 +3109,7 @@ extern "C" int32_t vb_shuffle_reduce_blob(vb_shuf *s, uint32_t r, void *out_blob
 {
     if (!s || !out_blob) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "bincode blobs");
+    if (s->str) return reject_str(s, "bincode blobs");
     if (r >= s->n_reduce) return set_err(VB_ERR_INVALID, "reduce_id %u >= n_reduce %u", r, s->n_reduce);
     if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
     TRY(wait_sealed(s));
@@ -3112,6 +3143,7 @@ extern "C" int32_t vb_shuffle_map_blob(vb_shuf *s, uint32_t map_id, const void *
 {
     if (!s || !blob) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "bincode blobs");
+    if (s->str) return reject_str(s, "bincode blobs");
     if (src_loc < VB_HOST || src_loc > VB_DEVICE_BORROWED) return set_err(VB_ERR_INVALID, "bad src_loc");
     if (s->agg == VB_AGG_SORT) return set_err(VB_ERR_UNSUPPORTED, "sort_by_key takes rows, not combined buckets");
     if (n_bytes < 8 || (n_bytes & 7)) return set_err(VB_ERR_INVALID, "corrupted blob: %llu bytes", (unsigned long long)n_bytes);
@@ -3178,6 +3210,7 @@ static int exclusive_scan_u64(vb_shuf *s, const u64 *in, u64 *out, u64 n, u64 *d
 static int join_check(vb_shuf *l, vb_shuf *r, u32 rid)
 {
     if (!l || !r) return set_err(VB_ERR_INVALID, "NULL shuffle");
+    if (l->str || r->str) return invalid_str(l->str ? l : r, "a join or cogroup");
     if (!is_group_op(l->agg) || !is_group_op(r->agg)) return set_err(VB_ERR_INVALID, "join needs two GROUP/COGROUP shuffles");
     if (l->n_reduce != r->n_reduce || l->key_width != r->key_width) return set_err(VB_ERR_INVALID, "join sides use different partitioners");
     if (l->ctx != r->ctx) return set_err(VB_ERR_INVALID, "join sides live on different contexts");
@@ -3529,6 +3562,540 @@ extern "C" int32_t vb_cogroup(vb_shuf *l, vb_shuf *r, uint32_t rid, void *out_ke
 }
 
 // ---------------------------------------------------------------------------------------------
+// string keys (vb_shuffle_create_str): byte-string keys placed like the reference's `String` keys
+// ---------------------------------------------------------------------------------------------
+// One shuffle's dictionary of distinct keys (strkeys.cuh: entries + arena + index), the map calls' rows as entry ids,
+// and after seal the partition-major key column (Arrow-style offsets + bytes) beside the usual res_* arrays.
+struct StrState {
+    StrDict d{};                          // device arrays; d.fp / d.id have 1 << d.log_cap slots
+    u64 cap_e = 0, cap_a = 0;             // entries / arena bytes reserved
+    u32 n_e = 0;                          // entries in use (ctl->n_entries after the last call)
+    u64 n_a = 0;                          // arena bytes in use
+    StrCtl *ctl = nullptr;
+    std::vector<u32 *> ids;               // per map id: the rows' entry ids (owned)
+    std::vector<const u64 *> vals;        // per map id: the rows' values
+    std::vector<char> vals_owned;         // per map id: vals is a copy (else borrowed, VB_DEVICE_BORROWED)
+    u64 *key_off = nullptr;               // [n_keys + 1] byte offset of every result key (partition-major, from 0)
+    unsigned char *key_bytes = nullptr;   // the result keys' bytes
+    std::vector<u64> kb_off;              // [n_reduce + 1] first key byte of each partition
+};
+
+constexpr u32 STR_MAX_LOG_CAP = 33;       // index slots: < 2^31 distinct keys at load <= 0.6
+
+// VEGA_B200_STR_FP_BITS=k keeps k bits of the hash in the index fingerprint (test switch: forces equal fingerprints of
+// distinct keys, which must then be told apart by their bytes).  Placement always uses the full hash.
+static u64 str_fp_mask()
+{
+    static const u64 m = [] {
+        const char *e = getenv("VEGA_B200_STR_FP_BITS");
+        const int k = e ? atoi(e) : 64;
+        return (k <= 0 || k >= 64) ? ~0ull : ((1ull << k) - 1);
+    }();
+    return m;
+}
+
+static void free_str_map(vb_shuf *s, u32 m)
+{
+    StrState *t = s->str;
+    dev_free(s->ctx, t->ids[m]);
+    if (t->vals_owned[m]) dev_free(s->ctx, t->vals[m]);
+    t->ids[m] = nullptr;
+    t->vals[m] = nullptr;
+    t->vals_owned[m] = 0;
+}
+
+static void free_str_dict(vb_shuf *s)
+{
+    StrState *t = s->str;
+    vb_ctx *c = s->ctx;
+    dev_free(c, t->d.fp); dev_free(c, t->d.id);
+    dev_free(c, t->d.e_hash); dev_free(c, t->d.e_off); dev_free(c, t->d.e_len); dev_free(c, t->d.arena);
+    dev_free(c, t->ctl);
+    t->d.fp = nullptr; t->d.id = nullptr;
+    t->d.e_hash = t->d.e_off = nullptr; t->d.e_len = nullptr; t->d.arena = nullptr;
+    t->ctl = nullptr;
+    t->cap_e = t->cap_a = 0;
+}
+
+static void free_str(vb_shuf *s)
+{
+    StrState *t = s->str;
+    if (!t) return;
+    for (u32 m = 0; m < s->n_map; ++m) free_str_map(s, m);
+    free_str_dict(s);
+    dev_free(s->ctx, t->key_off);
+    dev_free(s->ctx, t->key_bytes);
+    delete t;
+    s->str = nullptr;
+}
+
+extern "C" int32_t vb_shuffle_create_str(vb_ctx *c, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce, int32_t vdt, int32_t agg,
+                                         vb_shuf **out)
+{
+    if (!c || !out) return set_err(VB_ERR_INVALID, "vb_shuffle_create_str: NULL argument");
+    *out = nullptr;
+    if (agg != VB_AGG_SUM && agg != VB_AGG_MIN && agg != VB_AGG_MAX && agg != VB_AGG_COUNT && agg != VB_AGG_GROUP)
+        return set_err(VB_ERR_UNSUPPORTED, "string keys: agg %d is not supported (SUM, MIN, MAX, COUNT and GROUP are)", agg);
+    TRY(vb_shuffle_create(c, shuffle_id, n_map, n_reduce, VB_U64, vdt, agg, VB_PART_HASH_METRO64, out));
+    StrState *t = new StrState();
+    t->ids.assign(n_map, nullptr);
+    t->vals.assign(n_map, nullptr);
+    t->vals_owned.assign(n_map, 0);
+    t->d.fp_mask = str_fp_mask();
+    (*out)->str = t;
+    return VB_OK;
+}
+
+// Reallocate one device array to `cap` elements of `sz` bytes, keeping the first `keep`.
+template <typename T>
+static int str_regrow(vb_ctx *c, T **p, u64 cap, u64 keep)
+{
+    DevBuf nb(c);
+    TRY(nb.alloc(cap * sizeof(T)));
+    if (keep) CU(cudaMemcpyAsync(nb.p, *p, keep * sizeof(T), cudaMemcpyDeviceToDevice, c->stream));
+    dev_free(c, *p);
+    *p = (T *)nb.release();
+    return VB_OK;
+}
+
+// Entries and arena for the worst case of the next call (every row a new key), growing by doubling.
+static int str_reserve(vb_shuf *s, u64 want_e, u64 want_a)
+{
+    StrState *t = s->str;
+    vb_ctx *c = s->ctx;
+    if (want_e > t->cap_e || !t->d.e_hash) {
+        const u64 cap = std::max<u64>(want_e, std::max<u64>(2 * t->cap_e, 1024));
+        TRY(str_regrow(c, &t->d.e_hash, cap, t->n_e));
+        TRY(str_regrow(c, &t->d.e_off, cap, t->n_e));
+        TRY(str_regrow(c, &t->d.e_len, cap, t->n_e));
+        t->cap_e = cap;
+    }
+    if (want_a > t->cap_a || !t->d.arena) {
+        const u64 cap = std::max<u64>(want_a, std::max<u64>(2 * t->cap_a, 1 << 16));
+        TRY(str_regrow(c, &t->d.arena, cap, t->n_a));
+        t->cap_a = cap;
+    }
+    return VB_OK;
+}
+
+// A new index of at least 2^log_cap slots holding every entry (larger if the entries do not fit).
+static int str_index_build(vb_shuf *s, u32 log_cap)
+{
+    StrState *t = s->str;
+    vb_ctx *c = s->ctx;
+    for (;;) {
+        if (log_cap > STR_MAX_LOG_CAP) return set_err(VB_ERR_TOO_LARGE, "string-key index beyond 2^%u slots", STR_MAX_LOG_CAP);
+        const u64 cap = 1ull << log_cap;
+        DevBuf fp(c), id(c);
+        TRY(fp.alloc(cap * 8));
+        TRY(id.alloc(cap * 4));
+        CU(cudaMemsetAsync(fp.p, 0, cap * 8, c->stream));
+        CU(cudaMemsetAsync(id.p, 0xFF, cap * 4, c->stream));
+        StrDict nd = t->d;
+        nd.fp = fp.as<u64>();
+        nd.id = id.as<u32>();
+        nd.log_cap = log_cap;
+        u32 abort = 0;
+        if (t->n_e) {
+            CU(cudaMemsetAsync(&t->ctl->abort, 0, 4, c->stream));
+            KLaunch kl(s, K_DICT, t->n_e);
+            const u64 blocks = std::min<u64>((t->n_e + 255) / 256, (u64)c->sm_count * 8);
+            str_index_rebuild_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(nd, t->n_e, t->ctl);
+            TRY(kl.done("str_index_rebuild_kernel"));
+            TRY(fetch_status_unlocked(c, &t->ctl->abort, &abort, 4));
+        }
+        if (!abort) {
+            dev_free(c, t->d.fp);
+            dev_free(c, t->d.id);
+            t->d = nd;
+            fp.release();
+            id.release();
+            s->st.table_slots = std::max<u64>(s->st.table_slots, cap);
+            return VB_OK;
+        }
+        ++log_cap;
+    }
+}
+
+// Key offsets of one call: VB_ERR_INVALID when decreasing or beyond n_bytes, VB_ERR_TOO_LARGE for a key of 2^32 bytes
+// or more.  Host offsets are checked here, device offsets by str_check_offsets_kernel.  *first / *last: offs[0], offs[n].
+static int str_check_offsets(vb_shuf *s, const u64 *offs, u64 n, u64 n_bytes, int loc, u64 *first, u64 *last)
+{
+    vb_ctx *c = s->ctx;
+    u32 flags = 0;
+    if (loc == VB_HOST) {
+        for (u64 i = 0; i <= n; ++i) {
+            if (offs[i] > n_bytes) flags |= 1u;
+            if (i < n) {
+                if (offs[i + 1] < offs[i]) flags |= 1u;
+                else if (offs[i + 1] - offs[i] >= (1ull << 32)) flags |= 2u;
+            }
+        }
+        *first = offs[0];
+        *last = offs[n];
+    } else {
+        DevBuf f(c);
+        TRY(f.alloc(4));
+        CU(cudaMemsetAsync(f.p, 0, 4, c->stream));
+        {
+            KLaunch kl(s, K_MISC, n);
+            const u64 blocks = std::min<u64>((n + 256) / 256, (u64)c->sm_count * 8);
+            str_check_offsets_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(offs, n, n_bytes, f.as<u32>());
+            TRY(kl.done("str_check_offsets_kernel"));
+        }
+        u64 *h = (u64 *)c->h_scratch;
+        CU(cudaMemcpyAsync(h, offs, 8, cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaMemcpyAsync(h + 1, offs + n, 8, cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaMemcpyAsync(h + 2, f.p, 4, cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaStreamSynchronize(c->stream));
+        *first = h[0];
+        *last = h[1];
+        flags = (u32)h[2];
+    }
+    if (flags & 1u) return set_err(VB_ERR_INVALID, "key offsets decrease or exceed n_bytes %llu", (unsigned long long)n_bytes);
+    if (flags & 2u) return set_err(VB_ERR_TOO_LARGE, "a key of 2^32 bytes or more");
+    return VB_OK;
+}
+
+extern "C" int32_t vb_shuffle_map_str(vb_shuf *s, uint32_t map_id, const uint64_t *key_offsets, const void *key_bytes, uint64_t n_bytes,
+                                      const void *vals, uint64_t n, int32_t loc)
+{
+    if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
+    if (!s->str) return set_err(VB_ERR_INVALID, "vb_shuffle_map_str needs a shuffle from vb_shuffle_create_str");
+    if (map_id >= s->n_map) return set_err(VB_ERR_INVALID, "map_id %u >= n_map %u", map_id, s->n_map);
+    if (loc < VB_HOST || loc > VB_DEVICE_BORROWED) return set_err(VB_ERR_INVALID, "bad src_loc %d", loc);
+    if (n && !key_offsets) return set_err(VB_ERR_INVALID, "NULL key_offsets with n_rows > 0");
+    if (n && n_bytes && !key_bytes) return set_err(VB_ERR_INVALID, "NULL key_bytes with n_bytes > 0");
+    if (n && !vals && s->agg != VB_AGG_COUNT) return set_err(VB_ERR_INVALID, "values required for this aggregator");
+    if (n >= 0xFFFFFFFEull) return set_err(VB_ERR_TOO_LARGE, "map partition of %llu rows", (unsigned long long)n);
+    {
+        std::lock_guard<std::mutex> g(s->mu);
+        if (s->sealed || s->sealing || s->freed) return set_err(VB_ERR_STATE, "shuffle %llu: map after seal", (unsigned long long)s->id);
+    }
+    vb_ctx *c = s->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    KLaunch call(s, -1);
+    StrState *t = s->str;
+    u64 others = 0;
+    for (u32 j = 0; j < s->n_map; ++j)
+        if (j != map_id && s->maps[j].present) others += s->maps[j].n_rows;
+    if (others + n >= 0xFFFFFFFEull) return set_err(VB_ERR_TOO_LARGE, "shuffle of %llu rows on one device", (unsigned long long)(others + n));
+    DevBuf d_offs(c), d_bytes(c), d_vals(c), ids(c);
+    const u64 *offs = key_offsets;
+    const unsigned char *bytes = (const unsigned char *)key_bytes;
+    u64 first = 0, last = 0;
+    if (n) {
+        TRY(str_check_offsets(s, key_offsets, n, n_bytes, loc, &first, &last));
+        if ((u64)t->n_e + n > 0xFFFFFFFFull) return set_err(VB_ERR_TOO_LARGE, "more than 2^32 - 1 string keys submitted to one shuffle");
+        if (loc == VB_HOST) {       // the encode kernel reads key i at bytes + (offs[i] - first)
+            TRY(d_offs.alloc((n + 1) * 8));
+            TRY(d_bytes.alloc(last - first));
+            CU(cudaMemcpyAsync(d_offs.p, key_offsets, (n + 1) * 8, cudaMemcpyHostToDevice, c->stream));
+            if (last > first) CU(cudaMemcpyAsync(d_bytes.p, bytes + first, last - first, cudaMemcpyHostToDevice, c->stream));
+            s->st.h2d_bytes += (n + 1) * 8 + (last - first);
+            offs = d_offs.as<u64>();
+            bytes = d_bytes.as<unsigned char>();
+        } else {
+            bytes = bytes ? bytes + first : nullptr;
+        }
+        TRY(str_reserve(s, (u64)t->n_e + n, t->n_a + (last - first)));
+        if (!t->ctl) {
+            DevBuf ctl(c);
+            TRY(ctl.alloc(sizeof(StrCtl)));
+            CU(cudaMemsetAsync(ctl.p, 0, sizeof(StrCtl), c->stream));
+            t->ctl = (StrCtl *)ctl.release();
+        }
+        if (!t->d.fp) {
+            const u64 guess = n * std::max<u32>(1, s->n_map);
+            TRY(str_index_build(s, choose_log_cap(guess, s->hint, false, STR_MAX_LOG_CAP, c->l2_bytes, 12)));
+        }
+        TRY(ids.alloc(n * 4));
+        for (;;) {
+            const u64 cap = 1ull << t->d.log_cap;
+            const u32 max_entries = (u32)std::min<u64>((cap / 10) * 6, 0xFFFFFFFFull);
+            CU(cudaMemsetAsync(&t->ctl->abort, 0, 4, c->stream));
+            {
+                KLaunch kl(s, K_DICT, n);
+                const u64 blocks = std::min<u64>((n + 255) / 256, (u64)c->sm_count * 8);
+                str_encode_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(offs, bytes, first, n, t->d, t->ctl, max_entries, ids.as<u32>());
+                TRY(kl.done("str_encode_kernel"));
+            }
+            StrCtl h;
+            TRY(fetch_status_unlocked(c, t->ctl, &h, sizeof(StrCtl)));
+            t->n_e = h.n_entries;
+            t->n_a = h.n_arena;
+            if (!h.abort) break;
+            s->st.table_restarts++;                // grow the index (at least 4x) and rerun the whole call
+            TRY(str_index_build(s, std::max<u32>(t->d.log_cap + 2, ceil_log2_u64(3 * (u64)t->n_e))));
+        }
+        if (s->agg != VB_AGG_COUNT && loc != VB_DEVICE_BORROWED) {
+            TRY(d_vals.alloc(n * 8));
+            CU(cudaMemcpyAsync(d_vals.p, vals, n * 8, loc == VB_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, c->stream));
+            if (loc == VB_HOST) s->st.h2d_bytes += n * 8;
+        }
+    }
+    MapOut &m = s->maps[map_id];
+    if (m.present) {                               // stage resubmission: the new rows replace the old ones
+        s->st.rows_in -= m.n_rows;
+        free_str_map(s, map_id);
+    }
+    t->ids[map_id] = (u32 *)ids.release();
+    if (n && s->agg != VB_AGG_COUNT) {
+        t->vals_owned[map_id] = loc != VB_DEVICE_BORROWED;
+        t->vals[map_id] = loc == VB_DEVICE_BORROWED ? (const u64 *)vals : (const u64 *)d_vals.release();
+    }
+    m.present = true;
+    m.n_rows = n;
+    s->st.rows_in += n;
+    CU(cudaStreamSynchronize(c->stream));          // the caller's key column is free again when the call returns
+    TRY(call.done("map"));
+    return VB_OK;
+}
+
+template <int OPK, int TX>
+static int launch_str_reduce(vb_shuf *s, const u32 *ids, const u64 *vals, u64 n, const u32 *dense, u64 *acc)
+{
+    vb_ctx *c = s->ctx;
+    auto kern = str_reduce_kernel<OPK, TX>;
+    const int occ = occupancy(c, kern, 256, 0);
+    const u64 blocks = std::min<u64>((n + 255) / 256, (u64)c->sm_count * occ);
+    KLaunch kl(s, K_HASH_AGG, n);
+    kern<<<(unsigned)blocks, 256, 0, c->stream>>>(ids, vals, n, dense, acc);
+    return kl.done("str_reduce_kernel");
+}
+
+static int str_reduce_rows(vb_shuf *s, const u32 *ids, const u64 *vals, u64 n, const u32 *dense, u64 *acc)
+{
+    const int tx = val_tx(s);
+    switch (map_opk(s)) {
+    case OPK_ADD_U64: return launch_str_reduce<OPK_ADD_U64, TX_NONE>(s, ids, vals, n, dense, acc);
+    case OPK_ADD_F64: return launch_str_reduce<OPK_ADD_F64, TX_NONE>(s, ids, vals, n, dense, acc);
+    case OPK_COUNT: return launch_str_reduce<OPK_COUNT, TX_NONE>(s, ids, vals, n, dense, acc);
+    case OPK_MIN_U64:
+        if (tx == TX_I64) return launch_str_reduce<OPK_MIN_U64, TX_I64>(s, ids, vals, n, dense, acc);
+        if (tx == TX_F64) return launch_str_reduce<OPK_MIN_U64, TX_F64>(s, ids, vals, n, dense, acc);
+        return launch_str_reduce<OPK_MIN_U64, TX_NONE>(s, ids, vals, n, dense, acc);
+    case OPK_MAX_U64:
+        if (tx == TX_I64) return launch_str_reduce<OPK_MAX_U64, TX_I64>(s, ids, vals, n, dense, acc);
+        if (tx == TX_F64) return launch_str_reduce<OPK_MAX_U64, TX_F64>(s, ids, vals, n, dense, acc);
+        return launch_str_reduce<OPK_MAX_U64, TX_NONE>(s, ids, vals, n, dense, acc);
+    }
+    return set_err(VB_ERR_UNSUPPORTED, "string keys: op %d", s->agg);
+}
+
+// Seal of a string-key shuffle (world == 1, every map present):
+//   1. mark the entries the rows of the present maps reference (a key only a replaced submission had is dropped);
+//   2. split the live entries by h % n_reduce into partition-major dense ids, and lay their bytes out in that order;
+//   3. reduce ops: one RED per (warp, distinct id) into acc[dense id];  GROUP: the maps' (id, value) rows in map-id
+//      order, stably sorted by dense id, then the CSR (seal_group's steps 4-7).
+static int seal_str(vb_shuf *s)
+{
+    vb_ctx *c = s->ctx;
+    StrState *t = s->str;
+    const u32 R = s->n_reduce;
+    s->bucket_off.assign((size_t)R + 1, 0);
+    s->val_off.assign((size_t)R + 1, 0);
+    t->kb_off.assign((size_t)R + 1, 0);
+    u64 n = 0;
+    for (auto &m : s->maps) if (m.present) n += m.n_rows;
+    const u32 ne = t->n_e;
+    auto grid = [&](u64 x) { return (unsigned)std::min<u64>((x + 255) / 256, (u64)c->sm_count * 8); };
+    if (n && ne) {
+        // 1. live entries
+        DevBuf live(c), part(c), cnt(c), cur(c), dbase(c), dense(c), eod(c), klen(c), koff(c), kbytes(c);
+        TRY(live.alloc((u64)ne * 4));
+        CU(cudaMemsetAsync(live.p, 0, (u64)ne * 4, c->stream));
+        for (u32 m = 0; m < s->n_map; ++m) {
+            if (!s->maps[m].n_rows) continue;
+            KLaunch kl(s, K_MISC, s->maps[m].n_rows);
+            str_mark_live_kernel<<<grid(s->maps[m].n_rows), 256, 0, c->stream>>>(t->ids[m], s->maps[m].n_rows, live.as<u32>());
+            TRY(kl.done("str_mark_live_kernel"));
+        }
+        // 2. partitions, dense ids, key bytes
+        TRY(part.alloc((u64)ne * 4));
+        TRY(cnt.alloc((u64)R * 4));
+        TRY(cur.alloc((u64)R * 4));
+        CU(cudaMemsetAsync(cnt.p, 0, (u64)R * 4, c->stream));
+        CU(cudaMemsetAsync(cur.p, 0, (u64)R * 4, c->stream));
+        {
+            KLaunch kl(s, K_MISC, ne);
+            str_part_count_kernel<<<(ne + 255) / 256, 256, 0, c->stream>>>(t->d.e_hash, live.as<u32>(), ne, make_fastmod(R), part.as<u32>(), cnt.as<u32>());
+            TRY(kl.done("str_part_count_kernel"));
+        }
+        std::vector<u32> hc(R);
+        CU(cudaMemcpyAsync(hc.data(), cnt.p, (size_t)R * 4, cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaStreamSynchronize(c->stream));
+        for (u32 r = 0; r < R; ++r) s->bucket_off[r + 1] = s->bucket_off[r] + hc[r];
+        const u64 D = s->bucket_off[R];
+        if (D >= (1ull << 31)) return set_err(VB_ERR_TOO_LARGE, "%llu distinct string keys (fewer than 2^31 are supported)", (unsigned long long)D);
+        TRY(dbase.alloc(((u64)R + 1) * 8));
+        CU(cudaMemcpyAsync(dbase.p, s->bucket_off.data(), ((size_t)R + 1) * 8, cudaMemcpyHostToDevice, c->stream));
+        TRY(dense.alloc((u64)ne * 4));
+        TRY(eod.alloc(D * 4));
+        TRY(klen.alloc(D * 8));
+        TRY(koff.alloc((D + 1) * 8));
+        {
+            KLaunch kl(s, K_MISC, ne);
+            str_dense_kernel<<<(ne + 255) / 256, 256, 0, c->stream>>>(live.as<u32>(), part.as<u32>(), ne, dbase.as<u64>(), cur.as<u32>(), t->d.e_len,
+                                                                      dense.as<u32>(), eod.as<u32>(), klen.as<u64>());
+            TRY(kl.done("str_dense_kernel"));
+        }
+        TRY(exclusive_scan_u64(s, klen.as<u64>(), koff.as<u64>(), D, koff.as<u64>() + D));
+        {
+            DevBuf out(c);
+            TRY(out.alloc(((size_t)R + 1) * 8));
+            KLaunch kl(s, K_MISC);
+            gather_u64_kernel<<<(R + 1 + 255) / 256, 256, 0, c->stream>>>(koff.as<u64>(), dbase.as<u64>(), R + 1, out.as<u64>());
+            TRY(kl.done("gather_u64_kernel"));
+            CU(cudaMemcpyAsync(t->kb_off.data(), out.p, ((size_t)R + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
+            CU(cudaStreamSynchronize(c->stream));
+        }
+        TRY(kbytes.alloc(t->kb_off[R]));
+        {
+            KLaunch kl(s, K_MISC, D);
+            str_gather_bytes_kernel<<<(unsigned)((D * 32 + 255) / 256), 256, 0, c->stream>>>(eod.as<u32>(), (u32)D, t->d.e_off, koff.as<u64>(), t->d.arena,
+                                                                                            kbytes.as<unsigned char>());
+            TRY(kl.done("str_gather_bytes_kernel"));
+        }
+        // 3. values
+        if (is_reduce_op(s->agg)) {
+            DevBuf acc(c);
+            TRY(acc.alloc(D * 8));
+            {
+                KLaunch kl(s, K_MISC);
+                str_fill_kernel<<<grid(D), 256, 0, c->stream>>>(acc.as<u64>(), D, op_identity(map_opk(s)));
+                TRY(kl.done("str_fill_kernel"));
+            }
+            for (u32 m = 0; m < s->n_map; ++m)
+                if (s->maps[m].n_rows) TRY(str_reduce_rows(s, t->ids[m], t->vals[m], s->maps[m].n_rows, dense.as<u32>(), acc.as<u64>()));
+            const int tx = val_tx(s);
+            if (tx != TX_NONE) {
+                KLaunch kl(s, K_MISC);
+                tx_inv_kernel<<<(unsigned)((D + 255) / 256), 256, 0, c->stream>>>(acc.as<u64>(), D, tx);
+                TRY(kl.done("tx_inv_kernel"));
+            }
+            s->res_comb = (u64 *)acc.release();
+            s->st.rows_out = D;
+        } else {
+            DevBuf cids(c), cvals(c), offs(c);
+            TRY(cids.alloc(n * 4));
+            TRY(cvals.alloc(n * 8));
+            u64 at = 0;
+            for (u32 m = 0; m < s->n_map; ++m) {
+                const u64 k = s->maps[m].n_rows;
+                if (!k) continue;
+                CU(cudaMemcpyAsync(cids.as<u32>() + at, t->ids[m], k * 4, cudaMemcpyDeviceToDevice, c->stream));
+                CU(cudaMemcpyAsync(cvals.as<u64>() + at, t->vals[m], k * 8, cudaMemcpyDeviceToDevice, c->stream));
+                at += k;
+            }
+            TRY(offs.alloc((D + 1) * 8));
+            CU(cudaMemsetAsync(offs.p, 0xFF, (D + 1) * 8, c->stream));
+            u32 *sorted_ids = nullptr;
+            u64 *sorted_vals = nullptr;
+            bool csr_done = false;
+            TRY(sort_id_pairs(s, cids.as<u32>(), Loader{LD_KEY32_VAL_SOA, nullptr, cvals.as<u64>(), 0}, n, ceil_log2_u64(std::max<u64>(D, 2)), &sorted_ids,
+                              &sorted_vals, dense.as<u32>(), offs.as<u64>(), &csr_done));
+            DevBuf sid_guard(c), sval_guard(c);
+            if (sorted_ids != cids.as<u32>()) sid_guard.p = sorted_ids;
+            sval_guard.p = sorted_vals;
+            if (csr_done) {
+                CU(cudaMemcpyAsync(offs.as<u64>() + D, &n, 8, cudaMemcpyHostToDevice, c->stream));
+            } else {
+                KLaunch kl(s, K_MISC);
+                csr_bounds_kernel<<<grid(n), 256, 0, c->stream>>>(sorted_ids, n, offs.as<u64>(), D);
+                TRY(kl.done("csr_bounds_kernel"));
+            }
+            {
+                DevBuf out(c);
+                TRY(out.alloc(((size_t)R + 1) * 8));
+                KLaunch kl(s, K_MISC);
+                gather_u64_kernel<<<(R + 1 + 255) / 256, 256, 0, c->stream>>>(offs.as<u64>(), dbase.as<u64>(), R + 1, out.as<u64>());
+                TRY(kl.done("gather_u64_kernel"));
+                CU(cudaMemcpyAsync(s->val_off.data(), out.p, ((size_t)R + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
+                CU(cudaStreamSynchronize(c->stream));
+            }
+            s->n_vals = n;
+            s->res_offs = (u64 *)offs.release();
+            s->res_vals = (u64 *)sval_guard.release();
+            s->st.rows_out = n;
+        }
+        s->n_keys = D;
+        t->key_off = (u64 *)koff.release();
+        t->key_bytes = (unsigned char *)kbytes.release();
+        CU(cudaStreamSynchronize(c->stream));
+    }
+    for (u32 m = 0; m < s->n_map; ++m) free_str_map(s, m);
+    free_str_dict(s);
+    return VB_OK;
+}
+
+extern "C" int32_t vb_shuffle_reduce_str_size(vb_shuf *s, uint32_t r, uint64_t *n_keys, uint64_t *n_key_bytes, uint64_t *n_vals)
+{
+    if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
+    if (!s->str) return set_err(VB_ERR_INVALID, "vb_shuffle_reduce_str_size needs a shuffle from vb_shuffle_create_str");
+    if (r >= s->n_reduce) return set_err(VB_ERR_INVALID, "reduce_id %u >= n_reduce %u", r, s->n_reduce);
+    TRY(wait_sealed(s));
+    if (n_keys) *n_keys = s->bucket_off[r + 1] - s->bucket_off[r];
+    if (n_key_bytes) *n_key_bytes = s->str->kb_off[r + 1] - s->str->kb_off[r];
+    if (n_vals) *n_vals = is_group_op(s->agg) ? s->val_off[r + 1] - s->val_off[r] : 0;
+    return VB_OK;
+}
+
+// out[0 .. nk] = src[0 .. nk] - base (partition-relative CSR offsets starting at 0)
+static int copy_out_rebased(vb_shuf *s, u64 *dst, const u64 *src, u64 nk, u64 base, int dst_loc)
+{
+    vb_ctx *c = s->ctx;
+    if (!dst) return VB_OK;
+    if (nk == 0) {
+        static const u64 zero = 0;
+        CU(cudaMemcpyAsync(dst, &zero, 8, dst_loc == VB_HOST ? cudaMemcpyHostToHost : cudaMemcpyHostToDevice, c->stream));
+        return VB_OK;
+    }
+    DevBuf tmp(c);
+    TRY(tmp.alloc((nk + 1) * 8));
+    KLaunch kl(s, K_MISC);
+    rebase_kernel<<<(unsigned)((nk + 1 + 255) / 256), 256, 0, c->stream>>>(src, nk + 1, base, tmp.as<u64>());
+    TRY(kl.done("rebase_kernel"));
+    return copy_out(s, dst, tmp.p, (nk + 1) * 8, dst_loc);
+}
+
+extern "C" int32_t vb_shuffle_reduce_str(vb_shuf *s, uint32_t r, uint64_t *out_key_offsets, void *out_key_bytes, void *out_combined,
+                                         uint64_t *out_offsets, void *out_vals, int32_t dst_loc)
+{
+    if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
+    if (!s->str) return set_err(VB_ERR_INVALID, "vb_shuffle_reduce_str needs a shuffle from vb_shuffle_create_str");
+    if (r >= s->n_reduce) return set_err(VB_ERR_INVALID, "reduce_id %u >= n_reduce %u", r, s->n_reduce);
+    if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
+    TRY(wait_sealed(s));
+    vb_ctx *c = s->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    StrState *t = s->str;
+    const u64 b0 = s->bucket_off[r], nk = s->bucket_off[r + 1] - b0;
+    const u64 kb0 = t->kb_off[r], nkb = t->kb_off[r + 1] - kb0;
+    TRY(copy_out_rebased(s, out_key_offsets, t->key_off ? t->key_off + b0 : nullptr, nk, kb0, dst_loc));
+    TRY(copy_out(s, out_key_bytes, t->key_bytes ? t->key_bytes + kb0 : nullptr, nkb, dst_loc));
+    if (is_group_op(s->agg)) {
+        const u64 v0 = s->val_off[r], nv = s->val_off[r + 1] - v0;
+        TRY(copy_out_rebased(s, out_offsets, s->res_offs ? s->res_offs + b0 : nullptr, nk, v0, dst_loc));
+        TRY(copy_out(s, out_vals, s->res_vals ? s->res_vals + v0 : nullptr, nv * 8, dst_loc));
+    } else {
+        TRY(copy_out(s, out_combined, s->res_comb ? s->res_comb + b0 : nullptr, nk * 8, dst_loc));
+    }
+    CU(cudaStreamSynchronize(c->stream));
+    return VB_OK;
+}
+
+extern "C" uint64_t vb_hash_str(const void *bytes, uint64_t len) { return metro64_1_str((const unsigned char *)bytes, len); }
+
+extern "C" uint32_t vb_get_partition_str(const void *bytes, uint64_t len, uint32_t n_reduce)
+{
+    if (n_reduce == 0) return 0;
+    return (uint32_t)(metro64_1_str((const unsigned char *)bytes, len) % (uint64_t)n_reduce);
+}
+
+// ---------------------------------------------------------------------------------------------
 // free / stats
 // ---------------------------------------------------------------------------------------------
 extern "C" int32_t vb_shuffle_free(vb_shuf *s)
@@ -3552,6 +4119,7 @@ extern "C" int32_t vb_shuffle_free(vb_shuf *s)
         for (auto &kv : s->join_plans) { dev_free(c, kv.second.pos); dev_free(c, kv.second.match); }
         for (auto &kv : s->cogroup_plans) free_cogroup_plan(c, kv.second);
         free_lazy_rows(s);
+        free_str(s);
         cudaStreamSynchronize(c->stream);
     }
     for (auto &kv : s->filtered) { vb_shuffle_free(kv.second.first); vb_shuffle_free(kv.second.second); }

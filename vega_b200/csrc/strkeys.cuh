@@ -1,0 +1,314 @@
+// strkeys.cuh — byte-string keys (Rust `String` / `&str`): the hash the reference's HashPartitioner gives them, the
+// per-shuffle dictionary of distinct keys, and the seal-side kernels of the string-key shuffle (engine.cu,
+// "string keys").
+//
+// A key is a byte run of a caller column (Arrow-style offsets + bytes).  `impl Hash for str` writes the bytes and then
+// one 0xFF byte; the buffering MetroHasher hashes that stream with MetroHash64_1 (seed 0) at finish.  The suffix is
+// never materialised: every word of the stream is assembled from aligned 8-byte loads of the key and the 0xFF byte.
+//
+// Dictionary: dense entries (hash, arena offset, length) indexed by a u32 entry id, an arena holding each distinct
+// key's bytes once, and an open-addressing index of 4-slot buckets (fingerprint, entry id).  Entries are the source of
+// truth; the index is rebuilt from them whenever it has to grow.
+#pragma once
+#include "kernels.cuh"
+
+namespace vb {
+
+// Bytes [pos, pos + n) of p (1 <= n <= 8) as a little-endian word.  On the device: one or two aligned 8-byte loads,
+// never one of an aligned word that holds none of the requested bytes (so never past the end of the allocation).
+// CG: read through L2 only (arena bytes another thread of the same kernel may have just published).
+template <bool CG>
+VB_HD u64 load_le(const unsigned char *p, u64 pos, u32 n)
+{
+#ifdef __CUDA_ARCH__
+    const uintptr_t a = (uintptr_t)(p + pos);
+    const u32 sh = (u32)(a & 7u);
+    const unsigned long long *w = (const unsigned long long *)(a - sh);
+    u64 v = (CG ? __ldcg(w) : __ldg(w)) >> (8 * sh);
+    if (sh + n > 8) v |= (u64)(CG ? __ldcg(w + 1) : __ldg(w + 1)) << (64 - 8 * sh);
+#else
+    u64 v = 0;
+    for (u32 i = 0; i < n; ++i) v |= (u64)p[pos + i] << (8 * i);
+#endif
+    return n < 8 ? v & ((1ull << (8 * n)) - 1) : v;
+}
+
+// Bytes [pos, pos + n) of the hashed stream `key[0..len) ‖ 0xFF` (pos + n <= len + 1).
+VB_HD u64 str_word(const unsigned char *p, u64 len, u64 pos, u32 n)
+{
+    const u32 take = pos >= len ? 0u : (u32)((len - pos) < n ? (len - pos) : n);
+    u64 v = take ? load_le<false>(p, pos, take) : 0ull;
+    if (take < n) v |= 0xFFull << (8 * take);
+    return v;
+}
+
+// MetroHash64_1(key ‖ 0xFF, seed 0): `str::hash` fed to the reference's MetroHasher (fasthash 0.4.0).
+VB_HD u64 metro64_1_str(const unsigned char *p, u64 len)
+{
+    const u64 k0 = 0xC83A91E1ull, k1 = 0x8648DBDBull, k2 = 0x7BDEC03Bull, k3 = 0x2F5870A5ull;
+    const u64 n = len + 1;
+    u64 h = (k2 * k0) + n;
+    u64 pos = 0;
+    if (n >= 32) {
+        u64 v0 = h, v1 = h, v2 = h, v3 = h;
+        do {
+            v0 += str_word(p, len, pos, 8) * k0;      v0 = rotr64(v0, 29) + v2;
+            v1 += str_word(p, len, pos + 8, 8) * k1;  v1 = rotr64(v1, 29) + v3;
+            v2 += str_word(p, len, pos + 16, 8) * k2; v2 = rotr64(v2, 29) + v0;
+            v3 += str_word(p, len, pos + 24, 8) * k3; v3 = rotr64(v3, 29) + v1;
+            pos += 32;
+        } while (pos + 32 <= n);
+        v2 ^= rotr64(((v0 + v3) * k0) + v1, 33) * k1;
+        v3 ^= rotr64(((v1 + v2) * k1) + v0, 33) * k0;
+        v0 ^= rotr64(((v0 + v2) * k0) + v3, 33) * k1;
+        v1 ^= rotr64(((v1 + v3) * k1) + v2, 33) * k0;
+        h += v0 ^ v1;
+    }
+    if (n - pos >= 16) {
+        u64 a = h + str_word(p, len, pos, 8) * k0;     a = rotr64(a, 33) * k1;
+        u64 b = h + str_word(p, len, pos + 8, 8) * k1; b = rotr64(b, 33) * k2;
+        a ^= rotr64(a * k0, 35) + b;
+        b ^= rotr64(b * k3, 35) + a;
+        h += b;
+        pos += 16;
+    }
+    if (n - pos >= 8) { h += str_word(p, len, pos, 8) * k3; h ^= rotr64(h, 33) * k1; pos += 8; }
+    if (n - pos >= 4) { h += str_word(p, len, pos, 4) * k3; h ^= rotr64(h, 15) * k1; pos += 4; }
+    if (n - pos >= 2) { h += str_word(p, len, pos, 2) * k3; h ^= rotr64(h, 13) * k1; pos += 2; }
+    if (n - pos >= 1) { h += str_word(p, len, pos, 1) * k3; h ^= rotr64(h, 25) * k1; }
+    h ^= rotr64(h, 33);
+    h *= k0;
+    h ^= rotr64(h, 33);
+    return h;
+}
+
+constexpr u32 STR_UNPUBLISHED = 0xFFFFFFFFu;   // index slot claimed, entry id not written yet (or slot empty)
+constexpr u32 STR_MAX_PROBE = 64;              // buckets probed before a call gives up and the index grows
+
+struct StrDict {
+    u64 *fp;                  // [cap] index fingerprints: 0 = empty slot
+    u32 *id;                  // [cap] entry id of the slot
+    u32 log_cap;              // cap = 1 << log_cap slots, 4 per 32-byte bucket of fingerprints
+    u64 fp_mask;              // bits of the hash kept in the fingerprint (all of them unless VEGA_B200_STR_FP_BITS)
+    u64 *e_hash;              // [entries] full 64-bit hash
+    u64 *e_off;               // [entries] offset of the key's bytes in the arena
+    u32 *e_len;               // [entries] key length in bytes
+    unsigned char *arena;     // each distinct key's bytes, once
+};
+
+struct StrCtl {
+    u32 abort;                     // the index is too full or a probe ran too long: the host grows it and reruns the call
+    u32 n_entries;                 // entries in use (persistent across calls)
+    unsigned long long n_arena;    // arena bytes in use (persistent across calls)
+};
+
+VB_HD u64 str_fp(u64 h, u64 mask)
+{
+    const u64 f = h & mask;
+    return f ? f : 1ull;           // 0 marks an empty slot
+}
+// The probe starts at the bucket of the FULL hash: a masked fingerprint shortens only the compare, not the spread.
+VB_HD u64 str_bucket(u64 h, u32 log_cap) { return log_cap > 2 ? (h >> (66 - log_cap)) : 0ull; }
+
+VB_D u32 ld_acquire_u32(const u32 *p)
+{
+    u32 r;
+    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(r) : "l"(p) : "memory");
+    return r;
+}
+VB_D void st_release_u32(u32 *p, u32 v) { asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
+
+VB_D bool str_equal(const unsigned char *key, const unsigned char *stored, u64 len)
+{
+    for (u64 pos = 0; pos < len; pos += 8) {
+        const u32 n = (len - pos) < 8 ? (u32)(len - pos) : 8u;
+        if (load_le<false>(key, pos, n) != load_le<true>(stored, pos, n)) return false;
+    }
+    return true;
+}
+
+// One thread per row: hash the key, find or create its dictionary entry, write the entry id.  Key i is
+// bytes[offs[i] - base .. offs[i + 1] - base).  Entries and arena are reserved by the host for the worst case of the
+// call, so only the index can overflow; that is decided BEFORE a slot is claimed (load or probe length), so a claimed
+// slot is always published and no thread waits on one forever.  An aborted call is rerun whole after the index grows:
+// rows already encoded find the same entries again.
+__global__ void __launch_bounds__(256) str_encode_kernel(const u64 *__restrict__ offs, const unsigned char *__restrict__ bytes, u64 base,
+                                                         u64 n, StrDict d, StrCtl *ctl, u32 max_entries, u32 *__restrict__ ids_out)
+{
+    const u64 nb = 1ull << (d.log_cap - 2);
+    const u32 max_probe = nb < STR_MAX_PROBE ? (u32)nb : STR_MAX_PROBE;
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+        if (ld_volatile_u32(&ctl->abort)) return;
+        const u64 o0 = offs[i], len = offs[i + 1] - o0;
+        const unsigned char *p = bytes + (o0 - base);
+        const u64 h = metro64_1_str(p, len);
+        const u64 f = str_fp(h, d.fp_mask);
+        u64 b = str_bucket(h, d.log_cap);
+        u32 found = STR_UNPUBLISHED;
+        for (u32 probe = 0; probe < max_probe && found == STR_UNPUBLISHED; ++probe, b = (b + 1) & (nb - 1)) {
+            for (u32 j = 0; j < BUCKET; ++j) {
+                const u64 slot = BUCKET * b + j;
+                u64 cur = __ldcg((const unsigned long long *)&d.fp[slot]);
+                if (cur == 0) {
+                    if (ld_volatile_u32(&ctl->n_entries) >= max_entries) { atomicExch(&ctl->abort, 1u); return; }
+                    cur = atomicCAS((unsigned long long *)&d.fp[slot], 0ull, (unsigned long long)f);
+                    if (cur == 0) {                          // claimed: create the entry, then publish its id
+                        const u32 e = atomicAdd(&ctl->n_entries, 1u);
+                        const u64 ao = atomicAdd(&ctl->n_arena, (unsigned long long)len);
+                        for (u64 k = 0; k < len; ++k) d.arena[ao + k] = p[k];
+                        d.e_hash[e] = h;
+                        d.e_off[e] = ao;
+                        d.e_len[e] = (u32)len;
+                        __threadfence();
+                        st_release_u32(&d.id[slot], e);
+                        found = e;
+                        break;
+                    }
+                }
+                if (cur == f) {                              // same fingerprint: equal only if the bytes are
+                    u32 e, ns = 32;
+                    while ((e = ld_acquire_u32(&d.id[slot])) == STR_UNPUBLISHED) {
+                        __nanosleep(ns);
+                        if (ns < 1024) ns *= 2;
+                    }
+                    if (__ldcg(&d.e_len[e]) == len && str_equal(p, d.arena + __ldcg((const unsigned long long *)&d.e_off[e]), len)) {
+                        found = e;
+                        break;
+                    }
+                }
+            }
+        }
+        if (found == STR_UNPUBLISHED) { atomicExch(&ctl->abort, 1u); return; }
+        ids_out[i] = found;
+    }
+}
+
+// Re-insert entries [0, n) into an empty index (all keys distinct: no compares).
+__global__ void str_index_rebuild_kernel(StrDict d, u32 n, StrCtl *ctl)
+{
+    const u64 nb = 1ull << (d.log_cap - 2);
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 e = (u64)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += stride) {
+        const u64 h = d.e_hash[e], f = str_fp(h, d.fp_mask);
+        u64 b = str_bucket(h, d.log_cap);
+        bool placed = false;
+        for (u64 probe = 0; probe < nb && !placed; ++probe, b = (b + 1) & (nb - 1))
+            for (u32 j = 0; j < BUCKET; ++j)
+                if (atomicCAS((unsigned long long *)&d.fp[BUCKET * b + j], 0ull, (unsigned long long)f) == 0ull) {
+                    d.id[BUCKET * b + j] = (u32)e;
+                    placed = true;
+                    break;
+                }
+        if (!placed) atomicExch(&ctl->abort, 1u);
+    }
+}
+
+// Key offsets of a device-resident call: flags bit 0 = decreasing or beyond n_bytes, bit 1 = a key of 2^32 bytes or more.
+__global__ void str_check_offsets_kernel(const u64 *__restrict__ offs, u64 n, u64 n_bytes, u32 *flags)
+{
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    u32 f = 0;
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i <= n; i += stride) {
+        const u64 o = offs[i];
+        if (o > n_bytes) f |= 1u;
+        if (i < n) {
+            const u64 nx = offs[i + 1];
+            if (nx < o) f |= 1u;
+            else if (nx - o >= (1ull << 32)) f |= 2u;
+        }
+    }
+    if (f) atomicOr(flags, f);
+}
+
+// ---- seal ------------------------------------------------------------------------------------------------------
+__global__ void str_mark_live_kernel(const u32 *__restrict__ ids, u64 n, u32 *__restrict__ live)
+{
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) live[ids[i]] = 1u;
+}
+
+// Partition of every live entry (h % n_reduce) and the per-partition key counts.
+__global__ void str_part_count_kernel(const u64 *__restrict__ e_hash, const u32 *__restrict__ live, u32 n, FastMod fm,
+                                      u32 *__restrict__ part_of, u32 *__restrict__ cnt)
+{
+    const u32 e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n || !live[e]) return;
+    const u32 p = fastmod(e_hash[e], fm);
+    part_of[e] = p;
+    atomicAdd(&cnt[p], 1u);
+}
+
+// Partition-major dense ids (order inside a partition unspecified) and each dense key's length.
+__global__ void str_dense_kernel(const u32 *__restrict__ live, const u32 *__restrict__ part_of, u32 n, const u64 *__restrict__ part_base,
+                                 u32 *__restrict__ cursor, const u32 *__restrict__ e_len, u32 *__restrict__ dense_of_entry,
+                                 u32 *__restrict__ entry_of_dense, u64 *__restrict__ klen)
+{
+    const u32 e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n) return;
+    if (!live[e]) { dense_of_entry[e] = STR_UNPUBLISHED; return; }
+    const u32 p = part_of[e];
+    const u32 dn = (u32)part_base[p] + atomicAdd(&cursor[p], 1u);
+    dense_of_entry[e] = dn;
+    entry_of_dense[dn] = e;
+    klen[dn] = e_len[e];
+}
+
+// Key bytes in dense order: one warp per key.
+__global__ void str_gather_bytes_kernel(const u32 *__restrict__ entry_of_dense, u32 n, const u64 *__restrict__ e_off,
+                                        const u64 *__restrict__ key_off, const unsigned char *__restrict__ arena, unsigned char *__restrict__ out)
+{
+    const u64 w = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (w >= n) return;
+    const u64 src = e_off[entry_of_dense[w]], dst = key_off[w], len = key_off[w + 1] - dst;
+    for (u64 k = lane_id(); k < len; k += 32) out[dst + k] = arena[src + k];
+}
+
+__global__ void str_fill_kernel(u64 *__restrict__ a, u64 n, u64 v)
+{
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) a[i] = v;
+}
+
+// One RED per distinct id of each warp into acc[dense id]: lanes of a warp that carry the same id (match-any) are
+// combined first, so a frequent key costs one RED per warp, not per row.  OPK_COUNT counts rows (vals unused);
+// TX / NaN handling as hash_agg_kernel's: values enter MIN/MAX order-transformed, an f64 NaN becomes the identity.
+template <int OPK, int TX>
+__global__ void __launch_bounds__(256) str_reduce_kernel(const u32 *__restrict__ ids, const u64 *__restrict__ vals, u64 n,
+                                                         const u32 *__restrict__ dense_of_entry, u64 *__restrict__ acc)
+{
+    constexpr int RED = OPK == OPK_COUNT ? OPK_ADD_U64 : OPK;
+    constexpr bool NAN_IS_IDENTITY = (TX == TX_F64) && (OPK == OPK_MIN_U64 || OPK == OPK_MAX_U64);
+    const u32 lane = lane_id();
+    const u64 warp0 = ((u64)blockIdx.x * blockDim.x + threadIdx.x) & ~31ull;
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 w = warp0; w < n; w += stride) {
+        const u64 i = w + lane;
+        const bool ok = i < n;
+        u32 dn = STR_UNPUBLISHED;
+        u64 v = OPK == OPK_COUNT ? 1ull : 0ull;
+        if (ok) {
+            dn = dense_of_entry[ids[i]];
+            if (OPK != OPK_COUNT) {
+                v = vals[i];
+                if (NAN_IS_IDENTITY && (v & 0x7FFFFFFFFFFFFFFFull) > 0x7FF0000000000000ull) v = op_identity(OPK);
+                else v = tx_fwd(v, TX);
+            }
+        }
+        const u32 peers = __match_any_sync(0xFFFFFFFFu, dn);
+        const bool lead = (__ffs(peers) - 1) == (int)lane;
+        if (!__all_sync(0xFFFFFFFFu, peers == (1u << lane))) {       // some id repeats in this warp: fold into its leader
+            for (u32 j = 0; j < 32; ++j) {
+                const u64 x = __shfl_sync(0xFFFFFFFFu, v, j);
+                if (!lead || j == lane || !((peers >> j) & 1u)) continue;
+                if (RED == OPK_ADD_U64) v += x;
+                else if (RED == OPK_ADD_F64) v = (u64)__double_as_longlong(__longlong_as_double((long long)v) + __longlong_as_double((long long)x));
+                else if (RED == OPK_MIN_U64) v = x < v ? x : v;
+                else v = x > v ? x : v;
+            }
+        }
+        if (ok && lead) op_red<RED>(&acc[dn], v);
+    }
+}
+
+}  // namespace vb

@@ -6,7 +6,9 @@ Same names and argument meaning as the reference for the calls on the path
 `count_by_value / distinct / collect`), so the parity tests read like tests/test_pair_rdd.rs.
 Differences forced by the boundary (SURVEY.md F4): rows are 64-bit POD (K,V) arrays
 (numpy on the host or torch CUDA tensors), and `reduce_by_key` takes a *named* op
-("sum" | "min" | "max") because a closure cannot cross into CUDA.
+("sum" | "min" | "max") because a closure cannot cross into CUDA.  Keys may also be Rust `String`s: a
+sequence of Python `str` or a `StrKeys` column (offsets + UTF-8 bytes), for reduce_by_key / count_by_key /
+group_by_key / partition_by_key / count_by_value / distinct; they are placed as the reference places `String` keys.
 
 All compute happens in libvega_b200.so; this module slices the input exactly like
 ParallelCollection::slice, drives map tasks → seal → reduce tasks like the scheduler does
@@ -141,7 +143,15 @@ class Context:
 
     def parallelize(self, data, num_slices, values=None):
         """`sc.parallelize(vec, num_slices)`.  data: 1-D keys (→ Rdd), (n,2) rows or
-        (keys, values) (→ PairRdd).  values may also be a tuple of up to 4 value columns (combine_by_key)."""
+        (keys, values) (→ PairRdd).  values may also be a tuple of up to 4 value columns (combine_by_key).
+        String keys (a sequence of str, a numpy str array or a StrKeys column) give a StrRdd / StrPairRdd."""
+        if _is_str_keys(data):
+            keys = _StrCol(data)
+            if values is None:
+                return StrRdd(self, keys, num_slices)
+            return StrPairRdd(self, keys, _Col(values, role="value"), num_slices)
+        if values is None and isinstance(data, tuple) and len(data) == 2 and _is_str_keys(data[0]):
+            return StrPairRdd(self, _StrCol(data[0]), _Col(data[1], role="value"), num_slices)
         if isinstance(values, tuple):                 # a list stays one value column, as before
             if not 1 <= len(values) <= L.VB_MAX_VAL_COLS:
                 raise ValueError(f"{len(values)} value columns: 1 to {L.VB_MAX_VAL_COLS} are supported")
@@ -377,7 +387,8 @@ class Grouped:
 
     def to_list(self):
         o = self.offsets
-        return [(self.keys[i].item(), self.vals[int(o[i]):int(o[i + 1])]) for i in range(len(self.keys))]
+        item = lambda k: k.item() if isinstance(k, np.generic) else k      # numpy scalar keys, or str keys
+        return [(item(self.keys[i]), self.vals[int(o[i]):int(o[i + 1])]) for i in range(len(self.keys))]
 
     def to_dict(self):
         return {k: v for k, v in self.to_list()}
@@ -769,3 +780,255 @@ class _Distinct:
 
     def collect(self):
         return self.sh.collect()[0]
+
+
+# ---- string keys ------------------------------------------------------------------------------------------------
+class StrKeys:
+    """A column of byte-string keys, Arrow-style: key i is data[offsets[i]:offsets[i + 1]].  offsets has n + 1 64-bit
+    integers and need not start at 0 (a slice of a larger column works as is); data holds the keys' UTF-8 bytes.
+    Both are numpy arrays (data may also be `bytes`), or both torch CUDA tensors (int64 / uint64 offsets, uint8 data)."""
+
+    def __init__(self, offsets, data):
+        if _is_torch(offsets) or _is_torch(data):
+            import torch
+            if not (_is_torch(offsets) and _is_torch(data)) or not (offsets.is_cuda and data.is_cuda):
+                raise TypeError("StrKeys: offsets and data must both be CUDA tensors, or both host arrays")
+            if offsets.dtype not in (torch.int64, getattr(torch, "uint64", torch.int64)) or data.dtype != torch.uint8:
+                raise TypeError("StrKeys: int64 / uint64 offsets and uint8 data expected")
+            offsets, data = offsets.contiguous(), data.contiguous()
+        else:
+            if isinstance(data, (bytes, bytearray)):
+                data = np.frombuffer(bytes(data), dtype=np.uint8)
+            offsets, data = np.asarray(offsets), np.asarray(data)
+            if offsets.dtype.kind not in "iu" or data.dtype != np.uint8:
+                raise TypeError("StrKeys: integer offsets and uint8 data expected")
+            offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
+            data = np.ascontiguousarray(data)
+        if len(offsets.shape) != 1 or len(data.shape) != 1 or offsets.shape[0] < 1:
+            raise ValueError("StrKeys: 1-D offsets of n + 1 entries and 1-D data expected")
+        self.offsets, self.data = offsets, data
+
+    @staticmethod
+    def from_strs(strs):
+        """Encode Python strs as UTF-8 into (offsets, bytes) on the host."""
+        enc = [x.encode("utf-8") for x in strs]
+        offsets = np.zeros(len(enc) + 1, dtype=np.uint64)
+        np.cumsum(np.fromiter((len(b) for b in enc), dtype=np.uint64, count=len(enc)), out=offsets[1:])
+        return StrKeys(offsets, np.frombuffer(b"".join(enc), dtype=np.uint8))
+
+    def __len__(self):
+        return self.offsets.shape[0] - 1
+
+    def to_strs(self):
+        """The keys as Python strs (bytes that are not UTF-8 are kept as surrogate escapes)."""
+        return _decode_keys(np.asarray(self.offsets.cpu() if _is_torch(self.offsets) else self.offsets, dtype=np.uint64),
+                            self.data.cpu().numpy() if _is_torch(self.data) else self.data)
+
+
+def _is_str_keys(x):
+    """True for a StrKeys column or a non-empty sequence / numpy array of str; a sequence of bytes is refused: Rust
+    hashes a Vec<u8> with a length prefix, not like a String."""
+    if isinstance(x, StrKeys):
+        return True
+    if isinstance(x, np.ndarray):
+        if x.dtype.kind == "S":
+            raise TypeError("bytes keys: a Rust Vec<u8> hashes with a length prefix, unlike a String; pass str keys")
+        if x.dtype.kind == "U":
+            return True
+        if x.dtype.kind != "O" or x.size == 0:
+            return False
+        first = x.flat[0]
+    elif isinstance(x, (list, tuple)) and len(x) > 0:
+        first = x[0]
+    else:
+        return False
+    if isinstance(first, (bytes, bytearray)):
+        raise TypeError("bytes keys: a Rust Vec<u8> hashes with a length prefix, unlike a String; pass str keys")
+    if not isinstance(first, str):
+        return False
+    if not all(isinstance(k, str) for k in (x.flat if isinstance(x, np.ndarray) else x)):
+        raise TypeError("a key column mixes str and other types")
+    return True
+
+
+def _decode_keys(offsets, data):
+    """Key bytes → numpy object array of Python str (NUL bytes survive, unlike in a numpy 'U' array)."""
+    raw = data.tobytes()
+    o = offsets.astype(np.int64).tolist()
+    out = np.empty(len(o) - 1, dtype=object)
+    out[:] = [raw[o[i]:o[i + 1]].decode("utf-8", "surrogateescape") for i in range(len(o) - 1)]
+    return out
+
+
+class _StrCol:
+    """A string key column at the C ABI: offsets / bytes pointers, their location and the row count."""
+
+    def __init__(self, x):
+        k = x if isinstance(x, StrKeys) else StrKeys.from_strs(x.tolist() if isinstance(x, np.ndarray) else x)
+        if _is_torch(k.offsets):
+            import torch
+            torch.cuda.current_stream(k.offsets.device).synchronize()
+            self.loc = L.VB_DEVICE_BORROWED
+            self.offs_ptr, self.data_ptr = k.offsets.data_ptr(), k.data.data_ptr()
+            self.n_bytes = k.data.shape[0]
+        else:
+            self.loc = L.VB_HOST
+            self.offs_ptr, self.data_ptr = k.offsets.ctypes.data, k.data.ctypes.data
+            self.n_bytes = k.data.shape[0]
+        self.n = len(k)
+        self.owner = k
+        self.rows = False
+        self.key_width = 8
+        self.code = None
+
+
+class StrShuffle(Shuffle):
+    """One string-key shuffle (vb_shuffle_create_str).  seal / stats / free as for Shuffle."""
+
+    def __init__(self, sc, n_map, n_reduce, vcode, agg, hint=0):
+        self.sc, self._lib = sc, sc._lib
+        self.n_map, self.n_reduce, self.agg, self.vcode, self.kcode = n_map, n_reduce, agg, vcode, None
+        self.has_payload = True
+        self._keepalive = []
+        h = ctypes.c_void_p()
+        L.check(self._lib.vb_shuffle_create_str(sc._h, sc.new_shuffle_id(), n_map, n_reduce, vcode, agg, ctypes.byref(h)))
+        self._h = h
+        sc._shuffles.add(self)
+        if hint:
+            L.check(self._lib.vb_shuffle_set_hint(h, hint))
+
+    def map(self, map_id, keys, vals, start, stop):
+        """Rows [start, stop) of the string key column (and of the values) as map partition map_id."""
+        if vals is not None and vals.loc != keys.loc:
+            raise ValueError("keys and values must live in the same memory space")
+        if keys.loc == L.VB_DEVICE_BORROWED:
+            self._keepalive.append((keys.owner, vals.owner if vals is not None else None))
+        offs = ctypes.c_void_p(keys.offs_ptr + 8 * start)
+        data = ctypes.c_void_p(keys.data_ptr) if keys.n_bytes else None
+        L.check(self._lib.vb_shuffle_map_str(self._h, map_id, offs, data, keys.n_bytes,
+                                             vals.at(start) if vals is not None else None, stop - start, keys.loc))
+
+    def reduce_size(self, r):
+        nk, nb, nv = ctypes.c_uint64(), ctypes.c_uint64(), ctypes.c_uint64()
+        L.check(self._lib.vb_shuffle_reduce_str_size(self._h, r, ctypes.byref(nk), ctypes.byref(nb), ctypes.byref(nv)))
+        return nk.value, nb.value, nv.value
+
+    def reduce_raw(self, r):
+        """Partition r on the host: (key offsets, key bytes, combined) or (key offsets, key bytes, offsets, values)."""
+        nk, nb, nv = self.reduce_size(r)
+        ko, kb = np.empty(nk + 1, dtype=np.uint64), np.empty(nb, dtype=np.uint8)
+        p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
+        if self.agg == L.VB_AGG_GROUP:
+            offs, vals = np.empty(nk + 1, dtype=np.uint64), np.empty(nv, dtype=_NP_OF[self.vcode])
+            L.check(self._lib.vb_shuffle_reduce_str(self._h, r, p(ko), p(kb), None, p(offs), p(vals), L.VB_HOST))
+            return ko, kb, offs, vals
+        comb = np.empty(nk, dtype=np.uint64 if self.agg == L.VB_AGG_COUNT else _NP_OF[self.vcode])
+        L.check(self._lib.vb_shuffle_reduce_str(self._h, r, p(ko), p(kb), p(comb), None, None, L.VB_HOST))
+        return ko, kb, comb
+
+    def reduce(self, r):
+        """ShuffledRdd::compute(split r): keys as a numpy object array of str, then the combined values, or the CSR
+        offsets and values for GROUP."""
+        out = self.reduce_raw(r)
+        return (_decode_keys(out[0], out[1]),) + out[2:]
+
+    def reduce_device(self, r, out_key_offsets=None, out_key_bytes=None, out_comb=None, out_offs=None, out_vals=None):
+        """Partition r into caller-provided torch CUDA tensors (any may be None; sizes from reduce_size)."""
+        _sync_torch(out_key_offsets, out_key_bytes, out_comb, out_offs, out_vals)
+        p = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None
+        L.check(self._lib.vb_shuffle_reduce_str(self._h, r, p(out_key_offsets), p(out_key_bytes), p(out_comb), p(out_offs),
+                                                p(out_vals), L.VB_DEVICE))
+
+
+class StrShuffledRdd(ShuffledRdd):
+    """ShuffledRdd over string keys: collect() gives (keys, combined) or a Grouped whose keys are Python strs."""
+
+    def __init__(self, parent, agg_name, num_splits, hint=0):
+        if num_splits < 1:
+            raise ValueError("num_splits must be >= 1")
+        self.parent, self.agg_name, self.num_slices, self.hint = parent, agg_name, num_splits, hint
+        self.sc = parent.sc
+        self._sh = None
+
+    def _run(self):
+        if self._sh is not None:
+            return self._sh
+        p = self.parent
+        starts = slice_starts(p.n, p.num_slices)
+        vcode = p.vals.code if p.vals is not None else L.VB_U64
+        sh = StrShuffle(self.sc, len(starts) - 1, self.num_slices, vcode, _AGG[self.agg_name], hint=self.hint)
+        for m in range(len(starts) - 1):
+            sh.map(m, p.keys, p.vals, int(starts[m]), int(starts[m + 1]))
+        sh.seal()
+        self._sh = sh
+        return sh
+
+    def compute_device(self, split, **out):
+        """compute(split) into caller-provided torch CUDA tensors (see StrShuffle.reduce_device)."""
+        self._run().reduce_device(split, **out)
+
+
+def _no_str(what):
+    def f(self, *a, **k):
+        raise TypeError(f"{what} is not supported for string keys yet (reduce_by_key, count_by_key, group_by_key, "
+                        "partition_by_key, count_by_value and distinct are)")
+    return f
+
+
+class StrPairRdd(PairRdd):
+    """PairRdd<String, V>: the shuffle ops string keys support; the others raise TypeError before any device work."""
+
+    def __init__(self, sc, keys, vals, num_slices):
+        if vals is None and keys.n:
+            raise ValueError("a PairRdd needs values")
+        super().__init__(sc, keys, vals, num_slices)
+
+    def group_by_key(self, num_splits):
+        return StrShuffledRdd(self, "group", num_splits)
+
+    def reduce_by_key(self, op, num_splits, hint=0):
+        if op not in ("sum", "min", "max"):
+            raise ValueError("reduce_by_key takes a named op: 'sum' | 'min' | 'max' (closures cannot cross the C ABI)")
+        return StrShuffledRdd(self, op, num_splits, hint)
+
+    def count_by_key(self, num_splits=None, hint=0):
+        return StrShuffledRdd(self, "count", num_splits or self.num_slices, hint)
+
+    def partition_by_key(self, num_splits):
+        return _Repartitioned(StrShuffledRdd(self, "group", num_splits))
+
+    combine_by_key = _no_str("combine_by_key")
+    join = _no_str("join")
+    left_outer_join = _no_str("left_outer_join")
+    right_outer_join = _no_str("right_outer_join")
+    full_outer_join = _no_str("full_outer_join")
+    cogroup = _no_str("cogroup")
+    sort_by_key = _no_str("sort_by_key")
+
+
+class StrRdd(Rdd):
+    """Rdd<String>: count_by_value and distinct; the other shuffle ops raise TypeError before any device work."""
+
+    def count_by_value(self):
+        n_splits = len(slice_starts(self.n, self.num_slices)) - 1
+        return StrShuffledRdd(_StrKeysOnly(self), "count", n_splits)
+
+    def distinct(self, num_partitions=None):
+        n_splits = num_partitions or (len(slice_starts(self.n, self.num_slices)) - 1)
+        return _Distinct(StrShuffledRdd(_StrKeysOnly(self), "count", n_splits))
+
+    distinct_with_num_partitions = distinct
+    sort = _no_str("sort")
+    intersection = _no_str("intersection")
+    intersection_with_num_partitions = intersection
+    subtract = _no_str("subtract")
+    subtract_with_num_partition = subtract
+    group_by = _no_str("group_by")
+    group_by_with_num_partitions = group_by
+
+
+class _StrKeysOnly:
+    """(x, ()) rows of a StrRdd: the COUNT shuffle reads no values."""
+
+    def __init__(self, rdd):
+        self.sc, self.keys, self.vals, self.num_slices, self.n = rdd.sc, rdd.keys, None, rdd.num_slices, rdd.n
