@@ -317,19 +317,30 @@ def test_rejected_calls(sc):
 
 
 # ---- 10. cogroup, inner join and full outer join of the same two shuffles ---------------------------
-@pytest.mark.parametrize("order", [("cogroup", "inner", "full", "cogroup"), ("full", "inner", "cogroup", "cogroup")])
+@pytest.mark.parametrize("order", [("cogroup", "inner", "full", "cogroup"), ("full", "inner", "cogroup", "cogroup"),
+                                   ("group", "cogroup", "inner", "full")])
 def test_cogroup_and_joins_on_the_same_shuffles(sc, order):
     """cogroup shares the FULL filtered pair with full_outer_join; each call must give what it gives alone, and the
-    originals must still group as they did."""
+    originals must still group as they did.  "group" reads every partition of both sides first (Shuffle.reduce), so
+    the later calls start from grouped sides: the cogroup must then equal the one of two lazy sides."""
     rng = np.random.default_rng(len(order[0]))
-    ka, va = rand_pairs(rng, 12_000, 1500)
-    kb, vb_ = rand_pairs(rng, 9000, 2500)
+    values = "full" if order[0] == "group" else "default"     # "full" keys include 0 and 2^64-1
+    ka, va = rand_pairs(rng, 12_000, 1500, values=values)
+    kb, vb_ = rand_pairs(rng, 9000, 2500, values=values)
     R = 4
     sa, sb = _pair(sc, ka, va, 3, kb, vb_, 2, R)
+    lazy = _pair(sc, ka, va, 3, kb, vb_, 2, R) if order[0] == "group" else None
     want_cg = ref_parts(ka, va, 3, kb, vb_, 2, R)
     for op in order:
-        if op == "cogroup":
-            assert_parts_equal(abi_parts(sc, sa, sb, R), want_cg)
+        if op == "group":
+            for s_ in (sa, sb):
+                for r in range(R):
+                    s_.reduce(r)
+        elif op == "cogroup":
+            got = abi_parts(sc, sa, sb, R)
+            assert_parts_equal(got, want_cg)
+            if lazy:
+                assert got == abi_parts(sc, *lazy, R)
         elif op == "inner":
             want = []
             for k, v, w in O.join(ka, va, 3, kb, vb_, 2, R):
@@ -351,41 +362,7 @@ def test_cogroup_and_joins_on_the_same_shuffles(sc, order):
     assert_parts_equal(abi_parts(sc, sa, sb, R), want_cg)
 
 
-# ---- 11. the eager (grouped) cogroup path gives the same lists ---------------------------------------
-_EAGER_SCRIPT = r"""
-import pickle, sys
-sys.path.insert(0, sys.argv[1])
-import vega_b200 as vb
-from tests.test_gpu_cogroup import gpu_parts, _eager_data
-ka, va, kb, vb_ = _eager_data()
-with vb.Context(0) as sc:
-    out = gpu_parts(sc.parallelize((ka, va), 3).cogroup(sc.parallelize((kb, vb_), 2), 5))
-pickle.dump(out, open(sys.argv[2], "wb"))
-"""
-
-
-def _eager_data():
-    rng = np.random.default_rng(9)
-    ka, va = rand_pairs(rng, 10_000, 1000, values="full")
-    kb, vb_ = rand_pairs(rng, 7000, 1600, values="full")
-    return ka, va, kb, vb_
-
-
-def test_eager_cogroup_gives_the_same_lists(sc):
-    ka, va, kb, vb_ = _eager_data()
-    with tempfile.TemporaryDirectory() as d:
-        out = os.path.join(d, "eager.pkl")
-        env = dict(os.environ, VEGA_B200_EAGER_COGROUP="1")
-        res = subprocess.run([sys.executable, "-c", _EAGER_SCRIPT, ROOT, out], env=env, cwd=ROOT, capture_output=True,
-                             text=True, timeout=600)
-        assert res.returncode == 0, res.stderr[-3000:]
-        eager = pickle.load(open(out, "rb"))
-    want = ref_parts(ka, va, 3, kb, vb_, 2, 5)
-    assert_parts_equal(eager, want)
-    assert_parts_equal(gpu_parts(sc.parallelize((ka, va), 3).cogroup(sc.parallelize((kb, vb_), 2), 5)), want)
-
-
-# ---- 12. two ranks: only the owned partitions have keys ------------------------------------------
+# ---- 11. two ranks: only the owned partitions have keys ------------------------------------------
 def _dist_data():
     rng = np.random.default_rng(10)
     ka = rng.integers(0, 4000, 60_000).astype(np.uint64) * np.uint64(0x9E3779B97F4A7C15) + np.uint64(3)
@@ -451,7 +428,7 @@ def test_two_ranks(Ma, Mb, R, p2p):
         assert per_rank[1 - owner][r] == {}, f"partition {r} has keys on a rank that does not own it"
 
 
-# ---- 13. the benchmark's shape, scaled: unique keys, 2 % shared ------------------------------------
+# ---- 12. the benchmark's shape, scaled: unique keys, 2 % shared ------------------------------------
 def test_bench_shape_scaled(sc):
     import torch
     n, shared, R = 2_000_000, 40_000, 8

@@ -7,9 +7,6 @@ oracle_count with the sum read with the column's signedness, and f64 MEAN within
 count.  Each path asserts the statistic that proves it ran."""
 import ctypes
 import math
-import os
-import subprocess
-import sys
 from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
@@ -23,7 +20,6 @@ from vega_b200 import _lib as L
 from vega_b200.rdd import Shuffle, _Col
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 AGG = {"sum": L.VB_AGG_SUM, "min": L.VB_AGG_MIN, "max": L.VB_AGG_MAX, "count": L.VB_AGG_COUNT, "mean": L.VB_AGG_MEAN}
 NP = {"u64": np.uint64, "i64": np.int64, "f64": np.float64}
@@ -164,6 +160,8 @@ PATHS = {
     "restart_per_map": (300_000, 120_000, 0.0, 7),    # host input, hint=100: the per-map tables overflow
     "restart_shared": (300_000, 120_000, 0.0, 7),     # device input, hint=100: the shared table overflows
     "hot_key_cache": (4_000_000, 200_000, 0.12, 7),   # one map task, top key 12 % of rows: the per-CTA cache absorbs it
+    "register_hot": (4_000_000, 200_000, 0.12, 7),    # the hot_key_cache rows as misaligned device columns: the
+                                                      # register-staged kernel keeps its cache past the learning tiles
 }
 
 
@@ -174,20 +172,20 @@ def _cols(keys, cols, spec, device, misalign=False):
     return _col(_dev(keys, misalign), L.VB_U64), tuple(_col(_dev(c, misalign), CODE[d]) for c, (d, _) in zip(cols, dts))
 
 
-def _run_path(sc, path, spec, keys, cols, no_bulk=False):
+def _run_path(sc, path, spec, keys, cols):
     R, n = PATHS[path][3], len(keys)
-    device = path in ("bulk_soa_tail", "shared_borrowed", "restart_shared", "hot_key_cache")
-    kc, vcs = _cols(keys, cols, spec, device)
+    device = path in ("bulk_soa_tail", "shared_borrowed", "restart_shared", "hot_key_cache", "register_hot")
+    kc, vcs = _cols(keys, cols, spec, device, misalign=path == "register_hot")
     M = {"register_small": 5, "bulk_soa_tail": 1, "shared_borrowed": 4, "per_map_merge": 4, "restart_per_map": 2,
-         "restart_shared": 4, "hot_key_cache": 1}[path]
+         "restart_shared": 4, "hot_key_cache": 1, "register_hot": 1}[path]
     hint = 100 if path.startswith("restart") else 0
     parts, st = run_combine(sc, spec, kc, vcs, n, M, R, hint=hint)
-    if path == "register_small":
+    if path in ("register_small", "register_hot"):
         assert st["hot_kernel_variant"] == 0
     elif path in ("bulk_soa_tail", "hot_key_cache"):
-        assert st["hot_kernel_variant"] == (0 if no_bulk else 1)
+        assert st["hot_kernel_variant"] == 1
     elif path == "shared_borrowed":
-        assert st["hot_kernel_variant"] == (0 if no_bulk else 1) and st["kernels"]["merge"]["launches"] == 0
+        assert st["hot_kernel_variant"] == 1 and st["kernels"]["merge"]["launches"] == 0
     elif path == "per_map_merge":
         assert st["kernels"]["merge"]["launches"] >= 1
     else:
@@ -195,20 +193,17 @@ def _run_path(sc, path, spec, keys, cols, no_bulk=False):
     return parts, R
 
 
-def _path_data(path, spec, scale=1):
-    n, nkeys, hot, R = PATHS[path]
-    if scale != 1 and path != "shared_borrowed":            # it needs its row count to take the bulk kernel
-        n, nkeys = max(n // scale, 200_000 if path == "bulk_soa_tail" else 1), max(nkeys // scale, 10)
-        if path == "bulk_soa_tail":
-            n += 3
-    return make_data([sorted(PATHS).index(path), sorted(SPECS).index(spec), scale], spec, n, nkeys, hot)
+def _path_data(path, spec):
+    data = "hot_key_cache" if path == "register_hot" else path     # register_hot: the same rows, placed differently
+    n, nkeys, hot, R = PATHS[data]
+    return make_data([sorted(set(PATHS) - {"register_hot"}).index(data), sorted(SPECS).index(spec), 1], spec, n, nkeys, hot)
 
 
 @pytest.mark.parametrize("spec", list(SPECS))
 @pytest.mark.parametrize("path", list(PATHS))
 def test_combine_path_matches_single_column_references(sc, path, spec):
     keys, cols = _path_data(path, spec)
-    if path == "hot_key_cache":
+    if path in ("hot_key_cache", "register_hot"):
         assert np.unique(keys, return_counts=True)[1].max() > 0.05 * len(keys)
     parts, R = _run_path(sc, path, spec, keys, cols)
     check_combine(parts, spec, keys, cols, R)
@@ -348,29 +343,3 @@ def test_combine_rejections(sc):
     with pytest.raises(vb.VegaB200Error) as e:
         Shuffle(sc, 1, 2, L.VB_U64, L.VB_U64, L.VB_AGG_SUM, multi=([L.VB_U64] * 5, [(L.VB_AGG_SUM, 0)]))
     assert e.value.code == L.VB_ERR_INVALID
-
-
-# ---- A/B switches -----------------------------------------------------------------------------------------------------
-def _ab_cases(sc, switch):
-    no_bulk = switch == "VEGA_B200_NO_BULK"
-    for path in PATHS:
-        for spec in SPECS:
-            keys, cols = _path_data(path, spec, scale=4)
-            parts, R = _run_path(sc, path, spec, keys, cols, no_bulk=no_bulk)
-            check_combine(parts, spec, keys, cols, R)
-
-
-@pytest.mark.parametrize("switch", ["VEGA_B200_NO_BULK", "VEGA_B200_NO_L2_FIT"])
-def test_combine_ab_switch_matches_reference(switch):
-    """Each switch is read once per process: one subprocess per switch."""
-    code = r'''
-import os, vega_b200 as vb
-from tests.test_gpu_combine import _ab_cases
-with vb.Context(0) as sc:
-    _ab_cases(sc, os.environ["AB_SWITCH"])
-print("ab ok")
-'''
-    env = dict(os.environ, AB_SWITCH=switch)
-    env[switch] = "1"
-    out = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=900, env=env, cwd=ROOT)
-    assert out.returncode == 0 and "ab ok" in out.stdout, out.stdout[-2000:] + out.stderr[-4000:]

@@ -267,16 +267,26 @@ def test_rejected_calls(sc):
 
 
 # ---- 8. inner and outer joins of the same two shuffles -----------------------------------------
-@pytest.mark.parametrize("order", [("inner", "left", "right", "full", "inner"), ("full", "right", "left", "inner", "full")])
+@pytest.mark.parametrize("order", [("inner", "left", "right", "full", "inner"), ("full", "right", "left", "inner", "full"),
+                                   ("group", "left", "right", "full", "inner")])
 def test_inner_and_outer_on_the_same_shuffles(sc, order):
-    """The lazy path caches the filtered sides per (right side, kind): each join must give what it gives alone."""
+    """The lazy path caches the filtered sides per (right side, kind): each join must give what it gives alone.
+    "group" reads every partition of both sides first (Shuffle.reduce), so the joins start from grouped sides: the
+    outer joins must then give exactly the rows of two lazy sides."""
     rng = np.random.default_rng(len(order[0]))
-    ka, va = rand_pairs(rng, 12_000, 1500)
-    kb, vb_ = rand_pairs(rng, 9000, 2500)
+    values = "full" if order[0] == "group" else "default"     # "full" keys include 0 and 2^64-1
+    ka, va = rand_pairs(rng, 12_000, 1500, values=values)
+    kb, vb_ = rand_pairs(rng, 9000, 2500, values=values)
     R = 4
     sa, sb = _pair(sc, ka, va, 3, kb, vb_, 2, R)
+    lazy = _pair(sc, ka, va, 3, kb, vb_, 2, R) if order[0] == "group" else None
     inner = O.join(ka, va, 3, kb, vb_, 2, R)
     for kind in order:
+        if kind == "group":
+            for s_ in (sa, sb):
+                for r in range(R):
+                    s_.reduce(r)
+            continue
         if kind == "inner":
             want = []
             for k, v, w in inner:
@@ -288,47 +298,11 @@ def test_inner_and_outer_on_the_same_shuffles(sc, order):
             want = OJ.outer_join_parts(kind, ka, va, 3, kb, vb_, 2, R)
         got = [by_key(*abi_rows(sc, sa, sb, r, None if kind == "inner" else kind)) for r in range(R)]
         assert_parts_equal(got, want)
+        if lazy and kind != "inner":
+            assert got == [by_key(*abi_rows(sc, *lazy, r, kind)) for r in range(R)]
 
 
-# ---- 9. the eager (grouped) cogroup path gives the same rows ------------------------------------
-_EAGER_SCRIPT = r"""
-import pickle, sys
-import numpy as np
-sys.path.insert(0, sys.argv[1])
-import vega_b200 as vb
-from tests.test_gpu_outer_join import gpu_parts, _eager_data
-ka, va, kb, vb_ = _eager_data()
-with vb.Context(0) as sc:
-    a, b = sc.parallelize((ka, va), 3), sc.parallelize((kb, vb_), 2)
-    out = {kind: gpu_parts(getattr(a, kind + "_outer_join")(b, 5)) for kind in ("left", "right", "full")}
-pickle.dump(out, open(sys.argv[2], "wb"))
-"""
-
-
-def _eager_data():
-    rng = np.random.default_rng(9)
-    ka, va = rand_pairs(rng, 10_000, 1000, values="full")
-    kb, vb_ = rand_pairs(rng, 7000, 1600, values="full")
-    return ka, va, kb, vb_
-
-
-def test_eager_cogroup_gives_the_same_rows(sc):
-    ka, va, kb, vb_ = _eager_data()
-    with tempfile.TemporaryDirectory() as d:
-        out = os.path.join(d, "eager.pkl")
-        env = dict(os.environ, VEGA_B200_EAGER_COGROUP="1")
-        res = subprocess.run([sys.executable, "-c", _EAGER_SCRIPT, ROOT, out], env=env, cwd=ROOT, capture_output=True,
-                             text=True, timeout=600)
-        assert res.returncode == 0, res.stderr[-3000:]
-        eager = pickle.load(open(out, "rb"))
-    a, b = sc.parallelize((ka, va), 3), sc.parallelize((kb, vb_), 2)
-    for kind in KINDS:
-        lazy = gpu_parts(getattr(a, METHOD[kind])(b, 5))
-        assert_parts_equal(eager[kind], OJ.outer_join_parts(kind, ka, va, 3, kb, vb_, 2, 5))
-        assert eager[kind] == lazy
-
-
-# ---- 10. two ranks: only the owned partitions have rows -----------------------------------------
+# ---- 9. two ranks: only the owned partitions have rows -----------------------------------------
 def _dist_data():
     rng = np.random.default_rng(10)
     ka = rng.integers(0, 4000, 60_000).astype(np.uint64) * np.uint64(0x9E3779B97F4A7C15) + np.uint64(3)
@@ -395,7 +369,7 @@ def test_two_ranks(Ma, Mb, R, p2p):
             assert per_rank[1 - owner][kind][r] == {}, f"{kind} partition {r} has rows on a rank that does not own it"
 
 
-# ---- 11. configs[3] shape, scaled: unique keys, 2 % shared -----------------------------------
+# ---- 10. configs[3] shape, scaled: unique keys, 2 % shared -----------------------------------
 @pytest.mark.parametrize("kind", KINDS)
 def test_config3_shape_scaled(sc, kind):
     import torch

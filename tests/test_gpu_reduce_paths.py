@@ -4,10 +4,6 @@ Each path asserts the statistic that proves it ran, so a change in kernel select
 testing another path.  Integer ops, COUNT and f64 MIN/MAX are compared bit for bit with the CPU oracle (NaN results
 as one bit pattern); f64 SUM is compared with math.fsum per key by tests/util.py:assert_f64_sums, bit-exact on values
 whose partial sums are all representable and within the order-independent error bound otherwise."""
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 
@@ -19,7 +15,6 @@ from vega_b200 import _lib as L
 from vega_b200.rdd import PairRdd, Rdd, Shuffle, _Col
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 AGG = {"sum": L.VB_AGG_SUM, "min": L.VB_AGG_MIN, "max": L.VB_AGG_MAX, "count": L.VB_AGG_COUNT}
 CODE = {"u64": L.VB_U64, "i64": L.VB_I64, "f64": L.VB_F64, None: L.VB_U64}
@@ -89,6 +84,8 @@ PATHS = {
     "bulk_soa_tail": (1_000_003, 50_000, 0.0, 7),         # device columns, 1 map task, n % 1024 = 579 tail rows
     "bulk_aos": (1_000_003, 50_000, 0.0, 5),              # device (n, 2) rows, 2 map tasks
     "hot_key_cache": (8_000_000, 200_000, 0.12, 7),       # one map task, top key 12 % of rows: ~30 tiles per CTA
+    "register_hot": (8_000_000, 200_000, 0.12, 7),        # the hot_key_cache rows as misaligned device columns: the
+                                                          # register-staged kernel keeps its cache past the learning tiles
     "per_map_merge": (400_000, 100_000, 0.0, 7),          # host input, 4 map tasks: per-map tables merged at seal
     "shared_borrowed": (400_000, 100_000, 0.0, 7),        # device input, 4 map tasks at even starts: one shared table
     "restart_per_map": (300_000, 120_000, 0.0, 7),        # host input, hint=100: per-map tables overflow
@@ -97,7 +94,7 @@ PATHS = {
 }
 
 
-def _run_path(sc, path, op, vdt, keys, vals, n, R, no_bulk=False):
+def _run_path(sc, path, op, vdt, keys, vals, n, R):
     """Place the input as the path needs it, run it, and assert the path's statistic."""
     has_v = op != "count"
     vcode = CODE[vdt]
@@ -105,7 +102,7 @@ def _run_path(sc, path, op, vdt, keys, vals, n, R, no_bulk=False):
         kc, vc = _Col(keys), (_Col(vals, role="value") if has_v else None)
         parts, st = run_reduce(sc, op, vdt, kc, vc, n, 3, R)
         assert st["hot_kernel_variant"] == 0
-    elif path == "register_large":
+    elif path in ("register_large", "register_hot"):
         kc = _col(_dev(keys, misalign=True), L.VB_U64)
         vc = _col(_dev(vals, misalign=True), vcode) if has_v else None
         parts, st = run_reduce(sc, op, vdt, kc, vc, n, 1, R)
@@ -114,11 +111,11 @@ def _run_path(sc, path, op, vdt, keys, vals, n, R, no_bulk=False):
         kc = _col(_dev(keys), L.VB_U64)
         vc = _col(_dev(vals), vcode) if has_v else None
         parts, st = run_reduce(sc, op, vdt, kc, vc, n, 1, R)
-        assert st["hot_kernel_variant"] == (0 if no_bulk else 1)
+        assert st["hot_kernel_variant"] == 1
     elif path == "bulk_aos":
         rows = _col(_dev(np.stack([keys, np.ascontiguousarray(vals).view(np.uint64)], axis=1)), vcode, rows=True)
         parts, st = run_reduce(sc, op, vdt, rows, None, n, 2, R)
-        assert st["hot_kernel_variant"] == (0 if no_bulk else 1)
+        assert st["hot_kernel_variant"] == 1
     elif path == "per_map_merge":
         kc, vc = _Col(keys), (_Col(vals, role="value") if has_v else None)
         parts, st = run_reduce(sc, op, vdt, kc, vc, n, 4, R)
@@ -128,7 +125,7 @@ def _run_path(sc, path, op, vdt, keys, vals, n, R, no_bulk=False):
         vc = _col(_dev(vals), vcode) if has_v else None
         assert all(s % 2 == 0 for s in vb.slice_starts(n, 4))
         parts, st = run_reduce(sc, op, vdt, kc, vc, n, 4, R)
-        assert st["hot_kernel_variant"] == (0 if no_bulk else 1) and st["kernels"]["merge"]["launches"] == 0
+        assert st["hot_kernel_variant"] == 1 and st["kernels"]["merge"]["launches"] == 0
     elif path == "restart_per_map":
         kc, vc = _Col(keys), (_Col(vals, role="value") if has_v else None)
         parts, st = run_reduce(sc, op, vdt, kc, vc, n, 2, R, hint=100)
@@ -148,14 +145,11 @@ def _run_path(sc, path, op, vdt, keys, vals, n, R, no_bulk=False):
     return parts, st
 
 
-def _path_data(path, i_op, scale=1):
-    n, nkeys, hot, R = PATHS[path]
-    if scale != 1 and path not in ("partition_first", "shared_borrowed"):    # these need their row counts to take the path
-        n, nkeys = max(n // scale, 200_000 if path.startswith("bulk") else 1), max(nkeys // scale, 10)
-        if path.startswith("bulk"):
-            n += 3                                            # keep a tail
+def _path_data(path, i_op):
+    data = "hot_key_cache" if path == "register_hot" else path     # register_hot: the same rows, placed differently
+    n, nkeys, hot, R = PATHS[data]
     op, vdt, mode = OPS[i_op]
-    rng = np.random.default_rng([sorted(PATHS).index(path), i_op, scale])
+    rng = np.random.default_rng([sorted(set(PATHS) - {"register_hot"}).index(data), i_op, 1])
     keys, vals = rand_pairs(rng, n, nkeys, vdt or "u64", values=mode, hot=hot)
     return n, R, keys, vals
 
@@ -165,7 +159,7 @@ def _path_data(path, i_op, scale=1):
 def test_reduce_path_matches_exact_reference(sc, path, i_op):
     op, vdt, mode = OPS[i_op]
     n, R, keys, vals = _path_data(path, i_op)
-    if path == "hot_key_cache":
+    if path in ("hot_key_cache", "register_hot"):
         top = np.unique(keys, return_counts=True)[1].max()
         assert top > 0.05 * n
     parts, _ = _run_path(sc, path, op, vdt, keys, vals, n, R)
@@ -245,46 +239,3 @@ def test_f64_sort_keys_follow_total_order(sc, aligned, payload):
         assert np.array_equal(gv.view(np.uint64), ov)
     sizes = [len(rdd.compute(r)[0]) for r in range(R)]
     assert sizes == np.diff(ps.astype(np.int64)).tolist()
-
-
-# ---- A/B switches: the alternative of every default still computes the same results ----------------------------------
-def _ab_cases(sc, switch):
-    """The path matrix at reduced size over a subset of ops, the medium sort/group cases and one join."""
-    from tests.test_gpu_parity import _medium_sort_and_group_cases
-    no_bulk = switch == "VEGA_B200_NO_BULK"
-    for path in PATHS:
-        if path == "partition_first" and switch not in ("VEGA_B200_NO_PARTITION", "VEGA_B200_NO_BULK"):
-            continue                                          # full size only where the switch touches it
-        for i_op in (0, 4, 8, 9, 11):                        # u64 sum, f64 sum (cancel), i64 max, f64 min, count
-            op, vdt, mode = OPS[i_op]
-            n, R, keys, vals = _path_data(path, i_op, scale=4)
-            parts, st = _run_path(sc, path, op, vdt, keys, vals, n, R, no_bulk=no_bulk)
-            check_reduce(parts, op, vdt, mode, keys, vals, R)
-    if no_bulk:                                               # an aligned 1M-row input still takes the register kernel
-        keys, vals = rand_pairs(np.random.default_rng(3), 1 << 20, 1000)
-        _, st = run_reduce(sc, "sum", "u64", _col(_dev(keys), L.VB_U64), _col(_dev(vals), L.VB_U64), 1 << 20, 1, 3)
-        assert st["hot_kernel_variant"] == 0
-    _medium_sort_and_group_cases(sc)
-    rng = np.random.default_rng(8)
-    ka, va = rand_pairs(rng, 60_000, 9000)
-    kb, vb_ = rand_pairs(rng, 40_000, 9000)
-    want = sorted(zip(*[np.concatenate(x).tolist() for x in zip(*O.join(ka, va, 3, kb, vb_, 4, 6))]))
-    k, v, w = sc.parallelize((ka, va), 3).join(sc.parallelize((kb, vb_), 4), 6).collect()
-    assert sorted(zip(k.tolist(), v.tolist(), w.tolist())) == want
-
-
-@pytest.mark.parametrize("switch", ["VEGA_B200_NO_BULK", "VEGA_B200_NO_PARTITION", "VEGA_B200_NO_L2_FIT",
-                                    "VEGA_B200_STABLE_TABLE_SPLIT", "VEGA_B200_NO_CSR_FUSION", "VEGA_B200_EAGER_COGROUP"])
-def test_ab_switch_matches_reference(switch):
-    """Each switch is read once per process: one subprocess per switch."""
-    code = r'''
-import os, vega_b200 as vb
-from tests.test_gpu_reduce_paths import _ab_cases
-with vb.Context(0) as sc:
-    _ab_cases(sc, os.environ["AB_SWITCH"])
-print("ab ok")
-'''
-    env = dict(os.environ, AB_SWITCH=switch)
-    env[switch] = "1"
-    out = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=900, env=env, cwd=ROOT)
-    assert out.returncode == 0 and "ab ok" in out.stdout, out.stdout[-2000:] + out.stderr[-4000:]

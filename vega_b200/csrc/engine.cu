@@ -481,9 +481,8 @@ static int launch_hash_agg_t(vb_shuf *s, int klass, const u64 *a, const u64 *b, 
     vb_ctx *c = s->ctx;
     if constexpr (IN != IN_TABLE) {
         // bulk-staged (copy engine) variant: 16-byte aligned inputs of at least a few tiles per CTA
-        static const bool no_bulk = getenv("VEGA_B200_NO_BULK") != nullptr;
         const bool aligned = (((uintptr_t)a | (uintptr_t)(b ? b : a)) & 15u) == 0;
-        if (!no_bulk && aligned && n >= (u64)HB_TILE * 64) {
+        if (aligned && n >= (u64)HB_TILE * 64) {
             auto kb = hash_agg_bulk_kernel<IN, OPK, TX>;
             constexpr bool has_v = (IN == IN_AOS) || (OPK != OPK_COUNT && OPK != OPK_DICT);
             const size_t smem = hb_smem_bytes(has_v);
@@ -549,11 +548,10 @@ static int launch_hash_agg_multi_t(vb_shuf *s, int klass, const AccSpec &sp, con
     vb_ctx *c = s->ctx;
     const Table t = table_at(tab, log_cap);
     if constexpr (IN == IN_SOA) {
-        static const bool no_bulk = getenv("VEGA_B200_NO_BULK") != nullptr;
         uintptr_t addr = (uintptr_t)keys;
         for (int i = 0; i < NV; ++i) addr |= (uintptr_t)cols.c[i];
         constexpr u64 tile = (u64)HA_THREADS * ma_rows<NV>();
-        if (!no_bulk && (addr & 15u) == 0 && n >= tile * 64) {
+        if ((addr & 15u) == 0 && n >= tile * 64) {
             auto kb = hash_agg_multi_bulk_kernel<NV>;
             const size_t smem = ma_bulk_smem<NV>(MA_MAX_ACCS);     // sized for the widest spec: one occupancy for every spec
             if (c->occ_cache.find((const void *)kb) == c->occ_cache.end())
@@ -701,16 +699,15 @@ static int estimate_distinct(vb_shuf *s, const std::vector<AggInput> &inputs, u6
 // 4-key bucket costs a second dependent probe; <= 0.5 for bigger tables, which pay DRAM traffic instead.
 // When the load-0.4 table would spill out of L2 (2/3 of it is the budget: the input stream passes through the rest)
 // but a table at load <= 0.5 of an *estimated* key count fits, the fuller L2-resident table is taken (the estimate
-// already carries a 1.25x margin, so the real load stays under the 0.6 restart threshold).  VEGA_B200_NO_L2_FIT=1
-// disables that.  slot_bytes: 16 for a single accumulator, 8 * (1 + n_acc) for a multi-aggregate table.
+// already carries a 1.25x margin, so the real load stays under the 0.6 restart threshold).
+// slot_bytes: 16 for a single accumulator, 8 * (1 + n_acc) for a multi-aggregate table.
 static u32 choose_log_cap(u64 total, u64 hint_distinct, bool estimated, u32 max_log, u64 l2_bytes, u32 slot_bytes = 16)
 {
     u64 target = hint_distinct ? (hint_distinct * 5) / 2 : std::min<u64>(2 * std::max<u64>(total, 1), 1ull << 21);
     if (hint_distinct && target > (1ull << 22)) target = 2 * hint_distinct;
-    static const bool no_l2_fit = getenv("VEGA_B200_NO_L2_FIT") != nullptr;
     const u64 budget = l2_bytes / 3 * 2;
     auto bytes = [&](u32 lc) { return (((u64)1 << lc) + BUCKET) * slot_bytes; };
-    if (estimated && !no_l2_fit && bytes(ceil_log2_u64(target)) > budget &&
+    if (estimated && bytes(ceil_log2_u64(target)) > budget &&
         bytes(ceil_log2_u64(hint_distinct * 8 / 5)) <= budget)
         target = hint_distinct * 8 / 5;
     // an estimate from a sample is a lower bound under skew: never start a large input below 2^21 slots (32 MB)
@@ -722,7 +719,7 @@ static u32 choose_log_cap(u64 total, u64 hint_distinct, bool estimated, u32 max_
 // random DRAM access.  Such inputs are first radix-partitioned by the top bits of the slot hash (one stable pass),
 // so that consecutive tiles of hash_agg_kernel all probe the same <= 32 MB region of the table, which then
 // stays L2-resident while it is being filled.  Reduce ops on device-resident rows only (the dictionary of group ops
-// must keep row order, host inputs are PCIe-bound anyway).  VEGA_B200_NO_PARTITION=1 disables it.
+// must keep row order, host inputs are PCIe-bound anyway).
 struct PassPlan;
 template <typename KeyT, bool HAS_VAL> static PassPlan plan_pass(vb_ctx *c, u64 n);
 template <typename KeyT, bool HAS_VAL>
@@ -733,8 +730,7 @@ constexpr u32 PARTITION_MIN_LOG_CAP = 23;
 
 static bool want_partition(int in, int opk, u32 log_cap, u64 n)
 {
-    static const bool off = getenv("VEGA_B200_NO_PARTITION") != nullptr;
-    return !off && opk != OPK_DICT && (in == IN_AOS || in == IN_SOA) && log_cap >= PARTITION_MIN_LOG_CAP && n >= (1ull << 22);
+    return opk != OPK_DICT && (in == IN_AOS || in == IN_SOA) && log_cap >= PARTITION_MIN_LOG_CAP && n >= (1ull << 22);
 }
 
 static int launch_hash_agg_partitioned(vb_shuf *s, int klass, int in, int opk, int tx, const u64 *a, const u64 *b, u64 n, void *tab,
@@ -859,12 +855,15 @@ struct PassPlan {
     size_t hist_bytes() const { return ((size_t)RP_NB * num_parts + 1) * sizeof(u32); }
 };
 
-// (LDM, DGM) combinations the engine uses; anything else is a programming error.
-#define RP_COMBOS(X)                                                                                 \
-    X(LD_SOA64, DG_BITS) X(LD_AOS64, DG_BITS) X(LD_KEY32_VAL_SOA, DG_BITS) X(LD_KEY32_VAL_AOS, DG_BITS) \
-    X(LD_SOA64, DG_BUCKET) X(LD_TABLE_KV, DG_BUCKET) X(LD_TABLE_KI, DG_BUCKET)                         \
-    X(LD_SOA64, DG_DEST) X(LD_AOS64, DG_DEST) X(LD_TABLE_KV, DG_DEST)                                 \
-    X(LD_SOA64, DG_HASHTOP) X(LD_AOS64, DG_HASHTOP)
+// (LDM, DGM) combinations the engine passes per row type; anything else is a programming error.
+//   (u64, u64): seal_sort, the multisplits and the partition-first hash aggregate;
+//   u64 key only: seal_sort;  (u32 id, u64): sort_id_pairs.
+#define RP_COMBOS_U64V(X)                                                                            \
+    X(LD_SOA64, DG_BITS) X(LD_AOS64, DG_BITS) X(LD_SOA64, DG_BUCKET) X(LD_TABLE_KV, DG_BUCKET)         \
+    X(LD_TABLE_KI, DG_BUCKET) X(LD_SOA64, DG_DEST) X(LD_AOS64, DG_DEST) X(LD_SOA64, DG_HASHTOP)        \
+    X(LD_AOS64, DG_HASHTOP)
+#define RP_COMBOS_U64K(X) X(LD_SOA64, DG_BITS)
+#define RP_COMBOS_U32V(X) X(LD_KEY32_VAL_SOA, DG_BITS) X(LD_KEY32_VAL_AOS, DG_BITS)
 
 template <typename KeyT, int LDM> constexpr bool rp_key_ok()
 {
@@ -874,8 +873,10 @@ template <typename KeyT, int LDM> constexpr bool rp_key_ok()
 template <typename KeyT, bool HAS_VAL>
 static const void *scatter_fn(int ldm, int dgm)
 {
-#define X(L, D) if (ldm == L && dgm == D) { if constexpr (rp_key_ok<KeyT, L>()) return (const void *)rp_scatter_kernel<KeyT, HAS_VAL, L, D>; }
-    RP_COMBOS(X)
+#define X(L, D) if (ldm == L && dgm == D) return (const void *)rp_scatter_kernel<KeyT, HAS_VAL, L, D>;
+    if constexpr (sizeof(KeyT) == 8 && HAS_VAL) { RP_COMBOS_U64V(X) }
+    if constexpr (sizeof(KeyT) == 8 && !HAS_VAL) { RP_COMBOS_U64K(X) }
+    if constexpr (sizeof(KeyT) == 4 && HAS_VAL) { RP_COMBOS_U32V(X) }
 #undef X
     return nullptr;
 }
@@ -883,19 +884,14 @@ static const void *scatter_fn(int ldm, int dgm)
 template <typename KeyT>
 static const void *hist_fn(int ldm, int dgm)
 {
-#define X(L, D) if (ldm == L && dgm == D) { if constexpr (rp_key_ok<KeyT, L>()) return (const void *)rp_hist_kernel<KeyT, L, D>; }
-    RP_COMBOS(X)
+#define X(L, D) if (ldm == L && dgm == D) return (const void *)rp_hist_kernel<KeyT, L, D>;
+    if constexpr (sizeof(KeyT) == 8) { RP_COMBOS_U64V(X) }     // covers the key-only pairs
+    if constexpr (sizeof(KeyT) == 4) { RP_COMBOS_U32V(X) }
 #undef X
     return nullptr;
 }
 
-// The gather sweep (gsweep.cuh) is the scatter of the DG_BITS passes; VEGA_B200_NO_GSWEEP=1 falls back to rp_sweep_kernel.
-static bool gsweep_enabled()
-{
-    static const bool on = getenv("VEGA_B200_NO_GSWEEP") == nullptr;
-    return on;
-}
-
+// The gather sweep (gsweep.cuh) is the scatter of the DG_BITS passes.
 template <typename KeyT, bool HAS_VAL>
 static bool gsweep_lookup(int ldm, const void **kern, size_t *smem, u32 *tile, u32 *threads)
 {
@@ -919,25 +915,12 @@ static PassPlan plan_pass(vb_ctx *c, u64 n)
 {
     PassPlan p;
     if (n == 0) return p;
-    // one part per resident CTA of the scatter that will run
-    int occ;
-    if (gsweep_enabled()) {
-        occ = GsPlan<KeyT, HAS_VAL, (sizeof(KeyT) == 4 ? LD_KEY32_VAL_SOA : LD_SOA64)>::CTAS;
-    } else {
-        // occupancy of rp_scatter_kernel is the same for every loader/digit instantiation to within a CTA; use a representative one
-        const void *kern = scatter_fn<KeyT, HAS_VAL>(LD_SOA64, DG_BUCKET);
-        const size_t smem = rp_scatter_smem<KeyT, HAS_VAL>();
-        occ = 2;
-        if (kern) {
-            cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            occ = occupancy(c, kern, RPS_THREADS, smem);
-        }
-        occ = std::max(occ, sw_ctas<KeyT, HAS_VAL>());
-    }
+    // one part per resident CTA of the gather sweep
+    const int occ = GsPlan<KeyT, HAS_VAL, (sizeof(KeyT) == 4 ? LD_KEY32_VAL_SOA : LD_SOA64)>::CTAS;
     u64 tiles = (n + RP_TILE - 1) / RP_TILE;
     u64 parts = std::min<u64>(tiles, (u64)c->sm_count * occ);
     u64 tiles_per_part = (tiles + parts - 1) / parts;
-    if (tiles_per_part > 6) tiles_per_part = (tiles_per_part + 5) / 6 * 6;   // 24576-row units: a multiple of every sweep tile (3072 ... 8192 rows)
+    if (tiles_per_part > 6) tiles_per_part = (tiles_per_part + 5) / 6 * 6;   // 24576-row units: a multiple of the sweep tile (6144 rows)
     p.rows_per_part = tiles_per_part * RP_TILE;
     p.num_parts = (u32)((n + p.rows_per_part - 1) / p.rows_per_part);
     return p;
@@ -976,26 +959,10 @@ static int radix_hist_scan(vb_shuf *s, const Loader &ld, const Digit &dg, u64 n,
     return VB_OK;
 }
 
-// Row-stream loader / digit pairs rp_sweep_kernel is instantiated for (sweep.cuh)
-#define SW_COMBOS_U64V(X) X(LD_SOA64, DG_BITS) X(LD_AOS64, DG_BITS) X(LD_SOA64, DG_DEST) X(LD_AOS64, DG_DEST) X(LD_SOA64, DG_HASHTOP) X(LD_AOS64, DG_HASHTOP) X(LD_SOA64, DG_BUCKET)
-#define SW_COMBOS_U64K(X) X(LD_SOA64, DG_BITS)
-#define SW_COMBOS_U32V(X) X(LD_KEY32_VAL_SOA, DG_BITS) X(LD_KEY32_VAL_AOS, DG_BITS)
-
-template <typename KeyT, bool HAS_VAL>
-static bool sweep_lookup(int ldm, int dgm, const void **kern, size_t *smem)
-{
-#define X(L, D)                                                      \
-    if (ldm == L && dgm == D) {                                      \
-        *kern = (const void *)rp_sweep_kernel<KeyT, HAS_VAL, L, D>; \
-        *smem = SwSmem<KeyT, HAS_VAL, L>::total;                     \
-        return true;                                                 \
-    }
-    if constexpr (sizeof(KeyT) == 8 && HAS_VAL) { SW_COMBOS_U64V(X) }
-    if constexpr (sizeof(KeyT) == 8 && !HAS_VAL) { SW_COMBOS_U64K(X) }
-    if constexpr (sizeof(KeyT) == 4 && HAS_VAL) { SW_COMBOS_U32V(X) }
-#undef X
-    return false;
-}
+// Row-stream loader / digit pairs of the (u64, u64) multisplits rp_sweep_kernel is instantiated for (sweep.cuh).
+// The DG_BITS passes never reach it: where the gather sweep's n >= 4 x its tile fails and the sweep's would hold,
+// plan_pass gives 4096-row parts, which the sweep tile does not divide.
+#define SW_COMBOS(X) X(LD_SOA64, DG_DEST) X(LD_AOS64, DG_DEST) X(LD_SOA64, DG_HASHTOP) X(LD_AOS64, DG_HASHTOP) X(LD_SOA64, DG_BUCKET)
 
 template <typename KeyT, bool HAS_VAL>
 static int radix_pass(vb_shuf *s, const Loader &ld, const Digit &dg, u64 n, KeyT *out_keys, u64 *out_vals, u32 *d_hist,
@@ -1010,7 +977,7 @@ static int radix_pass(vb_shuf *s, const Loader &ld, const Digit &dg, u64 n, KeyT
         const void *gk = nullptr;
         size_t gsm = 0;
         u32 GT = 0, gthreads = 0;
-        if (gsweep_enabled() && dg.mode == DG_BITS && n < SW_ROW_LIMIT && plan.rows_per_part % 4096 == 0 &&
+        if (dg.mode == DG_BITS && n < SW_ROW_LIMIT && plan.rows_per_part % 4096 == 0 &&
             gsweep_lookup<KeyT, HAS_VAL>(ld.mode, &gk, &gsm, &GT, &gthreads) && n >= 4ull * GT &&
             !(((uintptr_t)ld.keys & 15u) || (ld.vals && ((uintptr_t)ld.vals & 15u))) && !(HAS_VAL && ld.mode != LD_AOS64 && !ld.vals)) {
             if (c->occ_cache.find(gk) == c->occ_cache.end()) CU(cudaFuncSetAttribute(gk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gsm));
@@ -1021,8 +988,7 @@ static int radix_pass(vb_shuf *s, const Loader &ld, const Digit &dg, u64 n, KeyT
             a.part_off = d_hist; a.num_parts = plan.num_parts; a.rows_per_part = plan.rows_per_part;
             if constexpr (sizeof(KeyT) == 4 && HAS_VAL) {
                 // last pass of group_by_key's sort: value-run starts recorded by the scatter itself, ids not written (rp_gsweep_kernel<CSR>)
-                static const bool no_csr = getenv("VEGA_B200_NO_CSR_FUSION") != nullptr;
-                if (csr && !no_csr && ld.mode == LD_KEY32_VAL_SOA) {
+                if (csr && ld.mode == LD_KEY32_VAL_SOA) {
                     const void *ck = (const void *)rp_gsweep_kernel<u32, true, LD_KEY32_VAL_SOA, true>;
                     if (c->occ_cache.find(ck) == c->occ_cache.end()) CU(cudaFuncSetAttribute(ck, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gsm));
                     (void)occupancy(c, ck, (int)gthreads, gsm);
@@ -1038,14 +1004,17 @@ static int radix_pass(vb_shuf *s, const Loader &ld, const Digit &dg, u64 n, KeyT
             return kl.done("rp_gsweep_kernel");
         }
     }
-    {   // other row streams: the sweep tile pipeline fed by the per-part offsets
+    if constexpr (sizeof(KeyT) == 8 && HAS_VAL) {   // multisplits of row streams: the sweep tile pipeline fed by the per-part offsets
         const void *sw = nullptr;
         size_t swsm = 0;
-        const u32 T = sw_tile<KeyT, HAS_VAL>();
-        if (n < SW_ROW_LIMIT && plan.rows_per_part % T == 0 && n >= 4ull * T && sweep_lookup<KeyT, HAS_VAL>(ld.mode, dg.mode, &sw, &swsm) &&
-            !(((uintptr_t)ld.keys & 15u) || (ld.vals && ((uintptr_t)ld.vals & 15u))) && !(HAS_VAL && ld.mode != LD_AOS64 && !ld.vals)) {
+#define X(L, D) if (ld.mode == L && dg.mode == D) { sw = (const void *)rp_sweep_kernel<L, D>; swsm = SwSmem<L>::total; }
+        SW_COMBOS(X)
+#undef X
+        const u32 T = SW_TILE;
+        if (sw && n < SW_ROW_LIMIT && plan.rows_per_part % T == 0 && n >= 4ull * T &&
+            !(((uintptr_t)ld.keys & 15u) || (ld.vals && ((uintptr_t)ld.vals & 15u))) && !(ld.mode != LD_AOS64 && !ld.vals)) {
             if (c->occ_cache.find(sw) == c->occ_cache.end()) CU(cudaFuncSetAttribute(sw, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)swsm));
-            (void)occupancy(c, sw, sw_threads<KeyT, HAS_VAL>(), swsm);
+            (void)occupancy(c, sw, SW_THREADS, swsm);
             SweepArgs a{};
             a.keys = ld.keys; a.vals = ld.vals; a.n = n; a.n_tiles = (u32)((n + T - 1) / T);
             a.out_keys = out_keys; a.out_vals = out_vals;
@@ -1053,7 +1022,7 @@ static int radix_pass(vb_shuf *s, const Loader &ld, const Digit &dg, u64 n, KeyT
             Digit dgs = dg;
             KLaunch kl(s, K_RP_SCATTER, n);
             void *args[] = {&a, &dgs};
-            CU(cudaLaunchKernel(sw, dim3(plan.num_parts), dim3(sw_threads<KeyT, HAS_VAL>()), args, swsm, c->stream));
+            CU(cudaLaunchKernel(sw, dim3(plan.num_parts), dim3(SW_THREADS), args, swsm, c->stream));
             return kl.done("rp_sweep_kernel");
         }
     }
@@ -1786,8 +1755,7 @@ static int finalize_reduce(vb_shuf *s, void *tab, u32 log_cap, u64 n_ins)
     TRY(v.alloc(max_d * 8));
     const Table ft = table_at(tab, log_cap);
     Loader lt{LD_TABLE_KV, ft.keys, ft.accs, cap};
-    static const bool ordered_only = getenv("VEGA_B200_STABLE_TABLE_SPLIT") != nullptr;     // A/B switch
-    if (R <= (u32)TS_MAX_BINS && !ordered_only) TRY(multisplit_table_unordered(s, ft, DG_BUCKET, R, k.as<u64>(), v.as<u64>(), s->bucket_off));
+    if (R <= (u32)TS_MAX_BINS) TRY(multisplit_table_unordered(s, ft, DG_BUCKET, R, k.as<u64>(), v.as<u64>(), s->bucket_off));
     else TRY(multisplit(s, lt, cap + 1, DG_BUCKET, R, max_d, k.as<u64>(), v.as<u64>(), s->bucket_off));
     const u64 D = s->bucket_off[R];
     const int tx = val_tx(s);
@@ -1910,10 +1878,8 @@ static int export_prepare_locked(vb_shuf *s, uint64_t *counts)
             TRY(k.alloc((n_ins + 1) * 8));
             TRY(v.alloc((n_ins + 1) * 8));
             const Table et = table_at(tab, log_cap);
-            Loader lt{LD_TABLE_KV, et.keys, et.accs, 1ull << log_cap};
-            static const bool ordered_only = getenv("VEGA_B200_STABLE_TABLE_SPLIT") != nullptr;
-            if (s->world <= (u32)TS_MAX_BINS && !ordered_only) TRY(multisplit_table_unordered(s, et, DG_DEST, s->world, k.as<u64>(), v.as<u64>(), off));
-            else TRY(multisplit(s, lt, (1ull << log_cap) + 1, DG_DEST, s->world, n_ins + 1, k.as<u64>(), v.as<u64>(), off));
+            // vb_shuffle_set_dist caps world at TS_MAX_BINS (256): the unordered table split always applies
+            TRY(multisplit_table_unordered(s, et, DG_DEST, s->world, k.as<u64>(), v.as<u64>(), off));
             s->exp_keys = (u64 *)k.release();
             s->exp_vals = (u64 *)v.release();
         }
@@ -2663,12 +2629,6 @@ extern "C" int32_t vb_shuffle_exchange_stats(vb_shuf *s, vb_xstats *out)
 // vb_join* first finds the matching keys (dictionary of the right keys, one probe per left row), compacts both sides
 // to the matching rows (stable) and groups just those.  vb_shuffle_reduce* (the cogroup itself) groups everything.
 // ---------------------------------------------------------------------------------------------
-static bool lazy_cogroup_enabled()
-{
-    static const bool off = getenv("VEGA_B200_EAGER_COGROUP") != nullptr;
-    return !off;
-}
-
 // take ownership of the gathered rows as SoA (copy when they are borrowed, in the shared arena, or AoS)
 static int seal_lazy(vb_shuf *s, const Gathered &g, bool rows_are_owned_imports)
 {
@@ -2938,7 +2898,7 @@ extern "C" int32_t vb_shuffle_seal(vb_shuf *s)
                     Gathered g;
                     TRY(gather_maps(s, &g));
                     if (s->agg == VB_AGG_SORT) TRY(seal_sort(s, g));
-                    else if (s->agg == VB_AGG_COGROUP && lazy_cogroup_enabled()) TRY(seal_lazy(s, g, false));
+                    else if (s->agg == VB_AGG_COGROUP) TRY(seal_lazy(s, g, false));
                     else TRY(seal_group(s, g));
                 }
             } else {
@@ -2962,7 +2922,7 @@ extern "C" int32_t vb_shuffle_seal(vb_shuf *s)
                 } else {
                     Gathered g;
                     g.keys = s->imp_keys; g.vals = s->imp_vals; g.n = s->imp_n;
-                    if (s->agg == VB_AGG_COGROUP && lazy_cogroup_enabled()) TRY(seal_lazy(s, g, s->imp_keys == s->imp_own_k && s->imp_own_k));
+                    if (s->agg == VB_AGG_COGROUP) TRY(seal_lazy(s, g, s->imp_keys == s->imp_own_k && s->imp_own_k));
                     else TRY(seal_group(s, g));
                 }
             }

@@ -1,4 +1,5 @@
-// gsweep.cuh — the scatter of the LSD sort passes (DG_BITS digits), third generation.
+// gsweep.cuh — the scatter of every LSD sort pass (DG_BITS digits) over row streams, third generation.
+// rp_sweep_kernel (sweep.cuh) is kept for the (u64,u64) multisplits; measured on the sort passes, it was the slower one:
 //
 // rp_sweep_kernel spends half of a pass issue-bound in the ballot ranking and the other half bound by the
 // shared-memory pipe while it permutes whole rows into a staging buffer (bank conflicts; mio_throttle + short_scoreboard

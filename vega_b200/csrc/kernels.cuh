@@ -51,38 +51,6 @@ enum : int { OPK_ADD_U64 = 0, OPK_ADD_F64 = 1, OPK_MIN_U64 = 2, OPK_MAX_U64 = 3,
 
 VB_HD u64 op_identity(int opk) { return opk == OPK_MIN_U64 ? ~0ull : 0ull; }
 
-// Table accesses can carry an L2 evict_last hint (the stream is evict_first): A/B-measured, see VB_TABLE_EVICT_LAST.
-#ifndef VB_TABLE_EVICT_LAST
-#define VB_TABLE_EVICT_LAST 0
-#endif
-VB_D u64 table_policy()
-{
-#if VB_TABLE_EVICT_LAST
-    return policy_evict_last();
-#else
-    return 0;
-#endif
-}
-
-template <int OPK>
-VB_D void op_red_hint(u64 *acc, u64 v, u64 pol)
-{
-#if VB_TABLE_EVICT_LAST
-    if (OPK == OPK_ADD_U64) asm volatile("red.global.add.L2::cache_hint.u64 [%0], %1, %2;" ::"l"(acc), "l"(v), "l"(pol) : "memory");
-    else if (OPK == OPK_COUNT) asm volatile("red.global.add.L2::cache_hint.u64 [%0], %1, %2;" ::"l"(acc), "l"(1ull), "l"(pol) : "memory");
-    else if (OPK == OPK_ADD_F64) asm volatile("red.global.add.L2::cache_hint.f64 [%0], %1, %2;" ::"l"(acc), "d"(__longlong_as_double((long long)v)), "l"(pol) : "memory");
-    else if (OPK == OPK_MIN_U64) asm volatile("red.global.min.L2::cache_hint.u64 [%0], %1, %2;" ::"l"(acc), "l"(v), "l"(pol) : "memory");
-    else if (OPK == OPK_MAX_U64) asm volatile("red.global.max.L2::cache_hint.u64 [%0], %1, %2;" ::"l"(acc), "l"(v), "l"(pol) : "memory");
-#else
-    (void)pol;
-    if (OPK == OPK_ADD_U64) atomicAdd((unsigned long long *)acc, (unsigned long long)v);
-    else if (OPK == OPK_COUNT) atomicAdd((unsigned long long *)acc, 1ull);
-    else if (OPK == OPK_ADD_F64) atomicAdd((double *)acc, __longlong_as_double((long long)v));
-    else if (OPK == OPK_MIN_U64) atomicMin((unsigned long long *)acc, (unsigned long long)v);
-    else if (OPK == OPK_MAX_U64) atomicMax((unsigned long long *)acc, (unsigned long long)v);
-#endif
-}
-
 template <int OPK>
 VB_D void op_red(u64 *acc, u64 v)
 {
@@ -116,20 +84,6 @@ VB_D Bucket4 ld_bucket(const u64 *p)
                  : "=l"(b.k0), "=l"(b.k1), "=l"(b.k2), "=l"(b.k3)
                  : "l"(p));
     return b;
-}
-VB_D Bucket4 ld_bucket_hint(const u64 *p, u64 pol)
-{
-#if VB_TABLE_EVICT_LAST
-    Bucket4 b;
-    asm volatile("ld.global.L1::no_allocate.L2::cache_hint.v2.u64 {%0, %1}, [%4], %5;\n\t"
-                 "ld.global.L1::no_allocate.L2::cache_hint.v2.u64 {%2, %3}, [%4+16], %5;"
-                 : "=l"(b.k0), "=l"(b.k1), "=l"(b.k2), "=l"(b.k3)
-                 : "l"(p), "l"(pol));
-    return b;
-#else
-    (void)pol;
-    return ld_bucket(p);
-#endif
 }
 VB_D int bucket_find(const Bucket4 &b, u64 key)
 {
@@ -187,9 +141,6 @@ VB_D bool table_resolve(const Table &t, u64 b, Bucket4 bk, u64 key, u64 v, u32 &
 // keys nothing hits, so every CTA measures its hit rate over its first 16 tiles and switches the
 // cache off below 1/16.
 constexpr int HC_SLOTS = 1024;
-#ifndef VB_HC_ENABLE
-#define VB_HC_ENABLE 1
-#endif
 
 template <int OPK>
 VB_D void op_shared(u64 *acc, u64 v)
@@ -238,7 +189,6 @@ VB_D void ha_process_rows(const Table &t, TableCtl *ctl, u64 (&k)[ROWS], u64 (&v
                           u32 *__restrict__ slot_out, u64 *hc_keys, u64 *hc_acc, bool use_cache, u32 &my_inserts, u32 &my_hits)
 {
     const u64 cap = 1ull << t.log_cap;
-    const u64 tpol = table_policy();
     // f64 MIN/MAX fold like Rust's f64::min / f64::max: a NaN value is ignored (it becomes the op's identity, so the
     // key is still inserted), and a key whose values are all NaN finalises to tx_inv(identity), which is a NaN.
     constexpr bool NAN_IS_IDENTITY = (TX == TX_F64) && (OPK == OPK_MIN_U64 || OPK == OPK_MAX_U64);
@@ -264,7 +214,7 @@ VB_D void ha_process_rows(const Table &t, TableCtl *ctl, u64 (&k)[ROWS], u64 (&v
         }
     }
     ha_probe_rows(t, ctl, k, ok, h, my_inserts, [&](u64 sl, int j) {
-        op_red_hint<OPK>(&t.accs[sl], v[j], tpol);
+        op_red<OPK>(&t.accs[sl], v[j]);
         if (OPK == OPK_DICT) st_stream_u32(slot_out + row0 + (u64)j * HA_THREADS, (u32)sl);
     });
 }
@@ -275,7 +225,6 @@ template <int ROWS, class OnHit>
 VB_D void ha_probe_rows(const Table &t, TableCtl *ctl, const u64 (&k)[ROWS], bool (&ok)[ROWS], const u64 (&h)[ROWS], u32 &my_inserts,
                         OnHit &&on_hit)
 {
-    const u64 tpol = table_policy();
     const u32 hshift = 64 - (t.log_cap - 2);
     // Probe rounds run in lockstep over the ROWS rows of a thread: every round first consumes the
     // buckets loaded by the previous one, then issues the next probes of all unresolved rows together,
@@ -286,7 +235,7 @@ VB_D void ha_probe_rows(const Table &t, TableCtl *ctl, const u64 (&k)[ROWS], boo
 #pragma unroll
     for (int j = 0; j < ROWS; ++j) {
         bidx[j] = h[j] >> hshift;
-        if (ok[j]) bk[j] = ld_bucket_hint(&t.keys[4 * bidx[j]], tpol);
+        if (ok[j]) bk[j] = ld_bucket(&t.keys[4 * bidx[j]]);
     }
     bool pending = true;
 #pragma unroll 1
@@ -317,7 +266,7 @@ VB_D void ha_probe_rows(const Table &t, TableCtl *ctl, const u64 (&k)[ROWS], boo
         if (pending) {
 #pragma unroll
             for (int j = 0; j < ROWS; ++j)
-                if (ok[j]) bk[j] = ld_bucket_hint(&t.keys[4 * bidx[j]], tpol);
+                if (ok[j]) bk[j] = ld_bucket(&t.keys[4 * bidx[j]]);
         }
     }
     if (pending) atomicExch(&ctl->abort, 1u);   // probe chain longer than HA_MAX_PROBE buckets
@@ -331,7 +280,7 @@ __global__ void __launch_bounds__(HA_THREADS, 3)   // 3 CTAs/SM: the A/B winner 
 hash_agg_kernel(const u64 *__restrict__ a, const u64 *__restrict__ b, u64 n, Table t, TableCtl *ctl, u64 max_inserts,
                 u32 *__restrict__ slot_out)
 {
-    constexpr bool CACHE = VB_HC_ENABLE && (OPK != OPK_DICT) && (IN != IN_TABLE);
+    constexpr bool CACHE = (OPK != OPK_DICT) && (IN != IN_TABLE);
     constexpr int OPK_FLUSH = (OPK == OPK_COUNT) ? OPK_ADD_U64 : OPK;      // partial counts are summed
     __shared__ u32 s_inserts;
     __shared__ u32 s_abort;
@@ -443,7 +392,7 @@ hash_agg_bulk_kernel(const u64 *__restrict__ a, const u64 *__restrict__ b, u64 n
                      u32 *__restrict__ slot_out)
 {
     static_assert(IN == IN_AOS || IN == IN_SOA, "table merges use hash_agg_kernel");
-    constexpr bool CACHE = VB_HC_ENABLE && (OPK != OPK_DICT);
+    constexpr bool CACHE = (OPK != OPK_DICT);
     constexpr int OPK_FLUSH = (OPK == OPK_COUNT) ? OPK_ADD_U64 : OPK;
     constexpr bool HAS_V = (IN == IN_AOS) || (OPK != OPK_COUNT && OPK != OPK_DICT);
     constexpr u32 STAGE_BYTES = HB_TILE * (HAS_V ? 16 : 8);
@@ -750,7 +699,7 @@ __global__ void __launch_bounds__(HA_THREADS, 2)
 hash_agg_multi_kernel(const u64 *__restrict__ keys, MaCols cols, u64 n, Table t, AccSpec sp, TableCtl *ctl, u64 max_inserts)
 {
     static_assert(IN == IN_SOA || (IN == IN_TABLE && NV == 1), "SoA rows or a table merge");
-    constexpr bool CACHE = VB_HC_ENABLE && (IN != IN_TABLE);
+    constexpr bool CACHE = (IN != IN_TABLE);
     constexpr int ROWS = ma_rows<NV>();
     constexpr int TILE = HA_THREADS * ROWS;
     extern __shared__ __align__(16) u64 ma_cache[];          // hc_keys[MA_HC_SLOTS], hc_acc[n][MA_HC_SLOTS]
@@ -810,7 +759,7 @@ template <int NV>
 __global__ void __launch_bounds__(HB_THREADS, 2)
 hash_agg_multi_bulk_kernel(const u64 *__restrict__ keys, MaCols cols, u64 n, Table t, AccSpec sp, TableCtl *ctl, u64 max_inserts)
 {
-    constexpr bool CACHE = VB_HC_ENABLE;
+    constexpr bool CACHE = true;
     constexpr int ROWS = ma_rows<NV>();
     constexpr int TILE = HA_THREADS * ROWS;
     constexpr u32 STAGE_BYTES = (u32)ma_stage_bytes<NV>();

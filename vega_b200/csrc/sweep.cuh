@@ -1,5 +1,5 @@
-// sweep.cuh — the scatter of a radix pass over row streams that the gather sweep (gsweep.cuh) does not take:
-// the multisplits (DG_BUCKET, DG_DEST, DG_HASHTOP digits) and, with VEGA_B200_NO_GSWEEP=1, the LSD sort passes.
+// sweep.cuh — the scatter of a radix pass over (u64, u64) row streams that the gather sweep (gsweep.cuh) does not take:
+// the multisplits (DG_BUCKET, DG_DEST, DG_HASHTOP digits).
 //
 //   * offsets come from the per-part histogram (rp_hist_kernel + rp_scan_kernel): CTA p walks its own contiguous
 //     part of the input and keeps running digit offsets in shared memory;
@@ -9,49 +9,41 @@
 //   * 4 CTA barriers per tile (rp_scatter_kernel has 5): warp-private u16 counters are cleared by their
 //     own warp, the staging buffer is only rewritten after the next tile's third barrier.
 //
-// With the CTA shape picked per row type (sw_threads) it is faster than rp_scatter_kernel on 1e9 rows.
+// With 1024-thread CTAs (SW_THREADS) it is faster than rp_scatter_kernel on 1e9 rows.
 // Stable: rows keep their input order inside every digit (tile order → warp order → lane-striped item order),
-// which the LSD sort and the group value order (SURVEY §8a, tests/test_pair_rdd.rs:30-36) rely on.
+// which the group value order (SURVEY §8a, tests/test_pair_rdd.rs:30-36) relies on.
 // Handles the row-stream loaders (all rows valid); table loaders and the REMOTE scatter stay on rp_scatter_kernel.
 #pragma once
 #include "kernels.cuh"
 
 namespace vb {
 
-// CTA shape by row type (A/B on 1e9 rows): key-only rows run fastest as 256 threads x 4 CTAs per SM (3072-key tiles, ahead of
-// 512 x 2 and 256 x 16 keys); rows with a value want the longest runs per digit: 1024 threads x 1 CTA (8192-row tiles of
-// (u32,u64), 6144 of (u64,u64)) beats 512 x 2 and 256 x 4.
+// CTA shape (A/B on 1e9 rows): (u64,u64) rows want the longest runs per digit: 1024 threads x 1 CTA (6144-row tiles)
+// beats 512 x 2 and 256 x 4.
 #ifndef VB_SW_THREADS_VAL
 #define VB_SW_THREADS_VAL 1024
 #endif
-#ifndef VB_SW_THREADS_KEY
-#define VB_SW_THREADS_KEY 256
-#endif
-#ifndef VB_SW_ITEMS_KEY
-#define VB_SW_ITEMS_KEY 12
-#endif
-template <typename KeyT, bool HAS_VAL> constexpr int sw_threads() { return HAS_VAL ? VB_SW_THREADS_VAL : VB_SW_THREADS_KEY; }
-template <typename KeyT, bool HAS_VAL> constexpr int sw_ctas() { return 1024 / sw_threads<KeyT, HAS_VAL>(); }
-constexpr int SW_MAX_CTAS = 4;
+constexpr int SW_THREADS = VB_SW_THREADS_VAL;
+constexpr int SW_CTAS = 1024 / SW_THREADS;
 constexpr int SW_NB = 256;
 constexpr u64 SW_ROW_LIMIT = 1ull << 31;    // the sweeps take n < SW_ROW_LIMIT rows (u32 output positions); larger inputs use rp_scatter_kernel
 
-// items per thread by row width: the tile buffers (raw + staged) of the resident CTAs fit the 227 KB of an SM
-template <typename KeyT, bool HAS_VAL> constexpr int sw_items() { return (sizeof(KeyT) + (HAS_VAL ? 8 : 0)) >= 16 ? 6 : (sizeof(KeyT) + (HAS_VAL ? 8 : 0)) == 12 ? 8 : VB_SW_ITEMS_KEY; }
-template <typename KeyT, bool HAS_VAL> constexpr int sw_tile() { return sw_threads<KeyT, HAS_VAL>() * sw_items<KeyT, HAS_VAL>(); }
+// 6 items per thread: the tile buffers (raw + staged) of the resident CTAs fit the 227 KB of an SM
+constexpr int SW_ITEMS = 6;
+constexpr int SW_TILE = SW_THREADS * SW_ITEMS;
 
 // shared-memory plan (bytes): [raw vals | raw keys] [staged vals | staged keys | staged digit] [warp counters u16]
-template <typename KeyT, bool HAS_VAL, int LDM>
+template <int LDM>
 struct SwSmem {
-    static constexpr int T = sw_tile<KeyT, HAS_VAL>();
+    static constexpr int T = SW_TILE;
     static constexpr bool AOS = (LDM == LD_AOS64);
-    static constexpr size_t raw_vals = (AOS || LDM == LD_KEY32_VAL_AOS) ? 0 : (HAS_VAL ? (size_t)T * 8 : 0);
-    static constexpr size_t raw_keys = AOS ? (size_t)T * 16 : (size_t)T * sizeof(KeyT);
+    static constexpr size_t raw_vals = AOS ? 0 : (size_t)T * 8;
+    static constexpr size_t raw_keys = AOS ? (size_t)T * 16 : (size_t)T * 8;
     static constexpr size_t raw = raw_vals + raw_keys;
-    static constexpr size_t st_vals = HAS_VAL ? (size_t)T * 8 : 0;
-    static constexpr size_t st_keys = (size_t)T * sizeof(KeyT);
+    static constexpr size_t st_vals = (size_t)T * 8;
+    static constexpr size_t st_keys = (size_t)T * 8;
     static constexpr size_t st_dig = (size_t)T;
-    static constexpr size_t cnt = (size_t)(sw_threads<KeyT, HAS_VAL>() / 32) * SW_NB * 2;
+    static constexpr size_t cnt = (size_t)(SW_THREADS / 32) * SW_NB * 2;
     static constexpr size_t total = raw + st_vals + st_keys + st_dig + cnt;
 };
 
@@ -72,27 +64,23 @@ struct SweepArgs {
 
 // Each CTA walks its own contiguous part tile by tile (copy-engine staging, warp-private u16 counters, 4 barriers,
 // full-tile fast path) and keeps running digit offsets in shared memory.
-template <typename KeyT, bool HAS_VAL, int LDM, int DGM>
-__global__ void __launch_bounds__((sw_threads<KeyT, HAS_VAL>()), (sw_ctas<KeyT, HAS_VAL>()))
+template <int LDM, int DGM>
+__global__ void __launch_bounds__(SW_THREADS, SW_CTAS)
 rp_sweep_kernel(SweepArgs a, Digit dg)
 {
-    constexpr int SW_THREADS = sw_threads<KeyT, HAS_VAL>();
     constexpr int SW_WARPS = SW_THREADS / 32;
     static_assert(SW_NB <= SW_THREADS, "one thread per digit in the column scan");
-    using SM = SwSmem<KeyT, HAS_VAL, LDM>;
-    constexpr int K = sw_items<KeyT, HAS_VAL>();
+    using SM = SwSmem<LDM>;
+    constexpr int K = SW_ITEMS;
     constexpr int T = SM::T;
     constexpr bool AOS = SM::AOS;
-    constexpr bool VAL_AOS = (LDM == LD_KEY32_VAL_AOS);    // values come from 16-byte rows: read with plain loads
-    constexpr bool BULK_VALS = HAS_VAL && !AOS && !VAL_AOS;
-    static_assert(LDM == LD_SOA64 || LDM == LD_AOS64 || LDM == LD_KEY32_VAL_SOA || LDM == LD_KEY32_VAL_AOS, "row-stream loaders only");
-    static_assert(!AOS || (sizeof(KeyT) == 8 && HAS_VAL), "AoS rows are (u64,u64)");
+    static_assert(LDM == LD_SOA64 || LDM == LD_AOS64, "(u64,u64) row-stream loaders only");
 
     extern __shared__ __align__(128) unsigned char sw_smem[];
     unsigned char *raw_vals_b = sw_smem;                                   // [T] u64 (SoA values)
-    unsigned char *raw_keys_b = sw_smem + SM::raw_vals;                    // [T] KeyT, or [T] 16-byte rows (AoS)
+    unsigned char *raw_keys_b = sw_smem + SM::raw_vals;                    // [T] u64 keys, or [T] 16-byte rows (AoS)
     u64 *st_vals = (u64 *)(sw_smem + SM::raw);
-    KeyT *st_keys = (KeyT *)(sw_smem + SM::raw + SM::st_vals);
+    u64 *st_keys = (u64 *)(sw_smem + SM::raw + SM::st_vals);
     unsigned char *st_dig = sw_smem + SM::raw + SM::st_vals + SM::st_keys;
     unsigned short *cnt = (unsigned short *)(sw_smem + SM::raw + SM::st_vals + SM::st_keys + SM::st_dig);   // [SW_WARPS][256]
     __shared__ __align__(8) u64 full_bar;
@@ -111,11 +99,13 @@ rp_sweep_kernel(SweepArgs a, Digit dg)
     // issue the copy-engine loads of full tile `t` into the raw buffer (one lane)
     auto issue_tile = [&](u32 t) {
         const u64 r0 = (u64)t * T;
-        u32 bytes = (u32)SM::raw_keys + (BULK_VALS ? (u32)SM::raw_vals : 0u);
-        mbar_arrive_expect_tx(&full_bar, bytes);
-        if (AOS) bulk_g2s(raw_keys_b, (const u64 *)a.keys + 2 * r0, (u32)SM::raw_keys, &full_bar, pol);
-        else bulk_g2s(raw_keys_b, (const KeyT *)a.keys + r0, (u32)SM::raw_keys, &full_bar, pol);
-        if (BULK_VALS) bulk_g2s(raw_vals_b, (const u64 *)a.vals + r0, (u32)SM::raw_vals, &full_bar, pol);
+        mbar_arrive_expect_tx(&full_bar, (u32)SM::raw);
+        if (AOS) {
+            bulk_g2s(raw_keys_b, (const u64 *)a.keys + 2 * r0, (u32)SM::raw_keys, &full_bar, pol);
+        } else {
+            bulk_g2s(raw_keys_b, (const u64 *)a.keys + r0, (u32)SM::raw_keys, &full_bar, pol);
+            bulk_g2s(raw_vals_b, (const u64 *)a.vals + r0, (u32)SM::raw_vals, &full_bar, pol);
+        }
     };
     auto tile_is_full = [&](u32 t) { return (u64)(t + 1) * T <= n; };
 
@@ -142,7 +132,7 @@ rp_sweep_kernel(SweepArgs a, Digit dg)
         const u32 rows_here = full ? (u32)T : (u32)(n - row0);
 
         // ---- 1. this thread's K items: warp-striped, item i of lane l is tile row warp*32K + i*32 + l
-        KeyT key[K];
+        u64 key[K];
         u64 val[K];
         u32 dr[K];                      // digit | rank << 16   (digit 256 = row past the end)
         if (full) {
@@ -153,14 +143,12 @@ rp_sweep_kernel(SweepArgs a, Digit dg)
                 const u32 r = warp * (32 * K) + (u32)i * 32 + lane;
                 if (AOS) {
                     const ulonglong2 row = reinterpret_cast<const ulonglong2 *>(raw_keys_b)[r];
-                    key[i] = (KeyT)row.x; val[i] = row.y;
+                    key[i] = row.x; val[i] = row.y;
                 } else {
-                    key[i] = reinterpret_cast<const KeyT *>(raw_keys_b)[r];
-                    if (BULK_VALS) val[i] = reinterpret_cast<const u64 *>(raw_vals_b)[r];
-                    else if (VAL_AOS) val[i] = ld_stream_u64((const u64 *)a.vals + 2 * (row0 + r) + 1, pol);
-                    else val[i] = 0;
+                    key[i] = reinterpret_cast<const u64 *>(raw_keys_b)[r];
+                    val[i] = reinterpret_cast<const u64 *>(raw_vals_b)[r];
                 }
-                dr[i] = rp_digit<KeyT, DGM>(dg, key[i]);
+                dr[i] = rp_digit<u64, DGM>(dg, key[i]);
             }
             fence_proxy_async();         // generic-proxy reads of the raw buffer before the copy engine refills it
         } else {
@@ -171,8 +159,8 @@ rp_sweep_kernel(SweepArgs a, Digit dg)
                 dr[i] = SW_NB;
                 if (r < rows_here) {
                     Loader l{LDM, a.keys, a.vals, 0};
-                    rp_load<KeyT, LDM>(l, row0 + r, key[i], val[i], pol);
-                    dr[i] = rp_digit<KeyT, DGM>(dg, key[i]);
+                    rp_load<u64, LDM>(l, row0 + r, key[i], val[i], pol);
+                    dr[i] = rp_digit<u64, DGM>(dg, key[i]);
                 }
             }
         }
@@ -234,7 +222,7 @@ rp_sweep_kernel(SweepArgs a, Digit dg)
             if (d < SW_NB) {
                 const u32 pos = dbase[d] + cnt[warp * SW_NB + d] + (dr[i] >> 16);
                 st_keys[pos] = key[i];
-                if (HAS_VAL) st_vals[pos] = val[i];
+                st_vals[pos] = val[i];
                 st_dig[pos] = (unsigned char)d;
             }
         }
@@ -243,11 +231,11 @@ rp_sweep_kernel(SweepArgs a, Digit dg)
         __syncthreads();                                                        // B4: tile staged
         for (u32 i = lane; i < SW_NB / 2; i += 32) ((u32 *)my_cnt)[i] = 0;      // own counters: next tile's ranking
         __syncwarp();
-        KeyT *ok = (KeyT *)a.out_keys;
+        u64 *ok = (u64 *)a.out_keys;
         for (u32 p = tid; p < rows_here; p += SW_THREADS) {
             const u32 o = gbase[st_dig[p]] + p;
             ok[o] = st_keys[p];
-            if (HAS_VAL) a.out_vals[o] = st_vals[p];
+            a.out_vals[o] = st_vals[p];
         }
         // no barrier here: the staging buffer is rewritten only after the next tile's B3, dbase/gbase after its B2
     }
