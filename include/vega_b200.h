@@ -19,6 +19,8 @@
  *                             + PairRdd::join cross product       src/rdd/pair_rdd.rs:104-121
  *   vb_join_outer*         <- nothing: vega has no outer joins (Spark's left/right/full outer join, new)
  *   vb_cogroup*            <- CoGroupedRdd::compute for PairRdd::cogroup  src/rdd/co_grouped_rdd.rs:206-249
+ *   vb_cogroup_n* / vb_join_n*
+ *                          <- CoGroupedRdd::compute with any number of parents (co_grouped_rdd.rs:75-135, 206-249)
  *   vb_shuffle_free        <- (the reference never evicts SHUFFLE_CACHE, src/env.rs:27)
  *   vb_slice               <- ParallelCollection::slice           src/rdd/parallel_collection_rdd.rs:116-145
  *   vb_shuffle_export_* / vb_shuffle_import
@@ -312,6 +314,44 @@ VB_API int32_t vb_cogroup_size(vb_shuf *left, vb_shuf *right, uint32_t reduce_id
 VB_API int32_t vb_cogroup(vb_shuf *left, vb_shuf *right, uint32_t reduce_id, void *out_keys,
                           uint64_t *out_left_offsets /*n_keys+1*/, void *out_left_vals,
                           uint64_t *out_right_offsets /*n_keys+1*/, void *out_right_vals, int32_t dst_loc);
+
+/* CoGroupedRdd::compute with n_sides parents (src/rdd/co_grouped_rdd.rs:75-135, 206-249): partition reduce_id of the
+ * cogroup of sides[0 .. n_sides), as one key list with one CSR value list per side, in side order.
+ *   keys     every key that occurs on any side in the partition, exactly once; the order of keys within the partition
+ *            is unspecified.
+ *   lists    side j's list for a key is exactly the value list vb_shuffle_reduce of side j gives for it (map-id order,
+ *            then encounter order), and empty where side j lacks the key.
+ *   offsets  out_offsets[j] [n_keys + 1] is relative to the partition and starts at 0: key i's values on side j are
+ *            out_vals[j][out_offsets[j][i] .. [i + 1]).
+ * For n_sides = 2 the keys and lists are those of vb_cogroup(sides[0], sides[1]); for n_sides = 1 those of
+ * vb_shuffle_reduce(sides[0]).
+ * Argument rules: vb_cogroup's, for every side.  Each side is a sealed GROUP or COGROUP shuffle (the calls block until
+ * every side is sealed); all sides have the same n_reduce and key width and live on the same context; none is a
+ * string, multi-column or reduce-op shuffle; reduce_id < n_reduce; 1 <= n_sides <= VB_MAX_COGROUP_SIDES.  The same
+ * shuffle may appear more than once and then gives equal lists.  Anything else, including a NULL sides array or a NULL
+ * entry in it, is VB_ERR_INVALID.  A COGROUP side that was not grouped yet is grouped whole by these calls.
+ * vb_cogroup_n_size gives n_keys and the value count of every side (n_vals[n_sides]; NULL pointers skipped);
+ * vb_cogroup_n writes to dst_loc VB_HOST or VB_DEVICE and skips NULL outputs: out_offsets / out_vals themselves, or
+ * single entries in them.  The size call keeps the partition's plan on sides[0] for the write call, which frees it (so
+ * does vb_shuffle_free of sides[0]).  On a rank of a multi-rank shuffle only the partitions that rank owns have keys. */
+#define VB_MAX_COGROUP_SIDES 16
+VB_API int32_t vb_cogroup_n_size(vb_shuf *const *sides, uint32_t n_sides, uint32_t reduce_id, uint64_t *n_keys,
+                                 uint64_t *n_vals /*[n_sides], may be NULL*/);
+VB_API int32_t vb_cogroup_n(vb_shuf *const *sides, uint32_t n_sides, uint32_t reduce_id, void *out_keys,
+                            uint64_t *const *out_offsets /*[n_sides] arrays of n_keys+1*/,
+                            void *const *out_vals /*[n_sides]*/, int32_t dst_loc);
+
+/* Inner join of all sides, for one partition, with vb_cogroup_n's argument rules: a key on every side with lists
+ * l_0 .. l_{n-1} (each in cogroup order) gives prod |l_j| rows, contiguous, in the order
+ *   for v0 in l0 { for v1 in l1 { ... } } -> (k, v0, v1, ..., v_{n-1})
+ * (the last side varies fastest; for n_sides = 2 this is vb_join's per-key order).  A key missing on any side gives no
+ * rows; the order of keys within the partition is unspecified.  Row i is (out_k[i], out_vals[0][i], ...,
+ * out_vals[n_sides-1][i]).  Once the partition has rows, out_k, out_vals and every entry of it must be non-NULL
+ * (VB_ERR_INVALID).  A key's product, or the partition's total, of 2^63 rows or more is VB_ERR_TOO_LARGE from the size
+ * call.                                                                                                              */
+VB_API int32_t vb_join_n_size(vb_shuf *const *sides, uint32_t n_sides, uint32_t reduce_id, uint64_t *n_out);
+VB_API int32_t vb_join_n(vb_shuf *const *sides, uint32_t n_sides, uint32_t reduce_id, void *out_k,
+                         void *const *out_vals /*[n_sides]*/, int32_t dst_loc);
 
 /* ---- string keys: byte-string keys that hash like Rust `String` (reduce_by_key / count_by_key / count_by_value /
  *      distinct / group_by_key / partition_by_key over `String` keys, examples/group_by.rs, tests/test_pair_rdd.rs:8-37)

@@ -274,11 +274,77 @@ public:
         return out;
     }
 
+    // CoGroupedRdd::new([self, others...], HashPartitioner::new(num_splits)).collect()  →  Vec<(K, Vec<Vec<V>>)>
+    // (src/rdd/co_grouped_rdd.rs:75-135, 206-249): every key of any parent once, with one value list per parent in
+    // parent order (this one first); a parent that lacks the key has an empty list.
+    std::vector<std::pair<K, std::vector<std::vector<V>>>> cogroup_n(const std::vector<PairRddT> &others, size_t num_splits) const
+    {
+        auto shs = cogroup_shuffles(others, num_splits);
+        std::vector<vb_shuf *> sides;
+        for (auto &s : shs) sides.push_back(s.get());
+        const uint32_t n = (uint32_t)sides.size();
+        std::vector<std::pair<K, std::vector<std::vector<V>>>> out;
+        for (uint32_t r = 0; r < num_splits; ++r) {
+            uint64_t nk = 0;
+            std::vector<uint64_t> nv(n);
+            check(vb_cogroup_n_size(sides.data(), n, r, &nk, nv.data()));
+            std::vector<uint64_t> k(nk);
+            std::vector<std::vector<uint64_t>> offs(n, std::vector<uint64_t>(nk + 1)), vals(n);
+            std::vector<uint64_t *> op(n);
+            std::vector<void *> vp(n);
+            for (uint32_t j = 0; j < n; ++j) { vals[j].resize(nv[j]); op[j] = offs[j].data(); vp[j] = vals[j].data(); }
+            check(vb_cogroup_n(sides.data(), n, r, k.data(), op.data(), vp.data(), VB_HOST));
+            for (uint64_t i = 0; i < nk; ++i) {
+                std::vector<std::vector<V>> lists(n);
+                for (uint32_t j = 0; j < n; ++j)
+                    for (uint64_t x = offs[j][i]; x < offs[j][i + 1]; ++x) lists[j].push_back(detail::from_bits<V>(vals[j][x]));
+                out.emplace_back(detail::from_bits<K>(k[i]), std::move(lists));
+            }
+        }
+        return out;
+    }
+
+    // inner join of [self, others...]  →  (k, [v_0, ..., v_{n-1}]) per row: for a key on every parent,
+    // for v0 in vs_0 { for v1 in vs_1 { ... } }
+    std::vector<std::pair<K, std::vector<V>>> join_n(const std::vector<PairRddT> &others, size_t num_splits) const
+    {
+        auto shs = cogroup_shuffles(others, num_splits);
+        std::vector<vb_shuf *> sides;
+        for (auto &s : shs) sides.push_back(s.get());
+        const uint32_t n = (uint32_t)sides.size();
+        std::vector<std::pair<K, std::vector<V>>> out;
+        for (uint32_t r = 0; r < num_splits; ++r) {
+            uint64_t rows = 0;
+            check(vb_join_n_size(sides.data(), n, r, &rows));
+            std::vector<uint64_t> k(rows);
+            std::vector<std::vector<uint64_t>> vals(n, std::vector<uint64_t>(rows));
+            std::vector<void *> vp(n);
+            for (uint32_t j = 0; j < n; ++j) vp[j] = vals[j].data();
+            check(vb_join_n(sides.data(), n, r, k.data(), vp.data(), VB_HOST));
+            for (uint64_t i = 0; i < rows; ++i) {
+                std::vector<V> row(n);
+                for (uint32_t j = 0; j < n; ++j) row[j] = detail::from_bits<V>(vals[j][i]);
+                out.emplace_back(detail::from_bits<K>(k[i]), std::move(row));
+            }
+        }
+        return out;
+    }
+
     std::shared_ptr<Context> sc_;
     size_t num_slices_;
     std::vector<uint64_t> keys_, vals_;
 
 private:
+    // one COGROUP shuffle per parent: this one, then others in order
+    std::vector<detail::ShufPtr> cogroup_shuffles(const std::vector<PairRddT> &others, size_t num_splits) const
+    {
+        std::vector<detail::ShufPtr> shs;
+        shs.push_back(detail::run_shuffle<K>(*sc_, keys_, &vals_, num_slices_, num_splits, detail::dtype<V>::code, VB_AGG_COGROUP));
+        for (auto &o : others)
+            shs.push_back(detail::run_shuffle<K>(*sc_, o.keys_, &o.vals_, o.num_slices_, num_splits, detail::dtype<V>::code, VB_AGG_COGROUP));
+        return shs;
+    }
+
     // every row of vb_join_outer, partition by partition, as emit(k, v or nullopt, w or nullopt)
     template <typename W, typename Emit>
     void outer_join_rows(const PairRddT<K, W> &other, size_t num_splits, int32_t kind, Emit emit) const

@@ -152,6 +152,39 @@ pub fn join_partition(left_shuffle: usize, right_shuffle: usize, reduce_id: usiz
     Ok((0..n as usize).map(|i| (k[i], (v[i], w[i]))).collect())
 }
 
+// 5. cogroup of any number of parents — replaces CoGroupedRdd::compute (co_grouped_rdd.rs:206-249); each item has the
+//    shape of CoGroupedRdd::Item: (K, Vec<Vec<V>>), one list per parent in parent order
+pub fn cogroup_partition(shuffles: &[usize], reduce_id: usize) -> Result<Vec<(u64, Vec<Vec<u64>>)>> {
+    let sides: Vec<*mut sys::vb_shuf> = shuffles.iter().map(|&id| GPU.get(id)).collect();
+    let (n, r) = (sides.len(), reduce_id as u32);
+    let (mut nk, mut nv) = (0u64, vec![0u64; n]);
+    check(unsafe { sys::vb_cogroup_n_size(sides.as_ptr(), n as u32, r, &mut nk, nv.as_mut_ptr()) }).map_err(Error::from)?;
+    let mut k = vec![0u64; nk as usize];
+    let mut offs: Vec<Vec<u64>> = (0..n).map(|_| vec![0u64; nk as usize + 1]).collect();
+    let mut vals: Vec<Vec<u64>> = nv.iter().map(|&c| vec![0u64; c as usize]).collect();
+    let op: Vec<*mut u64> = offs.iter_mut().map(|o| o.as_mut_ptr()).collect();
+    let vp: Vec<*mut c_void> = vals.iter_mut().map(|v| v.as_mut_ptr() as *mut c_void).collect();
+    check(unsafe { sys::vb_cogroup_n(sides.as_ptr(), n as u32, r, k.as_mut_ptr() as *mut c_void, op.as_ptr(), vp.as_ptr(),
+                                     sys::VB_HOST) }).map_err(Error::from)?;
+    Ok((0..nk as usize)
+        .map(|i| (k[i], (0..n).map(|j| vals[j][offs[j][i] as usize..offs[j][i + 1] as usize].to_vec()).collect()))
+        .collect())
+}
+
+//    and the inner join of all parents: (k, [v_0, ..., v_{n-1}]) per row
+pub fn join_n_partition(shuffles: &[usize], reduce_id: usize) -> Result<Vec<(u64, Vec<u64>)>> {
+    let sides: Vec<*mut sys::vb_shuf> = shuffles.iter().map(|&id| GPU.get(id)).collect();
+    let (n, r) = (sides.len(), reduce_id as u32);
+    let mut rows = 0u64;
+    check(unsafe { sys::vb_join_n_size(sides.as_ptr(), n as u32, r, &mut rows) }).map_err(Error::from)?;
+    let mut k = vec![0u64; rows as usize];
+    let mut vals: Vec<Vec<u64>> = (0..n).map(|_| vec![0u64; rows as usize]).collect();
+    let vp: Vec<*mut c_void> = vals.iter_mut().map(|v| v.as_mut_ptr() as *mut c_void).collect();
+    check(unsafe { sys::vb_join_n(sides.as_ptr(), n as u32, r, k.as_mut_ptr() as *mut c_void, vp.as_ptr(), sys::VB_HOST) })
+        .map_err(Error::from)?;
+    Ok((0..rows as usize).map(|i| (k[i], (0..n).map(|j| vals[j][i]).collect())).collect())
+}
+
 // 2. "all map outputs registered" — src/scheduler/base_scheduler.rs:315 gains one line:
 //        self.map_output_tracker.register_map_outputs(shuffle_id, locs);
 //    +   crate::gpu::GPU.seal(shuffle_id);

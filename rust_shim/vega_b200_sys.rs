@@ -20,6 +20,7 @@ pub const VB_PART_HASH_METRO64: i32 = 0;
 pub const VB_HOST: i32 = 0;
 /// include/vega_b200.h `vb_join_kind` (vb_join_outer; the inner join is vb_join)
 pub const VB_JOIN_LEFT: i32 = 1; pub const VB_JOIN_RIGHT: i32 = 2; pub const VB_JOIN_FULL: i32 = 3;
+pub const VB_MAX_COGROUP_SIDES: usize = 16;
 
 #[link(name = "vega_b200")]
 extern "C" {
@@ -49,6 +50,15 @@ extern "C" {
     pub fn vb_cogroup(left: *mut vb_shuf, right: *mut vb_shuf, reduce_id: u32, out_keys: *mut c_void,
                       out_left_offsets: *mut u64, out_left_vals: *mut c_void, out_right_offsets: *mut u64,
                       out_right_vals: *mut c_void, dst_loc: i32) -> i32;
+    // CoGroupedRdd::compute with n_sides parents (1 ..= VB_MAX_COGROUP_SIDES): one CSR value list per side, and the
+    // inner join of all sides as (k, v_0, ..., v_{n-1}) rows
+    pub fn vb_cogroup_n_size(sides: *const *mut vb_shuf, n_sides: u32, reduce_id: u32, n_keys: *mut u64,
+                             n_vals: *mut u64) -> i32;
+    pub fn vb_cogroup_n(sides: *const *mut vb_shuf, n_sides: u32, reduce_id: u32, out_keys: *mut c_void,
+                        out_offsets: *const *mut u64, out_vals: *const *mut c_void, dst_loc: i32) -> i32;
+    pub fn vb_join_n_size(sides: *const *mut vb_shuf, n_sides: u32, reduce_id: u32, n_out: *mut u64) -> i32;
+    pub fn vb_join_n(sides: *const *mut vb_shuf, n_sides: u32, reduce_id: u32, out_k: *mut c_void,
+                     out_vals: *const *mut c_void, dst_loc: i32) -> i32;
     // N1: bincode blobs (the payload format of SHUFFLE_CACHE)
     pub fn vb_shuffle_reduce_blob_size(s: *mut vb_shuf, reduce_id: u32, n_bytes: *mut u64) -> i32;
     pub fn vb_shuffle_reduce_blob(s: *mut vb_shuf, reduce_id: u32, out_blob: *mut c_void, dst_loc: i32) -> i32;

@@ -18,7 +18,7 @@ ap = argparse.ArgumentParser()
 ap.add_argument("--rows", type=float, default=1e9)
 ap.add_argument("--distinct", type=float, default=1e6)
 ap.add_argument("--ops", default="reduce,group,sort,sortkv,join,count")   # also: zipf, zipfgroup, combine, combinezipf,
-#                                                                             leftjoin, fulljoin, cogroup
+#                                                                             leftjoin, fulljoin, cogroup, cogroup3, join3
 ap.add_argument("--reps", type=int, default=3)
 args = ap.parse_args()
 N, D = int(args.rows), int(args.distinct)
@@ -93,7 +93,7 @@ if "sort" in ops:
     report("sort_by_key(keys only)", N, 16.0 * N, timed(lambda: run_shuffle(L.VB_AGG_SORT, keys=keys), max(1, args.reps - 1)))
     del keys
     torch.cuda.empty_cache()
-join_ops = [o for o in ("join", "leftjoin", "fulljoin", "cogroup") if o in ops]
+join_ops = [o for o in ("join", "leftjoin", "fulljoin", "cogroup", "cogroup3", "join3") if o in ops]
 if join_ops:
     # BASELINE config 4, per-GPU share at 8 GPUs: 6.25e7 rows per side, each rank once per side,
     # 1.25e6 shared keys per GPU (1e7 / 8)
@@ -143,7 +143,7 @@ if "join" in ops:
     res = timed(join, max(1, args.reps - 1))
     assert res[-1][1]["join_rows"] == shared, (res[-1][1]["join_rows"], shared)
     report("join", 2 * n_side, 32.0 * n_side + 24.0 * shared, res, {"join_rows": shared})
-if "leftjoin" in ops or "fulljoin" in ops or "cogroup" in ops:
+if "leftjoin" in ops or "fulljoin" in ops or "cogroup" in ops or "cogroup3" in ops:
     # Each outer join against the inner join of the same inputs and against the workaround without outer joins:
     # materialising the cogroup of both sides (vb_shuffle_reduce of every partition, device output), which the
     # caller then still has to expand.  All outputs stay on the device.
@@ -216,6 +216,112 @@ if "leftjoin" in ops or "fulljoin" in ops or "cogroup" in ops:
         extra = {"gpu": card["name"], "power_limit_w": card["power_limit_w"], "cogroup_keys": want,
                  "cogroup_both_sides_ms": round(med(r_cog), 3)}
         report("cogroup", 2 * n_side, 32.0 * n_side + 24.0 * want, res, extra)
+if "cogroup3" in ops or "join3" in ops:
+    # The join shape with a third side that shares the same 2 % of the keys (its other keys are on no other side), 8 -> 8,
+    # device outputs.  vb_cogroup_n of 3 sides against the grouping alone (vb_shuffle_reduce of every partition of the 3
+    # sides); vb_cogroup_n of 2 sides against vb_cogroup of the same pair; vb_join_n of 3 sides against vb_join of 2.
+    from bench import gpu_info
+    card = gpu_info(0)
+    p = lambda t: ctypes.c_void_p(t.data_ptr()) if t.numel() else None
+    dev = lambda n: torch.empty(n, dtype=torch.int64, device="cuda")
+    c = torch.empty((n_side, 2), dtype=torch.int64, device="cuda")
+    sc.gen_pairs(out_rows=c[:shared], first=0, n=shared, mode="unique", rank_base=n_side - shared)
+    sc.gen_pairs(out_rows=c[shared:], first=shared, n=n_side - shared, mode="unique", rank_base=2 * n_side - shared)
+    torch.cuda.synchronize()
+
+    def sides_of(ts):
+        shs = []
+        for t in ts:
+            s_ = vb.Shuffle(sc, 8, 8, L.VB_U64, L.VB_U64, L.VB_AGG_COGROUP)
+            col = vb.rdd._Col(t, allow_rows=True)
+            st = vb.slice_starts(col.n, 8)
+            for m in range(8):
+                s_.map(m, col, None, int(st[m]), int(st[m + 1]))
+            s_.seal()
+            shs.append(s_)
+        return shs
+
+    def finish(shs, **extra):
+        st = shs[0].stats()          # kernel times and launches of every side, summed
+        for s_ in shs[1:]:
+            o = s_.stats()
+            for kk in st["kernels"]:
+                st["kernels"][kk]["ms"] += o["kernels"][kk]["ms"]; st["kernels"][kk]["launches"] += o["kernels"][kk]["launches"]
+            st["kernel_launches"] += o["kernel_launches"]
+        st.update(extra)
+        for s_ in shs:
+            s_.free()
+        return st
+
+    def group_only(ts):
+        def run():
+            shs = sides_of(ts)
+            for r in range(8):
+                for s_ in shs:
+                    nk, nv = ctypes.c_uint64(), ctypes.c_uint64()
+                    L.check(sc._lib.vb_shuffle_reduce_size(s_._h, r, ctypes.byref(nk), ctypes.byref(nv)))
+                    k, o, v = dev(nk.value), dev(nk.value + 1), dev(nv.value)
+                    L.check(sc._lib.vb_shuffle_reduce(s_._h, r, p(k), None, p(o), p(v), L.VB_DEVICE))
+            return finish(shs)
+        return run
+
+    def cogroup_n(ts):
+        def run():
+            shs = sides_of(ts)
+            n = len(shs)
+            arr = (ctypes.c_void_p * n)(*[s_._h.value for s_ in shs])
+            tot = 0
+            for r in range(8):
+                nk, nv = ctypes.c_uint64(), (ctypes.c_uint64 * n)()
+                L.check(sc._lib.vb_cogroup_n_size(arr, n, r, ctypes.byref(nk), nv))
+                k = dev(nk.value)
+                offs = [dev(nk.value + 1) for _ in range(n)]
+                vals = [dev(nv[j]) for j in range(n)]
+                L.check(sc._lib.vb_cogroup_n(arr, n, r, p(k), (ctypes.c_void_p * n)(*[p(x) for x in offs]),
+                                             (ctypes.c_void_p * n)(*[p(x) for x in vals]), L.VB_DEVICE))
+                tot += nk.value
+            return finish(shs, cogroup_keys=tot)
+        return run
+
+    def join_n(ts):
+        def run():
+            shs = sides_of(ts)
+            n = len(shs)
+            arr = (ctypes.c_void_p * n)(*[s_._h.value for s_ in shs])
+            tot = 0
+            for r in range(8):
+                nn = ctypes.c_uint64()
+                L.check(sc._lib.vb_join_n_size(arr, n, r, ctypes.byref(nn)))
+                k, vs = dev(nn.value), [dev(nn.value) for _ in range(n)]
+                L.check(sc._lib.vb_join_n(arr, n, r, p(k), (ctypes.c_void_p * n)(*[p(x) for x in vs]), L.VB_DEVICE))
+                tot += nn.value
+            return finish(shs, join_rows=tot)
+        return run
+
+    med = lambda r: sorted(x[0] for x in r)[len(r) // 2]
+    info = {"gpu": card["name"], "power_limit_w": card["power_limit_w"]}
+    rows3 = 3 * n_side
+    if "cogroup3" in ops:
+        keys3 = 3 * n_side - 2 * shared
+        r_group = timed(group_only([a, b, c]), args.reps)
+        res = timed(cogroup_n([a, b, c]), args.reps)
+        assert res[-1][1]["cogroup_keys"] == keys3, (res[-1][1]["cogroup_keys"], keys3)
+        # algorithmic bytes: the input rows (16 B), then per output key the key and one offset per side, and every value
+        report("cogroup_n 3 sides", rows3, 16.0 * rows3 + (8.0 + 3 * 8.0) * keys3 + 8.0 * rows3, res,
+               dict(info, cogroup_keys=keys3, group_3_sides_ms=round(med(r_group), 3)))
+        keys2 = 2 * n_side - shared
+        r_two = timed(cogroup, args.reps)
+        res = timed(cogroup_n([a, b]), args.reps)
+        assert res[-1][1]["cogroup_keys"] == keys2, (res[-1][1]["cogroup_keys"], keys2)
+        report("cogroup_n 2 sides", 2 * n_side, 16.0 * 2 * n_side + (8.0 + 2 * 8.0) * keys2 + 8.0 * 2 * n_side, res,
+               dict(info, cogroup_keys=keys2, vb_cogroup_ms=round(med(r_two), 3)))
+    if "join3" in ops:
+        r_two = timed(join, args.reps)
+        res = timed(join_n([a, b, c]), args.reps)
+        assert res[-1][1]["join_rows"] == shared, (res[-1][1]["join_rows"], shared)
+        report("join_n 3 sides", rows3, 16.0 * rows3 + 8.0 * 4 * shared, res, dict(info, join_rows=shared, vb_join_2_sides_ms=round(med(r_two), 3)))
+    del c
+    torch.cuda.empty_cache()
 if "combine" in ops or "combinezipf" in ops:
     # combine_by_key: sum(v0), min(v1), max(v1), mean(v2), count in one shuffle (5 accumulators) against the baseline a
     # user has without it, one single-column shuffle per aggregate (the mean from a sum and the count).  v0 is gen_pairs'

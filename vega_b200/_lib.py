@@ -19,6 +19,7 @@ VB_HOST, VB_DEVICE, VB_DEVICE_BORROWED = 0, 1, 2
 VB_GEN_UNIFORM, VB_GEN_ZIPF, VB_GEN_UNIQUE = 0, 1, 2
 VB_XCHG_AUTO, VB_XCHG_NCCL, VB_XCHG_P2P = 0, 1, 2
 VB_JOIN_LEFT, VB_JOIN_RIGHT, VB_JOIN_FULL = 1, 2, 3
+VB_MAX_COGROUP_SIDES = 16
 VB_UNIQUE_ID_BYTES = 128
 
 KERNEL_CLASSES = ["hash_agg", "dict", "merge", "rp_hist", "rp_scan", "rp_scatter", "misc", "join"]
@@ -96,6 +97,10 @@ SYMBOLS = {
     "vb_join_outer": (_i32, [_vp, _vp, _u32, _i32, _vp, _vp, _vp, _vp, _vp, _i32]),
     "vb_cogroup_size": (_i32, [_vp, _vp, _u32, _pu64, _pu64, _pu64]),
     "vb_cogroup": (_i32, [_vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _i32]),
+    "vb_cogroup_n_size": (_i32, [_pvp, _u32, _u32, _pu64, _pu64]),
+    "vb_cogroup_n": (_i32, [_pvp, _u32, _u32, _vp, _pvp, _pvp, _i32]),
+    "vb_join_n_size": (_i32, [_pvp, _u32, _u32, _pu64]),
+    "vb_join_n": (_i32, [_pvp, _u32, _u32, _vp, _pvp, _i32]),
     "vb_shuffle_create_str": (_i32, [_vp, _u64, _u32, _u32, _i32, _i32, _pvp]),
     "vb_shuffle_map_str": (_i32, [_vp, _u32, _vp, _vp, _u64, _vp, _u64, _i32]),
     "vb_shuffle_reduce_str_size": (_i32, [_vp, _u32, _pu64, _pu64, _pu64]),

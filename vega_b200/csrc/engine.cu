@@ -295,6 +295,17 @@ struct CogroupPlan {
     u64 *ro_keys = nullptr, *ro_pos = nullptr;   // [n_ro] the right-only keys and their right-value positions
 };
 
+// vb_cogroup_n_size / vb_join_n_size's result for one (sides, partition), kept for the write call.  Cogroup output
+// keys: side 0's keys in its CSR order, then each later side's new keys (those no earlier side has) in that side's CSR
+// order.  A join reads side 0's keys only.
+struct CogroupNPlan {
+    u64 n_keys = 0;                // cogroup: output keys; join: side 0's keys of the partition
+    u64 *new_keys = nullptr;       // cogroup: [n_keys - side 0's keys] the keys after side 0's
+    u32 *match = nullptr;          // [n_keys][n_sides] the key's index on every side, 0xFFFFFFFF where a side lacks it
+    u64 *pos = nullptr;            // join: [n_keys] each key's first output row
+    u64 total = 0;                 // join: rows of the partition
+};
+
 struct vb_shuf {
     vb_ctx *ctx = nullptr;
     u64 id = 0;
@@ -353,6 +364,8 @@ struct vb_shuf {
     u32 *dense_of_slot = nullptr;
     std::map<std::tuple<const vb_shuf *, u32, int>, JoinPlan> join_plans;   // by (right side, partition, join kind)
     std::map<std::pair<const vb_shuf *, u32>, CogroupPlan> cogroup_plans;   // by (right side, partition)
+    // on side 0 of an N-way cogroup / join: by (every side's uid, partition, join?)
+    std::map<std::tuple<std::vector<u64>, u32, bool>, CogroupNPlan> n_plans;
     // COGROUP shuffles are grouped lazily: seal keeps the (owned) rows; the CSR is built by the first reduce call
     // (cogroup materialisation), or — if a join comes first — only for the rows the join kind needs: the keys on BOTH
     // sides (inner), every row of the preserved side plus the matching rows of the other (LEFT / RIGHT), or all (FULL).
@@ -3522,6 +3535,286 @@ extern "C" int32_t vb_cogroup(vb_shuf *l, vb_shuf *r, uint32_t rid, void *out_ke
 }
 
 // ---------------------------------------------------------------------------------------------
+// N-way cogroup and inner join (CoGroupedRdd::compute with n parents, co_grouped_rdd.rs:206-249)
+// Every side is grouped whole.  Side i's keys are probed against every other side's dictionary by one launch per side
+// (all sides' tables in one parameter struct): a key no earlier side has is new, and its row of the match matrix
+// records its index on every side.  The output keys are side 0's, then each later side's new keys taken by the stable
+// compaction; side j's lists are its value segments gathered into output key order.  The join reads side 0's rows of
+// the matrix only: the keys on every side are exactly the side-0 keys without a 0xFFFFFFFF.
+// ---------------------------------------------------------------------------------------------
+static_assert(CGN_MAX_SIDES == VB_MAX_COGROUP_SIDES, "cogroup side limit");
+
+static void free_cogroup_n_plan(vb_ctx *c, CogroupNPlan &p)
+{
+    dev_free(c, p.new_keys); dev_free(c, p.match); dev_free(c, p.pos);
+}
+
+// vb_cogroup's argument rules for every side; waits until every side is sealed
+static int cogroup_n_check(vb_shuf *const *sides, u32 n, u32 rid)
+{
+    if (!sides) return set_err(VB_ERR_INVALID, "sides is NULL");
+    if (n < 1 || n > VB_MAX_COGROUP_SIDES) return set_err(VB_ERR_INVALID, "n_sides %u is not in [1, %d]", n, VB_MAX_COGROUP_SIDES);
+    for (u32 j = 0; j < n; ++j) {
+        const vb_shuf *s = sides[j];
+        if (!s) return set_err(VB_ERR_INVALID, "side %u is NULL", j);
+        if (s->str) return invalid_str(s, "a join or cogroup");
+        if (!is_group_op(s->agg)) return set_err(VB_ERR_INVALID, "side %u is not a GROUP/COGROUP shuffle", j);
+        if (s->n_reduce != sides[0]->n_reduce || s->key_width != sides[0]->key_width)
+            return set_err(VB_ERR_INVALID, "side %u uses a different partitioner than side 0", j);
+        if (s->ctx != sides[0]->ctx) return set_err(VB_ERR_INVALID, "side %u lives on a different context than side 0", j);
+    }
+    if (rid >= sides[0]->n_reduce) return set_err(VB_ERR_INVALID, "reduce_id %u >= n_reduce %u", rid, sides[0]->n_reduce);
+    for (u32 j = 0; j < n; ++j) TRY(wait_sealed(sides[j]));
+    return VB_OK;
+}
+
+// group every side (caller holds the context lock) and describe them for the kernels
+static int cogroup_n_sides(vb_shuf *const *sides, u32 n, u32 rid, CogroupNSides *a)
+{
+    *a = CogroupNSides{};
+    a->n = n;
+    for (u32 j = 0; j < n; ++j) {
+        vb_shuf *s = sides[j];
+        TRY(ensure_grouped(s));
+        if (s->n_keys && !s->dict) return set_err(VB_ERR_STATE, "cogroup side without a key dictionary");
+        a->tab[j] = table_at(s->n_keys ? s->dict : nullptr, s->dict_log_cap);
+        a->dense[j] = s->dense_of_slot;
+        a->keys[j] = s->res_keys; a->offs[j] = s->res_offs; a->vals[j] = s->res_vals;
+        a->kb[j] = (u32)s->bucket_off[rid];
+    }
+    return VB_OK;
+}
+
+static int cogroup_n_plan(vb_shuf *const *sides, u32 n, u32 rid, bool join, const CogroupNSides &a, CogroupNPlan **out)
+{
+    vb_shuf *s0 = sides[0];
+    vb_ctx *c = s0->ctx;
+    std::vector<u64> uids(n);
+    for (u32 j = 0; j < n; ++j) uids[j] = sides[j]->uid;
+    auto key = std::make_tuple(uids, rid, join);
+    auto it = s0->n_plans.find(key);
+    if (it != s0->n_plans.end()) { *out = &it->second; return VB_OK; }
+    std::vector<u64> nk(n);
+    u64 cap = 0;                                       // output keys at most
+    for (u32 j = 0; j < n && (j == 0 || !join); ++j) {
+        nk[j] = sides[j]->bucket_off[rid + 1] - sides[j]->bucket_off[rid];
+        cap += nk[j];
+    }
+    if (cap >= 0xFFFFFFFFull) return set_err(VB_ERR_TOO_LARGE, "%llu keys in one cogroup partition", (unsigned long long)cap);
+    CogroupNPlan p;
+    DevBuf match(c), new_keys(c), pos(c);
+    TRY(match.alloc(cap * n * 4));
+    if (nk[0]) {
+        KLaunch kl(s0, K_JOIN);
+        cogroup_n_probe_kernel<<<(unsigned)((nk[0] + 255) / 256), 256, 0, c->stream>>>(a, 0, (u32)nk[0], match.as<u32>(), nullptr, nullptr);
+        TRY(kl.done("cogroup_n_probe_kernel"));
+    }
+    p.n_keys = nk[0];
+    if (!join && cap > nk[0]) {
+        TRY(new_keys.alloc((cap - nk[0]) * 8));
+        for (u32 i = 1; i < n; ++i) {
+            if (!nk[i]) continue;
+            DevBuf rows(c), flag(c), lidx(c), ok(c), ov(c);
+            TRY(rows.alloc(nk[i] * n * 4)); TRY(flag.alloc(nk[i])); TRY(lidx.alloc(nk[i] * 8));
+            {
+                KLaunch kl(s0, K_JOIN);
+                cogroup_n_probe_kernel<<<(unsigned)((nk[i] + 255) / 256), 256, 0, c->stream>>>(a, i, (u32)nk[i], rows.as<u32>(),
+                                                                                              flag.as<unsigned char>(), lidx.as<u64>());
+                TRY(kl.done("cogroup_n_probe_kernel"));
+            }
+            u64 m = 0;
+            TRY(compact_rows(s0, sides[i]->res_keys + a.kb[i], lidx.as<u64>(), nk[i], flag.as<unsigned char>(), ok, ov, &m));
+            if (!m) continue;
+            {
+                KLaunch kl(s0, K_JOIN);
+                const u64 blocks = std::min<u64>((m * n + 255) / 256, (u64)c->sm_count * 8);
+                cogroup_n_take_rows_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(rows.as<u32>(), n, ov.as<u64>(), m,
+                                                                                    match.as<u32>() + p.n_keys * n);
+                TRY(kl.done("cogroup_n_take_rows_kernel"));
+            }
+            CU(cudaMemcpyAsync(new_keys.as<u64>() + (p.n_keys - nk[0]), ok.p, m * 8, cudaMemcpyDeviceToDevice, c->stream));
+            p.n_keys += m;
+        }
+    }
+    if (join && p.n_keys) {
+        DevBuf cnt(c), flags(c);
+        TRY(cnt.alloc(p.n_keys * 8)); TRY(pos.alloc(p.n_keys * 8)); TRY(flags.alloc(24));
+        CU(cudaMemsetAsync(flags.p, 0, 24, c->stream));
+        unsigned long long *sums = flags.as<unsigned long long>();
+        u32 *too_large = (u32 *)(sums + 2);
+        {
+            KLaunch kl(s0, K_JOIN);
+            join_n_count_kernel<<<(unsigned)((p.n_keys + 255) / 256), 256, 0, c->stream>>>(a, match.as<u32>(), (u32)p.n_keys,
+                                                                                          cnt.as<u64>(), sums, too_large);
+            TRY(kl.done("join_n_count_kernel"));
+        }
+        TRY(exclusive_scan_u64(s0, cnt.as<u64>(), pos.as<u64>(), p.n_keys, nullptr));
+        u64 *h = (u64 *)c->h_scratch;
+        CU(cudaMemcpyAsync(h, flags.p, 24, cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaStreamSynchronize(c->stream));
+        const unsigned __int128 total = ((unsigned __int128)h[0] << 32) + h[1];
+        if (*(u32 *)(h + 2) || total >> 63)
+            return set_err(VB_ERR_TOO_LARGE, "partition %u of the join has 2^63 rows or more", rid);
+        p.total = (u64)total;
+    }
+    CU(cudaStreamSynchronize(c->stream));
+    p.match = (u32 *)match.release();
+    p.new_keys = (u64 *)new_keys.release();
+    p.pos = (u64 *)pos.release();
+    *out = &s0->n_plans.emplace(key, p).first->second;
+    return VB_OK;
+}
+
+static void drop_cogroup_n_plan(vb_shuf *const *sides, u32 n, u32 rid, bool join)
+{
+    std::vector<u64> uids(n);
+    for (u32 j = 0; j < n; ++j) uids[j] = sides[j]->uid;
+    auto it = sides[0]->n_plans.find(std::make_tuple(uids, rid, join));
+    if (it == sides[0]->n_plans.end()) return;
+    free_cogroup_n_plan(sides[0]->ctx, it->second);
+    sides[0]->n_plans.erase(it);
+}
+
+extern "C" int32_t vb_cogroup_n_size(vb_shuf *const *sides, uint32_t n_sides, uint32_t rid, uint64_t *n_keys, uint64_t *n_vals)
+{
+    TRY(cogroup_n_check(sides, n_sides, rid));
+    vb_ctx *c = sides[0]->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    CogroupNSides a;
+    TRY(cogroup_n_sides(sides, n_sides, rid, &a));
+    CogroupNPlan *p = nullptr;
+    TRY(cogroup_n_plan(sides, n_sides, rid, false, a, &p));
+    if (n_keys) *n_keys = p->n_keys;
+    for (u32 j = 0; n_vals && j < n_sides; ++j) n_vals[j] = sides[j]->val_off[rid + 1] - sides[j]->val_off[rid];
+    return VB_OK;
+}
+
+extern "C" int32_t vb_cogroup_n(vb_shuf *const *sides, uint32_t n_sides, uint32_t rid, void *out_keys,
+                                uint64_t *const *out_offsets, void *const *out_vals, int32_t dst_loc)
+{
+    TRY(cogroup_n_check(sides, n_sides, rid));
+    if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
+    vb_shuf *s0 = sides[0];
+    vb_ctx *c = s0->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    CogroupNSides a;
+    TRY(cogroup_n_sides(sides, n_sides, rid, &a));
+    CogroupNPlan *p = nullptr;
+    TRY(cogroup_n_plan(sides, n_sides, rid, false, a, &p));
+    const u64 nk = p->n_keys, nk0 = s0->bucket_off[rid + 1] - s0->bucket_off[rid];
+    int rc = [&]() -> int {
+        TRY(copy_out(s0, out_keys, s0->res_keys ? s0->res_keys + a.kb[0] : nullptr, nk0 * 8, dst_loc));
+        TRY(copy_out(s0, out_keys ? (u64 *)out_keys + nk0 : nullptr, p->new_keys, (nk - nk0) * 8, dst_loc));
+        for (u32 j = 0; j < n_sides; ++j) {
+            u64 *o_offs = out_offsets ? out_offsets[j] : nullptr;
+            void *o_vals = out_vals ? out_vals[j] : nullptr;
+            if (!o_offs && !o_vals) continue;
+            vb_shuf *s = sides[j];
+            const u64 nv = s->val_off[rid + 1] - s->val_off[rid];
+            // side j's list offsets: the list lengths of the output keys, scanned (on the device even for a host output)
+            DevBuf pos(c), cnt(c);
+            u64 *d_pos = (o_offs && dst_loc == VB_DEVICE) ? o_offs : nullptr;
+            if (!d_pos) { TRY(pos.alloc((nk + 1) * 8)); d_pos = pos.as<u64>(); }
+            if (nk == 0) {
+                CU(cudaMemsetAsync(d_pos, 0, 8, c->stream));
+            } else {
+                TRY(cnt.alloc(nk * 8));
+                {
+                    KLaunch kl(s0, K_JOIN);
+                    cogroup_n_count_kernel<<<(unsigned)((nk + 255) / 256), 256, 0, c->stream>>>(p->match, n_sides, j, (u32)nk,
+                                                                                                s->res_offs, cnt.as<u64>());
+                    TRY(kl.done("cogroup_n_count_kernel"));
+                }
+                TRY(exclusive_scan_u64(s0, cnt.as<u64>(), d_pos, nk, d_pos + nk));
+            }
+            if (o_offs && dst_loc == VB_HOST) TRY(copy_out(s0, o_offs, d_pos, (nk + 1) * 8, VB_HOST));
+            if (!o_vals || !nv) continue;
+            if (j == 0) {                                  // side 0's lists are its partition's value slice as it is
+                TRY(copy_out(s0, o_vals, s->res_vals + s->val_off[rid], nv * 8, dst_loc));
+                continue;
+            }
+            DevBuf tmp(c);
+            u64 *d = (u64 *)o_vals;
+            if (dst_loc == VB_HOST) { TRY(tmp.alloc(nv * 8)); d = tmp.as<u64>(); }
+            {
+                KLaunch kl(s0, K_JOIN);
+                const u64 blocks = std::min<u64>((nv + 255) / 256, (u64)c->sm_count * 8);
+                cogroup_n_gather_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(d_pos, (u32)nk, p->match, n_sides, j,
+                                                                                s->res_offs, s->res_vals, d);
+                TRY(kl.done("cogroup_n_gather_kernel"));
+            }
+            if (dst_loc == VB_HOST) TRY(copy_out(s0, o_vals, d, nv * 8, VB_HOST));
+        }
+        return VB_OK;
+    }();
+    cudaStreamSynchronize(c->stream);
+    drop_cogroup_n_plan(sides, n_sides, rid, false);
+    return rc;
+}
+
+extern "C" int32_t vb_join_n_size(vb_shuf *const *sides, uint32_t n_sides, uint32_t rid, uint64_t *n_out)
+{
+    TRY(cogroup_n_check(sides, n_sides, rid));
+    if (!n_out) return set_err(VB_ERR_INVALID, "n_out is NULL");
+    vb_ctx *c = sides[0]->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    CogroupNSides a;
+    TRY(cogroup_n_sides(sides, n_sides, rid, &a));
+    CogroupNPlan *p = nullptr;
+    TRY(cogroup_n_plan(sides, n_sides, rid, true, a, &p));
+    *n_out = p->total;
+    return VB_OK;
+}
+
+extern "C" int32_t vb_join_n(vb_shuf *const *sides, uint32_t n_sides, uint32_t rid, void *out_k, void *const *out_vals,
+                             int32_t dst_loc)
+{
+    TRY(cogroup_n_check(sides, n_sides, rid));
+    if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
+    vb_shuf *s0 = sides[0];
+    vb_ctx *c = s0->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    CogroupNSides a;
+    TRY(cogroup_n_sides(sides, n_sides, rid, &a));
+    CogroupNPlan *p = nullptr;
+    TRY(cogroup_n_plan(sides, n_sides, rid, true, a, &p));
+    const u64 total = p->total;
+    int rc = [&]() -> int {
+        if (!total) return VB_OK;
+        bool missing = !out_k || !out_vals;
+        for (u32 j = 0; !missing && j < n_sides; ++j) missing = !out_vals[j];
+        if (missing) return set_err(VB_ERR_INVALID, "NULL output with %llu rows to write", (unsigned long long)total);
+        JoinNOut o{};
+        DevBuf bufs[CGN_MAX_SIDES + 1];
+        o.k = (u64 *)out_k;
+        for (u32 j = 0; j < n_sides; ++j) o.v[j] = (u64 *)out_vals[j];
+        if (dst_loc == VB_HOST) {
+            for (u32 j = 0; j <= n_sides; ++j) { bufs[j].c = c; TRY(bufs[j].alloc(total * 8)); }
+            o.k = bufs[n_sides].as<u64>();
+            for (u32 j = 0; j < n_sides; ++j) o.v[j] = bufs[j].as<u64>();
+        }
+        {
+            KLaunch kl(s0, K_JOIN);
+            const u64 blocks = std::min<u64>((total + 255) / 256, (u64)c->sm_count * 8);
+            join_n_expand_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(a, p->pos, (u32)p->n_keys, total, p->match, o);
+            TRY(kl.done("join_n_expand_kernel"));
+        }
+        if (dst_loc == VB_HOST) {
+            TRY(copy_out(s0, out_k, o.k, total * 8, VB_HOST));
+            for (u32 j = 0; j < n_sides; ++j) TRY(copy_out(s0, out_vals[j], o.v[j], total * 8, VB_HOST));
+        }
+        return VB_OK;
+    }();
+    cudaStreamSynchronize(c->stream);
+    drop_cogroup_n_plan(sides, n_sides, rid, true);
+    return rc;
+}
+
+// ---------------------------------------------------------------------------------------------
 // string keys (vb_shuffle_create_str): byte-string keys placed like the reference's `String` keys
 // ---------------------------------------------------------------------------------------------
 // One shuffle's dictionary of distinct keys (strkeys.cuh: entries + arena + index), the map calls' rows as entry ids,
@@ -4078,6 +4371,7 @@ extern "C" int32_t vb_shuffle_free(vb_shuf *s)
         dev_free(c, s->dict); dev_free(c, s->dense_of_slot);
         for (auto &kv : s->join_plans) { dev_free(c, kv.second.pos); dev_free(c, kv.second.match); }
         for (auto &kv : s->cogroup_plans) free_cogroup_plan(c, kv.second);
+        for (auto &kv : s->n_plans) free_cogroup_n_plan(c, kv.second);
         free_lazy_rows(s);
         free_str(s);
         cudaStreamSynchronize(c->stream);

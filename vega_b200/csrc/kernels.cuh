@@ -1690,6 +1690,149 @@ __global__ void cogroup_gather_right_kernel(const u64 *__restrict__ pos, u32 n, 
 }
 
 // ---------------------------------------------------------------------------------------------
+// N-way cogroup and inner join (CoGroupedRdd::compute with n parents).  The output keys are side 0's keys, then each
+// later side's new keys (those no earlier side has).  match is key-major: row o holds output key o's index on every
+// side (a global key index of that side's CSR), 0xFFFFFFFF where the side lacks the key.
+// ---------------------------------------------------------------------------------------------
+constexpr u32 CGN_MAX_SIDES = 16;
+struct CogroupNSides {
+    Table tab[CGN_MAX_SIDES];            // key dictionaries; keys NULL: the side has no rows
+    const u32 *dense[CGN_MAX_SIDES];     // dictionary slot -> key index
+    const u64 *keys[CGN_MAX_SIDES];      // CSR keys, offsets and values (res_*)
+    const u64 *offs[CGN_MAX_SIDES];
+    const u64 *vals[CGN_MAX_SIDES];
+    u32 kb[CGN_MAX_SIDES];               // the partition's first key on each side
+    u32 n;
+};
+struct JoinNOut {
+    u64 *k;
+    u64 *v[CGN_MAX_SIDES];
+};
+
+// Keys [kb_i, kb_i + nk) of side i: row t = the key's index on every side (its own: kb_i + t).  Side i > 0 sets
+// flag[t] = 1 and lidx[t] = t for a key no side j < i has, and leaves the row of any other key unfinished: only the
+// rows of new keys are used.
+__global__ void cogroup_n_probe_kernel(const __grid_constant__ CogroupNSides a, u32 i, u32 nk, u32 *__restrict__ rows,
+                                       unsigned char *__restrict__ flag, u64 *__restrict__ lidx)
+{
+    const u32 t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= nk) return;
+    const u64 key = a.keys[i][a.kb[i] + t];
+    for (u32 j = 0; j < a.n; ++j) {
+        u32 m = a.kb[i] + t;
+        if (j != i) {
+            const u32 s = a.tab[j].keys ? table_find(a.tab[j], key) : 0xFFFFFFFFu;
+            m = s != 0xFFFFFFFFu ? a.dense[j][s] : 0xFFFFFFFFu;
+        }
+        if (j < i && m != 0xFFFFFFFFu) { flag[t] = 0; return; }     // an earlier side already gave this key
+        rows[(u64)t * a.n + j] = m;
+    }
+    if (i) { flag[t] = 1; lidx[t] = t; }
+}
+
+// out[o] = row lidx[o] of rows (n entries per row) for the m new keys of a side, in output order
+__global__ void cogroup_n_take_rows_kernel(const u32 *__restrict__ rows, u32 n, const u64 *__restrict__ lidx, u64 m,
+                                           u32 *__restrict__ out)
+{
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 e = (u64)blockIdx.x * blockDim.x + threadIdx.x; e < m * n; e += stride) {
+        const u64 o = e / n;
+        out[e] = rows[lidx[o] * n + (e - o * n)];
+    }
+}
+
+// cnt[o] = the length of output key o's list on side j (0 where the side lacks the key)
+__global__ void cogroup_n_count_kernel(const u32 *__restrict__ match, u32 n, u32 j, u32 nk, const u64 *__restrict__ offs,
+                                       u64 *__restrict__ cnt)
+{
+    const u32 o = blockIdx.x * blockDim.x + threadIdx.x;
+    if (o >= nk) return;
+    const u32 m = match[(u64)o * n + j];
+    cnt[o] = m != 0xFFFFFFFFu ? offs[m + 1] - offs[m] : 0;
+}
+
+// Side j's values in output key order, one thread per value: value o belongs to the largest key index k with
+// pos[k] <= o (keys with an empty list share pos with the next key), and its source segment is side j's key match[k][j].
+// The values written are the ones the scanned lengths cover (pos[nk]), so no thread reads past a segment even if the key
+// list missed a key of the side.
+__global__ void cogroup_n_gather_kernel(const u64 *__restrict__ pos, u32 nk, const u32 *__restrict__ match, u32 n, u32 j,
+                                        const u64 *__restrict__ offs, const u64 *__restrict__ vals, u64 *__restrict__ out)
+{
+    const u64 stride = (u64)gridDim.x * blockDim.x, total = pos[nk];
+    for (u64 o = (u64)blockIdx.x * blockDim.x + threadIdx.x; o < total; o += stride) {
+        u32 lo = 0, hi = nk;
+        while (hi - lo > 1) {
+            const u32 mid = (lo + hi) >> 1;
+            if (pos[mid] <= o) lo = mid; else hi = mid;
+        }
+        out[o] = vals[offs[match[(u64)lo * n + j]] + (o - pos[lo])];
+    }
+}
+
+// Inner join, side 0's keys o < nk: cnt[o] = the product of the key's list lengths over all sides, 0 when a side lacks
+// the key.  A product of 2^63 or more sets *too_large (cnt 0).  sums[0] / sums[1] accumulate the sum of cnt >> 32 and
+// of cnt & 0xFFFFFFFF, so the host can tell an exact partition total of 2^63 or more from a wrapped one.
+__global__ void join_n_count_kernel(const __grid_constant__ CogroupNSides a, const u32 *__restrict__ match, u32 nk,
+                                    u64 *__restrict__ cnt, unsigned long long *__restrict__ sums, u32 *__restrict__ too_large)
+{
+    const u32 o = blockIdx.x * blockDim.x + threadIdx.x;
+    u64 c = 0;
+    if (o < nk) {
+        const u32 *row = match + (u64)o * a.n;
+        bool all = true;
+        for (u32 j = 0; j < a.n; ++j) all = all && row[j] != 0xFFFFFFFFu;
+        if (all) {
+            c = 1;
+            for (u32 j = 0; j < a.n && c; ++j) {
+                const u64 len = a.offs[j][row[j] + 1] - a.offs[j][row[j]];
+                const u64 p = c * len;
+                if (__umul64hi(c, len) || (p >> 63)) { atomicOr(too_large, 1u); c = 0; }
+                else c = p;
+            }
+        }
+        cnt[o] = c;
+    }
+    u64 hi = c >> 32, lo = c & 0xFFFFFFFFull;
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+        hi += __shfl_down_sync(0xffffffffu, hi, off);
+        lo += __shfl_down_sync(0xffffffffu, lo, off);
+    }
+    if ((threadIdx.x & 31) == 0 && (hi | lo)) {
+        atomicAdd(&sums[0], (unsigned long long)hi);
+        atomicAdd(&sums[1], (unsigned long long)lo);
+    }
+}
+
+// One thread per output row: the owning key k is the largest with pos[k] <= row; the row's position within the key is
+// split into one digit per side, the last side varying fastest (for v0 in l0 { for v1 in l1 { ... } }).
+__global__ void join_n_expand_kernel(const __grid_constant__ CogroupNSides a, const u64 *__restrict__ pos, u32 nk, u64 total,
+                                     const u32 *__restrict__ match, const __grid_constant__ JoinNOut out)
+{
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 o = (u64)blockIdx.x * blockDim.x + threadIdx.x; o < total; o += stride) {
+        u32 lo = 0, hi = nk;
+        while (hi - lo > 1) {
+            const u32 mid = (lo + hi) >> 1;
+            if (pos[mid] <= o) lo = mid; else hi = mid;
+        }
+        const u32 *row = match + (u64)lo * a.n;
+        u64 local = o - pos[lo];
+        for (u32 j = a.n; j-- > 0;) {
+            const u64 b = a.offs[j][row[j]];
+            u64 d = local;
+            if (j) {
+                const u64 len = a.offs[j][row[j] + 1] - b;
+                local = d / len;
+                d -= local * len;
+            }
+            out.v[j][o] = a.vals[j][b + d];
+        }
+        out.k[o] = a.keys[0][a.kb[0] + lo];
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
 // bincode 1.2.1 blob codec (SURVEY §8(f) N1): pure byte shuffling, HBM-bound
 // ---------------------------------------------------------------------------------------------
 // Vec<(u64,u64)>: out = u64 n | n x (k, c)

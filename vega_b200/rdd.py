@@ -541,6 +541,85 @@ class JoinedRdd(_Base):
         return out
 
 
+class CoGroupedRdd(_Base):
+    """CoGroupedRdd::new(rdds, HashPartitioner::new(num_splits)) (src/rdd/co_grouped_rdd.rs:75-135): the cogroup of any
+    number of PairRdds (1 to 16), each shuffled with the Vec-append aggregator as JoinedRdd does.
+
+    compute(r) -> (keys, [(offsets, values) per parent]): every key of the partition once; key i's list from parent j
+    is values_j[offsets_j[i]:offsets_j[i + 1]], empty where that parent lacks the key.  collect() gives the
+    reference's Vec<(K, Vec<Vec<V>>)> as a list of (k, [vs_0, ..., vs_{n-1}]).  join_compute(r) / join_collect() give
+    the inner join of all parents as (k, [v_0, ..., v_{n-1}]) arrays: per key, for v0 in vs_0 { for v1 in vs_1 { ... } }.
+    Each parent's values keep that parent's dtype."""
+
+    def __init__(self, rdds, num_splits):
+        rdds = list(rdds)
+        if not 1 <= len(rdds) <= L.VB_MAX_COGROUP_SIDES:
+            raise ValueError(f"a cogroup takes 1 to {L.VB_MAX_COGROUP_SIDES} parents, got {len(rdds)}")
+        if num_splits < 1:
+            raise ValueError("num_splits must be >= 1")
+        for j, r in enumerate(rdds):
+            if isinstance(r, StrPairRdd):
+                raise TypeError(f"parent {j}: String keys do not support cogroup")
+            if not isinstance(r, PairRdd):
+                raise TypeError(f"parent {j} is not a PairRdd")
+            if len(r.cols) > 1:
+                raise TypeError(f"parent {j}: a PairRdd with several value columns supports combine_by_key only")
+        if any(r.sc is not rdds[0].sc for r in rdds):
+            raise ValueError("the parents live on different contexts")
+        k0 = rdds[0].keys
+        if any(r.keys.key_width != k0.key_width or r.keys.code != k0.code for r in rdds):
+            raise TypeError("the parents have different key types")
+        self.rdds, self.num_slices, self.sc = rdds, num_splits, rdds[0].sc
+        self._shs = None
+
+    def _run(self):
+        if self._shs is None:
+            self._shs = [ShuffledRdd(r, "cogroup", self.num_slices)._run() for r in self.rdds]
+        return self._shs
+
+    def _sides(self):
+        shs = self._run()
+        return shs, (ctypes.c_void_p * len(shs))(*[s._h.value for s in shs])
+
+    def compute(self, split):
+        """Partition `split` of the cogroup (co_grouped_rdd.rs:206-249), aligned on the device by vb_cogroup_n."""
+        shs, sides = self._sides()
+        n, lib = len(shs), self.sc._lib
+        nk, nv = ctypes.c_uint64(), (ctypes.c_uint64 * n)()
+        L.check(lib.vb_cogroup_n_size(sides, n, split, ctypes.byref(nk), nv))
+        keys = np.empty(nk.value, dtype=_NP_OF[shs[0].kcode])
+        offs = [np.empty(nk.value + 1, dtype=np.uint64) for _ in shs]
+        vals = [np.empty(nv[j], dtype=_NP_OF[s.vcode]) for j, s in enumerate(shs)]
+        ptrs = lambda xs: (ctypes.c_void_p * n)(*[x.ctypes.data for x in xs])
+        L.check(lib.vb_cogroup_n(sides, n, split, keys.ctypes.data_as(ctypes.c_void_p), ptrs(offs), ptrs(vals), L.VB_HOST))
+        return keys, list(zip(offs, vals))
+
+    def collect(self):
+        out = []
+        for r in range(self.num_slices):
+            keys, lists = self.compute(r)
+            lists = [(o.tolist(), v) for o, v in lists]
+            out.extend((k, [v[o[i]:o[i + 1]] for o, v in lists]) for i, k in enumerate(keys.tolist()))
+        return out
+
+    def join_compute(self, split):
+        """Partition `split` of the inner join of all parents (vb_join_n): (k, [v_0, ..., v_{n-1}])."""
+        shs, sides = self._sides()
+        n, lib = len(shs), self.sc._lib
+        nn = ctypes.c_uint64()
+        L.check(lib.vb_join_n_size(sides, n, split, ctypes.byref(nn)))
+        k = np.empty(nn.value, dtype=_NP_OF[shs[0].kcode])
+        vs = [np.empty(nn.value, dtype=_NP_OF[s.vcode]) for s in shs]
+        L.check(lib.vb_join_n(sides, n, split, k.ctypes.data_as(ctypes.c_void_p),
+                              (ctypes.c_void_p * n)(*[v.ctypes.data for v in vs]), L.VB_HOST))
+        return k, vs
+
+    def join_collect(self):
+        parts = [self.join_compute(r) for r in range(self.num_slices)]
+        return (np.concatenate([p[0] for p in parts]),
+                [np.concatenate([p[1][j] for p in parts]) for j in range(len(self.rdds))])
+
+
 class CombinedRdd(_Base):
     """`combine_by_key` with named aggregates (src/rdd/pair_rdd.rs:20-33): one shuffle, several aggregates per key.
     `compute(r)` / `collect()` return (keys, {name: array}) with the aggregates in the order they were given."""
