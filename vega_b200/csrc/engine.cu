@@ -275,6 +275,7 @@ struct Timer {
     u64 rows;
 };
 
+// vb_join_outer_size's result for one (right side, partition, outer kind), kept for vb_join_outer
 struct JoinPlan {
     u64 total = 0;
     u32 nl = 0;
@@ -282,17 +283,6 @@ struct JoinPlan {
     u32 *match = nullptr;
     u32 nr = 0;                    // RIGHT / FULL: right keys of the partition
     u64 total_left = 0;            // rows of the left keys (pos[nl])
-};
-
-// vb_cogroup_size's result for one (right side, partition), kept for vb_cogroup.  Output keys: the nl left keys in
-// the left CSR's order, then the n_ro right-only keys in the right CSR's order.
-struct CogroupPlan {
-    u32 nl = 0, nr = 0;            // left / right keys of the partition
-    u64 n_ro = 0;                  // right-only keys
-    u64 n_lv = 0, n_rv = 0;        // left / right values of the partition
-    u64 *pos = nullptr;            // [nl + nr + 1] exclusive right-value positions: the left keys', then the right keys'
-    u32 *match = nullptr;          // [nl] matched right key index, 0xFFFFFFFF if none
-    u64 *ro_keys = nullptr, *ro_pos = nullptr;   // [n_ro] the right-only keys and their right-value positions
 };
 
 // vb_cogroup_n_size / vb_join_n_size's result for one (sides, partition), kept for the write call.  Cogroup output
@@ -362,9 +352,8 @@ struct vb_shuf {
     void *dict = nullptr;          // group ops: key → slot table, kept for joins
     u32 dict_log_cap = 0;
     u32 *dense_of_slot = nullptr;
-    std::map<std::tuple<const vb_shuf *, u32, int>, JoinPlan> join_plans;   // by (right side, partition, join kind)
-    std::map<std::pair<const vb_shuf *, u32>, CogroupPlan> cogroup_plans;   // by (right side, partition)
-    // on side 0 of an N-way cogroup / join: by (every side's uid, partition, join?)
+    std::map<std::tuple<const vb_shuf *, u32, int>, JoinPlan> join_plans;   // by (right side, partition, outer kind)
+    // on side 0 of a cogroup or an inner join, of two sides or N: by (every side's uid, partition, join?)
     std::map<std::tuple<std::vector<u64>, u32, bool>, CogroupNPlan> n_plans;
     // COGROUP shuffles are grouped lazily: seal keeps the (owned) rows; the CSR is built by the first reduce call
     // (cogroup materialisation), or — if a join comes first — only for the rows the join kind needs: the keys on BOTH
@@ -1242,6 +1231,8 @@ static int sort_id_pairs(vb_shuf *s, u32 *ids_a, const Loader &first, u64 n, u32
 // ---------------------------------------------------------------------------------------------
 // shuffle lifecycle
 // ---------------------------------------------------------------------------------------------
+static std::atomic<u64> next_uid{1};   // vb_shuf::uid of every shuffle, the internal ones of a filtered join included
+
 extern "C" int32_t vb_shuffle_create(vb_ctx *c, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce, int32_t kdt,
                                      int32_t vdt, int32_t agg, int32_t part, vb_shuf **out)
 {
@@ -1254,7 +1245,6 @@ extern "C" int32_t vb_shuffle_create(vb_ctx *c, uint64_t shuffle_id, uint32_t n_
     if ((agg == VB_AGG_SORT) != (part == VB_PART_RANGE)) return set_err(VB_ERR_INVALID, "VB_PART_RANGE goes with VB_AGG_SORT only");
     if (n_reduce > 65536) return set_err(VB_ERR_UNSUPPORTED, "more than 65536 reduce partitions");
     vb_shuf *s = new vb_shuf();
-    static std::atomic<u64> next_uid{1};
     s->uid = next_uid.fetch_add(1);
     s->ctx = c;
     s->id = shuffle_id;
@@ -2758,7 +2748,9 @@ compact_scatter_kernel(const unsigned char *__restrict__ match, u64 n, const u64
 
 static int exclusive_scan_u64(vb_shuf *s, const u64 *in, u64 *out, u64 n, u64 *d_total);
 
-static int compact_rows(vb_shuf *s, const u64 *keys, const u64 *vals, u64 n, const unsigned char *match, DevBuf &ok, DevBuf &ov, u64 *m_out)
+// keys_to: write the kept keys there (room for every kept key) instead of into ok
+static int compact_rows(vb_shuf *s, const u64 *keys, const u64 *vals, u64 n, const unsigned char *match, DevBuf &ok, DevBuf &ov, u64 *m_out,
+                        u64 *keys_to = nullptr)
 {
     vb_ctx *c = s->ctx;
     *m_out = 0;
@@ -2778,16 +2770,17 @@ static int compact_rows(vb_shuf *s, const u64 *keys, const u64 *vals, u64 n, con
     m = *(u64 *)c->h_scratch;
     *m_out = m;
     if (m == 0) return VB_OK;
-    TRY(ok.alloc(m * 8));
+    if (!keys_to) { TRY(ok.alloc(m * 8)); keys_to = ok.as<u64>(); }
     TRY(ov.alloc(m * 8));
     KLaunch kl(s, K_JOIN);
-    compact_scatter_kernel<<<(unsigned)blocks, CP_THREADS, 0, c->stream>>>(match, n, off.as<u64>(), keys, vals, ok.as<u64>(), ov.as<u64>());
+    compact_scatter_kernel<<<(unsigned)blocks, CP_THREADS, 0, c->stream>>>(match, n, off.as<u64>(), keys, vals, keys_to, ov.as<u64>());
     return kl.done("compact_scatter_kernel");
 }
 
 static vb_shuf *make_internal_like(const vb_shuf *s)
 {
     vb_shuf *t = new vb_shuf();
+    t->uid = next_uid.fetch_add(1);                 // N-way plans are cached by the sides' uids
     t->ctx = s->ctx; t->id = s->id; t->n_map = 0; t->n_reduce = s->n_reduce;
     t->kdt = s->kdt; t->vdt = s->vdt; t->agg = s->agg; t->part = s->part; t->key_width = s->key_width;
     t->rank = 0; t->world = 1;                      // internal shuffles are device-local
@@ -3195,9 +3188,10 @@ static int join_check(vb_shuf *l, vb_shuf *r, u32 rid)
 
 static_assert(JK_LEFT == (int)VB_JOIN_LEFT && JK_RIGHT == (int)VB_JOIN_RIGHT && JK_FULL == (int)VB_JOIN_FULL, "join kinds");
 
-// Row counts and output positions of partition rid.  Left-driven rows first: per left key |vs| * |ws| when the right
-// side has the key, |vs| when it does not and the kind keeps the left side (LEFT / FULL), else 0.  RIGHT / FULL then
-// place the right-only keys (|ws| rows each, found by probing the left dictionary); one exclusive scan covers both.
+// Row counts and output positions of partition rid for an outer kind.  Left-driven rows first: per left key |vs| * |ws|
+// when the right side has the key, |vs| when it does not and the kind keeps the left side (LEFT / FULL), else 0.
+// RIGHT / FULL then place the right-only keys (|ws| rows each, found by probing the left dictionary); one exclusive
+// scan covers both.
 static int join_plan(vb_shuf *l, vb_shuf *r, u32 rid, int kind, JoinPlan **out)
 {
     vb_ctx *c = l->ctx;
@@ -3207,70 +3201,47 @@ static int join_plan(vb_shuf *l, vb_shuf *r, u32 rid, int kind, JoinPlan **out)
     JoinPlan p;
     const u64 lb = l->bucket_off[rid], le = l->bucket_off[rid + 1];
     p.nl = (u32)(le - lb);
-    if (kind == JK_INNER) {
-        if (p.nl && r->n_keys && r->dict) {
-            DevBuf cnt(c), pos(c), match(c), tot(c);
-            TRY(cnt.alloc((u64)p.nl * 8));
-            TRY(pos.alloc((u64)p.nl * 8));
-            TRY(match.alloc((u64)p.nl * 4));
-            TRY(tot.alloc(8));
-            {
-                KLaunch kl(l, K_JOIN);
-                join_probe_kernel<JK_INNER><<<(p.nl + 255) / 256, 256, 0, c->stream>>>(l->res_keys, l->res_offs, (u32)lb, (u32)le,
-                                                                                   table_at(r->dict, r->dict_log_cap), r->dense_of_slot,
-                                                                                   r->res_offs, cnt.as<u64>(), match.as<u32>());
-                TRY(kl.done("join_probe_kernel"));
-            }
-            TRY(exclusive_scan_u64(l, cnt.as<u64>(), pos.as<u64>(), p.nl, tot.as<u64>()));
-            CU(cudaMemcpyAsync(c->h_scratch, tot.p, 8, cudaMemcpyDeviceToHost, c->stream));
-            CU(cudaStreamSynchronize(c->stream));
-            p.total = *(u64 *)c->h_scratch;
-            p.pos = (u64 *)pos.release();
-            p.match = (u32 *)match.release();
+    const u64 rb = r->bucket_off[rid], re = r->bucket_off[rid + 1];
+    p.nr = (kind == JK_LEFT) ? 0 : (u32)(re - rb);
+    const u64 n = (u64)p.nl + p.nr;
+    if (n) {
+        if ((r->n_keys && !r->dict) || (l->n_keys && !l->dict)) return set_err(VB_ERR_STATE, "join side without a key dictionary");
+        const Table rtab = table_at(r->n_keys ? r->dict : nullptr, r->dict_log_cap);   // keys NULL: that side is empty
+        const Table ltab = table_at(l->n_keys ? l->dict : nullptr, l->dict_log_cap);
+        DevBuf cnt(c), pos(c), match(c), tot(c);
+        TRY(cnt.alloc(n * 8));
+        TRY(pos.alloc(n * 8));
+        TRY(match.alloc(std::max<u64>(p.nl, 1) * 4));
+        TRY(tot.alloc(8));
+        if (p.nl) {
+            KLaunch kl(l, K_JOIN);
+            const unsigned g = (p.nl + 255) / 256;
+            if (kind == JK_LEFT)
+                join_probe_kernel<JK_LEFT><<<g, 256, 0, c->stream>>>(l->res_keys, l->res_offs, (u32)lb, (u32)le, rtab, r->dense_of_slot,
+                                                                     r->res_offs, cnt.as<u64>(), match.as<u32>());
+            else if (kind == JK_RIGHT)
+                join_probe_kernel<JK_RIGHT><<<g, 256, 0, c->stream>>>(l->res_keys, l->res_offs, (u32)lb, (u32)le, rtab, r->dense_of_slot,
+                                                                      r->res_offs, cnt.as<u64>(), match.as<u32>());
+            else
+                join_probe_kernel<JK_FULL><<<g, 256, 0, c->stream>>>(l->res_keys, l->res_offs, (u32)lb, (u32)le, rtab, r->dense_of_slot,
+                                                                     r->res_offs, cnt.as<u64>(), match.as<u32>());
+            TRY(kl.done("join_probe_kernel"));
         }
-    } else {
-        const u64 rb = r->bucket_off[rid], re = r->bucket_off[rid + 1];
-        p.nr = (kind == JK_LEFT) ? 0 : (u32)(re - rb);
-        const u64 n = (u64)p.nl + p.nr;
-        if (n) {
-            if ((r->n_keys && !r->dict) || (l->n_keys && !l->dict)) return set_err(VB_ERR_STATE, "join side without a key dictionary");
-            const Table rtab = table_at(r->n_keys ? r->dict : nullptr, r->dict_log_cap);   // keys NULL: that side is empty
-            const Table ltab = table_at(l->n_keys ? l->dict : nullptr, l->dict_log_cap);
-            DevBuf cnt(c), pos(c), match(c), tot(c);
-            TRY(cnt.alloc(n * 8));
-            TRY(pos.alloc(n * 8));
-            TRY(match.alloc(std::max<u64>(p.nl, 1) * 4));
-            TRY(tot.alloc(8));
-            if (p.nl) {
-                KLaunch kl(l, K_JOIN);
-                const unsigned g = (p.nl + 255) / 256;
-                if (kind == JK_LEFT)
-                    join_probe_kernel<JK_LEFT><<<g, 256, 0, c->stream>>>(l->res_keys, l->res_offs, (u32)lb, (u32)le, rtab, r->dense_of_slot,
-                                                                         r->res_offs, cnt.as<u64>(), match.as<u32>());
-                else if (kind == JK_RIGHT)
-                    join_probe_kernel<JK_RIGHT><<<g, 256, 0, c->stream>>>(l->res_keys, l->res_offs, (u32)lb, (u32)le, rtab, r->dense_of_slot,
-                                                                          r->res_offs, cnt.as<u64>(), match.as<u32>());
-                else
-                    join_probe_kernel<JK_FULL><<<g, 256, 0, c->stream>>>(l->res_keys, l->res_offs, (u32)lb, (u32)le, rtab, r->dense_of_slot,
-                                                                         r->res_offs, cnt.as<u64>(), match.as<u32>());
-                TRY(kl.done("join_probe_kernel"));
-            }
-            if (p.nr) {
-                KLaunch kl(l, K_JOIN);
-                join_probe_right_kernel<<<(p.nr + 255) / 256, 256, 0, c->stream>>>(r->res_keys, r->res_offs, (u32)rb, (u32)re, ltab,
-                                                                                   cnt.as<u64>() + p.nl);
-                TRY(kl.done("join_probe_right_kernel"));
-            }
-            TRY(exclusive_scan_u64(l, cnt.as<u64>(), pos.as<u64>(), n, tot.as<u64>()));
-            u64 *h = (u64 *)c->h_scratch;
-            CU(cudaMemcpyAsync(h, tot.p, 8, cudaMemcpyDeviceToHost, c->stream));
-            if (p.nr) CU(cudaMemcpyAsync(h + 1, pos.as<u64>() + p.nl, 8, cudaMemcpyDeviceToHost, c->stream));
-            CU(cudaStreamSynchronize(c->stream));
-            p.total = h[0];
-            p.total_left = p.nr ? h[1] : p.total;
-            p.pos = (u64 *)pos.release();
-            p.match = (u32 *)match.release();
+        if (p.nr) {
+            KLaunch kl(l, K_JOIN);
+            join_probe_right_kernel<<<(p.nr + 255) / 256, 256, 0, c->stream>>>(r->res_keys, r->res_offs, (u32)rb, (u32)re, ltab,
+                                                                               cnt.as<u64>() + p.nl);
+            TRY(kl.done("join_probe_right_kernel"));
         }
+        TRY(exclusive_scan_u64(l, cnt.as<u64>(), pos.as<u64>(), n, tot.as<u64>()));
+        u64 *h = (u64 *)c->h_scratch;
+        CU(cudaMemcpyAsync(h, tot.p, 8, cudaMemcpyDeviceToHost, c->stream));
+        if (p.nr) CU(cudaMemcpyAsync(h + 1, pos.as<u64>() + p.nl, 8, cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaStreamSynchronize(c->stream));
+        p.total = h[0];
+        p.total_left = p.nr ? h[1] : p.total;
+        p.pos = (u64 *)pos.release();
+        p.match = (u32 *)match.release();
     }
     auto ins = l->join_plans.emplace(key, p);
     *out = &ins.first->second;
@@ -3329,14 +3300,13 @@ static int join_rows(vb_shuf *l, vb_shuf *r, uint32_t rid, int kind, void *out_k
             if (out_wv) { TRY(bwv.alloc(total)); dwv = bwv.as<unsigned char>(); }
         }
         const u64 lb = l->bucket_off[rid];
-        const u64 total_left = kind == JK_INNER ? total : p->total_left;
+        const u64 total_left = p->total_left;
         if (total_left) {
             KLaunch kl(l, K_JOIN);
             u64 blocks = std::min<u64>((total_left + 255) / 256, (u64)c->sm_count * 8);
 #define VB_JOIN_EXPAND(KIND) join_expand_kernel<KIND><<<(unsigned)blocks, 256, 0, c->stream>>>(p->pos, p->nl, total_left, l->res_keys, \
                                  l->res_offs, l->res_vals, (u32)lb, p->match, r->res_offs, r->res_vals, dk, dv, dw, dvv, dwv)
             switch (kind) {
-            case JK_INNER: VB_JOIN_EXPAND(JK_INNER); break;
             case JK_LEFT: VB_JOIN_EXPAND(JK_LEFT); break;
             case JK_RIGHT: VB_JOIN_EXPAND(JK_RIGHT); break;
             default: VB_JOIN_EXPAND(JK_FULL); break;
@@ -3366,16 +3336,6 @@ static int join_rows(vb_shuf *l, vb_shuf *r, uint32_t rid, int kind, void *out_k
     return rc;
 }
 
-extern "C" int32_t vb_join_size(vb_shuf *l, vb_shuf *r, uint32_t rid, uint64_t *n_out)
-{
-    return join_size(l, r, rid, JK_INNER, n_out);
-}
-
-extern "C" int32_t vb_join(vb_shuf *l, vb_shuf *r, uint32_t rid, void *out_k, void *out_v, void *out_w, int32_t dst_loc)
-{
-    return join_rows(l, r, rid, JK_INNER, out_k, out_v, out_w, nullptr, nullptr, dst_loc);
-}
-
 static bool outer_kind(int32_t kind) { return kind == VB_JOIN_LEFT || kind == VB_JOIN_RIGHT || kind == VB_JOIN_FULL; }
 
 extern "C" int32_t vb_join_outer_size(vb_shuf *l, vb_shuf *r, uint32_t rid, int32_t kind, uint64_t *n_out)
@@ -3392,155 +3352,14 @@ extern "C" int32_t vb_join_outer(vb_shuf *l, vb_shuf *r, uint32_t rid, int32_t k
 }
 
 // ---------------------------------------------------------------------------------------------
-// cogroup (CoGroupedRdd::compute for PairRdd::cogroup, co_grouped_rdd.rs:206-249)
-// Both sides are grouped completely (the FULL filtered pair while both are lazy, shared with full_outer_join), so the
-// result is the two CSRs aligned by key: the left keys in the left CSR's order, then the right-only keys in the right
-// CSR's order.  The left values are the left partition's value slice as it is; the right values are the right
-// partition's value segments permuted into output key order by cogroup_gather_right_kernel.
-// ---------------------------------------------------------------------------------------------
-static void free_cogroup_plan(vb_ctx *c, CogroupPlan &p)
-{
-    dev_free(c, p.pos); dev_free(c, p.match); dev_free(c, p.ro_keys); dev_free(c, p.ro_pos);
-}
-
-static int cogroup_plan(vb_shuf *l, vb_shuf *r, u32 rid, CogroupPlan **out)
-{
-    vb_ctx *c = l->ctx;
-    const auto key = std::make_pair((const vb_shuf *)r, rid);
-    auto it = l->cogroup_plans.find(key);
-    if (it != l->cogroup_plans.end()) { *out = &it->second; return VB_OK; }
-    CogroupPlan p;
-    const u64 lb = l->bucket_off[rid], le = l->bucket_off[rid + 1];
-    const u64 rb = r->bucket_off[rid], re = r->bucket_off[rid + 1];
-    p.nl = (u32)(le - lb);
-    p.nr = (u32)(re - rb);
-    p.n_lv = l->val_off[rid + 1] - l->val_off[rid];
-    const u64 n = (u64)p.nl + p.nr;
-    DevBuf pos(c), match(c), ro_keys(c), ro_pos(c);
-    TRY(pos.alloc((n + 1) * 8));
-    if (n == 0) {
-        CU(cudaMemsetAsync(pos.p, 0, 8, c->stream));
-    } else {
-        if ((r->n_keys && !r->dict) || (l->n_keys && !l->dict)) return set_err(VB_ERR_STATE, "cogroup side without a key dictionary");
-        const Table rtab = table_at(r->n_keys ? r->dict : nullptr, r->dict_log_cap);   // keys NULL: that side is empty
-        const Table ltab = table_at(l->n_keys ? l->dict : nullptr, l->dict_log_cap);
-        DevBuf cnt(c), flag(c);
-        TRY(cnt.alloc(n * 8));
-        TRY(match.alloc(std::max<u64>(p.nl, 1) * 4));
-        if (p.nl) {
-            KLaunch kl(l, K_JOIN);
-            cogroup_probe_kernel<<<(p.nl + 255) / 256, 256, 0, c->stream>>>(l->res_keys, (u32)lb, (u32)le, rtab, r->dense_of_slot,
-                                                                            r->res_offs, cnt.as<u64>(), match.as<u32>());
-            TRY(kl.done("cogroup_probe_kernel"));
-        }
-        if (p.nr) {
-            TRY(flag.alloc(p.nr));
-            {
-                KLaunch kl(l, K_JOIN);
-                join_probe_right_kernel<<<(p.nr + 255) / 256, 256, 0, c->stream>>>(r->res_keys, r->res_offs, (u32)rb, (u32)re, ltab,
-                                                                                   cnt.as<u64>() + p.nl);
-                TRY(kl.done("join_probe_right_kernel"));
-            }
-            KLaunch kl(l, K_JOIN);
-            cogroup_flag_kernel<<<(p.nr + 255) / 256, 256, 0, c->stream>>>(cnt.as<u64>() + p.nl, p.nr, flag.as<unsigned char>());
-            TRY(kl.done("cogroup_flag_kernel"));
-        }
-        TRY(exclusive_scan_u64(l, cnt.as<u64>(), pos.as<u64>(), n, pos.as<u64>() + n));
-        // the right-only keys and their positions, in the right CSR's order (stable compaction)
-        if (p.nr) TRY(compact_rows(l, r->res_keys + rb, pos.as<u64>() + p.nl, p.nr, flag.as<unsigned char>(), ro_keys, ro_pos, &p.n_ro));
-    }
-    CU(cudaMemcpyAsync(c->h_scratch, pos.as<u64>() + n, 8, cudaMemcpyDeviceToHost, c->stream));
-    CU(cudaStreamSynchronize(c->stream));
-    p.n_rv = *(u64 *)c->h_scratch;
-    p.pos = (u64 *)pos.release();
-    p.match = (u32 *)match.release();
-    p.ro_keys = (u64 *)ro_keys.release();
-    p.ro_pos = (u64 *)ro_pos.release();
-    *out = &l->cogroup_plans.emplace(key, p).first->second;
-    return VB_OK;
-}
-
-extern "C" int32_t vb_cogroup_size(vb_shuf *l, vb_shuf *r, uint32_t rid, uint64_t *n_keys, uint64_t *n_left_vals,
-                                   uint64_t *n_right_vals)
-{
-    TRY(join_check(l, r, rid));
-    std::lock_guard<std::mutex> lk(l->ctx->mu);
-    CU(cudaSetDevice(l->ctx->device));
-    TRY(join_sides(l, r, JK_FULL));
-    CogroupPlan *p = nullptr;
-    TRY(cogroup_plan(l, r, rid, &p));
-    if (n_keys) *n_keys = p->nl + p->n_ro;
-    if (n_left_vals) *n_left_vals = p->n_lv;
-    if (n_right_vals) *n_right_vals = p->n_rv;
-    return VB_OK;
-}
-
-extern "C" int32_t vb_cogroup(vb_shuf *l, vb_shuf *r, uint32_t rid, void *out_keys, uint64_t *out_left_offsets,
-                              void *out_left_vals, uint64_t *out_right_offsets, void *out_right_vals, int32_t dst_loc)
-{
-    TRY(join_check(l, r, rid));
-    if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
-    vb_ctx *c = l->ctx;
-    std::lock_guard<std::mutex> lk(c->mu);
-    CU(cudaSetDevice(c->device));
-    TRY(join_sides(l, r, JK_FULL));
-    CogroupPlan *p = nullptr;
-    TRY(cogroup_plan(l, r, rid, &p));
-    const u64 nl = p->nl, nk = nl + p->n_ro, n = nl + p->nr;
-    const u64 lb = l->bucket_off[rid], lv0 = l->val_off[rid];
-    int rc = [&]() -> int {
-        // keys: the left keys, then the right-only keys
-        TRY(copy_out(l, out_keys, l->res_keys ? l->res_keys + lb : nullptr, nl * 8, dst_loc));
-        TRY(copy_out(l, out_keys ? (u64 *)out_keys + nl : nullptr, p->ro_keys, p->n_ro * 8, dst_loc));
-        // left lists: the partition's value slice as it is; offsets rebased, then flat for the right-only keys
-        if (out_left_offsets) {
-            DevBuf tmp(c);
-            u64 *d = out_left_offsets;
-            if (dst_loc == VB_HOST) { TRY(tmp.alloc((nk + 1) * 8)); d = tmp.as<u64>(); }
-            {
-                KLaunch kl(l, K_JOIN);
-                cogroup_left_offsets_kernel<<<(unsigned)((nk + 1 + 255) / 256), 256, 0, c->stream>>>(l->res_offs, (u32)lb, (u32)nl, nk + 1,
-                                                                                                    lv0, p->n_lv, d);
-                TRY(kl.done("cogroup_left_offsets_kernel"));
-            }
-            if (dst_loc == VB_HOST) TRY(copy_out(l, out_left_offsets, d, (nk + 1) * 8, VB_HOST));
-        }
-        TRY(copy_out(l, out_left_vals, l->res_vals ? l->res_vals + lv0 : nullptr, p->n_lv * 8, dst_loc));
-        // right offsets: the left keys' positions, the right-only keys' positions, the total
-        if (out_right_offsets) {
-            TRY(copy_out(l, out_right_offsets, p->pos, nl * 8, dst_loc));
-            TRY(copy_out(l, out_right_offsets + nl, p->ro_pos, p->n_ro * 8, dst_loc));
-            TRY(copy_out(l, out_right_offsets + nk, p->pos + n, 8, dst_loc));
-        }
-        // right lists: each right key's value segment, gathered into output key order
-        if (out_right_vals && p->n_rv) {
-            DevBuf tmp(c);
-            u64 *d = (u64 *)out_right_vals;
-            if (dst_loc == VB_HOST) { TRY(tmp.alloc(p->n_rv * 8)); d = tmp.as<u64>(); }
-            {
-                KLaunch kl(l, K_JOIN);
-                const u64 blocks = std::min<u64>((p->n_rv + 255) / 256, (u64)c->sm_count * 8);
-                cogroup_gather_right_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(p->pos, (u32)n, p->n_rv, p->match, (u32)nl,
-                                                                                    (u32)r->bucket_off[rid], r->res_offs, r->res_vals, d);
-                TRY(kl.done("cogroup_gather_right_kernel"));
-            }
-            if (dst_loc == VB_HOST) TRY(copy_out(l, out_right_vals, d, p->n_rv * 8, VB_HOST));
-        }
-        return VB_OK;
-    }();
-    cudaStreamSynchronize(c->stream);
-    free_cogroup_plan(c, *p);
-    l->cogroup_plans.erase(std::make_pair((const vb_shuf *)r, rid));
-    return rc;
-}
-
-// ---------------------------------------------------------------------------------------------
-// N-way cogroup and inner join (CoGroupedRdd::compute with n parents, co_grouped_rdd.rs:206-249)
-// Every side is grouped whole.  Side i's keys are probed against every other side's dictionary by one launch per side
-// (all sides' tables in one parameter struct): a key no earlier side has is new, and its row of the match matrix
-// records its index on every side.  The output keys are side 0's, then each later side's new keys taken by the stable
-// compaction; side j's lists are its value segments gathered into output key order.  The join reads side 0's rows of
-// the matrix only: the keys on every side are exactly the side-0 keys without a 0xFFFFFFFF.
+// cogroup and inner join of n sides (CoGroupedRdd::compute with n parents, co_grouped_rdd.rs:206-249)
+// Side i's keys are probed against every other side's dictionary by one launch per side (all sides' tables in one
+// parameter struct): a key no earlier side has is new, and its row of the match matrix records its index on every side.
+// The output keys are side 0's, then each later side's new keys taken by the stable compaction.  Side 0's lists are its
+// partition's value slice as it is; side j's lists are its value segments gathered into output key order.  The join
+// reads side 0's rows of the matrix only: the keys on every side are exactly the side-0 keys without a 0xFFFFFFFF.
+// vb_cogroup_n* / vb_join_n* group every side whole.  vb_cogroup* / vb_join* are the two-side case over the pair
+// join_sides picks: the FULL (cogroup) or INNER (join) filtered pair while both sides are still lazy.
 // ---------------------------------------------------------------------------------------------
 static_assert(CGN_MAX_SIDES == VB_MAX_COGROUP_SIDES, "cogroup side limit");
 
@@ -3568,14 +3387,13 @@ static int cogroup_n_check(vb_shuf *const *sides, u32 n, u32 rid)
     return VB_OK;
 }
 
-// group every side (caller holds the context lock) and describe them for the kernels
+// describe the grouped sides for the kernels
 static int cogroup_n_sides(vb_shuf *const *sides, u32 n, u32 rid, CogroupNSides *a)
 {
     *a = CogroupNSides{};
     a->n = n;
     for (u32 j = 0; j < n; ++j) {
-        vb_shuf *s = sides[j];
-        TRY(ensure_grouped(s));
+        const vb_shuf *s = sides[j];
         if (s->n_keys && !s->dict) return set_err(VB_ERR_STATE, "cogroup side without a key dictionary");
         a->tab[j] = table_at(s->n_keys ? s->dict : nullptr, s->dict_log_cap);
         a->dense[j] = s->dense_of_slot;
@@ -3615,7 +3433,7 @@ static int cogroup_n_plan(vb_shuf *const *sides, u32 n, u32 rid, bool join, cons
         for (u32 i = 1; i < n; ++i) {
             if (!nk[i]) continue;
             DevBuf rows(c), flag(c), lidx(c), ok(c), ov(c);
-            TRY(rows.alloc(nk[i] * n * 4)); TRY(flag.alloc(nk[i])); TRY(lidx.alloc(nk[i] * 8));
+            TRY(rows.alloc(i + 1 < n ? nk[i] * n * 4 : 0)); TRY(flag.alloc(nk[i])); TRY(lidx.alloc(nk[i] * 8));
             {
                 KLaunch kl(s0, K_JOIN);
                 cogroup_n_probe_kernel<<<(unsigned)((nk[i] + 255) / 256), 256, 0, c->stream>>>(a, i, (u32)nk[i], rows.as<u32>(),
@@ -3623,16 +3441,16 @@ static int cogroup_n_plan(vb_shuf *const *sides, u32 n, u32 rid, bool join, cons
                 TRY(kl.done("cogroup_n_probe_kernel"));
             }
             u64 m = 0;
-            TRY(compact_rows(s0, sides[i]->res_keys + a.kb[i], lidx.as<u64>(), nk[i], flag.as<unsigned char>(), ok, ov, &m));
+            TRY(compact_rows(s0, sides[i]->res_keys + a.kb[i], lidx.as<u64>(), nk[i], flag.as<unsigned char>(), ok, ov, &m,
+                             new_keys.as<u64>() + (p.n_keys - nk[0])));
             if (!m) continue;
             {
                 KLaunch kl(s0, K_JOIN);
                 const u64 blocks = std::min<u64>((m * n + 255) / 256, (u64)c->sm_count * 8);
-                cogroup_n_take_rows_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(rows.as<u32>(), n, ov.as<u64>(), m,
+                cogroup_n_take_rows_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(rows.as<u32>(), n, i, a.kb[i], ov.as<u64>(), m,
                                                                                     match.as<u32>() + p.n_keys * n);
                 TRY(kl.done("cogroup_n_take_rows_kernel"));
             }
-            CU(cudaMemcpyAsync(new_keys.as<u64>() + (p.n_keys - nk[0]), ok.p, m * 8, cudaMemcpyDeviceToDevice, c->stream));
             p.n_keys += m;
         }
     }
@@ -3675,12 +3493,10 @@ static void drop_cogroup_n_plan(vb_shuf *const *sides, u32 n, u32 rid, bool join
     sides[0]->n_plans.erase(it);
 }
 
-extern "C" int32_t vb_cogroup_n_size(vb_shuf *const *sides, uint32_t n_sides, uint32_t rid, uint64_t *n_keys, uint64_t *n_vals)
+// The plan and the write of a cogroup / inner join, over sides that are grouped, with the context locked
+
+static int cogroup_n_size(vb_shuf *const *sides, u32 n_sides, u32 rid, u64 *n_keys, u64 *n_vals)
 {
-    TRY(cogroup_n_check(sides, n_sides, rid));
-    vb_ctx *c = sides[0]->ctx;
-    std::lock_guard<std::mutex> lk(c->mu);
-    CU(cudaSetDevice(c->device));
     CogroupNSides a;
     TRY(cogroup_n_sides(sides, n_sides, rid, &a));
     CogroupNPlan *p = nullptr;
@@ -3690,15 +3506,11 @@ extern "C" int32_t vb_cogroup_n_size(vb_shuf *const *sides, uint32_t n_sides, ui
     return VB_OK;
 }
 
-extern "C" int32_t vb_cogroup_n(vb_shuf *const *sides, uint32_t n_sides, uint32_t rid, void *out_keys,
-                                uint64_t *const *out_offsets, void *const *out_vals, int32_t dst_loc)
+static int cogroup_n_write(vb_shuf *const *sides, u32 n_sides, u32 rid, void *out_keys, u64 *const *out_offsets,
+                           void *const *out_vals, int dst_loc)
 {
-    TRY(cogroup_n_check(sides, n_sides, rid));
-    if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
     vb_shuf *s0 = sides[0];
     vb_ctx *c = s0->ctx;
-    std::lock_guard<std::mutex> lk(c->mu);
-    CU(cudaSetDevice(c->device));
     CogroupNSides a;
     TRY(cogroup_n_sides(sides, n_sides, rid, &a));
     CogroupNPlan *p = nullptr;
@@ -3713,6 +3525,24 @@ extern "C" int32_t vb_cogroup_n(vb_shuf *const *sides, uint32_t n_sides, uint32_
             if (!o_offs && !o_vals) continue;
             vb_shuf *s = sides[j];
             const u64 nv = s->val_off[rid + 1] - s->val_off[rid];
+            if (j == 0) {
+                // side 0's lists are its partition's value slice as it is: its CSR offsets rebased, then flat (nv) for
+                // the keys after side 0's
+                if (o_offs) {
+                    DevBuf tmp(c);
+                    u64 *d = o_offs;
+                    if (dst_loc == VB_HOST) { TRY(tmp.alloc((nk + 1) * 8)); d = tmp.as<u64>(); }
+                    {
+                        KLaunch kl(s0, K_JOIN);
+                        cogroup_left_offsets_kernel<<<(unsigned)((nk + 1 + 255) / 256), 256, 0, c->stream>>>(s->res_offs, a.kb[0], (u32)nk0,
+                                                                                                            nk + 1, s->val_off[rid], nv, d);
+                        TRY(kl.done("cogroup_left_offsets_kernel"));
+                    }
+                    if (dst_loc == VB_HOST) TRY(copy_out(s0, o_offs, d, (nk + 1) * 8, VB_HOST));
+                }
+                if (o_vals && nv) TRY(copy_out(s0, o_vals, s->res_vals + s->val_off[rid], nv * 8, dst_loc));
+                continue;
+            }
             // side j's list offsets: the list lengths of the output keys, scanned (on the device even for a host output)
             DevBuf pos(c), cnt(c);
             u64 *d_pos = (o_offs && dst_loc == VB_DEVICE) ? o_offs : nullptr;
@@ -3731,10 +3561,6 @@ extern "C" int32_t vb_cogroup_n(vb_shuf *const *sides, uint32_t n_sides, uint32_
             }
             if (o_offs && dst_loc == VB_HOST) TRY(copy_out(s0, o_offs, d_pos, (nk + 1) * 8, VB_HOST));
             if (!o_vals || !nv) continue;
-            if (j == 0) {                                  // side 0's lists are its partition's value slice as it is
-                TRY(copy_out(s0, o_vals, s->res_vals + s->val_off[rid], nv * 8, dst_loc));
-                continue;
-            }
             DevBuf tmp(c);
             u64 *d = (u64 *)o_vals;
             if (dst_loc == VB_HOST) { TRY(tmp.alloc(nv * 8)); d = tmp.as<u64>(); }
@@ -3754,13 +3580,8 @@ extern "C" int32_t vb_cogroup_n(vb_shuf *const *sides, uint32_t n_sides, uint32_
     return rc;
 }
 
-extern "C" int32_t vb_join_n_size(vb_shuf *const *sides, uint32_t n_sides, uint32_t rid, uint64_t *n_out)
+static int join_n_size(vb_shuf *const *sides, u32 n_sides, u32 rid, u64 *n_out)
 {
-    TRY(cogroup_n_check(sides, n_sides, rid));
-    if (!n_out) return set_err(VB_ERR_INVALID, "n_out is NULL");
-    vb_ctx *c = sides[0]->ctx;
-    std::lock_guard<std::mutex> lk(c->mu);
-    CU(cudaSetDevice(c->device));
     CogroupNSides a;
     TRY(cogroup_n_sides(sides, n_sides, rid, &a));
     CogroupNPlan *p = nullptr;
@@ -3769,15 +3590,10 @@ extern "C" int32_t vb_join_n_size(vb_shuf *const *sides, uint32_t n_sides, uint3
     return VB_OK;
 }
 
-extern "C" int32_t vb_join_n(vb_shuf *const *sides, uint32_t n_sides, uint32_t rid, void *out_k, void *const *out_vals,
-                             int32_t dst_loc)
+static int join_n_write(vb_shuf *const *sides, u32 n_sides, u32 rid, void *out_k, void *const *out_vals, int dst_loc)
 {
-    TRY(cogroup_n_check(sides, n_sides, rid));
-    if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
     vb_shuf *s0 = sides[0];
     vb_ctx *c = s0->ctx;
-    std::lock_guard<std::mutex> lk(c->mu);
-    CU(cudaSetDevice(c->device));
     CogroupNSides a;
     TRY(cogroup_n_sides(sides, n_sides, rid, &a));
     CogroupNPlan *p = nullptr;
@@ -3812,6 +3628,103 @@ extern "C" int32_t vb_join_n(vb_shuf *const *sides, uint32_t n_sides, uint32_t r
     cudaStreamSynchronize(c->stream);
     drop_cogroup_n_plan(sides, n_sides, rid, true);
     return rc;
+}
+
+extern "C" int32_t vb_cogroup_n_size(vb_shuf *const *sides, uint32_t n_sides, uint32_t rid, uint64_t *n_keys, uint64_t *n_vals)
+{
+    TRY(cogroup_n_check(sides, n_sides, rid));
+    vb_ctx *c = sides[0]->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    for (u32 j = 0; j < n_sides; ++j) TRY(ensure_grouped(sides[j]));
+    return cogroup_n_size(sides, n_sides, rid, n_keys, n_vals);
+}
+
+extern "C" int32_t vb_cogroup_n(vb_shuf *const *sides, uint32_t n_sides, uint32_t rid, void *out_keys,
+                                uint64_t *const *out_offsets, void *const *out_vals, int32_t dst_loc)
+{
+    TRY(cogroup_n_check(sides, n_sides, rid));
+    if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
+    vb_ctx *c = sides[0]->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    for (u32 j = 0; j < n_sides; ++j) TRY(ensure_grouped(sides[j]));
+    return cogroup_n_write(sides, n_sides, rid, out_keys, out_offsets, out_vals, dst_loc);
+}
+
+extern "C" int32_t vb_join_n_size(vb_shuf *const *sides, uint32_t n_sides, uint32_t rid, uint64_t *n_out)
+{
+    TRY(cogroup_n_check(sides, n_sides, rid));
+    if (!n_out) return set_err(VB_ERR_INVALID, "n_out is NULL");
+    vb_ctx *c = sides[0]->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    for (u32 j = 0; j < n_sides; ++j) TRY(ensure_grouped(sides[j]));
+    return join_n_size(sides, n_sides, rid, n_out);
+}
+
+extern "C" int32_t vb_join_n(vb_shuf *const *sides, uint32_t n_sides, uint32_t rid, void *out_k, void *const *out_vals,
+                             int32_t dst_loc)
+{
+    TRY(cogroup_n_check(sides, n_sides, rid));
+    if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
+    vb_ctx *c = sides[0]->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    for (u32 j = 0; j < n_sides; ++j) TRY(ensure_grouped(sides[j]));
+    return join_n_write(sides, n_sides, rid, out_k, out_vals, dst_loc);
+}
+
+extern "C" int32_t vb_cogroup_size(vb_shuf *l, vb_shuf *r, uint32_t rid, uint64_t *n_keys, uint64_t *n_left_vals,
+                                   uint64_t *n_right_vals)
+{
+    TRY(join_check(l, r, rid));
+    std::lock_guard<std::mutex> lk(l->ctx->mu);
+    CU(cudaSetDevice(l->ctx->device));
+    TRY(join_sides(l, r, JK_FULL));
+    vb_shuf *const sides[2] = {l, r};
+    u64 n_vals[2];
+    TRY(cogroup_n_size(sides, 2, rid, n_keys, n_vals));
+    if (n_left_vals) *n_left_vals = n_vals[0];
+    if (n_right_vals) *n_right_vals = n_vals[1];
+    return VB_OK;
+}
+
+extern "C" int32_t vb_cogroup(vb_shuf *l, vb_shuf *r, uint32_t rid, void *out_keys, uint64_t *out_left_offsets,
+                              void *out_left_vals, uint64_t *out_right_offsets, void *out_right_vals, int32_t dst_loc)
+{
+    TRY(join_check(l, r, rid));
+    if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
+    std::lock_guard<std::mutex> lk(l->ctx->mu);
+    CU(cudaSetDevice(l->ctx->device));
+    TRY(join_sides(l, r, JK_FULL));
+    vb_shuf *const sides[2] = {l, r};
+    u64 *const out_offsets[2] = {out_left_offsets, out_right_offsets};
+    void *const out_vals[2] = {out_left_vals, out_right_vals};
+    return cogroup_n_write(sides, 2, rid, out_keys, out_offsets, out_vals, dst_loc);
+}
+
+extern "C" int32_t vb_join_size(vb_shuf *l, vb_shuf *r, uint32_t rid, uint64_t *n_out)
+{
+    TRY(join_check(l, r, rid));
+    if (!n_out) return set_err(VB_ERR_INVALID, "n_out is NULL");
+    std::lock_guard<std::mutex> lk(l->ctx->mu);
+    CU(cudaSetDevice(l->ctx->device));
+    TRY(join_sides(l, r, JK_INNER));
+    vb_shuf *const sides[2] = {l, r};
+    return join_n_size(sides, 2, rid, n_out);
+}
+
+extern "C" int32_t vb_join(vb_shuf *l, vb_shuf *r, uint32_t rid, void *out_k, void *out_v, void *out_w, int32_t dst_loc)
+{
+    TRY(join_check(l, r, rid));
+    if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
+    std::lock_guard<std::mutex> lk(l->ctx->mu);
+    CU(cudaSetDevice(l->ctx->device));
+    TRY(join_sides(l, r, JK_INNER));
+    vb_shuf *const sides[2] = {l, r};
+    void *const out_vals[2] = {out_v, out_w};
+    return join_n_write(sides, 2, rid, out_k, out_vals, dst_loc);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -4370,7 +4283,6 @@ extern "C" int32_t vb_shuffle_free(vb_shuf *s)
         dev_free(c, s->res_keys); dev_free(c, s->res_comb); dev_free(c, s->res_offs); dev_free(c, s->res_vals); dev_free(c, s->res_cols);
         dev_free(c, s->dict); dev_free(c, s->dense_of_slot);
         for (auto &kv : s->join_plans) { dev_free(c, kv.second.pos); dev_free(c, kv.second.match); }
-        for (auto &kv : s->cogroup_plans) free_cogroup_plan(c, kv.second);
         for (auto &kv : s->n_plans) free_cogroup_n_plan(c, kv.second);
         free_lazy_rows(s);
         free_str(s);

@@ -1536,12 +1536,13 @@ __global__ void aos_to_soa_kernel(const u64 *__restrict__ rows, u64 n, u64 *__re
 // ---------------------------------------------------------------------------------------------
 // join (CoGroupedRdd::compute + cross product)
 // ---------------------------------------------------------------------------------------------
-// Join kinds: the inner join, and the outer joins with the values of vb_join_kind (include/vega_b200.h).
+// Join kinds: the inner join (the N-way join below; here only the kind of a filtered pair), and the outer joins with the
+// values of vb_join_kind (include/vega_b200.h).
 enum : int { JK_INNER = 0, JK_LEFT = 1, JK_RIGHT = 2, JK_FULL = 3 };
 template <int KIND> constexpr bool jk_keeps_left() { return KIND == JK_LEFT || KIND == JK_FULL; }
 
-// For left keys [lb, le): find the key in the right shuffle's dictionary; cnt = lenL * lenR.  An unmatched key counts
-// lenL rows (k, v, None) when the kind keeps the left side.  The outer kinds accept an empty right side (rtab.keys NULL).
+// Outer join, left keys [lb, le): find the key in the right shuffle's dictionary; cnt = lenL * lenR.  An unmatched key
+// counts lenL rows (k, v, None) when the kind keeps the left side.  rtab.keys is NULL when the right side has no rows.
 template <int KIND>
 __global__ void join_probe_kernel(const u64 *__restrict__ lkeys, const u64 *__restrict__ loffs, u32 lb, u32 le,
                                   Table rtab, const u32 *__restrict__ r_dense,
@@ -1550,7 +1551,7 @@ __global__ void join_probe_kernel(const u64 *__restrict__ lkeys, const u64 *__re
     u32 j = lb + blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= le) return;
     u64 key = lkeys[j];
-    u32 s = (KIND == JK_INNER || rtab.keys) ? table_find(rtab, key) : 0xFFFFFFFFu;
+    u32 s = rtab.keys ? table_find(rtab, key) : 0xFFFFFFFFu;
     u64 c = 0;
     u32 m = 0xFFFFFFFFu;
     if (s != 0xFFFFFFFFu) {
@@ -1574,8 +1575,8 @@ __global__ void join_probe_right_kernel(const u64 *__restrict__ rkeys, const u64
     cnt[j - rb] = in_left ? 0 : roffs[j + 1] - roffs[j];
 }
 
-// One thread per output row: binary-search the owning left key, then (v, w) = divmod.  The outer kinds also write the
-// rows of unmatched left keys as (k, v, 0), and the validity bytes when out_vv / out_wv are given.
+// Outer join, one thread per output row: binary-search the owning left key, then (v, w) = divmod.  LEFT / FULL also
+// write the rows of unmatched left keys as (k, v, 0); every kind writes the validity bytes when out_vv / out_wv are given.
 template <int KIND>
 __global__ void join_expand_kernel(const u64 *__restrict__ pos /*[nl] exclusive*/, u32 nl, u64 total,
                                    const u64 *__restrict__ lkeys, const u64 *__restrict__ loffs, const u64 *__restrict__ lvals,
@@ -1607,10 +1608,8 @@ __global__ void join_expand_kernel(const u64 *__restrict__ pos /*[nl] exclusive*
         out_k[o] = lkeys[lb + j];
         out_v[o] = lvals[loffs[lb + j] + vi];
         out_w[o] = rvals[roffs[m] + wi];
-        if (KIND != JK_INNER) {
-            if (out_vv) out_vv[o] = 1;
-            if (out_wv) out_wv[o] = 1;
-        }
+        if (out_vv) out_vv[o] = 1;
+        if (out_wv) out_wv[o] = 1;
     }
 }
 
@@ -1638,58 +1637,6 @@ __global__ void join_expand_right_kernel(const u64 *__restrict__ pos, u32 nr, u6
 }
 
 // ---------------------------------------------------------------------------------------------
-// cogroup (CoGroupedRdd::compute): every key of a partition once, the left keys first, then the right-only keys
-// ---------------------------------------------------------------------------------------------
-// For left keys [lb, le): match = the right key's index (0xFFFFFFFF when the right side lacks the key) and
-// cnt = lenR, the number of right values the key's output list gets (0 when unmatched).  rtab.keys NULL: no right rows.
-__global__ void cogroup_probe_kernel(const u64 *__restrict__ lkeys, u32 lb, u32 le, Table rtab, const u32 *__restrict__ r_dense,
-                                     const u64 *__restrict__ roffs, u64 *__restrict__ cnt, u32 *__restrict__ match)
-{
-    const u32 j = lb + blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= le) return;
-    const u32 s = rtab.keys ? table_find(rtab, lkeys[j]) : 0xFFFFFFFFu;
-    const u32 m = s != 0xFFFFFFFFu ? r_dense[s] : 0xFFFFFFFFu;
-    cnt[j - lb] = m != 0xFFFFFFFFu ? roffs[m + 1] - roffs[m] : 0;
-    match[j - lb] = m;
-}
-
-// flag[i] = 1 for a right-only key: join_probe_right_kernel counted its values (a key always has at least one)
-__global__ void cogroup_flag_kernel(const u64 *__restrict__ cnt, u32 n, unsigned char *__restrict__ flag)
-{
-    const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) flag[i] = cnt[i] != 0;
-}
-
-// out[i] for i in [0, n): the left CSR's offsets of keys [lb, lb + nl) rebased to base, then n_lv (an empty left list)
-// for the right-only keys.
-__global__ void cogroup_left_offsets_kernel(const u64 *__restrict__ loffs, u32 lb, u32 nl, u64 n, u64 base, u64 n_lv,
-                                            u64 *__restrict__ out)
-{
-    const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) out[i] = i < nl ? loffs[lb + i] - base : n_lv;
-}
-
-// The right values in output key order, one thread per value (a key with 10^6 values spreads over 10^6 threads).
-// pos[n] holds the exclusive output positions of the partition's left keys (their matched right lists) followed by its
-// right keys (the right-only ones; 0 values for a key the left side has).  Output value o belongs to the largest j with
-// pos[j] <= o; its source segment is the right key match[j] (j < nl) or rb + j - nl.
-__global__ void cogroup_gather_right_kernel(const u64 *__restrict__ pos, u32 n, u64 total, const u32 *__restrict__ match,
-                                            u32 nl, u32 rb, const u64 *__restrict__ roffs, const u64 *__restrict__ rvals,
-                                            u64 *__restrict__ out)
-{
-    const u64 stride = (u64)gridDim.x * blockDim.x;
-    for (u64 o = (u64)blockIdx.x * blockDim.x + threadIdx.x; o < total; o += stride) {
-        u32 lo = 0, hi = n;
-        while (hi - lo > 1) {
-            const u32 mid = (lo + hi) >> 1;
-            if (pos[mid] <= o) lo = mid; else hi = mid;
-        }
-        const u32 src = lo < nl ? match[lo] : rb + (lo - nl);
-        out[o] = rvals[roffs[src] + (o - pos[lo])];
-    }
-}
-
-// ---------------------------------------------------------------------------------------------
 // N-way cogroup and inner join (CoGroupedRdd::compute with n parents).  The output keys are side 0's keys, then each
 // later side's new keys (those no earlier side has).  match is key-major: row o holds output key o's index on every
 // side (a global key index of that side's CSR), 0xFFFFFFFF where the side lacks the key.
@@ -1710,8 +1657,8 @@ struct JoinNOut {
 };
 
 // Keys [kb_i, kb_i + nk) of side i: row t = the key's index on every side (its own: kb_i + t).  Side i > 0 sets
-// flag[t] = 1 and lidx[t] = t for a key no side j < i has, and leaves the row of any other key unfinished: only the
-// rows of new keys are used.
+// flag[t] = 1 and lidx[t] = t for a key no side j < i has, and writes only the entries j > i of its row (the others
+// are known: 0xFFFFFFFF before i, kb_i + t at i); the rows of other keys are left unfinished and never used.
 __global__ void cogroup_n_probe_kernel(const __grid_constant__ CogroupNSides a, u32 i, u32 nk, u32 *__restrict__ rows,
                                        unsigned char *__restrict__ flag, u64 *__restrict__ lidx)
 {
@@ -1725,20 +1672,31 @@ __global__ void cogroup_n_probe_kernel(const __grid_constant__ CogroupNSides a, 
             m = s != 0xFFFFFFFFu ? a.dense[j][s] : 0xFFFFFFFFu;
         }
         if (j < i && m != 0xFFFFFFFFu) { flag[t] = 0; return; }     // an earlier side already gave this key
-        rows[(u64)t * a.n + j] = m;
+        if (i == 0 || j > i) rows[(u64)t * a.n + j] = m;
     }
     if (i) { flag[t] = 1; lidx[t] = t; }
 }
 
-// out[o] = row lidx[o] of rows (n entries per row) for the m new keys of a side, in output order
-__global__ void cogroup_n_take_rows_kernel(const u32 *__restrict__ rows, u32 n, const u64 *__restrict__ lidx, u64 m,
+// out[o] = the match row of side i's new key lidx[o] (n entries per row), for its m new keys in output order: 0xFFFFFFFF
+// for the sides before i, its own index kb_i + lidx[o] for side i, and the probe's entries of rows after i
+__global__ void cogroup_n_take_rows_kernel(const u32 *__restrict__ rows, u32 n, u32 i, u32 kb_i, const u64 *__restrict__ lidx, u64 m,
                                            u32 *__restrict__ out)
 {
     const u64 stride = (u64)gridDim.x * blockDim.x;
     for (u64 e = (u64)blockIdx.x * blockDim.x + threadIdx.x; e < m * n; e += stride) {
         const u64 o = e / n;
-        out[e] = rows[lidx[o] * n + (e - o * n)];
+        const u32 j = (u32)(e - o * n);
+        out[e] = j < i ? 0xFFFFFFFFu : j == i ? kb_i + (u32)lidx[o] : rows[lidx[o] * n + j];
     }
+}
+
+// Side 0's list offsets, out[i] for i in [0, n): its CSR offsets of keys [lb, lb + nl) rebased to base, then n_lv (an
+// empty list) for the keys after side 0's.
+__global__ void cogroup_left_offsets_kernel(const u64 *__restrict__ loffs, u32 lb, u32 nl, u64 n, u64 base, u64 n_lv,
+                                            u64 *__restrict__ out)
+{
+    const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) out[i] = i < nl ? loffs[lb + i] - base : n_lv;
 }
 
 // cnt[o] = the length of output key o's list on side j (0 where the side lacks the key)
