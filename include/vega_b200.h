@@ -147,7 +147,8 @@ VB_API int32_t vb_shuffle_set_dist(vb_shuf *s, uint32_t rank, uint32_t world);
 /* do_shuffle_task for one map partition.  AoS = the reference's native Vec<(K,V)> layout
  * (16-byte rows); SoA = separate key/value arrays (vals may be NULL for VB_AGG_COUNT and
  * key-only VB_AGG_SORT).  Re-submitting a map_id overwrites it (stage resubmission,
- * src/scheduler/local_scheduler.rs:248-256).                                                */
+ * src/scheduler/local_scheduler.rs:248-256).  AoS rows on the device must start on a 16-byte
+ * boundary (VB_ERR_INVALID otherwise); host rows may start anywhere.                         */
 VB_API int32_t vb_shuffle_map_aos(vb_shuf *s, uint32_t map_id, const void *rows, uint64_t n_rows, int32_t src_loc);
 VB_API int32_t vb_shuffle_map_soa(vb_shuf *s, uint32_t map_id, const void *keys, const void *vals,
                                   uint64_t n_rows, int32_t src_loc);

@@ -1484,6 +1484,9 @@ static int shuffle_map(vb_shuf *s, u32 map_id, const u64 *rows, const u64 *keys,
 extern "C" int32_t vb_shuffle_map_aos(vb_shuf *s, uint32_t map_id, const void *rows, uint64_t n, int32_t loc)
 {
     if (s && s->multi) return reject_multi(s, "AoS rows");
+    // every AoS loader reads a row as one 16-byte vector load; host rows are copied into aligned buffers first
+    if (n && loc != VB_HOST && ((uintptr_t)rows & 15u))
+        return set_err(VB_ERR_INVALID, "device AoS rows at %p: 16-byte rows must start on a 16-byte boundary", rows);
     return shuffle_map(s, map_id, (const u64 *)rows, nullptr, nullptr, n, loc);
 }
 extern "C" int32_t vb_shuffle_map_soa(vb_shuf *s, uint32_t map_id, const void *keys, const void *vals, uint64_t n, int32_t loc)
