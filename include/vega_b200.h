@@ -21,6 +21,7 @@
  *   vb_cogroup*            <- CoGroupedRdd::compute for PairRdd::cogroup  src/rdd/co_grouped_rdd.rs:206-249
  *   vb_cogroup_n* / vb_join_n*
  *                          <- CoGroupedRdd::compute with any number of parents (co_grouped_rdd.rs:75-135, 206-249)
+ *   vb_join_n_outer*       <- nothing: vega has no outer joins (N-way, over the same cogroup, new)
  *   vb_shuffle_free        <- (the reference never evicts SHUFFLE_CACHE, src/env.rs:27)
  *   vb_slice               <- ParallelCollection::slice           src/rdd/parallel_collection_rdd.rs:116-145
  *   vb_shuffle_export_* / vb_shuffle_import
@@ -353,6 +354,28 @@ VB_API int32_t vb_cogroup_n(vb_shuf *const *sides, uint32_t n_sides, uint32_t re
 VB_API int32_t vb_join_n_size(vb_shuf *const *sides, uint32_t n_sides, uint32_t reduce_id, uint64_t *n_out);
 VB_API int32_t vb_join_n(vb_shuf *const *sides, uint32_t n_sides, uint32_t reduce_id, void *out_k,
                          void *const *out_vals /*[n_sides]*/, int32_t dst_loc);
+
+/* Outer join of all sides, for one partition (CoGroupedRdd::compute, src/rdd/co_grouped_rdd.rs:206-249, expanded as
+ * PairRdd::join does, src/rdd/pair_rdd.rs:104-121; the reference has no outer join, so there is no reference output to
+ * compare against).  Bit j of `required` marks side j as required.  A key of the partition, with lists l_0 .. l_{n-1}
+ * in cogroup order, gives rows only if every required side has it.  A side that has the key contributes l_j; an
+ * optional side that lacks it contributes the single slot [None].  So the key gives prod_j max(|l_j|, 1) rows,
+ * contiguous, in the order
+ *   for v0 in L0 { for v1 in L1 { ... } } -> (k, v0, v1, ..., v_{n-1})      (the last side varies fastest)
+ * and the order of keys within the partition is unspecified.  A None slot holds 0 and its validity byte is 0.
+ * required = all sides is vb_join_n; for two sides 0b01 is vb_join_outer LEFT, 0b10 RIGHT and 0 FULL.  For more sides
+ * required = 1 is `a LEFT JOIN b LEFT JOIN c ...` on the same key, and 0 the chained full outer join.
+ * Argument rules: vb_cogroup_n's, and a required bit at n_sides or above is VB_ERR_INVALID.  Once the partition has
+ * rows, out_k, out_vals and every entry of it must be non-NULL (VB_ERR_INVALID).  out_valid [n_sides] (one byte per
+ * row, same dst_loc) is optional, and so is each entry: an entry given is written for every row, including the 1s.  A
+ * key's product, or the partition's total, of 2^63 rows or more is VB_ERR_TOO_LARGE from the size call.  The size call
+ * keeps the plan on sides[0] for the write call, as vb_join_n_size does.  On a rank of a multi-rank shuffle only the
+ * partitions that rank owns have rows.                                                                               */
+VB_API int32_t vb_join_n_outer_size(vb_shuf *const *sides, uint32_t n_sides, uint32_t reduce_id, uint32_t required,
+                                    uint64_t *n_out);
+VB_API int32_t vb_join_n_outer(vb_shuf *const *sides, uint32_t n_sides, uint32_t reduce_id, uint32_t required,
+                               void *out_k, void *const *out_vals /*[n_sides]*/,
+                               uint8_t *const *out_valid /*[n_sides] or NULL; entries may be NULL*/, int32_t dst_loc);
 
 /* ---- string keys: byte-string keys that hash like Rust `String` (reduce_by_key / count_by_key / count_by_value /
  *      distinct / group_by_key / partition_by_key over `String` keys, examples/group_by.rs, tests/test_pair_rdd.rs:8-37)

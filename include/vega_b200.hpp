@@ -330,6 +330,37 @@ public:
         return out;
     }
 
+    // outer join of [self, others...] (vega has none): bit j of `required` marks parent j (this one is 0) required.  A
+    // key on every required parent gives, for v0 in L0 { for v1 in L1 { ... } }, (k, [v_0, ..., v_{n-1}]) where L_j is
+    // parent j's list, or [std::nullopt] for an optional parent that lacks the key.  A key's rows are contiguous.
+    std::vector<std::pair<K, std::vector<std::optional<V>>>> join_n_outer(const std::vector<PairRddT> &others, size_t num_splits,
+                                                                          uint32_t required) const
+    {
+        auto shs = cogroup_shuffles(others, num_splits);
+        std::vector<vb_shuf *> sides;
+        for (auto &s : shs) sides.push_back(s.get());
+        const uint32_t n = (uint32_t)sides.size();
+        std::vector<std::pair<K, std::vector<std::optional<V>>>> out;
+        for (uint32_t r = 0; r < num_splits; ++r) {
+            uint64_t rows = 0;
+            check(vb_join_n_outer_size(sides.data(), n, r, required, &rows));
+            std::vector<uint64_t> k(rows);
+            std::vector<std::vector<uint64_t>> vals(n, std::vector<uint64_t>(rows));
+            std::vector<std::vector<uint8_t>> valid(n, std::vector<uint8_t>(rows));
+            std::vector<void *> vp(n);
+            std::vector<uint8_t *> ok(n);
+            for (uint32_t j = 0; j < n; ++j) { vp[j] = vals[j].data(); ok[j] = valid[j].data(); }
+            check(vb_join_n_outer(sides.data(), n, r, required, k.data(), vp.data(), ok.data(), VB_HOST));
+            for (uint64_t i = 0; i < rows; ++i) {
+                std::vector<std::optional<V>> row(n);
+                for (uint32_t j = 0; j < n; ++j)
+                    if (valid[j][i]) row[j] = detail::from_bits<V>(vals[j][i]);
+                out.emplace_back(detail::from_bits<K>(k[i]), std::move(row));
+            }
+        }
+        return out;
+    }
+
     std::shared_ptr<Context> sc_;
     size_t num_slices_;
     std::vector<uint64_t> keys_, vals_;

@@ -59,6 +59,12 @@ extern "C" {
     pub fn vb_join_n_size(sides: *const *mut vb_shuf, n_sides: u32, reduce_id: u32, n_out: *mut u64) -> i32;
     pub fn vb_join_n(sides: *const *mut vb_shuf, n_sides: u32, reduce_id: u32, out_k: *mut c_void,
                      out_vals: *const *mut c_void, dst_loc: i32) -> i32;
+    // outer join of all sides: bit j of `required` marks side j required; a missing optional side is one None slot
+    // (value 0, validity byte 0).  out_valid and its entries may be NULL
+    pub fn vb_join_n_outer_size(sides: *const *mut vb_shuf, n_sides: u32, reduce_id: u32, required: u32,
+                                n_out: *mut u64) -> i32;
+    pub fn vb_join_n_outer(sides: *const *mut vb_shuf, n_sides: u32, reduce_id: u32, required: u32, out_k: *mut c_void,
+                           out_vals: *const *mut c_void, out_valid: *const *mut u8, dst_loc: i32) -> i32;
     // N1: bincode blobs (the payload format of SHUFFLE_CACHE)
     pub fn vb_shuffle_reduce_blob_size(s: *mut vb_shuf, reduce_id: u32, n_bytes: *mut u64) -> i32;
     pub fn vb_shuffle_reduce_blob(s: *mut vb_shuf, reduce_id: u32, out_blob: *mut c_void, dst_loc: i32) -> i32;

@@ -18,7 +18,8 @@ ap = argparse.ArgumentParser()
 ap.add_argument("--rows", type=float, default=1e9)
 ap.add_argument("--distinct", type=float, default=1e6)
 ap.add_argument("--ops", default="reduce,group,sort,sortkv,join,count")   # also: zipf, zipfgroup, combine, combinezipf,
-#                                                                             leftjoin, fulljoin, cogroup, cogroup3, join3
+#                                                                             leftjoin, fulljoin, cogroup, cogroup3, join3,
+#                                                                             join3outer
 ap.add_argument("--reps", type=int, default=3)
 args = ap.parse_args()
 N, D = int(args.rows), int(args.distinct)
@@ -93,7 +94,7 @@ if "sort" in ops:
     report("sort_by_key(keys only)", N, 16.0 * N, timed(lambda: run_shuffle(L.VB_AGG_SORT, keys=keys), max(1, args.reps - 1)))
     del keys
     torch.cuda.empty_cache()
-join_ops = [o for o in ("join", "leftjoin", "fulljoin", "cogroup", "cogroup3", "join3") if o in ops]
+join_ops = [o for o in ("join", "leftjoin", "fulljoin", "cogroup", "cogroup3", "join3", "join3outer") if o in ops]
 if join_ops:
     # BASELINE config 4, per-GPU share at 8 GPUs: 6.25e7 rows per side, each rank once per side,
     # 1.25e6 shared keys per GPU (1e7 / 8)
@@ -216,7 +217,7 @@ if "leftjoin" in ops or "fulljoin" in ops or "cogroup" in ops or "cogroup3" in o
         extra = {"gpu": card["name"], "power_limit_w": card["power_limit_w"], "cogroup_keys": want,
                  "cogroup_both_sides_ms": round(med(r_cog), 3)}
         report("cogroup", 2 * n_side, 32.0 * n_side + 24.0 * want, res, extra)
-if "cogroup3" in ops or "join3" in ops:
+if "cogroup3" in ops or "join3" in ops or "join3outer" in ops:
     # The join shape with a third side that shares the same 2 % of the keys (its other keys are on no other side), 8 -> 8,
     # device outputs.  vb_cogroup_n of 3 sides against the grouping alone (vb_shuffle_reduce of every partition of the 3
     # sides); vb_cogroup_n of 2 sides against vb_cogroup of the same pair; vb_join_n of 3 sides against vb_join of 2.
@@ -320,6 +321,34 @@ if "cogroup3" in ops or "join3" in ops:
         res = timed(join_n([a, b, c]), args.reps)
         assert res[-1][1]["join_rows"] == shared, (res[-1][1]["join_rows"], shared)
         report("join_n 3 sides", rows3, 16.0 * rows3 + 8.0 * 4 * shared, res, dict(info, join_rows=shared, vb_join_2_sides_ms=round(med(r_two), 3)))
+    if "join3outer" in ops:
+        # vb_join_n_outer of the same 3 sides with every side required (the inner join's rows, plus validity) and
+        # with side 0 required (a LEFT JOIN b LEFT JOIN c: every key of a once), against vb_join_n of the 3 sides.
+        # Written bytes per row: the key, 3 values and 3 validity bytes.
+        def join_n_outer(ts, mask):
+            def run():
+                shs = sides_of(ts)
+                n = len(shs)
+                arr = (ctypes.c_void_p * n)(*[s_._h.value for s_ in shs])
+                tot = 0
+                for r in range(8):
+                    nn = ctypes.c_uint64()
+                    L.check(sc._lib.vb_join_n_outer_size(arr, n, r, mask, ctypes.byref(nn)))
+                    k, vs = dev(nn.value), [dev(nn.value) for _ in range(n)]
+                    oks = [torch.empty(nn.value, dtype=torch.uint8, device="cuda") for _ in range(n)]
+                    L.check(sc._lib.vb_join_n_outer(arr, n, r, mask, p(k), (ctypes.c_void_p * n)(*[p(x) for x in vs]),
+                                                    (ctypes.c_void_p * n)(*[p(x) for x in oks]), L.VB_DEVICE))
+                    tot += nn.value
+                return finish(shs, join_rows=tot)
+            return run
+
+        r_inner = timed(join_n([a, b, c]), args.reps)
+        for mask, want in ((0b111, shared), (0b001, n_side)):
+            res = timed(join_n_outer([a, b, c], mask), args.reps)
+            assert res[-1][1]["join_rows"] == want, (res[-1][1]["join_rows"], want)
+            written = (8.0 + 3 * 8.0 + 3.0) * want
+            report(f"join_n_outer 3 sides required={mask:#05b}", rows3, 16.0 * rows3 + written, res,
+                   dict(info, join_rows=want, written_GBps=written / med(res) / 1e6, join_n_3_sides_ms=round(med(r_inner), 3)))
     del c
     torch.cuda.empty_cache()
 if "combine" in ops or "combinezipf" in ops:

@@ -285,16 +285,18 @@ struct JoinPlan {
     u64 total_left = 0;            // rows of the left keys (pos[nl])
 };
 
-// vb_cogroup_n_size / vb_join_n_size's result for one (sides, partition), kept for the write call.  Cogroup output
-// keys: side 0's keys in its CSR order, then each later side's new keys (those no earlier side has) in that side's CSR
-// order.  A join reads side 0's keys only.
+// vb_cogroup_n_size / vb_join_n_size / vb_join_n_outer_size's result for one (sides, partition, kind), kept for the
+// write call.  Cogroup output keys: side 0's keys in its CSR order, then each later side's new keys (those no earlier
+// side has) in that side's CSR order.  A join whose side 0 is required (every inner join) reads side 0's keys only.
 struct CogroupNPlan {
-    u64 n_keys = 0;                // cogroup: output keys; join: side 0's keys of the partition
-    u64 *new_keys = nullptr;       // cogroup: [n_keys - side 0's keys] the keys after side 0's
+    u64 n_keys = 0;                // output keys: every key, or side 0's keys of the partition
+    u64 *new_keys = nullptr;       // [n_keys - side 0's keys] the keys after side 0's
     u32 *match = nullptr;          // [n_keys][n_sides] the key's index on every side, 0xFFFFFFFF where a side lacks it
     u64 *pos = nullptr;            // join: [n_keys] each key's first output row
     u64 total = 0;                 // join: rows of the partition
 };
+// n_plans kinds: the cogroup, the inner join, or (>= 0) an outer join by its mask of required sides
+constexpr i64 NP_COGROUP = -2, NP_INNER = -1;
 
 struct vb_shuf {
     vb_ctx *ctx = nullptr;
@@ -353,8 +355,8 @@ struct vb_shuf {
     u32 dict_log_cap = 0;
     u32 *dense_of_slot = nullptr;
     std::map<std::tuple<const vb_shuf *, u32, int>, JoinPlan> join_plans;   // by (right side, partition, outer kind)
-    // on side 0 of a cogroup or an inner join, of two sides or N: by (every side's uid, partition, join?)
-    std::map<std::tuple<std::vector<u64>, u32, bool>, CogroupNPlan> n_plans;
+    // on side 0 of a cogroup or a join, of two sides or N: by (every side's uid, partition, NP_* kind or outer mask)
+    std::map<std::tuple<std::vector<u64>, u32, i64>, CogroupNPlan> n_plans;
     // COGROUP shuffles are grouped lazily: seal keeps the (owned) rows; the CSR is built by the first reduce call
     // (cogroup materialisation), or — if a join comes first — only for the rows the join kind needs: the keys on BOTH
     // sides (inner), every row of the preserved side plus the matching rows of the other (LEFT / RIGHT), or all (FULL).
@@ -3406,18 +3408,22 @@ static int cogroup_n_sides(vb_shuf *const *sides, u32 n, u32 rid, CogroupNSides 
     return VB_OK;
 }
 
-static int cogroup_n_plan(vb_shuf *const *sides, u32 n, u32 rid, bool join, const CogroupNSides &a, CogroupNPlan **out)
+// kind: NP_COGROUP, NP_INNER, or an outer join's mask of required sides
+static int cogroup_n_plan(vb_shuf *const *sides, u32 n, u32 rid, i64 kind, const CogroupNSides &a, CogroupNPlan **out)
 {
     vb_shuf *s0 = sides[0];
     vb_ctx *c = s0->ctx;
     std::vector<u64> uids(n);
     for (u32 j = 0; j < n; ++j) uids[j] = sides[j]->uid;
-    auto key = std::make_tuple(uids, rid, join);
+    auto key = std::make_tuple(uids, rid, kind);
     auto it = s0->n_plans.find(key);
     if (it != s0->n_plans.end()) { *out = &it->second; return VB_OK; }
+    const bool join = kind != NP_COGROUP;
+    // a join that requires side 0 has rows only for side 0's keys; every other plan takes the union of the keys
+    const bool all_keys = kind == NP_COGROUP || (kind >= 0 && !(kind & 1));
     std::vector<u64> nk(n);
     u64 cap = 0;                                       // output keys at most
-    for (u32 j = 0; j < n && (j == 0 || !join); ++j) {
+    for (u32 j = 0; j < n && (j == 0 || all_keys); ++j) {
         nk[j] = sides[j]->bucket_off[rid + 1] - sides[j]->bucket_off[rid];
         cap += nk[j];
     }
@@ -3431,7 +3437,7 @@ static int cogroup_n_plan(vb_shuf *const *sides, u32 n, u32 rid, bool join, cons
         TRY(kl.done("cogroup_n_probe_kernel"));
     }
     p.n_keys = nk[0];
-    if (!join && cap > nk[0]) {
+    if (all_keys && cap > nk[0]) {
         TRY(new_keys.alloc((cap - nk[0]) * 8));
         for (u32 i = 1; i < n; ++i) {
             if (!nk[i]) continue;
@@ -3463,11 +3469,16 @@ static int cogroup_n_plan(vb_shuf *const *sides, u32 n, u32 rid, bool join, cons
         CU(cudaMemsetAsync(flags.p, 0, 24, c->stream));
         unsigned long long *sums = flags.as<unsigned long long>();
         u32 *too_large = (u32 *)(sums + 2);
-        {
+        if (kind == NP_INNER) {
             KLaunch kl(s0, K_JOIN);
             join_n_count_kernel<<<(unsigned)((p.n_keys + 255) / 256), 256, 0, c->stream>>>(a, match.as<u32>(), (u32)p.n_keys,
                                                                                           cnt.as<u64>(), sums, too_large);
             TRY(kl.done("join_n_count_kernel"));
+        } else {
+            KLaunch kl(s0, K_JOIN);
+            join_n_outer_count_kernel<<<(unsigned)((p.n_keys + 255) / 256), 256, 0, c->stream>>>(
+                a, match.as<u32>(), (u32)p.n_keys, (u32)kind, cnt.as<u64>(), sums, too_large);
+            TRY(kl.done("join_n_outer_count_kernel"));
         }
         TRY(exclusive_scan_u64(s0, cnt.as<u64>(), pos.as<u64>(), p.n_keys, nullptr));
         u64 *h = (u64 *)c->h_scratch;
@@ -3486,11 +3497,11 @@ static int cogroup_n_plan(vb_shuf *const *sides, u32 n, u32 rid, bool join, cons
     return VB_OK;
 }
 
-static void drop_cogroup_n_plan(vb_shuf *const *sides, u32 n, u32 rid, bool join)
+static void drop_cogroup_n_plan(vb_shuf *const *sides, u32 n, u32 rid, i64 kind)
 {
     std::vector<u64> uids(n);
     for (u32 j = 0; j < n; ++j) uids[j] = sides[j]->uid;
-    auto it = sides[0]->n_plans.find(std::make_tuple(uids, rid, join));
+    auto it = sides[0]->n_plans.find(std::make_tuple(uids, rid, kind));
     if (it == sides[0]->n_plans.end()) return;
     free_cogroup_n_plan(sides[0]->ctx, it->second);
     sides[0]->n_plans.erase(it);
@@ -3503,7 +3514,7 @@ static int cogroup_n_size(vb_shuf *const *sides, u32 n_sides, u32 rid, u64 *n_ke
     CogroupNSides a;
     TRY(cogroup_n_sides(sides, n_sides, rid, &a));
     CogroupNPlan *p = nullptr;
-    TRY(cogroup_n_plan(sides, n_sides, rid, false, a, &p));
+    TRY(cogroup_n_plan(sides, n_sides, rid, NP_COGROUP, a, &p));
     if (n_keys) *n_keys = p->n_keys;
     for (u32 j = 0; n_vals && j < n_sides; ++j) n_vals[j] = sides[j]->val_off[rid + 1] - sides[j]->val_off[rid];
     return VB_OK;
@@ -3517,7 +3528,7 @@ static int cogroup_n_write(vb_shuf *const *sides, u32 n_sides, u32 rid, void *ou
     CogroupNSides a;
     TRY(cogroup_n_sides(sides, n_sides, rid, &a));
     CogroupNPlan *p = nullptr;
-    TRY(cogroup_n_plan(sides, n_sides, rid, false, a, &p));
+    TRY(cogroup_n_plan(sides, n_sides, rid, NP_COGROUP, a, &p));
     const u64 nk = p->n_keys, nk0 = s0->bucket_off[rid + 1] - s0->bucket_off[rid];
     int rc = [&]() -> int {
         TRY(copy_out(s0, out_keys, s0->res_keys ? s0->res_keys + a.kb[0] : nullptr, nk0 * 8, dst_loc));
@@ -3579,7 +3590,7 @@ static int cogroup_n_write(vb_shuf *const *sides, u32 n_sides, u32 rid, void *ou
         return VB_OK;
     }();
     cudaStreamSynchronize(c->stream);
-    drop_cogroup_n_plan(sides, n_sides, rid, false);
+    drop_cogroup_n_plan(sides, n_sides, rid, NP_COGROUP);
     return rc;
 }
 
@@ -3588,7 +3599,7 @@ static int join_n_size(vb_shuf *const *sides, u32 n_sides, u32 rid, u64 *n_out)
     CogroupNSides a;
     TRY(cogroup_n_sides(sides, n_sides, rid, &a));
     CogroupNPlan *p = nullptr;
-    TRY(cogroup_n_plan(sides, n_sides, rid, true, a, &p));
+    TRY(cogroup_n_plan(sides, n_sides, rid, NP_INNER, a, &p));
     *n_out = p->total;
     return VB_OK;
 }
@@ -3600,7 +3611,7 @@ static int join_n_write(vb_shuf *const *sides, u32 n_sides, u32 rid, void *out_k
     CogroupNSides a;
     TRY(cogroup_n_sides(sides, n_sides, rid, &a));
     CogroupNPlan *p = nullptr;
-    TRY(cogroup_n_plan(sides, n_sides, rid, true, a, &p));
+    TRY(cogroup_n_plan(sides, n_sides, rid, NP_INNER, a, &p));
     const u64 total = p->total;
     int rc = [&]() -> int {
         if (!total) return VB_OK;
@@ -3629,7 +3640,75 @@ static int join_n_write(vb_shuf *const *sides, u32 n_sides, u32 rid, void *out_k
         return VB_OK;
     }();
     cudaStreamSynchronize(c->stream);
-    drop_cogroup_n_plan(sides, n_sides, rid, true);
+    drop_cogroup_n_plan(sides, n_sides, rid, NP_INNER);
+    return rc;
+}
+
+// Outer join of n sides (a key is kept when every side of `required` has it; a missing optional side gives one None
+// slot): the plan of the union of the keys (side 0's keys alone when side 0 is required), counted with max(len, 1)
+static int join_n_outer_size(vb_shuf *const *sides, u32 n_sides, u32 rid, u32 required, u64 *n_out)
+{
+    CogroupNSides a;
+    TRY(cogroup_n_sides(sides, n_sides, rid, &a));
+    CogroupNPlan *p = nullptr;
+    TRY(cogroup_n_plan(sides, n_sides, rid, required, a, &p));
+    *n_out = p->total;
+    return VB_OK;
+}
+
+static int join_n_outer_write(vb_shuf *const *sides, u32 n_sides, u32 rid, u32 required, void *out_k, void *const *out_vals,
+                              uint8_t *const *out_valid, int dst_loc)
+{
+    vb_shuf *s0 = sides[0];
+    vb_ctx *c = s0->ctx;
+    CogroupNSides a;
+    TRY(cogroup_n_sides(sides, n_sides, rid, &a));
+    CogroupNPlan *p = nullptr;
+    TRY(cogroup_n_plan(sides, n_sides, rid, required, a, &p));
+    const u64 total = p->total;
+    int rc = [&]() -> int {
+        if (!total) return VB_OK;
+        bool missing = !out_k || !out_vals;
+        for (u32 j = 0; !missing && j < n_sides; ++j) missing = !out_vals[j];
+        if (missing) return set_err(VB_ERR_INVALID, "NULL output with %llu rows to write", (unsigned long long)total);
+        JoinNOuterOut o{};
+        DevBuf bufs[2 * CGN_MAX_SIDES + 1];     // host output: keys, values per side, validity per side
+        o.k = (u64 *)out_k;
+        o.new_keys = p->new_keys;
+        o.nk0 = (u32)(s0->bucket_off[rid + 1] - s0->bucket_off[rid]);
+        for (u32 j = 0; j < n_sides; ++j) {
+            o.v[j] = (u64 *)out_vals[j];
+            o.valid[j] = out_valid ? out_valid[j] : nullptr;
+        }
+        if (dst_loc == VB_HOST) {
+            for (u32 j = 0; j <= n_sides; ++j) { bufs[j].c = c; TRY(bufs[j].alloc(total * 8)); }
+            o.k = bufs[n_sides].as<u64>();
+            for (u32 j = 0; j < n_sides; ++j) {
+                o.v[j] = bufs[j].as<u64>();
+                if (!o.valid[j]) continue;
+                DevBuf &b = bufs[n_sides + 1 + j];
+                b.c = c;
+                TRY(b.alloc(total));
+                o.valid[j] = b.as<unsigned char>();
+            }
+        }
+        {
+            KLaunch kl(s0, K_JOIN);
+            const u64 blocks = std::min<u64>((total + 255) / 256, (u64)c->sm_count * 8);
+            join_n_outer_expand_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(a, p->pos, (u32)p->n_keys, total, p->match, o);
+            TRY(kl.done("join_n_outer_expand_kernel"));
+        }
+        if (dst_loc == VB_HOST) {
+            TRY(copy_out(s0, out_k, o.k, total * 8, VB_HOST));
+            for (u32 j = 0; j < n_sides; ++j) {
+                TRY(copy_out(s0, out_vals[j], o.v[j], total * 8, VB_HOST));
+                if (o.valid[j]) TRY(copy_out(s0, out_valid[j], o.valid[j], total, VB_HOST));
+            }
+        }
+        return VB_OK;
+    }();
+    cudaStreamSynchronize(c->stream);
+    drop_cogroup_n_plan(sides, n_sides, rid, required);
     return rc;
 }
 
@@ -3676,6 +3755,39 @@ extern "C" int32_t vb_join_n(vb_shuf *const *sides, uint32_t n_sides, uint32_t r
     CU(cudaSetDevice(c->device));
     for (u32 j = 0; j < n_sides; ++j) TRY(ensure_grouped(sides[j]));
     return join_n_write(sides, n_sides, rid, out_k, out_vals, dst_loc);
+}
+
+// vb_cogroup_n's rules, and no required bit at or above n_sides
+static int join_n_outer_check(vb_shuf *const *sides, u32 n_sides, u32 rid, u32 required)
+{
+    TRY(cogroup_n_check(sides, n_sides, rid));
+    if (required >> n_sides)                           // n_sides <= 16 here
+        return set_err(VB_ERR_INVALID, "required mask %#x names a side >= n_sides %u", required, n_sides);
+    return VB_OK;
+}
+
+extern "C" int32_t vb_join_n_outer_size(vb_shuf *const *sides, uint32_t n_sides, uint32_t rid, uint32_t required,
+                                        uint64_t *n_out)
+{
+    TRY(join_n_outer_check(sides, n_sides, rid, required));
+    if (!n_out) return set_err(VB_ERR_INVALID, "n_out is NULL");
+    vb_ctx *c = sides[0]->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    for (u32 j = 0; j < n_sides; ++j) TRY(ensure_grouped(sides[j]));
+    return join_n_outer_size(sides, n_sides, rid, required, n_out);
+}
+
+extern "C" int32_t vb_join_n_outer(vb_shuf *const *sides, uint32_t n_sides, uint32_t rid, uint32_t required, void *out_k,
+                                   void *const *out_vals, uint8_t *const *out_valid, int32_t dst_loc)
+{
+    TRY(join_n_outer_check(sides, n_sides, rid, required));
+    if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
+    vb_ctx *c = sides[0]->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    for (u32 j = 0; j < n_sides; ++j) TRY(ensure_grouped(sides[j]));
+    return join_n_outer_write(sides, n_sides, rid, required, out_k, out_vals, out_valid, dst_loc);
 }
 
 extern "C" int32_t vb_cogroup_size(vb_shuf *l, vb_shuf *r, uint32_t rid, uint64_t *n_keys, uint64_t *n_left_vals,

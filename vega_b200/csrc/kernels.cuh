@@ -1790,6 +1790,88 @@ __global__ void join_n_expand_kernel(const __grid_constant__ CogroupNSides a, co
     }
 }
 
+// N-way outer join over the keys of a cogroup plan (side 0's nk0 keys, then new_keys).  A side is required when its bit
+// of `required` is set; an optional side that lacks the key takes one None slot (value 0, validity 0).  The expand
+// needs no mask: a key that lacks a required side has no rows, so every 0xFFFFFFFF it meets is an optional side.
+struct JoinNOuterOut {
+    u64 *k;
+    u64 *v[CGN_MAX_SIDES];
+    unsigned char *valid[CGN_MAX_SIDES];   // NULL entries are not written
+    const u64 *new_keys;                   // output keys nk0 .. of the plan
+    u32 nk0;
+};
+
+// Output keys o < nk: cnt[o] = 0 if a required side lacks the key, else the product over all sides of max(len, 1).
+// Overflow and the hi / lo sums as join_n_count_kernel.
+__global__ void join_n_outer_count_kernel(const __grid_constant__ CogroupNSides a, const u32 *__restrict__ match, u32 nk,
+                                          u32 required, u64 *__restrict__ cnt, unsigned long long *__restrict__ sums,
+                                          u32 *__restrict__ too_large)
+{
+    const u32 o = blockIdx.x * blockDim.x + threadIdx.x;
+    u64 c = 0;
+    if (o < nk) {
+        const u32 *row = match + (u64)o * a.n;
+        bool kept = true;
+        for (u32 j = 0; j < a.n; ++j) kept = kept && (row[j] != 0xFFFFFFFFu || !((required >> j) & 1u));
+        if (kept) {
+            c = 1;
+            for (u32 j = 0; j < a.n && c; ++j) {
+                if (row[j] == 0xFFFFFFFFu) continue;
+                const u64 len = a.offs[j][row[j] + 1] - a.offs[j][row[j]];
+                const u64 p = c * len;
+                if (__umul64hi(c, len) || (p >> 63)) { atomicOr(too_large, 1u); c = 0; }
+                else c = p;
+            }
+        }
+        cnt[o] = c;
+    }
+    u64 hi = c >> 32, lo = c & 0xFFFFFFFFull;
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+        hi += __shfl_down_sync(0xffffffffu, hi, off);
+        lo += __shfl_down_sync(0xffffffffu, lo, off);
+    }
+    if ((threadIdx.x & 31) == 0 && (hi | lo)) {
+        atomicAdd(&sums[0], (unsigned long long)hi);
+        atomicAdd(&sums[1], (unsigned long long)lo);
+    }
+}
+
+// One thread per output row, as join_n_expand_kernel: the digit of a side that lacks the key has radix 1 (always 0)
+// and gives a None slot.
+__global__ void join_n_outer_expand_kernel(const __grid_constant__ CogroupNSides a, const u64 *__restrict__ pos, u32 nk,
+                                           u64 total, const u32 *__restrict__ match, const __grid_constant__ JoinNOuterOut out)
+{
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 o = (u64)blockIdx.x * blockDim.x + threadIdx.x; o < total; o += stride) {
+        u32 lo = 0, hi = nk;
+        while (hi - lo > 1) {
+            const u32 mid = (lo + hi) >> 1;
+            if (pos[mid] <= o) lo = mid; else hi = mid;
+        }
+        const u32 *row = match + (u64)lo * a.n;
+        u64 local = o - pos[lo];
+        for (u32 j = a.n; j-- > 0;) {
+            const u32 m = row[j];
+            if (m == 0xFFFFFFFFu) {
+                out.v[j][o] = 0;
+                if (out.valid[j]) out.valid[j][o] = 0;
+                continue;
+            }
+            const u64 b = a.offs[j][m];
+            u64 d = local;
+            if (j) {
+                const u64 len = a.offs[j][m + 1] - b;
+                local = d / len;
+                d -= local * len;
+            }
+            out.v[j][o] = a.vals[j][b + d];
+            if (out.valid[j]) out.valid[j][o] = 1;
+        }
+        out.k[o] = lo < out.nk0 ? a.keys[0][a.kb[0] + lo] : out.new_keys[lo - out.nk0];
+    }
+}
+
 // ---------------------------------------------------------------------------------------------
 // bincode 1.2.1 blob codec (SURVEY §8(f) N1): pure byte shuffling, HBM-bound
 // ---------------------------------------------------------------------------------------------

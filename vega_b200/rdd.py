@@ -549,7 +549,8 @@ class CoGroupedRdd(_Base):
     is values_j[offsets_j[i]:offsets_j[i + 1]], empty where that parent lacks the key.  collect() gives the
     reference's Vec<(K, Vec<Vec<V>>)> as a list of (k, [vs_0, ..., vs_{n-1}]).  join_compute(r) / join_collect() give
     the inner join of all parents as (k, [v_0, ..., v_{n-1}]) arrays: per key, for v0 in vs_0 { for v1 in vs_1 { ... } }.
-    Each parent's values keep that parent's dtype."""
+    outer_join_compute(r, required) / outer_join_collect(required) give the outer join in which only the required
+    parents must have the key.  Each parent's values keep that parent's dtype."""
 
     def __init__(self, rdds, num_splits):
         rdds = list(rdds)
@@ -618,6 +619,53 @@ class CoGroupedRdd(_Base):
         parts = [self.join_compute(r) for r in range(self.num_slices)]
         return (np.concatenate([p[0] for p in parts]),
                 [np.concatenate([p[1][j] for p in parts]) for j in range(len(self.rdds))])
+
+    def _required_mask(self, required):
+        """`required` as a bitmask over the parents: an int mask, or an iterable of parent indices."""
+        n = len(self.rdds)
+        is_int = lambda x: isinstance(x, (int, np.integer)) and not isinstance(x, (bool, np.bool_))
+        if is_int(required):
+            mask = int(required)
+            if not 0 <= mask < 1 << n:
+                raise ValueError(f"required mask {mask:#x} names a parent outside 0..{n - 1}")
+            return mask
+        try:
+            sides = list(required)
+        except TypeError:
+            raise TypeError(f"required must be a bitmask or an iterable of parent indices, got {required!r}") from None
+        mask = 0
+        for j in sides:
+            if not is_int(j):
+                raise TypeError(f"required: parent index {j!r} is not an integer")
+            if not 0 <= j < n:
+                raise ValueError(f"required: parent index {j} is outside 0..{n - 1}")
+            mask |= 1 << int(j)
+        return mask
+
+    def outer_join_compute(self, split, required):
+        """Partition `split` of the outer join of all parents (vb_join_n_outer): (k, [v_0, ..., v_{n-1}]).  A key is
+        kept if every required parent has it; an optional parent that lacks it gives one None slot, so the key gives
+        prod max(len(vs_j), 1) rows, for v0 in vs_0 { for v1 in vs_1 { ... } }.  An optional parent's column is a
+        numpy.ma.MaskedArray (masked = None, data 0), a required parent's a plain array.  `required` is a bitmask over
+        the parents or an iterable of parent indices: all of them is join_compute, none is the full outer join."""
+        mask = self._required_mask(required)
+        shs, sides = self._sides()
+        n, lib = len(shs), self.sc._lib
+        nn = ctypes.c_uint64()
+        L.check(lib.vb_join_n_outer_size(sides, n, split, mask, ctypes.byref(nn)))
+        k = np.empty(nn.value, dtype=_NP_OF[shs[0].kcode])
+        vs = [np.empty(nn.value, dtype=_NP_OF[s.vcode]) for s in shs]
+        valid = [None if mask >> j & 1 else np.empty(nn.value, dtype=np.uint8) for j in range(n)]
+        ptrs = lambda xs: (ctypes.c_void_p * n)(*[x.ctypes.data if x is not None else None for x in xs])
+        L.check(lib.vb_join_n_outer(sides, n, split, mask, k.ctypes.data_as(ctypes.c_void_p), ptrs(vs), ptrs(valid),
+                                    L.VB_HOST))
+        return k, [v if ok is None else np.ma.MaskedArray(v, mask=ok == 0) for v, ok in zip(vs, valid)]
+
+    def outer_join_collect(self, required):
+        mask = self._required_mask(required)
+        parts = [self.outer_join_compute(r, mask) for r in range(self.num_slices)]
+        cat = lambda xs: np.ma.concatenate(xs) if isinstance(xs[0], np.ma.MaskedArray) else np.concatenate(xs)
+        return np.concatenate([p[0] for p in parts]), [cat([p[1][j] for p in parts]) for j in range(len(self.rdds))]
 
 
 class CombinedRdd(_Base):
