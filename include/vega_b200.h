@@ -158,7 +158,8 @@ VB_API int32_t vb_shuffle_map_soa(vb_shuf *s, uint32_t map_id, const void *keys,
  * rank (combined rows for reduce ops, raw rows in map order for group ops); counts[world] gets
  * rows per destination.  export_buffers returns the packed device arrays (destination-major).
  * The host exchanges them (one all-to-all-v over NCCL) and hands the received rows, source-rank
- * major, to vb_shuffle_import (the buffers are borrowed until vb_shuffle_seal returns).  Then vb_shuffle_seal. */
+ * major, to vb_shuffle_import (the buffers are borrowed until vb_shuffle_seal returns).  Then vb_shuffle_seal.
+ * A VB_AGG_SORT shuffle is refused (VB_ERR_UNSUPPORTED): a multi-rank sort_by_key goes through vb_shuffle_exchange. */
 VB_API int32_t vb_shuffle_export_prepare(vb_shuf *s, uint64_t *counts);
 VB_API int32_t vb_shuffle_export_buffers(vb_shuf *s, void **keys_dev, void **vals_dev);
 VB_API int32_t vb_shuffle_import(vb_shuf *s, const void *keys_dev, const void *vals_dev, const uint64_t *counts);

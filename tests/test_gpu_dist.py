@@ -1,5 +1,5 @@
-"""N>1 path on the GPU: two ranks run the real CudaEngine (export multisplit by destination rank,
-import, seal) and must reproduce the single-process oracle.  With >= 2 GPUs the exchange is the
+"""N>1 path on the GPU: two ranks (three in one fused-exchange case) run the real CudaEngine (export multisplit by
+destination rank, import, seal) and must reproduce the single-process oracle.  With >= 2 GPUs the exchange is the
 library's own (vb_ctx_comm_init + vb_shuffle_exchange: NCCL grouped send/recv or the fused P2P scatter,
 one rank per GPU); on a 1-GPU box both ranks share GPU 0 (NCCL refuses duplicate devices) and the
 all-to-all-v is staged through gloo — the pack/unpack/seal code under test is the same."""
@@ -109,6 +109,26 @@ def test_two_rank_cuda_shuffle_matches_oracle(agg, M, R, p2p):
             assert gd == wd
         else:
             assert dict(zip(got[0].tolist(), got[1].tolist())) == dict(zip(w["keys"].tolist(), w["combined"].tolist()))
+    assert sum(s["sent_rows"] for _, s in per_rank) == sum(s["recv_rows"] for _, s in per_rank) > 0
+
+
+def test_three_rank_p2p_group_matches_oracle():
+    """The fused exchange with two foreign sources per destination: every rank writes its block at its own offset
+    (source-rank major) into the arena of each of the other two.  One rank per GPU with >= 3 GPUs, else all on GPU 0."""
+    from oracle import oracle as O
+    world, M, R = 3, 5, 7
+    nccl = torch.cuda.device_count() >= world
+    with tempfile.TemporaryDirectory() as d:
+        mp.spawn(_worker, args=(world, _free_port(), 0, M, R, nccl, d, True), nprocs=world, join=True)
+        per_rank = [pickle.load(open(os.path.join(d, f"r{r}.pkl"), "rb")) for r in range(world)]
+    keys, vals = _dataset()
+    want = O.shuffle("group", keys, vals, M, R)
+    for r in range(R):
+        got, w = per_rank[r % world][0][r], want[r]
+        gd = {int(k): got[2][int(got[1][i]):int(got[1][i + 1])].tolist() for i, k in enumerate(got[0])}
+        wd = {int(k): w["vals"][int(w["offsets"][i]):int(w["offsets"][i + 1])].tolist() for i, k in enumerate(w["keys"])}
+        assert gd == wd, f"partition {r}"
+    assert all(s["exchange_kind"] == "p2p" for _, s in per_rank)
     assert sum(s["sent_rows"] for _, s in per_rank) == sum(s["recv_rows"] for _, s in per_rank) > 0
 
 

@@ -1916,6 +1916,8 @@ extern "C" int32_t vb_shuffle_export_prepare(vb_shuf *s, uint64_t *counts)
     if (!s || !counts) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "multi-rank exchange");
     if (s->str) return reject_str(s, "multi-rank exchange");
+    // the packing below splits by hash destination; a sort shuffle is range-partitioned by cuts agreed across ranks
+    if (s->agg == VB_AGG_SORT) return set_err(VB_ERR_UNSUPPORTED, "multi-rank sort_by_key goes through vb_shuffle_exchange");
     if (s->world < 2) return set_err(VB_ERR_STATE, "vb_shuffle_export_prepare needs vb_shuffle_set_dist(world > 1)");
     vb_ctx *c = s->ctx;
     std::lock_guard<std::mutex> lk(c->mu);
