@@ -276,6 +276,23 @@ VB_API int32_t vb_shuffle_map_cols(vb_shuf *s, uint32_t map_id, const void *keys
 /* one reduce partition: out_keys[n_keys] and out_aggs[a][n_keys] per aggregate (NULL entries are skipped) */
 VB_API int32_t vb_shuffle_reduce_cols(vb_shuf *s, uint32_t reduce_id, void *out_keys, void *const *out_aggs, int32_t dst_loc);
 
+/* A sealed reduce-op or combine_by_key shuffle as a cogroup / join parent under the same partitioner, without a
+ * shuffle (CoGroupedRdd::new's OneToOneDependency, co_grouped_rdd.rs:103-112).  *out is a new sealed COGROUP-kind
+ * shuffle: its partition r holds partition r of `parent`, each key once, with the one-element list [its result].
+ * out_col: the combine_by_key output column (0 for a single-column shuffle).  Blocks until `parent` is sealed.
+ *   parents   SUM / MIN / MAX / COUNT shuffles, and any output column of a vb_shuffle_create_multi shuffle (MEAN too).
+ *             The view's values are the results bit for bit: the parent's value dtype for SUM / MIN / MAX, u64 for COUNT
+ *             and f64 for MEAN.
+ *   refused   VB_ERR_INVALID, the parent staying usable: NULL arguments, GROUP / COGROUP parents (their lists are
+ *             cogroup sides already; a view is one of them), SORT and string-key parents, out_col out of range.
+ *   use       an ordinary sealed group shuffle: vb_shuffle_reduce* gives the parent's keys, offsets 0..n and the
+ *             results, and every join / cogroup call takes it as any side, next to COGROUP shuffles and other views.
+ *             It has the parent's n_reduce, key width, rank and world: on a rank of a multi-rank shuffle it holds the
+ *             partitions that rank owns.
+ *   memory    the view owns copies of the keys and of the column (16 B per key) and its key dictionary, so the parent
+ *             and the view may be freed in either order; free it with vb_shuffle_free.                              */
+VB_API int32_t vb_shuffle_create_narrow(vb_shuf *parent, uint32_t out_col, vb_shuf **out);
+
 /* Inner join of two sealed GROUP/COGROUP shuffles with equal n_reduce, for one partition:
  * per key `for v in left { for w in right }` (src/rdd/pair_rdd.rs:109-115).                  */
 VB_API int32_t vb_join_size(vb_shuf *left, vb_shuf *right, uint32_t reduce_id, uint64_t *n_out);

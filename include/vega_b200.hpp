@@ -6,6 +6,7 @@
 //   PairRdd::group_by_key / reduce_by_key / join   src/rdd/pair_rdd.rs:35-52,54-80,104-121
 //   Rdd::count_by_value / distinct / collect       src/rdd/rdd.rs:450-459,502-522,420-434
 //   Rdd::intersection / subtract                   src/rdd/rdd.rs:838-946
+//   CoGroupedRdd::new over reduce results          src/rdd/co_grouped_rdd.rs:103-112 (OneToOneDependency; reduce_by_key_rdd)
 // Rows are Vec<(K,V)> with K in {u64,i64,i32,u32,std::string} and V in {u64,i64,f64}; std::string keys are placed
 // like the reference's String keys and support group_by_key / reduce_by_key / count_by_key / count_by_value /
 // distinct.  reduce_by_key takes a named Op (the reference's serde_closure cannot cross into CUDA).  Errors throw vega::Error
@@ -74,6 +75,7 @@ public:
     uint64_t new_shuffle_id() { return next_id_++; }
 
     template <typename K, typename V> class PairRddT;
+    template <typename K, typename V> class ReducedRddT;
     template <typename K> class KeyRddT;
 
     template <typename K, typename V>
@@ -118,6 +120,59 @@ inline ShufPtr run_shuffle(Context &sc, const std::vector<uint64_t> &keys, const
     }
     check(vb_shuffle_seal(raw));
     return s;
+}
+
+// partitions [0, num_splits) of vb_cogroup_n over sealed sides  →  Vec<(K, Vec<Vec<V>>)>
+template <typename K, typename V>
+inline std::vector<std::pair<K, std::vector<std::vector<V>>>> read_cogroup_n(std::vector<vb_shuf *> sides, size_t num_splits)
+{
+    const uint32_t n = (uint32_t)sides.size();
+    std::vector<std::pair<K, std::vector<std::vector<V>>>> out;
+    for (uint32_t r = 0; r < num_splits; ++r) {
+        uint64_t nk = 0;
+        std::vector<uint64_t> nv(n);
+        check(vb_cogroup_n_size(sides.data(), n, r, &nk, nv.data()));
+        std::vector<uint64_t> k(nk);
+        std::vector<std::vector<uint64_t>> offs(n, std::vector<uint64_t>(nk + 1)), vals(n);
+        std::vector<uint64_t *> op(n);
+        std::vector<void *> vp(n);
+        for (uint32_t j = 0; j < n; ++j) { vals[j].resize(nv[j]); op[j] = offs[j].data(); vp[j] = vals[j].data(); }
+        check(vb_cogroup_n(sides.data(), n, r, k.data(), op.data(), vp.data(), VB_HOST));
+        for (uint64_t i = 0; i < nk; ++i) {
+            std::vector<std::vector<V>> lists(n);
+            for (uint32_t j = 0; j < n; ++j)
+                for (uint64_t x = offs[j][i]; x < offs[j][i + 1]; ++x) lists[j].push_back(detail::from_bits<V>(vals[j][x]));
+            out.emplace_back(detail::from_bits<K>(k[i]), std::move(lists));
+        }
+    }
+    return out;
+}
+
+// partitions [0, num_splits) of vb_join_n_outer over sealed sides  →  (k, [v_0 or nullopt, ...]) per row
+template <typename K, typename V>
+inline std::vector<std::pair<K, std::vector<std::optional<V>>>> read_join_n_outer(std::vector<vb_shuf *> sides, size_t num_splits,
+                                                                              uint32_t required)
+{
+    const uint32_t n = (uint32_t)sides.size();
+    std::vector<std::pair<K, std::vector<std::optional<V>>>> out;
+    for (uint32_t r = 0; r < num_splits; ++r) {
+        uint64_t rows = 0;
+        check(vb_join_n_outer_size(sides.data(), n, r, required, &rows));
+        std::vector<uint64_t> k(rows);
+        std::vector<std::vector<uint64_t>> vals(n, std::vector<uint64_t>(rows));
+        std::vector<std::vector<uint8_t>> valid(n, std::vector<uint8_t>(rows));
+        std::vector<void *> vp(n);
+        std::vector<uint8_t *> ok(n);
+        for (uint32_t j = 0; j < n; ++j) { vp[j] = vals[j].data(); ok[j] = valid[j].data(); }
+        check(vb_join_n_outer(sides.data(), n, r, required, k.data(), vp.data(), ok.data(), VB_HOST));
+        for (uint64_t i = 0; i < rows; ++i) {
+            std::vector<std::optional<V>> row(n);
+            for (uint32_t j = 0; j < n; ++j)
+                if (valid[j][i]) row[j] = detail::from_bits<V>(vals[j][i]);
+            out.emplace_back(detail::from_bits<K>(k[i]), std::move(row));
+        }
+    }
+    return out;
 }
 }  // namespace detail
 
@@ -165,6 +220,14 @@ public:
             for (uint64_t i = 0; i < nk; ++i) out.emplace_back(detail::from_bits<K>(k[i]), detail::from_bits<V>(c[i]));
         }
         return out;
+    }
+
+    // reduce_by_key(op, num_splits) kept on the device: a ReducedRddT to collect, or to join / cogroup with other results
+    // under the same num_splits without a second shuffle
+    ReducedRddT<K, V> reduce_by_key_rdd(Op op, size_t num_splits) const
+    {
+        auto s = detail::run_shuffle<K>(*sc_, keys_, &vals_, num_slices_, num_splits, detail::dtype<V>::code, (int)op);
+        return ReducedRddT<K, V>(std::shared_ptr<vb_shuf>(s.release(), detail::ShufDeleter()), num_splits);
     }
 
     // combine_by_key with named aggregates of the value column (VB_AGG_SUM / MIN / MAX / COUNT / MEAN), one shuffle:
@@ -282,26 +345,7 @@ public:
         auto shs = cogroup_shuffles(others, num_splits);
         std::vector<vb_shuf *> sides;
         for (auto &s : shs) sides.push_back(s.get());
-        const uint32_t n = (uint32_t)sides.size();
-        std::vector<std::pair<K, std::vector<std::vector<V>>>> out;
-        for (uint32_t r = 0; r < num_splits; ++r) {
-            uint64_t nk = 0;
-            std::vector<uint64_t> nv(n);
-            check(vb_cogroup_n_size(sides.data(), n, r, &nk, nv.data()));
-            std::vector<uint64_t> k(nk);
-            std::vector<std::vector<uint64_t>> offs(n, std::vector<uint64_t>(nk + 1)), vals(n);
-            std::vector<uint64_t *> op(n);
-            std::vector<void *> vp(n);
-            for (uint32_t j = 0; j < n; ++j) { vals[j].resize(nv[j]); op[j] = offs[j].data(); vp[j] = vals[j].data(); }
-            check(vb_cogroup_n(sides.data(), n, r, k.data(), op.data(), vp.data(), VB_HOST));
-            for (uint64_t i = 0; i < nk; ++i) {
-                std::vector<std::vector<V>> lists(n);
-                for (uint32_t j = 0; j < n; ++j)
-                    for (uint64_t x = offs[j][i]; x < offs[j][i + 1]; ++x) lists[j].push_back(detail::from_bits<V>(vals[j][x]));
-                out.emplace_back(detail::from_bits<K>(k[i]), std::move(lists));
-            }
-        }
-        return out;
+        return detail::read_cogroup_n<K, V>(sides, num_splits);
     }
 
     // inner join of [self, others...]  →  (k, [v_0, ..., v_{n-1}]) per row: for a key on every parent,
@@ -339,26 +383,7 @@ public:
         auto shs = cogroup_shuffles(others, num_splits);
         std::vector<vb_shuf *> sides;
         for (auto &s : shs) sides.push_back(s.get());
-        const uint32_t n = (uint32_t)sides.size();
-        std::vector<std::pair<K, std::vector<std::optional<V>>>> out;
-        for (uint32_t r = 0; r < num_splits; ++r) {
-            uint64_t rows = 0;
-            check(vb_join_n_outer_size(sides.data(), n, r, required, &rows));
-            std::vector<uint64_t> k(rows);
-            std::vector<std::vector<uint64_t>> vals(n, std::vector<uint64_t>(rows));
-            std::vector<std::vector<uint8_t>> valid(n, std::vector<uint8_t>(rows));
-            std::vector<void *> vp(n);
-            std::vector<uint8_t *> ok(n);
-            for (uint32_t j = 0; j < n; ++j) { vp[j] = vals[j].data(); ok[j] = valid[j].data(); }
-            check(vb_join_n_outer(sides.data(), n, r, required, k.data(), vp.data(), ok.data(), VB_HOST));
-            for (uint64_t i = 0; i < rows; ++i) {
-                std::vector<std::optional<V>> row(n);
-                for (uint32_t j = 0; j < n; ++j)
-                    if (valid[j][i]) row[j] = detail::from_bits<V>(vals[j][i]);
-                out.emplace_back(detail::from_bits<K>(k[i]), std::move(row));
-            }
-        }
-        return out;
+        return detail::read_join_n_outer<K, V>(sides, num_splits, required);
     }
 
     std::shared_ptr<Context> sc_;
@@ -392,6 +417,89 @@ private:
                 emit(detail::from_bits<K>(k[i]), vv[i] ? std::optional<V>(detail::from_bits<V>(v[i])) : std::nullopt,
                      wv[i] ? std::optional<W>(detail::from_bits<W>(w[i])) : std::nullopt);
         }
+    }
+};
+
+// A sealed reduce_by_key result on the device (PairRddT::reduce_by_key_rdd).  Partition r holds the keys with
+// hash % num_splits == r, each once, so as a join / cogroup parent under the same num_splits it is read through a view
+// (vb_shuffle_create_narrow: CoGroupedRdd::new's OneToOneDependency, co_grouped_rdd.rs:103-112) and not shuffled again;
+// each key's list is [its result].  Parents of a join / cogroup must have the same num_splits (vega::Error otherwise).
+template <typename K, typename V>
+class Context::ReducedRddT {
+public:
+    ReducedRddT(std::shared_ptr<vb_shuf> s, size_t num_splits) : s_(std::move(s)), num_splits_(num_splits) {}
+    size_t number_of_splits() const { return num_splits_; }
+
+    // collect()  →  Vec<(K, V)>
+    std::vector<std::pair<K, V>> collect() const
+    {
+        std::vector<std::pair<K, V>> out;
+        for (uint32_t r = 0; r < num_splits_; ++r) {
+            uint64_t nk = 0, nv = 0;
+            check(vb_shuffle_reduce_size(s_.get(), r, &nk, &nv));
+            std::vector<uint64_t> k(nk), c(nk);
+            check(vb_shuffle_reduce(s_.get(), r, k.data(), c.data(), nullptr, nullptr, VB_HOST));
+            for (uint64_t i = 0; i < nk; ++i) out.emplace_back(detail::from_bits<K>(k[i]), detail::from_bits<V>(c[i]));
+        }
+        return out;
+    }
+
+    // self.join(other).collect()  →  Vec<(K, (V, W))>: the keys both results have, with both results
+    template <typename W>
+    std::vector<std::pair<K, std::pair<V, W>>> join(const ReducedRddT<K, W> &other) const
+    {
+        auto a = view(*this), b = view(other);
+        std::vector<std::pair<K, std::pair<V, W>>> out;
+        for (uint32_t r = 0; r < num_splits_; ++r) {
+            uint64_t n = 0;
+            check(vb_join_size(a.get(), b.get(), r, &n));
+            std::vector<uint64_t> k(n), v(n), w(n);
+            check(vb_join(a.get(), b.get(), r, k.data(), v.data(), w.data(), VB_HOST));
+            for (uint64_t i = 0; i < n; ++i)
+                out.emplace_back(detail::from_bits<K>(k[i]), std::make_pair(detail::from_bits<V>(v[i]), detail::from_bits<W>(w[i])));
+        }
+        return out;
+    }
+
+    // CoGroupedRdd::new([self, others...]).collect()  →  Vec<(K, Vec<Vec<V>>)>: every key of any result once, with the
+    // list [result] from each result that has it and [] from the others
+    std::vector<std::pair<K, std::vector<std::vector<V>>>> cogroup_n(const std::vector<ReducedRddT> &others) const
+    {
+        auto views = views_of(others);
+        return detail::read_cogroup_n<K, V>(raw(views), num_splits_);
+    }
+
+    // outer join of [self, others...] with PairRddT::join_n_outer's `required` bitmask and row order
+    std::vector<std::pair<K, std::vector<std::optional<V>>>> join_n_outer(const std::vector<ReducedRddT> &others, uint32_t required) const
+    {
+        auto views = views_of(others);
+        return detail::read_join_n_outer<K, V>(raw(views), num_splits_, required);
+    }
+
+    std::shared_ptr<vb_shuf> s_;
+    size_t num_splits_;
+
+private:
+    template <typename W>
+    detail::ShufPtr view(const ReducedRddT<K, W> &p) const
+    {
+        if (p.num_splits_ != num_splits_) throw Error(VB_ERR_INVALID, "join / cogroup parents of reduce results need the same num_splits");
+        vb_shuf *v = nullptr;
+        check(vb_shuffle_create_narrow(p.s_.get(), 0, &v));
+        return detail::ShufPtr(v);
+    }
+    std::vector<detail::ShufPtr> views_of(const std::vector<ReducedRddT> &others) const
+    {
+        std::vector<detail::ShufPtr> vs;
+        vs.push_back(view(*this));
+        for (auto &o : others) vs.push_back(view(o));
+        return vs;
+    }
+    static std::vector<vb_shuf *> raw(const std::vector<detail::ShufPtr> &vs)
+    {
+        std::vector<vb_shuf *> r;
+        for (auto &v : vs) r.push_back(v.get());
+        return r;
     }
 };
 

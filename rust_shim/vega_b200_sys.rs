@@ -94,6 +94,8 @@ extern "C" {
                                    val_dtypes: *const i32, n_aggs: u32, aggs: *const vb_agg_col, out: *mut *mut vb_shuf) -> i32;
     pub fn vb_shuffle_map_cols(s: *mut vb_shuf, map_id: u32, keys: *const c_void, vals: *const *const c_void, n_rows: u64, src_loc: i32) -> i32;
     pub fn vb_shuffle_reduce_cols(s: *mut vb_shuf, reduce_id: u32, out_keys: *mut c_void, out_aggs: *const *mut c_void, dst_loc: i32) -> i32;
+    // a sealed reduce-op / combine_by_key shuffle as a cogroup or join side under the same partitioner (OneToOneDependency)
+    pub fn vb_shuffle_create_narrow(parent: *mut vb_shuf, out_col: u32, out: *mut *mut vb_shuf) -> i32;
     // String keys (Arrow-style offsets + bytes; placed by MetroHash64_1(bytes ‖ 0xFF) like `str::hash`)
     pub fn vb_shuffle_create_str(ctx: *mut vb_ctx, shuffle_id: u64, n_map: u32, n_reduce: u32, val_dtype: i32, agg: i32,
                                  out: *mut *mut vb_shuf) -> i32;

@@ -6,8 +6,8 @@ interface for the path (rdd.py) plus the one-process-per-GPU exchange (dist.py).
 Importing works without a GPU (so the C ABI can be inspected); computing does not.
 """
 from ._lib import (LIB_PATH, SYMBOLS, VegaB200Error, lib)  # noqa: F401
-from .rdd import (CoGroupedRdd, CombinedRdd, Context, Grouped, JoinedRdd, PairRdd, Rdd, Shuffle, ShuffledRdd, StrKeys, StrPairRdd,  # noqa: F401
-                  StrRdd, StrShuffle, StrShuffledRdd, slice_starts)
+from .rdd import (AggregateRdd, CoGroupedRdd, CombinedRdd, Context, Grouped, JoinedRdd, PairRdd, Rdd, Shuffle, ShuffledRdd,  # noqa: F401
+                  StrKeys, StrPairRdd, StrRdd, StrShuffle, StrShuffledRdd, slice_starts)
 
-__all__ = ["Context", "PairRdd", "CoGroupedRdd", "CombinedRdd", "Rdd", "Shuffle", "ShuffledRdd", "JoinedRdd", "Grouped", "slice_starts",
+__all__ = ["Context", "PairRdd", "CoGroupedRdd", "CombinedRdd", "AggregateRdd", "Rdd", "Shuffle", "ShuffledRdd", "JoinedRdd", "Grouped", "slice_starts",
            "StrKeys", "StrPairRdd", "StrRdd", "StrShuffle", "StrShuffledRdd", "VegaB200Error", "lib", "LIB_PATH", "SYMBOLS"]

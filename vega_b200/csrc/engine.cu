@@ -309,6 +309,7 @@ struct vb_shuf {
     u32 n_cols = 0;
     AccSpec acc_map{}, acc_merge{};   // map-side combine / table merge (COUNT merges as ADD, no order transform)
     OutSpec outs{};                   // one output column per vb_agg_col
+    int out_dt[VB_MAX_AGGS] = {};     // each output column's dtype (a narrow view's value dtype)
     u64 *res_cols = nullptr;          // [outs.n][n_keys], partition-major like res_keys
     u32 key_width = 8;
     u64 hint = 0;
@@ -1308,6 +1309,7 @@ extern "C" int32_t vb_shuffle_create_multi(vb_ctx *c, uint64_t shuffle_id, uint3
         spec_set(mp.op, a, opk); spec_set(mp.tx, a, tx); spec_set(mp.src, a, src);
         spec_set(mg.op, a, merge_op(opk)); spec_set(mg.src, a, a);
         if (a >= n_aggs) continue;
+        s->out_dt[a] = op == VB_AGG_COUNT ? VB_U64 : op == VB_AGG_MEAN ? VB_F64 : dt;
         os.acc[a] = (unsigned char)a;
         os.cnt[a] = (unsigned char)count_acc;
         os.tx[a] = (unsigned char)tx;
@@ -3049,6 +3051,92 @@ extern "C" int32_t vb_shuffle_reduce_cols(vb_shuf *s, uint32_t r, void *out_keys
     for (u32 o = 0; out_aggs && o < s->outs.n; ++o)
         TRY(copy_out(s, out_aggs[o], s->res_cols ? s->res_cols + (u64)o * s->n_keys + b0 : nullptr, nk * 8, dst_loc));
     CU(cudaStreamSynchronize(c->stream));
+    return VB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// a reduce result as a cogroup / join side without a second shuffle (CoGroupedRdd::new's OneToOneDependency,
+// co_grouped_rdd.rs:103-112)
+// ---------------------------------------------------------------------------------------------
+// Partition r of a reduce result already holds exactly the keys with hash % n_reduce == r, each once, so the view is a
+// grouped COGROUP shuffle over the same placement: copies of the keys and of one result column, offsets 0..n (one value
+// per key), and the key dictionary the joins probe, built by one narrow_dict_kernel pass (the keys are distinct, so there
+// is no hash_agg, no id sort and no CSR build).  The table is keys only: dictionaries never read the accumulator half.
+static int narrow_build(vb_shuf *v, const u64 *keys, const u64 *col, u64 n)
+{
+    vb_ctx *c = v->ctx;
+    if (n == 0) return VB_OK;                         // an empty side: no arrays, no dictionary (as seal_group leaves it)
+    DevBuf k(c), vals(c), offs(c), ctl(c);
+    TRY(k.alloc(n * 8)); TRY(vals.alloc(n * 8)); TRY(offs.alloc((n + 1) * 8)); TRY(ctl.alloc(sizeof(TableCtl)));
+    CU(cudaMemcpyAsync(k.p, keys, n * 8, cudaMemcpyDeviceToDevice, c->stream));
+    CU(cudaMemcpyAsync(vals.p, col, n * 8, cudaMemcpyDeviceToDevice, c->stream));
+    // load <= 0.5 by construction, so only a probe chain longer than HA_MAX_PROBE buckets makes the kernel give up
+    const u32 max_log = std::min<u32>(MAX_LOG_CAP, std::max<u32>(4, ceil_log2_u64(2 * n)));
+    u32 log_cap = choose_log_cap(n, n, false, max_log, c->l2_bytes);
+    for (;;) {
+        const u64 cap = 1ull << log_cap;
+        DevBuf tab(c), dense(c);
+        TRY(tab.alloc((cap + BUCKET) * 8));
+        TRY(dense.alloc((cap + 1) * 4));
+        CU(cudaMemsetAsync(tab.p, 0xFF, cap * 8, c->stream));                 // EMPTY_KEY
+        CU(cudaMemsetAsync(tab.as<u64>() + cap, 0, BUCKET * 8, c->stream));   // special-slot marker: absent
+        CU(cudaMemsetAsync(ctl.p, 0, sizeof(TableCtl), c->stream));
+        {
+            KLaunch kl(v, K_DICT, n);
+            narrow_dict_kernel<<<(unsigned)((n + 1 + 255) / 256), 256, 0, c->stream>>>(k.as<u64>(), n, table_at(tab.p, log_cap),
+                                                                                      dense.as<u32>(), offs.as<u64>(), ctl.as<TableCtl>());
+            TRY(kl.done("narrow_dict_kernel"));
+        }
+        TableCtl h;
+        TRY(fetch_status_unlocked(c, ctl.p, &h, sizeof(h)));
+        if (!h.abort) {
+            v->dict = tab.release();
+            v->dict_log_cap = log_cap;
+            v->dense_of_slot = (u32 *)dense.release();
+            v->st.table_slots = cap;
+            break;
+        }
+        if (log_cap >= max_log) return set_err(VB_ERR_CUDA, "key dictionary overflow at maximum capacity 2^%u (internal error)", log_cap);
+        log_cap = std::min(max_log, log_cap + 2);
+        v->st.table_restarts++;
+    }
+    v->res_keys = (u64 *)k.release();
+    v->res_vals = (u64 *)vals.release();
+    v->res_offs = (u64 *)offs.release();
+    return VB_OK;
+}
+
+extern "C" int32_t vb_shuffle_create_narrow(vb_shuf *p, uint32_t out_col, vb_shuf **out)
+{
+    if (!p || !out) return set_err(VB_ERR_INVALID, "vb_shuffle_create_narrow: NULL argument");
+    *out = nullptr;
+    if (p->str) return invalid_str(p, "vb_shuffle_create_narrow");
+    if (!is_reduce_op(p->agg))
+        return set_err(VB_ERR_INVALID, "vb_shuffle_create_narrow: shuffle %llu is not a reduce-op or combine_by_key shuffle",
+                       (unsigned long long)p->id);
+    const u32 n_cols = p->multi ? p->outs.n : 1;
+    if (out_col >= n_cols) return set_err(VB_ERR_INVALID, "vb_shuffle_create_narrow: output column %u of %u", out_col, n_cols);
+    TRY(wait_sealed(p));
+    vb_ctx *c = p->ctx;
+    vb_shuf *v = make_internal_like(p);
+    v->agg = VB_AGG_COGROUP;
+    v->vdt = p->multi ? p->out_dt[out_col] : p->agg == VB_AGG_COUNT ? VB_U64 : p->vdt;
+    v->rank = p->rank; v->world = p->world;
+    v->bucket_off = p->bucket_off; v->val_off = p->bucket_off;
+    v->n_keys = v->n_vals = v->st.rows_out = p->n_keys;
+    int rc;
+    {
+        std::lock_guard<std::mutex> lk(c->mu);
+        rc = [&]() -> int {
+            CU(cudaSetDevice(c->device));
+            const u64 *col = p->multi ? (p->res_cols ? p->res_cols + (u64)out_col * p->n_keys : nullptr) : p->res_comb;
+            TRY(narrow_build(v, p->res_keys, col, p->n_keys));
+            CU(cudaStreamSynchronize(c->stream));
+            return VB_OK;
+        }();
+    }
+    if (rc != VB_OK) { vb_shuffle_free(v); return rc; }
+    *out = v;
     return VB_OK;
 }
 

@@ -1490,6 +1490,30 @@ __global__ void translate_ids_kernel(u32 *__restrict__ ids, u64 n, const u32 *__
     for (; i < n; i += stride) ids[i] = dense_of_slot[ids[i]];
 }
 
+// Key dictionary of n keys known to be distinct (a reduce result taken as a cogroup side), one thread per key: insert key i
+// into the table (keys[] pre-set to EMPTY_KEY, keys[cap..cap+4) to 0), dense_of_slot[its slot] = i, and offs[i] = i (one
+// value per key), offs[n] = n.  A key equal to EMPTY_KEY takes the special slot cap.  A probe chain longer than
+// HA_MAX_PROBE buckets raises ctl->abort and the host rebuilds the table larger.
+__global__ void narrow_dict_kernel(const u64 *__restrict__ keys, u64 n, Table t, u32 *__restrict__ dense_of_slot,
+                                   u64 *__restrict__ offs, TableCtl *ctl)
+{
+    const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i > n) return;
+    offs[i] = i;
+    if (i == n) return;
+    const u64 key = keys[i];
+    const u64 cap = 1ull << t.log_cap;
+    if (key == EMPTY_KEY) {
+        t.keys[cap] = 1ull;
+        dense_of_slot[cap] = (u32)i;
+        return;
+    }
+    const u64 b = home_bucket(key, t.log_cap);
+    u32 inserted = 0;
+    if (!table_resolve_with(t, b, ld_bucket(&t.keys[4 * b]), key, inserted, [&](u64 slot) { dense_of_slot[slot] = (u32)i; }))
+        atomicExch(&ctl->abort, 1u);
+}
+
 // CSR offsets from sorted dense ids: offsets[id] = first row of id; offsets[n_ids] = n.
 __global__ void csr_bounds_kernel(const u32 *__restrict__ ids, u64 n, u64 *__restrict__ offsets, u64 n_ids)
 {

@@ -260,6 +260,20 @@ class Shuffle:
         if world > 1:
             L.check(self._lib.vb_shuffle_set_dist(h, rank, world))
 
+    @classmethod
+    def narrow(cls, parent, out_col, vcode):
+        """vb_shuffle_create_narrow: the sealed reduce result `parent` (output column out_col) as a sealed COGROUP side
+        under the same partitioner, each key with the one-element list [its result] (vcode: the result's dtype)."""
+        self = cls.__new__(cls)
+        self.sc, self._lib = parent.sc, parent._lib
+        self.n_map, self.n_reduce, self.agg, self.vcode, self.kcode = 0, parent.n_reduce, L.VB_AGG_COGROUP, vcode, parent.kcode
+        self.has_payload, self._keepalive = True, []
+        h = ctypes.c_void_p()
+        L.check(self._lib.vb_shuffle_create_narrow(parent._h, out_col, ctypes.byref(h)))
+        self._h = h
+        self.sc._shuffles.add(self)
+        return self
+
     def map(self, map_id, keys, vals, start, stop):
         """ShuffleMapTask::run for one map partition = rows [start, stop) of the parent."""
         n = stop - start
@@ -402,8 +416,72 @@ class _Base:
         return self.num_slices
 
 
-class ShuffledRdd(_Base):
-    """ShuffledRdd<K,V,C> (src/rdd/shuffled_rdd.rs): lazy; `collect()` runs the job."""
+_REDUCE_AGGS = ("sum", "min", "max", "count")
+_CODE_OF = {np.uint64: L.VB_U64, np.int64: L.VB_I64, np.float64: L.VB_F64}
+
+
+class _AggregatedParent(_Base):
+    """A reduce result (reduce_by_key / count_by_key, or one aggregate of combine_by_key) as a join or cogroup parent,
+    next to PairRdds.  Its partition r already holds the keys with hash % num_splits == r, each once, so under the same
+    num_splits it joins through a view of the sealed result (vb_shuffle_create_narrow: vega's OneToOneDependency,
+    co_grouped_rdd.rs:103-112) with no second shuffle.  Under another num_splits each result partition is read into
+    device tensors and becomes one map task of an ordinary COGROUP shuffle (vega's ShuffleDependency over the
+    ShuffledRdd), with no host round trip.  Either way the key's list on this side is [its result]."""
+
+    def join(self, other, num_splits):
+        return JoinedRdd(self, other, num_splits)
+
+    def left_outer_join(self, other, num_splits):
+        return JoinedRdd(self, other, num_splits, "left")
+
+    def right_outer_join(self, other, num_splits):
+        return JoinedRdd(self, other, num_splits, "right")
+
+    def full_outer_join(self, other, num_splits):
+        return JoinedRdd(self, other, num_splits, "full")
+
+    def cogroup(self, other, num_splits):
+        return JoinedRdd(self, other, num_splits)
+
+    def _cogroup_side(self, num_splits):
+        """The sealed COGROUP-kind shuffle a cogroup over num_splits partitions reads for this parent."""
+        sh = self._run()
+        if num_splits == sh.n_reduce:
+            col, _, vcode = self._result_col(sh)
+            return Shuffle.narrow(sh, col, vcode)
+        return self._reshuffled(num_splits)
+
+    def _reshuffled(self, num_splits):
+        """The result shuffled again over num_splits partitions, one map task per result partition read on the device."""
+        sh = self._run()
+        col, n_cols, vcode = self._result_col(sh)
+        import torch
+        dev = f"cuda:{sh._lib.vb_ctx_device(self.sc._h)}"
+        out = Shuffle(self.sc, sh.n_reduce, num_splits, sh.kcode, vcode, L.VB_AGG_COGROUP, key_width=self.keys.key_width)
+        for r in range(sh.n_reduce):
+            nk = sh.reduce_size(r)[0]
+            k, v = (torch.empty(nk, dtype=torch.int64, device=dev) for _ in range(2))
+            if n_cols is None:
+                sh.reduce_device(r, out_keys=k, out_comb=v)
+            else:
+                sh.reduce_cols(r, None, L.VB_DEVICE, out_keys=k, out_aggs=[v if c == col else None for c in range(n_cols)])
+            out.map(r, _Col(k), _Col(v, role="value"), 0, nk)
+        out.seal()
+        return out
+
+
+def _check_parent(r, j):
+    """TypeError, before any device work, for an aggregated parent that cannot be a cogroup side."""
+    if isinstance(r, StrShuffledRdd):
+        raise TypeError(f"parent {j}: String keys do not support cogroup")
+    if isinstance(r, ShuffledRdd) and r.agg_name not in _REDUCE_AGGS:
+        raise TypeError(f"parent {j}: a {r.agg_name} result is not a join parent (reduce_by_key, count_by_key and "
+                        "combine_by_key results are)")
+
+
+class ShuffledRdd(_AggregatedParent):
+    """ShuffledRdd<K,V,C> (src/rdd/shuffled_rdd.rs): lazy; `collect()` runs the job.  A sum / min / max / count result
+    is also a join and cogroup parent (see _AggregatedParent)."""
 
     def __init__(self, parent, agg_name, num_splits, hint=0):
         if num_splits < 1:
@@ -413,6 +491,18 @@ class ShuffledRdd(_Base):
         self.parent, self.agg_name, self.num_slices, self.hint = parent, agg_name, num_splits, hint
         self.sc = parent.sc
         self._sh = None
+
+    @property
+    def keys(self):
+        return self.parent.keys
+
+    def _result_col(self, sh):
+        return 0, None, L.VB_U64 if sh.agg == L.VB_AGG_COUNT else sh.vcode
+
+    def _cogroup_side(self, num_splits):
+        if self.agg_name == "cogroup":                  # a PairRdd parent's own shuffle (JoinedRdd, CoGroupedRdd)
+            return self._run()
+        return super()._cogroup_side(num_splits)
 
     def _run(self):
         if self._sh is not None:
@@ -471,17 +561,28 @@ class JoinedRdd(_Base):
                 raise ValueError("num_splits must be >= 1")
             if left.keys.key_width != right.keys.key_width:
                 raise TypeError("join sides have different key types")
+        sides = (left, right)
+        if any(isinstance(r, _AggregatedParent) for r in sides):     # a reduce result as a parent (_AggregatedParent)
+            for j, r in enumerate(sides):
+                if isinstance(r, _AggregatedParent):
+                    _check_parent(r, j)
+                elif not isinstance(r, PairRdd) or isinstance(r, StrPairRdd):
+                    raise TypeError(f"parent {j} is not an integer-key PairRdd or reduce result")
+            if num_splits < 1:
+                raise ValueError("num_splits must be >= 1")
+            if left.keys.key_width != right.keys.key_width or left.keys.code != right.keys.code:
+                raise TypeError("join sides have different key types")
         self.left, self.right, self.num_slices, self.sc = left, right, num_splits, left.sc
         self.kind = kind
         self._shs = None
 
     def _run(self):
         if self._shs is None:
-            a = ShuffledRdd(self.left, "cogroup", self.num_slices)
-            b = ShuffledRdd(self.right, "cogroup", self.num_slices)
+            a, b = (r if isinstance(r, _AggregatedParent) else ShuffledRdd(r, "cogroup", self.num_slices)
+                    for r in (self.left, self.right))
             if self.left.keys.key_width != self.right.keys.key_width:
                 raise TypeError("join sides have different key types")
-            self._shs = (a._run(), b._run())
+            self._shs = (a._cogroup_side(self.num_slices), b._cogroup_side(self.num_slices))
         return self._shs
 
     def compute(self, split):
@@ -543,7 +644,9 @@ class JoinedRdd(_Base):
 
 class CoGroupedRdd(_Base):
     """CoGroupedRdd::new(rdds, HashPartitioner::new(num_splits)) (src/rdd/co_grouped_rdd.rs:75-135): the cogroup of any
-    number of PairRdds (1 to 16), each shuffled with the Vec-append aggregator as JoinedRdd does.
+    number of PairRdds (1 to 16), each shuffled with the Vec-append aggregator as JoinedRdd does.  A reduce result
+    (reduce_by_key / count_by_key, or CombinedRdd.aggregate(name)) is a parent too, with the list [its result] per key;
+    under the same num_splits it is not shuffled again (_AggregatedParent).
 
     compute(r) -> (keys, [(offsets, values) per parent]): every key of the partition once; key i's list from parent j
     is values_j[offsets_j[i]:offsets_j[i + 1]], empty where that parent lacks the key.  collect() gives the
@@ -561,6 +664,9 @@ class CoGroupedRdd(_Base):
         for j, r in enumerate(rdds):
             if isinstance(r, StrPairRdd):
                 raise TypeError(f"parent {j}: String keys do not support cogroup")
+            if isinstance(r, _AggregatedParent):
+                _check_parent(r, j)
+                continue
             if not isinstance(r, PairRdd):
                 raise TypeError(f"parent {j} is not a PairRdd")
             if len(r.cols) > 1:
@@ -575,7 +681,8 @@ class CoGroupedRdd(_Base):
 
     def _run(self):
         if self._shs is None:
-            self._shs = [ShuffledRdd(r, "cogroup", self.num_slices)._run() for r in self.rdds]
+            self._shs = [(r if isinstance(r, _AggregatedParent) else ShuffledRdd(r, "cogroup", self.num_slices))
+                         ._cogroup_side(self.num_slices) for r in self.rdds]
         return self._shs
 
     def _sides(self):
@@ -715,6 +822,12 @@ class CombinedRdd(_Base):
         self._sh = sh
         return sh
 
+    def aggregate(self, name):
+        """The named aggregate as a join / cogroup parent: (key, that aggregate's result) rows (_AggregatedParent)."""
+        if name not in self.names:
+            raise ValueError(f"no aggregate named {name!r} (the aggregates are {self.names})")
+        return AggregateRdd(self, name)
+
     def compute(self, split):
         keys, outs = self._run().reduce_cols(split, self.out_dtypes)
         return keys, dict(zip(self.names, outs))
@@ -726,6 +839,26 @@ class CombinedRdd(_Base):
 
     def stats(self):
         return self._run().stats()
+
+
+class AggregateRdd(_AggregatedParent):
+    """One named aggregate of a CombinedRdd as a join / cogroup parent (CombinedRdd.aggregate(name)).  The combine
+    shuffle runs once and is shared by every aggregate taken from it."""
+
+    def __init__(self, combined, name):
+        self.combined, self.name = combined, name
+        self.sc, self.num_slices = combined.sc, combined.num_slices
+
+    @property
+    def keys(self):
+        return self.combined.parent.keys
+
+    def _run(self):
+        return self.combined._run()
+
+    def _result_col(self, sh):
+        i = self.combined.names.index(self.name)
+        return i, len(self.combined.names), _CODE_OF[self.combined.out_dtypes[i]]
 
 
 class PairRdd(_Base):
@@ -1067,6 +1200,13 @@ class StrShuffle(Shuffle):
                                                 p(out_vals), L.VB_DEVICE))
 
 
+def _no_str(what):
+    def f(self, *a, **k):
+        raise TypeError(f"{what} is not supported for string keys yet (reduce_by_key, count_by_key, group_by_key, "
+                        "partition_by_key, count_by_value and distinct are)")
+    return f
+
+
 class StrShuffledRdd(ShuffledRdd):
     """ShuffledRdd over string keys: collect() gives (keys, combined) or a Grouped whose keys are Python strs."""
 
@@ -1094,12 +1234,11 @@ class StrShuffledRdd(ShuffledRdd):
         """compute(split) into caller-provided torch CUDA tensors (see StrShuffle.reduce_device)."""
         self._run().reduce_device(split, **out)
 
-
-def _no_str(what):
-    def f(self, *a, **k):
-        raise TypeError(f"{what} is not supported for string keys yet (reduce_by_key, count_by_key, group_by_key, "
-                        "partition_by_key, count_by_value and distinct are)")
-    return f
+    join = _no_str("join")
+    left_outer_join = _no_str("left_outer_join")
+    right_outer_join = _no_str("right_outer_join")
+    full_outer_join = _no_str("full_outer_join")
+    cogroup = _no_str("cogroup")
 
 
 class StrPairRdd(PairRdd):
