@@ -22,6 +22,8 @@
  *   vb_cogroup_n* / vb_join_n*
  *                          <- CoGroupedRdd::compute with any number of parents (co_grouped_rdd.rs:75-135, 206-249)
  *   vb_join_n_outer*       <- nothing: vega has no outer joins (N-way, over the same cogroup, new)
+ *   vb_cogroup_n_str* / vb_join_n_str*
+ *                          <- the same two over `String` keys (keys matched by their bytes; join keys once per key)
  *   vb_shuffle_free        <- (the reference never evicts SHUFFLE_CACHE, src/env.rs:27)
  *   vb_slice               <- ParallelCollection::slice           src/rdd/parallel_collection_rdd.rs:116-145
  *   vb_shuffle_export_* / vb_shuffle_import
@@ -411,7 +413,8 @@ VB_API int32_t vb_join_n_outer(vb_shuf *const *sides, uint32_t n_sides, uint32_t
  * than 2^32 bytes (VB_ERR_TOO_LARGE beyond them).  Key offsets that decrease or exceed n_bytes are VB_ERR_INVALID,
  * for device input too (checked on the device).  One process only: vb_shuffle_set_dist with world > 1, export /
  * import / exchange and the blob calls return VB_ERR_UNSUPPORTED; vb_shuffle_set_key_width, the integer map and
- * reduce calls and the join / cogroup calls return VB_ERR_INVALID on a string shuffle, and the string calls return
+ * reduce calls and the join / cogroup calls return VB_ERR_INVALID on a string shuffle (vb_cogroup_n_str / vb_join_n_str
+ * below join and cogroup string GROUP shuffles), and the string calls return
  * VB_ERR_INVALID on any other shuffle.  seal / is_sealed / stats / kernel_time / set_hint / free work as for any
  * shuffle (table_slots: largest dictionary index, table_restarts: index growths).
  * vb_shuffle_reduce_str_size / vb_shuffle_reduce_str block until the shuffle is sealed and skip NULL outputs; the
@@ -428,6 +431,41 @@ VB_API int32_t vb_shuffle_reduce_str_size(vb_shuf *s, uint32_t reduce_id, uint64
 VB_API int32_t vb_shuffle_reduce_str(vb_shuf *s, uint32_t reduce_id, uint64_t *out_key_offsets /*n_keys+1*/,
                                      void *out_key_bytes, void *out_combined, uint64_t *out_offsets /*n_keys+1*/,
                                      void *out_vals, int32_t dst_loc);
+/* Cogroup and join of string-key shuffles, for one partition: vb_cogroup_n and vb_join_n_outer with keys compared as
+ * byte strings (CoGroupedRdd::compute over `String` keys, co_grouped_rdd.rs:75-135, 206-249).  Each side is a sealed
+ * GROUP shuffle of vb_shuffle_create_str (the calls block until every side is sealed); 1 <= n_sides <=
+ * VB_MAX_COGROUP_SIDES, all sides with the same n_reduce on the same context; value dtypes may differ and the same
+ * shuffle may appear more than once.  Integer shuffles, string reduce-op shuffles, NULL or out-of-range arguments and
+ * a `required` bit at n_sides or above are VB_ERR_INVALID.  The first call that reads a side builds an index of its
+ * keys, kept until vb_shuffle_free.
+ *   cogroup  vb_cogroup_n's keys and lists: every key of any side in the partition exactly once, in unspecified
+ *            order, as out_key_offsets [n_keys + 1] (from 0) into out_key_bytes [n_key_bytes]; side j's list is the
+ *            one vb_shuffle_reduce_str of side j gives for the key, empty where side j lacks it.  NULL outputs, or
+ *            NULL entries of out_offsets / out_vals, are skipped.
+ *   join     vb_join_n_outer's rows: a key gives rows only if every side of `required` has it (all bits set: the inner
+ *            join); a side that lacks it gives one None slot (value 0, validity 0); the key's prod max(|l_j|, 1) rows
+ *            are contiguous, the last side varying fastest.  The keys are written once each, not once per row: the
+ *            n_keys keys of the partition that have rows, in row order, as out_key_offsets / out_key_bytes, and key
+ *            i's rows are [out_row_offsets[i], out_row_offsets[i + 1]) of out_vals[j] (out_row_offsets [n_keys + 1],
+ *            ending at n_rows).  A caller that wants one (key, v_0, ..., v_{n-1}) per row repeats key i over its
+ *            range.  Once the partition has rows, out_key_offsets, out_row_offsets, out_vals and every entry of it,
+ *            and out_key_bytes unless n_key_bytes is 0, must be non-NULL (VB_ERR_INVALID); out_valid and its entries
+ *            are optional.  A key's product, or the partition's total, of 2^63 rows or more is VB_ERR_TOO_LARGE from
+ *            the size call.
+ * The size calls keep the partition's plan on sides[0] for the write call, which frees it.  dst_loc: VB_HOST or
+ * VB_DEVICE.  Limit: fewer than 2^32 - 1 keys over all sides of one partition.                                     */
+VB_API int32_t vb_cogroup_n_str_size(vb_shuf *const *sides, uint32_t n_sides, uint32_t reduce_id, uint64_t *n_keys,
+                                     uint64_t *n_key_bytes, uint64_t *n_vals /*[n_sides], may be NULL*/);
+VB_API int32_t vb_cogroup_n_str(vb_shuf *const *sides, uint32_t n_sides, uint32_t reduce_id,
+                                uint64_t *out_key_offsets /*n_keys+1*/, void *out_key_bytes,
+                                uint64_t *const *out_offsets /*[n_sides] arrays of n_keys+1*/,
+                                void *const *out_vals /*[n_sides]*/, int32_t dst_loc);
+VB_API int32_t vb_join_n_str_size(vb_shuf *const *sides, uint32_t n_sides, uint32_t reduce_id, uint32_t required,
+                                  uint64_t *n_rows, uint64_t *n_keys, uint64_t *n_key_bytes);
+VB_API int32_t vb_join_n_str(vb_shuf *const *sides, uint32_t n_sides, uint32_t reduce_id, uint32_t required,
+                             uint64_t *out_key_offsets /*n_keys+1*/, void *out_key_bytes,
+                             uint64_t *out_row_offsets /*n_keys+1*/, void *const *out_vals /*[n_sides] of n_rows*/,
+                             uint8_t *const *out_valid /*[n_sides] or NULL; entries may be NULL*/, int32_t dst_loc);
 /* MetroHash64_1(bytes ‖ 0xFF, seed 0): the reference's hash of a `String` / `&str` key */
 VB_API uint64_t vb_hash_str(const void *bytes, uint64_t len);
 VB_API uint32_t vb_get_partition_str(const void *bytes, uint64_t len, uint32_t n_reduce);

@@ -9,7 +9,7 @@
 //   CoGroupedRdd::new over reduce results          src/rdd/co_grouped_rdd.rs:103-112 (OneToOneDependency; reduce_by_key_rdd)
 // Rows are Vec<(K,V)> with K in {u64,i64,i32,u32,std::string} and V in {u64,i64,f64}; std::string keys are placed
 // like the reference's String keys and support group_by_key / reduce_by_key / count_by_key / count_by_value /
-// distinct.  reduce_by_key takes a named Op (the reference's serde_closure cannot cross into CUDA).  Errors throw vega::Error
+// distinct, and cogroup / join / outer joins of any number of parents.  reduce_by_key takes a named Op (the reference's serde_closure cannot cross into CUDA).  Errors throw vega::Error
 // (the reference returns Result<_> / panics).
 #pragma once
 #include <cstdint>
@@ -676,7 +676,116 @@ public:
         return out;
     }
 
+    // CoGroupedRdd::new([self, others...], HashPartitioner::new(num_splits)).collect() over String keys
+    // (vb_cogroup_n_str): every key of any parent once, with one value list per parent (this one first)
+    std::vector<std::pair<std::string, std::vector<std::vector<V>>>> cogroup_n(const std::vector<StrPairRddT> &others,
+                                                                               size_t num_splits) const
+    {
+        auto shs = group_shuffles(others, num_splits);
+        std::vector<vb_shuf *> sides = raw(shs);
+        const uint32_t n = (uint32_t)sides.size();
+        std::vector<std::pair<std::string, std::vector<std::vector<V>>>> out;
+        for (uint32_t r = 0; r < num_splits; ++r) {
+            uint64_t nk = 0, nb = 0;
+            std::vector<uint64_t> nv(n);
+            check(vb_cogroup_n_str_size(sides.data(), n, r, &nk, &nb, nv.data()));
+            std::vector<uint64_t> ko(nk + 1);
+            std::string kb(nb, '\0');
+            std::vector<std::vector<uint64_t>> offs(n, std::vector<uint64_t>(nk + 1)), vals(n);
+            std::vector<uint64_t *> op(n);
+            std::vector<void *> vp(n);
+            for (uint32_t j = 0; j < n; ++j) { vals[j].resize(nv[j]); op[j] = offs[j].data(); vp[j] = vals[j].data(); }
+            check(vb_cogroup_n_str(sides.data(), n, r, ko.data(), kb.data(), op.data(), vp.data(), VB_HOST));
+            for (uint64_t i = 0; i < nk; ++i) {
+                std::vector<std::vector<V>> lists(n);
+                for (uint32_t j = 0; j < n; ++j)
+                    for (uint64_t x = offs[j][i]; x < offs[j][i + 1]; ++x) lists[j].push_back(detail::from_bits<V>(vals[j][x]));
+                out.emplace_back(std::string(kb, ko[i], ko[i + 1] - ko[i]), std::move(lists));
+            }
+        }
+        return out;
+    }
+
+    // outer join of [self, others...] (vb_join_n_str): bit j of `required` marks parent j (this one is 0) required;
+    // an optional parent that lacks the key gives std::nullopt.  (k, [v_0, ..., v_{n-1}]) per row, a key's rows
+    // contiguous, for v0 in L0 { for v1 in L1 { ... } }
+    std::vector<std::pair<std::string, std::vector<std::optional<V>>>> join_n_outer(const std::vector<StrPairRddT> &others,
+                                                                                    size_t num_splits, uint32_t required) const
+    {
+        auto shs = group_shuffles(others, num_splits);
+        std::vector<vb_shuf *> sides = raw(shs);
+        const uint32_t n = (uint32_t)sides.size();
+        std::vector<std::pair<std::string, std::vector<std::optional<V>>>> out;
+        for (uint32_t r = 0; r < num_splits; ++r) {
+            uint64_t rows = 0, nk = 0, nb = 0;
+            check(vb_join_n_str_size(sides.data(), n, r, required, &rows, &nk, &nb));
+            std::vector<uint64_t> ko(nk + 1), ro(nk + 1);
+            std::string kb(nb, '\0');
+            std::vector<std::vector<uint64_t>> vals(n, std::vector<uint64_t>(rows));
+            std::vector<std::vector<uint8_t>> valid(n, std::vector<uint8_t>(rows));
+            std::vector<void *> vp(n);
+            std::vector<uint8_t *> ok(n);
+            for (uint32_t j = 0; j < n; ++j) { vp[j] = vals[j].data(); ok[j] = valid[j].data(); }
+            check(vb_join_n_str(sides.data(), n, r, required, ko.data(), kb.data(), ro.data(), vp.data(), ok.data(), VB_HOST));
+            for (uint64_t i = 0; i < nk; ++i) {
+                const std::string k(kb, ko[i], ko[i + 1] - ko[i]);
+                for (uint64_t x = ro[i]; x < ro[i + 1]; ++x) {
+                    std::vector<std::optional<V>> row(n);
+                    for (uint32_t j = 0; j < n; ++j)
+                        if (valid[j][x]) row[j] = detail::from_bits<V>(vals[j][x]);
+                    out.emplace_back(k, std::move(row));
+                }
+            }
+        }
+        return out;
+    }
+
+    // inner join of [self, others...]  →  (k, [v_0, ..., v_{n-1}]) per row
+    std::vector<std::pair<std::string, std::vector<V>>> join_n(const std::vector<StrPairRddT> &others, size_t num_splits) const
+    {
+        std::vector<std::pair<std::string, std::vector<V>>> out;
+        for (auto &kv : join_n_outer(others, num_splits, (uint32_t)((1ull << (others.size() + 1)) - 1))) {
+            std::vector<V> row;
+            for (auto &v : kv.second) row.push_back(*v);
+            out.emplace_back(std::move(kv.first), std::move(row));
+        }
+        return out;
+    }
+
+    // PairRdd::join (src/rdd/pair_rdd.rs:104-121)  →  Vec<(String, (V, V))>
+    std::vector<std::pair<std::string, std::pair<V, V>>> join(const StrPairRddT &other, size_t num_splits) const
+    {
+        std::vector<std::pair<std::string, std::pair<V, V>>> out;
+        for (auto &kv : join_n({other}, num_splits)) out.emplace_back(std::move(kv.first), std::make_pair(kv.second[0], kv.second[1]));
+        return out;
+    }
+
+    // PairRdd::cogroup (src/rdd/pair_rdd.rs:123-155)  →  Vec<(String, (Vec<V>, Vec<V>))>
+    std::vector<std::pair<std::string, std::pair<std::vector<V>, std::vector<V>>>> cogroup(const StrPairRddT &other, size_t num_splits) const
+    {
+        std::vector<std::pair<std::string, std::pair<std::vector<V>, std::vector<V>>>> out;
+        for (auto &kv : cogroup_n({other}, num_splits))
+            out.emplace_back(std::move(kv.first), std::make_pair(std::move(kv.second[0]), std::move(kv.second[1])));
+        return out;
+    }
+
 private:
+    // this parent and the others, each shuffled into a string GROUP shuffle over num_splits
+    std::vector<detail::ShufPtr> group_shuffles(const std::vector<StrPairRddT> &others, size_t num_splits) const
+    {
+        std::vector<detail::ShufPtr> shs;
+        shs.push_back(detail::run_str_shuffle(*sc_, keys_, &vals_, num_slices_, num_splits, detail::dtype<V>::code, VB_AGG_GROUP));
+        for (auto &o : others)
+            shs.push_back(detail::run_str_shuffle(*o.sc_, o.keys_, &o.vals_, o.num_slices_, num_splits, detail::dtype<V>::code, VB_AGG_GROUP));
+        return shs;
+    }
+    static std::vector<vb_shuf *> raw(const std::vector<detail::ShufPtr> &shs)
+    {
+        std::vector<vb_shuf *> out;
+        for (auto &s : shs) out.push_back(s.get());
+        return out;
+    }
+
     std::shared_ptr<Context> sc_;
     size_t num_slices_;
     detail::StrCol keys_;

@@ -105,6 +105,18 @@ extern "C" {
                                       n_vals: *mut u64) -> i32;
     pub fn vb_shuffle_reduce_str(s: *mut vb_shuf, reduce_id: u32, out_key_offsets: *mut u64, out_key_bytes: *mut c_void,
                                  out_combined: *mut c_void, out_offsets: *mut u64, out_vals: *mut c_void, dst_loc: i32) -> i32;
+    // CoGroupedRdd::compute over String GROUP shuffles: the cogroup, and the join with a `required` mask whose keys
+    // come once per key (key i's rows are out_row_offsets[i] .. [i + 1])
+    pub fn vb_cogroup_n_str_size(sides: *const *mut vb_shuf, n_sides: u32, reduce_id: u32, n_keys: *mut u64,
+                                 n_key_bytes: *mut u64, n_vals: *mut u64) -> i32;
+    pub fn vb_cogroup_n_str(sides: *const *mut vb_shuf, n_sides: u32, reduce_id: u32, out_key_offsets: *mut u64,
+                            out_key_bytes: *mut c_void, out_offsets: *const *mut u64, out_vals: *const *mut c_void,
+                            dst_loc: i32) -> i32;
+    pub fn vb_join_n_str_size(sides: *const *mut vb_shuf, n_sides: u32, reduce_id: u32, required: u32, n_rows: *mut u64,
+                              n_keys: *mut u64, n_key_bytes: *mut u64) -> i32;
+    pub fn vb_join_n_str(sides: *const *mut vb_shuf, n_sides: u32, reduce_id: u32, required: u32, out_key_offsets: *mut u64,
+                         out_key_bytes: *mut c_void, out_row_offsets: *mut u64, out_vals: *const *mut c_void,
+                         out_valid: *const *mut u8, dst_loc: i32) -> i32;
     pub fn vb_hash_str(bytes: *const c_void, len: u64) -> u64;
     pub fn vb_get_partition_str(bytes: *const c_void, len: u64, n_reduce: u32) -> u32;
     pub fn vb_shuffle_free(s: *mut vb_shuf) -> i32;

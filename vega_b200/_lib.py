@@ -108,6 +108,10 @@ SYMBOLS = {
     "vb_shuffle_map_str": (_i32, [_vp, _u32, _vp, _vp, _u64, _vp, _u64, _i32]),
     "vb_shuffle_reduce_str_size": (_i32, [_vp, _u32, _pu64, _pu64, _pu64]),
     "vb_shuffle_reduce_str": (_i32, [_vp, _u32, _vp, _vp, _vp, _vp, _vp, _i32]),
+    "vb_cogroup_n_str_size": (_i32, [_pvp, _u32, _u32, _pu64, _pu64, _pu64]),
+    "vb_cogroup_n_str": (_i32, [_pvp, _u32, _u32, _vp, _vp, _pvp, _pvp, _i32]),
+    "vb_join_n_str_size": (_i32, [_pvp, _u32, _u32, _u32, _pu64, _pu64, _pu64]),
+    "vb_join_n_str": (_i32, [_pvp, _u32, _u32, _u32, _vp, _vp, _vp, _pvp, _pvp, _i32]),
     "vb_hash_str": (_u64, [_vp, _u64]),
     "vb_get_partition_str": (_u32, [_vp, _u64, _u32]),
     "vb_shuffle_reduce_blob_size": (_i32, [_vp, _u32, _pu64]),

@@ -294,6 +294,12 @@ struct CogroupNPlan {
     u32 *match = nullptr;          // [n_keys][n_sides] the key's index on every side, 0xFFFFFFFF where a side lacks it
     u64 *pos = nullptr;            // join: [n_keys] each key's first output row
     u64 total = 0;                 // join: rows of the partition
+    // string sides (str_plan_keys): the keys the call writes (a join's: those with rows) as Arrow-style offsets
+    bool str_done = false;
+    u64 str_nk = 0, str_nkb = 0;   // keys written, and their bytes
+    u64 *str_sel = nullptr;        // join: [str_nk] the plan keys with rows
+    u64 *str_koff = nullptr;       // [str_nk + 1] key byte offsets from 0
+    u64 *str_roff = nullptr;       // join: [str_nk + 1] each key's first row, then the total
 };
 // n_plans kinds: the cogroup, the inner join, or (>= 0) an outer join by its mask of required sides
 constexpr i64 NP_COGROUP = -2, NP_INNER = -1;
@@ -3461,7 +3467,10 @@ static_assert(CGN_MAX_SIDES == VB_MAX_COGROUP_SIDES, "cogroup side limit");
 static void free_cogroup_n_plan(vb_ctx *c, CogroupNPlan &p)
 {
     dev_free(c, p.new_keys); dev_free(c, p.match); dev_free(c, p.pos);
+    dev_free(c, p.str_sel); dev_free(c, p.str_koff); dev_free(c, p.str_roff);
 }
+
+static int str_n_sides(vb_shuf *const *sides, u32 n, u32 rid, StrNSides *a);
 
 // vb_cogroup's argument rules for every side; waits until every side is sealed
 static int cogroup_n_check(vb_shuf *const *sides, u32 n, u32 rid)
@@ -3489,7 +3498,7 @@ static int cogroup_n_sides(vb_shuf *const *sides, u32 n, u32 rid, CogroupNSides 
     a->n = n;
     for (u32 j = 0; j < n; ++j) {
         const vb_shuf *s = sides[j];
-        if (s->n_keys && !s->dict) return set_err(VB_ERR_STATE, "cogroup side without a key dictionary");
+        if (s->n_keys && !s->dict && !s->str) return set_err(VB_ERR_STATE, "cogroup side without a key dictionary");
         a->tab[j] = table_at(s->n_keys ? s->dict : nullptr, s->dict_log_cap);
         a->dense[j] = s->dense_of_slot;
         a->keys[j] = s->res_keys; a->offs[j] = s->res_offs; a->vals[j] = s->res_vals;
@@ -3521,27 +3530,35 @@ static int cogroup_n_plan(vb_shuf *const *sides, u32 n, u32 rid, i64 kind, const
     CogroupNPlan p;
     DevBuf match(c), new_keys(c), pos(c);
     TRY(match.alloc(cap * n * 4));
-    if (nk[0]) {
+    // string sides: the lookup reads each side's key index (the keys themselves are written from the match rows)
+    const bool str = s0->str != nullptr;
+    StrNSides sa;
+    if (str) TRY(str_n_sides(sides, n, rid, &sa));
+    auto probe = [&](u32 i, u32 *rows, unsigned char *flag, u64 *lidx) -> int {
         KLaunch kl(s0, K_JOIN);
-        cogroup_n_probe_kernel<<<(unsigned)((nk[0] + 255) / 256), 256, 0, c->stream>>>(a, 0, (u32)nk[0], match.as<u32>(), nullptr, nullptr);
-        TRY(kl.done("cogroup_n_probe_kernel"));
-    }
+        const unsigned g = (unsigned)((nk[i] + 255) / 256);
+        if (str) {
+            cogroup_n_str_probe_kernel<<<g, 256, 0, c->stream>>>(sa, i, (u32)nk[i], rows, flag, lidx);
+            return kl.done("cogroup_n_str_probe_kernel");
+        }
+        cogroup_n_probe_kernel<<<g, 256, 0, c->stream>>>(a, i, (u32)nk[i], rows, flag, lidx);
+        return kl.done("cogroup_n_probe_kernel");
+    };
+    if (nk[0]) TRY(probe(0, match.as<u32>(), nullptr, nullptr));
     p.n_keys = nk[0];
     if (all_keys && cap > nk[0]) {
-        TRY(new_keys.alloc((cap - nk[0]) * 8));
+        if (!str) TRY(new_keys.alloc((cap - nk[0]) * 8));
         for (u32 i = 1; i < n; ++i) {
             if (!nk[i]) continue;
             DevBuf rows(c), flag(c), lidx(c), ok(c), ov(c);
             TRY(rows.alloc(i + 1 < n ? nk[i] * n * 4 : 0)); TRY(flag.alloc(nk[i])); TRY(lidx.alloc(nk[i] * 8));
-            {
-                KLaunch kl(s0, K_JOIN);
-                cogroup_n_probe_kernel<<<(unsigned)((nk[i] + 255) / 256), 256, 0, c->stream>>>(a, i, (u32)nk[i], rows.as<u32>(),
-                                                                                              flag.as<unsigned char>(), lidx.as<u64>());
-                TRY(kl.done("cogroup_n_probe_kernel"));
-            }
+            TRY(probe(i, rows.as<u32>(), flag.as<unsigned char>(), lidx.as<u64>()));
             u64 m = 0;
-            TRY(compact_rows(s0, sides[i]->res_keys + a.kb[i], lidx.as<u64>(), nk[i], flag.as<unsigned char>(), ok, ov, &m,
-                             new_keys.as<u64>() + (p.n_keys - nk[0])));
+            if (str)      // no key values: only the new keys' local indices (ov) are kept
+                TRY(compact_rows(s0, lidx.as<u64>(), lidx.as<u64>(), nk[i], flag.as<unsigned char>(), ok, ov, &m));
+            else
+                TRY(compact_rows(s0, sides[i]->res_keys + a.kb[i], lidx.as<u64>(), nk[i], flag.as<unsigned char>(), ok, ov, &m,
+                                 new_keys.as<u64>() + (p.n_keys - nk[0])));
             if (!m) continue;
             {
                 KLaunch kl(s0, K_JOIN);
@@ -3610,8 +3627,13 @@ static int cogroup_n_size(vb_shuf *const *sides, u32 n_sides, u32 rid, u64 *n_ke
     return VB_OK;
 }
 
+static int str_plan_keys(vb_shuf *const *sides, u32 n, u32 rid, i64 kind, CogroupNPlan *p);
+static int str_write_keys(vb_shuf *const *sides, u32 n, u32 rid, i64 kind, CogroupNPlan *p, u64 *out_key_offsets,
+                          void *out_key_bytes, int dst_loc);
+
+// string sides: out_keys is the key bytes, out_key_offsets their offsets
 static int cogroup_n_write(vb_shuf *const *sides, u32 n_sides, u32 rid, void *out_keys, u64 *const *out_offsets,
-                           void *const *out_vals, int dst_loc)
+                           void *const *out_vals, int dst_loc, u64 *out_key_offsets = nullptr)
 {
     vb_shuf *s0 = sides[0];
     vb_ctx *c = s0->ctx;
@@ -3621,8 +3643,12 @@ static int cogroup_n_write(vb_shuf *const *sides, u32 n_sides, u32 rid, void *ou
     TRY(cogroup_n_plan(sides, n_sides, rid, NP_COGROUP, a, &p));
     const u64 nk = p->n_keys, nk0 = s0->bucket_off[rid + 1] - s0->bucket_off[rid];
     int rc = [&]() -> int {
-        TRY(copy_out(s0, out_keys, s0->res_keys ? s0->res_keys + a.kb[0] : nullptr, nk0 * 8, dst_loc));
-        TRY(copy_out(s0, out_keys ? (u64 *)out_keys + nk0 : nullptr, p->new_keys, (nk - nk0) * 8, dst_loc));
+        if (s0->str) {
+            TRY(str_write_keys(sides, n_sides, rid, NP_COGROUP, p, out_key_offsets, out_keys, dst_loc));
+        } else {
+            TRY(copy_out(s0, out_keys, s0->res_keys ? s0->res_keys + a.kb[0] : nullptr, nk0 * 8, dst_loc));
+            TRY(copy_out(s0, out_keys ? (u64 *)out_keys + nk0 : nullptr, p->new_keys, (nk - nk0) * 8, dst_loc));
+        }
         for (u32 j = 0; j < n_sides; ++j) {
             u64 *o_offs = out_offsets ? out_offsets[j] : nullptr;
             void *o_vals = out_vals ? out_vals[j] : nullptr;
@@ -3746,33 +3772,52 @@ static int join_n_outer_size(vb_shuf *const *sides, u32 n_sides, u32 rid, u32 re
     return VB_OK;
 }
 
+// string sides: out_k is the key bytes of the keys with rows, out_key_offsets their offsets and out_row_offsets their
+// rows; the rows carry no key
 static int join_n_outer_write(vb_shuf *const *sides, u32 n_sides, u32 rid, u32 required, void *out_k, void *const *out_vals,
-                              uint8_t *const *out_valid, int dst_loc)
+                              uint8_t *const *out_valid, int dst_loc, u64 *out_key_offsets = nullptr, u64 *out_row_offsets = nullptr)
 {
     vb_shuf *s0 = sides[0];
     vb_ctx *c = s0->ctx;
+    const bool str = s0->str != nullptr;
     CogroupNSides a;
     TRY(cogroup_n_sides(sides, n_sides, rid, &a));
     CogroupNPlan *p = nullptr;
     TRY(cogroup_n_plan(sides, n_sides, rid, required, a, &p));
     const u64 total = p->total;
     int rc = [&]() -> int {
-        if (!total) return VB_OK;
-        bool missing = !out_k || !out_vals;
+        if (!total) {
+            if (str) TRY(str_write_keys(sides, n_sides, rid, required, p, out_key_offsets, out_k, dst_loc));
+            if (str && out_row_offsets) TRY(copy_out(s0, out_row_offsets, p->str_roff, 8, dst_loc));
+            return VB_OK;
+        }
+        bool missing = !out_vals;
+        if (str) {
+            TRY(str_plan_keys(sides, n_sides, rid, required, p));
+            missing = missing || !out_key_offsets || !out_row_offsets || (p->str_nkb && !out_k);
+        } else {
+            missing = missing || !out_k;
+        }
         for (u32 j = 0; !missing && j < n_sides; ++j) missing = !out_vals[j];
         if (missing) return set_err(VB_ERR_INVALID, "NULL output with %llu rows to write", (unsigned long long)total);
         JoinNOuterOut o{};
         DevBuf bufs[2 * CGN_MAX_SIDES + 1];     // host output: keys, values per side, validity per side
-        o.k = (u64 *)out_k;
-        o.new_keys = p->new_keys;
-        o.nk0 = (u32)(s0->bucket_off[rid + 1] - s0->bucket_off[rid]);
+        if (!str) {
+            o.k = (u64 *)out_k;
+            o.new_keys = p->new_keys;
+            o.nk0 = (u32)(s0->bucket_off[rid + 1] - s0->bucket_off[rid]);
+        }
         for (u32 j = 0; j < n_sides; ++j) {
             o.v[j] = (u64 *)out_vals[j];
             o.valid[j] = out_valid ? out_valid[j] : nullptr;
         }
         if (dst_loc == VB_HOST) {
-            for (u32 j = 0; j <= n_sides; ++j) { bufs[j].c = c; TRY(bufs[j].alloc(total * 8)); }
-            o.k = bufs[n_sides].as<u64>();
+            for (u32 j = 0; j <= n_sides; ++j) {
+                if (str && j == n_sides) continue;
+                bufs[j].c = c;
+                TRY(bufs[j].alloc(total * 8));
+            }
+            if (!str) o.k = bufs[n_sides].as<u64>();
             for (u32 j = 0; j < n_sides; ++j) {
                 o.v[j] = bufs[j].as<u64>();
                 if (!o.valid[j]) continue;
@@ -3785,11 +3830,20 @@ static int join_n_outer_write(vb_shuf *const *sides, u32 n_sides, u32 rid, u32 r
         {
             KLaunch kl(s0, K_JOIN);
             const u64 blocks = std::min<u64>((total + 255) / 256, (u64)c->sm_count * 8);
-            join_n_outer_expand_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(a, p->pos, (u32)p->n_keys, total, p->match, o);
-            TRY(kl.done("join_n_outer_expand_kernel"));
+            if (str) {
+                join_n_outer_expand_nokey_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(a, p->pos, (u32)p->n_keys, total, p->match, o);
+                TRY(kl.done("join_n_outer_expand_nokey_kernel"));
+            } else {
+                join_n_outer_expand_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(a, p->pos, (u32)p->n_keys, total, p->match, o);
+                TRY(kl.done("join_n_outer_expand_kernel"));
+            }
+        }
+        if (str) {
+            TRY(str_write_keys(sides, n_sides, rid, required, p, out_key_offsets, out_k, dst_loc));
+            TRY(copy_out(s0, out_row_offsets, p->str_roff, (p->str_nk + 1) * 8, dst_loc));
         }
         if (dst_loc == VB_HOST) {
-            TRY(copy_out(s0, out_k, o.k, total * 8, VB_HOST));
+            if (!str) TRY(copy_out(s0, out_k, o.k, total * 8, VB_HOST));
             for (u32 j = 0; j < n_sides; ++j) {
                 TRY(copy_out(s0, out_vals[j], o.v[j], total * 8, VB_HOST));
                 if (o.valid[j]) TRY(copy_out(s0, out_valid[j], o.valid[j], total, VB_HOST));
@@ -3949,6 +4003,11 @@ struct StrState {
     u64 *key_off = nullptr;               // [n_keys + 1] byte offset of every result key (partition-major, from 0)
     unsigned char *key_bytes = nullptr;   // the result keys' bytes
     std::vector<u64> kb_off;              // [n_reduce + 1] first key byte of each partition
+    // key index of the result keys (str_key_index), built by the first cogroup or join that reads the shuffle
+    u64 *res_hash = nullptr;              // [n_keys] each key's hash
+    u64 *ix_fp = nullptr;                 // [1 << ix_log_cap] fingerprints, 0 = empty
+    u32 *ix_id = nullptr;                 // [1 << ix_log_cap] dense key id of each slot
+    u32 ix_log_cap = 0;
 };
 
 constexpr u32 STR_MAX_LOG_CAP = 33;       // index slots: < 2^31 distinct keys at load <= 0.6
@@ -3996,6 +4055,9 @@ static void free_str(vb_shuf *s)
     free_str_dict(s);
     dev_free(s->ctx, t->key_off);
     dev_free(s->ctx, t->key_bytes);
+    dev_free(s->ctx, t->res_hash);
+    dev_free(s->ctx, t->ix_fp);
+    dev_free(s->ctx, t->ix_id);
     delete t;
     s->str = nullptr;
 }
@@ -4456,6 +4518,231 @@ extern "C" int32_t vb_shuffle_reduce_str(vb_shuf *s, uint32_t r, uint64_t *out_k
     }
     CU(cudaStreamSynchronize(c->stream));
     return VB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// cogroup and join of string keys (CoGroupedRdd::compute over `String` keys, co_grouped_rdd.rs:75-135, 206-249)
+// The N-way plan of the integer sides (cogroup_n_plan) runs on the match matrix of per-side key indices; for string
+// sides only the lookup (cogroup_n_str_probe_kernel over each side's key index) and the output keys differ.  An output
+// key's bytes come from the first side of its match row that has it.  Every join goes through the outer-join plan
+// with its `required` mask (all bits: the inner join) and writes each key with rows once, with its row offsets.
+// ---------------------------------------------------------------------------------------------
+
+// The key index of a sealed string shuffle's result keys, built on first use with the context locked and kept until
+// vb_shuffle_free.  Sized like the dictionary index (load <= 0.5, 12 bytes per slot).
+static int str_key_index(vb_shuf *s)
+{
+    StrState *t = s->str;
+    vb_ctx *c = s->ctx;
+    if (t->ix_fp || !s->n_keys) return VB_OK;
+    const u64 D = s->n_keys;
+    const u32 log_cap = choose_log_cap(D, D, false, STR_MAX_LOG_CAP, c->l2_bytes, 12);
+    const u64 cap = 1ull << log_cap;
+    DevBuf fp(c), id(c), h(c);
+    TRY(fp.alloc(cap * 8));
+    TRY(id.alloc(cap * 4));
+    TRY(h.alloc(D * 8));
+    CU(cudaMemsetAsync(fp.p, 0, cap * 8, c->stream));
+    {
+        KLaunch kl(s, K_DICT, D);
+        const u64 blocks = std::min<u64>((D + 255) / 256, (u64)c->sm_count * 8);
+        str_key_index_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(t->key_off, t->key_bytes, (u32)D, fp.as<u64>(), id.as<u32>(),
+                                                                      log_cap, str_fp_mask(), h.as<u64>());
+        TRY(kl.done("str_key_index_kernel"));
+    }
+    CU(cudaStreamSynchronize(c->stream));
+    t->ix_fp = (u64 *)fp.release();
+    t->ix_id = (u32 *)id.release();
+    t->res_hash = (u64 *)h.release();
+    t->ix_log_cap = log_cap;
+    return VB_OK;
+}
+
+// describe the indexed string sides for the kernels
+static int str_n_sides(vb_shuf *const *sides, u32 n, u32 rid, StrNSides *a)
+{
+    *a = StrNSides{};
+    a->n = n;
+    a->fp_mask = str_fp_mask();
+    for (u32 j = 0; j < n; ++j) {
+        const vb_shuf *s = sides[j];
+        const StrState *t = s->str;
+        if (s->n_keys && !t->ix_fp) return set_err(VB_ERR_STATE, "string cogroup side without a key index");
+        a->fp[j] = t->ix_fp; a->id[j] = t->ix_id; a->log_cap[j] = t->ix_log_cap;
+        a->hash[j] = t->res_hash; a->key_off[j] = t->key_off; a->bytes[j] = t->key_bytes;
+        a->kb[j] = (u32)s->bucket_off[rid];
+    }
+    return VB_OK;
+}
+
+// The keys a call over the plan writes (all of a cogroup's; a join's with rows, taken in order by the stable
+// compaction with their first rows), their byte offsets and total bytes.  Done once per plan.
+static int str_plan_keys(vb_shuf *const *sides, u32 n, u32 rid, i64 kind, CogroupNPlan *p)
+{
+    if (p->str_done) return VB_OK;
+    vb_shuf *s0 = sides[0];
+    vb_ctx *c = s0->ctx;
+    const bool join = kind != NP_COGROUP;
+    StrNSides sa;
+    TRY(str_n_sides(sides, n, rid, &sa));
+    DevBuf sel(c), koff(c), roff(c), len(c), ov(c);
+    u64 nk = p->n_keys, nkb = 0;
+    if (join) {
+        if (nk) {
+            DevBuf flag(c), idx(c);
+            TRY(flag.alloc(nk));
+            TRY(idx.alloc(nk * 8));
+            {
+                KLaunch kl(s0, K_JOIN);
+                str_join_keep_kernel<<<(unsigned)((nk + 255) / 256), 256, 0, c->stream>>>(p->pos, nk, p->total, flag.as<unsigned char>(),
+                                                                                          idx.as<u64>());
+                TRY(kl.done("str_join_keep_kernel"));
+            }
+            u64 m = 0;
+            TRY(compact_rows(s0, idx.as<u64>(), p->pos, nk, flag.as<unsigned char>(), sel, ov, &m));
+            nk = m;
+        }
+        TRY(roff.alloc((nk + 1) * 8));
+        if (nk) CU(cudaMemcpyAsync(roff.p, ov.p, nk * 8, cudaMemcpyDeviceToDevice, c->stream));
+        CU(cudaMemcpyAsync(roff.as<u64>() + nk, &p->total, 8, cudaMemcpyHostToDevice, c->stream));
+    }
+    TRY(koff.alloc((nk + 1) * 8));
+    if (nk) {
+        TRY(len.alloc(nk * 8));
+        {
+            KLaunch kl(s0, K_JOIN);
+            str_n_key_len_kernel<<<(unsigned)((nk + 255) / 256), 256, 0, c->stream>>>(sa, p->match, sel.as<u64>(), nk, len.as<u64>());
+            TRY(kl.done("str_n_key_len_kernel"));
+        }
+        TRY(exclusive_scan_u64(s0, len.as<u64>(), koff.as<u64>(), nk, koff.as<u64>() + nk));
+        CU(cudaMemcpyAsync(c->h_scratch, koff.as<u64>() + nk, 8, cudaMemcpyDeviceToHost, c->stream));
+    } else {
+        CU(cudaMemsetAsync(koff.p, 0, 8, c->stream));
+    }
+    CU(cudaStreamSynchronize(c->stream));
+    if (nk) nkb = *(u64 *)c->h_scratch;
+    p->str_sel = (u64 *)sel.release();
+    p->str_koff = (u64 *)koff.release();
+    p->str_roff = (u64 *)roff.release();
+    p->str_nk = nk;
+    p->str_nkb = nkb;
+    p->str_done = true;
+    return VB_OK;
+}
+
+// out_key_offsets [str_nk + 1] and out_key_bytes [str_nkb] of the plan's keys (NULL outputs skipped)
+static int str_write_keys(vb_shuf *const *sides, u32 n, u32 rid, i64 kind, CogroupNPlan *p, u64 *out_key_offsets,
+                          void *out_key_bytes, int dst_loc)
+{
+    TRY(str_plan_keys(sides, n, rid, kind, p));
+    vb_shuf *s0 = sides[0];
+    vb_ctx *c = s0->ctx;
+    TRY(copy_out(s0, out_key_offsets, p->str_koff, (p->str_nk + 1) * 8, dst_loc));
+    if (!out_key_bytes || !p->str_nkb) return VB_OK;
+    StrNSides sa;
+    TRY(str_n_sides(sides, n, rid, &sa));
+    DevBuf tmp(c);
+    unsigned char *d = (unsigned char *)out_key_bytes;
+    if (dst_loc == VB_HOST) { TRY(tmp.alloc(p->str_nkb)); d = tmp.as<unsigned char>(); }
+    {
+        KLaunch kl(s0, K_JOIN);
+        str_n_key_bytes_kernel<<<(unsigned)((p->str_nk * 32 + 255) / 256), 256, 0, c->stream>>>(sa, p->match, p->str_sel, p->str_nk,
+                                                                                               p->str_koff, d);
+        TRY(kl.done("str_n_key_bytes_kernel"));
+    }
+    if (dst_loc == VB_HOST) TRY(copy_out(s0, out_key_bytes, d, p->str_nkb, VB_HOST));
+    return VB_OK;
+}
+
+// vb_cogroup_n's argument rules over string GROUP shuffles; waits until every side is sealed
+static int cogroup_n_str_check(vb_shuf *const *sides, u32 n, u32 rid)
+{
+    if (!sides) return set_err(VB_ERR_INVALID, "sides is NULL");
+    if (n < 1 || n > VB_MAX_COGROUP_SIDES) return set_err(VB_ERR_INVALID, "n_sides %u is not in [1, %d]", n, VB_MAX_COGROUP_SIDES);
+    for (u32 j = 0; j < n; ++j) {
+        const vb_shuf *s = sides[j];
+        if (!s) return set_err(VB_ERR_INVALID, "side %u is NULL", j);
+        if (!s->str) return set_err(VB_ERR_INVALID, "side %u is not a string-key shuffle (use vb_cogroup_n / vb_join_n_outer)", j);
+        if (s->agg != VB_AGG_GROUP) return set_err(VB_ERR_INVALID, "side %u is not a GROUP shuffle", j);
+        if (s->n_reduce != sides[0]->n_reduce) return set_err(VB_ERR_INVALID, "side %u uses a different partitioner than side 0", j);
+        if (s->ctx != sides[0]->ctx) return set_err(VB_ERR_INVALID, "side %u lives on a different context than side 0", j);
+    }
+    if (rid >= sides[0]->n_reduce) return set_err(VB_ERR_INVALID, "reduce_id %u >= n_reduce %u", rid, sides[0]->n_reduce);
+    for (u32 j = 0; j < n; ++j) TRY(wait_sealed(sides[j]));
+    return VB_OK;
+}
+
+static int join_n_str_check(vb_shuf *const *sides, u32 n, u32 rid, u32 required)
+{
+    TRY(cogroup_n_str_check(sides, n, rid));
+    if (required >> n) return set_err(VB_ERR_INVALID, "required mask %#x names a side >= n_sides %u", required, n);
+    return VB_OK;
+}
+
+// the plan of (sides, rid, kind) with its string keys, every side indexed; the context is locked
+static int str_plan(vb_shuf *const *sides, u32 n, u32 rid, i64 kind, CogroupNPlan **p)
+{
+    for (u32 j = 0; j < n; ++j) TRY(str_key_index(sides[j]));
+    CogroupNSides a;
+    TRY(cogroup_n_sides(sides, n, rid, &a));
+    TRY(cogroup_n_plan(sides, n, rid, kind, a, p));
+    return str_plan_keys(sides, n, rid, kind, *p);
+}
+
+extern "C" int32_t vb_cogroup_n_str_size(vb_shuf *const *sides, uint32_t n_sides, uint32_t rid, uint64_t *n_keys,
+                                         uint64_t *n_key_bytes, uint64_t *n_vals)
+{
+    TRY(cogroup_n_str_check(sides, n_sides, rid));
+    vb_ctx *c = sides[0]->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    CogroupNPlan *p = nullptr;
+    TRY(str_plan(sides, n_sides, rid, NP_COGROUP, &p));
+    if (n_keys) *n_keys = p->str_nk;
+    if (n_key_bytes) *n_key_bytes = p->str_nkb;
+    for (u32 j = 0; n_vals && j < n_sides; ++j) n_vals[j] = sides[j]->val_off[rid + 1] - sides[j]->val_off[rid];
+    return VB_OK;
+}
+
+extern "C" int32_t vb_cogroup_n_str(vb_shuf *const *sides, uint32_t n_sides, uint32_t rid, uint64_t *out_key_offsets,
+                                    void *out_key_bytes, uint64_t *const *out_offsets, void *const *out_vals, int32_t dst_loc)
+{
+    TRY(cogroup_n_str_check(sides, n_sides, rid));
+    if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
+    vb_ctx *c = sides[0]->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    for (u32 j = 0; j < n_sides; ++j) TRY(str_key_index(sides[j]));
+    return cogroup_n_write(sides, n_sides, rid, out_key_bytes, out_offsets, out_vals, dst_loc, out_key_offsets);
+}
+
+extern "C" int32_t vb_join_n_str_size(vb_shuf *const *sides, uint32_t n_sides, uint32_t rid, uint32_t required,
+                                      uint64_t *n_rows, uint64_t *n_keys, uint64_t *n_key_bytes)
+{
+    TRY(join_n_str_check(sides, n_sides, rid, required));
+    vb_ctx *c = sides[0]->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    CogroupNPlan *p = nullptr;
+    TRY(str_plan(sides, n_sides, rid, required, &p));
+    if (n_rows) *n_rows = p->total;
+    if (n_keys) *n_keys = p->str_nk;
+    if (n_key_bytes) *n_key_bytes = p->str_nkb;
+    return VB_OK;
+}
+
+extern "C" int32_t vb_join_n_str(vb_shuf *const *sides, uint32_t n_sides, uint32_t rid, uint32_t required, uint64_t *out_key_offsets,
+                                 void *out_key_bytes, uint64_t *out_row_offsets, void *const *out_vals, uint8_t *const *out_valid,
+                                 int32_t dst_loc)
+{
+    TRY(join_n_str_check(sides, n_sides, rid, required));
+    if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
+    vb_ctx *c = sides[0]->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    for (u32 j = 0; j < n_sides; ++j) TRY(str_key_index(sides[j]));
+    return join_n_outer_write(sides, n_sides, rid, required, out_key_bytes, out_vals, out_valid, dst_loc, out_key_offsets,
+                              out_row_offsets);
 }
 
 extern "C" uint64_t vb_hash_str(const void *bytes, uint64_t len) { return metro64_1_str((const unsigned char *)bytes, len); }

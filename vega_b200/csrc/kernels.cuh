@@ -1862,9 +1862,11 @@ __global__ void join_n_outer_count_kernel(const __grid_constant__ CogroupNSides 
 }
 
 // One thread per output row, as join_n_expand_kernel: the digit of a side that lacks the key has radix 1 (always 0)
-// and gives a None slot.
-__global__ void join_n_outer_expand_kernel(const __grid_constant__ CogroupNSides a, const u64 *__restrict__ pos, u32 nk,
-                                           u64 total, const u32 *__restrict__ match, const __grid_constant__ JoinNOuterOut out)
+// and gives a None slot.  KEYS: write out.k (the string join writes its keys once per key instead, and leaves out.k,
+// out.new_keys and out.nk0 unset).
+template <bool KEYS>
+__device__ __forceinline__ void join_n_outer_expand_rows(const CogroupNSides &a, const u64 *__restrict__ pos, u32 nk, u64 total,
+                                                         const u32 *__restrict__ match, const JoinNOuterOut &out)
 {
     const u64 stride = (u64)gridDim.x * blockDim.x;
     for (u64 o = (u64)blockIdx.x * blockDim.x + threadIdx.x; o < total; o += stride) {
@@ -1892,8 +1894,20 @@ __global__ void join_n_outer_expand_kernel(const __grid_constant__ CogroupNSides
             out.v[j][o] = a.vals[j][b + d];
             if (out.valid[j]) out.valid[j][o] = 1;
         }
-        out.k[o] = lo < out.nk0 ? a.keys[0][a.kb[0] + lo] : out.new_keys[lo - out.nk0];
+        if (KEYS) out.k[o] = lo < out.nk0 ? a.keys[0][a.kb[0] + lo] : out.new_keys[lo - out.nk0];
     }
+}
+
+__global__ void join_n_outer_expand_kernel(const __grid_constant__ CogroupNSides a, const u64 *__restrict__ pos, u32 nk,
+                                           u64 total, const u32 *__restrict__ match, const __grid_constant__ JoinNOuterOut out)
+{
+    join_n_outer_expand_rows<true>(a, pos, nk, total, match, out);
+}
+
+__global__ void join_n_outer_expand_nokey_kernel(const __grid_constant__ CogroupNSides a, const u64 *__restrict__ pos, u32 nk,
+                                                 u64 total, const u32 *__restrict__ match, const __grid_constant__ JoinNOuterOut out)
+{
+    join_n_outer_expand_rows<false>(a, pos, nk, total, match, out);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -311,4 +311,122 @@ __global__ void __launch_bounds__(256) str_reduce_kernel(const u32 *__restrict__
     }
 }
 
+// ---- cogroup and join of string GROUP shuffles (engine.cu, "cogroup and join of string keys") --------------------
+// Seal drops the dictionary, so a side read by a cogroup or join first gets a key index of its result keys: each dense
+// key's hash, and an index of StrDict's layout (4-slot buckets of fingerprints, parallel dense key ids).  The N-way
+// plan (cogroup_n_*) then runs unchanged on the match matrix; only the probe, and the output keys, read bytes.
+struct StrNSides {
+    const u64 *fp[CGN_MAX_SIDES];                 // index fingerprints, 0 = empty slot; NULL: the side has no keys
+    const u32 *id[CGN_MAX_SIDES];                 // dense key id of each index slot
+    u32 log_cap[CGN_MAX_SIDES];
+    const u64 *hash[CGN_MAX_SIDES];               // [n_keys] hash of each dense key
+    const u64 *key_off[CGN_MAX_SIDES];            // [n_keys + 1] byte offset of each dense key (StrState::key_off)
+    const unsigned char *bytes[CGN_MAX_SIDES];    // the keys' bytes (StrState::key_bytes)
+    u32 kb[CGN_MAX_SIDES];                        // the partition's first key on each side
+    u64 fp_mask;
+    u32 n;
+};
+
+// One thread per dense key: hash its bytes, then claim a slot.  The keys are distinct, so nothing is compared; the
+// index is sized for load <= 0.6, so every key finds a free slot.
+__global__ void str_key_index_kernel(const u64 *__restrict__ key_off, const unsigned char *__restrict__ bytes, u32 n, u64 *fp,
+                                     u32 *__restrict__ id, u32 log_cap, u64 fp_mask, u64 *__restrict__ hash)
+{
+    const u64 nb = 1ull << (log_cap - 2);
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 e = (u64)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += stride) {
+        const u64 o = key_off[e];
+        const u64 h = metro64_1_str(bytes + o, key_off[e + 1] - o), f = str_fp(h, fp_mask);
+        hash[e] = h;
+        u64 b = str_bucket(h, log_cap);
+        bool placed = false;
+        for (u64 probe = 0; probe < nb && !placed; ++probe, b = (b + 1) & (nb - 1))
+            for (u32 j = 0; j < BUCKET; ++j)
+                if (atomicCAS((unsigned long long *)&fp[BUCKET * b + j], 0ull, (unsigned long long)f) == 0ull) {
+                    id[BUCKET * b + j] = (u32)e;
+                    placed = true;
+                    break;
+                }
+    }
+}
+
+// Side j's dense key id of the key (h, key[0..len)), or 0xFFFFFFFF: a fingerprint match is a key only if its length
+// and bytes are equal too; an empty slot ends the probe.
+VB_D u32 str_side_find(const StrNSides &a, u32 j, u64 h, const unsigned char *key, u64 len)
+{
+    if (!a.fp[j]) return 0xFFFFFFFFu;
+    const u64 nb = 1ull << (a.log_cap[j] - 2), f = str_fp(h, a.fp_mask);
+    u64 b = str_bucket(h, a.log_cap[j]);
+    for (u64 probe = 0; probe < nb; ++probe, b = (b + 1) & (nb - 1))
+        for (u32 s = 0; s < BUCKET; ++s) {
+            const u64 slot = BUCKET * b + s, cur = a.fp[j][slot];
+            if (cur == 0) return 0xFFFFFFFFu;
+            if (cur != f) continue;
+            const u32 e = a.id[j][slot];
+            const u64 o = a.key_off[j][e];
+            if (a.key_off[j][e + 1] - o == len && str_equal(key, a.bytes[j] + o, len)) return e;
+        }
+    return 0xFFFFFFFFu;
+}
+
+// cogroup_n_probe_kernel over string sides: the same rows, flags and lidx, with the key looked up by hash and bytes.
+// A key's hash decides its partition, so a key found through a side's shuffle-wide index is in the same partition.
+__global__ void cogroup_n_str_probe_kernel(const __grid_constant__ StrNSides a, u32 i, u32 nk, u32 *__restrict__ rows,
+                                           unsigned char *__restrict__ flag, u64 *__restrict__ lidx)
+{
+    const u32 t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= nk) return;
+    const u32 e = a.kb[i] + t;
+    const u64 h = a.hash[i][e], o = a.key_off[i][e], len = a.key_off[i][e + 1] - o;
+    const unsigned char *key = a.bytes[i] + o;
+    for (u32 j = 0; j < a.n; ++j) {
+        const u32 m = j == i ? e : str_side_find(a, j, h, key, len);
+        if (j < i && m != 0xFFFFFFFFu) { flag[t] = 0; return; }     // an earlier side already gave this key
+        if (i == 0 || j > i) rows[(u64)t * a.n + j] = m;
+    }
+    if (i) { flag[t] = 1; lidx[t] = t; }
+}
+
+// The side an output key's bytes come from: the first side of its match row that has it.
+VB_D u32 str_key_owner(const u32 *row, u32 n)
+{
+    u32 j = 0;
+    while (j + 1 < n && row[j] == 0xFFFFFFFFu) ++j;
+    return j;
+}
+
+// len[o] = the byte length of output key sel[o] (sel NULL: o) of the plan
+__global__ void str_n_key_len_kernel(const __grid_constant__ StrNSides a, const u32 *__restrict__ match, const u64 *__restrict__ sel,
+                                     u64 nk, u64 *__restrict__ len)
+{
+    const u64 o = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (o >= nk) return;
+    const u32 *row = match + (sel ? sel[o] : o) * a.n;
+    const u32 j = str_key_owner(row, a.n);
+    len[o] = a.key_off[j][row[j] + 1] - a.key_off[j][row[j]];
+}
+
+// Output key o's bytes at out[off[o] .. off[o + 1]): one warp per key, as str_gather_bytes_kernel
+__global__ void str_n_key_bytes_kernel(const __grid_constant__ StrNSides a, const u32 *__restrict__ match, const u64 *__restrict__ sel,
+                                       u64 nk, const u64 *__restrict__ off, unsigned char *__restrict__ out)
+{
+    const u64 w = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (w >= nk) return;
+    const u32 *row = match + (sel ? sel[w] : w) * a.n;
+    const u32 j = str_key_owner(row, a.n);
+    const unsigned char *src = a.bytes[j] + a.key_off[j][row[j]];
+    const u64 dst = off[w], len = off[w + 1] - dst;
+    for (u64 k = lane_id(); k < len; k += 32) out[dst + k] = src[k];
+}
+
+// flag[o] = 1 for a join plan key with rows (pos[o + 1] > pos[o], pos[nk] read as total), idx[o] = o
+__global__ void str_join_keep_kernel(const u64 *__restrict__ pos, u64 nk, u64 total, unsigned char *__restrict__ flag,
+                                     u64 *__restrict__ idx)
+{
+    const u64 o = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (o >= nk) return;
+    flag[o] = (o + 1 < nk ? pos[o + 1] : total) > pos[o];
+    idx[o] = o;
+}
+
 }  // namespace vb

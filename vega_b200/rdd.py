@@ -1272,6 +1272,127 @@ class StrPairRdd(PairRdd):
     sort_by_key = _no_str("sort_by_key")
 
 
+class StrCoGroupedRdd(_Base):
+    """CoGroupedRdd::new(rdds, HashPartitioner::new(num_splits)) over `String` keys (vb_cogroup_n_str / vb_join_n_str):
+    the cogroup and the joins of 1 to 16 parents, with keys matched by their bytes.  A parent is a StrPairRdd, shuffled
+    with the Vec-append aggregator, or a string reduce_by_key / count_by_key result, whose partitions are read on the
+    device and shuffled again with the list [its result] per key.  The methods are CoGroupedRdd's, with keys as a
+    numpy object array of str:
+      compute(r) -> (keys, [(offsets, values) per parent]);  collect() -> [(k, [vs_0, ..., vs_{n-1}])]
+      join_compute(r) / join_collect() -> (k, [v_0, ..., v_{n-1}]), one k per row
+      outer_join_compute(r, required) / outer_join_collect(required): optional parents as numpy.ma.MaskedArray
+    join_raw(r, required) returns the device's keyed form without decoding: (key offsets, key bytes, row offsets,
+    [values], [validity or None]), each key once with its rows [row_offsets[i], row_offsets[i + 1])."""
+
+    def __init__(self, rdds, num_splits):
+        rdds = list(rdds)
+        if not 1 <= len(rdds) <= L.VB_MAX_COGROUP_SIDES:
+            raise ValueError(f"a cogroup takes 1 to {L.VB_MAX_COGROUP_SIDES} parents, got {len(rdds)}")
+        if num_splits < 1:
+            raise ValueError("num_splits must be >= 1")
+        for j, r in enumerate(rdds):
+            if isinstance(r, StrShuffledRdd):
+                if r.agg_name not in _REDUCE_AGGS:
+                    raise TypeError(f"parent {j}: a {r.agg_name} result is not a join parent (reduce_by_key and "
+                                    "count_by_key results are)")
+            elif not isinstance(r, StrPairRdd):
+                raise TypeError(f"parent {j} is not a String-key PairRdd or reduce result")
+        if any(r.sc is not rdds[0].sc for r in rdds):
+            raise TypeError("the parents live on different contexts")
+        self.rdds, self.num_slices, self.sc = rdds, num_splits, rdds[0].sc
+        self._shs = None
+
+    _required_mask = CoGroupedRdd._required_mask
+
+    def _side(self, r):
+        """The sealed string GROUP shuffle over num_splits partitions this parent gives."""
+        if isinstance(r, StrPairRdd):
+            return StrShuffledRdd(r, "group", self.num_slices)._run()
+        import torch
+        sh = r._run()
+        dev = f"cuda:{sh._lib.vb_ctx_device(self.sc._h)}"
+        vcode = L.VB_U64 if sh.agg == L.VB_AGG_COUNT else sh.vcode
+        out = StrShuffle(self.sc, sh.n_reduce, self.num_slices, vcode, L.VB_AGG_GROUP)
+        for p in range(sh.n_reduce):
+            nk, nb, _ = sh.reduce_size(p)
+            ko = torch.empty(nk + 1, dtype=torch.int64, device=dev)
+            kb = torch.empty(nb, dtype=torch.uint8, device=dev)
+            v = torch.empty(nk, dtype=torch.int64, device=dev)
+            sh.reduce_device(p, out_key_offsets=ko, out_key_bytes=kb, out_comb=v)
+            out.map(p, _StrCol(StrKeys(ko, kb)), _Col(v, role="value"), 0, nk)
+        out.seal()
+        return out
+
+    def _sides(self):
+        if self._shs is None:
+            self._shs = [self._side(r) for r in self.rdds]
+        return self._shs, (ctypes.c_void_p * len(self._shs))(*[s._h.value for s in self._shs])
+
+    def compute_raw(self, split):
+        """Partition `split` of the cogroup without decoding: (key offsets, key bytes, [(offsets, values) per parent])."""
+        shs, sides = self._sides()
+        n, lib = len(shs), self.sc._lib
+        nk, nb, nv = ctypes.c_uint64(), ctypes.c_uint64(), (ctypes.c_uint64 * n)()
+        L.check(lib.vb_cogroup_n_str_size(sides, n, split, ctypes.byref(nk), ctypes.byref(nb), nv))
+        ko, kb = np.empty(nk.value + 1, dtype=np.uint64), np.empty(nb.value, dtype=np.uint8)
+        offs = [np.empty(nk.value + 1, dtype=np.uint64) for _ in shs]
+        vals = [np.empty(nv[j], dtype=_NP_OF[s.vcode]) for j, s in enumerate(shs)]
+        ptrs = lambda xs: (ctypes.c_void_p * n)(*[x.ctypes.data for x in xs])
+        L.check(lib.vb_cogroup_n_str(sides, n, split, ko.ctypes.data_as(ctypes.c_void_p), kb.ctypes.data_as(ctypes.c_void_p),
+                                     ptrs(offs), ptrs(vals), L.VB_HOST))
+        return ko, kb, list(zip(offs, vals))
+
+    def compute(self, split):
+        ko, kb, lists = self.compute_raw(split)
+        return _decode_keys(ko, kb), lists
+
+    def collect(self):
+        out = []
+        for r in range(self.num_slices):
+            keys, lists = self.compute(r)
+            lists = [(o.tolist(), v) for o, v in lists]
+            out.extend((k, [v[o[i]:o[i + 1]] for o, v in lists]) for i, k in enumerate(keys.tolist()))
+        return out
+
+    def join_raw(self, split, required):
+        """Partition `split` of the join in the device's keyed form: (key offsets, key bytes, row offsets, [values],
+        [validity, None for a required parent])."""
+        mask = self._required_mask(required)
+        shs, sides = self._sides()
+        n, lib = len(shs), self.sc._lib
+        nr, nk, nb = ctypes.c_uint64(), ctypes.c_uint64(), ctypes.c_uint64()
+        L.check(lib.vb_join_n_str_size(sides, n, split, mask, ctypes.byref(nr), ctypes.byref(nk), ctypes.byref(nb)))
+        ko, kb = np.empty(nk.value + 1, dtype=np.uint64), np.empty(nb.value, dtype=np.uint8)
+        ro = np.empty(nk.value + 1, dtype=np.uint64)
+        vs = [np.empty(nr.value, dtype=_NP_OF[s.vcode]) for s in shs]
+        valid = [None if mask >> j & 1 else np.empty(nr.value, dtype=np.uint8) for j in range(n)]
+        ptrs = lambda xs: (ctypes.c_void_p * n)(*[x.ctypes.data if x is not None else None for x in xs])
+        p = lambda x: x.ctypes.data_as(ctypes.c_void_p)
+        L.check(lib.vb_join_n_str(sides, n, split, mask, p(ko), p(kb), p(ro), ptrs(vs), ptrs(valid), L.VB_HOST))
+        return ko, kb, ro, vs, valid
+
+    def outer_join_compute(self, split, required):
+        """Partition `split` of the outer join of all parents: (k, [v_0, ..., v_{n-1}]) with one key per row; see
+        CoGroupedRdd.outer_join_compute."""
+        ko, kb, ro, vs, valid = self.join_raw(split, required)
+        keys = _decode_keys(ko, kb)
+        k = np.repeat(keys, np.diff(ro.astype(np.int64))) if len(keys) else np.empty(0, dtype=object)
+        return k, [v if ok is None else np.ma.MaskedArray(v, mask=ok == 0) for v, ok in zip(vs, valid)]
+
+    def outer_join_collect(self, required):
+        mask = self._required_mask(required)
+        parts = [self.outer_join_compute(r, mask) for r in range(self.num_slices)]
+        cat = lambda xs: np.ma.concatenate(xs) if isinstance(xs[0], np.ma.MaskedArray) else np.concatenate(xs)
+        return np.concatenate([p[0] for p in parts]), [cat([p[1][j] for p in parts]) for j in range(len(self.rdds))]
+
+    def join_compute(self, split):
+        """Partition `split` of the inner join of all parents: (k, [v_0, ..., v_{n-1}])."""
+        return self.outer_join_compute(split, (1 << len(self.rdds)) - 1)
+
+    def join_collect(self):
+        return self.outer_join_collect((1 << len(self.rdds)) - 1)
+
+
 class StrRdd(Rdd):
     """Rdd<String>: count_by_value and distinct; the other shuffle ops raise TypeError before any device work."""
 
