@@ -411,8 +411,9 @@ VB_API int32_t vb_join_n_outer(vb_shuf *const *sides, uint32_t n_sides, uint32_t
  * Re-submitting a map_id overwrites it: a key only the replaced submission had is not in the output.
  * Limits: fewer than 2^32 - 2 rows per map partition and per shuffle, fewer than 2^31 distinct keys, every key shorter
  * than 2^32 bytes (VB_ERR_TOO_LARGE beyond them).  Key offsets that decrease or exceed n_bytes are VB_ERR_INVALID,
- * for device input too (checked on the device).  One process only: vb_shuffle_set_dist with world > 1, export /
- * import / exchange and the blob calls return VB_ERR_UNSUPPORTED; vb_shuffle_set_key_width, the integer map and
+ * for device input too (checked on the device).  Several ranks: vb_shuffle_create_str_dist and the string export /
+ * import calls below (vb_shuffle_set_dist with world > 1, the integer export / import / P2P calls and the blob calls
+ * return VB_ERR_UNSUPPORTED on a string shuffle); vb_shuffle_set_key_width, the integer map and
  * reduce calls and the join / cogroup calls return VB_ERR_INVALID on a string shuffle (vb_cogroup_n_str / vb_join_n_str
  * below join and cogroup string GROUP shuffles), and the string calls return
  * VB_ERR_INVALID on any other shuffle.  seal / is_sealed / stats / kernel_time / set_hint / free work as for any
@@ -466,6 +467,46 @@ VB_API int32_t vb_join_n_str(vb_shuf *const *sides, uint32_t n_sides, uint32_t r
                              uint64_t *out_key_offsets /*n_keys+1*/, void *out_key_bytes,
                              uint64_t *out_row_offsets /*n_keys+1*/, void *const *out_vals /*[n_sides] of n_rows*/,
                              uint8_t *const *out_valid /*[n_sides] or NULL; entries may be NULL*/, int32_t dst_loc);
+/* String keys across ranks (one process per GPU; ShuffleFetcher::fetch over `String` keys, shuffle_fetcher.rs:16-119).
+ * vb_shuffle_create_str_dist is vb_shuffle_create_str for rank `rank` of `world` (1 <= world <= 256, VB_ERR_INVALID
+ * otherwise); world == 1 gives the same shuffle as vb_shuffle_create_str.  Placement is unchanged: partition
+ * vb_hash_str(key) % n_reduce, owned by rank r % world.  Each rank runs its map tasks (vb_shuffle_map_str, any src_loc,
+ * resubmission allowed), then:
+ *   vb_shuffle_export_str_prepare  finishes the local map side and packs it by destination rank; n_keys / n_key_bytes /
+ *                                  n_vals [world] get what goes to each rank.  Reduce ops send combined rows: one
+ *                                  accumulator per distinct live key (n_vals == n_keys); GROUP sends raw values.
+ *   vb_shuffle_export_str_buffers  the four device columns, destination-major, owned by the library until seal (NULL
+ *                                  output pointers are skipped).  This is the wire format:
+ *                                    key_lens   u32 [keys]    each key's length in bytes
+ *                                    key_bytes  u8  [bytes]   the keys' bytes, concatenated in key order
+ *                                    val_counts u32 [keys]    GROUP: each key's value count (NULL for reduce ops)
+ *                                    vals       u64 [vals]    reduce ops: one accumulator per key (the op's result for
+ *                                                             the rank's rows; COUNT: a partial count); GROUP: the
+ *                                                             values key by key, each key's run in map order
+ *                                  Lengths and counts rather than offsets: slices concatenate without rebasing.
+ *   vb_shuffle_import_str          the received columns, source-rank major (concatenated in ascending source rank), with
+ *                                  the counts each source sent; borrowed until vb_shuffle_seal returns.  Then seal.
+ * The seal merges the received accumulators with merge_combiners (partial COUNTs summed, MIN / MAX / SUM by their
+ * vb_agg rules), so every owner's partitions equal those of the one-process shuffle over the same map tasks, whatever
+ * `world` is (f64 SUM up to summation order).  GROUP value lists are in source-rank order, which is map-id order when
+ * rank r's map ids precede rank r + 1's (vega_b200/dist.py map_block).  Partitions a rank does not own are empty on it;
+ * a sealed GROUP shuffle is a side of vb_cogroup_n_str / vb_join_n_str for the partitions the calling rank owns.
+ * vb_shuffle_exchange(s, VB_XCHG_AUTO or VB_XCHG_NCCL) does all of it on the library's stream: export, one all-gather of
+ * 3 x world counts per rank, one grouped send/recv of the four columns; VB_XCHG_P2P is VB_ERR_UNSUPPORTED.
+ * Errors: the export / import calls on a string shuffle of world 1: VB_ERR_STATE (VB_ERR_INVALID on a non-string
+ * shuffle); import before export, twice, or after seal: VB_ERR_STATE; map after export: VB_ERR_STATE; a NULL column
+ * whose count is non-zero, or reduce-op counts with n_vals != n_keys: VB_ERR_INVALID; an import of 2^32 - 2 rows or
+ * more (keys for reduce ops, values for GROUP) or of 2^31 keys or more: VB_ERR_TOO_LARGE, from the counts; key lengths
+ * or value counts that do not add up to the announced totals: VB_ERR_INVALID from the seal.                         */
+VB_API int32_t vb_shuffle_create_str_dist(vb_ctx *ctx, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce,
+                                          int32_t val_dtype, int32_t agg, uint32_t rank, uint32_t world, vb_shuf **out);
+VB_API int32_t vb_shuffle_export_str_prepare(vb_shuf *s, uint64_t *n_keys /*[world]*/, uint64_t *n_key_bytes /*[world]*/,
+                                             uint64_t *n_vals /*[world]*/);
+VB_API int32_t vb_shuffle_export_str_buffers(vb_shuf *s, uint32_t **key_lens, void **key_bytes, uint32_t **val_counts,
+                                             uint64_t **vals);
+VB_API int32_t vb_shuffle_import_str(vb_shuf *s, const uint32_t *key_lens, const void *key_bytes, const uint32_t *val_counts,
+                                     const uint64_t *vals, const uint64_t *n_keys /*[world]*/,
+                                     const uint64_t *n_key_bytes /*[world]*/, const uint64_t *n_vals /*[world]*/);
 /* MetroHash64_1(bytes ‖ 0xFF, seed 0): the reference's hash of a `String` / `&str` key */
 VB_API uint64_t vb_hash_str(const void *bytes, uint64_t len);
 VB_API uint32_t vb_get_partition_str(const void *bytes, uint64_t len, uint32_t n_reduce);

@@ -117,6 +117,15 @@ extern "C" {
     pub fn vb_join_n_str(sides: *const *mut vb_shuf, n_sides: u32, reduce_id: u32, required: u32, out_key_offsets: *mut u64,
                          out_key_bytes: *mut c_void, out_row_offsets: *mut u64, out_vals: *const *mut c_void,
                          out_valid: *const *mut u8, dst_loc: i32) -> i32;
+    // String keys across ranks: export packs by destination rank as four columns (u32 key lengths, key bytes, u32 value
+    // counts for GROUP, u64 values), import takes them source-rank major (borrowed until seal)
+    pub fn vb_shuffle_create_str_dist(ctx: *mut vb_ctx, shuffle_id: u64, n_map: u32, n_reduce: u32, val_dtype: i32, agg: i32,
+                                      rank: u32, world: u32, out: *mut *mut vb_shuf) -> i32;
+    pub fn vb_shuffle_export_str_prepare(s: *mut vb_shuf, n_keys: *mut u64, n_key_bytes: *mut u64, n_vals: *mut u64) -> i32;
+    pub fn vb_shuffle_export_str_buffers(s: *mut vb_shuf, key_lens: *mut *mut u32, key_bytes: *mut *mut c_void,
+                                         val_counts: *mut *mut u32, vals: *mut *mut u64) -> i32;
+    pub fn vb_shuffle_import_str(s: *mut vb_shuf, key_lens: *const u32, key_bytes: *const c_void, val_counts: *const u32,
+                                 vals: *const u64, n_keys: *const u64, n_key_bytes: *const u64, n_vals: *const u64) -> i32;
     pub fn vb_hash_str(bytes: *const c_void, len: u64) -> u64;
     pub fn vb_get_partition_str(bytes: *const c_void, len: u64, n_reduce: u32) -> u32;
     pub fn vb_shuffle_free(s: *mut vb_shuf) -> i32;

@@ -383,6 +383,10 @@ struct vb_shuf {
 };
 
 static int seal_str(vb_shuf *s);
+static int seal_str_import(vb_shuf *s);
+static int export_str_locked(vb_shuf *s, u64 *n_keys, u64 *n_key_bytes, u64 *n_vals);
+static int str_import_limits(const vb_shuf *s, u64 nk, u64 nv);
+static int exchange_str_locked(vb_shuf *s);
 static void free_str(vb_shuf *s);
 
 static bool is_reduce_op(int agg) { return agg == VB_AGG_SUM || agg == VB_AGG_MIN || agg == VB_AGG_MAX || agg == VB_AGG_COUNT; }
@@ -1360,7 +1364,7 @@ extern "C" int32_t vb_shuffle_set_dist(vb_shuf *s, uint32_t rank, uint32_t world
 {
     if (!s || world < 1 || rank >= world || world > 256) return set_err(VB_ERR_INVALID, "bad rank/world");
     if (s->multi && world > 1) return reject_multi(s, "multi-rank use (the exchange moves one value column)");
-    if (s->str && world > 1) return reject_str(s, "multi-rank use");
+    if (s->str && (world > 1 || s->world > 1)) return reject_str(s, "multi-rank use through vb_shuffle_set_dist (vb_shuffle_create_str_dist is)");
     s->rank = rank;
     s->world = world;
     return VB_OK;
@@ -2218,14 +2222,17 @@ static int nccl_load()
 struct Comm {
     ncclComm_t comm = nullptr;
     u32 rank = 0, world = 1;
-    u64 *d_send = nullptr;     // [world + 2]: counts to every destination, arena bytes, arena generation
-    u64 *d_recv = nullptr;     // [world][world + 2]
+    u64 *d_send = nullptr;     // [comm_row(world)]: counts to every destination, arena bytes, arena generation (or a
+                               // string shuffle's key, key byte and value counts to every destination)
+    u64 *d_recv = nullptr;     // [world][comm_row(world)]
     unsigned char *d_hs = nullptr, *d_hr = nullptr;   // IPC handle + generation: 80 bytes, [world] x 80
     std::vector<u64> peer_arena_bytes, peer_gen_seen;
     bool handles_valid = false;
 };
 constexpr u32 COMM_MAX_WORLD = 64;
 constexpr size_t COMM_HOST_OFF = 256 << 10;   // staging region inside vb_ctx::h_scratch
+// u64 per rank of the count scratch: world + 2 for the integer exchanges, 3 * world for string keys
+static size_t comm_row(u32 world) { return std::max<size_t>((size_t)world + 2, 3 * (size_t)world); }
 
 static void comm_teardown(vb_ctx *c)
 {
@@ -2269,11 +2276,11 @@ extern "C" int32_t vb_ctx_comm_init(vb_ctx *c, const void *unique_id, uint32_t r
     ncclResult_t r = g_nccl.CommInitRank(&m->comm, (int)world, id, (int)rank);
     if (r != ncclSuccess) { delete m; return set_err(VB_ERR_CUDA, "ncclCommInitRank: %s", g_nccl.GetErrorString(r)); }
     c->comm = m;
-    CU(cudaMalloc((void **)&m->d_send, (world + 2) * 8));
-    CU(cudaMalloc((void **)&m->d_recv, (size_t)world * (world + 2) * 8));
+    CU(cudaMalloc((void **)&m->d_send, comm_row(world) * 8));
+    CU(cudaMalloc((void **)&m->d_recv, (size_t)world * comm_row(world) * 8));
     CU(cudaMalloc((void **)&m->d_hs, 80));
     CU(cudaMalloc((void **)&m->d_hr, (size_t)world * 80));
-    CU(cudaMemset(m->d_send, 0, (world + 2) * 8));
+    CU(cudaMemset(m->d_send, 0, comm_row(world) * 8));
     m->peer_arena_bytes.assign(world, 0);
     m->peer_gen_seen.assign(world, 0);
     return VB_OK;
@@ -2614,12 +2621,18 @@ extern "C" int32_t vb_shuffle_exchange(vb_shuf *s, int32_t mode)
 {
     if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
     if (s->multi) return reject_multi(s, "multi-rank exchange");
-    if (s->str) return reject_str(s, "multi-rank exchange");
+    if (s->str && s->world < 2) return reject_str(s, "an exchange of a one-process shuffle (vb_shuffle_create_str_dist has world > 1)");
+    if (s->str && mode == VB_XCHG_P2P) return reject_str(s, "the fused P2P exchange (VB_XCHG_NCCL is supported)");
     vb_ctx *c = s->ctx;
     if (s->world < 2) return set_err(VB_ERR_STATE, "vb_shuffle_exchange needs vb_shuffle_set_dist(world > 1)");
     if (!c->comm) return set_err(VB_ERR_STATE, "vb_shuffle_exchange needs vb_ctx_comm_init");
     if (c->comm->world != s->world || c->comm->rank != s->rank) return set_err(VB_ERR_INVALID, "shuffle rank/world differ from the communicator's");
     if (mode < VB_XCHG_AUTO || mode > VB_XCHG_P2P) return set_err(VB_ERR_INVALID, "bad exchange mode");
+    if (s->str) {
+        std::lock_guard<std::mutex> lk(c->mu);
+        CU(cudaSetDevice(c->device));
+        return exchange_str_locked(s);
+    }
     if (mode == VB_XCHG_AUTO) mode = is_group_op(s->agg) ? VB_XCHG_P2P : VB_XCHG_NCCL;
     if (mode == VB_XCHG_P2P && !is_group_op(s->agg)) return set_err(VB_ERR_UNSUPPORTED, "the fused P2P exchange is for GROUP/COGROUP shuffles");
     std::lock_guard<std::mutex> lk(c->mu);
@@ -2924,7 +2937,9 @@ extern "C" int32_t vb_shuffle_seal(vb_shuf *s)
                 }
             } else {
                 if (!s->exported || !s->imported) return set_err(VB_ERR_STATE, "world > 1: seal needs export_prepare + import");
-                if (is_reduce_op(s->agg)) {
+                if (s->str) {
+                    TRY(seal_str_import(s));
+                } else if (is_reduce_op(s->agg)) {
                     void *tab = nullptr; u32 log_cap = 0; u64 n_ins = 0;
                     if (s->imp_n) {
                         std::vector<AggInput> in(1);
@@ -4008,6 +4023,16 @@ struct StrState {
     u64 *ix_fp = nullptr;                 // [1 << ix_log_cap] fingerprints, 0 = empty
     u32 *ix_id = nullptr;                 // [1 << ix_log_cap] dense key id of each slot
     u32 ix_log_cap = 0;
+    // across ranks (vb_shuffle_create_str_dist): the exported columns, destination-major, owned until seal ...
+    u32 *x_lens = nullptr, *x_cnts = nullptr;
+    unsigned char *x_bytes = nullptr;
+    u64 *x_vals = nullptr;
+    // ... and the imported ones, source-rank major: borrowed until seal, or received by vb_shuffle_exchange (i_own)
+    const u32 *i_lens = nullptr, *i_cnts = nullptr;
+    const unsigned char *i_bytes = nullptr;
+    const u64 *i_vals = nullptr;
+    u64 i_nk = 0, i_nkb = 0, i_nv = 0;
+    void *i_own[4] = {};
 };
 
 constexpr u32 STR_MAX_LOG_CAP = 33;       // index slots: < 2^31 distinct keys at load <= 0.6
@@ -4047,12 +4072,24 @@ static void free_str_dict(vb_shuf *s)
     t->cap_e = t->cap_a = 0;
 }
 
+static void free_str_xchg(vb_shuf *s)
+{
+    StrState *t = s->str;
+    vb_ctx *c = s->ctx;
+    dev_free(c, t->x_lens); dev_free(c, t->x_cnts); dev_free(c, t->x_bytes); dev_free(c, t->x_vals);
+    t->x_lens = t->x_cnts = nullptr; t->x_bytes = nullptr; t->x_vals = nullptr;
+    for (void *&p : t->i_own) { dev_free(c, p); p = nullptr; }
+    t->i_lens = t->i_cnts = nullptr; t->i_bytes = nullptr; t->i_vals = nullptr;
+    t->i_nk = t->i_nkb = t->i_nv = 0;
+}
+
 static void free_str(vb_shuf *s)
 {
     StrState *t = s->str;
     if (!t) return;
     for (u32 m = 0; m < s->n_map; ++m) free_str_map(s, m);
     free_str_dict(s);
+    free_str_xchg(s);
     dev_free(s->ctx, t->key_off);
     dev_free(s->ctx, t->key_bytes);
     dev_free(s->ctx, t->res_hash);
@@ -4190,6 +4227,42 @@ static int str_check_offsets(vb_shuf *s, const u64 *offs, u64 n, u64 n_bytes, in
     return VB_OK;
 }
 
+// Entry ids of n keys (key i is bytes[offs[i] - first .. offs[i + 1] - first), n_bytes in all) in the shuffle's
+// dictionary, creating the entries of new keys.  A missing index is first sized from (guess, hint); when it fills,
+// it grows and the whole call reruns.
+static int str_encode(vb_shuf *s, const u64 *offs, const unsigned char *bytes, u64 first, u64 n, u64 n_bytes, u64 guess, u64 hint,
+                      u32 *ids)
+{
+    StrState *t = s->str;
+    vb_ctx *c = s->ctx;
+    TRY(str_reserve(s, (u64)t->n_e + n, t->n_a + n_bytes));
+    if (!t->ctl) {
+        DevBuf ctl(c);
+        TRY(ctl.alloc(sizeof(StrCtl)));
+        CU(cudaMemsetAsync(ctl.p, 0, sizeof(StrCtl), c->stream));
+        t->ctl = (StrCtl *)ctl.release();
+    }
+    if (!t->d.fp) TRY(str_index_build(s, choose_log_cap(guess, hint, false, STR_MAX_LOG_CAP, c->l2_bytes, 12)));
+    for (;;) {
+        const u64 cap = 1ull << t->d.log_cap;
+        const u32 max_entries = (u32)std::min<u64>((cap / 10) * 6, 0xFFFFFFFFull);
+        CU(cudaMemsetAsync(&t->ctl->abort, 0, 4, c->stream));
+        {
+            KLaunch kl(s, K_DICT, n);
+            const u64 blocks = std::min<u64>((n + 255) / 256, (u64)c->sm_count * 8);
+            str_encode_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(offs, bytes, first, n, t->d, t->ctl, max_entries, ids);
+            TRY(kl.done("str_encode_kernel"));
+        }
+        StrCtl h;
+        TRY(fetch_status_unlocked(c, t->ctl, &h, sizeof(StrCtl)));
+        t->n_e = h.n_entries;
+        t->n_a = h.n_arena;
+        if (!h.abort) return VB_OK;
+        s->st.table_restarts++;                // grow the index (at least 4x) and rerun the whole call
+        TRY(str_index_build(s, std::max<u32>(t->d.log_cap + 2, ceil_log2_u64(3 * (u64)t->n_e))));
+    }
+}
+
 extern "C" int32_t vb_shuffle_map_str(vb_shuf *s, uint32_t map_id, const uint64_t *key_offsets, const void *key_bytes, uint64_t n_bytes,
                                       const void *vals, uint64_t n, int32_t loc)
 {
@@ -4204,6 +4277,7 @@ extern "C" int32_t vb_shuffle_map_str(vb_shuf *s, uint32_t map_id, const uint64_
     {
         std::lock_guard<std::mutex> g(s->mu);
         if (s->sealed || s->sealing || s->freed) return set_err(VB_ERR_STATE, "shuffle %llu: map after seal", (unsigned long long)s->id);
+        if (s->exported) return set_err(VB_ERR_STATE, "shuffle %llu: map after export", (unsigned long long)s->id);
     }
     vb_ctx *c = s->ctx;
     std::lock_guard<std::mutex> lk(c->mu);
@@ -4232,36 +4306,8 @@ extern "C" int32_t vb_shuffle_map_str(vb_shuf *s, uint32_t map_id, const uint64_
         } else {
             bytes = bytes ? bytes + first : nullptr;
         }
-        TRY(str_reserve(s, (u64)t->n_e + n, t->n_a + (last - first)));
-        if (!t->ctl) {
-            DevBuf ctl(c);
-            TRY(ctl.alloc(sizeof(StrCtl)));
-            CU(cudaMemsetAsync(ctl.p, 0, sizeof(StrCtl), c->stream));
-            t->ctl = (StrCtl *)ctl.release();
-        }
-        if (!t->d.fp) {
-            const u64 guess = n * std::max<u32>(1, s->n_map);
-            TRY(str_index_build(s, choose_log_cap(guess, s->hint, false, STR_MAX_LOG_CAP, c->l2_bytes, 12)));
-        }
         TRY(ids.alloc(n * 4));
-        for (;;) {
-            const u64 cap = 1ull << t->d.log_cap;
-            const u32 max_entries = (u32)std::min<u64>((cap / 10) * 6, 0xFFFFFFFFull);
-            CU(cudaMemsetAsync(&t->ctl->abort, 0, 4, c->stream));
-            {
-                KLaunch kl(s, K_DICT, n);
-                const u64 blocks = std::min<u64>((n + 255) / 256, (u64)c->sm_count * 8);
-                str_encode_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(offs, bytes, first, n, t->d, t->ctl, max_entries, ids.as<u32>());
-                TRY(kl.done("str_encode_kernel"));
-            }
-            StrCtl h;
-            TRY(fetch_status_unlocked(c, t->ctl, &h, sizeof(StrCtl)));
-            t->n_e = h.n_entries;
-            t->n_a = h.n_arena;
-            if (!h.abort) break;
-            s->st.table_restarts++;                // grow the index (at least 4x) and rerun the whole call
-            TRY(str_index_build(s, std::max<u32>(t->d.log_cap + 2, ceil_log2_u64(3 * (u64)t->n_e))));
-        }
+        TRY(str_encode(s, offs, bytes, first, n, last - first, n * std::max<u32>(1, s->n_map), s->hint, ids.as<u32>()));
         if (s->agg != VB_AGG_COUNT && loc != VB_DEVICE_BORROWED) {
             TRY(d_vals.alloc(n * 8));
             CU(cudaMemcpyAsync(d_vals.p, vals, n * 8, loc == VB_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, c->stream));
@@ -4298,10 +4344,9 @@ static int launch_str_reduce(vb_shuf *s, const u32 *ids, const u64 *vals, u64 n,
     return kl.done("str_reduce_kernel");
 }
 
-static int str_reduce_rows(vb_shuf *s, const u32 *ids, const u64 *vals, u64 n, const u32 *dense, u64 *acc)
+static int str_reduce_rows(vb_shuf *s, int opk, int tx, const u32 *ids, const u64 *vals, u64 n, const u32 *dense, u64 *acc)
 {
-    const int tx = val_tx(s);
-    switch (map_opk(s)) {
+    switch (opk) {
     case OPK_ADD_U64: return launch_str_reduce<OPK_ADD_U64, TX_NONE>(s, ids, vals, n, dense, acc);
     case OPK_ADD_F64: return launch_str_reduce<OPK_ADD_F64, TX_NONE>(s, ids, vals, n, dense, acc);
     case OPK_COUNT: return launch_str_reduce<OPK_COUNT, TX_NONE>(s, ids, vals, n, dense, acc);
@@ -4317,12 +4362,173 @@ static int str_reduce_rows(vb_shuf *s, const u32 *ids, const u64 *vals, u64 n, c
     return set_err(VB_ERR_UNSUPPORTED, "string keys: op %d", s->agg);
 }
 
-// Seal of a string-key shuffle (world == 1, every map present):
-//   1. mark the entries the rows of the present maps reference (a key only a replaced submission had is dropped);
+// Rows as dictionary entry ids and their values: one map task's, or the rows a rank imported.
+struct StrRun {
+    const u32 *ids;
+    const u64 *vals;
+    u64 n;
+};
+
+static std::vector<StrRun> str_map_runs(const vb_shuf *s)
+{
+    std::vector<StrRun> runs;
+    for (u32 m = 0; m < s->n_map; ++m)
+        if (s->maps[m].n_rows) runs.push_back(StrRun{s->str->ids[m], s->str->vals[m], s->maps[m].n_rows});
+    return runs;
+}
+
+static unsigned str_grid(const vb_ctx *c, u64 x) { return (unsigned)std::min<u64>((x + 255) / 256, (u64)c->sm_count * 8); }
+
+// out[i] = a[at[i]] for host positions at[] (one gather, one D2H)
+static int str_read_at(vb_shuf *s, const u64 *a, const std::vector<u64> &at, std::vector<u64> &out)
+{
+    vb_ctx *c = s->ctx;
+    const u32 n = (u32)at.size();
+    out.assign(n, 0);
+    DevBuf idx(c), o(c);
+    TRY(idx.alloc((size_t)n * 8));
+    TRY(o.alloc((size_t)n * 8));
+    CU(cudaMemcpyAsync(idx.p, at.data(), (size_t)n * 8, cudaMemcpyHostToDevice, c->stream));
+    {
+        KLaunch kl(s, K_MISC);
+        gather_u64_kernel<<<(n + 255) / 256, 256, 0, c->stream>>>(a, idx.as<u64>(), n, o.as<u64>());
+        TRY(kl.done("gather_u64_kernel"));
+    }
+    CU(cudaMemcpyAsync(out.data(), o.p, (size_t)n * 8, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    return VB_OK;
+}
+
+// Steps 1-2 of a string seal over `runs`: mark the entries the rows reference (a key only a replaced submission had is
+// dropped), split them by h % n_reduce into dense ids laid out partition by partition in the order `order` (a
+// permutation of [0, n_reduce)), and lay the keys' bytes out in that order.  cnt[r]: keys of partition r; base[r]: its
+// first dense id, base[n_reduce] = D; dense [entries]: each entry's dense id; koff [D + 1]: byte offsets from 0.
+static int str_dense_keys(vb_shuf *s, const std::vector<StrRun> &runs, const std::vector<u32> &order, std::vector<u64> &cnt,
+                          std::vector<u64> &base, DevBuf &dense, DevBuf &koff, DevBuf &kbytes)
+{
+    vb_ctx *c = s->ctx;
+    StrState *t = s->str;
+    const u32 R = s->n_reduce, ne = t->n_e;
+    DevBuf live(c), part(c), dcnt(c), cur(c), dbase(c), eod(c), klen(c);
+    TRY(live.alloc((u64)ne * 4));
+    CU(cudaMemsetAsync(live.p, 0, (u64)ne * 4, c->stream));
+    for (const StrRun &r : runs) {
+        KLaunch kl(s, K_MISC, r.n);
+        str_mark_live_kernel<<<str_grid(c, r.n), 256, 0, c->stream>>>(r.ids, r.n, live.as<u32>());
+        TRY(kl.done("str_mark_live_kernel"));
+    }
+    TRY(part.alloc((u64)ne * 4));
+    TRY(dcnt.alloc((u64)R * 4));
+    TRY(cur.alloc((u64)R * 4));
+    CU(cudaMemsetAsync(dcnt.p, 0, (u64)R * 4, c->stream));
+    CU(cudaMemsetAsync(cur.p, 0, (u64)R * 4, c->stream));
+    {
+        KLaunch kl(s, K_MISC, ne);
+        str_part_count_kernel<<<(ne + 255) / 256, 256, 0, c->stream>>>(t->d.e_hash, live.as<u32>(), ne, make_fastmod(R), part.as<u32>(), dcnt.as<u32>());
+        TRY(kl.done("str_part_count_kernel"));
+    }
+    std::vector<u32> hc(R);
+    CU(cudaMemcpyAsync(hc.data(), dcnt.p, (size_t)R * 4, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    cnt.assign(R, 0);
+    base.assign((size_t)R + 1, 0);
+    u64 D = 0;
+    for (u32 r : order) {
+        cnt[r] = hc[r];
+        base[r] = D;
+        D += hc[r];
+    }
+    base[R] = D;
+    if (D >= (1ull << 31)) return set_err(VB_ERR_TOO_LARGE, "%llu distinct string keys (fewer than 2^31 are supported)", (unsigned long long)D);
+    TRY(dbase.alloc(((u64)R + 1) * 8));
+    CU(cudaMemcpyAsync(dbase.p, base.data(), ((size_t)R + 1) * 8, cudaMemcpyHostToDevice, c->stream));
+    TRY(dense.alloc((u64)ne * 4));
+    TRY(eod.alloc(D * 4));
+    TRY(klen.alloc(D * 8));
+    TRY(koff.alloc((D + 1) * 8));
+    {
+        KLaunch kl(s, K_MISC, ne);
+        str_dense_kernel<<<(ne + 255) / 256, 256, 0, c->stream>>>(live.as<u32>(), part.as<u32>(), ne, dbase.as<u64>(), cur.as<u32>(), t->d.e_len,
+                                                                  dense.as<u32>(), eod.as<u32>(), klen.as<u64>());
+        TRY(kl.done("str_dense_kernel"));
+    }
+    TRY(exclusive_scan_u64(s, klen.as<u64>(), koff.as<u64>(), D, koff.as<u64>() + D));
+    u64 nb = 0;
+    CU(cudaMemcpyAsync(c->h_scratch, koff.as<u64>() + D, 8, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    if (D) nb = *(u64 *)c->h_scratch;
+    TRY(kbytes.alloc(nb));
+    {
+        KLaunch kl(s, K_MISC, D);
+        str_gather_bytes_kernel<<<(unsigned)((D * 32 + 255) / 256), 256, 0, c->stream>>>(eod.as<u32>(), (u32)D, t->d.e_off, koff.as<u64>(), t->d.arena,
+                                                                                        kbytes.as<unsigned char>());
+        TRY(kl.done("str_gather_bytes_kernel"));
+    }
+    return VB_OK;
+}
+
+// Reduce ops: acc [D] = op `opk` (values entering in order `tx`) folded over every row of `runs`, by dense id.
+static int str_fold_values(vb_shuf *s, const std::vector<StrRun> &runs, int opk, int tx, const u32 *dense, u64 D, DevBuf &acc)
+{
+    vb_ctx *c = s->ctx;
+    TRY(acc.alloc(D * 8));
+    {
+        KLaunch kl(s, K_MISC);
+        str_fill_kernel<<<str_grid(c, D), 256, 0, c->stream>>>(acc.as<u64>(), D, op_identity(opk));
+        TRY(kl.done("str_fill_kernel"));
+    }
+    for (const StrRun &r : runs) TRY(str_reduce_rows(s, opk, tx, r.ids, r.vals, r.n, dense, acc.as<u64>()));
+    if (tx != TX_NONE) {
+        KLaunch kl(s, K_MISC);
+        tx_inv_kernel<<<(unsigned)((D + 255) / 256), 256, 0, c->stream>>>(acc.as<u64>(), D, tx);
+        TRY(kl.done("tx_inv_kernel"));
+    }
+    return VB_OK;
+}
+
+// GROUP: the n rows of `runs`, concatenated in run order and stably sorted by dense id (seal_group's steps 4-7):
+// offs [D + 1] (the CSR) and vals [n].
+static int str_group_values(vb_shuf *s, const std::vector<StrRun> &runs, u64 n, const u32 *dense, u64 D, DevBuf &offs, DevBuf &vals)
+{
+    vb_ctx *c = s->ctx;
+    DevBuf cids(c), cvals(c);
+    TRY(cids.alloc(n * 4));
+    TRY(cvals.alloc(n * 8));
+    u64 at = 0;
+    for (const StrRun &r : runs) {
+        CU(cudaMemcpyAsync(cids.as<u32>() + at, r.ids, r.n * 4, cudaMemcpyDeviceToDevice, c->stream));
+        CU(cudaMemcpyAsync(cvals.as<u64>() + at, r.vals, r.n * 8, cudaMemcpyDeviceToDevice, c->stream));
+        at += r.n;
+    }
+    TRY(offs.alloc((D + 1) * 8));
+    CU(cudaMemsetAsync(offs.p, 0xFF, (D + 1) * 8, c->stream));
+    u32 *sorted_ids = nullptr;
+    u64 *sorted_vals = nullptr;
+    bool csr_done = false;
+    TRY(sort_id_pairs(s, cids.as<u32>(), Loader{LD_KEY32_VAL_SOA, nullptr, cvals.as<u64>(), 0}, n, ceil_log2_u64(std::max<u64>(D, 2)), &sorted_ids,
+                      &sorted_vals, dense, offs.as<u64>(), &csr_done));
+    DevBuf sid_guard(c);
+    if (sorted_ids != cids.as<u32>()) sid_guard.p = sorted_ids;
+    vals.reset();
+    vals.p = sorted_vals;
+    if (csr_done) {
+        CU(cudaMemcpyAsync(offs.as<u64>() + D, &n, 8, cudaMemcpyHostToDevice, c->stream));
+    } else {
+        KLaunch kl(s, K_MISC);
+        csr_bounds_kernel<<<str_grid(c, n), 256, 0, c->stream>>>(sorted_ids, n, offs.as<u64>(), D);
+        TRY(kl.done("csr_bounds_kernel"));
+    }
+    return VB_OK;
+}
+
+// The reduce side of a string-key shuffle over `runs` (reduce ops fold with `opk`: the map op, or the merge op over
+// imported accumulators):
+//   1. mark the entries the rows reference;
 //   2. split the live entries by h % n_reduce into partition-major dense ids, and lay their bytes out in that order;
-//   3. reduce ops: one RED per (warp, distinct id) into acc[dense id];  GROUP: the maps' (id, value) rows in map-id
-//      order, stably sorted by dense id, then the CSR (seal_group's steps 4-7).
-static int seal_str(vb_shuf *s)
+//   3. reduce ops: one RED per (warp, distinct id) into acc[dense id];  GROUP: the rows in run order (map-id order, or
+//      source-rank major), stably sorted by dense id, then the CSR (seal_group's steps 4-7).
+// The per-map ids and the dictionary are freed at the end.
+static int seal_str_runs(vb_shuf *s, const std::vector<StrRun> &runs, int opk)
 {
     vb_ctx *c = s->ctx;
     StrState *t = s->str;
@@ -4331,126 +4537,27 @@ static int seal_str(vb_shuf *s)
     s->val_off.assign((size_t)R + 1, 0);
     t->kb_off.assign((size_t)R + 1, 0);
     u64 n = 0;
-    for (auto &m : s->maps) if (m.present) n += m.n_rows;
-    const u32 ne = t->n_e;
-    auto grid = [&](u64 x) { return (unsigned)std::min<u64>((x + 255) / 256, (u64)c->sm_count * 8); };
-    if (n && ne) {
-        // 1. live entries
-        DevBuf live(c), part(c), cnt(c), cur(c), dbase(c), dense(c), eod(c), klen(c), koff(c), kbytes(c);
-        TRY(live.alloc((u64)ne * 4));
-        CU(cudaMemsetAsync(live.p, 0, (u64)ne * 4, c->stream));
-        for (u32 m = 0; m < s->n_map; ++m) {
-            if (!s->maps[m].n_rows) continue;
-            KLaunch kl(s, K_MISC, s->maps[m].n_rows);
-            str_mark_live_kernel<<<grid(s->maps[m].n_rows), 256, 0, c->stream>>>(t->ids[m], s->maps[m].n_rows, live.as<u32>());
-            TRY(kl.done("str_mark_live_kernel"));
-        }
-        // 2. partitions, dense ids, key bytes
-        TRY(part.alloc((u64)ne * 4));
-        TRY(cnt.alloc((u64)R * 4));
-        TRY(cur.alloc((u64)R * 4));
-        CU(cudaMemsetAsync(cnt.p, 0, (u64)R * 4, c->stream));
-        CU(cudaMemsetAsync(cur.p, 0, (u64)R * 4, c->stream));
-        {
-            KLaunch kl(s, K_MISC, ne);
-            str_part_count_kernel<<<(ne + 255) / 256, 256, 0, c->stream>>>(t->d.e_hash, live.as<u32>(), ne, make_fastmod(R), part.as<u32>(), cnt.as<u32>());
-            TRY(kl.done("str_part_count_kernel"));
-        }
-        std::vector<u32> hc(R);
-        CU(cudaMemcpyAsync(hc.data(), cnt.p, (size_t)R * 4, cudaMemcpyDeviceToHost, c->stream));
-        CU(cudaStreamSynchronize(c->stream));
-        for (u32 r = 0; r < R; ++r) s->bucket_off[r + 1] = s->bucket_off[r] + hc[r];
+    for (const StrRun &r : runs) n += r.n;
+    if (n && t->n_e) {
+        std::vector<u32> order(R);
+        for (u32 r = 0; r < R; ++r) order[r] = r;
+        std::vector<u64> cnt;
+        DevBuf dense(c), koff(c), kbytes(c);
+        TRY(str_dense_keys(s, runs, order, cnt, s->bucket_off, dense, koff, kbytes));
         const u64 D = s->bucket_off[R];
-        if (D >= (1ull << 31)) return set_err(VB_ERR_TOO_LARGE, "%llu distinct string keys (fewer than 2^31 are supported)", (unsigned long long)D);
-        TRY(dbase.alloc(((u64)R + 1) * 8));
-        CU(cudaMemcpyAsync(dbase.p, s->bucket_off.data(), ((size_t)R + 1) * 8, cudaMemcpyHostToDevice, c->stream));
-        TRY(dense.alloc((u64)ne * 4));
-        TRY(eod.alloc(D * 4));
-        TRY(klen.alloc(D * 8));
-        TRY(koff.alloc((D + 1) * 8));
-        {
-            KLaunch kl(s, K_MISC, ne);
-            str_dense_kernel<<<(ne + 255) / 256, 256, 0, c->stream>>>(live.as<u32>(), part.as<u32>(), ne, dbase.as<u64>(), cur.as<u32>(), t->d.e_len,
-                                                                      dense.as<u32>(), eod.as<u32>(), klen.as<u64>());
-            TRY(kl.done("str_dense_kernel"));
-        }
-        TRY(exclusive_scan_u64(s, klen.as<u64>(), koff.as<u64>(), D, koff.as<u64>() + D));
-        {
-            DevBuf out(c);
-            TRY(out.alloc(((size_t)R + 1) * 8));
-            KLaunch kl(s, K_MISC);
-            gather_u64_kernel<<<(R + 1 + 255) / 256, 256, 0, c->stream>>>(koff.as<u64>(), dbase.as<u64>(), R + 1, out.as<u64>());
-            TRY(kl.done("gather_u64_kernel"));
-            CU(cudaMemcpyAsync(t->kb_off.data(), out.p, ((size_t)R + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
-            CU(cudaStreamSynchronize(c->stream));
-        }
-        TRY(kbytes.alloc(t->kb_off[R]));
-        {
-            KLaunch kl(s, K_MISC, D);
-            str_gather_bytes_kernel<<<(unsigned)((D * 32 + 255) / 256), 256, 0, c->stream>>>(eod.as<u32>(), (u32)D, t->d.e_off, koff.as<u64>(), t->d.arena,
-                                                                                            kbytes.as<unsigned char>());
-            TRY(kl.done("str_gather_bytes_kernel"));
-        }
-        // 3. values
+        TRY(str_read_at(s, koff.as<u64>(), s->bucket_off, t->kb_off));
         if (is_reduce_op(s->agg)) {
             DevBuf acc(c);
-            TRY(acc.alloc(D * 8));
-            {
-                KLaunch kl(s, K_MISC);
-                str_fill_kernel<<<grid(D), 256, 0, c->stream>>>(acc.as<u64>(), D, op_identity(map_opk(s)));
-                TRY(kl.done("str_fill_kernel"));
-            }
-            for (u32 m = 0; m < s->n_map; ++m)
-                if (s->maps[m].n_rows) TRY(str_reduce_rows(s, t->ids[m], t->vals[m], s->maps[m].n_rows, dense.as<u32>(), acc.as<u64>()));
-            const int tx = val_tx(s);
-            if (tx != TX_NONE) {
-                KLaunch kl(s, K_MISC);
-                tx_inv_kernel<<<(unsigned)((D + 255) / 256), 256, 0, c->stream>>>(acc.as<u64>(), D, tx);
-                TRY(kl.done("tx_inv_kernel"));
-            }
+            TRY(str_fold_values(s, runs, opk, val_tx(s), dense.as<u32>(), D, acc));
             s->res_comb = (u64 *)acc.release();
             s->st.rows_out = D;
         } else {
-            DevBuf cids(c), cvals(c), offs(c);
-            TRY(cids.alloc(n * 4));
-            TRY(cvals.alloc(n * 8));
-            u64 at = 0;
-            for (u32 m = 0; m < s->n_map; ++m) {
-                const u64 k = s->maps[m].n_rows;
-                if (!k) continue;
-                CU(cudaMemcpyAsync(cids.as<u32>() + at, t->ids[m], k * 4, cudaMemcpyDeviceToDevice, c->stream));
-                CU(cudaMemcpyAsync(cvals.as<u64>() + at, t->vals[m], k * 8, cudaMemcpyDeviceToDevice, c->stream));
-                at += k;
-            }
-            TRY(offs.alloc((D + 1) * 8));
-            CU(cudaMemsetAsync(offs.p, 0xFF, (D + 1) * 8, c->stream));
-            u32 *sorted_ids = nullptr;
-            u64 *sorted_vals = nullptr;
-            bool csr_done = false;
-            TRY(sort_id_pairs(s, cids.as<u32>(), Loader{LD_KEY32_VAL_SOA, nullptr, cvals.as<u64>(), 0}, n, ceil_log2_u64(std::max<u64>(D, 2)), &sorted_ids,
-                              &sorted_vals, dense.as<u32>(), offs.as<u64>(), &csr_done));
-            DevBuf sid_guard(c), sval_guard(c);
-            if (sorted_ids != cids.as<u32>()) sid_guard.p = sorted_ids;
-            sval_guard.p = sorted_vals;
-            if (csr_done) {
-                CU(cudaMemcpyAsync(offs.as<u64>() + D, &n, 8, cudaMemcpyHostToDevice, c->stream));
-            } else {
-                KLaunch kl(s, K_MISC);
-                csr_bounds_kernel<<<grid(n), 256, 0, c->stream>>>(sorted_ids, n, offs.as<u64>(), D);
-                TRY(kl.done("csr_bounds_kernel"));
-            }
-            {
-                DevBuf out(c);
-                TRY(out.alloc(((size_t)R + 1) * 8));
-                KLaunch kl(s, K_MISC);
-                gather_u64_kernel<<<(R + 1 + 255) / 256, 256, 0, c->stream>>>(offs.as<u64>(), dbase.as<u64>(), R + 1, out.as<u64>());
-                TRY(kl.done("gather_u64_kernel"));
-                CU(cudaMemcpyAsync(s->val_off.data(), out.p, ((size_t)R + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
-                CU(cudaStreamSynchronize(c->stream));
-            }
+            DevBuf offs(c), vals(c);
+            TRY(str_group_values(s, runs, n, dense.as<u32>(), D, offs, vals));
+            TRY(str_read_at(s, offs.as<u64>(), s->bucket_off, s->val_off));
             s->n_vals = n;
             s->res_offs = (u64 *)offs.release();
-            s->res_vals = (u64 *)sval_guard.release();
+            s->res_vals = (u64 *)vals.release();
             s->st.rows_out = n;
         }
         s->n_keys = D;
@@ -4460,6 +4567,306 @@ static int seal_str(vb_shuf *s)
     }
     for (u32 m = 0; m < s->n_map; ++m) free_str_map(s, m);
     free_str_dict(s);
+    return VB_OK;
+}
+
+// Seal of a string-key shuffle (world == 1, every map present)
+static int seal_str(vb_shuf *s) { return seal_str_runs(s, str_map_runs(s), map_opk(s)); }
+
+// ---------------------------------------------------------------------------------------------
+// string keys across ranks (vb_shuffle_create_str_dist): the map side of each rank is exported as key columns, packed
+// by destination rank; the owner imports every rank's columns into a fresh dictionary and seals them as one run.
+// ---------------------------------------------------------------------------------------------
+// Export: steps 1-2 of the seal with the partitions laid out destination-major (rank 0's partitions, then rank 1's,
+// ...), so the dense ids come out grouped by destination; then the values of step 3, as one accumulator per key
+// (reduce ops) or each key's values in map order (GROUP).  The per-map ids and the dictionary are freed.  The caller
+// holds c->mu.
+static int export_str_locked(vb_shuf *s, u64 *n_keys, u64 *n_key_bytes, u64 *n_vals)
+{
+    vb_ctx *c = s->ctx;
+    StrState *t = s->str;
+    {
+        std::lock_guard<std::mutex> g(s->mu);
+        if (s->sealed || s->sealing || s->exported || s->freed) return set_err(VB_ERR_STATE, "export after seal/export");
+    }
+    const u32 W = s->world, R = s->n_reduce;
+    for (u32 d = 0; d < W; ++d) n_keys[d] = n_key_bytes[d] = n_vals[d] = 0;
+    const std::vector<StrRun> runs = str_map_runs(s);
+    u64 n = 0;
+    for (const StrRun &r : runs) n += r.n;
+    if (n && t->n_e) {
+        std::vector<u32> order;
+        for (u32 d = 0; d < W; ++d)
+            for (u32 r = d; r < R; r += W) order.push_back(r);
+        std::vector<u64> cnt, base;
+        DevBuf dense(c), koff(c), kbytes(c), lens(c);
+        TRY(str_dense_keys(s, runs, order, cnt, base, dense, koff, kbytes));
+        const u64 D = base[R];
+        std::vector<u64> cut((size_t)W + 1, 0), at;                  // first dense id of each destination
+        for (u32 d = 0; d < W; ++d) {
+            u64 k = 0;
+            for (u32 r = d; r < R; r += W) k += cnt[r];
+            cut[d + 1] = cut[d] + k;
+            n_keys[d] = k;
+        }
+        TRY(str_read_at(s, koff.as<u64>(), cut, at));
+        for (u32 d = 0; d < W; ++d) n_key_bytes[d] = at[d + 1] - at[d];
+        TRY(lens.alloc(D * 4));
+        {
+            KLaunch kl(s, K_MISC, D);
+            str_diff_u32_kernel<<<str_grid(c, D), 256, 0, c->stream>>>(koff.as<u64>(), D, lens.as<u32>());
+            TRY(kl.done("str_diff_u32_kernel"));
+        }
+        if (is_reduce_op(s->agg)) {
+            DevBuf acc(c);
+            TRY(str_fold_values(s, runs, map_opk(s), val_tx(s), dense.as<u32>(), D, acc));
+            for (u32 d = 0; d < W; ++d) n_vals[d] = n_keys[d];
+            t->x_vals = (u64 *)acc.release();
+        } else {
+            DevBuf offs(c), vals(c), cnts(c);
+            TRY(str_group_values(s, runs, n, dense.as<u32>(), D, offs, vals));
+            TRY(cnts.alloc(D * 4));
+            {
+                KLaunch kl(s, K_MISC, D);
+                str_diff_u32_kernel<<<str_grid(c, D), 256, 0, c->stream>>>(offs.as<u64>(), D, cnts.as<u32>());
+                TRY(kl.done("str_diff_u32_kernel"));
+            }
+            TRY(str_read_at(s, offs.as<u64>(), cut, at));
+            for (u32 d = 0; d < W; ++d) n_vals[d] = at[d + 1] - at[d];
+            t->x_cnts = (u32 *)cnts.release();
+            t->x_vals = (u64 *)vals.release();
+        }
+        t->x_lens = (u32 *)lens.release();
+        t->x_bytes = (unsigned char *)kbytes.release();
+        CU(cudaStreamSynchronize(c->stream));
+    }
+    for (u32 m = 0; m < s->n_map; ++m) free_str_map(s, m);
+    free_str_dict(s);
+    std::lock_guard<std::mutex> g(s->mu);
+    s->exported = true;
+    return VB_OK;
+}
+
+// The limits of one import, from its totals: rows (accumulators, or GROUP values) and received keys
+static int str_import_limits(const vb_shuf *s, u64 nk, u64 nv)
+{
+    const u64 rows = is_reduce_op(s->agg) ? nk : nv;
+    if (rows >= 0xFFFFFFFEull) return set_err(VB_ERR_TOO_LARGE, "import of %llu rows (fewer than 2^32 - 2 are supported)", (unsigned long long)rows);
+    if (nk >= (1ull << 31)) return set_err(VB_ERR_TOO_LARGE, "import of %llu keys (fewer than 2^31 are supported)", (unsigned long long)nk);
+    return VB_OK;
+}
+
+// Seal of an imported string shuffle: the received keys' byte offsets (widened lengths, one scan), a fresh dictionary
+// of them (str_encode_kernel; the received key count bounds the distinct keys), for GROUP each key's entry id over its
+// run of values, then seal_str_runs over the rows as one source-rank-major run: reduce ops merge the accumulators with
+// the merge op (COUNT: ADD_U64), GROUP keeps source-rank order, which is map-id order.
+static int seal_str_import(vb_shuf *s)
+{
+    vb_ctx *c = s->ctx;
+    StrState *t = s->str;
+    const u64 nk = t->i_nk, nkb = t->i_nkb, nv = t->i_nv;
+    const bool group = !is_reduce_op(s->agg);
+    std::vector<StrRun> runs;
+    DevBuf wide(c), koff(c), voff(c), ids(c), row_ids(c);
+    if (nk) {
+        TRY(wide.alloc(nk * 8));
+        TRY(koff.alloc((nk + 1) * 8));
+        {
+            KLaunch kl(s, K_MISC, nk);
+            str_widen_u32_kernel<<<str_grid(c, nk), 256, 0, c->stream>>>(t->i_lens, nk, wide.as<u64>());
+            TRY(kl.done("str_widen_u32_kernel"));
+        }
+        TRY(exclusive_scan_u64(s, wide.as<u64>(), koff.as<u64>(), nk, koff.as<u64>() + nk));
+        u64 *h = (u64 *)c->h_scratch;
+        CU(cudaMemcpyAsync(h, koff.as<u64>() + nk, 8, cudaMemcpyDeviceToHost, c->stream));
+        if (group) {
+            TRY(voff.alloc((nk + 1) * 8));
+            {
+                KLaunch kl(s, K_MISC, nk);
+                str_widen_u32_kernel<<<str_grid(c, nk), 256, 0, c->stream>>>(t->i_cnts, nk, wide.as<u64>());
+                TRY(kl.done("str_widen_u32_kernel"));
+            }
+            TRY(exclusive_scan_u64(s, wide.as<u64>(), voff.as<u64>(), nk, voff.as<u64>() + nk));
+            CU(cudaMemcpyAsync(h + 1, voff.as<u64>() + nk, 8, cudaMemcpyDeviceToHost, c->stream));
+        }
+        CU(cudaStreamSynchronize(c->stream));
+        if (h[0] != nkb) return set_err(VB_ERR_INVALID, "imported key lengths add up to %llu bytes, %llu announced", (unsigned long long)h[0], (unsigned long long)nkb);
+        if (group && h[1] != nv) return set_err(VB_ERR_INVALID, "imported value counts add up to %llu, %llu announced", (unsigned long long)h[1], (unsigned long long)nv);
+        t->n_e = 0;
+        t->n_a = 0;
+        TRY(ids.alloc(nk * 4));
+        TRY(str_encode(s, koff.as<u64>(), t->i_bytes, 0, nk, nkb, nk, nk, ids.as<u32>()));
+        if (group) {
+            if (nv) {
+                TRY(row_ids.alloc(nv * 4));
+                KLaunch kl(s, K_MISC, nv);
+                const int occ = occupancy(c, str_expand_ids_kernel, 256, 0);
+                const u64 blocks = std::min<u64>((nv + 255) / 256, (u64)c->sm_count * occ);
+                str_expand_ids_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(voff.as<u64>(), nk, ids.as<u32>(), nv, row_ids.as<u32>());
+                TRY(kl.done("str_expand_ids_kernel"));
+                runs.push_back(StrRun{row_ids.as<u32>(), t->i_vals, nv});
+            }
+        } else {
+            runs.push_back(StrRun{ids.as<u32>(), t->i_vals, nk});
+        }
+    }
+    TRY(seal_str_runs(s, runs, merge_opk(s)));
+    free_str_xchg(s);
+    return VB_OK;
+}
+
+extern "C" int32_t vb_shuffle_create_str_dist(vb_ctx *c, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce, int32_t vdt, int32_t agg,
+                                              uint32_t rank, uint32_t world, vb_shuf **out)
+{
+    if (!c || !out) return set_err(VB_ERR_INVALID, "vb_shuffle_create_str_dist: NULL argument");
+    *out = nullptr;
+    if (world < 1 || world > 256 || rank >= world) return set_err(VB_ERR_INVALID, "bad rank %u / world %u (1 <= world <= 256)", rank, world);
+    TRY(vb_shuffle_create_str(c, shuffle_id, n_map, n_reduce, vdt, agg, out));
+    (*out)->rank = rank;
+    (*out)->world = world;
+    return VB_OK;
+}
+
+// the checks every string export / import call makes first
+static int str_dist_check(const vb_shuf *s, const char *what)
+{
+    if (!s->str) return set_err(VB_ERR_INVALID, "%s needs a shuffle from vb_shuffle_create_str_dist", what);
+    if (s->world < 2) return set_err(VB_ERR_STATE, "%s needs a string shuffle of world > 1 (vb_shuffle_create_str_dist)", what);
+    return VB_OK;
+}
+
+extern "C" int32_t vb_shuffle_export_str_prepare(vb_shuf *s, uint64_t *n_keys, uint64_t *n_key_bytes, uint64_t *n_vals)
+{
+    if (!s || !n_keys || !n_key_bytes || !n_vals) return set_err(VB_ERR_INVALID, "NULL argument");
+    TRY(str_dist_check(s, "vb_shuffle_export_str_prepare"));
+    vb_ctx *c = s->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    TRY(export_str_locked(s, n_keys, n_key_bytes, n_vals));
+    CU(cudaStreamSynchronize(c->stream));
+    return VB_OK;
+}
+
+extern "C" int32_t vb_shuffle_export_str_buffers(vb_shuf *s, uint32_t **key_lens, void **key_bytes, uint32_t **val_counts, uint64_t **vals)
+{
+    if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
+    TRY(str_dist_check(s, "vb_shuffle_export_str_buffers"));
+    {
+        std::lock_guard<std::mutex> g(s->mu);
+        if (!s->exported || s->sealed || s->freed) return set_err(VB_ERR_STATE, "vb_shuffle_export_str_buffers needs vb_shuffle_export_str_prepare first and no seal yet");
+    }
+    const StrState *t = s->str;
+    if (key_lens) *key_lens = t->x_lens;
+    if (key_bytes) *key_bytes = t->x_bytes;
+    if (val_counts) *val_counts = t->x_cnts;
+    if (vals) *vals = t->x_vals;
+    return VB_OK;
+}
+
+extern "C" int32_t vb_shuffle_import_str(vb_shuf *s, const uint32_t *key_lens, const void *key_bytes, const uint32_t *val_counts,
+                                         const uint64_t *vals, const uint64_t *n_keys, const uint64_t *n_key_bytes, const uint64_t *n_vals)
+{
+    if (!s || !n_keys || !n_key_bytes || !n_vals) return set_err(VB_ERR_INVALID, "NULL argument");
+    TRY(str_dist_check(s, "vb_shuffle_import_str"));
+    {
+        std::lock_guard<std::mutex> g(s->mu);
+        if (!s->exported || s->imported || s->sealed || s->sealing || s->freed)
+            return set_err(VB_ERR_STATE, "vb_shuffle_import_str needs vb_shuffle_export_str_prepare first, once, and no seal yet");
+    }
+    u64 nk = 0, nkb = 0, nv = 0;
+    for (u32 r = 0; r < s->world; ++r) { nk += n_keys[r]; nkb += n_key_bytes[r]; nv += n_vals[r]; }
+    const bool group = !is_reduce_op(s->agg);
+    if ((nk && !key_lens) || (nkb && !key_bytes) || (group && nk && !val_counts) || (nv && !vals))
+        return set_err(VB_ERR_INVALID, "NULL column with a non-zero count");
+    if (!group && nv != nk) return set_err(VB_ERR_INVALID, "reduce ops import one accumulator per key (%llu keys, %llu values)", (unsigned long long)nk, (unsigned long long)nv);
+    TRY(str_import_limits(s, nk, nv));
+    StrState *t = s->str;
+    t->i_lens = key_lens; t->i_bytes = (const unsigned char *)key_bytes; t->i_cnts = group ? val_counts : nullptr; t->i_vals = vals;
+    t->i_nk = nk; t->i_nkb = nkb; t->i_nv = nv;
+    std::lock_guard<std::mutex> g(s->mu);
+    s->imported = true;
+    return VB_OK;
+}
+
+// vb_shuffle_exchange of a string shuffle: export, then ONE all-gather of the world x 3 world count matrix (keys, key
+// bytes and values to every destination) and ONE grouped send/recv carrying the four columns of every peer, as
+// exchange_nccl_locked does for two.  The received columns are owned by the shuffle until seal.
+static int exchange_str_locked(vb_shuf *s)
+{
+    vb_ctx *c = s->ctx;
+    Comm *m = c->comm;
+    StrState *t = s->str;
+    const u32 W = m->world, me = m->rank;
+    const bool group = !is_reduce_op(s->agg);
+    std::vector<u64> cnt(3 * (size_t)W, 0);      // n_keys[W], n_key_bytes[W], n_vals[W]
+    auto ms_since = [](std::chrono::steady_clock::time_point t0) { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count(); };
+    auto t0 = std::chrono::steady_clock::now();
+    TRY(export_str_locked(s, cnt.data(), cnt.data() + W, cnt.data() + 2 * (size_t)W));
+    s->xst.prepare_wall_ms += ms_since(t0);
+    t0 = std::chrono::steady_clock::now();
+    const size_t row = 3 * (size_t)W;
+    u64 *h = (u64 *)((char *)c->h_scratch + COMM_HOST_OFF);
+    u64 *hs = h + (size_t)W * row;
+    memcpy(hs, cnt.data(), row * 8);
+    CU(cudaMemcpyAsync(m->d_send, hs, row * 8, cudaMemcpyHostToDevice, c->stream));
+    NC(g_nccl.AllGather(m->d_send, m->d_recv, row, ncclUint64, m->comm, c->stream));
+    CU(cudaMemcpyAsync(h, m->d_recv, (size_t)W * row * 8, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    s->xst.counts_wall_ms += ms_since(t0);
+    t0 = std::chrono::steady_clock::now();
+    // per peer p: what I send (cnt) and receive (column me of p's row), and where each run starts
+    std::vector<u64> rk(W), rb(W), rv(W), sk(W + 1, 0), sb(W + 1, 0), sv(W + 1, 0), ok(W + 1, 0), ob(W + 1, 0), ov(W + 1, 0);
+    for (u32 p = 0; p < W; ++p) {
+        rk[p] = h[p * row + me];
+        rb[p] = h[p * row + W + me];
+        rv[p] = h[p * row + 2 * (size_t)W + me];
+        sk[p + 1] = sk[p] + cnt[p];
+        sb[p + 1] = sb[p] + cnt[W + p];
+        sv[p + 1] = sv[p] + cnt[2 * (size_t)W + p];
+        ok[p + 1] = ok[p] + rk[p];
+        ob[p + 1] = ob[p] + rb[p];
+        ov[p + 1] = ov[p] + rv[p];
+    }
+    const u64 nk = ok[W], nkb = ob[W], nv = ov[W];
+    TRY(str_import_limits(s, nk, nv));
+    DevBuf lens(c), bytes(c), cnts(c), vals(c);
+    TRY(lens.alloc(nk * 4));
+    TRY(bytes.alloc(nkb));
+    if (group) TRY(cnts.alloc(nk * 4));
+    TRY(vals.alloc(nv * 8));
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    if (c->profile) { cudaEventCreate(&e0); cudaEventCreate(&e1); cudaEventRecord(e0, c->stream); }
+    NC(g_nccl.GroupStart());
+    for (u32 p = 0; p < W; ++p) {
+        const u64 k = cnt[p], b = cnt[W + p], v = cnt[2 * (size_t)W + p];
+        if (k) {
+            NC(g_nccl.Send(t->x_lens + sk[p], k, ncclUint32, (int)p, m->comm, c->stream));
+            if (group) NC(g_nccl.Send(t->x_cnts + sk[p], k, ncclUint32, (int)p, m->comm, c->stream));
+        }
+        if (b) NC(g_nccl.Send(t->x_bytes + sb[p], b, ncclUint8, (int)p, m->comm, c->stream));
+        if (v) NC(g_nccl.Send(t->x_vals + sv[p], v, ncclUint64, (int)p, m->comm, c->stream));
+        if (rk[p]) {
+            NC(g_nccl.Recv(lens.as<u32>() + ok[p], rk[p], ncclUint32, (int)p, m->comm, c->stream));
+            if (group) NC(g_nccl.Recv(cnts.as<u32>() + ok[p], rk[p], ncclUint32, (int)p, m->comm, c->stream));
+        }
+        if (rb[p]) NC(g_nccl.Recv(bytes.as<unsigned char>() + ob[p], rb[p], ncclUint8, (int)p, m->comm, c->stream));
+        if (rv[p]) NC(g_nccl.Recv(vals.as<u64>() + ov[p], rv[p], ncclUint64, (int)p, m->comm, c->stream));
+    }
+    NC(g_nccl.GroupEnd());
+    if (e0) {
+        cudaEventRecord(e1, c->stream);
+        s->timers.push_back(Timer{e0, e1, -3, 0});
+    }
+    s->xst.post_wall_ms += ms_since(t0);
+    s->xst.sent_rows += sv[W] - cnt[2 * (size_t)W + me];
+    s->xst.recv_rows += nv - rv[me];
+    s->xst.exchanges += 1;
+    s->xst.kind = VB_XCHG_NCCL;
+    t->i_lens = lens.as<u32>(); t->i_bytes = bytes.as<unsigned char>(); t->i_cnts = group ? cnts.as<u32>() : nullptr; t->i_vals = vals.as<u64>();
+    t->i_nk = nk; t->i_nkb = nkb; t->i_nv = nv;
+    t->i_own[0] = lens.release(); t->i_own[1] = bytes.release(); t->i_own[2] = cnts.release(); t->i_own[3] = vals.release();
+    std::lock_guard<std::mutex> g(s->mu);
+    s->imported = true;
     return VB_OK;
 }
 

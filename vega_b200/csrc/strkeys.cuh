@@ -311,6 +311,41 @@ __global__ void __launch_bounds__(256) str_reduce_kernel(const u32 *__restrict__
     }
 }
 
+// ---- across ranks (engine.cu, "string keys across ranks") --------------------------------------------------------
+// The wire columns carry a u32 length per key and, for GROUP, a u32 value count per key, so that the host can
+// concatenate slices of them without rebasing anything.
+
+// out[i] = off[i + 1] - off[i] as u32: key lengths from key byte offsets, value counts from CSR offsets
+__global__ void str_diff_u32_kernel(const u64 *__restrict__ off, u64 n, u32 *__restrict__ out)
+{
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) out[i] = (u32)(off[i + 1] - off[i]);
+}
+
+// out[i] = in[i]: received lengths / counts widened for exclusive_scan_u64
+__global__ void str_widen_u32_kernel(const u32 *__restrict__ in, u64 n, u64 *__restrict__ out)
+{
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) out[i] = in[i];
+}
+
+// Imported GROUP rows: row j belongs to the received key k with voff[k] <= j < voff[k + 1] (voff: the scanned value
+// counts, voff[nk] = n), found by a binary search per row, and gets that key's entry id.  A key with no values is
+// skipped by the search (the last k with voff[k] <= j is the one whose run holds j).
+__global__ void str_expand_ids_kernel(const u64 *__restrict__ voff, u64 nk, const u32 *__restrict__ key_ids, u64 n,
+                                      u32 *__restrict__ row_ids)
+{
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 j = (u64)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += stride) {
+        u64 lo = 0, hi = nk;
+        while (hi - lo > 1) {
+            const u64 mid = (lo + hi) >> 1;
+            if (voff[mid] <= j) lo = mid; else hi = mid;
+        }
+        row_ids[j] = key_ids[lo];
+    }
+}
+
 // ---- cogroup and join of string GROUP shuffles (engine.cu, "cogroup and join of string keys") --------------------
 // Seal drops the dictionary, so a side read by a cogroup or join first gets a key index of its result keys: each dense
 // key's hash, and an index of StrDict's layout (4-slot buckets of fingerprints, parallel dense key ids).  The N-way

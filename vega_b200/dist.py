@@ -10,7 +10,8 @@ owned by rank r % world; map partitions are assigned to ranks in contiguous bloc
 source-rank-major receive order IS map-id order (group value order, SURVEY.md F5).
 
 reduce ops exchange *combined* rows (≤ distinct keys per rank — map-side combine,
-src/dependency.rs:203-209), group ops exchange raw rows.
+src/dependency.rs:203-209), group ops exchange raw rows.  String keys (StrCudaEngine, run_str_shuffle) travel as four
+columns instead of two: u32 key lengths, key bytes, u32 value counts (GROUP) and u64 values.
 
 The exchange itself lives in libvega_b200.so (vb_ctx_comm_init + vb_shuffle_exchange: NCCL grouped
 send/recv, or the fused peer-memory scatter, on the library's stream).  `run_shuffle` calls it whenever the
@@ -23,7 +24,7 @@ import ctypes
 import numpy as np
 
 from . import _lib as L
-from .rdd import Shuffle, _Col
+from .rdd import Shuffle, StrShuffle, _Col, _StrCol
 
 
 def map_block(rank, world, n_map):
@@ -202,6 +203,103 @@ def run_shuffle(engine, local_maps, n_map, n_reduce, kcode, vcode, agg, rank, wo
             stats["recv_rows"] = sum(rcounts) - rcounts[rank]
             stats["exchanges"] = stats.get("exchanges", 0) + 1
         engine.import_(sh, rk, rv, rcounts)
+    engine.seal(sh)
+    return sh
+
+
+class StrCudaEngine:
+    """libvega_b200 on this rank's GPU, for String keys: CudaEngine's calls over vb_shuffle_create_str_dist.
+    export gives ((n_keys, n_key_bytes, n_vals) per destination, (key_lens, key_bytes, val_counts, vals)), the wire
+    columns of include/vega_b200.h (val_counts None for reduce ops); import_ takes the same shape, source-rank major."""
+
+    def __init__(self, sc):
+        self.sc = sc
+
+    def create(self, n_map, n_reduce, vcode, agg, rank, world, hint=0):
+        return StrShuffle(self.sc, n_map, n_reduce, vcode, agg, hint=hint, rank=rank, world=world)
+
+    def map(self, sh, map_id, keys, vals):
+        """keys: a StrKeys column or a sequence of str; vals: a numpy array or torch CUDA tensor (None for count)."""
+        k = keys if isinstance(keys, _StrCol) else _StrCol(keys)
+        v = None if vals is None else (vals if isinstance(vals, _Col) else _Col(vals, role="value"))
+        sh.map(map_id, k, v, 0, k.n)
+
+    def export(self, sh, world):
+        return sh.export()
+
+    def import_(self, sh, cols, counts):
+        sh.import_(*cols, *counts)
+
+    def seal(self, sh):
+        sh.seal()
+
+    def reduce(self, sh, r):
+        return sh.reduce(r)
+
+
+def all_to_all_v_str(cols, counts, group=None):
+    """The String exchange step: one all_to_all_single of the three counts per destination (keys, key bytes,
+    values), then one per column.  cols = (key_lens, key_bytes, val_counts or None, vals), destination-major.
+    Returns (received columns, received counts), source-rank major, in the same shapes."""
+    import torch
+    import torch.distributed as dist
+    world = len(counts[0])
+    dev = cols[3].device
+    cin = torch.tensor(list(zip(*counts)), dtype=torch.int64, device=dev).reshape(world, 3)    # row d: what d gets
+    cout = torch.empty_like(cin)
+    dist.all_to_all_single(cout, cin, group=group)
+    rows = cout.tolist()                                                                      # row s: what s sends me
+    rcounts = tuple([r[i] for r in rows] for i in range(3))
+    splits = (0, 1, 0, 2)                        # the count each column is split by: keys, bytes, keys, values
+
+    def a2a(t, i):
+        if t is None:
+            return None
+        out = torch.empty(sum(rcounts[splits[i]]), dtype=t.dtype, device=t.device)
+        dist.all_to_all_single(out, t, output_split_sizes=rcounts[splits[i]], input_split_sizes=list(counts[splits[i]]),
+                               group=group)
+        return out
+    return tuple(a2a(t, i) for i, t in enumerate(cols)), rcounts
+
+
+def run_str_shuffle(engine, local_maps, n_map, n_reduce, vcode, agg, rank, world, group=None, hint=0, stats=None,
+                    exchange_device=None):
+    """run_shuffle for String keys: map side on this rank's partitions → exchange → reduce side for the partitions
+    this rank owns.  local_maps: [(map_id, keys, vals_or_None)], ascending map ids from map_block(rank, world, n_map).
+    With a communicator on the context the exchange is vb_shuffle_exchange (NCCL inside the library); otherwise four
+    all_to_all_single calls after the count swap (exchange_device: "cpu" for a gloo group on a one-GPU box)."""
+    sh = engine.create(n_map, n_reduce, vcode, agg, rank, world, hint=hint)
+    for map_id, keys, vals in local_maps:
+        engine.map(sh, map_id, keys, vals)
+    if world > 1 and isinstance(engine, StrCudaEngine) and getattr(engine.sc, "comm", None) and exchange_device is None:
+        sh.exchange(L.VB_XCHG_NCCL)
+        engine.seal(sh)
+        if stats is not None:
+            for k_, v_ in sh.exchange_stats().items():
+                stats[k_] = (stats.get(k_, 0) + v_) if k_ in ("exchange_ms", "exchanges", "prepare_wall_ms", "counts_wall_ms", "post_wall_ms") else v_
+        return sh
+    if world > 1:
+        counts, cols = engine.export(sh, world)
+        home = cols[3].device
+        if exchange_device is not None:
+            cols = tuple(None if c is None else c.to(exchange_device) for c in cols)
+        ev = None
+        if stats is not None and cols[3].is_cuda:
+            import torch
+            ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
+            ev[0].record()
+        rcols, rcounts = all_to_all_v_str(cols, counts, group)
+        if ev is not None:
+            ev[1].record()
+            ev[1].synchronize()
+            stats["exchange_ms"] = stats.get("exchange_ms", 0.0) + ev[0].elapsed_time(ev[1])
+        if exchange_device is not None:
+            rcols = tuple(None if c is None else c.to(home) for c in rcols)
+        if stats is not None:
+            stats["sent_rows"] = sum(counts[2]) - counts[2][rank]
+            stats["recv_rows"] = sum(rcounts[2]) - rcounts[2][rank]
+            stats["exchanges"] = stats.get("exchanges", 0) + 1
+        engine.import_(sh, rcols, rcounts)
     engine.seal(sh)
     return sh
 

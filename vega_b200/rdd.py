@@ -1142,20 +1142,72 @@ class _StrCol:
         self.code = None
 
 
-class StrShuffle(Shuffle):
-    """One string-key shuffle (vb_shuffle_create_str).  seal / stats / free as for Shuffle."""
+class _DevView:
+    """Zero-copy view of a library-owned device buffer for torch.as_tensor."""
 
-    def __init__(self, sc, n_map, n_reduce, vcode, agg, hint=0):
+    def __init__(self, ptr, n, typestr):
+        self.__cuda_array_interface__ = {"shape": (n,), "typestr": typestr, "data": (ptr, False), "version": 2}
+
+
+class StrShuffle(Shuffle):
+    """One string-key shuffle (vb_shuffle_create_str; vb_shuffle_create_str_dist for rank `rank` of `world` > 1).
+    seal / exchange / stats / free as for Shuffle."""
+
+    def __init__(self, sc, n_map, n_reduce, vcode, agg, hint=0, rank=0, world=1):
         self.sc, self._lib = sc, sc._lib
         self.n_map, self.n_reduce, self.agg, self.vcode, self.kcode = n_map, n_reduce, agg, vcode, None
+        self.rank, self.world = rank, world
         self.has_payload = True
         self._keepalive = []
         h = ctypes.c_void_p()
-        L.check(self._lib.vb_shuffle_create_str(sc._h, sc.new_shuffle_id(), n_map, n_reduce, vcode, agg, ctypes.byref(h)))
+        if world > 1:
+            L.check(self._lib.vb_shuffle_create_str_dist(sc._h, sc.new_shuffle_id(), n_map, n_reduce, vcode, agg, rank, world,
+                                                         ctypes.byref(h)))
+        else:
+            L.check(self._lib.vb_shuffle_create_str(sc._h, sc.new_shuffle_id(), n_map, n_reduce, vcode, agg, ctypes.byref(h)))
         self._h = h
         sc._shuffles.add(self)
         if hint:
             L.check(self._lib.vb_shuffle_set_hint(h, hint))
+
+    def export(self):
+        """vb_shuffle_export_str_prepare + buffers (world > 1): ((n_keys, n_key_bytes, n_vals), (key_lens, key_bytes,
+        val_counts, vals)).  The counts are lists with one entry per destination rank; the columns are torch views of
+        the library's device buffers (int32 lengths and counts, uint8 bytes, int64 values; val_counts is None for
+        reduce ops), destination-major and valid until seal."""
+        import torch
+        W = self.world
+        nk, nb, nv = (ctypes.c_uint64 * W)(), (ctypes.c_uint64 * W)(), (ctypes.c_uint64 * W)()
+        L.check(self._lib.vb_shuffle_export_str_prepare(self._h, nk, nb, nv))
+        counts = tuple([int(x) for x in c] for c in (nk, nb, nv))
+        ptrs = [ctypes.c_void_p() for _ in range(4)]
+        L.check(self._lib.vb_shuffle_export_str_buffers(self._h, *[ctypes.byref(p) for p in ptrs]))
+        dev = f"cuda:{self._lib.vb_ctx_device(self.sc._h)}"
+        K, B, V = sum(counts[0]), sum(counts[1]), sum(counts[2])
+        group = self.agg == L.VB_AGG_GROUP
+
+        def view(p, n, typestr, dtype):
+            if n == 0 or not p.value:
+                return torch.empty(0, dtype=dtype, device=dev)
+            return torch.as_tensor(_DevView(p.value, n, typestr), device=dev)
+        cols = (view(ptrs[0], K, "<i4", torch.int32), view(ptrs[1], B, "|u1", torch.uint8),
+                view(ptrs[2], K, "<i4", torch.int32) if group else None, view(ptrs[3], V, "<i8", torch.int64))
+        return counts, cols
+
+    def import_(self, key_lens, key_bytes, val_counts, vals, n_keys, n_key_bytes, n_vals):
+        """vb_shuffle_import_str: the received columns (torch CUDA tensors, source-rank major) and the counts every
+        source rank sent.  The tensors are kept alive until seal."""
+        import torch
+        ts = [t for t in (key_lens, key_bytes, val_counts, vals) if t is not None]
+        for t in ts:
+            if t.is_cuda:
+                torch.cuda.current_stream(t.device).synchronize()   # the library reads on its own stream
+                break
+        self._keepalive.append(tuple(ts))
+        p = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None and t.numel() else None
+        arr = lambda c: (ctypes.c_uint64 * len(c))(*c)
+        L.check(self._lib.vb_shuffle_import_str(self._h, p(key_lens), p(key_bytes), p(val_counts), p(vals),
+                                                arr(n_keys), arr(n_key_bytes), arr(n_vals)))
 
     def map(self, map_id, keys, vals, start, stop):
         """Rows [start, stop) of the string key column (and of the values) as map partition map_id."""
