@@ -412,3 +412,58 @@ def test_config3_shape_scaled(sc, kind):
     assert n_only_l == (n - shared if kind != "right" else 0) and n_only_r == (n - shared if kind != "left" else 0)
     del a, b
     torch.cuda.empty_cache()
+
+
+# ---- 11. the right side freed after a size call, and a new shuffle at its address ------------------------------
+def _grouped(sc, k, v, R):
+    """A sealed COGROUP shuffle of (k, v) in one map task, grouped by reading every partition."""
+    s = vb.Shuffle(sc, 1, R, L.VB_U64, L.VB_U64, L.VB_AGG_COGROUP)
+    s.map(0, vb.rdd._Col(k), vb.rdd._Col(v), 0, len(k))
+    s.seal()
+    for r in range(R):
+        s.reduce(r)
+    return s
+
+
+def test_right_side_address_reused(sc):
+    """A size call with no write, then the right side freed: a later join with another shuffle that the allocator
+    places at the freed side's address gets that shuffle's sizes and rows.  The sizes are checked before any write."""
+    R = 3
+    rng = np.random.default_rng(11)
+    ka, va = rand_pairs(rng, 6000, 800)
+    k1, v1 = rand_pairs(rng, 4000, 1000)
+    k2, v2 = rand_pairs(rng, 9000, 3000)                # other rows: every partition's sizes differ from r1's
+    lib, n = sc._lib, ctypes.c_uint64()
+    mask = {"left": 0b01, "right": 0b10, "full": 0}
+    want = {kind: OJ.outer_join_parts(kind, ka, va, 1, k2, v2, 1, R) for kind in KINDS}
+    sa, r1 = _grouped(sc, ka, va, R), _grouped(sc, k1, v1, R)
+    old = {}
+    for kind in KINDS:
+        for r in range(R):
+            L.check(lib.vb_join_outer_size(sa._h, r1._h, r, CODE[kind], ctypes.byref(n)))
+            old[kind, r] = n.value
+    addr = r1._h.value
+    r1.free()
+    others = []
+    try:
+        for _ in range(64):
+            r2 = _grouped(sc, k2, v2, R)
+            if r2._h.value == addr:
+                break
+            others.append(r2)
+        else:
+            pytest.skip("the allocator never placed a new shuffle at the freed right side's address")
+        nn = ctypes.c_uint64()
+        for kind in KINDS:
+            for r in range(R):
+                L.check(lib.vb_join_outer_size(sa._h, r2._h, r, CODE[kind], ctypes.byref(n)))
+                L.check(lib.vb_join_n_outer_size((ctypes.c_void_p * 2)(sa._h.value, r2._h.value), 2, r, mask[kind],
+                                                 ctypes.byref(nn)))
+                rows = sum(len(x) for x in want[kind][r].values())
+                assert rows != old[kind, r]
+                assert (n.value, nn.value) == (rows, rows), (kind, r, old[kind, r])
+        for kind in KINDS:
+            assert_parts_equal([by_key(*abi_rows(sc, sa, r2, r, kind)) for r in range(R)], want[kind])
+    finally:
+        for s_ in others:
+            s_.free()

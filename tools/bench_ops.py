@@ -18,11 +18,14 @@ ap = argparse.ArgumentParser()
 ap.add_argument("--rows", type=float, default=1e9)
 ap.add_argument("--distinct", type=float, default=1e6)
 ap.add_argument("--ops", default="reduce,group,sort,sortkv,join,count")   # also: zipf, zipfgroup, combine, combinezipf,
-#                                                                             leftjoin, fulljoin, cogroup, cogroup3, join3,
-#                                                                             join3outer
+#                                                                             leftjoin, rightjoin, fulljoin, cogroup, cogroup3,
+#                                                                             join3, join3outer
 ap.add_argument("--reps", type=int, default=3)
+# reduce partitions of join, leftjoin, rightjoin, fulljoin and cogroup; many partitions of a small input (--rows 1.6e6
+# gives 2e5 rows per side) time the fixed cost of every partition's plan
+ap.add_argument("--join-splits", type=int, default=8)
 args = ap.parse_args()
-N, D = int(args.rows), int(args.distinct)
+N, D, JR = int(args.rows), int(args.distinct), args.join_splits
 sc = vb.Context(0, profile=True)
 stream = sc.stream()
 PEAK = 3350.0      # GB/s, NVIDIA H100 SXM data sheet (HBM3); the fraction columns are of this peak
@@ -94,7 +97,7 @@ if "sort" in ops:
     report("sort_by_key(keys only)", N, 16.0 * N, timed(lambda: run_shuffle(L.VB_AGG_SORT, keys=keys), max(1, args.reps - 1)))
     del keys
     torch.cuda.empty_cache()
-join_ops = [o for o in ("join", "leftjoin", "fulljoin", "cogroup", "cogroup3", "join3", "join3outer") if o in ops]
+join_ops = [o for o in ("join", "leftjoin", "rightjoin", "fulljoin", "cogroup", "cogroup3", "join3", "join3outer") if o in ops]
 if join_ops:
     # BASELINE config 4, per-GPU share at 8 GPUs: 6.25e7 rows per side, each rank once per side,
     # 1.25e6 shared keys per GPU (1e7 / 8)
@@ -107,8 +110,8 @@ if join_ops:
     sc.gen_pairs(out_rows=b, first=0, n=n_side, mode="unique", rank_base=n_side - shared)
 
     def cogroup_pair():
-        sa = vb.Shuffle(sc, 8, 8, L.VB_U64, L.VB_U64, L.VB_AGG_COGROUP)
-        sb = vb.Shuffle(sc, 8, 8, L.VB_U64, L.VB_U64, L.VB_AGG_COGROUP)
+        sa = vb.Shuffle(sc, 8, JR, L.VB_U64, L.VB_U64, L.VB_AGG_COGROUP)
+        sb = vb.Shuffle(sc, 8, JR, L.VB_U64, L.VB_U64, L.VB_AGG_COGROUP)
         for s_, t in ((sa, a), (sb, b)):
             col = vb.rdd._Col(t, allow_rows=True)
             st = vb.slice_starts(col.n, 8)
@@ -128,7 +131,7 @@ if join_ops:
     def join():
         sa, sb = cogroup_pair()
         tot = 0
-        for r in range(8):
+        for r in range(JR):
             nn = ctypes.c_uint64()
             L.check(sc._lib.vb_join_size(sa._h, sb._h, r, ctypes.byref(nn)))
             k, v, w = (torch.empty(nn.value, dtype=torch.int64, device="cuda") for _ in range(3))
@@ -143,8 +146,8 @@ if join_ops:
 if "join" in ops:
     res = timed(join, max(1, args.reps - 1))
     assert res[-1][1]["join_rows"] == shared, (res[-1][1]["join_rows"], shared)
-    report("join", 2 * n_side, 32.0 * n_side + 24.0 * shared, res, {"join_rows": shared})
-if "leftjoin" in ops or "fulljoin" in ops or "cogroup" in ops or "cogroup3" in ops:
+    report("join", 2 * n_side, 32.0 * n_side + 24.0 * shared, res, {"join_rows": shared, "reduce_splits": JR})
+if "leftjoin" in ops or "rightjoin" in ops or "fulljoin" in ops or "cogroup" in ops or "cogroup3" in ops:
     # Each outer join against the inner join of the same inputs and against the workaround without outer joins:
     # materialising the cogroup of both sides (vb_shuffle_reduce of every partition, device output), which the
     # caller then still has to expand.  All outputs stay on the device.
@@ -157,7 +160,7 @@ if "leftjoin" in ops or "fulljoin" in ops or "cogroup" in ops or "cogroup3" in o
         def run():
             sa, sb = cogroup_pair()
             tot = 0
-            for r in range(8):
+            for r in range(JR):
                 nn = ctypes.c_uint64()
                 L.check(sc._lib.vb_join_outer_size(sa._h, sb._h, r, kind, ctypes.byref(nn)))
                 k, v, w = dev(nn.value), dev(nn.value), dev(nn.value)
@@ -172,7 +175,7 @@ if "leftjoin" in ops or "fulljoin" in ops or "cogroup" in ops or "cogroup3" in o
 
     def cogroup_both():
         sa, sb = cogroup_pair()
-        for r in range(8):
+        for r in range(JR):
             for s_ in (sa, sb):
                 nk, nv = ctypes.c_uint64(), ctypes.c_uint64()
                 L.check(sc._lib.vb_shuffle_reduce_size(s_._h, r, ctypes.byref(nk), ctypes.byref(nv)))
@@ -186,7 +189,7 @@ if "leftjoin" in ops or "fulljoin" in ops or "cogroup" in ops or "cogroup3" in o
         # vb_cogroup of every partition: both sides grouped and aligned by key, device output
         sa, sb = cogroup_pair()
         tot = 0
-        for r in range(8):
+        for r in range(JR):
             nk, nl, nr = ctypes.c_uint64(), ctypes.c_uint64(), ctypes.c_uint64()
             L.check(sc._lib.vb_cogroup_size(sa._h, sb._h, r, ctypes.byref(nk), ctypes.byref(nl), ctypes.byref(nr)))
             k, lo, lv, ro, rv = dev(nk.value), dev(nk.value + 1), dev(nl.value), dev(nk.value + 1), dev(nr.value)
@@ -199,16 +202,18 @@ if "leftjoin" in ops or "fulljoin" in ops or "cogroup" in ops or "cogroup3" in o
 
     med = lambda r: sorted(x[0] for x in r)[len(r) // 2]
     reps = max(1, args.reps - 1)
-    r_inner = timed(join, reps) if "leftjoin" in ops or "fulljoin" in ops else None
+    outer_ops = (("leftjoin", "left_outer_join", L.VB_JOIN_LEFT, n_side), ("rightjoin", "right_outer_join", L.VB_JOIN_RIGHT, n_side),
+                 ("fulljoin", "full_outer_join", L.VB_JOIN_FULL, 2 * n_side - shared))
+    r_inner = timed(join, reps) if any(o[0] in ops for o in outer_ops) else None
     r_cog = timed(cogroup_both, reps)
-    for op, kind, want in (("leftjoin", L.VB_JOIN_LEFT, n_side), ("fulljoin", L.VB_JOIN_FULL, 2 * n_side - shared)):
+    for op, name, kind, want in outer_ops:
         if op not in ops:
             continue
         res = timed(outer(kind), reps)
         assert res[-1][1]["join_rows"] == want, (res[-1][1]["join_rows"], want)
-        extra = {"gpu": card["name"], "power_limit_w": card["power_limit_w"], "join_rows": want,
+        extra = {"gpu": card["name"], "power_limit_w": card["power_limit_w"], "join_rows": want, "reduce_splits": JR,
                  "inner_join_ms": round(med(r_inner), 3), "cogroup_both_sides_ms": round(med(r_cog), 3)}
-        report({"leftjoin": "left_outer_join", "fulljoin": "full_outer_join"}[op], 2 * n_side, 32.0 * n_side + 26.0 * want, res, extra)
+        report(name, 2 * n_side, 32.0 * n_side + 26.0 * want, res, extra)
     if "cogroup" in ops:
         # against cogroup_both (two vb_shuffle_reduce per partition): the grouping alone, without the alignment by key
         res = timed(cogroup, reps)

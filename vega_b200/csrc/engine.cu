@@ -275,7 +275,7 @@ struct Timer {
     u64 rows;
 };
 
-// vb_join_outer_size's result for one (right side, partition, outer kind), kept for vb_join_outer
+// vb_join_outer_size's result for one (right side's uid, partition, outer kind), kept for vb_join_outer
 struct JoinPlan {
     u64 total = 0;
     u32 nl = 0;
@@ -361,7 +361,7 @@ struct vb_shuf {
     void *dict = nullptr;          // group ops: key → slot table, kept for joins
     u32 dict_log_cap = 0;
     u32 *dense_of_slot = nullptr;
-    std::map<std::tuple<const vb_shuf *, u32, int>, JoinPlan> join_plans;   // by (right side, partition, outer kind)
+    std::map<std::tuple<u64, u32, int>, JoinPlan> join_plans;   // by (right side's uid, partition, outer kind)
     // on side 0 of a cogroup or a join, of two sides or N: by (every side's uid, partition, NP_* kind or outer mask)
     std::map<std::tuple<std::vector<u64>, u32, i64>, CogroupNPlan> n_plans;
     // COGROUP shuffles are grouped lazily: seal keeps the (owned) rows; the CSR is built by the first reduce call
@@ -3311,7 +3311,7 @@ static_assert(JK_LEFT == (int)VB_JOIN_LEFT && JK_RIGHT == (int)VB_JOIN_RIGHT && 
 static int join_plan(vb_shuf *l, vb_shuf *r, u32 rid, int kind, JoinPlan **out)
 {
     vb_ctx *c = l->ctx;
-    auto key = std::make_tuple((const vb_shuf *)r, rid, kind);
+    auto key = std::make_tuple(r->uid, rid, kind);    // by uid: a freed side's address may be reused
     auto it = l->join_plans.find(key);
     if (it != l->join_plans.end()) { *out = &it->second; return VB_OK; }
     JoinPlan p;
@@ -3448,7 +3448,7 @@ static int join_rows(vb_shuf *l, vb_shuf *r, uint32_t rid, int kind, void *out_k
     }
     dev_free(c, p->pos);
     dev_free(c, p->match);
-    l->join_plans.erase(std::make_tuple((const vb_shuf *)r, rid, kind));
+    l->join_plans.erase(std::make_tuple(r->uid, rid, kind));
     return rc;
 }
 
