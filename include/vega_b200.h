@@ -259,8 +259,9 @@ VB_API int32_t vb_shuffle_reduce(vb_shuf *s, uint32_t reduce_id, void *out_keys,
  * internal one); that internal COUNT counts against VB_MAX_AGGS.  Keys are placed by MetroHash64_1(k) % n_reduce,
  * the same partition as any single-column shuffle of the same keys; vb_shuffle_set_key_width / set_hint apply.
  * VB_ERR_INVALID: more than VB_MAX_VAL_COLS columns or VB_MAX_AGGS aggregates, src out of range, or a GROUP /
- * COGROUP / SORT op.  Not supported (VB_ERR_UNSUPPORTED): world > 1 (vb_shuffle_set_dist, export / import /
- * exchange), the bincode blob calls, AoS rows (vb_shuffle_map_aos).  vb_shuffle_map_soa returns VB_ERR_INVALID;
+ * COGROUP / SORT op.  Several ranks: vb_shuffle_create_multi_dist and the _cols export / import calls below.  Not
+ * supported (VB_ERR_UNSUPPORTED): vb_shuffle_set_dist with world > 1, the single-column export / import and P2P calls,
+ * the bincode blob calls, AoS rows (vb_shuffle_map_aos).  vb_shuffle_map_soa returns VB_ERR_INVALID;
  * vb_shuffle_reduce returns the keys only (VB_ERR_INVALID with out_combined != NULL); the join calls return
  * VB_ERR_INVALID; vb_shuffle_reduce_size / seal / stats / kernel_time / free work as for any reduce shuffle.   */
 #define VB_MAX_VAL_COLS 4
@@ -277,6 +278,44 @@ VB_API int32_t vb_shuffle_map_cols(vb_shuf *s, uint32_t map_id, const void *keys
                                    int32_t src_loc);
 /* one reduce partition: out_keys[n_keys] and out_aggs[a][n_keys] per aggregate (NULL entries are skipped) */
 VB_API int32_t vb_shuffle_reduce_cols(vb_shuf *s, uint32_t reduce_id, void *out_keys, void *const *out_aggs, int32_t dst_loc);
+/* combine_by_key across ranks (one process per GPU; ShuffleFetcher::fetch of the combiners, shuffle_fetcher.rs:16-119).
+ * vb_shuffle_create_multi_dist is vb_shuffle_create_multi for rank `rank` of `world` (1 <= world <= 256, VB_ERR_INVALID
+ * otherwise); world == 1 gives the same shuffle as vb_shuffle_create_multi.  Placement is unchanged: partition
+ * MetroHash64_1(k) % n_reduce with the shuffle's key width, owned by rank r % world.  Each rank runs its map tasks
+ * (vb_shuffle_map_cols, any src_loc, resubmission allowed), then:
+ *   vb_shuffle_export_cols_prepare  finishes the local map side (merges the map tables) and packs one row per distinct
+ *                                   key by destination rank; counts[world] gets the rows going to each rank.
+ *   vb_shuffle_export_cols_buffers  the device columns, destination-major, owned by the library until seal (NULL output
+ *                                   pointers are skipped); n_acc gets the accumulator count.  This is the wire format:
+ *                                     keys  u64 [rows]
+ *                                     accs  u64 [n_acc][rows]   accumulator a of row i at accs[a * rows + i], rows = the
+ *                                                               sum of counts; each the rank's partial in plain value form:
+ *                                       SUM, and a MEAN's sum   the wrapping u64 sum, or the f64 sum
+ *                                       COUNT (the spec's, or   the partial count
+ *                                       the internal one a MEAN adds after the aggregates)
+ *                                       MIN / MAX               the rank's result in the column's dtype; f64: NaN when all
+ *                                                               the rank's values of the key were NaN
+ *                                   Accumulator a is aggregate a's; n_acc = n_aggs, plus 1 for the internal COUNT.
+ *   vb_shuffle_import_cols          the received columns, source-rank major, accs as [n_acc][n] with n = the sum of
+ *                                   counts (what each source sent); borrowed until vb_shuffle_seal returns.  Then seal.
+ * The seal merges the partials with merge_combiners (partial COUNTs summed, SUM added, MIN / MAX by their vb_agg rules)
+ * and finalizes as the one-process seal does, so every owner's partitions equal those of the one-process
+ * vb_shuffle_create_multi shuffle over the same map tasks, whatever `world` is (f64 SUM and MEAN up to summation
+ * order).  Partitions a rank does not own are empty on it.
+ * vb_shuffle_exchange(s, VB_XCHG_AUTO or VB_XCHG_NCCL) does all of it on the library's stream: export, one all-gather of
+ * the counts and a fingerprint of the spec (n_acc, every accumulator's op and order transform, key width, n_reduce),
+ * one grouped send/recv of the key column and the n_acc accumulator columns.  Ranks whose specs differ all return
+ * VB_ERR_INVALID before any send; VB_XCHG_P2P, and any exchange of a world-1 shuffle, is VB_ERR_UNSUPPORTED.
+ * Errors: the _cols calls on a multi-aggregate shuffle of world 1: VB_ERR_STATE (VB_ERR_INVALID on any other shuffle);
+ * import before export, twice, or after seal: VB_ERR_STATE; map after export: VB_ERR_STATE; seal without import:
+ * VB_ERR_STATE; an n_acc that differs from the shuffle's, or a NULL column with a non-zero count: VB_ERR_INVALID; an
+ * import of 2^32 - 2 rows or more: VB_ERR_TOO_LARGE, from the counts.                                                  */
+VB_API int32_t vb_shuffle_create_multi_dist(vb_ctx *ctx, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce, int32_t key_dtype,
+                                            uint32_t n_val_cols, const int32_t *val_dtypes, uint32_t n_aggs, const vb_agg_col *aggs,
+                                            uint32_t rank, uint32_t world, vb_shuf **out);
+VB_API int32_t vb_shuffle_export_cols_prepare(vb_shuf *s, uint64_t *counts /*[world]*/);
+VB_API int32_t vb_shuffle_export_cols_buffers(vb_shuf *s, void **keys, void **accs, uint32_t *n_acc);
+VB_API int32_t vb_shuffle_import_cols(vb_shuf *s, const void *keys, const void *accs, uint32_t n_acc, const uint64_t *counts /*[world]*/);
 
 /* A sealed reduce-op or combine_by_key shuffle as a cogroup / join parent under the same partitioner, without a
  * shuffle (CoGroupedRdd::new's OneToOneDependency, co_grouped_rdd.rs:103-112).  *out is a new sealed COGROUP-kind

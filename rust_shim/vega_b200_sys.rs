@@ -94,6 +94,14 @@ extern "C" {
                                    val_dtypes: *const i32, n_aggs: u32, aggs: *const vb_agg_col, out: *mut *mut vb_shuf) -> i32;
     pub fn vb_shuffle_map_cols(s: *mut vb_shuf, map_id: u32, keys: *const c_void, vals: *const *const c_void, n_rows: u64, src_loc: i32) -> i32;
     pub fn vb_shuffle_reduce_cols(s: *mut vb_shuf, reduce_id: u32, out_keys: *mut c_void, out_aggs: *const *mut c_void, dst_loc: i32) -> i32;
+    // combine_by_key across ranks: export packs one row per distinct key by destination rank (u64 keys, u64 accumulator
+    // columns [n_acc][rows] in plain value form), import takes them source-rank major (borrowed until seal)
+    pub fn vb_shuffle_create_multi_dist(ctx: *mut vb_ctx, shuffle_id: u64, n_map: u32, n_reduce: u32, key_dtype: i32, n_val_cols: u32,
+                                        val_dtypes: *const i32, n_aggs: u32, aggs: *const vb_agg_col, rank: u32, world: u32,
+                                        out: *mut *mut vb_shuf) -> i32;
+    pub fn vb_shuffle_export_cols_prepare(s: *mut vb_shuf, counts: *mut u64) -> i32;
+    pub fn vb_shuffle_export_cols_buffers(s: *mut vb_shuf, keys: *mut *mut c_void, accs: *mut *mut c_void, n_acc: *mut u32) -> i32;
+    pub fn vb_shuffle_import_cols(s: *mut vb_shuf, keys: *const c_void, accs: *const c_void, n_acc: u32, counts: *const u64) -> i32;
     // a sealed reduce-op / combine_by_key shuffle as a cogroup or join side under the same partitioner (OneToOneDependency)
     pub fn vb_shuffle_create_narrow(parent: *mut vb_shuf, out_col: u32, out: *mut *mut vb_shuf) -> i32;
     // String keys (Arrow-style offsets + bytes; placed by MetroHash64_1(bytes ‖ 0xFF) like `str::hash`)

@@ -4,6 +4,8 @@
   zipf   configs[4]: reduce_by_key(sum), rows/GPU Zipf(1.1) pairs over 1e6 keys, 8 map partitions/GPU, 8*N reduce
   join   configs[3]: join of two RDDs with unique keys (rows/GPU per side), shared keys = rows/50, N map x 8 reduce... (R = max(8, N))
   group  group_by_key of rows/GPU uniform pairs: raw rows cross NVLink in ONE all-to-all-v (exchange GB/s)
+  combine  combine_by_key of rows/GPU uniform rows, tools/bench_ops.py's spec (sum, min, max, mean, count: 5
+         accumulators); one row per distinct key and rank crosses NVLink with its 5 partials
 
 Each line: whole-job rows/s (max over ranks), exchange bytes/time, and a size-independent parity property."""
 import argparse
@@ -176,6 +178,48 @@ if "zipf" in ops:
           "exchange_ms": st.get("exchange_ms"), "bytes_sent_per_rank": 16 * st.get("sent_rows", 0),
           "note": "time includes the D2H read-back of every owned partition"})
     del rows
+    torch.cuda.empty_cache()
+
+if "combine" in ops:
+    keys = torch.empty(N, dtype=torch.int64, device=dev)
+    v0 = torch.empty(N, dtype=torch.int64, device=dev)
+    sc.gen_pairs(out_keys=keys, out_vals=v0, first=rank * N, n=N, mode="uniform", n_distinct=D)
+    v1 = v0 * 7 - 3_000_000
+    v2 = v0.to(torch.float64) * 0.5
+    torch.cuda.synchronize()
+    spec = ([L.VB_U64, L.VB_I64, L.VB_F64],
+            [(L.VB_AGG_SUM, 0), (L.VB_AGG_MIN, 1), (L.VB_AGG_MAX, 1), (L.VB_AGG_MEAN, 2), (L.VB_AGG_COUNT, 0)])
+    ceng = vdist.CombineCudaEngine(sc)
+    R = 8 * world
+    starts = vb.slice_starts(N, 8)
+    lo, _ = vdist.map_block(rank, world, 8 * world)
+
+    def col(t, code):
+        c = vb.rdd._Col(t)
+        c.code = code
+        return c
+    maps = [(lo + m, col(keys[int(starts[m]):int(starts[m + 1])], L.VB_U64),
+             tuple(col(t[int(starts[m]):int(starts[m + 1])], code) for t, code in ((v0, L.VB_U64), (v1, L.VB_I64), (v2, L.VB_F64))))
+            for m in range(8)]
+
+    def run():
+        st = {}
+        sh = vdist.run_combine_shuffle(ceng, maps, 8 * world, R, L.VB_U64, spec, rank, world, hint=D, stats=st)
+        nk = cnt = 0
+        for r in vdist.owned_partitions(rank, world, R):
+            k, outs = sh.reduce_cols(r, [np.uint64, np.int64, np.int64, np.float64, np.uint64])
+            nk += len(k)
+            cnt += int(outs[4].sum(dtype=np.uint64))
+        sh.free()
+        return nk, cnt, st
+
+    dt, (nk, cnt, st) = timed(run)
+    emit({"op": "combine_by_key 5 aggs", "n_gpus": world, "rows_total": N * world, "partitions": R, "s": dt,
+          "rows_per_s": N * world / dt, "distinct_keys_out": int(allsum(float(nk))),
+          "counts_match_input": int(allsum(float(cnt))) == N * world, "exchange_ms": st.get("exchange_ms"),
+          "sent_rows": st.get("sent_rows"), "bytes_sent_per_rank": 48 * st.get("sent_rows", 0),
+          "note": "a sent row is the key and 5 partials (48 B); time includes the D2H read-back of every owned partition"})
+    del keys, v0, v1, v2, maps
     torch.cuda.empty_cache()
 
 if "group" in ops:

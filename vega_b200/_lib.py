@@ -91,6 +91,11 @@ SYMBOLS = {
     "vb_shuffle_create_multi": (_i32, [_vp, _u64, _u32, _u32, _i32, _u32, _vp, _u32, ctypes.POINTER(vb_agg_col), _pvp]),
     "vb_shuffle_map_cols": (_i32, [_vp, _u32, _vp, _pvp, _u64, _i32]),
     "vb_shuffle_reduce_cols": (_i32, [_vp, _u32, _vp, _pvp, _i32]),
+    "vb_shuffle_create_multi_dist": (_i32, [_vp, _u64, _u32, _u32, _i32, _u32, _vp, _u32, ctypes.POINTER(vb_agg_col), _u32, _u32,
+                                            _pvp]),
+    "vb_shuffle_export_cols_prepare": (_i32, [_vp, _pu64]),
+    "vb_shuffle_export_cols_buffers": (_i32, [_vp, _pvp, _pvp, ctypes.POINTER(_u32)]),
+    "vb_shuffle_import_cols": (_i32, [_vp, _vp, _vp, _u32, _pu64]),
     "vb_shuffle_create_narrow": (_i32, [_vp, _u32, _pvp]),
     "vb_join_size": (_i32, [_vp, _vp, _u32, _pu64]),
     "vb_join": (_i32, [_vp, _vp, _u32, _vp, _vp, _vp, _i32]),

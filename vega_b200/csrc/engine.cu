@@ -314,6 +314,7 @@ struct vb_shuf {
     bool multi = false;
     u32 n_cols = 0;
     AccSpec acc_map{}, acc_merge{};   // map-side combine / table merge (COUNT merges as ADD, no order transform)
+    AccSpec acc_imp{};                // merge of partials received from other ranks: merge ops, the map spec's transforms
     OutSpec outs{};                   // one output column per vb_agg_col
     int out_dt[VB_MAX_AGGS] = {};     // each output column's dtype (a narrow view's value dtype)
     u64 *res_cols = nullptr;          // [outs.n][n_keys], partition-major like res_keys
@@ -338,7 +339,7 @@ struct vb_shuf {
     u32 waiters = 0;               // threads blocked in wait_sealed: vb_shuffle_free drains them before deleting
     // export / import (world > 1)
     bool exported = false, imported = false;
-    u64 *exp_keys = nullptr, *exp_vals = nullptr;
+    u64 *exp_keys = nullptr, *exp_vals = nullptr;     // multi-aggregate shuffles: exp_vals = the accumulators [n_acc][rows]
     // fused export (P2P): plan + scanned histogram + gathered input kept between export_counts and export_direct
     u32 *exp_hist = nullptr;
     u32 exp_parts = 0;
@@ -346,7 +347,7 @@ struct vb_shuf {
     const u64 *exp_rows = nullptr, *exp_k = nullptr, *exp_v = nullptr;
     std::vector<u64> exp_digit_start;
     bool exp_counted = false;
-    const u64 *imp_keys = nullptr, *imp_vals = nullptr;
+    const u64 *imp_keys = nullptr, *imp_vals = nullptr;   // multi-aggregate shuffles: imp_vals = the partials [n_acc][imp_n]
     u64 imp_n = 0;
     u64 *imp_own_k = nullptr, *imp_own_v = nullptr;   // receive buffers of vb_shuffle_exchange (freed with the inputs)
     std::vector<u64> sort_part_rows;                  // multi-rank sort: exact rows of every output partition this rank owns (0 elsewhere)
@@ -598,6 +599,11 @@ static int launch_hash_agg_multi(vb_shuf *s, int klass, const AccSpec &sp, const
         mc.c[0] = in.b;
         mc.stride = (in.n - 1) + BUCKET;                    // the source has in.n - 1 regular slots
         return launch_hash_agg_multi_t<IN_TABLE, 1>(s, klass, sp, keys, mc, n, tab, log_cap, ctl, mi);
+    }
+    if (in.in == IN_ACCS) {
+        mc.c[0] = in.b;
+        mc.stride = in.n;                                   // received partials: [n_acc][in.n]
+        return launch_hash_agg_multi_t<IN_ACCS, 1>(s, klass, sp, keys, mc, n, tab, log_cap, ctl, mi);
     }
     for (u32 i = 0; i < s->n_cols; ++i) mc.c[i] = vcols[i];
     switch (s->n_cols) {
@@ -1304,7 +1310,7 @@ extern "C" int32_t vb_shuffle_create_multi(vb_ctx *c, uint64_t shuffle_id, uint3
     s->n_cols = n_val_cols;
     AccSpec &mp = s->acc_map, &mg = s->acc_merge;
     OutSpec &os = s->outs;
-    mp.n = mg.n = n_acc;
+    mp.n = mg.n = s->acc_imp.n = n_acc;
     os.n = n_aggs;
     for (u32 a = 0; a < n_acc; ++a) {
         const int op = a < n_aggs ? aggs[a].agg : VB_AGG_COUNT;
@@ -1318,6 +1324,7 @@ extern "C" int32_t vb_shuffle_create_multi(vb_ctx *c, uint64_t shuffle_id, uint3
         }
         spec_set(mp.op, a, opk); spec_set(mp.tx, a, tx); spec_set(mp.src, a, src);
         spec_set(mg.op, a, merge_op(opk)); spec_set(mg.src, a, a);
+        spec_set(s->acc_imp.op, a, merge_op(opk)); spec_set(s->acc_imp.tx, a, tx);
         if (a >= n_aggs) continue;
         s->out_dt[a] = op == VB_AGG_COUNT ? VB_U64 : op == VB_AGG_MEAN ? VB_F64 : dt;
         os.acc[a] = (unsigned char)a;
@@ -1363,7 +1370,7 @@ extern "C" int32_t vb_shuffle_set_hint(vb_shuf *s, uint64_t d)
 extern "C" int32_t vb_shuffle_set_dist(vb_shuf *s, uint32_t rank, uint32_t world)
 {
     if (!s || world < 1 || rank >= world || world > 256) return set_err(VB_ERR_INVALID, "bad rank/world");
-    if (s->multi && world > 1) return reject_multi(s, "multi-rank use (the exchange moves one value column)");
+    if (s->multi && (world > 1 || s->world > 1)) return reject_multi(s, "multi-rank use through vb_shuffle_set_dist (vb_shuffle_create_multi_dist is)");
     if (s->str && (world > 1 || s->world > 1)) return reject_str(s, "multi-rank use through vb_shuffle_set_dist (vb_shuffle_create_str_dist is)");
     s->rank = rank;
     s->world = world;
@@ -2465,6 +2472,210 @@ static int exchange_p2p_locked(vb_shuf *s)
 }
 
 
+// ---------------------------------------------------------------------------------------------
+// combine_by_key across ranks (vb_shuffle_create_multi_dist): each rank exports one row per distinct key it holds,
+// the key plus the partial of every accumulator in plain value form, packed by destination rank; the owner merges the
+// received partials into a fresh table (hash_agg_multi_kernel<IN_ACCS>) and finalizes it as the one-process seal does.
+// ---------------------------------------------------------------------------------------------
+extern "C" int32_t vb_shuffle_create_multi_dist(vb_ctx *c, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce, int32_t kdt,
+                                                uint32_t n_val_cols, const int32_t *val_dtypes, uint32_t n_aggs, const vb_agg_col *aggs,
+                                                uint32_t rank, uint32_t world, vb_shuf **out)
+{
+    if (!c || !out) return set_err(VB_ERR_INVALID, "vb_shuffle_create_multi_dist: NULL argument");
+    *out = nullptr;
+    if (world < 1 || world > 256 || rank >= world) return set_err(VB_ERR_INVALID, "bad rank %u / world %u (1 <= world <= 256)", rank, world);
+    TRY(vb_shuffle_create_multi(c, shuffle_id, n_map, n_reduce, kdt, n_val_cols, val_dtypes, n_aggs, aggs, out));
+    (*out)->rank = rank;
+    (*out)->world = world;
+    return VB_OK;
+}
+
+// the checks every _cols export / import call makes first
+static int multi_dist_check(const vb_shuf *s, const char *what)
+{
+    if (!s->multi) return set_err(VB_ERR_INVALID, "%s needs a shuffle from vb_shuffle_create_multi_dist", what);
+    if (s->world < 2) return set_err(VB_ERR_STATE, "%s needs a multi-aggregate shuffle of world > 1 (vb_shuffle_create_multi_dist)", what);
+    return VB_OK;
+}
+
+// Merge the local map tables and split the merged table's keys by owner rank: count, read the counts back, then one
+// scatter of the key and every accumulator column with the exact exported total as column stride.  Caller holds c->mu.
+static int export_cols_locked(vb_shuf *s, u64 *counts)
+{
+    vb_ctx *c = s->ctx;
+    {
+        std::lock_guard<std::mutex> g(s->mu);
+        if (s->sealed || s->sealing || s->exported || s->freed) return set_err(VB_ERR_STATE, "export after seal/export");
+    }
+    const u32 W = s->world;
+    for (u32 d = 0; d < W; ++d) counts[d] = 0;
+    void *tab = nullptr; u32 log_cap = 0; u64 n_ins = 0;
+    TRY(merge_map_tables(s, &tab, &log_cap, &n_ins));
+    if (tab) {
+        DevBuf guard(c); guard.p = tab;
+        const Table et = table_at(tab, log_cap);
+        const u64 cap = 1ull << log_cap;
+        DevBuf cc(c);
+        TRY(cc.alloc(2 * TS_MAX_BINS * 4));
+        CU(cudaMemsetAsync(cc.p, 0, 2 * TS_MAX_BINS * 4, c->stream));
+        u32 *cnt = cc.as<u32>(), *cursors = cc.as<u32>() + TS_MAX_BINS;
+        const Digit dg = make_bucket_digit(s, DG_DEST, 0, 0xFFFFFFFFu);
+        const unsigned grid = (unsigned)std::min<u64>((cap + TS_TILE) / TS_TILE, (u64)c->sm_count * 4);
+        {
+            KLaunch kl(s, K_RP_HIST, cap + 1);
+            table_bin_count_kernel<DG_DEST><<<grid, TS_THREADS, 0, c->stream>>>(et.keys, cap, dg, cnt);
+            TRY(kl.done("table_bin_count_kernel"));
+        }
+        u32 *h = (u32 *)c->h_scratch;
+        CU(cudaMemcpyAsync(h, cnt, W * 4, cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaStreamSynchronize(c->stream));
+        u64 total = 0;
+        for (u32 d = 0; d < W; ++d) { counts[d] = h[d]; total += h[d]; }
+        if (total) {
+            DevBuf k(c), a(c);
+            TRY(k.alloc(total * 8));
+            TRY(a.alloc(total * 8 * s->acc_map.n));
+            KLaunch kl(s, K_RP_SCATTER, cap + 1);
+            table_bin_scatter_multi_kernel<<<grid, TS_THREADS, 0, c->stream>>>(et.keys, et.accs, acc_stride(log_cap), cap, dg, s->acc_map, cnt,
+                                                                               cursors, total, k.as<u64>(), a.as<u64>());
+            TRY(kl.done("table_bin_scatter_multi_kernel"));
+            s->exp_keys = (u64 *)k.release();
+            s->exp_vals = (u64 *)a.release();
+        }
+        CU(cudaStreamSynchronize(c->stream));
+    }
+    std::lock_guard<std::mutex> g(s->mu);
+    s->exported = true;
+    return VB_OK;
+}
+
+extern "C" int32_t vb_shuffle_export_cols_prepare(vb_shuf *s, uint64_t *counts)
+{
+    if (!s || !counts) return set_err(VB_ERR_INVALID, "NULL argument");
+    TRY(multi_dist_check(s, "vb_shuffle_export_cols_prepare"));
+    vb_ctx *c = s->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    return export_cols_locked(s, counts);
+}
+
+extern "C" int32_t vb_shuffle_export_cols_buffers(vb_shuf *s, void **keys, void **accs, uint32_t *n_acc)
+{
+    if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
+    TRY(multi_dist_check(s, "vb_shuffle_export_cols_buffers"));
+    {
+        std::lock_guard<std::mutex> g(s->mu);
+        if (!s->exported || s->sealed || s->freed) return set_err(VB_ERR_STATE, "vb_shuffle_export_cols_buffers needs vb_shuffle_export_cols_prepare first and no seal yet");
+    }
+    if (keys) *keys = s->exp_keys;
+    if (accs) *accs = s->exp_vals;
+    if (n_acc) *n_acc = s->acc_map.n;
+    return VB_OK;
+}
+
+extern "C" int32_t vb_shuffle_import_cols(vb_shuf *s, const void *keys, const void *accs, uint32_t n_acc, const uint64_t *counts)
+{
+    if (!s || !counts) return set_err(VB_ERR_INVALID, "NULL argument");
+    TRY(multi_dist_check(s, "vb_shuffle_import_cols"));
+    if (n_acc != s->acc_map.n) return set_err(VB_ERR_INVALID, "%u accumulator columns imported, the shuffle has %u", n_acc, s->acc_map.n);
+    {
+        std::lock_guard<std::mutex> g(s->mu);
+        if (!s->exported || s->imported || s->sealed || s->sealing || s->freed)
+            return set_err(VB_ERR_STATE, "vb_shuffle_import_cols needs vb_shuffle_export_cols_prepare first, once, and no seal yet");
+    }
+    u64 n = 0;
+    for (u32 r = 0; r < s->world; ++r) n += counts[r];
+    if (n >= 0xFFFFFFFEull) return set_err(VB_ERR_TOO_LARGE, "import of %llu rows (fewer than 2^32 - 2 are supported)", (unsigned long long)n);
+    if (n && (!keys || !accs)) return set_err(VB_ERR_INVALID, "NULL column with a non-zero count");
+    std::lock_guard<std::mutex> g(s->mu);
+    s->imp_keys = (const u64 *)keys;
+    s->imp_vals = (const u64 *)accs;
+    s->imp_n = n;
+    s->imported = true;
+    return VB_OK;
+}
+
+// vb_shuffle_exchange of a multi-aggregate shuffle: export, then ONE all-gather of (counts[world], the spec's
+// fingerprint) per rank and ONE grouped send/recv of the key column and the n_acc accumulator columns of every peer.
+// Every decision after the all-gather is taken from the gathered matrix, which all ranks see alike, so either every
+// rank enters the send/recv group or none does.
+static int exchange_multi_locked(vb_shuf *s)
+{
+    vb_ctx *c = s->ctx;
+    Comm *m = c->comm;
+    const u32 W = m->world, me = m->rank, NA = s->acc_map.n;
+    std::vector<u64> counts(W, 0);
+    auto ms_since = [](std::chrono::steady_clock::time_point t0) { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count(); };
+    auto t0 = std::chrono::steady_clock::now();
+    TRY(export_cols_locked(s, counts.data()));
+    s->xst.prepare_wall_ms += ms_since(t0);
+    t0 = std::chrono::steady_clock::now();
+    const size_t row = (size_t)W + 3;          // counts, then the fingerprint: <= comm_row(W) for W >= 2
+    u64 *h = (u64 *)((char *)c->h_scratch + COMM_HOST_OFF);
+    u64 *hs = h + (size_t)W * row;
+    for (u32 d = 0; d < W; ++d) hs[d] = counts[d];
+    hs[W] = s->acc_map.op;
+    hs[W + 1] = s->acc_map.tx;
+    hs[W + 2] = (u64)NA | (u64)s->key_width << 8 | (u64)s->n_reduce << 32;
+    CU(cudaMemcpyAsync(m->d_send, hs, row * 8, cudaMemcpyHostToDevice, c->stream));
+    NC(g_nccl.AllGather(m->d_send, m->d_recv, row, ncclUint64, m->comm, c->stream));
+    CU(cudaMemcpyAsync(h, m->d_recv, (size_t)W * row * 8, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    s->xst.counts_wall_ms += ms_since(t0);
+    t0 = std::chrono::steady_clock::now();
+    for (u32 p = 1; p < W; ++p)
+        for (u32 i = 0; i < 3; ++i)
+            if (h[p * row + W + i] != h[W + i])
+                return set_err(VB_ERR_INVALID, "rank %u's combine spec differs from rank 0's (accumulators, ops, transforms, key width or n_reduce)", p);
+    for (u32 d = 0; d < W; ++d) {
+        u64 nd = 0;
+        for (u32 p = 0; p < W; ++p) nd += h[p * row + d];
+        if (nd >= 0xFFFFFFFEull) return set_err(VB_ERR_TOO_LARGE, "rank %u would receive %llu rows", d, (unsigned long long)nd);
+    }
+    std::vector<u64> rcnt(W), soff(W + 1, 0), roff(W + 1, 0);
+    for (u32 p = 0; p < W; ++p) {
+        rcnt[p] = h[p * row + me];
+        soff[p + 1] = soff[p] + counts[p];
+        roff[p + 1] = roff[p] + rcnt[p];
+    }
+    const u64 n_sent = soff[W], n_recv = roff[W];
+    DevBuf rk(c), ra(c);
+    TRY(rk.alloc(std::max<u64>(n_recv, 1) * 8));
+    TRY(ra.alloc(std::max<u64>(n_recv, 1) * 8 * NA));
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    if (c->profile) { cudaEventCreate(&e0); cudaEventCreate(&e1); cudaEventRecord(e0, c->stream); }
+    NC(g_nccl.GroupStart());
+    for (u32 p = 0; p < W; ++p) {
+        if (counts[p]) {
+            NC(g_nccl.Send(s->exp_keys + soff[p], counts[p], ncclUint64, (int)p, m->comm, c->stream));
+            for (u32 a = 0; a < NA; ++a)
+                NC(g_nccl.Send(s->exp_vals + (u64)a * n_sent + soff[p], counts[p], ncclUint64, (int)p, m->comm, c->stream));
+        }
+        if (rcnt[p]) {
+            NC(g_nccl.Recv(rk.as<u64>() + roff[p], rcnt[p], ncclUint64, (int)p, m->comm, c->stream));
+            for (u32 a = 0; a < NA; ++a)
+                NC(g_nccl.Recv(ra.as<u64>() + (u64)a * n_recv + roff[p], rcnt[p], ncclUint64, (int)p, m->comm, c->stream));
+        }
+    }
+    NC(g_nccl.GroupEnd());
+    if (e0) {
+        cudaEventRecord(e1, c->stream);
+        s->timers.push_back(Timer{e0, e1, -3, 0});
+    }
+    s->xst.post_wall_ms += ms_since(t0);
+    s->xst.sent_rows += n_sent - counts[me];
+    s->xst.recv_rows += n_recv - rcnt[me];
+    s->xst.exchanges += 1;
+    s->xst.kind = VB_XCHG_NCCL;
+    s->imp_own_k = (u64 *)rk.release();
+    s->imp_own_v = (u64 *)ra.release();
+    std::lock_guard<std::mutex> g(s->mu);
+    s->imp_keys = s->imp_own_k; s->imp_vals = s->imp_own_v; s->imp_n = n_recv;
+    s->imported = true;
+    return VB_OK;
+}
+
+
 // ---- multi-rank sort_by_key -----------------------------------------------------------------------------------
 // (no reference code: sort_by_key is absent from vega, SURVEY.md F2 — semantics = the single-GPU ones: output
 // partition p is the p-th contiguous key range, cut at floor(p*N/R) moved past equal keys, stable.)
@@ -2620,7 +2831,8 @@ static int exchange_sort_locked(vb_shuf *s)
 extern "C" int32_t vb_shuffle_exchange(vb_shuf *s, int32_t mode)
 {
     if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
-    if (s->multi) return reject_multi(s, "multi-rank exchange");
+    if (s->multi && s->world < 2) return reject_multi(s, "an exchange of a one-process shuffle (vb_shuffle_create_multi_dist has world > 1)");
+    if (s->multi && mode == VB_XCHG_P2P) return reject_multi(s, "the fused P2P exchange (VB_XCHG_NCCL is supported)");
     if (s->str && s->world < 2) return reject_str(s, "an exchange of a one-process shuffle (vb_shuffle_create_str_dist has world > 1)");
     if (s->str && mode == VB_XCHG_P2P) return reject_str(s, "the fused P2P exchange (VB_XCHG_NCCL is supported)");
     vb_ctx *c = s->ctx;
@@ -2628,10 +2840,10 @@ extern "C" int32_t vb_shuffle_exchange(vb_shuf *s, int32_t mode)
     if (!c->comm) return set_err(VB_ERR_STATE, "vb_shuffle_exchange needs vb_ctx_comm_init");
     if (c->comm->world != s->world || c->comm->rank != s->rank) return set_err(VB_ERR_INVALID, "shuffle rank/world differ from the communicator's");
     if (mode < VB_XCHG_AUTO || mode > VB_XCHG_P2P) return set_err(VB_ERR_INVALID, "bad exchange mode");
-    if (s->str) {
+    if (s->str || s->multi) {
         std::lock_guard<std::mutex> lk(c->mu);
         CU(cudaSetDevice(c->device));
-        return exchange_str_locked(s);
+        return s->str ? exchange_str_locked(s) : exchange_multi_locked(s);
     }
     if (mode == VB_XCHG_AUTO) mode = is_group_op(s->agg) ? VB_XCHG_P2P : VB_XCHG_NCCL;
     if (mode == VB_XCHG_P2P && !is_group_op(s->agg)) return set_err(VB_ERR_UNSUPPORTED, "the fused P2P exchange is for GROUP/COGROUP shuffles");
@@ -2943,8 +3155,9 @@ extern "C" int32_t vb_shuffle_seal(vb_shuf *s)
                     void *tab = nullptr; u32 log_cap = 0; u64 n_ins = 0;
                     if (s->imp_n) {
                         std::vector<AggInput> in(1);
-                        in[0] = AggInput{IN_SOA, s->imp_keys, s->imp_vals, s->imp_n, VB_DEVICE};
-                        TRY(build_table(s, K_MERGE, in, merge_opk(s), TX_NONE, s->hint, &tab, &log_cap, &n_ins, nullptr));
+                        in[0] = AggInput{s->multi ? IN_ACCS : IN_SOA, s->imp_keys, s->imp_vals, s->imp_n, VB_DEVICE};
+                        TRY(build_table(s, K_MERGE, in, merge_opk(s), TX_NONE, s->hint, &tab, &log_cap, &n_ins, nullptr,
+                                        s->multi ? &s->acc_imp : nullptr));
                     }
                     DevBuf guard(c); guard.p = tab;
                     TRY(finalize_reduce(s, tab, log_cap, n_ins));

@@ -46,7 +46,7 @@ struct TableCtl {
     unsigned long long n_inserted;
 };
 
-enum : int { IN_AOS = 0, IN_SOA = 1, IN_TABLE = 2 };
+enum : int { IN_AOS = 0, IN_SOA = 1, IN_TABLE = 2, IN_ACCS = 3 };   // IN_ACCS: received partials (hash_agg_multi_kernel)
 enum : int { OPK_ADD_U64 = 0, OPK_ADD_F64 = 1, OPK_MIN_U64 = 2, OPK_MAX_U64 = 3, OPK_COUNT = 4, OPK_DICT = 5 };
 
 VB_HD u64 op_identity(int opk) { return opk == OPK_MIN_U64 ? ~0ull : 0ull; }
@@ -541,8 +541,8 @@ struct AccSpec {
 VB_HD int spec_at(u64 packed, int a) { return (int)(packed >> (8 * a)) & 0xFF; }
 VB_HD void spec_set(u64 &packed, int a, int v) { packed = (packed & ~(0xFFull << (8 * a))) | ((u64)(v & 0xFF) << (8 * a)); }
 struct MaCols {
-    const u64 *c[MA_MAX_COLS];           // value columns (IN_TABLE: c[0] = the source table's first accumulator column)
-    u64 stride;                          // IN_TABLE: distance between the source's accumulator columns
+    const u64 *c[MA_MAX_COLS];           // value columns (IN_TABLE / IN_ACCS: c[0] = the source's first accumulator column)
+    u64 stride;                          // IN_TABLE / IN_ACCS: distance between the source's accumulator columns
 };
 VB_HD size_t table_bytes_multi(u32 log_cap, u32 n_acc) { return (((size_t)1 << log_cap) + BUCKET) * 8 * (1 + n_acc); }
 VB_HD u64 acc_stride(u32 log_cap) { return (1ull << log_cap) + BUCKET; }
@@ -602,7 +602,8 @@ __global__ void table_init_multi_kernel(Table t, AccSpec sp)
 }
 
 // Special key, hot-key cache, probe + one RED per accumulator for ROWS rows of a thread.  IN_SOA: v[c][j] is the
-// value of column c; IN_TABLE (merge): v[0][j] is the source slot, whose accumulators are read at the RED.
+// value of column c; IN_TABLE (merge): v[0][j] is the source slot, whose accumulators are read at the RED; IN_ACCS
+// (import merge): v[0][j] is the received row, whose plain-value partials are read at the RED and order-transformed.
 template <int IN, int NV, int ROWS, bool CACHE>
 VB_D void ma_process_rows(const Table &t, TableCtl *ctl, const AccSpec &sp, const MaCols &src, u64 (&k)[ROWS], u64 (&v)[NV][ROWS],
                           bool (&ok)[ROWS], u64 *hc_keys, u64 *hc_acc, bool use_cache, u32 &my_inserts, u32 &my_hits)
@@ -615,8 +616,10 @@ VB_D void ma_process_rows(const Table &t, TableCtl *ctl, const AccSpec &sp, cons
 #pragma unroll 1
         for (int a = 0; a < n_acc; ++a) {
             const int op = spec_at(ops, a);
-            const u64 x = IN == IN_TABLE ? ld_cg_u64(src.c[0] + (u64)a * src.stride + v[0][j])
-                                         : ma_prep(ma_pick<NV, ROWS>(v, spec_at(srcs, a), j), op, spec_at(txs, a));
+            u64 x;
+            if constexpr (IN == IN_TABLE) x = ld_cg_u64(src.c[0] + (u64)a * src.stride + v[0][j]);
+            else if constexpr (IN == IN_ACCS) x = ma_prep(ld_cg_u64(src.c[0] + (u64)a * src.stride + v[0][j]), op, spec_at(txs, a));
+            else x = ma_prep(ma_pick<NV, ROWS>(v, spec_at(srcs, a), j), op, spec_at(txs, a));
             op_red_rt(base + (u64)a * col_stride, op, x);
         }
     };
@@ -692,14 +695,17 @@ VB_D bool ma_check(TableCtl *ctl, u64 max_inserts, u32 iter, u32 tile_rows, u32 
     return *s_abort != 0;
 }
 
-// Register-staged multi-aggregate combine: IN_SOA (keys + NV value columns) or IN_TABLE (merge of a per-map
-// table of the same spec: NV = 1, sp = the merge spec).  Dynamic shared memory: the hot-key cache (IN_SOA).
+// Register-staged multi-aggregate combine: IN_SOA (keys + NV value columns), IN_TABLE (merge of a per-map
+// table of the same spec: NV = 1, sp = the merge spec) or IN_ACCS (merge of partials received from other ranks:
+// keys[n] + accumulator a of row i at cols.c[0][a * n + i] in plain value form, NV = 1, sp = the merge ops with the
+// map spec's order transforms; every row is a real key, and a key arrives at most once per rank, so no hot-key
+// cache).  Dynamic shared memory: the hot-key cache (IN_SOA).
 template <int IN, int NV>
 __global__ void __launch_bounds__(HA_THREADS, 2)
 hash_agg_multi_kernel(const u64 *__restrict__ keys, MaCols cols, u64 n, Table t, AccSpec sp, TableCtl *ctl, u64 max_inserts)
 {
-    static_assert(IN == IN_SOA || (IN == IN_TABLE && NV == 1), "SoA rows or a table merge");
-    constexpr bool CACHE = (IN != IN_TABLE);
+    static_assert(IN == IN_SOA || ((IN == IN_TABLE || IN == IN_ACCS) && NV == 1), "SoA rows, a table merge or received partials");
+    constexpr bool CACHE = (IN == IN_SOA);
     constexpr int ROWS = ma_rows<NV>();
     constexpr int TILE = HA_THREADS * ROWS;
     extern __shared__ __align__(16) u64 ma_cache[];          // hc_keys[MA_HC_SLOTS], hc_acc[n][MA_HC_SLOTS]
@@ -730,6 +736,8 @@ hash_agg_multi_kernel(const u64 *__restrict__ keys, MaCols cols, u64 n, Table t,
 #pragma unroll
                     for (int c = 0; c < NV; ++c)
                         if (cols.c[c]) v[c][j] = ld_stream_u64(cols.c[c] + idx, pol);
+                } else if (IN == IN_ACCS) {
+                    v[0][j] = idx;
                 } else {
                     v[0][j] = idx;
                     if (idx == n - 1) { ok[j] = (k[j] == 1ull); k[j] = EMPTY_KEY; }   // special slot
@@ -1394,6 +1402,60 @@ table_bin_scatter_kernel(const u64 *__restrict__ keys, const u64 *__restrict__ a
             const u32 o = tile_base[br[j] & 0xFFu] + (br[j] >> 8);
             out_keys[o] = key[j];
             out_vals[o] = val[j];
+        }
+        tile_cnt[tid] = 0;
+        __syncthreads();
+    }
+}
+
+// The same split of a multi-aggregate table by owner rank (combine_by_key export): the key and every accumulator
+// column, destination-major.  Accumulator a of output row o goes to out_accs[a * total + o] in plain value form
+// (tx_inv with its own order transform; total = the exported rows, from table_bin_count_kernel's counts); stride is
+// the distance between the table's accumulator columns.
+__global__ void __launch_bounds__(TS_THREADS)
+table_bin_scatter_multi_kernel(const u64 *__restrict__ keys, const u64 *__restrict__ accs, u64 stride, u64 cap, Digit dg, AccSpec sp,
+                               const u32 *__restrict__ counts, u32 *__restrict__ cursors, u64 total, u64 *__restrict__ out_keys,
+                               u64 *__restrict__ out_accs)
+{
+    __shared__ u32 base[TS_MAX_BINS], tile_cnt[TS_MAX_BINS], tile_base[TS_MAX_BINS], ws[TS_THREADS / 32];
+    const u32 tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    {
+        const u32 c = counts[tid];
+        u32 incl = c;
+#pragma unroll
+        for (int off = 1; off < 32; off <<= 1) { const u32 t = __shfl_up_sync(0xffffffffu, incl, off); if (lane >= (u32)off) incl += t; }
+        if (lane == 31) ws[warp] = incl;
+        __syncthreads();
+        u32 b = 0;
+        for (u32 w = 0; w < warp; ++w) b += ws[w];
+        base[tid] = b + incl - c;
+        tile_cnt[tid] = 0;
+    }
+    __syncthreads();
+    const u64 n_tiles = (cap + 1 + TS_TILE - 1) / TS_TILE;
+    for (u64 tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        u64 key[TS_ITEMS], slot[TS_ITEMS];
+        u32 br[TS_ITEMS];
+#pragma unroll
+        for (int j = 0; j < TS_ITEMS; ++j) {
+            const u64 i = tile * TS_TILE + (u64)j * TS_THREADS + tid;
+            u32 bin;
+            br[j] = 0xFFFFFFFFu;
+            if (ts_load<DG_DEST>(keys, cap, i, dg, key[j], bin)) {
+                slot[j] = i;
+                br[j] = bin | (atomicAdd(&tile_cnt[bin], 1u) << 8);
+            }
+        }
+        __syncthreads();
+        { const u32 c = tile_cnt[tid]; if (c) tile_base[tid] = base[tid] + atomicAdd(&cursors[tid], c); }
+        __syncthreads();
+#pragma unroll
+        for (int j = 0; j < TS_ITEMS; ++j) {
+            if (br[j] == 0xFFFFFFFFu) continue;
+            const u64 o = tile_base[br[j] & 0xFFu] + (br[j] >> 8);
+            out_keys[o] = key[j];
+#pragma unroll 1
+            for (int a = 0; a < (int)sp.n; ++a) out_accs[(u64)a * total + o] = tx_inv(accs[(u64)a * stride + slot[j]], spec_at(sp.tx, a));
         }
         tile_cnt[tid] = 0;
         __syncthreads();

@@ -11,7 +11,8 @@ source-rank-major receive order IS map-id order (group value order, SURVEY.md F5
 
 reduce ops exchange *combined* rows (≤ distinct keys per rank — map-side combine,
 src/dependency.rs:203-209), group ops exchange raw rows.  String keys (StrCudaEngine, run_str_shuffle) travel as four
-columns instead of two: u32 key lengths, key bytes, u32 value counts (GROUP) and u64 values.
+columns instead of two: u32 key lengths, key bytes, u32 value counts (GROUP) and u64 values.  combine_by_key
+(CombineCudaEngine, run_combine_shuffle) sends one row per distinct key: the key and the partial of every accumulator.
 
 The exchange itself lives in libvega_b200.so (vb_ctx_comm_init + vb_shuffle_exchange: NCCL grouped
 send/recv, or the fused peer-memory scatter, on the library's stream).  `run_shuffle` calls it whenever the
@@ -300,6 +301,102 @@ def run_str_shuffle(engine, local_maps, n_map, n_reduce, vcode, agg, rank, world
             stats["recv_rows"] = sum(rcounts[2]) - rcounts[2][rank]
             stats["exchanges"] = stats.get("exchanges", 0) + 1
         engine.import_(sh, rcols, rcounts)
+    engine.seal(sh)
+    return sh
+
+
+class CombineCudaEngine:
+    """libvega_b200 on this rank's GPU, for combine_by_key: CudaEngine's calls over vb_shuffle_create_multi_dist.
+    multi is Shuffle's (value column dtype codes, [(vb_agg, column), ...]).  export gives (counts per destination, keys,
+    accs), accs an (n_acc, rows) view, the wire columns of include/vega_b200.h; import_ takes the same, source-rank major."""
+
+    def __init__(self, sc):
+        self.sc = sc
+
+    def create(self, n_map, n_reduce, kcode, multi, rank, world, key_width=8, hint=0):
+        return Shuffle.combine_dist(self.sc, n_map, n_reduce, kcode, multi, rank, world, key_width=key_width, hint=hint)
+
+    def map(self, sh, map_id, keys, cols):
+        """keys and every value column: numpy arrays or torch CUDA tensors of one location."""
+        k = keys if isinstance(keys, _Col) else _Col(keys)
+        cs = tuple(c if isinstance(c, _Col) else _Col(c, role="value") for c in cols)
+        sh.map_cols(map_id, k, cs, 0, k.n)
+
+    def export(self, sh, world):
+        return sh.export_cols()
+
+    def import_(self, sh, keys, accs, counts):
+        sh.import_cols(keys, accs, counts)
+
+    def seal(self, sh):
+        sh.seal()
+
+    def reduce(self, sh, r, out_dtypes):
+        return sh.reduce_cols(r, out_dtypes)
+
+
+def all_to_all_v_cols(keys, accs, counts, group=None):
+    """The combine_by_key exchange step: one all_to_all_single of the counts, then one of the rows, each row the key
+    and its n_acc partials.  keys[rows] and accs[n_acc][rows] are destination-major; returns (keys, accs, counts)
+    received, source-rank major, in the same shapes."""
+    import torch
+    import torch.distributed as dist
+    dev = keys.device
+    cin = torch.tensor(counts, dtype=torch.int64, device=dev)
+    cout = torch.empty_like(cin)
+    dist.all_to_all_single(cout, cin, group=group)
+    rcounts = [int(x) for x in cout.tolist()]
+    rows = torch.cat([keys.view(-1, 1), accs.t()], dim=1).contiguous()          # [rows][1 + n_acc]
+    out = torch.empty((sum(rcounts), rows.shape[1]), dtype=rows.dtype, device=dev)
+    dist.all_to_all_single(out, rows, output_split_sizes=rcounts, input_split_sizes=list(counts), group=group)
+    return out[:, 0].contiguous(), out[:, 1:].t().contiguous(), rcounts
+
+
+def run_combine_shuffle(engine, local_maps, n_map, n_reduce, kcode, multi, rank, world, group=None, key_width=8, hint=0,
+                        stats=None, exchange_device=None):
+    """run_shuffle for combine_by_key: map side on this rank's partitions → exchange → reduce side for the partitions
+    this rank owns.  local_maps: [(map_id, keys, value columns)], ascending map ids from map_block(rank, world, n_map).
+    With a communicator on the context the exchange is vb_shuffle_exchange (NCCL inside the library); otherwise one
+    all-to-all-v of the 1 + n_acc columns after the count swap (exchange_device: "cpu" for a gloo group on a one-GPU
+    box)."""
+    if not 0 <= rank < world <= 256:
+        raise ValueError(f"rank {rank} of world {world}: 0 <= rank < world <= 256")
+    lo, hi = map_block(rank, world, n_map)
+    ids = [m for m, _, _ in local_maps]
+    if any(not lo <= m < hi for m in ids) or ids != sorted(set(ids)):
+        raise ValueError(f"rank {rank} runs map tasks {ids}: ascending ids in its block [{lo}, {hi}) expected")
+    sh = engine.create(n_map, n_reduce, kcode, multi, rank, world, key_width=key_width, hint=hint)
+    for map_id, keys, cols in local_maps:
+        engine.map(sh, map_id, keys, cols)
+    if world > 1 and isinstance(engine, CombineCudaEngine) and getattr(engine.sc, "comm", None) and exchange_device is None:
+        sh.exchange(L.VB_XCHG_NCCL)
+        engine.seal(sh)
+        if stats is not None:
+            for k_, v_ in sh.exchange_stats().items():
+                stats[k_] = (stats.get(k_, 0) + v_) if k_ in ("exchange_ms", "exchanges", "prepare_wall_ms", "counts_wall_ms", "post_wall_ms") else v_
+        return sh
+    if world > 1:
+        counts, keys, accs = engine.export(sh, world)
+        home = keys.device
+        if exchange_device is not None:
+            keys, accs = keys.to(exchange_device), accs.to(exchange_device)
+        ev = None
+        if stats is not None and keys.is_cuda:
+            import torch
+            ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
+            ev[0].record()
+        rk, ra, rcounts = all_to_all_v_cols(keys, accs, counts, group)
+        if ev is not None:
+            ev[1].record()
+            ev[1].synchronize()
+            stats["exchange_ms"] = stats.get("exchange_ms", 0.0) + ev[0].elapsed_time(ev[1])
+        if exchange_device is not None:
+            rk, ra = rk.to(home), ra.to(home)
+        if stats is not None:
+            stats["sent_rows"] = sum(counts) - counts[rank]
+            stats["recv_rows"] = sum(rcounts) - rcounts[rank]
+            stats["exchanges"] = stats.get("exchanges", 0) + 1
+        engine.import_(sh, rk, ra, rcounts)
     engine.seal(sh)
     return sh
 

@@ -261,6 +261,61 @@ class Shuffle:
             L.check(self._lib.vb_shuffle_set_dist(h, rank, world))
 
     @classmethod
+    def combine_dist(cls, sc, n_map, n_reduce, kcode, multi, rank, world, key_width=8, hint=0):
+        """vb_shuffle_create_multi_dist: the multi-aggregate shuffle `multi` (as for Shuffle) on rank `rank` of `world`.
+        Exchange it with export_cols / import_cols, or with exchange() when the context has a communicator."""
+        self = cls.__new__(cls)
+        self.sc, self._lib = sc, sc._lib
+        self.n_map, self.n_reduce, self.agg, self.vcode, self.kcode = n_map, n_reduce, L.VB_AGG_SUM, L.VB_U64, kcode
+        self.rank, self.world = rank, world
+        self.has_payload, self._keepalive = True, []
+        codes, aggs = multi
+        dts = (ctypes.c_int32 * len(codes))(*codes)
+        spec = (L.vb_agg_col * len(aggs))(*[L.vb_agg_col(a, c) for a, c in aggs])
+        h = ctypes.c_void_p()
+        L.check(self._lib.vb_shuffle_create_multi_dist(sc._h, sc.new_shuffle_id(), n_map, n_reduce, kcode, len(codes), dts,
+                                                       len(aggs), spec, rank, world, ctypes.byref(h)))
+        self._h = h
+        sc._shuffles.add(self)
+        if key_width != 8:
+            L.check(self._lib.vb_shuffle_set_key_width(h, key_width))
+        if hint:
+            L.check(self._lib.vb_shuffle_set_hint(h, hint))
+        return self
+
+    def export_cols(self):
+        """vb_shuffle_export_cols_prepare + buffers (combine_dist, world > 1): (counts, keys, accs).  counts has one entry
+        per destination rank; keys (int64, rows) and accs (int64, (n_acc, rows)) are torch views of the library's device
+        buffers, destination-major, in the wire format of include/vega_b200.h and valid until seal."""
+        import torch
+        cnt = (ctypes.c_uint64 * self.world)()
+        L.check(self._lib.vb_shuffle_export_cols_prepare(self._h, cnt))
+        counts = [int(x) for x in cnt]
+        kp, ap, na = ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_uint32()
+        L.check(self._lib.vb_shuffle_export_cols_buffers(self._h, ctypes.byref(kp), ctypes.byref(ap), ctypes.byref(na)))
+        dev = f"cuda:{self._lib.vb_ctx_device(self.sc._h)}"
+        n, A = sum(counts), na.value
+        if n == 0:
+            return counts, torch.empty(0, dtype=torch.int64, device=dev), torch.empty((A, 0), dtype=torch.int64, device=dev)
+        keys = torch.as_tensor(_DevView(kp.value, n, "<i8"), device=dev)
+        accs = torch.as_tensor(_DevView(ap.value, A * n, "<i8"), device=dev).view(A, n)
+        return counts, keys, accs
+
+    def import_cols(self, keys, accs, counts):
+        """vb_shuffle_import_cols: the received keys (rows) and accumulators ((n_acc, rows), both torch CUDA tensors,
+        source-rank major) and the row count every source rank sent.  The tensors are kept alive until seal."""
+        import torch
+        if accs.dim() != 2 or accs.shape[1] != keys.numel() or len(counts) != self.world or sum(counts) != keys.numel():
+            raise ValueError(f"import of {keys.numel()} keys, accumulators of shape {tuple(accs.shape)} and counts {list(counts)} "
+                             f"on a world of {self.world}: (n_acc, keys) accumulators and one count per rank expected")
+        accs = accs.contiguous()
+        if keys.is_cuda:
+            torch.cuda.current_stream(keys.device).synchronize()       # the library reads on its own stream
+        self._keepalive.append((keys, accs))
+        p = lambda t: ctypes.c_void_p(t.data_ptr()) if t.numel() else None
+        L.check(self._lib.vb_shuffle_import_cols(self._h, p(keys), p(accs), accs.shape[0], (ctypes.c_uint64 * len(counts))(*counts)))
+
+    @classmethod
     def narrow(cls, parent, out_col, vcode):
         """vb_shuffle_create_narrow: the sealed reduce result `parent` (output column out_col) as a sealed COGROUP side
         under the same partitioner, each key with the one-element list [its result] (vcode: the result's dtype)."""
