@@ -1,7 +1,8 @@
 """W ranks of one shuffle in one process (test infrastructure).
 
-Export and import are plain buffers plus host counts, so W shuffles created with set_dist(rank, W) can swap their rows
-with a few torch.cat calls: the all-to-all-v of vega_b200/dist.py without a second process or GPU.  `run_ranks` drives
+Export and import are plain buffers plus host counts, so W shuffles created with set_dist(rank, W) can swap their columns
+with a few torch.cat calls (swap_columns, used by the integer, String and combine_by_key harnesses): the all-to-all-v of
+vega_b200/dist.py without a second process or GPU.  `run_ranks` drives
 any engine with the five calls of vega_b200.dist.CudaEngine (create, map, export, import_, seal): the library itself,
 or tests/fake_engine.FakeEngine on the CPU.
 """
@@ -50,21 +51,20 @@ def run_ranks(engine, W, agg, maps, R, kcode, vcode, key_width=8, hint=0, n_map=
     return shs, snaps
 
 
+def swap_columns(exports):
+    """The all-to-all-v of vega_b200/dist.py in one process.  exports[src] = (columns, splits): each column (None
+    allowed) destination-major along its first dimension, cut by splits[i][dst] rows per destination -> per destination
+    (columns, splits[i][src] per source) with the sources concatenated in ascending order (source-rank major: map-id
+    order).  The received columns are new tensors: a rank's exported buffers belong to the library and are freed by
+    that rank's seal."""
+    parts = [[None if c is None else torch.split(c, list(n)) for c, n in zip(cols, splits)] for cols, splits in exports]
+    return [([None if p is None else torch.cat([src[i][d] for src in parts]) for i, p in enumerate(parts[0])],
+             [[splits[i][d] for _, splits in exports] for i in range(len(parts[0]))]) for d in range(len(exports))]
+
+
 def all_to_all_v(exports):
-    """exports[src] = (counts[dst], keys, vals), destination-major -> per destination (keys, vals, counts[src]) with
-    the sources concatenated in ascending order (source-rank major: map-id order).  The received buffers are new
-    tensors: a rank's exported buffers belong to the library and are freed by that rank's seal."""
-    W = len(exports)
-    recv = []
-    for d in range(W):
-        ks, vs, counts = [], [], []
-        for c, k, v in exports:
-            lo = sum(c[:d])
-            ks.append(k[lo:lo + c[d]])
-            vs.append(v[lo:lo + c[d]])
-            counts.append(c[d])
-        recv.append((torch.cat(ks), torch.cat(vs), counts))
-    return recv
+    """exports[src] = (counts[dst], keys, vals), destination-major -> per destination (keys, vals, counts[src])."""
+    return [(k, v, n[0]) for (k, v), n in swap_columns([([k, v], [c, c]) for c, k, v in exports])]
 
 
 def owned_parts(engine, shs, R):

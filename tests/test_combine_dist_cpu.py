@@ -1,5 +1,5 @@
 """world_size-2 gloo test of the combine_by_key exchange's host logic (vega_b200/dist.py: run_combine_shuffle,
-all_to_all_v_cols): the count swap, one row per distinct key carrying the key and every accumulator partial, source-rank
+all_to_all_v): the count swap, one row per distinct key carrying the key and every accumulator partial, source-rank
 major receive order, and partition ownership r % world.  The per-rank compute is a numpy stand-in for
 dist.CombineCudaEngine that speaks the same wire columns (u64 keys, u64 accumulators [n_acc][rows]); on the GPU the same
 run_combine_shuffle drives the library (tests/test_gpu_combine_dist.py)."""
@@ -131,8 +131,9 @@ def test_two_rank_combine_matches_numpy(M, R):
     assert sent == sum(s["recv_rows"] for _, s in per_rank) and sent > 0
 
 
-def test_all_to_all_v_cols_on_one_rank():
-    """The column layout of the exchange step without a peer: rows keep their order, accumulators stay [n_acc][rows]."""
+def test_all_to_all_v_on_one_rank():
+    """The column layout of the combine exchange step without a peer: rows keep their order, accumulators stay
+    [n_acc][rows]."""
     from vega_b200 import dist as vdist
     port = _free_port()
     os.environ["MASTER_ADDR"], os.environ["MASTER_PORT"] = "127.0.0.1", str(port)
@@ -140,7 +141,7 @@ def test_all_to_all_v_cols_on_one_rank():
     try:
         k = torch.arange(5, dtype=torch.int64)
         a = torch.arange(15, dtype=torch.int64).view(3, 5)
-        rk, ra, rc = vdist.all_to_all_v_cols(k, a, [5])
+        rk, ra, rc = vdist._combine_unpack(*vdist.all_to_all_v(*vdist._combine_pack([5], k, a)))
         assert rc == [5] and torch.equal(rk, k) and torch.equal(ra, a)
     finally:
         dist.destroy_process_group()

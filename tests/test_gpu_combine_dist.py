@@ -2,7 +2,7 @@
 against the CPU oracle's single-column references (tests/test_gpu_combine.py:check_combine).  With >= 2 GPUs each rank
 has its own GPU and the exchange is the library's (vb_ctx_comm_init + vb_shuffle_exchange: one grouped NCCL send/recv
 of the key and accumulator columns); on a one-GPU box both ranks share GPU 0 and the columns are staged through gloo on
-the host (run_combine_shuffle's all_to_all_v_cols)."""
+the host (run_combine_shuffle's all_to_all_v)."""
 import os
 import pickle
 import socket

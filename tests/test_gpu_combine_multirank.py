@@ -45,17 +45,8 @@ def n_acc_of(spec):
 def swap(exports):
     """exports[src] = (counts[dst], keys[rows], accs[n_acc][rows]), destination-major -> per destination (keys, accs,
     counts[src]) with the sources concatenated in ascending order.  New tensors: the exported ones die with the seal."""
-    W = len(exports)
-    out = []
-    for d in range(W):
-        ks, accs, counts = [], [], []
-        for c, k, a in exports:
-            lo = sum(c[:d])
-            ks.append(k[lo:lo + c[d]])
-            accs.append(a[:, lo:lo + c[d]])
-            counts.append(c[d])
-        out.append((torch.cat(ks), torch.cat(accs, dim=1), counts))
-    return out
+    recv = MR.swap_columns([([k, a.t()], [c, c]) for c, k, a in exports])
+    return [(k, a.t().contiguous(), n[0]) for (k, a), n in recv]
 
 
 def placer(keys, cols, loc):

@@ -1,7 +1,7 @@
 """String keys on two ranks with the real StrCudaEngine (export by destination rank, import, seal), checked against
 oracle/pyref.py.  With >= 2 GPUs each rank has its own GPU and the exchange is the library's (vb_ctx_comm_init +
 vb_shuffle_exchange: one grouped NCCL send/recv of the four columns); on a one-GPU box both ranks share GPU 0 and the
-columns are staged through gloo on the host (run_str_shuffle's all_to_all_v_str)."""
+columns are staged through gloo on the host (run_str_shuffle's all_to_all_v)."""
 import os
 import pickle
 import socket

@@ -17,6 +17,7 @@ import torch
 import vega_b200 as vb
 from vega_b200 import _lib as L
 from vega_b200 import dist as vdist
+from tests import multirank as MR
 from tests.test_gpu_str_keys import check_parts, key_pool, ref_parts, rows_from_pool
 from tests.test_gpu_str_join import cogroup_part, join_part
 from tests.util import rand_pairs
@@ -34,19 +35,11 @@ def sc():
 
 
 # ---- the W-rank harness ---------------------------------------------------------------------------------------------
-SPLIT = (0, 1, 0, 2)        # the count each column is sliced by: keys, key bytes, keys, values
-
-
 def swap(exports):
     """exports[src] = ((n_keys, n_key_bytes, n_vals) per destination, (key_lens, key_bytes, val_counts, vals)) ->
     per destination (columns, counts per source), the sources concatenated in ascending order."""
-    W = len(exports)
-    split = [[None if c[i] is None else torch.split(c[i], counts[SPLIT[i]]) for i in range(4)] for counts, c in exports]
-    out = []
-    for d in range(W):
-        cols = tuple(None if split[0][i] is None else torch.cat([sp[i][d] for sp in split]) for i in range(4))
-        out.append((cols, tuple([e[0][j][d] for e in exports] for j in range(3))))
-    return out
+    recv = MR.swap_columns([(cols, (nk, nb, nk, nv)) for (nk, nb, nv), cols in exports])
+    return [(tuple(cols), (n[0], n[1], n[3])) for cols, n in recv]
 
 
 def columns(keys, vals, where):

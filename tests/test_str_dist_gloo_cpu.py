@@ -1,4 +1,4 @@
-"""world_size-2 gloo test of the String exchange's host logic (vega_b200/dist.py: run_str_shuffle, all_to_all_v_str):
+"""world_size-2 gloo test of the String exchange's host logic (vega_b200/dist.py: run_str_shuffle, all_to_all_v):
 the swap of three counts per destination, the four columns split by keys, key bytes, keys and values, source-rank
 major receive order (= map-id order), and partition ownership r % world.  The per-rank compute is a small pyref-backed
 stand-in for dist.StrCudaEngine that speaks the same wire columns (u32 key lengths, key bytes, u32 value counts, u64

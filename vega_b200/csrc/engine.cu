@@ -2229,8 +2229,7 @@ static int nccl_load()
 struct Comm {
     ncclComm_t comm = nullptr;
     u32 rank = 0, world = 1;
-    u64 *d_send = nullptr;     // [comm_row(world)]: counts to every destination, arena bytes, arena generation (or a
-                               // string shuffle's key, key byte and value counts to every destination)
+    u64 *d_send = nullptr;     // [comm_row(world)]: this rank's row of the count all-gather (comm_all_gather)
     u64 *d_recv = nullptr;     // [world][comm_row(world)]
     unsigned char *d_hs = nullptr, *d_hr = nullptr;   // IPC handle + generation: 80 bytes, [world] x 80
     std::vector<u64> peer_arena_bytes, peer_gen_seen;
@@ -2238,7 +2237,8 @@ struct Comm {
 };
 constexpr u32 COMM_MAX_WORLD = 64;
 constexpr size_t COMM_HOST_OFF = 256 << 10;   // staging region inside vb_ctx::h_scratch
-// u64 per rank of the count scratch: world + 2 for the integer exchanges, 3 * world for string keys
+// u64 per rank of the count all-gather: world + 2 for integer rows (counts, arena bytes and generation), world + 3 for
+// combine_by_key (counts and the spec's fingerprint), 3 * world for String keys, 2 for sort
 static size_t comm_row(u32 world) { return std::max<size_t>((size_t)world + 2, 3 * (size_t)world); }
 
 static void comm_teardown(vb_ctx *c)
@@ -2315,23 +2315,123 @@ extern "C" int32_t vb_ctx_comm_info(vb_ctx *c, uint32_t *rank, uint32_t *world, 
     return VB_OK;
 }
 
-// All-gather of (counts[world], my arena bytes, my arena generation) — ONE small collective + one D2H —
-// into the pinned staging area.  Returns the matrix as host rows of (world + 2) u64.
-static int comm_gather_counts(vb_ctx *c, const u64 *counts, const u64 **matrix)
+// ---- the exchange, written once -------------------------------------------------------------------------------
+// Every kind runs the same steps: export; ONE all-gather of a row of u64 counts per rank (comm_all_gather); limit
+// checks taken from the gathered matrix for every rank, so all ranks return the same code and either every rank
+// enters the send/recv group or none does; receive buffers; ONE grouped send/recv (post_group); bookkeeping
+// (xchg_done).  The column kinds (integer rows, combine_by_key, String keys) describe their columns to xfers, which
+// splits each by one count vector of the matrix; sort sends per output partition and builds its own transfer list.
+// A failed local allocation after the checks can still leave one rank out of the group: that is not covered.
+
+// All-gather of this rank's row of `len` u64 (at most comm_row(world)) through the pinned staging area: one small
+// collective and one D2H.  Returns the host matrix [world][len].
+static int comm_all_gather(vb_ctx *c, const u64 *row, size_t len, const u64 **matrix)
 {
     Comm *m = c->comm;
     const u32 W = m->world;
+    if (len > comm_row(W)) return set_err(VB_ERR_INVALID, "count row of %zu u64 exceeds the communicator's %zu", len, comm_row(W));
     u64 *h = (u64 *)((char *)c->h_scratch + COMM_HOST_OFF);
-    u64 *hs = h + (size_t)W * (W + 2);
-    for (u32 d = 0; d < W; ++d) hs[d] = counts[d];
-    hs[W] = c->arena_bytes;
-    hs[W + 1] = c->arena_gen;
-    CU(cudaMemcpyAsync(m->d_send, hs, (W + 2) * 8, cudaMemcpyHostToDevice, c->stream));
-    NC(g_nccl.AllGather(m->d_send, m->d_recv, W + 2, ncclUint64, m->comm, c->stream));
-    CU(cudaMemcpyAsync(h, m->d_recv, (size_t)W * (W + 2) * 8, cudaMemcpyDeviceToHost, c->stream));
+    u64 *hs = h + (size_t)W * len;
+    memcpy(hs, row, len * 8);
+    CU(cudaMemcpyAsync(m->d_send, hs, len * 8, cudaMemcpyHostToDevice, c->stream));
+    NC(g_nccl.AllGather(m->d_send, m->d_recv, len, ncclUint64, m->comm, c->stream));
+    CU(cudaMemcpyAsync(h, m->d_recv, (size_t)W * len * 8, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
     *matrix = h;
     return VB_OK;
+}
+
+struct Xfer {   // one transfer of a grouped send/recv: n elements of type dt to (send) or from peer at p
+    bool send;
+    u32 peer;
+    const void *p;
+    u64 n;
+    ncclDataType_t dt;
+};
+
+// Device interval of the exchange, resolved later by vb_shuffle_exchange_stats / vb_shuffle_stats (no host wait here)
+static cudaEvent_t xchg_mark(vb_ctx *c)
+{
+    cudaEvent_t e = nullptr;
+    if (c->profile) { cudaEventCreate(&e); cudaEventRecord(e, c->stream); }
+    return e;
+}
+
+static void xchg_timed(vb_shuf *s, cudaEvent_t e0)
+{
+    if (!e0) return;
+    cudaEvent_t e1 = nullptr;
+    cudaEventCreate(&e1);
+    cudaEventRecord(e1, s->ctx->stream);
+    s->timers.push_back(Timer{e0, e1, -3, 0});
+}
+
+// The one GroupStart ... GroupEnd: every transfer of `xs` with a non-zero count, timed as the exchange
+static int post_group(vb_shuf *s, const std::vector<Xfer> &xs)
+{
+    vb_ctx *c = s->ctx;
+    Comm *m = c->comm;
+    const cudaEvent_t e0 = xchg_mark(c);
+    NC(g_nccl.GroupStart());
+    for (const Xfer &x : xs) {
+        if (!x.n) continue;
+        if (x.send) NC(g_nccl.Send(x.p, x.n, x.dt, (int)x.peer, m->comm, c->stream));
+        else NC(g_nccl.Recv((void *)x.p, x.n, x.dt, (int)x.peer, m->comm, c->stream));
+    }
+    NC(g_nccl.GroupEnd());
+    xchg_timed(s, e0);
+    return VB_OK;
+}
+
+// What rank `me` sends to and receives from every peer by count vector `vec` (entries [vec * W, vec * W + W) of every
+// row) of the gathered matrix, and where each peer's run starts on either side (source-rank major at the receiver)
+struct XSplit { std::vector<u64> send, recv, soff, roff; };   // [W], [W], [W + 1], [W + 1]
+
+static XSplit xsplit(const u64 *mat, size_t len, u32 W, u32 me, u32 vec)
+{
+    XSplit x{std::vector<u64>(W), std::vector<u64>(W), std::vector<u64>(W + 1, 0), std::vector<u64>(W + 1, 0)};
+    for (u32 p = 0; p < W; ++p) {
+        x.send[p] = mat[me * len + (size_t)vec * W + p];
+        x.recv[p] = mat[p * len + (size_t)vec * W + me];
+        x.soff[p + 1] = x.soff[p] + x.send[p];
+        x.roff[p + 1] = x.roff[p] + x.recv[p];
+    }
+    return x;
+}
+
+// One column of a per-peer exchange: element type, send and receive base, and the count vector that splits it
+struct XCol { ncclDataType_t dt; const void *send; void *recv; u32 vec; };
+
+// The transfer list of the column kinds: to and from every peer, each column's run at its offset
+static std::vector<Xfer> xfers(const std::vector<XSplit> &sp, const std::vector<XCol> &cols, u32 W)
+{
+    auto bytes = [](ncclDataType_t dt) -> u64 { return dt == ncclUint8 ? 1 : dt == ncclUint32 ? 4 : 8; };
+    std::vector<Xfer> xs;
+    for (u32 p = 0; p < W; ++p) {
+        for (const XCol &k : cols)
+            xs.push_back(Xfer{true, p, (const char *)k.send + sp[k.vec].soff[p] * bytes(k.dt), sp[k.vec].send[p], k.dt});
+        for (const XCol &k : cols)
+            xs.push_back(Xfer{false, p, (char *)k.recv + sp[k.vec].roff[p] * bytes(k.dt), sp[k.vec].recv[p], k.dt});
+    }
+    return xs;
+}
+
+// vb_shuffle_exchange_stats of one exchange.  Host wall clock of each of the three phases (export, count all-gather,
+// the rest): lap() = ms since t, and t = now.  `sent` and `recv` count what crossed to or from other ranks, in the
+// kind's unit of a row: values for String keys, keys for combine_by_key, rows otherwise.
+static double lap(std::chrono::steady_clock::time_point &t)
+{
+    const auto t0 = t;
+    t = std::chrono::steady_clock::now();
+    return std::chrono::duration<double, std::milli>(t - t0).count();
+}
+
+static void xchg_done(vb_shuf *s, int kind, u64 sent, u64 recv)
+{
+    s->xst.sent_rows += sent;
+    s->xst.recv_rows += recv;
+    s->xst.exchanges += 1;
+    s->xst.kind = kind;
 }
 
 // reduce ops and non-P2P group ops: pack by destination, then ONE grouped send/recv carrying both columns
@@ -2340,53 +2440,31 @@ static int exchange_nccl_locked(vb_shuf *s)
     vb_ctx *c = s->ctx;
     Comm *m = c->comm;
     const u32 W = m->world, me = m->rank;
-    std::vector<u64> counts(W, 0);
-    auto now = [] { return std::chrono::steady_clock::now(); };
-    auto ms_since = [](std::chrono::steady_clock::time_point t0) { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count(); };
-    auto t0 = now();
-    TRY(export_prepare_locked(s, counts.data()));
-    s->xst.prepare_wall_ms += ms_since(t0);
-    t0 = now();
+    const size_t len = (size_t)W + 2;            // counts[W], arena bytes, arena generation
+    std::vector<u64> row(len, 0);
+    auto clk = std::chrono::steady_clock::now();
+    TRY(export_prepare_locked(s, row.data()));
+    s->xst.prepare_wall_ms += lap(clk);
+    row[W] = c->arena_bytes;
+    row[W + 1] = c->arena_gen;
     const u64 *mat = nullptr;
-    TRY(comm_gather_counts(c, counts.data(), &mat));
-    s->xst.counts_wall_ms += ms_since(t0);
-    t0 = now();
-    std::vector<u64> rcnt(W), soff(W + 1, 0), roff(W + 1, 0);
-    for (u32 p = 0; p < W; ++p) {
-        rcnt[p] = mat[(size_t)p * (W + 2) + me];
-        soff[p + 1] = soff[p] + counts[p];
-        roff[p + 1] = roff[p] + rcnt[p];
+    TRY(comm_all_gather(c, row.data(), len, &mat));
+    s->xst.counts_wall_ms += lap(clk);
+    for (u32 d = 0; d < W; ++d) {
+        const u64 nd = xsplit(mat, len, W, d, 0).roff[W];
+        if (nd >= 0xFFFFFFFEull) return set_err(VB_ERR_TOO_LARGE, "rank %u would receive %llu rows", d, (unsigned long long)nd);
     }
-    const u64 n_recv = roff[W];
-    if (n_recv >= 0xFFFFFFFEull) return set_err(VB_ERR_TOO_LARGE, "rank %u would receive %llu rows", me, (unsigned long long)n_recv);
+    const std::vector<XSplit> sp{xsplit(mat, len, W, me, 0)};
+    const u64 n_recv = sp[0].roff[W];
     DevBuf rk(c), rv(c);
     TRY(rk.alloc(std::max<u64>(n_recv, 1) * 8));
     TRY(rv.alloc(std::max<u64>(n_recv, 1) * 8));
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    if (c->profile) { cudaEventCreate(&e0); cudaEventCreate(&e1); cudaEventRecord(e0, c->stream); }
-    NC(g_nccl.GroupStart());
-    for (u32 p = 0; p < W; ++p) {
-        if (counts[p]) {
-            NC(g_nccl.Send(s->exp_keys + soff[p], counts[p], ncclUint64, (int)p, m->comm, c->stream));
-            NC(g_nccl.Send(s->exp_vals + soff[p], counts[p], ncclUint64, (int)p, m->comm, c->stream));
-        }
-        if (rcnt[p]) {
-            NC(g_nccl.Recv(rk.as<u64>() + roff[p], rcnt[p], ncclUint64, (int)p, m->comm, c->stream));
-            NC(g_nccl.Recv(rv.as<u64>() + roff[p], rcnt[p], ncclUint64, (int)p, m->comm, c->stream));
-        }
-    }
-    NC(g_nccl.GroupEnd());
-    if (e0) {       // resolved later (vb_shuffle_exchange_stats / vb_shuffle_stats): no host wait here
-        cudaEventRecord(e1, c->stream);
-        s->timers.push_back(Timer{e0, e1, -3, 0});
-    }
-    s->xst.post_wall_ms += ms_since(t0);
-    s->xst.sent_rows += soff[W] - counts[me];
-    s->xst.recv_rows += n_recv - rcnt[me];
-    s->xst.exchanges += 1;
-    s->xst.kind = VB_XCHG_NCCL;
+    TRY(post_group(s, xfers(sp, {{ncclUint64, s->exp_keys, rk.p, 0}, {ncclUint64, s->exp_vals, rv.p, 0}}, W)));
+    s->xst.post_wall_ms += lap(clk);
+    xchg_done(s, VB_XCHG_NCCL, sp[0].soff[W] - sp[0].send[me], n_recv - sp[0].recv[me]);
     s->imp_own_k = (u64 *)rk.release();
     s->imp_own_v = (u64 *)rv.release();
+    std::lock_guard<std::mutex> g(s->mu);
     s->imp_keys = s->imp_own_k; s->imp_vals = s->imp_own_v; s->imp_n = n_recv;
     s->imported = true;
     return VB_OK;
@@ -2398,25 +2476,29 @@ static int exchange_p2p_locked(vb_shuf *s)
     vb_ctx *c = s->ctx;
     Comm *m = c->comm;
     const u32 W = m->world, me = m->rank;
-    std::vector<u64> counts(W, 0);
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    if (c->profile) { cudaEventCreate(&e0); cudaEventCreate(&e1); cudaEventRecord(e0, c->stream); }
-    TRY(export_counts_locked(s, counts.data()));
+    const size_t len = (size_t)W + 2;            // counts[W], arena bytes, arena generation
+    std::vector<u64> row(len, 0);
+    const cudaEvent_t e0 = xchg_mark(c);
+    auto clk = std::chrono::steady_clock::now();
+    TRY(export_counts_locked(s, row.data()));
+    s->xst.prepare_wall_ms += lap(clk);
+    row[W] = c->arena_bytes;
+    row[W + 1] = c->arena_gen;
     const u64 *mat = nullptr;
-    TRY(comm_gather_counts(c, counts.data(), &mat));
+    TRY(comm_all_gather(c, row.data(), len, &mat));
+    s->xst.counts_wall_ms += lap(clk);
     // arena layout (source-rank major = map-id order) from the count matrix
-    std::vector<u64> total(W, 0), my_off(W, 0), rcnt(W);
+    std::vector<u64> total(W, 0), my_off(W, 0);
     for (u32 dst = 0; dst < W; ++dst)
         for (u32 src = 0; src < W; ++src) {
-            const u64 x = mat[(size_t)src * (W + 2) + dst];
+            const u64 x = mat[src * len + dst];
             if (src < me) my_off[dst] += x;
             total[dst] += x;
         }
-    for (u32 src = 0; src < W; ++src) rcnt[src] = mat[(size_t)src * (W + 2) + me];
     // who must (re)grow its arena is a pure function of the gathered matrix: handles are re-exchanged only then
     bool any_regrow = !m->handles_valid;
     for (u32 p = 0; p < W; ++p) {
-        const u64 need = 16 * std::max<u64>(total[p], 1), have = mat[(size_t)p * (W + 2) + W], gen = mat[(size_t)p * (W + 2) + W + 1];
+        const u64 need = 16 * std::max<u64>(total[p], 1), have = mat[p * len + W], gen = mat[p * len + W + 1];
         if (need > have || gen == 0 || gen != m->peer_gen_seen[p]) any_regrow = true;
     }
     unsigned char hbuf[80];
@@ -2447,27 +2529,17 @@ static int exchange_p2p_locked(vb_shuf *s)
         for (void *p : c->retired_arenas) CU(cudaFree(p));
         c->retired_arenas.clear();
     }
-    u64 n = 0;
-    for (u32 r = 0; r < W; ++r) n += rcnt[r];
+    const XSplit sp = xsplit(mat, len, W, me, 0);
+    const u64 n = sp.roff[W];
     if (n >= 0xFFFFFFFEull) return set_err(VB_ERR_TOO_LARGE, "import of %llu rows", (unsigned long long)n);
+    xchg_timed(s, e0);
+    s->xst.post_wall_ms += lap(clk);
+    xchg_done(s, VB_XCHG_P2P, sp.soff[W] - sp.send[me], n - sp.recv[me]);
+    std::lock_guard<std::mutex> g(s->mu);
     s->imp_keys = (const u64 *)c->arena;
     s->imp_vals = s->imp_keys + n;
     s->imp_n = n;
     s->imported = true;
-    if (e0) {
-        cudaEventRecord(e1, c->stream);
-        cudaEventSynchronize(e1);
-        float ms = 0;
-        cudaEventElapsedTime(&ms, e0, e1);
-        s->xst.exchange_ms += ms;
-        cudaEventDestroy(e0); cudaEventDestroy(e1);
-    }
-    u64 sent = 0;
-    for (u32 p = 0; p < W; ++p) if (p != me) sent += counts[p];
-    s->xst.sent_rows += sent;
-    s->xst.recv_rows += n - rcnt[me];
-    s->xst.exchanges += 1;
-    s->xst.kind = VB_XCHG_P2P;
     return VB_OK;
 }
 
@@ -2595,78 +2667,43 @@ extern "C" int32_t vb_shuffle_import_cols(vb_shuf *s, const void *keys, const vo
     return VB_OK;
 }
 
-// vb_shuffle_exchange of a multi-aggregate shuffle: export, then ONE all-gather of (counts[world], the spec's
-// fingerprint) per rank and ONE grouped send/recv of the key column and the n_acc accumulator columns of every peer.
-// Every decision after the all-gather is taken from the gathered matrix, which all ranks see alike, so either every
-// rank enters the send/recv group or none does.
+// vb_shuffle_exchange of a multi-aggregate shuffle: export, then the exchange of the key column and the n_acc
+// accumulator columns, all split by the key counts.  The gathered row carries the spec's fingerprint after the counts,
+// so a rank whose spec differs is refused on every rank.
 static int exchange_multi_locked(vb_shuf *s)
 {
     vb_ctx *c = s->ctx;
     Comm *m = c->comm;
     const u32 W = m->world, me = m->rank, NA = s->acc_map.n;
-    std::vector<u64> counts(W, 0);
-    auto ms_since = [](std::chrono::steady_clock::time_point t0) { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count(); };
-    auto t0 = std::chrono::steady_clock::now();
-    TRY(export_cols_locked(s, counts.data()));
-    s->xst.prepare_wall_ms += ms_since(t0);
-    t0 = std::chrono::steady_clock::now();
-    const size_t row = (size_t)W + 3;          // counts, then the fingerprint: <= comm_row(W) for W >= 2
-    u64 *h = (u64 *)((char *)c->h_scratch + COMM_HOST_OFF);
-    u64 *hs = h + (size_t)W * row;
-    for (u32 d = 0; d < W; ++d) hs[d] = counts[d];
-    hs[W] = s->acc_map.op;
-    hs[W + 1] = s->acc_map.tx;
-    hs[W + 2] = (u64)NA | (u64)s->key_width << 8 | (u64)s->n_reduce << 32;
-    CU(cudaMemcpyAsync(m->d_send, hs, row * 8, cudaMemcpyHostToDevice, c->stream));
-    NC(g_nccl.AllGather(m->d_send, m->d_recv, row, ncclUint64, m->comm, c->stream));
-    CU(cudaMemcpyAsync(h, m->d_recv, (size_t)W * row * 8, cudaMemcpyDeviceToHost, c->stream));
-    CU(cudaStreamSynchronize(c->stream));
-    s->xst.counts_wall_ms += ms_since(t0);
-    t0 = std::chrono::steady_clock::now();
+    const size_t len = (size_t)W + 3;            // counts[W], then the fingerprint: <= comm_row(W) for W >= 2
+    std::vector<u64> row(len, 0);
+    auto clk = std::chrono::steady_clock::now();
+    TRY(export_cols_locked(s, row.data()));
+    s->xst.prepare_wall_ms += lap(clk);
+    row[W] = s->acc_map.op;
+    row[W + 1] = s->acc_map.tx;
+    row[W + 2] = (u64)NA | (u64)s->key_width << 8 | (u64)s->n_reduce << 32;
+    const u64 *mat = nullptr;
+    TRY(comm_all_gather(c, row.data(), len, &mat));
+    s->xst.counts_wall_ms += lap(clk);
     for (u32 p = 1; p < W; ++p)
         for (u32 i = 0; i < 3; ++i)
-            if (h[p * row + W + i] != h[W + i])
+            if (mat[p * len + W + i] != mat[W + i])
                 return set_err(VB_ERR_INVALID, "rank %u's combine spec differs from rank 0's (accumulators, ops, transforms, key width or n_reduce)", p);
     for (u32 d = 0; d < W; ++d) {
-        u64 nd = 0;
-        for (u32 p = 0; p < W; ++p) nd += h[p * row + d];
+        const u64 nd = xsplit(mat, len, W, d, 0).roff[W];
         if (nd >= 0xFFFFFFFEull) return set_err(VB_ERR_TOO_LARGE, "rank %u would receive %llu rows", d, (unsigned long long)nd);
     }
-    std::vector<u64> rcnt(W), soff(W + 1, 0), roff(W + 1, 0);
-    for (u32 p = 0; p < W; ++p) {
-        rcnt[p] = h[p * row + me];
-        soff[p + 1] = soff[p] + counts[p];
-        roff[p + 1] = roff[p] + rcnt[p];
-    }
-    const u64 n_sent = soff[W], n_recv = roff[W];
+    const std::vector<XSplit> sp{xsplit(mat, len, W, me, 0)};
+    const u64 n_sent = sp[0].soff[W], n_recv = sp[0].roff[W];
     DevBuf rk(c), ra(c);
     TRY(rk.alloc(std::max<u64>(n_recv, 1) * 8));
     TRY(ra.alloc(std::max<u64>(n_recv, 1) * 8 * NA));
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    if (c->profile) { cudaEventCreate(&e0); cudaEventCreate(&e1); cudaEventRecord(e0, c->stream); }
-    NC(g_nccl.GroupStart());
-    for (u32 p = 0; p < W; ++p) {
-        if (counts[p]) {
-            NC(g_nccl.Send(s->exp_keys + soff[p], counts[p], ncclUint64, (int)p, m->comm, c->stream));
-            for (u32 a = 0; a < NA; ++a)
-                NC(g_nccl.Send(s->exp_vals + (u64)a * n_sent + soff[p], counts[p], ncclUint64, (int)p, m->comm, c->stream));
-        }
-        if (rcnt[p]) {
-            NC(g_nccl.Recv(rk.as<u64>() + roff[p], rcnt[p], ncclUint64, (int)p, m->comm, c->stream));
-            for (u32 a = 0; a < NA; ++a)
-                NC(g_nccl.Recv(ra.as<u64>() + (u64)a * n_recv + roff[p], rcnt[p], ncclUint64, (int)p, m->comm, c->stream));
-        }
-    }
-    NC(g_nccl.GroupEnd());
-    if (e0) {
-        cudaEventRecord(e1, c->stream);
-        s->timers.push_back(Timer{e0, e1, -3, 0});
-    }
-    s->xst.post_wall_ms += ms_since(t0);
-    s->xst.sent_rows += n_sent - counts[me];
-    s->xst.recv_rows += n_recv - rcnt[me];
-    s->xst.exchanges += 1;
-    s->xst.kind = VB_XCHG_NCCL;
+    std::vector<XCol> cols{{ncclUint64, s->exp_keys, rk.p, 0}};
+    for (u32 a = 0; a < NA; ++a) cols.push_back({ncclUint64, s->exp_vals + (u64)a * n_sent, ra.as<u64>() + (u64)a * n_recv, 0});
+    TRY(post_group(s, xfers(sp, cols, W)));
+    s->xst.post_wall_ms += lap(clk);
+    xchg_done(s, VB_XCHG_NCCL, n_sent - sp[0].send[me], n_recv - sp[0].recv[me]);
     s->imp_own_k = (u64 *)rk.release();
     s->imp_own_v = (u64 *)ra.release();
     std::lock_guard<std::mutex> g(s->mu);
@@ -2708,6 +2745,7 @@ static int exchange_sort_locked(vb_shuf *s)
         if (s->sealed || s->exported || s->freed) return set_err(VB_ERR_STATE, "export after seal/export");
     }
     const int tx = s->kdt == VB_I64 ? TX_I64 : s->kdt == VB_F64 ? TX_F64 : TX_NONE;
+    auto clk = std::chrono::steady_clock::now();
     // 1. local sort
     Gathered g;
     TRY(gather_maps(s, &g));
@@ -2719,12 +2757,13 @@ static int exchange_sort_locked(vb_shuf *s)
     DevBuf lk_guard(c), lv_guard(c);
     lk_guard.p = lk; lv_guard.p = lv;
     // every rank must agree on whether a payload travels (a rank with zero rows has no way to know locally)
-    std::vector<u64> c0(W, 0);
-    c0[0] = n_local; if (W > 1) c0[1] = has_val ? 1 : 0;
+    s->xst.prepare_wall_ms += lap(clk);
+    const u64 c0[2] = {n_local, has_val ? 1ull : 0ull};
     const u64 *mat = nullptr;
-    TRY(comm_gather_counts(c, c0.data(), &mat));
+    TRY(comm_all_gather(c, c0, 2, &mat));
+    s->xst.counts_wall_ms += lap(clk);
     u64 N = 0; bool any_val = false;
-    for (u32 r = 0; r < W; ++r) { N += mat[(size_t)r * (W + 2)]; if (W > 1 && mat[(size_t)r * (W + 2)] && mat[(size_t)r * (W + 2) + 1]) any_val = true; }
+    for (u32 r = 0; r < W; ++r) { N += mat[2 * r]; if (mat[2 * r] && mat[2 * r + 1]) any_val = true; }
     // 2. exact cut keys: s_p = the key of global rank c_p - 1, c_p = floor(p N / R); rows with key <= s_p go to partitions < p
     const u32 P = R - 1;
     std::vector<u64> need(P), lo(P, 0), hi(P, ~0ull), cut(R + 1, 0);
@@ -2779,51 +2818,46 @@ static int exchange_sort_locked(vb_shuf *s)
     NC(g_nccl.AllGather(d_seg.p, d_segall.p, R, ncclUint64, m->comm, c->stream));
     CU(cudaMemcpyAsync(segall.data(), d_segall.p, (size_t)W * R * 8, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
+    // every rank's receive total, so that all ranks refuse alike
+    for (u32 d = 0; d < W; ++d) {
+        u64 nd = 0;
+        for (u32 p = d; p < R; p += W)
+            for (u32 r = 0; r < W; ++r) nd += segall[(size_t)r * R + p];
+        if (nd >= 0xFFFFFFFEull) return set_err(VB_ERR_TOO_LARGE, "rank %u would receive %llu rows", d, (unsigned long long)nd);
+    }
     s->sort_part_rows.assign(R, 0);
     u64 n_recv = 0;
     for (u32 p = me; p < R; p += W)
         for (u32 r = 0; r < W; ++r) { s->sort_part_rows[p] += segall[(size_t)r * R + p]; n_recv += segall[(size_t)r * R + p]; }
-    if (n_recv >= 0xFFFFFFFEull) return set_err(VB_ERR_TOO_LARGE, "rank %u would receive %llu rows", me, (unsigned long long)n_recv);
     // 4. one grouped send/recv: partition-major, source-rank-major at the receiver
     DevBuf rk(c), rv(c);
     TRY(rk.alloc(std::max<u64>(n_recv, 1) * 8));
     if (any_val) TRY(rv.alloc(std::max<u64>(n_recv, 1) * 8));
     DevBuf zero_v(c);
     if (any_val && !lv && n_local) { TRY(zero_v.alloc(n_local * 8)); CU(cudaMemsetAsync(zero_v.p, 0, n_local * 8, c->stream)); lv = zero_v.as<u64>(); }
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    if (c->profile) { cudaEventCreate(&e0); cudaEventCreate(&e1); cudaEventRecord(e0, c->stream); }
-    NC(g_nccl.GroupStart());
+    std::vector<Xfer> xs;
+    u64 sent = 0, own = 0;
     for (u32 p = 0; p < R; ++p) {
-        if (!seg[p]) continue;
-        NC(g_nccl.Send(lk + cut[p], seg[p], ncclUint64, (int)(p % W), m->comm, c->stream));
-        if (any_val) NC(g_nccl.Send(lv + cut[p], seg[p], ncclUint64, (int)(p % W), m->comm, c->stream));
+        xs.push_back(Xfer{true, p % W, lk + cut[p], seg[p], ncclUint64});
+        if (any_val) xs.push_back(Xfer{true, p % W, lv + cut[p], seg[p], ncclUint64});
+        (p % W == me ? own : sent) += seg[p];
     }
-    u64 off = 0, sent = 0;
+    u64 off = 0;
     for (u32 p = me; p < R; p += W)
         for (u32 r = 0; r < W; ++r) {
             const u64 cnt = segall[(size_t)r * R + p];
-            if (!cnt) continue;
-            NC(g_nccl.Recv(rk.as<u64>() + off, cnt, ncclUint64, (int)r, m->comm, c->stream));
-            if (any_val) NC(g_nccl.Recv(rv.as<u64>() + off, cnt, ncclUint64, (int)r, m->comm, c->stream));
+            xs.push_back(Xfer{false, r, rk.as<u64>() + off, cnt, ncclUint64});
+            if (any_val) xs.push_back(Xfer{false, r, rv.as<u64>() + off, cnt, ncclUint64});
             off += cnt;
         }
-    NC(g_nccl.GroupEnd());
-    if (e0) {
-        cudaEventRecord(e1, c->stream); cudaEventSynchronize(e1);
-        float ms = 0; cudaEventElapsedTime(&ms, e0, e1);
-        s->xst.exchange_ms += ms;
-        cudaEventDestroy(e0); cudaEventDestroy(e1);
-    }
-    for (u32 p = 0; p < R; ++p) if (p % W != me) sent += seg[p];
-    s->xst.sent_rows += sent;
-    s->xst.recv_rows += n_recv - [&] { u64 own = 0; for (u32 p = me; p < R; p += W) own += seg[p]; return own; }();
-    s->xst.exchanges += 1;
-    s->xst.kind = VB_XCHG_NCCL;
+    TRY(post_group(s, xs));
+    s->xst.post_wall_ms += lap(clk);
+    xchg_done(s, VB_XCHG_NCCL, sent, n_recv - own);
     s->imp_own_k = (u64 *)rk.release();
     s->imp_own_v = any_val ? (u64 *)rv.release() : nullptr;
+    std::lock_guard<std::mutex> gg(s->mu);
     s->imp_keys = s->imp_own_k; s->imp_vals = s->imp_own_v; s->imp_n = n_recv;
     s->imported = true;
-    std::lock_guard<std::mutex> gg(s->mu);
     s->exported = true;
     return VB_OK;
 }
@@ -5001,9 +5035,10 @@ extern "C" int32_t vb_shuffle_import_str(vb_shuf *s, const uint32_t *key_lens, c
     return VB_OK;
 }
 
-// vb_shuffle_exchange of a string shuffle: export, then ONE all-gather of the world x 3 world count matrix (keys, key
-// bytes and values to every destination) and ONE grouped send/recv carrying the four columns of every peer, as
-// exchange_nccl_locked does for two.  The received columns are owned by the shuffle until seal.
+// vb_shuffle_exchange of a string shuffle: export, then the exchange of four columns: u32 key lengths and (GROUP)
+// u32 value counts split by the key counts, key bytes by the byte counts, u64 values by the value counts.  The
+// gathered row is the three count vectors (keys, key bytes, values to every destination).  The received columns
+// are owned by the shuffle until seal.
 static int exchange_str_locked(vb_shuf *s)
 {
     vb_ctx *c = s->ctx;
@@ -5011,70 +5046,27 @@ static int exchange_str_locked(vb_shuf *s)
     StrState *t = s->str;
     const u32 W = m->world, me = m->rank;
     const bool group = !is_reduce_op(s->agg);
-    std::vector<u64> cnt(3 * (size_t)W, 0);      // n_keys[W], n_key_bytes[W], n_vals[W]
-    auto ms_since = [](std::chrono::steady_clock::time_point t0) { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count(); };
-    auto t0 = std::chrono::steady_clock::now();
-    TRY(export_str_locked(s, cnt.data(), cnt.data() + W, cnt.data() + 2 * (size_t)W));
-    s->xst.prepare_wall_ms += ms_since(t0);
-    t0 = std::chrono::steady_clock::now();
-    const size_t row = 3 * (size_t)W;
-    u64 *h = (u64 *)((char *)c->h_scratch + COMM_HOST_OFF);
-    u64 *hs = h + (size_t)W * row;
-    memcpy(hs, cnt.data(), row * 8);
-    CU(cudaMemcpyAsync(m->d_send, hs, row * 8, cudaMemcpyHostToDevice, c->stream));
-    NC(g_nccl.AllGather(m->d_send, m->d_recv, row, ncclUint64, m->comm, c->stream));
-    CU(cudaMemcpyAsync(h, m->d_recv, (size_t)W * row * 8, cudaMemcpyDeviceToHost, c->stream));
-    CU(cudaStreamSynchronize(c->stream));
-    s->xst.counts_wall_ms += ms_since(t0);
-    t0 = std::chrono::steady_clock::now();
-    // per peer p: what I send (cnt) and receive (column me of p's row), and where each run starts
-    std::vector<u64> rk(W), rb(W), rv(W), sk(W + 1, 0), sb(W + 1, 0), sv(W + 1, 0), ok(W + 1, 0), ob(W + 1, 0), ov(W + 1, 0);
-    for (u32 p = 0; p < W; ++p) {
-        rk[p] = h[p * row + me];
-        rb[p] = h[p * row + W + me];
-        rv[p] = h[p * row + 2 * (size_t)W + me];
-        sk[p + 1] = sk[p] + cnt[p];
-        sb[p + 1] = sb[p] + cnt[W + p];
-        sv[p + 1] = sv[p] + cnt[2 * (size_t)W + p];
-        ok[p + 1] = ok[p] + rk[p];
-        ob[p + 1] = ob[p] + rb[p];
-        ov[p + 1] = ov[p] + rv[p];
-    }
-    const u64 nk = ok[W], nkb = ob[W], nv = ov[W];
-    TRY(str_import_limits(s, nk, nv));
+    const size_t len = 3 * (size_t)W;            // n_keys[W], n_key_bytes[W], n_vals[W]
+    std::vector<u64> row(len, 0);
+    auto clk = std::chrono::steady_clock::now();
+    TRY(export_str_locked(s, row.data(), row.data() + W, row.data() + 2 * (size_t)W));
+    s->xst.prepare_wall_ms += lap(clk);
+    const u64 *mat = nullptr;
+    TRY(comm_all_gather(c, row.data(), len, &mat));
+    s->xst.counts_wall_ms += lap(clk);
+    for (u32 d = 0; d < W; ++d) TRY(str_import_limits(s, xsplit(mat, len, W, d, 0).roff[W], xsplit(mat, len, W, d, 2).roff[W]));
+    const std::vector<XSplit> sp{xsplit(mat, len, W, me, 0), xsplit(mat, len, W, me, 1), xsplit(mat, len, W, me, 2)};
+    const u64 nk = sp[0].roff[W], nkb = sp[1].roff[W], nv = sp[2].roff[W];
     DevBuf lens(c), bytes(c), cnts(c), vals(c);
     TRY(lens.alloc(nk * 4));
     TRY(bytes.alloc(nkb));
     if (group) TRY(cnts.alloc(nk * 4));
     TRY(vals.alloc(nv * 8));
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    if (c->profile) { cudaEventCreate(&e0); cudaEventCreate(&e1); cudaEventRecord(e0, c->stream); }
-    NC(g_nccl.GroupStart());
-    for (u32 p = 0; p < W; ++p) {
-        const u64 k = cnt[p], b = cnt[W + p], v = cnt[2 * (size_t)W + p];
-        if (k) {
-            NC(g_nccl.Send(t->x_lens + sk[p], k, ncclUint32, (int)p, m->comm, c->stream));
-            if (group) NC(g_nccl.Send(t->x_cnts + sk[p], k, ncclUint32, (int)p, m->comm, c->stream));
-        }
-        if (b) NC(g_nccl.Send(t->x_bytes + sb[p], b, ncclUint8, (int)p, m->comm, c->stream));
-        if (v) NC(g_nccl.Send(t->x_vals + sv[p], v, ncclUint64, (int)p, m->comm, c->stream));
-        if (rk[p]) {
-            NC(g_nccl.Recv(lens.as<u32>() + ok[p], rk[p], ncclUint32, (int)p, m->comm, c->stream));
-            if (group) NC(g_nccl.Recv(cnts.as<u32>() + ok[p], rk[p], ncclUint32, (int)p, m->comm, c->stream));
-        }
-        if (rb[p]) NC(g_nccl.Recv(bytes.as<unsigned char>() + ob[p], rb[p], ncclUint8, (int)p, m->comm, c->stream));
-        if (rv[p]) NC(g_nccl.Recv(vals.as<u64>() + ov[p], rv[p], ncclUint64, (int)p, m->comm, c->stream));
-    }
-    NC(g_nccl.GroupEnd());
-    if (e0) {
-        cudaEventRecord(e1, c->stream);
-        s->timers.push_back(Timer{e0, e1, -3, 0});
-    }
-    s->xst.post_wall_ms += ms_since(t0);
-    s->xst.sent_rows += sv[W] - cnt[2 * (size_t)W + me];
-    s->xst.recv_rows += nv - rv[me];
-    s->xst.exchanges += 1;
-    s->xst.kind = VB_XCHG_NCCL;
+    std::vector<XCol> cols{{ncclUint32, t->x_lens, lens.p, 0}, {ncclUint8, t->x_bytes, bytes.p, 1}, {ncclUint64, t->x_vals, vals.p, 2}};
+    if (group) cols.push_back({ncclUint32, t->x_cnts, cnts.p, 0});
+    TRY(post_group(s, xfers(sp, cols, W)));
+    s->xst.post_wall_ms += lap(clk);
+    xchg_done(s, VB_XCHG_NCCL, sp[2].soff[W] - sp[2].send[me], nv - sp[2].recv[me]);
     t->i_lens = lens.as<u32>(); t->i_bytes = bytes.as<unsigned char>(); t->i_cnts = group ? cnts.as<u32>() : nullptr; t->i_vals = vals.as<u64>();
     t->i_nk = nk; t->i_nkb = nkb; t->i_nv = nv;
     t->i_own[0] = lens.release(); t->i_own[1] = bytes.release(); t->i_own[2] = cnts.release(); t->i_own[3] = vals.release();

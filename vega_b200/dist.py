@@ -3,22 +3,26 @@
 The reference moves shuffle blocks with one HTTP GET per (map, reduce) pair
 (src/shuffle/shuffle_fetcher.rs:61-86 → src/shuffle/shuffle_manager.rs:176-251).  Here every
 rank packs its map output by destination rank on the device (vb_shuffle_export_prepare: a
-stable multisplit, so rows stay in map-id / encounter order), the ranks swap a world×world
-count vector, and ONE all-to-all-v per column (torch.distributed → NCCL grouped send/recv over
-NVLink/NVSwitch; gloo on CPU for the host-logic tests) delivers them.  Reduce partition r is
+stable multisplit, so rows stay in map-id / encounter order) as a few columns, each split by one
+vector of per-destination counts.  The ranks swap the counts and ONE all-to-all-v per column
+(torch.distributed → NCCL grouped send/recv over NVLink/NVSwitch; gloo on CPU for the host-logic
+tests) delivers them: all_to_all_v, the one exchange of every shuffle kind.  Reduce partition r is
 owned by rank r % world; map partitions are assigned to ranks in contiguous blocks so that the
 source-rank-major receive order IS map-id order (group value order, SURVEY.md F5).
 
-reduce ops exchange *combined* rows (≤ distinct keys per rank — map-side combine,
-src/dependency.rs:203-209), group ops exchange raw rows.  String keys (StrCudaEngine, run_str_shuffle) travel as four
-columns instead of two: u32 key lengths, key bytes, u32 value counts (GROUP) and u64 values.  combine_by_key
-(CombineCudaEngine, run_combine_shuffle) sends one row per distinct key: the key and the partial of every accumulator.
+The columns of each kind (run_shuffle, run_str_shuffle and run_combine_shuffle share one driver, _exchange):
+- integer rows (CudaEngine): keys and values, both split by the row counts.  Reduce ops exchange *combined* rows
+  (≤ distinct keys per rank — map-side combine, src/dependency.rs:203-209), group ops raw rows.
+- String keys (StrCudaEngine): u32 key lengths and u32 value counts (GROUP) split by the key counts, key bytes by the
+  byte counts, u64 values by the value counts.
+- combine_by_key (CombineCudaEngine): one row per distinct key, the key and the partial of every accumulator, packed
+  as one [rows][1 + n_acc] column.
 
 The exchange itself lives in libvega_b200.so (vb_ctx_comm_init + vb_shuffle_exchange: NCCL grouped
-send/recv, or the fused peer-memory scatter, on the library's stream).  `run_shuffle` calls it whenever the
-context has a communicator; the torch.distributed code paths below remain for the two cases the library's
-NCCL communicator cannot cover: the CPU (gloo) tests of the host logic with an oracle-backed stand-in engine,
-and two ranks sharing ONE GPU on a single-GPU test box (NCCL refuses duplicate devices).
+send/recv, or the fused peer-memory scatter, on the library's stream).  The run_*shuffle functions call it
+whenever the context has a communicator; the torch.distributed code paths below remain for the two cases the
+library's NCCL communicator cannot cover: the CPU (gloo) tests of the host logic with an oracle-backed stand-in
+engine, and two ranks sharing ONE GPU on a single-GPU test box (NCCL refuses duplicate devices).
 """
 import ctypes
 
@@ -141,21 +145,82 @@ def p2p_exchange(engine, sh, rank, world, group=None, stats=None):
         stats["exchange_kind"] = "p2p"
 
 
-def all_to_all_v(send_keys, send_vals, send_counts, group=None):
-    """The shuffle's single exchange step: counts, then keys and values, each one
-    all_to_all_single.  Returns (recv_keys, recv_vals, recv_counts), source-rank major."""
+def all_to_all_v(cols, splits, group=None):
+    """The shuffle's exchange step over torch.distributed: one all_to_all_single of the stacked counts, then one per
+    column.  cols: tensors (None allowed), destination-major along their first dimension; splits[i]: the rows of
+    cols[i] for every destination.  Returns (received columns, the rows of each received from every source), both
+    source-rank major."""
     import torch
     import torch.distributed as dist
-    dev = send_keys.device
-    cin = torch.tensor(send_counts, dtype=torch.int64, device=dev)
+    dev = next(c for c in cols if c is not None).device
+    cin = torch.tensor(list(zip(*splits)), dtype=torch.int64, device=dev)      # row d: what d gets of every column
     cout = torch.empty_like(cin)
     dist.all_to_all_single(cout, cin, group=group)
-    recv_counts = [int(x) for x in cout.tolist()]
-    rk = torch.empty(sum(recv_counts), dtype=send_keys.dtype, device=dev)
-    rv = torch.empty(sum(recv_counts), dtype=send_vals.dtype, device=dev)
-    dist.all_to_all_single(rk, send_keys, output_split_sizes=recv_counts, input_split_sizes=list(send_counts), group=group)
-    dist.all_to_all_single(rv, send_vals, output_split_sizes=recv_counts, input_split_sizes=list(send_counts), group=group)
-    return rk, rv, recv_counts
+    rsplits = [list(r) for r in zip(*cout.tolist())]                           # rsplits[i][s]: what s sends me
+
+    def a2a(t, sent, got):
+        if t is None:
+            return None
+        out = torch.empty((sum(got), *t.shape[1:]), dtype=t.dtype, device=t.device)
+        dist.all_to_all_single(out, t, output_split_sizes=got, input_split_sizes=list(sent), group=group)
+        return out
+    return [a2a(t, sent, got) for t, sent, got in zip(cols, splits, rsplits)], rsplits
+
+
+_SUMMED_STATS = ("exchange_ms", "exchanges", "prepare_wall_ms", "counts_wall_ms", "post_wall_ms")
+
+
+def _exchange(engine, sh, kind, rank, world, group, stats, exchange_device, mode=L.VB_XCHG_NCCL, p2p=False):
+    """The exchange step of every run_*shuffle, then the seal.  kind = (the engine class that drives the library,
+    export(engine, sh, world) -> (columns, splits), import_(engine, sh, columns, splits), index of the column whose
+    counts are the kind's rows in `stats`).  With a communicator on the context the exchange is vb_shuffle_exchange
+    (`mode`); otherwise the fused P2P exchange (p2p) or all_to_all_v (exchange_device: stage the columns there, "cpu"
+    for a gloo group on a one-GPU box)."""
+    cls, export, import_, rows = kind
+    if world > 1 and isinstance(engine, cls) and getattr(engine.sc, "comm", None) and exchange_device is None:
+        # the product path: count exchange + ONE grouped NCCL send/recv (or the fused P2P scatter) inside
+        # libvega_b200, on the library's stream; torch.distributed is not involved
+        sh.exchange(mode)
+        engine.seal(sh)
+        if stats is not None:           # after the seal: reading the event timers synchronises the stream
+            for k_, v_ in sh.exchange_stats().items():
+                stats[k_] = (stats.get(k_, 0) + v_) if k_ in _SUMMED_STATS else v_
+        return sh
+    if world > 1 and p2p:
+        p2p_exchange(engine, sh, rank, world, group, stats)
+    elif world > 1:
+        cols, splits = export(engine, sh, world)
+        home = cols[rows].device
+        if exchange_device is not None:
+            cols = [None if c is None else c.to(exchange_device) for c in cols]
+        ev = None
+        if stats is not None and cols[rows].is_cuda:
+            import torch
+            ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
+            ev[0].record()
+        rcols, rsplits = all_to_all_v(cols, splits, group)
+        if ev is not None:
+            ev[1].record()
+            ev[1].synchronize()
+            stats["exchange_ms"] = stats.get("exchange_ms", 0.0) + ev[0].elapsed_time(ev[1])
+        if exchange_device is not None:
+            rcols = [None if c is None else c.to(home) for c in rcols]
+        if stats is not None:
+            stats["sent_rows"] = sum(splits[rows]) - splits[rows][rank]
+            stats["recv_rows"] = sum(rsplits[rows]) - rsplits[rows][rank]
+            stats["exchanges"] = stats.get("exchanges", 0) + 1
+        import_(engine, sh, rcols, rsplits)
+    engine.seal(sh)
+    return sh
+
+
+def _rows_export(engine, sh, world):
+    counts, keys, vals = engine.export(sh, world)
+    return [keys, vals], [counts, counts]
+
+
+def _rows_import(engine, sh, cols, splits):
+    engine.import_(sh, cols[0], cols[1], splits[0])
 
 
 def run_shuffle(engine, local_maps, n_map, n_reduce, kcode, vcode, agg, rank, world, group=None, key_width=8, hint=0,
@@ -170,42 +235,9 @@ def run_shuffle(engine, local_maps, n_map, n_reduce, kcode, vcode, agg, rank, wo
     sh = engine.create(n_map, n_reduce, kcode, vcode, agg, rank, world, key_width=key_width, hint=hint)
     for map_id, keys, vals in local_maps:
         engine.map(sh, map_id, keys, vals)
-    if world > 1 and isinstance(engine, CudaEngine) and getattr(engine.sc, "comm", None) and exchange_device is None:
-        # the product path: count exchange + ONE grouped NCCL send/recv (or the fused P2P scatter) inside
-        # libvega_b200, on the library's stream; torch.distributed is not involved
-        group_op = agg in (L.VB_AGG_GROUP, L.VB_AGG_COGROUP)
-        sh.exchange(L.VB_XCHG_P2P if (p2p and group_op) else L.VB_XCHG_NCCL)
-        engine.seal(sh)
-        if stats is not None:           # after the seal: reading the event timers synchronises the stream
-            for k_, v_ in sh.exchange_stats().items():
-                stats[k_] = (stats.get(k_, 0) + v_) if k_ in ("exchange_ms", "exchanges", "prepare_wall_ms", "counts_wall_ms", "post_wall_ms") else v_
-        return sh
-    elif world > 1 and p2p and agg in (L.VB_AGG_GROUP, L.VB_AGG_COGROUP) and isinstance(engine, CudaEngine):
-        p2p_exchange(engine, sh, rank, world, group, stats)
-    elif world > 1:
-        counts, sk, sv = engine.export(sh, world)
-        home = sk.device
-        if exchange_device is not None:        # e.g. "cpu" for a gloo group: stage the exchange through the host
-            sk, sv = sk.to(exchange_device), sv.to(exchange_device)
-        ev = None
-        if stats is not None and sk.is_cuda:
-            import torch
-            ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
-            ev[0].record()
-        rk, rv, rcounts = all_to_all_v(sk, sv, counts, group)
-        if ev is not None:
-            ev[1].record()
-            ev[1].synchronize()
-            stats["exchange_ms"] = stats.get("exchange_ms", 0.0) + ev[0].elapsed_time(ev[1])
-        if exchange_device is not None:
-            rk, rv = rk.to(home), rv.to(home)
-        if stats is not None:
-            stats["sent_rows"] = sum(counts) - counts[rank]
-            stats["recv_rows"] = sum(rcounts) - rcounts[rank]
-            stats["exchanges"] = stats.get("exchanges", 0) + 1
-        engine.import_(sh, rk, rv, rcounts)
-    engine.seal(sh)
-    return sh
+    p2p = p2p and agg in (L.VB_AGG_GROUP, L.VB_AGG_COGROUP)
+    return _exchange(engine, sh, (CudaEngine, _rows_export, _rows_import, 0), rank, world, group, stats, exchange_device,
+                     L.VB_XCHG_P2P if p2p else L.VB_XCHG_NCCL, p2p and isinstance(engine, CudaEngine))
 
 
 class StrCudaEngine:
@@ -238,71 +270,25 @@ class StrCudaEngine:
         return sh.reduce(r)
 
 
-def all_to_all_v_str(cols, counts, group=None):
-    """The String exchange step: one all_to_all_single of the three counts per destination (keys, key bytes,
-    values), then one per column.  cols = (key_lens, key_bytes, val_counts or None, vals), destination-major.
-    Returns (received columns, received counts), source-rank major, in the same shapes."""
-    import torch
-    import torch.distributed as dist
-    world = len(counts[0])
-    dev = cols[3].device
-    cin = torch.tensor(list(zip(*counts)), dtype=torch.int64, device=dev).reshape(world, 3)    # row d: what d gets
-    cout = torch.empty_like(cin)
-    dist.all_to_all_single(cout, cin, group=group)
-    rows = cout.tolist()                                                                      # row s: what s sends me
-    rcounts = tuple([r[i] for r in rows] for i in range(3))
-    splits = (0, 1, 0, 2)                        # the count each column is split by: keys, bytes, keys, values
+def _str_export(engine, sh, world):
+    (n_keys, n_key_bytes, n_vals), cols = engine.export(sh, world)
+    return list(cols), [n_keys, n_key_bytes, n_keys, n_vals]     # key lengths, key bytes, value counts, values
 
-    def a2a(t, i):
-        if t is None:
-            return None
-        out = torch.empty(sum(rcounts[splits[i]]), dtype=t.dtype, device=t.device)
-        dist.all_to_all_single(out, t, output_split_sizes=rcounts[splits[i]], input_split_sizes=list(counts[splits[i]]),
-                               group=group)
-        return out
-    return tuple(a2a(t, i) for i, t in enumerate(cols)), rcounts
+
+def _str_import(engine, sh, cols, splits):
+    engine.import_(sh, tuple(cols), (splits[0], splits[1], splits[3]))
 
 
 def run_str_shuffle(engine, local_maps, n_map, n_reduce, vcode, agg, rank, world, group=None, hint=0, stats=None,
                     exchange_device=None):
     """run_shuffle for String keys: map side on this rank's partitions → exchange → reduce side for the partitions
     this rank owns.  local_maps: [(map_id, keys, vals_or_None)], ascending map ids from map_block(rank, world, n_map).
-    With a communicator on the context the exchange is vb_shuffle_exchange (NCCL inside the library); otherwise four
-    all_to_all_single calls after the count swap (exchange_device: "cpu" for a gloo group on a one-GPU box)."""
+    With a communicator on the context the exchange is vb_shuffle_exchange (NCCL inside the library); otherwise
+    all_to_all_v of the four columns (exchange_device: "cpu" for a gloo group on a one-GPU box)."""
     sh = engine.create(n_map, n_reduce, vcode, agg, rank, world, hint=hint)
     for map_id, keys, vals in local_maps:
         engine.map(sh, map_id, keys, vals)
-    if world > 1 and isinstance(engine, StrCudaEngine) and getattr(engine.sc, "comm", None) and exchange_device is None:
-        sh.exchange(L.VB_XCHG_NCCL)
-        engine.seal(sh)
-        if stats is not None:
-            for k_, v_ in sh.exchange_stats().items():
-                stats[k_] = (stats.get(k_, 0) + v_) if k_ in ("exchange_ms", "exchanges", "prepare_wall_ms", "counts_wall_ms", "post_wall_ms") else v_
-        return sh
-    if world > 1:
-        counts, cols = engine.export(sh, world)
-        home = cols[3].device
-        if exchange_device is not None:
-            cols = tuple(None if c is None else c.to(exchange_device) for c in cols)
-        ev = None
-        if stats is not None and cols[3].is_cuda:
-            import torch
-            ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
-            ev[0].record()
-        rcols, rcounts = all_to_all_v_str(cols, counts, group)
-        if ev is not None:
-            ev[1].record()
-            ev[1].synchronize()
-            stats["exchange_ms"] = stats.get("exchange_ms", 0.0) + ev[0].elapsed_time(ev[1])
-        if exchange_device is not None:
-            rcols = tuple(None if c is None else c.to(home) for c in rcols)
-        if stats is not None:
-            stats["sent_rows"] = sum(counts[2]) - counts[2][rank]
-            stats["recv_rows"] = sum(rcounts[2]) - rcounts[2][rank]
-            stats["exchanges"] = stats.get("exchanges", 0) + 1
-        engine.import_(sh, rcols, rcounts)
-    engine.seal(sh)
-    return sh
+    return _exchange(engine, sh, (StrCudaEngine, _str_export, _str_import, 3), rank, world, group, stats, exchange_device)
 
 
 class CombineCudaEngine:
@@ -335,29 +321,31 @@ class CombineCudaEngine:
         return sh.reduce_cols(r, out_dtypes)
 
 
-def all_to_all_v_cols(keys, accs, counts, group=None):
-    """The combine_by_key exchange step: one all_to_all_single of the counts, then one of the rows, each row the key
-    and its n_acc partials.  keys[rows] and accs[n_acc][rows] are destination-major; returns (keys, accs, counts)
-    received, source-rank major, in the same shapes."""
+def _combine_pack(counts, keys, accs):
+    """keys[rows] and accs[n_acc][rows] as one [rows][1 + n_acc] column: one all_to_all_single carries every row."""
     import torch
-    import torch.distributed as dist
-    dev = keys.device
-    cin = torch.tensor(counts, dtype=torch.int64, device=dev)
-    cout = torch.empty_like(cin)
-    dist.all_to_all_single(cout, cin, group=group)
-    rcounts = [int(x) for x in cout.tolist()]
-    rows = torch.cat([keys.view(-1, 1), accs.t()], dim=1).contiguous()          # [rows][1 + n_acc]
-    out = torch.empty((sum(rcounts), rows.shape[1]), dtype=rows.dtype, device=dev)
-    dist.all_to_all_single(out, rows, output_split_sizes=rcounts, input_split_sizes=list(counts), group=group)
-    return out[:, 0].contiguous(), out[:, 1:].t().contiguous(), rcounts
+    return [torch.cat([keys.view(-1, 1), accs.t()], dim=1).contiguous()], [counts]
+
+
+def _combine_unpack(cols, splits):
+    """The received [rows][1 + n_acc] column as (keys[rows], accs[n_acc][rows], rows from every source)."""
+    return cols[0][:, 0].contiguous(), cols[0][:, 1:].t().contiguous(), splits[0]
+
+
+def _combine_export(engine, sh, world):
+    return _combine_pack(*engine.export(sh, world))
+
+
+def _combine_import(engine, sh, cols, splits):
+    engine.import_(sh, *_combine_unpack(cols, splits))
 
 
 def run_combine_shuffle(engine, local_maps, n_map, n_reduce, kcode, multi, rank, world, group=None, key_width=8, hint=0,
                         stats=None, exchange_device=None):
     """run_shuffle for combine_by_key: map side on this rank's partitions → exchange → reduce side for the partitions
     this rank owns.  local_maps: [(map_id, keys, value columns)], ascending map ids from map_block(rank, world, n_map).
-    With a communicator on the context the exchange is vb_shuffle_exchange (NCCL inside the library); otherwise one
-    all-to-all-v of the 1 + n_acc columns after the count swap (exchange_device: "cpu" for a gloo group on a one-GPU
+    With a communicator on the context the exchange is vb_shuffle_exchange (NCCL inside the library); otherwise
+    all_to_all_v of the rows, each the key and its n_acc partials (exchange_device: "cpu" for a gloo group on a one-GPU
     box)."""
     if not 0 <= rank < world <= 256:
         raise ValueError(f"rank {rank} of world {world}: 0 <= rank < world <= 256")
@@ -368,37 +356,8 @@ def run_combine_shuffle(engine, local_maps, n_map, n_reduce, kcode, multi, rank,
     sh = engine.create(n_map, n_reduce, kcode, multi, rank, world, key_width=key_width, hint=hint)
     for map_id, keys, cols in local_maps:
         engine.map(sh, map_id, keys, cols)
-    if world > 1 and isinstance(engine, CombineCudaEngine) and getattr(engine.sc, "comm", None) and exchange_device is None:
-        sh.exchange(L.VB_XCHG_NCCL)
-        engine.seal(sh)
-        if stats is not None:
-            for k_, v_ in sh.exchange_stats().items():
-                stats[k_] = (stats.get(k_, 0) + v_) if k_ in ("exchange_ms", "exchanges", "prepare_wall_ms", "counts_wall_ms", "post_wall_ms") else v_
-        return sh
-    if world > 1:
-        counts, keys, accs = engine.export(sh, world)
-        home = keys.device
-        if exchange_device is not None:
-            keys, accs = keys.to(exchange_device), accs.to(exchange_device)
-        ev = None
-        if stats is not None and keys.is_cuda:
-            import torch
-            ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
-            ev[0].record()
-        rk, ra, rcounts = all_to_all_v_cols(keys, accs, counts, group)
-        if ev is not None:
-            ev[1].record()
-            ev[1].synchronize()
-            stats["exchange_ms"] = stats.get("exchange_ms", 0.0) + ev[0].elapsed_time(ev[1])
-        if exchange_device is not None:
-            rk, ra = rk.to(home), ra.to(home)
-        if stats is not None:
-            stats["sent_rows"] = sum(counts) - counts[rank]
-            stats["recv_rows"] = sum(rcounts) - rcounts[rank]
-            stats["exchanges"] = stats.get("exchanges", 0) + 1
-        engine.import_(sh, rk, ra, rcounts)
-    engine.seal(sh)
-    return sh
+    return _exchange(engine, sh, (CombineCudaEngine, _combine_export, _combine_import, 0), rank, world, group, stats,
+                     exchange_device)
 
 
 def owned_partitions(rank, world, n_reduce):
