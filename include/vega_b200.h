@@ -546,6 +546,70 @@ VB_API int32_t vb_shuffle_export_str_buffers(vb_shuf *s, uint32_t **key_lens, vo
 VB_API int32_t vb_shuffle_import_str(vb_shuf *s, const uint32_t *key_lens, const void *key_bytes, const uint32_t *val_counts,
                                      const uint64_t *vals, const uint64_t *n_keys /*[world]*/,
                                      const uint64_t *n_key_bytes /*[world]*/, const uint64_t *n_vals /*[world]*/);
+/* ---- combine_by_key over string keys: several named aggregates per `String` key in one shuffle (PairRdd::combine_by_key,
+ *      src/rdd/pair_rdd.rs:20-33, over `String` keys) -----------------------------------------------------------------
+ * vb_shuffle_create_str_multi takes the spec of vb_shuffle_create_multi (1 to VB_MAX_VAL_COLS value columns of VB_U64 /
+ * VB_I64 / VB_F64, 1 to VB_MAX_AGGS aggregates of SUM / MIN / MAX / COUNT / MEAN, a MEAN's internal COUNT counted against
+ * VB_MAX_AGGS; VB_ERR_INVALID otherwise) and places keys as any string shuffle does: vb_hash_str(key) % n_reduce.  For
+ * every key, aggregate a is what vb_shuffle_create_str with op aggs[a].agg over column aggs[a].src gives (integer ops,
+ * COUNT and f64 MIN / MAX bit for bit, NaN rules included; f64 SUM up to summation order), and a MEAN is (double)S / n
+ * with S read with the column's signedness, as the integer-key combine computes it.  Every key of the input appears
+ * exactly once, in its partition; the order of keys within a partition is unspecified.  Re-submitting a map_id replaces
+ * its rows (a key only the replaced rows had is dropped).  Limits: those of vb_shuffle_create_str (fewer than 2^32 - 2
+ * rows per map partition and per shuffle, fewer than 2^31 distinct keys, keys shorter than 2^32 bytes).
+ *   vb_shuffle_map_str_cols    keys as for vb_shuffle_map_str (Arrow-style offsets that may start anywhere, any src_loc)
+ *                              and vals[c][n_rows] for c < n_val_cols; a column no aggregate reads may be NULL and is not
+ *                              copied (VB_ERR_INVALID for a NULL column that one reads).
+ *   vb_shuffle_reduce_str_cols one partition: out_key_offsets [n_keys + 1] (from 0) into out_key_bytes [n_key_bytes], and
+ *                              out_aggs[a][n_keys] per aggregate in the output dtype of vb_shuffle_reduce_cols; sizes from
+ *                              vb_shuffle_reduce_str_size (n_vals == n_keys); NULL outputs are skipped; blocks until sealed.
+ * On this shuffle kind vb_shuffle_map_str, the integer map / reduce / join calls, vb_shuffle_set_key_width,
+ * vb_cogroup_n_str / vb_join_n_str, vb_shuffle_create_narrow and the single-column string export / import calls return
+ * VB_ERR_INVALID; vb_shuffle_reduce_str returns the keys only (VB_ERR_INVALID with out_combined, out_offsets or out_vals
+ * non-NULL); vb_shuffle_set_dist with world > 1, VB_XCHG_P2P and the bincode blob calls return VB_ERR_UNSUPPORTED.  The
+ * calls below return VB_ERR_INVALID on any other shuffle.  seal / stats / kernel_time / set_hint / free work as for any
+ * string shuffle.
+ * Several ranks (one process per GPU): vb_shuffle_create_str_multi_dist is vb_shuffle_create_str_multi for rank `rank` of
+ * `world` (1 <= world <= 256, VB_ERR_INVALID otherwise; world == 1 gives the same shuffle as the plain call).  Partition
+ * r is owned by rank r % world.  Each rank runs its map tasks, then:
+ *   vb_shuffle_export_str_cols_prepare  finishes the local map side and packs one row per distinct live key by
+ *                                       destination rank; n_keys / n_key_bytes [world] get what goes to each rank.
+ *   vb_shuffle_export_str_cols_buffers  the device columns, destination-major, owned by the library until seal (NULL
+ *                                       output pointers are skipped); n_acc gets the accumulator count.  Wire format:
+ *                                         key_lens   u32 [keys]          each key's length in bytes
+ *                                         key_bytes  u8  [bytes]         the keys' bytes, concatenated in key order
+ *                                         accs       u64 [n_acc][keys]   accumulator a of key i at accs[a * keys + i],
+ *                                                                        keys = the sum of n_keys; the rank's partials in
+ *                                                                        the plain value form of vb_shuffle_export_cols_buffers
+ *   vb_shuffle_import_str_cols          the received columns, source-rank major, with the key and byte counts each
+ *                                       source sent; borrowed until vb_shuffle_seal returns.  Then seal.
+ * The seal merges the partials with merge_combiners and finalizes as the one-process seal does, so every owner's
+ * partitions equal those of the one-process shuffle over the same map tasks, whatever `world` is (f64 SUM and MEAN up to
+ * summation order); partitions a rank does not own are empty on it.  vb_shuffle_exchange(s, VB_XCHG_AUTO or
+ * VB_XCHG_NCCL) does all of it on the library's stream: export, one all-gather of 2 x world counts and the spec's
+ * fingerprint (n_acc, every accumulator's op and order transform, n_reduce), one grouped send/recv of the 2 + n_acc
+ * columns; ranks whose specs differ all return VB_ERR_INVALID before any send.
+ * Errors: the _str_cols export / import calls on a world-1 shuffle, import before export, twice or after seal, map after
+ * export, and seal without import: VB_ERR_STATE; an n_acc that differs from the shuffle's, or a NULL column with a
+ * non-zero count: VB_ERR_INVALID; an import of 2^31 keys or more: VB_ERR_TOO_LARGE, from the counts; key lengths that do
+ * not add up to the announced bytes: VB_ERR_INVALID from the seal.                                                     */
+VB_API int32_t vb_shuffle_create_str_multi(vb_ctx *ctx, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce,
+                                           uint32_t n_val_cols, const int32_t *val_dtypes, uint32_t n_aggs,
+                                           const vb_agg_col *aggs, vb_shuf **out);
+VB_API int32_t vb_shuffle_create_str_multi_dist(vb_ctx *ctx, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce,
+                                                uint32_t n_val_cols, const int32_t *val_dtypes, uint32_t n_aggs,
+                                                const vb_agg_col *aggs, uint32_t rank, uint32_t world, vb_shuf **out);
+VB_API int32_t vb_shuffle_map_str_cols(vb_shuf *s, uint32_t map_id, const uint64_t *key_offsets /*n_rows+1*/,
+                                       const void *key_bytes, uint64_t n_bytes, const void *const *vals /*[n_val_cols]*/,
+                                       uint64_t n_rows, int32_t src_loc);
+VB_API int32_t vb_shuffle_reduce_str_cols(vb_shuf *s, uint32_t reduce_id, uint64_t *out_key_offsets /*n_keys+1*/,
+                                          void *out_key_bytes, void *const *out_aggs /*[n_aggs]*/, int32_t dst_loc);
+VB_API int32_t vb_shuffle_export_str_cols_prepare(vb_shuf *s, uint64_t *n_keys /*[world]*/, uint64_t *n_key_bytes /*[world]*/);
+VB_API int32_t vb_shuffle_export_str_cols_buffers(vb_shuf *s, uint32_t **key_lens, void **key_bytes, uint64_t **accs,
+                                                  uint32_t *n_acc);
+VB_API int32_t vb_shuffle_import_str_cols(vb_shuf *s, const uint32_t *key_lens, const void *key_bytes, const uint64_t *accs,
+                                          uint32_t n_acc, const uint64_t *n_keys /*[world]*/,
+                                          const uint64_t *n_key_bytes /*[world]*/);
 /* MetroHash64_1(bytes ‖ 0xFF, seed 0): the reference's hash of a `String` / `&str` key */
 VB_API uint64_t vb_hash_str(const void *bytes, uint64_t len);
 VB_API uint32_t vb_get_partition_str(const void *bytes, uint64_t len, uint32_t n_reduce);

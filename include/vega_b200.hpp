@@ -676,6 +676,48 @@ public:
         return out;
     }
 
+    // combine_by_key with named aggregates of the value column (VB_AGG_SUM / MIN / MAX / COUNT / MEAN) over String keys,
+    // one shuffle (vb_shuffle_create_str_multi): per key one result per aggregate, as 64-bit patterns (COUNT: uint64_t,
+    // MEAN: double, others: V; read them with detail::from_bits<T>)
+    std::vector<std::pair<std::string, std::vector<uint64_t>>> combine_by_key(const std::vector<int32_t> &aggs, size_t num_splits) const
+    {
+        if (num_slices_ < 1) throw Error(VB_ERR_INVALID, "Number of slices should be greater than or equal to 1");
+        const uint64_t n = keys_.size();
+        std::vector<uint64_t> starts(std::min<uint64_t>(n, num_slices_) + 2);
+        const uint64_t n_map = vb_slice(n, num_slices_, starts.data());
+        std::vector<vb_agg_col> spec;
+        for (int32_t a : aggs) spec.push_back(vb_agg_col{a, 0});
+        const int32_t vcode = detail::dtype<V>::code;
+        vb_shuf *raw = nullptr;
+        check(vb_shuffle_create_str_multi(sc_->raw(), sc_->new_shuffle_id(), (uint32_t)n_map, (uint32_t)num_splits, 1, &vcode,
+                                          (uint32_t)spec.size(), spec.data(), &raw));
+        detail::ShufPtr s(raw);
+        for (uint64_t m = 0; m < n_map; ++m) {
+            const uint64_t lo = starts[m], cnt = starts[m + 1] - lo;
+            const void *col = cnt ? vals_.data() + lo : nullptr;
+            check(vb_shuffle_map_str_cols(raw, (uint32_t)m, keys_.offs.data() + lo, keys_.bytes.data(), keys_.bytes.size(), &col, cnt,
+                                          VB_HOST));
+        }
+        check(vb_shuffle_seal(raw));
+        std::vector<std::pair<std::string, std::vector<uint64_t>>> out;
+        for (uint32_t r = 0; r < num_splits; ++r) {
+            uint64_t nk = 0, nb = 0;
+            check(vb_shuffle_reduce_str_size(raw, r, &nk, &nb, nullptr));
+            std::vector<uint64_t> ko(nk + 1);
+            std::string kb(nb, '\0');
+            std::vector<std::vector<uint64_t>> cols(aggs.size(), std::vector<uint64_t>(nk));
+            std::vector<void *> ptrs;
+            for (auto &c : cols) ptrs.push_back(c.data());
+            check(vb_shuffle_reduce_str_cols(raw, r, ko.data(), kb.data(), ptrs.data(), VB_HOST));
+            for (uint64_t i = 0; i < nk; ++i) {
+                std::vector<uint64_t> row;
+                for (auto &c : cols) row.push_back(c[i]);
+                out.emplace_back(std::string(kb, ko[i], ko[i + 1] - ko[i]), std::move(row));
+            }
+        }
+        return out;
+    }
+
     // CoGroupedRdd::new([self, others...], HashPartitioner::new(num_splits)).collect() over String keys
     // (vb_cogroup_n_str): every key of any parent once, with one value list per parent (this one first)
     std::vector<std::pair<std::string, std::vector<std::vector<V>>>> cogroup_n(const std::vector<StrPairRddT> &others,

@@ -134,6 +134,22 @@ extern "C" {
                                          val_counts: *mut *mut u32, vals: *mut *mut u64) -> i32;
     pub fn vb_shuffle_import_str(s: *mut vb_shuf, key_lens: *const u32, key_bytes: *const c_void, val_counts: *const u32,
                                  vals: *const u64, n_keys: *const u64, n_key_bytes: *const u64, n_vals: *const u64) -> i32;
+    // combine_by_key over String keys: the combine spec of vb_shuffle_create_multi, keys as for vb_shuffle_map_str; across
+    // ranks the wire is u32 key lengths, key bytes and u64 accumulators [n_acc][keys] in plain value form
+    pub fn vb_shuffle_create_str_multi(ctx: *mut vb_ctx, shuffle_id: u64, n_map: u32, n_reduce: u32, n_val_cols: u32,
+                                       val_dtypes: *const i32, n_aggs: u32, aggs: *const vb_agg_col, out: *mut *mut vb_shuf) -> i32;
+    pub fn vb_shuffle_create_str_multi_dist(ctx: *mut vb_ctx, shuffle_id: u64, n_map: u32, n_reduce: u32, n_val_cols: u32,
+                                            val_dtypes: *const i32, n_aggs: u32, aggs: *const vb_agg_col, rank: u32, world: u32,
+                                            out: *mut *mut vb_shuf) -> i32;
+    pub fn vb_shuffle_map_str_cols(s: *mut vb_shuf, map_id: u32, key_offsets: *const u64, key_bytes: *const c_void, n_bytes: u64,
+                                   vals: *const *const c_void, n_rows: u64, src_loc: i32) -> i32;
+    pub fn vb_shuffle_reduce_str_cols(s: *mut vb_shuf, reduce_id: u32, out_key_offsets: *mut u64, out_key_bytes: *mut c_void,
+                                      out_aggs: *const *mut c_void, dst_loc: i32) -> i32;
+    pub fn vb_shuffle_export_str_cols_prepare(s: *mut vb_shuf, n_keys: *mut u64, n_key_bytes: *mut u64) -> i32;
+    pub fn vb_shuffle_export_str_cols_buffers(s: *mut vb_shuf, key_lens: *mut *mut u32, key_bytes: *mut *mut c_void,
+                                              accs: *mut *mut u64, n_acc: *mut u32) -> i32;
+    pub fn vb_shuffle_import_str_cols(s: *mut vb_shuf, key_lens: *const u32, key_bytes: *const c_void, accs: *const u64, n_acc: u32,
+                                      n_keys: *const u64, n_key_bytes: *const u64) -> i32;
     pub fn vb_hash_str(bytes: *const c_void, len: u64) -> u64;
     pub fn vb_get_partition_str(bytes: *const c_void, len: u64, n_reduce: u32) -> u32;
     pub fn vb_shuffle_free(s: *mut vb_shuf) -> i32;

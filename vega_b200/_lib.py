@@ -121,6 +121,14 @@ SYMBOLS = {
     "vb_shuffle_export_str_prepare": (_i32, [_vp, _pu64, _pu64, _pu64]),
     "vb_shuffle_export_str_buffers": (_i32, [_vp, _pvp, _pvp, _pvp, _pvp]),
     "vb_shuffle_import_str": (_i32, [_vp, _vp, _vp, _vp, _vp, _pu64, _pu64, _pu64]),
+    "vb_shuffle_create_str_multi": (_i32, [_vp, _u64, _u32, _u32, _u32, _vp, _u32, ctypes.POINTER(vb_agg_col), _pvp]),
+    "vb_shuffle_create_str_multi_dist": (_i32, [_vp, _u64, _u32, _u32, _u32, _vp, _u32, ctypes.POINTER(vb_agg_col), _u32, _u32,
+                                                _pvp]),
+    "vb_shuffle_map_str_cols": (_i32, [_vp, _u32, _vp, _vp, _u64, _pvp, _u64, _i32]),
+    "vb_shuffle_reduce_str_cols": (_i32, [_vp, _u32, _vp, _vp, _pvp, _i32]),
+    "vb_shuffle_export_str_cols_prepare": (_i32, [_vp, _pu64, _pu64]),
+    "vb_shuffle_export_str_cols_buffers": (_i32, [_vp, _pvp, _pvp, _pvp, ctypes.POINTER(_u32)]),
+    "vb_shuffle_import_str_cols": (_i32, [_vp, _vp, _vp, _vp, _u32, _pu64, _pu64]),
     "vb_hash_str": (_u64, [_vp, _u64]),
     "vb_get_partition_str": (_u32, [_vp, _u64, _u32]),
     "vb_shuffle_reduce_blob_size": (_i32, [_vp, _u32, _pu64]),

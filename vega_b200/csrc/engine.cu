@@ -388,6 +388,7 @@ static int seal_str_import(vb_shuf *s);
 static int export_str_locked(vb_shuf *s, u64 *n_keys, u64 *n_key_bytes, u64 *n_vals);
 static int str_import_limits(const vb_shuf *s, u64 nk, u64 nv);
 static int exchange_str_locked(vb_shuf *s);
+static int exchange_str_multi_locked(vb_shuf *s);
 static void free_str(vb_shuf *s);
 
 static bool is_reduce_op(int agg) { return agg == VB_AGG_SUM || agg == VB_AGG_MIN || agg == VB_AGG_MAX || agg == VB_AGG_COUNT; }
@@ -1280,12 +1281,17 @@ extern "C" int32_t vb_shuffle_create(vb_ctx *c, uint64_t shuffle_id, uint32_t n_
 
 // Accumulators of a multi-aggregate shuffle: aggregate a owns accumulator a; a MEAN's is its SUM, and every MEAN
 // divides by the spec's first COUNT accumulator, or by one appended after the aggregates when the spec has none.
-extern "C" int32_t vb_shuffle_create_multi(vb_ctx *c, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce, int32_t kdt,
-                                           uint32_t n_val_cols, const int32_t *val_dtypes, uint32_t n_aggs, const vb_agg_col *aggs,
-                                           vb_shuf **out)
+// The specs of the map-side combine, the table merge and the import merge, and the output columns: filled in by
+// multi_spec, shared by the integer-key and the string-key combine.
+struct MultiSpec {
+    u32 n_cols = 0;
+    AccSpec map{}, merge{}, imp{};
+    OutSpec outs{};
+    int out_dt[VB_MAX_AGGS] = {};
+};
+
+static int multi_spec(uint32_t n_val_cols, const int32_t *val_dtypes, uint32_t n_aggs, const vb_agg_col *aggs, MultiSpec *ms)
 {
-    if (!c || !out || !val_dtypes || !aggs) return set_err(VB_ERR_INVALID, "vb_shuffle_create_multi: NULL argument");
-    *out = nullptr;
     if (n_val_cols < 1 || n_val_cols > VB_MAX_VAL_COLS) return set_err(VB_ERR_INVALID, "%u value columns (1..%d)", n_val_cols, VB_MAX_VAL_COLS);
     if (n_aggs < 1 || n_aggs > VB_MAX_AGGS) return set_err(VB_ERR_INVALID, "%u aggregates (1..%d)", n_aggs, VB_MAX_AGGS);
     for (u32 i = 0; i < n_val_cols; ++i)
@@ -1304,13 +1310,10 @@ extern "C" int32_t vb_shuffle_create_multi(vb_ctx *c, uint64_t shuffle_id, uint3
     const u32 n_acc = n_aggs + ((any_mean && count_acc < 0) ? 1 : 0);
     if (n_acc > VB_MAX_AGGS) return set_err(VB_ERR_INVALID, "%u aggregates plus the COUNT a MEAN needs exceed %d", n_aggs, VB_MAX_AGGS);
     if (count_acc < 0) count_acc = (int)n_aggs;
-    TRY(vb_shuffle_create(c, shuffle_id, n_map, n_reduce, kdt, VB_U64, VB_AGG_SUM, VB_PART_HASH_METRO64, out));
-    vb_shuf *s = *out;
-    s->multi = true;
-    s->n_cols = n_val_cols;
-    AccSpec &mp = s->acc_map, &mg = s->acc_merge;
-    OutSpec &os = s->outs;
-    mp.n = mg.n = s->acc_imp.n = n_acc;
+    ms->n_cols = n_val_cols;
+    AccSpec &mp = ms->map, &mg = ms->merge;
+    OutSpec &os = ms->outs;
+    mp.n = mg.n = ms->imp.n = n_acc;
     os.n = n_aggs;
     for (u32 a = 0; a < n_acc; ++a) {
         const int op = a < n_aggs ? aggs[a].agg : VB_AGG_COUNT;
@@ -1324,14 +1327,38 @@ extern "C" int32_t vb_shuffle_create_multi(vb_ctx *c, uint64_t shuffle_id, uint3
         }
         spec_set(mp.op, a, opk); spec_set(mp.tx, a, tx); spec_set(mp.src, a, src);
         spec_set(mg.op, a, merge_op(opk)); spec_set(mg.src, a, a);
-        spec_set(s->acc_imp.op, a, merge_op(opk)); spec_set(s->acc_imp.tx, a, tx);
+        spec_set(ms->imp.op, a, merge_op(opk)); spec_set(ms->imp.tx, a, tx);
         if (a >= n_aggs) continue;
-        s->out_dt[a] = op == VB_AGG_COUNT ? VB_U64 : op == VB_AGG_MEAN ? VB_F64 : dt;
+        ms->out_dt[a] = op == VB_AGG_COUNT ? VB_U64 : op == VB_AGG_MEAN ? VB_F64 : dt;
         os.acc[a] = (unsigned char)a;
         os.cnt[a] = (unsigned char)count_acc;
         os.tx[a] = (unsigned char)tx;
         os.kind[a] = op != VB_AGG_MEAN ? MO_COPY : dt == VB_U64 ? MO_MEAN_U64 : dt == VB_I64 ? MO_MEAN_I64 : MO_MEAN_F64;
     }
+    return VB_OK;
+}
+
+static void set_multi(vb_shuf *s, const MultiSpec &ms)
+{
+    s->multi = true;
+    s->n_cols = ms.n_cols;
+    s->acc_map = ms.map;
+    s->acc_merge = ms.merge;
+    s->acc_imp = ms.imp;
+    s->outs = ms.outs;
+    std::copy(ms.out_dt, ms.out_dt + VB_MAX_AGGS, s->out_dt);
+}
+
+extern "C" int32_t vb_shuffle_create_multi(vb_ctx *c, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce, int32_t kdt,
+                                           uint32_t n_val_cols, const int32_t *val_dtypes, uint32_t n_aggs, const vb_agg_col *aggs,
+                                           vb_shuf **out)
+{
+    if (!c || !out || !val_dtypes || !aggs) return set_err(VB_ERR_INVALID, "vb_shuffle_create_multi: NULL argument");
+    *out = nullptr;
+    MultiSpec ms;
+    TRY(multi_spec(n_val_cols, val_dtypes, n_aggs, aggs, &ms));
+    TRY(vb_shuffle_create(c, shuffle_id, n_map, n_reduce, kdt, VB_U64, VB_AGG_SUM, VB_PART_HASH_METRO64, out));
+    set_multi(*out, ms);
     return VB_OK;
 }
 
@@ -1504,7 +1531,7 @@ static int shuffle_map(vb_shuf *s, u32 map_id, const u64 *rows, const u64 *keys,
 
 extern "C" int32_t vb_shuffle_map_aos(vb_shuf *s, uint32_t map_id, const void *rows, uint64_t n, int32_t loc)
 {
-    if (s && s->multi) return reject_multi(s, "AoS rows");
+    if (s && s->multi && !s->str) return reject_multi(s, "AoS rows");
     // every AoS loader reads a row as one 16-byte vector load; host rows are copied into aligned buffers first
     if (n && loc != VB_HOST && ((uintptr_t)rows & 15u))
         return set_err(VB_ERR_INVALID, "device AoS rows at %p: 16-byte rows must start on a 16-byte boundary", rows);
@@ -2238,8 +2265,9 @@ struct Comm {
 constexpr u32 COMM_MAX_WORLD = 64;
 constexpr size_t COMM_HOST_OFF = 256 << 10;   // staging region inside vb_ctx::h_scratch
 // u64 per rank of the count all-gather: world + 2 for integer rows (counts, arena bytes and generation), world + 3 for
-// combine_by_key (counts and the spec's fingerprint), 3 * world for String keys, 2 for sort
-static size_t comm_row(u32 world) { return std::max<size_t>((size_t)world + 2, 3 * (size_t)world); }
+// combine_by_key (counts and the spec's fingerprint), 3 * world for String keys, 2 * world + 3 for String-key
+// combine_by_key (key and byte counts, and the spec's fingerprint), 2 for sort
+static size_t comm_row(u32 world) { return std::max<size_t>({(size_t)world + 2, 3 * (size_t)world, 2 * (size_t)world + 3}); }
 
 static void comm_teardown(vb_ctx *c)
 {
@@ -2565,7 +2593,7 @@ extern "C" int32_t vb_shuffle_create_multi_dist(vb_ctx *c, uint64_t shuffle_id, 
 // the checks every _cols export / import call makes first
 static int multi_dist_check(const vb_shuf *s, const char *what)
 {
-    if (!s->multi) return set_err(VB_ERR_INVALID, "%s needs a shuffle from vb_shuffle_create_multi_dist", what);
+    if (!s->multi || s->str) return set_err(VB_ERR_INVALID, "%s needs a shuffle from vb_shuffle_create_multi_dist", what);
     if (s->world < 2) return set_err(VB_ERR_STATE, "%s needs a multi-aggregate shuffle of world > 1 (vb_shuffle_create_multi_dist)", what);
     return VB_OK;
 }
@@ -2877,7 +2905,7 @@ extern "C" int32_t vb_shuffle_exchange(vb_shuf *s, int32_t mode)
     if (s->str || s->multi) {
         std::lock_guard<std::mutex> lk(c->mu);
         CU(cudaSetDevice(c->device));
-        return s->str ? exchange_str_locked(s) : exchange_multi_locked(s);
+        return s->str ? (s->multi ? exchange_str_multi_locked(s) : exchange_str_locked(s)) : exchange_multi_locked(s);
     }
     if (mode == VB_XCHG_AUTO) mode = is_group_op(s->agg) ? VB_XCHG_P2P : VB_XCHG_NCCL;
     if (mode == VB_XCHG_P2P && !is_group_op(s->agg)) return set_err(VB_ERR_UNSUPPORTED, "the fused P2P exchange is for GROUP/COGROUP shuffles");
@@ -3308,6 +3336,7 @@ extern "C" int32_t vb_shuffle_reduce_cols(vb_shuf *s, uint32_t r, void *out_keys
 {
     if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
     if (!s->multi) return set_err(VB_ERR_INVALID, "vb_shuffle_reduce_cols needs a shuffle from vb_shuffle_create_multi");
+    if (s->str) return invalid_str(s, "vb_shuffle_reduce_cols (read it with vb_shuffle_reduce_str_cols)");
     if (r >= s->n_reduce) return set_err(VB_ERR_INVALID, "reduce_id %u >= n_reduce %u", r, s->n_reduce);
     if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
     TRY(wait_sealed(s));
@@ -4261,7 +4290,9 @@ struct StrState {
     StrCtl *ctl = nullptr;
     std::vector<u32 *> ids;               // per map id: the rows' entry ids (owned)
     std::vector<const u64 *> vals;        // per map id: the rows' values
-    std::vector<char> vals_owned;         // per map id: vals is a copy (else borrowed, VB_DEVICE_BORROWED)
+    struct Cols { const u64 *c[MA_MAX_COLS]; };
+    std::vector<Cols> cols;               // combine_by_key (vb_shuffle_create_str_multi), per map id: the value columns
+    std::vector<char> vals_owned;         // per map id: vals / cols are copies (else borrowed, VB_DEVICE_BORROWED)
     u64 *key_off = nullptr;               // [n_keys + 1] byte offset of every result key (partition-major, from 0)
     unsigned char *key_bytes = nullptr;   // the result keys' bytes
     std::vector<u64> kb_off;              // [n_reduce + 1] first key byte of each partition
@@ -4274,7 +4305,8 @@ struct StrState {
     u32 *x_lens = nullptr, *x_cnts = nullptr;
     unsigned char *x_bytes = nullptr;
     u64 *x_vals = nullptr;
-    // ... and the imported ones, source-rank major: borrowed until seal, or received by vb_shuffle_exchange (i_own)
+    // ... and the imported ones, source-rank major: borrowed until seal, or received by vb_shuffle_exchange (i_own).
+    // combine_by_key: x_vals / i_vals are the accumulators [n_acc][keys], in plain value form
     const u32 *i_lens = nullptr, *i_cnts = nullptr;
     const unsigned char *i_bytes = nullptr;
     const u64 *i_vals = nullptr;
@@ -4300,9 +4332,13 @@ static void free_str_map(vb_shuf *s, u32 m)
 {
     StrState *t = s->str;
     dev_free(s->ctx, t->ids[m]);
-    if (t->vals_owned[m]) dev_free(s->ctx, t->vals[m]);
+    if (t->vals_owned[m]) {
+        dev_free(s->ctx, t->vals[m]);
+        for (const u64 *p : t->cols[m].c) dev_free(s->ctx, p);
+    }
     t->ids[m] = nullptr;
     t->vals[m] = nullptr;
+    t->cols[m] = StrState::Cols{};
     t->vals_owned[m] = 0;
 }
 
@@ -4357,6 +4393,7 @@ extern "C" int32_t vb_shuffle_create_str(vb_ctx *c, uint64_t shuffle_id, uint32_
     StrState *t = new StrState();
     t->ids.assign(n_map, nullptr);
     t->vals.assign(n_map, nullptr);
+    t->cols.assign(n_map, StrState::Cols{});
     t->vals_owned.assign(n_map, 0);
     t->d.fp_mask = str_fp_mask();
     (*out)->str = t;
@@ -4510,17 +4547,12 @@ static int str_encode(vb_shuf *s, const u64 *offs, const unsigned char *bytes, u
     }
 }
 
-extern "C" int32_t vb_shuffle_map_str(vb_shuf *s, uint32_t map_id, const uint64_t *key_offsets, const void *key_bytes, uint64_t n_bytes,
-                                      const void *vals, uint64_t n, int32_t loc)
+// One map call of a string shuffle after the argument checks: the keys' entry ids, and the value columns in[0 .. n_in)
+// (a NULL column is neither read nor copied), copied, or borrowed for VB_DEVICE_BORROWED.  A single-column shuffle
+// passes its one column (none for COUNT), a combine_by_key shuffle every column an aggregate reads.
+static int str_map(vb_shuf *s, u32 map_id, const uint64_t *key_offsets, const void *key_bytes, u64 n_bytes, const u64 *const *in, u32 n_in,
+                   u64 n, int loc)
 {
-    if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
-    if (!s->str) return set_err(VB_ERR_INVALID, "vb_shuffle_map_str needs a shuffle from vb_shuffle_create_str");
-    if (map_id >= s->n_map) return set_err(VB_ERR_INVALID, "map_id %u >= n_map %u", map_id, s->n_map);
-    if (loc < VB_HOST || loc > VB_DEVICE_BORROWED) return set_err(VB_ERR_INVALID, "bad src_loc %d", loc);
-    if (n && !key_offsets) return set_err(VB_ERR_INVALID, "NULL key_offsets with n_rows > 0");
-    if (n && n_bytes && !key_bytes) return set_err(VB_ERR_INVALID, "NULL key_bytes with n_bytes > 0");
-    if (n && !vals && s->agg != VB_AGG_COUNT) return set_err(VB_ERR_INVALID, "values required for this aggregator");
-    if (n >= 0xFFFFFFFEull) return set_err(VB_ERR_TOO_LARGE, "map partition of %llu rows", (unsigned long long)n);
     {
         std::lock_guard<std::mutex> g(s->mu);
         if (s->sealed || s->sealing || s->freed) return set_err(VB_ERR_STATE, "shuffle %llu: map after seal", (unsigned long long)s->id);
@@ -4535,7 +4567,9 @@ extern "C" int32_t vb_shuffle_map_str(vb_shuf *s, uint32_t map_id, const uint64_
     for (u32 j = 0; j < s->n_map; ++j)
         if (j != map_id && s->maps[j].present) others += s->maps[j].n_rows;
     if (others + n >= 0xFFFFFFFEull) return set_err(VB_ERR_TOO_LARGE, "shuffle of %llu rows on one device", (unsigned long long)(others + n));
-    DevBuf d_offs(c), d_bytes(c), d_vals(c), ids(c);
+    DevBuf d_offs(c), d_bytes(c), ids(c);
+    DevBuf d_vals[MA_MAX_COLS];
+    for (DevBuf &b : d_vals) b.c = c;
     const u64 *offs = key_offsets;
     const unsigned char *bytes = (const unsigned char *)key_bytes;
     u64 first = 0, last = 0;
@@ -4555,9 +4589,10 @@ extern "C" int32_t vb_shuffle_map_str(vb_shuf *s, uint32_t map_id, const uint64_
         }
         TRY(ids.alloc(n * 4));
         TRY(str_encode(s, offs, bytes, first, n, last - first, n * std::max<u32>(1, s->n_map), s->hint, ids.as<u32>()));
-        if (s->agg != VB_AGG_COUNT && loc != VB_DEVICE_BORROWED) {
-            TRY(d_vals.alloc(n * 8));
-            CU(cudaMemcpyAsync(d_vals.p, vals, n * 8, loc == VB_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, c->stream));
+        for (u32 j = 0; j < n_in && loc != VB_DEVICE_BORROWED; ++j) {
+            if (!in[j]) continue;
+            TRY(d_vals[j].alloc(n * 8));
+            CU(cudaMemcpyAsync(d_vals[j].p, in[j], n * 8, loc == VB_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, c->stream));
             if (loc == VB_HOST) s->st.h2d_bytes += n * 8;
         }
     }
@@ -4567,9 +4602,13 @@ extern "C" int32_t vb_shuffle_map_str(vb_shuf *s, uint32_t map_id, const uint64_
         free_str_map(s, map_id);
     }
     t->ids[map_id] = (u32 *)ids.release();
-    if (n && s->agg != VB_AGG_COUNT) {
+    if (n && n_in) {
         t->vals_owned[map_id] = loc != VB_DEVICE_BORROWED;
-        t->vals[map_id] = loc == VB_DEVICE_BORROWED ? (const u64 *)vals : (const u64 *)d_vals.release();
+        for (u32 j = 0; j < n_in; ++j) {
+            const u64 *p = loc == VB_DEVICE_BORROWED ? in[j] : (const u64 *)d_vals[j].release();
+            if (s->multi) t->cols[map_id].c[j] = p;
+            else t->vals[map_id] = p;
+        }
     }
     m.present = true;
     m.n_rows = n;
@@ -4577,6 +4616,42 @@ extern "C" int32_t vb_shuffle_map_str(vb_shuf *s, uint32_t map_id, const uint64_
     CU(cudaStreamSynchronize(c->stream));          // the caller's key column is free again when the call returns
     TRY(call.done("map"));
     return VB_OK;
+}
+
+extern "C" int32_t vb_shuffle_map_str(vb_shuf *s, uint32_t map_id, const uint64_t *key_offsets, const void *key_bytes, uint64_t n_bytes,
+                                      const void *vals, uint64_t n, int32_t loc)
+{
+    if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
+    if (!s->str) return set_err(VB_ERR_INVALID, "vb_shuffle_map_str needs a shuffle from vb_shuffle_create_str");
+    if (s->multi) return set_err(VB_ERR_INVALID, "shuffle %llu has several aggregates per key: map it with vb_shuffle_map_str_cols", (unsigned long long)s->id);
+    if (map_id >= s->n_map) return set_err(VB_ERR_INVALID, "map_id %u >= n_map %u", map_id, s->n_map);
+    if (loc < VB_HOST || loc > VB_DEVICE_BORROWED) return set_err(VB_ERR_INVALID, "bad src_loc %d", loc);
+    if (n && !key_offsets) return set_err(VB_ERR_INVALID, "NULL key_offsets with n_rows > 0");
+    if (n && n_bytes && !key_bytes) return set_err(VB_ERR_INVALID, "NULL key_bytes with n_bytes > 0");
+    if (n && !vals && s->agg != VB_AGG_COUNT) return set_err(VB_ERR_INVALID, "values required for this aggregator");
+    if (n >= 0xFFFFFFFEull) return set_err(VB_ERR_TOO_LARGE, "map partition of %llu rows", (unsigned long long)n);
+    const u64 *col = (const u64 *)vals;
+    return str_map(s, map_id, key_offsets, key_bytes, n_bytes, &col, s->agg != VB_AGG_COUNT ? 1u : 0u, n, loc);
+}
+
+extern "C" int32_t vb_shuffle_map_str_cols(vb_shuf *s, uint32_t map_id, const uint64_t *key_offsets, const void *key_bytes, uint64_t n_bytes,
+                                           const void *const *vals, uint64_t n, int32_t loc)
+{
+    if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
+    if (!s->str || !s->multi) return set_err(VB_ERR_INVALID, "vb_shuffle_map_str_cols needs a shuffle from vb_shuffle_create_str_multi");
+    if (map_id >= s->n_map) return set_err(VB_ERR_INVALID, "map_id %u >= n_map %u", map_id, s->n_map);
+    if (loc < VB_HOST || loc > VB_DEVICE_BORROWED) return set_err(VB_ERR_INVALID, "bad src_loc %d", loc);
+    if (n && !key_offsets) return set_err(VB_ERR_INVALID, "NULL key_offsets with n_rows > 0");
+    if (n && n_bytes && !key_bytes) return set_err(VB_ERR_INVALID, "NULL key_bytes with n_bytes > 0");
+    const u64 *cols[MA_MAX_COLS] = {};
+    bool read[MA_MAX_COLS] = {};
+    for (u32 a = 0; a < s->acc_map.n; ++a)
+        if (spec_at(s->acc_map.op, a) != OPK_COUNT) read[spec_at(s->acc_map.src, a)] = true;
+    for (u32 i = 0; vals && i < s->n_cols; ++i) cols[i] = read[i] ? (const u64 *)vals[i] : nullptr;   // an unread column is not copied
+    for (u32 i = 0; i < s->n_cols; ++i)
+        if (n && read[i] && !cols[i]) return set_err(VB_ERR_INVALID, "value column %u is read by an aggregate but NULL", i);
+    if (n >= 0xFFFFFFFEull) return set_err(VB_ERR_TOO_LARGE, "map partition of %llu rows", (unsigned long long)n);
+    return str_map(s, map_id, key_offsets, key_bytes, n_bytes, cols, s->n_cols, n, loc);
 }
 
 template <int OPK, int TX>
@@ -4609,18 +4684,20 @@ static int str_reduce_rows(vb_shuf *s, int opk, int tx, const u32 *ids, const u6
     return set_err(VB_ERR_UNSUPPORTED, "string keys: op %d", s->agg);
 }
 
-// Rows as dictionary entry ids and their values: one map task's, or the rows a rank imported.
+// Rows as dictionary entry ids and their values: one map task's, or the rows a rank imported.  combine_by_key: a map
+// task's value columns in cols, or the imported accumulators [n_acc][n] in vals.
 struct StrRun {
     const u32 *ids;
     const u64 *vals;
     u64 n;
+    StrState::Cols cols{};
 };
 
 static std::vector<StrRun> str_map_runs(const vb_shuf *s)
 {
     std::vector<StrRun> runs;
     for (u32 m = 0; m < s->n_map; ++m)
-        if (s->maps[m].n_rows) runs.push_back(StrRun{s->str->ids[m], s->str->vals[m], s->maps[m].n_rows});
+        if (s->maps[m].n_rows) runs.push_back(StrRun{s->str->ids[m], s->str->vals[m], s->maps[m].n_rows, s->str->cols[m]});
     return runs;
 }
 
@@ -4733,6 +4810,56 @@ static int str_fold_values(vb_shuf *s, const std::vector<StrRun> &runs, int opk,
     return VB_OK;
 }
 
+// combine_by_key: acc [n_acc][D] = every accumulator of the spec folded over the rows of `runs`, by dense id, in the
+// spec's order transform (IN_SOA: the map rows and the map spec; IN_ACCS: imported partials and the merge spec).
+__global__ void range_kernel(u64 *__restrict__ out, u64 start, u64 step, u64 n);
+
+static int str_fold_multi(vb_shuf *s, const std::vector<StrRun> &runs, int in, const u32 *dense, u64 D, DevBuf &acc)
+{
+    vb_ctx *c = s->ctx;
+    const AccSpec &sp = in == IN_ACCS ? s->acc_imp : s->acc_map;
+    TRY(acc.alloc(D * 8 * sp.n));
+    for (u32 a = 0; a < sp.n; ++a) {
+        KLaunch kl(s, K_MISC);
+        str_fill_kernel<<<str_grid(c, D), 256, 0, c->stream>>>(acc.as<u64>() + (u64)a * D, D, op_identity(spec_at(sp.op, a)));
+        TRY(kl.done("str_fill_kernel"));
+    }
+    for (const StrRun &r : runs) {
+        MaCols mc{};
+        if (in == IN_ACCS) {
+            mc.c[0] = r.vals;
+            mc.stride = r.n;
+        } else {
+            std::copy(r.cols.c, r.cols.c + MA_MAX_COLS, mc.c);
+        }
+        auto kern = in == IN_ACCS ? str_reduce_multi_kernel<IN_ACCS> : str_reduce_multi_kernel<IN_SOA>;
+        const int occ = occupancy(c, kern, 256, 0);
+        const u64 blocks = std::min<u64>((r.n + 255) / 256, (u64)c->sm_count * occ);
+        KLaunch kl(s, K_HASH_AGG, r.n);
+        kern<<<(unsigned)blocks, 256, 0, c->stream>>>(r.ids, mc, r.n, dense, sp, D, acc.as<u64>());
+        TRY(kl.done("str_reduce_multi_kernel"));
+    }
+    return VB_OK;
+}
+
+// The output columns [outs.n][D] of the folded accumulators: multi_finalize_kernel's rules (inverse order transform;
+// MEAN = sum / count) over dense ids, read through an identity index.
+static int str_finalize_multi(vb_shuf *s, const u64 *acc, u64 D, DevBuf &out)
+{
+    vb_ctx *c = s->ctx;
+    DevBuf idx(c);
+    TRY(idx.alloc(D * 8));
+    TRY(out.alloc(D * 8 * s->outs.n));
+    {
+        KLaunch kl(s, K_MISC);
+        range_kernel<<<str_grid(c, D), 256, 0, c->stream>>>(idx.as<u64>(), 0, 1, D);
+        TRY(kl.done("range_kernel"));
+    }
+    KLaunch kl(s, K_MISC);
+    multi_finalize_kernel<<<str_grid(c, D), 256, 0, c->stream>>>(acc, D, idx.as<u64>(), D, s->outs, out.as<u64>());
+    return kl.done("multi_finalize_kernel");
+}
+
 // GROUP: the n rows of `runs`, concatenated in run order and stably sorted by dense id (seal_group's steps 4-7):
 // offs [D + 1] (the CSR) and vals [n].
 static int str_group_values(vb_shuf *s, const std::vector<StrRun> &runs, u64 n, const u32 *dense, u64 D, DevBuf &offs, DevBuf &vals)
@@ -4772,10 +4899,11 @@ static int str_group_values(vb_shuf *s, const std::vector<StrRun> &runs, u64 n, 
 // imported accumulators):
 //   1. mark the entries the rows reference;
 //   2. split the live entries by h % n_reduce into partition-major dense ids, and lay their bytes out in that order;
-//   3. reduce ops: one RED per (warp, distinct id) into acc[dense id];  GROUP: the rows in run order (map-id order, or
-//      source-rank major), stably sorted by dense id, then the CSR (seal_group's steps 4-7).
+//   3. reduce ops: one RED per (warp, distinct id) into acc[dense id];  combine_by_key: the same for every accumulator
+//      of the spec (`in`: map rows or imported partials), then the output columns;  GROUP: the rows in run order
+//      (map-id order, or source-rank major), stably sorted by dense id, then the CSR (seal_group's steps 4-7).
 // The per-map ids and the dictionary are freed at the end.
-static int seal_str_runs(vb_shuf *s, const std::vector<StrRun> &runs, int opk)
+static int seal_str_runs(vb_shuf *s, const std::vector<StrRun> &runs, int opk, int in = IN_SOA)
 {
     vb_ctx *c = s->ctx;
     StrState *t = s->str;
@@ -4793,7 +4921,13 @@ static int seal_str_runs(vb_shuf *s, const std::vector<StrRun> &runs, int opk)
         TRY(str_dense_keys(s, runs, order, cnt, s->bucket_off, dense, koff, kbytes));
         const u64 D = s->bucket_off[R];
         TRY(str_read_at(s, koff.as<u64>(), s->bucket_off, t->kb_off));
-        if (is_reduce_op(s->agg)) {
+        if (s->multi) {                // combine_by_key: fold every accumulator, then the output columns
+            DevBuf acc(c), out(c);
+            TRY(str_fold_multi(s, runs, in, dense.as<u32>(), D, acc));
+            TRY(str_finalize_multi(s, acc.as<u64>(), D, out));
+            s->res_cols = (u64 *)out.release();
+            s->st.rows_out = D;
+        } else if (is_reduce_op(s->agg)) {
             DevBuf acc(c);
             TRY(str_fold_values(s, runs, opk, val_tx(s), dense.as<u32>(), D, acc));
             s->res_comb = (u64 *)acc.release();
@@ -4864,7 +4998,19 @@ static int export_str_locked(vb_shuf *s, u64 *n_keys, u64 *n_key_bytes, u64 *n_v
             str_diff_u32_kernel<<<str_grid(c, D), 256, 0, c->stream>>>(koff.as<u64>(), D, lens.as<u32>());
             TRY(kl.done("str_diff_u32_kernel"));
         }
-        if (is_reduce_op(s->agg)) {
+        if (s->multi) {                // combine_by_key: every accumulator of the map spec, in plain value form
+            DevBuf acc(c);
+            TRY(str_fold_multi(s, runs, IN_SOA, dense.as<u32>(), D, acc));
+            for (u32 a = 0; a < s->acc_map.n; ++a) {
+                const int tx = spec_at(s->acc_map.tx, a);
+                if (tx == TX_NONE) continue;
+                KLaunch kl(s, K_MISC);
+                tx_inv_kernel<<<(unsigned)((D + 255) / 256), 256, 0, c->stream>>>(acc.as<u64>() + (u64)a * D, D, tx);
+                TRY(kl.done("tx_inv_kernel"));
+            }
+            for (u32 d = 0; d < W; ++d) n_vals[d] = n_keys[d];
+            t->x_vals = (u64 *)acc.release();
+        } else if (is_reduce_op(s->agg)) {
             DevBuf acc(c);
             TRY(str_fold_values(s, runs, map_opk(s), val_tx(s), dense.as<u32>(), D, acc));
             for (u32 d = 0; d < W; ++d) n_vals[d] = n_keys[d];
@@ -4957,7 +5103,7 @@ static int seal_str_import(vb_shuf *s)
             runs.push_back(StrRun{ids.as<u32>(), t->i_vals, nk});
         }
     }
-    TRY(seal_str_runs(s, runs, merge_opk(s)));
+    TRY(seal_str_runs(s, runs, merge_opk(s), IN_ACCS));
     free_str_xchg(s);
     return VB_OK;
 }
@@ -4977,7 +5123,7 @@ extern "C" int32_t vb_shuffle_create_str_dist(vb_ctx *c, uint64_t shuffle_id, ui
 // the checks every string export / import call makes first
 static int str_dist_check(const vb_shuf *s, const char *what)
 {
-    if (!s->str) return set_err(VB_ERR_INVALID, "%s needs a shuffle from vb_shuffle_create_str_dist", what);
+    if (!s->str || s->multi) return set_err(VB_ERR_INVALID, "%s needs a shuffle from vb_shuffle_create_str_dist", what);
     if (s->world < 2) return set_err(VB_ERR_STATE, "%s needs a string shuffle of world > 1 (vb_shuffle_create_str_dist)", what);
     return VB_OK;
 }
@@ -5083,7 +5229,7 @@ extern "C" int32_t vb_shuffle_reduce_str_size(vb_shuf *s, uint32_t r, uint64_t *
     TRY(wait_sealed(s));
     if (n_keys) *n_keys = s->bucket_off[r + 1] - s->bucket_off[r];
     if (n_key_bytes) *n_key_bytes = s->str->kb_off[r + 1] - s->str->kb_off[r];
-    if (n_vals) *n_vals = is_group_op(s->agg) ? s->val_off[r + 1] - s->val_off[r] : 0;
+    if (n_vals) *n_vals = is_group_op(s->agg) ? s->val_off[r + 1] - s->val_off[r] : s->multi ? s->bucket_off[r + 1] - s->bucket_off[r] : 0;
     return VB_OK;
 }
 
@@ -5112,6 +5258,8 @@ extern "C" int32_t vb_shuffle_reduce_str(vb_shuf *s, uint32_t r, uint64_t *out_k
     if (!s->str) return set_err(VB_ERR_INVALID, "vb_shuffle_reduce_str needs a shuffle from vb_shuffle_create_str");
     if (r >= s->n_reduce) return set_err(VB_ERR_INVALID, "reduce_id %u >= n_reduce %u", r, s->n_reduce);
     if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
+    if (s->multi && (out_combined || out_offsets || out_vals))
+        return set_err(VB_ERR_INVALID, "shuffle %llu has several aggregates per key: read them with vb_shuffle_reduce_str_cols", (unsigned long long)s->id);
     TRY(wait_sealed(s));
     vb_ctx *c = s->ctx;
     std::lock_guard<std::mutex> lk(c->mu);
@@ -5129,6 +5277,168 @@ extern "C" int32_t vb_shuffle_reduce_str(vb_shuf *s, uint32_t r, uint64_t *out_k
         TRY(copy_out(s, out_combined, s->res_comb ? s->res_comb + b0 : nullptr, nk * 8, dst_loc));
     }
     CU(cudaStreamSynchronize(c->stream));
+    return VB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// combine_by_key over string keys (vb_shuffle_create_str_multi): the string map and seal steps (dictionary encode,
+// dense ids by partition) with the accumulators of vb_shuffle_create_multi folded over dense ids
+// (str_reduce_multi_kernel) and finalized by the integer combine's rules.  Across ranks the string wire columns carry
+// the accumulators [n_acc][keys] in the plain value form of vb_shuffle_export_cols_buffers.
+// ---------------------------------------------------------------------------------------------
+extern "C" int32_t vb_shuffle_create_str_multi(vb_ctx *c, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce, uint32_t n_val_cols,
+                                               const int32_t *val_dtypes, uint32_t n_aggs, const vb_agg_col *aggs, vb_shuf **out)
+{
+    if (!c || !out || !val_dtypes || !aggs) return set_err(VB_ERR_INVALID, "vb_shuffle_create_str_multi: NULL argument");
+    *out = nullptr;
+    MultiSpec ms;
+    TRY(multi_spec(n_val_cols, val_dtypes, n_aggs, aggs, &ms));
+    TRY(vb_shuffle_create_str(c, shuffle_id, n_map, n_reduce, VB_U64, VB_AGG_SUM, out));
+    set_multi(*out, ms);
+    return VB_OK;
+}
+
+extern "C" int32_t vb_shuffle_create_str_multi_dist(vb_ctx *c, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce, uint32_t n_val_cols,
+                                                    const int32_t *val_dtypes, uint32_t n_aggs, const vb_agg_col *aggs, uint32_t rank,
+                                                    uint32_t world, vb_shuf **out)
+{
+    if (!c || !out) return set_err(VB_ERR_INVALID, "vb_shuffle_create_str_multi_dist: NULL argument");
+    *out = nullptr;
+    if (world < 1 || world > 256 || rank >= world) return set_err(VB_ERR_INVALID, "bad rank %u / world %u (1 <= world <= 256)", rank, world);
+    TRY(vb_shuffle_create_str_multi(c, shuffle_id, n_map, n_reduce, n_val_cols, val_dtypes, n_aggs, aggs, out));
+    (*out)->rank = rank;
+    (*out)->world = world;
+    return VB_OK;
+}
+
+extern "C" int32_t vb_shuffle_reduce_str_cols(vb_shuf *s, uint32_t r, uint64_t *out_key_offsets, void *out_key_bytes, void *const *out_aggs,
+                                              int32_t dst_loc)
+{
+    if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
+    if (!s->str || !s->multi) return set_err(VB_ERR_INVALID, "vb_shuffle_reduce_str_cols needs a shuffle from vb_shuffle_create_str_multi");
+    if (r >= s->n_reduce) return set_err(VB_ERR_INVALID, "reduce_id %u >= n_reduce %u", r, s->n_reduce);
+    if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
+    TRY(wait_sealed(s));
+    vb_ctx *c = s->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    StrState *t = s->str;
+    const u64 b0 = s->bucket_off[r], nk = s->bucket_off[r + 1] - b0;
+    const u64 kb0 = t->kb_off[r], nkb = t->kb_off[r + 1] - kb0;
+    TRY(copy_out_rebased(s, out_key_offsets, t->key_off ? t->key_off + b0 : nullptr, nk, kb0, dst_loc));
+    TRY(copy_out(s, out_key_bytes, t->key_bytes ? t->key_bytes + kb0 : nullptr, nkb, dst_loc));
+    for (u32 o = 0; out_aggs && o < s->outs.n; ++o)
+        TRY(copy_out(s, out_aggs[o], s->res_cols ? s->res_cols + (u64)o * s->n_keys + b0 : nullptr, nk * 8, dst_loc));
+    CU(cudaStreamSynchronize(c->stream));
+    return VB_OK;
+}
+
+// the checks every string _cols export / import call makes first
+static int str_multi_dist_check(const vb_shuf *s, const char *what)
+{
+    if (!s->str || !s->multi) return set_err(VB_ERR_INVALID, "%s needs a shuffle from vb_shuffle_create_str_multi_dist", what);
+    if (s->world < 2) return set_err(VB_ERR_STATE, "%s needs a string-key combine shuffle of world > 1 (vb_shuffle_create_str_multi_dist)", what);
+    return VB_OK;
+}
+
+extern "C" int32_t vb_shuffle_export_str_cols_prepare(vb_shuf *s, uint64_t *n_keys, uint64_t *n_key_bytes)
+{
+    if (!s || !n_keys || !n_key_bytes) return set_err(VB_ERR_INVALID, "NULL argument");
+    TRY(str_multi_dist_check(s, "vb_shuffle_export_str_cols_prepare"));
+    vb_ctx *c = s->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    std::vector<u64> n_vals(s->world);
+    TRY(export_str_locked(s, n_keys, n_key_bytes, n_vals.data()));
+    CU(cudaStreamSynchronize(c->stream));
+    return VB_OK;
+}
+
+extern "C" int32_t vb_shuffle_export_str_cols_buffers(vb_shuf *s, uint32_t **key_lens, void **key_bytes, uint64_t **accs, uint32_t *n_acc)
+{
+    if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
+    TRY(str_multi_dist_check(s, "vb_shuffle_export_str_cols_buffers"));
+    {
+        std::lock_guard<std::mutex> g(s->mu);
+        if (!s->exported || s->sealed || s->freed)
+            return set_err(VB_ERR_STATE, "vb_shuffle_export_str_cols_buffers needs vb_shuffle_export_str_cols_prepare first and no seal yet");
+    }
+    const StrState *t = s->str;
+    if (key_lens) *key_lens = t->x_lens;
+    if (key_bytes) *key_bytes = t->x_bytes;
+    if (accs) *accs = t->x_vals;
+    if (n_acc) *n_acc = s->acc_map.n;
+    return VB_OK;
+}
+
+extern "C" int32_t vb_shuffle_import_str_cols(vb_shuf *s, const uint32_t *key_lens, const void *key_bytes, const uint64_t *accs, uint32_t n_acc,
+                                              const uint64_t *n_keys, const uint64_t *n_key_bytes)
+{
+    if (!s || !n_keys || !n_key_bytes) return set_err(VB_ERR_INVALID, "NULL argument");
+    TRY(str_multi_dist_check(s, "vb_shuffle_import_str_cols"));
+    if (n_acc != s->acc_map.n) return set_err(VB_ERR_INVALID, "%u accumulator columns imported, the shuffle has %u", n_acc, s->acc_map.n);
+    {
+        std::lock_guard<std::mutex> g(s->mu);
+        if (!s->exported || s->imported || s->sealed || s->sealing || s->freed)
+            return set_err(VB_ERR_STATE, "vb_shuffle_import_str_cols needs vb_shuffle_export_str_cols_prepare first, once, and no seal yet");
+    }
+    u64 nk = 0, nkb = 0;
+    for (u32 r = 0; r < s->world; ++r) { nk += n_keys[r]; nkb += n_key_bytes[r]; }
+    if ((nk && (!key_lens || !accs)) || (nkb && !key_bytes)) return set_err(VB_ERR_INVALID, "NULL column with a non-zero count");
+    TRY(str_import_limits(s, nk, nk));
+    StrState *t = s->str;
+    t->i_lens = key_lens; t->i_bytes = (const unsigned char *)key_bytes; t->i_cnts = nullptr; t->i_vals = accs;
+    t->i_nk = nk; t->i_nkb = nkb; t->i_nv = nk;
+    std::lock_guard<std::mutex> g(s->mu);
+    s->imported = true;
+    return VB_OK;
+}
+
+// vb_shuffle_exchange of a string-key combine: export, then the exchange of 2 + n_acc columns: u32 key lengths and the
+// n_acc u64 accumulator columns split by the key counts, key bytes by the byte counts.  The gathered row is the key and
+// byte counts to every destination, then exchange_multi_locked's spec fingerprint (no key width: keys are strings),
+// so a rank whose spec differs is refused on every rank before any send.
+static int exchange_str_multi_locked(vb_shuf *s)
+{
+    vb_ctx *c = s->ctx;
+    Comm *m = c->comm;
+    StrState *t = s->str;
+    const u32 W = m->world, me = m->rank, NA = s->acc_map.n;
+    const size_t len = 2 * (size_t)W + 3;        // n_keys[W], n_key_bytes[W], the fingerprint
+    std::vector<u64> row(len, 0), n_vals(W);
+    auto clk = std::chrono::steady_clock::now();
+    TRY(export_str_locked(s, row.data(), row.data() + W, n_vals.data()));
+    s->xst.prepare_wall_ms += lap(clk);
+    row[2 * W] = s->acc_map.op;
+    row[2 * W + 1] = s->acc_map.tx;
+    row[2 * W + 2] = (u64)NA | (u64)s->n_reduce << 32;
+    const u64 *mat = nullptr;
+    TRY(comm_all_gather(c, row.data(), len, &mat));
+    s->xst.counts_wall_ms += lap(clk);
+    for (u32 p = 1; p < W; ++p)
+        for (u32 i = 0; i < 3; ++i)
+            if (mat[p * len + 2 * W + i] != mat[2 * W + i])
+                return set_err(VB_ERR_INVALID, "rank %u's combine spec differs from rank 0's (accumulators, ops, transforms or n_reduce)", p);
+    for (u32 d = 0; d < W; ++d) {
+        const u64 nd = xsplit(mat, len, W, d, 0).roff[W];
+        TRY(str_import_limits(s, nd, nd));
+    }
+    const std::vector<XSplit> sp{xsplit(mat, len, W, me, 0), xsplit(mat, len, W, me, 1)};
+    const u64 n_sent = sp[0].soff[W], nk = sp[0].roff[W], nkb = sp[1].roff[W];
+    DevBuf lens(c), bytes(c), accs(c);
+    TRY(lens.alloc(nk * 4));
+    TRY(bytes.alloc(nkb));
+    TRY(accs.alloc(nk * 8 * NA));
+    std::vector<XCol> cols{{ncclUint32, t->x_lens, lens.p, 0}, {ncclUint8, t->x_bytes, bytes.p, 1}};
+    for (u32 a = 0; a < NA; ++a) cols.push_back({ncclUint64, t->x_vals + (u64)a * n_sent, accs.as<u64>() + (u64)a * nk, 0});
+    TRY(post_group(s, xfers(sp, cols, W)));
+    s->xst.post_wall_ms += lap(clk);
+    xchg_done(s, VB_XCHG_NCCL, n_sent - sp[0].send[me], nk - sp[0].recv[me]);
+    t->i_lens = lens.as<u32>(); t->i_bytes = bytes.as<unsigned char>(); t->i_cnts = nullptr; t->i_vals = accs.as<u64>();
+    t->i_nk = nk; t->i_nkb = nkb; t->i_nv = nk;
+    t->i_own[0] = lens.release(); t->i_own[1] = bytes.release(); t->i_own[3] = accs.release();
+    std::lock_guard<std::mutex> g(s->mu);
+    s->imported = true;
     return VB_OK;
 }
 

@@ -311,6 +311,69 @@ __global__ void __launch_bounds__(256) str_reduce_kernel(const u32 *__restrict__
     }
 }
 
+// v op x for a run-time reduce op (warp-uniform); str_reduce_kernel's fold with the op taken from an AccSpec
+VB_D u64 op_fold_rt(int opk, u64 v, u64 x)
+{
+    switch (opk) {
+    case OPK_ADD_F64: return (u64)__double_as_longlong(__longlong_as_double((long long)v) + __longlong_as_double((long long)x));
+    case OPK_MIN_U64: return x < v ? x : v;
+    case OPK_MAX_U64: return x > v ? x : v;
+    default: return v + x;                                        // OPK_ADD_U64, and a COUNT's ones
+    }
+}
+
+// combine_by_key over dense ids: str_reduce_kernel with the accumulator list of `sp` (acc is [sp.n][D], each column
+// initialised to its op's identity).  One match-any per warp on the dense id; then, accumulator by accumulator (a
+// run-time loop: hash_agg_multi spilled when unrolled), load the value, ma_prep it, fold it into the id's leader lane
+// and issue one RED.  IN_SOA: value src(a) of map row i from cols.c[src] (a COUNT counts ones); IN_ACCS: partial a of
+// received row i at cols.c[0][a * cols.stride + i], merged with the merge spec (COUNT as ADD).
+template <int IN>
+__global__ void __launch_bounds__(256) str_reduce_multi_kernel(const u32 *__restrict__ ids, MaCols cols, u64 n,
+                                                               const u32 *__restrict__ dense_of_entry, AccSpec sp, u64 D, u64 *__restrict__ acc)
+{
+    static_assert(IN == IN_SOA || IN == IN_ACCS, "map rows or received partials");
+    const u32 lane = lane_id();
+    const u64 warp0 = ((u64)blockIdx.x * blockDim.x + threadIdx.x) & ~31ull;
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    const u64 ops = sp.op, txs = sp.tx, srcs = sp.src;
+    const int n_acc = (int)sp.n;
+    for (u64 w = warp0; w < n; w += stride) {
+        const u64 i = w + lane;
+        const bool ok = i < n;
+        const u32 dn = ok ? dense_of_entry[ids[i]] : STR_UNPUBLISHED;
+        const u32 peers = __match_any_sync(0xFFFFFFFFu, dn);
+        const bool lead = (__ffs(peers) - 1) == (int)lane;
+        const bool distinct = __all_sync(0xFFFFFFFFu, peers == (1u << lane));
+#pragma unroll 1
+        for (int a = 0; a < n_acc; ++a) {
+            const int op = spec_at(ops, a), red = merge_op(op);
+            u64 v = 0;
+            if (ok) {
+                if constexpr (IN == IN_ACCS) {
+                    v = ma_prep(cols.c[0][(u64)a * cols.stride + i], op, spec_at(txs, a));
+                } else if (op == OPK_COUNT) {
+                    v = 1;
+                } else {
+                    const int src = spec_at(srcs, a);
+                    const u64 *col = cols.c[0];
+#pragma unroll
+                    for (int c = 1; c < MA_MAX_COLS; ++c)
+                        if (src == c) col = cols.c[c];
+                    v = ma_prep(col[i], op, spec_at(txs, a));
+                }
+            }
+            if (!distinct) {                                          // some id repeats in this warp: fold into its leader
+                for (u32 j = 0; j < 32; ++j) {
+                    const u64 x = __shfl_sync(0xFFFFFFFFu, v, j);
+                    if (!lead || j == lane || !((peers >> j) & 1u)) continue;
+                    v = op_fold_rt(red, v, x);
+                }
+            }
+            if (ok && lead) op_red_rt(&acc[(u64)a * D + dn], red, v);
+        }
+    }
+}
+
 // ---- across ranks (engine.cu, "string keys across ranks") --------------------------------------------------------
 // The wire columns carry a u32 length per key and, for GROUP, a u32 value count per key, so that the host can
 // concatenate slices of them without rebasing anything.

@@ -10,13 +10,16 @@ tests) delivers them: all_to_all_v, the one exchange of every shuffle kind.  Red
 owned by rank r % world; map partitions are assigned to ranks in contiguous blocks so that the
 source-rank-major receive order IS map-id order (group value order, SURVEY.md F5).
 
-The columns of each kind (run_shuffle, run_str_shuffle and run_combine_shuffle share one driver, _exchange):
+The columns of each kind (run_shuffle, run_str_shuffle, run_combine_shuffle and run_str_combine_shuffle share one
+driver, _exchange):
 - integer rows (CudaEngine): keys and values, both split by the row counts.  Reduce ops exchange *combined* rows
   (≤ distinct keys per rank — map-side combine, src/dependency.rs:203-209), group ops raw rows.
 - String keys (StrCudaEngine): u32 key lengths and u32 value counts (GROUP) split by the key counts, key bytes by the
   byte counts, u64 values by the value counts.
 - combine_by_key (CombineCudaEngine): one row per distinct key, the key and the partial of every accumulator, packed
   as one [rows][1 + n_acc] column.
+- combine_by_key over String keys (StrCombineCudaEngine): u32 key lengths split by the key counts, key bytes by the
+  byte counts, and the partials of every accumulator packed as one [keys][n_acc] column split by the key counts.
 
 The exchange itself lives in libvega_b200.so (vb_ctx_comm_init + vb_shuffle_exchange: NCCL grouped
 send/recv, or the fused peer-memory scatter, on the library's stream).  The run_*shuffle functions call it
@@ -358,6 +361,68 @@ def run_combine_shuffle(engine, local_maps, n_map, n_reduce, kcode, multi, rank,
         engine.map(sh, map_id, keys, cols)
     return _exchange(engine, sh, (CombineCudaEngine, _combine_export, _combine_import, 0), rank, world, group, stats,
                      exchange_device)
+
+
+class StrCombineCudaEngine:
+    """libvega_b200 on this rank's GPU, for combine_by_key over String keys: CudaEngine's calls over
+    vb_shuffle_create_str_multi_dist.  multi is StrShuffle's (value column dtype codes, [(vb_agg, column), ...]).  export
+    gives ((n_keys, n_key_bytes) per destination, (key_lens, key_bytes, accs)), accs an (n_acc, keys) view, the wire
+    columns of include/vega_b200.h; import_ takes the same shape, source-rank major."""
+
+    def __init__(self, sc):
+        self.sc = sc
+
+    def create(self, n_map, n_reduce, multi, rank, world, hint=0):
+        return StrShuffle(self.sc, n_map, n_reduce, L.VB_U64, L.VB_AGG_SUM, hint=hint, rank=rank, world=world, multi=multi)
+
+    def map(self, sh, map_id, keys, cols):
+        """keys: a StrKeys column or a sequence of str; cols: the value columns (numpy arrays or torch CUDA tensors of
+        the keys' location)."""
+        k = keys if isinstance(keys, _StrCol) else _StrCol(keys)
+        cs = tuple(c if isinstance(c, _Col) else _Col(c, role="value") for c in cols)
+        sh.map_cols(map_id, k, cs, 0, k.n)
+
+    def export(self, sh, world):
+        return sh.export_cols()
+
+    def import_(self, sh, cols, counts):
+        sh.import_cols(*cols, *counts)
+
+    def seal(self, sh):
+        sh.seal()
+
+    def reduce(self, sh, r, out_dtypes):
+        return sh.reduce_cols(r, out_dtypes)
+
+
+def _str_combine_export(engine, sh, world):
+    """The accumulators travel as one [keys][n_acc] column beside the key lengths and bytes."""
+    (n_keys, n_key_bytes), (lens, data, accs) = engine.export(sh, world)
+    return [lens, data, accs.t().contiguous()], [n_keys, n_key_bytes, n_keys]
+
+
+def _str_combine_import(engine, sh, cols, splits):
+    engine.import_(sh, (cols[0], cols[1], cols[2].t().contiguous()), (splits[0], splits[1]))
+
+
+def run_str_combine_shuffle(engine, local_maps, n_map, n_reduce, multi, rank, world, group=None, hint=0, stats=None,
+                            exchange_device=None):
+    """run_shuffle for combine_by_key over String keys: map side on this rank's partitions → exchange → reduce side for
+    the partitions this rank owns.  local_maps: [(map_id, keys, value columns)], ascending map ids from
+    map_block(rank, world, n_map).  With a communicator on the context the exchange is vb_shuffle_exchange (NCCL inside
+    the library); otherwise all_to_all_v of the key lengths, key bytes and the [keys][n_acc] partials (exchange_device:
+    "cpu" for a gloo group on a one-GPU box)."""
+    if not 0 <= rank < world <= 256:
+        raise ValueError(f"rank {rank} of world {world}: 0 <= rank < world <= 256")
+    lo, hi = map_block(rank, world, n_map)
+    ids = [m for m, _, _ in local_maps]
+    if any(not lo <= m < hi for m in ids) or ids != sorted(set(ids)):
+        raise ValueError(f"rank {rank} runs map tasks {ids}: ascending ids in its block [{lo}, {hi}) expected")
+    sh = engine.create(n_map, n_reduce, multi, rank, world, hint=hint)
+    for map_id, keys, cols in local_maps:
+        engine.map(sh, map_id, keys, cols)
+    return _exchange(engine, sh, (StrCombineCudaEngine, _str_combine_export, _str_combine_import, 0), rank, world, group,
+                     stats, exchange_device)
 
 
 def owned_partitions(rank, world, n_reduce):

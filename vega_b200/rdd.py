@@ -8,7 +8,8 @@ Differences forced by the boundary (SURVEY.md F4): rows are 64-bit POD (K,V) arr
 (numpy on the host or torch CUDA tensors), and `reduce_by_key` takes a *named* op
 ("sum" | "min" | "max") because a closure cannot cross into CUDA.  Keys may also be Rust `String`s: a
 sequence of Python `str` or a `StrKeys` column (offsets + UTF-8 bytes), for reduce_by_key / count_by_key /
-group_by_key / partition_by_key / count_by_value / distinct; they are placed as the reference places `String` keys.
+group_by_key / partition_by_key / combine_by_key / count_by_value / distinct; they are placed as the reference places
+`String` keys.
 
 All compute happens in libvega_b200.so; this module slices the input exactly like
 ParallelCollection::slice, drives map tasks → seal → reduce tasks like the scheduler does
@@ -144,11 +145,17 @@ class Context:
     def parallelize(self, data, num_slices, values=None):
         """`sc.parallelize(vec, num_slices)`.  data: 1-D keys (→ Rdd), (n,2) rows or
         (keys, values) (→ PairRdd).  values may also be a tuple of up to 4 value columns (combine_by_key).
-        String keys (a sequence of str, a numpy str array or a StrKeys column) give a StrRdd / StrPairRdd."""
+        String keys (a sequence of str, a numpy str array or a StrKeys column) give a StrRdd / StrPairRdd; a tuple of
+        value columns gives a StrPairRdd with value columns, the one kind whose combine_by_key runs."""
         if _is_str_keys(data):
             keys = _StrCol(data)
             if values is None:
                 return StrRdd(self, keys, num_slices)
+            if isinstance(values, tuple) and values and all(_is_torch(v) or np.ndim(v) >= 1 for v in values):
+                if not 1 <= len(values) <= L.VB_MAX_VAL_COLS:
+                    raise ValueError(f"{len(values)} value columns: 1 to {L.VB_MAX_VAL_COLS} are supported")
+                cols = tuple(_Col(v, role="value") for v in values)
+                return StrPairRdd(self, keys, cols[0] if len(cols) == 1 else None, num_slices, cols=cols)
             return StrPairRdd(self, keys, _Col(values, role="value"), num_slices)
         if values is None and isinstance(data, tuple) and len(data) == 2 and _is_str_keys(data[0]):
             return StrPairRdd(self, _StrCol(data[0]), _Col(data[1], role="value"), num_slices)
@@ -830,38 +837,43 @@ class CoGroupedRdd(_Base):
         return np.concatenate([p[0] for p in parts]), [cat([p[1][j] for p in parts]) for j in range(len(self.rdds))]
 
 
+def _combine_spec(aggs, cols, num_splits):
+    """combine_by_key's arguments over value columns `cols` (ValueError before any device work): the vb_agg_col spec
+    [(vb_agg, column)], the aggregate names and each aggregate's output dtype, in the order given."""
+    if num_splits < 1:
+        raise ValueError("num_splits must be >= 1")
+    if not hasattr(aggs, "items") or not aggs:
+        raise ValueError("aggs must be a non-empty mapping name -> (op, column)")
+    spec, names = [], []
+    for name, item in aggs.items():
+        if not isinstance(item, (tuple, list)) or len(item) != 2:
+            raise ValueError(f"aggregate {name!r}: expected (op, column), got {item!r}")
+        op, col = item
+        if op not in _COMBINE_OPS:
+            raise ValueError(f"aggregate {name!r}: op {op!r} is not one of {sorted(_COMBINE_OPS)}")
+        if op == "count":
+            col = 0
+        elif not isinstance(col, (int, np.integer)) or isinstance(col, bool) or not 0 <= col < len(cols):
+            raise ValueError(f"aggregate {name!r}: column {col!r} out of range for {len(cols)} value columns")
+        spec.append((_COMBINE_OPS[op], int(col)))
+        names.append(name)
+    ops = [op for op, _ in aggs.values()]
+    n_acc = len(ops) + (1 if "mean" in ops and "count" not in ops else 0)
+    if n_acc > L.VB_MAX_AGGS:
+        raise ValueError(f"{len(ops)} aggregates{' plus the count a mean needs' if n_acc > len(ops) else ''} "
+                         f"exceed {L.VB_MAX_AGGS}")
+    out_dtypes = [np.uint64 if a == L.VB_AGG_COUNT else np.float64 if a == L.VB_AGG_MEAN else _NP_OF[cols[c].code]
+                  for a, c in spec]
+    return spec, names, out_dtypes
+
+
 class CombinedRdd(_Base):
     """`combine_by_key` with named aggregates (src/rdd/pair_rdd.rs:20-33): one shuffle, several aggregates per key.
     `compute(r)` / `collect()` return (keys, {name: array}) with the aggregates in the order they were given."""
 
     def __init__(self, parent, aggs, num_splits, hint=0):
-        if num_splits < 1:
-            raise ValueError("num_splits must be >= 1")
-        if not hasattr(aggs, "items") or not aggs:
-            raise ValueError("aggs must be a non-empty mapping name -> (op, column)")
-        cols = parent.cols
-        spec, names = [], []
-        for name, item in aggs.items():
-            if not isinstance(item, (tuple, list)) or len(item) != 2:
-                raise ValueError(f"aggregate {name!r}: expected (op, column), got {item!r}")
-            op, col = item
-            if op not in _COMBINE_OPS:
-                raise ValueError(f"aggregate {name!r}: op {op!r} is not one of {sorted(_COMBINE_OPS)}")
-            if op == "count":
-                col = 0
-            elif not isinstance(col, (int, np.integer)) or isinstance(col, bool) or not 0 <= col < len(cols):
-                raise ValueError(f"aggregate {name!r}: column {col!r} out of range for {len(cols)} value columns")
-            spec.append((_COMBINE_OPS[op], int(col)))
-            names.append(name)
-        ops = [op for op, _ in aggs.values()]
-        n_acc = len(ops) + (1 if "mean" in ops and "count" not in ops else 0)
-        if n_acc > L.VB_MAX_AGGS:
-            raise ValueError(f"{len(ops)} aggregates{' plus the count a mean needs' if n_acc > len(ops) else ''} "
-                             f"exceed {L.VB_MAX_AGGS}")
+        self.spec, self.names, self.out_dtypes = _combine_spec(aggs, parent.cols, num_splits)
         self.parent, self.num_slices, self.hint, self.sc = parent, num_splits, hint, parent.sc
-        self.spec, self.names = spec, names
-        self.out_dtypes = [np.uint64 if a == L.VB_AGG_COUNT else np.float64 if a == L.VB_AGG_MEAN else _NP_OF[cols[c].code]
-                           for a, c in spec]
         self._sh = None
 
     def _run(self):
@@ -1206,16 +1218,29 @@ class _DevView:
 
 class StrShuffle(Shuffle):
     """One string-key shuffle (vb_shuffle_create_str; vb_shuffle_create_str_dist for rank `rank` of `world` > 1).
-    seal / exchange / stats / free as for Shuffle."""
+    multi: (value column dtype codes, [(vb_agg, column), ...]) for a combine_by_key shuffle (vb_shuffle_create_str_multi /
+    _dist; vcode and agg are then ignored), mapped with map_cols and read with reduce_cols, exchanged with export_cols /
+    import_cols.  seal / exchange / stats / free as for Shuffle."""
 
-    def __init__(self, sc, n_map, n_reduce, vcode, agg, hint=0, rank=0, world=1):
+    def __init__(self, sc, n_map, n_reduce, vcode, agg, hint=0, rank=0, world=1, multi=None):
         self.sc, self._lib = sc, sc._lib
         self.n_map, self.n_reduce, self.agg, self.vcode, self.kcode = n_map, n_reduce, agg, vcode, None
         self.rank, self.world = rank, world
         self.has_payload = True
         self._keepalive = []
         h = ctypes.c_void_p()
-        if world > 1:
+        if multi is not None:
+            self.agg, self.vcode = L.VB_AGG_SUM, L.VB_U64
+            codes, aggs = multi
+            dts = (ctypes.c_int32 * len(codes))(*codes)
+            spec = (L.vb_agg_col * len(aggs))(*[L.vb_agg_col(a, c) for a, c in aggs])
+            if world > 1:
+                L.check(self._lib.vb_shuffle_create_str_multi_dist(sc._h, sc.new_shuffle_id(), n_map, n_reduce, len(codes), dts,
+                                                                   len(aggs), spec, rank, world, ctypes.byref(h)))
+            else:
+                L.check(self._lib.vb_shuffle_create_str_multi(sc._h, sc.new_shuffle_id(), n_map, n_reduce, len(codes), dts,
+                                                              len(aggs), spec, ctypes.byref(h)))
+        elif world > 1:
             L.check(self._lib.vb_shuffle_create_str_dist(sc._h, sc.new_shuffle_id(), n_map, n_reduce, vcode, agg, rank, world,
                                                          ctypes.byref(h)))
         else:
@@ -1306,11 +1331,82 @@ class StrShuffle(Shuffle):
         L.check(self._lib.vb_shuffle_reduce_str(self._h, r, p(out_key_offsets), p(out_key_bytes), p(out_comb), p(out_offs),
                                                 p(out_vals), L.VB_DEVICE))
 
+    # ---- combine_by_key (multi=) ----
+    def map_cols(self, map_id, keys, cols, start, stop):
+        """Rows [start, stop) of the string key column and of every value column (None: a column no aggregate reads)
+        as map partition map_id."""
+        if any(c is not None and c.loc != keys.loc for c in cols):
+            raise ValueError("keys and values must live in the same memory space")
+        if keys.loc == L.VB_DEVICE_BORROWED:
+            self._keepalive.append((keys.owner,) + tuple(c.owner for c in cols if c is not None))
+        offs = ctypes.c_void_p(keys.offs_ptr + 8 * start)
+        data = ctypes.c_void_p(keys.data_ptr) if keys.n_bytes else None
+        ptrs = (ctypes.c_void_p * len(cols))(*[c.at(start) if c is not None else None for c in cols])
+        L.check(self._lib.vb_shuffle_map_str_cols(self._h, map_id, offs, data, keys.n_bytes, ptrs, stop - start, keys.loc))
+
+    def reduce_cols(self, r, out_dtypes, dst_loc=L.VB_HOST, out_key_offsets=None, out_key_bytes=None, out_aggs=None):
+        """Partition r: (key offsets, key bytes, [one array per aggregate]) on the host, or into caller-provided torch
+        CUDA tensors with dst_loc=VB_DEVICE (any may be None; sizes from reduce_size)."""
+        if dst_loc == L.VB_DEVICE:
+            _sync_torch(out_key_offsets, out_key_bytes, *(out_aggs or []))
+            p = lambda t: t.data_ptr() if t is not None else None
+            ptrs = (ctypes.c_void_p * len(out_aggs))(*[p(t) for t in out_aggs]) if out_aggs else None
+            L.check(self._lib.vb_shuffle_reduce_str_cols(self._h, r, p(out_key_offsets), p(out_key_bytes), ptrs, L.VB_DEVICE))
+            return out_key_offsets, out_key_bytes, out_aggs
+        nk, nb, _ = self.reduce_size(r)
+        ko, kb = np.empty(nk + 1, dtype=np.uint64), np.empty(nb, dtype=np.uint8)
+        outs = [np.empty(nk, dtype=dt) for dt in out_dtypes]
+        ptrs = (ctypes.c_void_p * len(outs))(*[o.ctypes.data for o in outs])
+        L.check(self._lib.vb_shuffle_reduce_str_cols(self._h, r, ko.ctypes.data_as(ctypes.c_void_p), kb.ctypes.data_as(ctypes.c_void_p),
+                                                     ptrs, L.VB_HOST))
+        return ko, kb, outs
+
+    def export_cols(self):
+        """vb_shuffle_export_str_cols_prepare + buffers (multi, world > 1): ((n_keys, n_key_bytes), (key_lens, key_bytes,
+        accs)).  The counts are lists with one entry per destination rank; the columns are torch views of the library's
+        device buffers (int32 lengths, uint8 bytes, int64 accumulators of shape (n_acc, keys)), destination-major, in the
+        wire format of include/vega_b200.h and valid until seal."""
+        import torch
+        W = self.world
+        nk, nb = (ctypes.c_uint64 * W)(), (ctypes.c_uint64 * W)()
+        L.check(self._lib.vb_shuffle_export_str_cols_prepare(self._h, nk, nb))
+        counts = tuple([int(x) for x in c] for c in (nk, nb))
+        lp, bp, ap, na = ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_uint32()
+        L.check(self._lib.vb_shuffle_export_str_cols_buffers(self._h, ctypes.byref(lp), ctypes.byref(bp), ctypes.byref(ap),
+                                                             ctypes.byref(na)))
+        dev = f"cuda:{self._lib.vb_ctx_device(self.sc._h)}"
+        K, B, A = sum(counts[0]), sum(counts[1]), na.value
+
+        def view(p, n, typestr, dtype):
+            if n == 0 or not p.value:
+                return torch.empty(0, dtype=dtype, device=dev)
+            return torch.as_tensor(_DevView(p.value, n, typestr), device=dev)
+        return counts, (view(lp, K, "<i4", torch.int32), view(bp, B, "|u1", torch.uint8),
+                        view(ap, A * K, "<i8", torch.int64).view(A, K))
+
+    def import_cols(self, key_lens, key_bytes, accs, n_keys, n_key_bytes):
+        """vb_shuffle_import_str_cols: the received columns (torch CUDA tensors, source-rank major; accs of shape
+        (n_acc, keys)) and the key and byte counts every source rank sent.  The tensors are kept alive until seal."""
+        import torch
+        if accs.dim() != 2 or accs.shape[1] != key_lens.numel() or len(n_keys) != self.world or sum(n_keys) != key_lens.numel():
+            raise ValueError(f"import of {key_lens.numel()} keys, accumulators of shape {tuple(accs.shape)} and counts "
+                             f"{list(n_keys)} on a world of {self.world}: (n_acc, keys) accumulators and one count per rank expected")
+        accs = accs.contiguous()
+        for t in (key_lens, key_bytes, accs):
+            if t.is_cuda:
+                torch.cuda.current_stream(t.device).synchronize()   # the library reads on its own stream
+                break
+        self._keepalive.append((key_lens, key_bytes, accs))
+        p = lambda t: ctypes.c_void_p(t.data_ptr()) if t.numel() else None
+        arr = lambda c: (ctypes.c_uint64 * len(c))(*c)
+        L.check(self._lib.vb_shuffle_import_str_cols(self._h, p(key_lens), p(key_bytes), p(accs), accs.shape[0],
+                                                     arr(n_keys), arr(n_key_bytes)))
+
 
 def _no_str(what):
     def f(self, *a, **k):
         raise TypeError(f"{what} is not supported for string keys yet (reduce_by_key, count_by_key, group_by_key, "
-                        "partition_by_key, count_by_value and distinct are)")
+                        "partition_by_key, combine_by_key, count_by_value and distinct are)")
     return f
 
 
@@ -1320,6 +1416,8 @@ class StrShuffledRdd(ShuffledRdd):
     def __init__(self, parent, agg_name, num_splits, hint=0):
         if num_splits < 1:
             raise ValueError("num_splits must be >= 1")
+        if len(getattr(parent, "cols", ())) > 1:
+            raise TypeError("a PairRdd with several value columns supports combine_by_key only")
         self.parent, self.agg_name, self.num_slices, self.hint = parent, agg_name, num_splits, hint
         self.sc = parent.sc
         self._sh = None
@@ -1349,12 +1447,23 @@ class StrShuffledRdd(ShuffledRdd):
 
 
 class StrPairRdd(PairRdd):
-    """PairRdd<String, V>: the shuffle ops string keys support; the others raise TypeError before any device work."""
+    """PairRdd<String, V>: the shuffle ops string keys support; the others raise TypeError before any device work.
+    combine_by_key takes value columns given as a tuple (Context.parallelize(keys, n, values=(c0, ...)), one to four
+    columns); with several columns it is the only shuffle.  A PairRdd of one plain value array has no combine_by_key."""
 
-    def __init__(self, sc, keys, vals, num_slices):
-        if vals is None and keys.n:
+    def __init__(self, sc, keys, vals, num_slices, cols=None):
+        if vals is None and not cols and keys.n:
             raise ValueError("a PairRdd needs values")
-        super().__init__(sc, keys, vals, num_slices)
+        super().__init__(sc, keys, vals, num_slices, cols=cols)
+        self.has_columns = cols is not None
+
+    def combine_by_key(self, aggs, num_splits, hint=0):
+        """PairRdd.combine_by_key over `String` keys: the same {name: (op, column)} mapping, one shuffle that encodes
+        every key once.  Returns a StrCombinedRdd."""
+        if not self.has_columns:
+            raise TypeError("combine_by_key over String keys takes value columns given as a tuple: "
+                            "Context.parallelize(keys, num_slices, values=(c0, ...))")
+        return StrCombinedRdd(self, aggs, num_splits, hint)
 
     def group_by_key(self, num_splits):
         return StrShuffledRdd(self, "group", num_splits)
@@ -1370,13 +1479,56 @@ class StrPairRdd(PairRdd):
     def partition_by_key(self, num_splits):
         return _Repartitioned(StrShuffledRdd(self, "group", num_splits))
 
-    combine_by_key = _no_str("combine_by_key")
     join = _no_str("join")
     left_outer_join = _no_str("left_outer_join")
     right_outer_join = _no_str("right_outer_join")
     full_outer_join = _no_str("full_outer_join")
     cogroup = _no_str("cogroup")
     sort_by_key = _no_str("sort_by_key")
+
+
+class StrCombinedRdd(_Base):
+    """CombinedRdd over `String` keys (vb_shuffle_create_str_multi): several named aggregates per key in one shuffle.
+    compute(r) / collect() give (keys as a numpy object array of str, {name: array}); compute_raw(r) gives (key offsets,
+    key bytes, [one array per aggregate]); compute_device(r, ...) writes into torch CUDA tensors."""
+
+    def __init__(self, parent, aggs, num_splits, hint=0):
+        self.spec, self.names, self.out_dtypes = _combine_spec(aggs, parent.cols, num_splits)
+        self.parent, self.num_slices, self.hint, self.sc = parent, num_splits, hint, parent.sc
+        self._sh = None
+
+    def _run(self):
+        if self._sh is not None:
+            return self._sh
+        p = self.parent
+        starts = slice_starts(p.n, p.num_slices)
+        sh = StrShuffle(self.sc, len(starts) - 1, self.num_slices, L.VB_U64, L.VB_AGG_SUM, hint=self.hint,
+                        multi=([c.code for c in p.cols], self.spec))
+        for m in range(len(starts) - 1):
+            sh.map_cols(m, p.keys, p.cols, int(starts[m]), int(starts[m + 1]))
+        sh.seal()
+        self._sh = sh
+        return sh
+
+    def compute_raw(self, split):
+        return self._run().reduce_cols(split, self.out_dtypes)
+
+    def compute(self, split):
+        ko, kb, outs = self.compute_raw(split)
+        return _decode_keys(ko, kb), dict(zip(self.names, outs))
+
+    def compute_device(self, split, out_key_offsets=None, out_key_bytes=None, out_aggs=None):
+        """compute(split) into caller-provided torch CUDA tensors (any may be None; sizes from the shuffle's
+        reduce_size): key offsets [n_keys + 1], key bytes, and one tensor per aggregate in the order given."""
+        return self._run().reduce_cols(split, self.out_dtypes, L.VB_DEVICE, out_key_offsets, out_key_bytes, out_aggs)
+
+    def collect(self):
+        parts = [self.compute(r) for r in range(self.num_slices)]
+        return (np.concatenate([p[0] for p in parts]),
+                {name: np.concatenate([p[1][name] for p in parts]) for name in self.names})
+
+    def stats(self):
+        return self._run().stats()
 
 
 class StrCoGroupedRdd(_Base):
