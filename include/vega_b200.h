@@ -531,7 +531,10 @@ VB_API int32_t vb_join_n_str(vb_shuf *const *sides, uint32_t n_sides, uint32_t r
  * rank r's map ids precede rank r + 1's (vega_b200/dist.py map_block).  Partitions a rank does not own are empty on it;
  * a sealed GROUP shuffle is a side of vb_cogroup_n_str / vb_join_n_str for the partitions the calling rank owns.
  * vb_shuffle_exchange(s, VB_XCHG_AUTO or VB_XCHG_NCCL) does all of it on the library's stream: export, one all-gather of
- * 3 x world counts per rank, one grouped send/recv of the four columns; VB_XCHG_P2P is VB_ERR_UNSUPPORTED.
+ * counts per rank, one grouped send/recv of the columns; VB_XCHG_P2P is VB_ERR_UNSUPPORTED.  GROUP gathers 3 x world
+ * counts (keys, key bytes, values).  Reduce ops gather 2 x world counts (keys, key bytes) and a fingerprint of the op
+ * and its order transform, as vb_shuffle_create_str_multi_dist does: ranks whose op or transform differ all return
+ * VB_ERR_INVALID before any send.
  * Errors: the export / import calls on a string shuffle of world 1: VB_ERR_STATE (VB_ERR_INVALID on a non-string
  * shuffle); import before export, twice, or after seal: VB_ERR_STATE; map after export: VB_ERR_STATE; a NULL column
  * whose count is non-zero, or reduce-op counts with n_vals != n_keys: VB_ERR_INVALID; an import of 2^32 - 2 rows or

@@ -2,8 +2,8 @@
 child processes on ONE GPU (each with its own NCCL_HOSTID, talking over NCCL's loopback socket transport, as
 tests/test_gpu_exchange_one_gpu.py does), and on two GPUs when the machine has them.  The owners' partitions must equal
 the one-process shuffle over the same map tasks, the exchange stats must count the keys that crossed, and ranks whose
-specs differ must both return VB_ERR_INVALID.  If NCCL refuses to initialise two ranks on one GPU, that case skips with
-NCCL's message."""
+specs differ must both return VB_ERR_INVALID, as must ranks whose single-column String reduce ops differ (they share
+the combine's exchange).  If NCCL refuses to initialise two ranks on one GPU, that case skips with NCCL's message."""
 import os
 import pickle
 import subprocess
@@ -82,8 +82,19 @@ def _child(rank, outdir, device):
         mismatch = None
     except vb.VegaB200Error as e:
         mismatch = e.code
+    from vega_b200 import _lib as L
+    from vega_b200 import dist as vdist
+    strs, vals, _ = _data()
+    starts = vb.slice_starts(N, M)
+    lo, hi = vdist.map_block(rank, 2, M)
+    maps = [(m, strs[starts[m]:starts[m + 1]], vals[starts[m]:starts[m + 1]]) for m in range(lo, hi)]
+    try:                                               # a single-column reduce_by_key, SUM on rank 0 and MAX on rank 1
+        vdist.run_str_shuffle(vdist.StrCudaEngine(sc), maps, M, R, L.VB_U64, (L.VB_AGG_SUM, L.VB_AGG_MAX)[rank], rank, 2).free()
+        op_mismatch = None
+    except vb.VegaB200Error as e:
+        op_mismatch = e.code
     with open(os.path.join(outdir, f"r{rank}.pkl"), "wb") as f:
-        pickle.dump((res, stats, mismatch), f)
+        pickle.dump((res, stats, mismatch, op_mismatch), f)
     sc.close()
 
 
@@ -130,6 +141,7 @@ def _check(ranks):
     # the keys that crossed: rank q's exported keys owned by the other rank
     assert all(s["exchanges"] == 1 and s["exchange_kind"] == "nccl" for s in st)
     assert [ranks[q][2] for q in range(2)] == [L.VB_ERR_INVALID, L.VB_ERR_INVALID]
+    assert [ranks[q][3] for q in range(2)] == [L.VB_ERR_INVALID, L.VB_ERR_INVALID]     # reduce ops that differ
 
 
 def test_two_ranks_on_one_gpu(tmp_path):

@@ -309,8 +309,9 @@ struct vb_shuf {
     u64 id = 0;
     u32 n_map = 0, n_reduce = 0;
     int kdt = 0, vdt = 0, agg = 0, part = 0;
-    // multi-aggregate shuffle (vb_shuffle_create_multi): agg is VB_AGG_SUM for the reduce-op plumbing, the
-    // accumulators are described by the specs below and the results live in res_cols
+    // multi-aggregate shuffle (vb_shuffle_create_multi, _str_multi): agg is VB_AGG_SUM for the reduce-op plumbing, the
+    // accumulators are described by the specs below and the results live in res_cols.  A string-key reduce op has
+    // the specs and res_cols too (one value column, one aggregate), with multi false: multi selects the _multi calls.
     bool multi = false;
     u32 n_cols = 0;
     AccSpec acc_map{}, acc_merge{};   // map-side combine / table merge (COUNT merges as ADD, no order transform)
@@ -388,7 +389,7 @@ static int seal_str_import(vb_shuf *s);
 static int export_str_locked(vb_shuf *s, u64 *n_keys, u64 *n_key_bytes, u64 *n_vals);
 static int str_import_limits(const vb_shuf *s, u64 nk, u64 nv);
 static int exchange_str_locked(vb_shuf *s);
-static int exchange_str_multi_locked(vb_shuf *s);
+static int exchange_str_accs_locked(vb_shuf *s);
 static void free_str(vb_shuf *s);
 
 static bool is_reduce_op(int agg) { return agg == VB_AGG_SUM || agg == VB_AGG_MIN || agg == VB_AGG_MAX || agg == VB_AGG_COUNT; }
@@ -1338,9 +1339,9 @@ static int multi_spec(uint32_t n_val_cols, const int32_t *val_dtypes, uint32_t n
     return VB_OK;
 }
 
-static void set_multi(vb_shuf *s, const MultiSpec &ms)
+// The accumulator spec only: s->multi (the _multi ABI) is set by the callers that create such a shuffle.
+static void set_spec(vb_shuf *s, const MultiSpec &ms)
 {
-    s->multi = true;
     s->n_cols = ms.n_cols;
     s->acc_map = ms.map;
     s->acc_merge = ms.merge;
@@ -1358,7 +1359,8 @@ extern "C" int32_t vb_shuffle_create_multi(vb_ctx *c, uint64_t shuffle_id, uint3
     MultiSpec ms;
     TRY(multi_spec(n_val_cols, val_dtypes, n_aggs, aggs, &ms));
     TRY(vb_shuffle_create(c, shuffle_id, n_map, n_reduce, kdt, VB_U64, VB_AGG_SUM, VB_PART_HASH_METRO64, out));
-    set_multi(*out, ms);
+    set_spec(*out, ms);
+    (*out)->multi = true;
     return VB_OK;
 }
 
@@ -2905,7 +2907,7 @@ extern "C" int32_t vb_shuffle_exchange(vb_shuf *s, int32_t mode)
     if (s->str || s->multi) {
         std::lock_guard<std::mutex> lk(c->mu);
         CU(cudaSetDevice(c->device));
-        return s->str ? (s->multi ? exchange_str_multi_locked(s) : exchange_str_locked(s)) : exchange_multi_locked(s);
+        return s->str ? (is_reduce_op(s->agg) ? exchange_str_accs_locked(s) : exchange_str_locked(s)) : exchange_multi_locked(s);
     }
     if (mode == VB_XCHG_AUTO) mode = is_group_op(s->agg) ? VB_XCHG_P2P : VB_XCHG_NCCL;
     if (mode == VB_XCHG_P2P && !is_group_op(s->agg)) return set_err(VB_ERR_UNSUPPORTED, "the fused P2P exchange is for GROUP/COGROUP shuffles");
@@ -4289,9 +4291,9 @@ struct StrState {
     u64 n_a = 0;                          // arena bytes in use
     StrCtl *ctl = nullptr;
     std::vector<u32 *> ids;               // per map id: the rows' entry ids (owned)
-    std::vector<const u64 *> vals;        // per map id: the rows' values
+    std::vector<const u64 *> vals;        // GROUP, per map id: the rows' values
     struct Cols { const u64 *c[MA_MAX_COLS]; };
-    std::vector<Cols> cols;               // combine_by_key (vb_shuffle_create_str_multi), per map id: the value columns
+    std::vector<Cols> cols;               // reduce ops and combine_by_key, per map id: the value columns of the spec
     std::vector<char> vals_owned;         // per map id: vals / cols are copies (else borrowed, VB_DEVICE_BORROWED)
     u64 *key_off = nullptr;               // [n_keys + 1] byte offset of every result key (partition-major, from 0)
     unsigned char *key_bytes = nullptr;   // the result keys' bytes
@@ -4306,7 +4308,7 @@ struct StrState {
     unsigned char *x_bytes = nullptr;
     u64 *x_vals = nullptr;
     // ... and the imported ones, source-rank major: borrowed until seal, or received by vb_shuffle_exchange (i_own).
-    // combine_by_key: x_vals / i_vals are the accumulators [n_acc][keys], in plain value form
+    // Reduce ops and combine_by_key: x_vals / i_vals are the accumulators [n_acc][keys], in plain value form
     const u32 *i_lens = nullptr, *i_cnts = nullptr;
     const unsigned char *i_bytes = nullptr;
     const u64 *i_vals = nullptr;
@@ -4390,6 +4392,13 @@ extern "C" int32_t vb_shuffle_create_str(vb_ctx *c, uint64_t shuffle_id, uint32_
     if (agg != VB_AGG_SUM && agg != VB_AGG_MIN && agg != VB_AGG_MAX && agg != VB_AGG_COUNT && agg != VB_AGG_GROUP)
         return set_err(VB_ERR_UNSUPPORTED, "string keys: agg %d is not supported (SUM, MIN, MAX, COUNT and GROUP are)", agg);
     TRY(vb_shuffle_create(c, shuffle_id, n_map, n_reduce, VB_U64, vdt, agg, VB_PART_HASH_METRO64, out));
+    if (is_reduce_op(agg)) {       // a reduce op is the combine of one value column with one aggregate
+        const vb_agg_col one{agg, 0};
+        MultiSpec ms;
+        const int rc = multi_spec(1, &vdt, 1, &one, &ms);
+        if (rc != VB_OK) { vb_shuffle_free(*out); *out = nullptr; return rc; }
+        set_spec(*out, ms);
+    }
     StrState *t = new StrState();
     t->ids.assign(n_map, nullptr);
     t->vals.assign(n_map, nullptr);
@@ -4549,7 +4558,8 @@ static int str_encode(vb_shuf *s, const u64 *offs, const unsigned char *bytes, u
 
 // One map call of a string shuffle after the argument checks: the keys' entry ids, and the value columns in[0 .. n_in)
 // (a NULL column is neither read nor copied), copied, or borrowed for VB_DEVICE_BORROWED.  A single-column shuffle
-// passes its one column (none for COUNT), a combine_by_key shuffle every column an aggregate reads.
+// passes its one column (none for COUNT), a combine_by_key shuffle every column an aggregate reads.  Reduce ops keep
+// them as the spec's value columns (cols), GROUP as its values (vals).
 static int str_map(vb_shuf *s, u32 map_id, const uint64_t *key_offsets, const void *key_bytes, u64 n_bytes, const u64 *const *in, u32 n_in,
                    u64 n, int loc)
 {
@@ -4606,7 +4616,7 @@ static int str_map(vb_shuf *s, u32 map_id, const uint64_t *key_offsets, const vo
         t->vals_owned[map_id] = loc != VB_DEVICE_BORROWED;
         for (u32 j = 0; j < n_in; ++j) {
             const u64 *p = loc == VB_DEVICE_BORROWED ? in[j] : (const u64 *)d_vals[j].release();
-            if (s->multi) t->cols[map_id].c[j] = p;
+            if (is_reduce_op(s->agg)) t->cols[map_id].c[j] = p;
             else t->vals[map_id] = p;
         }
     }
@@ -4684,8 +4694,8 @@ static int str_reduce_rows(vb_shuf *s, int opk, int tx, const u32 *ids, const u6
     return set_err(VB_ERR_UNSUPPORTED, "string keys: op %d", s->agg);
 }
 
-// Rows as dictionary entry ids and their values: one map task's, or the rows a rank imported.  combine_by_key: a map
-// task's value columns in cols, or the imported accumulators [n_acc][n] in vals.
+// Rows as dictionary entry ids and their values: one map task's, or the rows a rank imported.  Reduce ops and
+// combine_by_key: a map task's value columns in cols, or the imported accumulators [n_acc][n] in vals.
 struct StrRun {
     const u32 *ids;
     const u64 *vals;
@@ -4791,27 +4801,11 @@ static int str_dense_keys(vb_shuf *s, const std::vector<StrRun> &runs, const std
     return VB_OK;
 }
 
-// Reduce ops: acc [D] = op `opk` (values entering in order `tx`) folded over every row of `runs`, by dense id.
-static int str_fold_values(vb_shuf *s, const std::vector<StrRun> &runs, int opk, int tx, const u32 *dense, u64 D, DevBuf &acc)
-{
-    vb_ctx *c = s->ctx;
-    TRY(acc.alloc(D * 8));
-    {
-        KLaunch kl(s, K_MISC);
-        str_fill_kernel<<<str_grid(c, D), 256, 0, c->stream>>>(acc.as<u64>(), D, op_identity(opk));
-        TRY(kl.done("str_fill_kernel"));
-    }
-    for (const StrRun &r : runs) TRY(str_reduce_rows(s, opk, tx, r.ids, r.vals, r.n, dense, acc.as<u64>()));
-    if (tx != TX_NONE) {
-        KLaunch kl(s, K_MISC);
-        tx_inv_kernel<<<(unsigned)((D + 255) / 256), 256, 0, c->stream>>>(acc.as<u64>(), D, tx);
-        TRY(kl.done("tx_inv_kernel"));
-    }
-    return VB_OK;
-}
-
-// combine_by_key: acc [n_acc][D] = every accumulator of the spec folded over the rows of `runs`, by dense id, in the
-// spec's order transform (IN_SOA: the map rows and the map spec; IN_ACCS: imported partials and the merge spec).
+// Reduce ops and combine_by_key: acc [n_acc][D] = every accumulator of the spec folded over the rows of `runs`, by
+// dense id, in the spec's order transform (IN_SOA: the map rows and the map spec; IN_ACCS: imported partials and the
+// merge spec).  A spec of one accumulator (every reduce op, and a combine of one aggregate) folds with
+// str_reduce_kernel, whose 26-28 registers keep about twice the warps of str_reduce_multi_kernel resident (DESIGN
+// §3.5, §5.2).
 __global__ void range_kernel(u64 *__restrict__ out, u64 start, u64 step, u64 n);
 
 static int str_fold_multi(vb_shuf *s, const std::vector<StrRun> &runs, int in, const u32 *dense, u64 D, DevBuf &acc)
@@ -4825,6 +4819,11 @@ static int str_fold_multi(vb_shuf *s, const std::vector<StrRun> &runs, int in, c
         TRY(kl.done("str_fill_kernel"));
     }
     for (const StrRun &r : runs) {
+        if (sp.n == 1) {               // a COUNT reads no column (its c[0] may be NULL)
+            const u64 *vals = in == IN_ACCS ? r.vals : r.cols.c[spec_at(sp.src, 0)];
+            TRY(str_reduce_rows(s, spec_at(sp.op, 0), spec_at(sp.tx, 0), r.ids, vals, r.n, dense, acc.as<u64>()));
+            continue;
+        }
         MaCols mc{};
         if (in == IN_ACCS) {
             mc.c[0] = r.vals;
@@ -4895,15 +4894,15 @@ static int str_group_values(vb_shuf *s, const std::vector<StrRun> &runs, u64 n, 
     return VB_OK;
 }
 
-// The reduce side of a string-key shuffle over `runs` (reduce ops fold with `opk`: the map op, or the merge op over
-// imported accumulators):
+// The reduce side of a string-key shuffle over `runs`:
 //   1. mark the entries the rows reference;
 //   2. split the live entries by h % n_reduce into partition-major dense ids, and lay their bytes out in that order;
-//   3. reduce ops: one RED per (warp, distinct id) into acc[dense id];  combine_by_key: the same for every accumulator
-//      of the spec (`in`: map rows or imported partials), then the output columns;  GROUP: the rows in run order
-//      (map-id order, or source-rank major), stably sorted by dense id, then the CSR (seal_group's steps 4-7).
+//   3. reduce ops and combine_by_key: one RED per (warp, distinct id) into acc[accumulator][dense id] for every
+//      accumulator of the spec (`in`: map rows or imported partials), then the output columns;  GROUP: the rows in
+//      run order (map-id order, or source-rank major), stably sorted by dense id, then the CSR (seal_group's steps
+//      4-7).
 // The per-map ids and the dictionary are freed at the end.
-static int seal_str_runs(vb_shuf *s, const std::vector<StrRun> &runs, int opk, int in = IN_SOA)
+static int seal_str_runs(vb_shuf *s, const std::vector<StrRun> &runs, int in = IN_SOA)
 {
     vb_ctx *c = s->ctx;
     StrState *t = s->str;
@@ -4921,16 +4920,11 @@ static int seal_str_runs(vb_shuf *s, const std::vector<StrRun> &runs, int opk, i
         TRY(str_dense_keys(s, runs, order, cnt, s->bucket_off, dense, koff, kbytes));
         const u64 D = s->bucket_off[R];
         TRY(str_read_at(s, koff.as<u64>(), s->bucket_off, t->kb_off));
-        if (s->multi) {                // combine_by_key: fold every accumulator, then the output columns
+        if (is_reduce_op(s->agg)) {    // fold every accumulator, then the output columns
             DevBuf acc(c), out(c);
             TRY(str_fold_multi(s, runs, in, dense.as<u32>(), D, acc));
             TRY(str_finalize_multi(s, acc.as<u64>(), D, out));
             s->res_cols = (u64 *)out.release();
-            s->st.rows_out = D;
-        } else if (is_reduce_op(s->agg)) {
-            DevBuf acc(c);
-            TRY(str_fold_values(s, runs, opk, val_tx(s), dense.as<u32>(), D, acc));
-            s->res_comb = (u64 *)acc.release();
             s->st.rows_out = D;
         } else {
             DevBuf offs(c), vals(c);
@@ -4952,16 +4946,16 @@ static int seal_str_runs(vb_shuf *s, const std::vector<StrRun> &runs, int opk, i
 }
 
 // Seal of a string-key shuffle (world == 1, every map present)
-static int seal_str(vb_shuf *s) { return seal_str_runs(s, str_map_runs(s), map_opk(s)); }
+static int seal_str(vb_shuf *s) { return seal_str_runs(s, str_map_runs(s)); }
 
 // ---------------------------------------------------------------------------------------------
 // string keys across ranks (vb_shuffle_create_str_dist): the map side of each rank is exported as key columns, packed
 // by destination rank; the owner imports every rank's columns into a fresh dictionary and seals them as one run.
 // ---------------------------------------------------------------------------------------------
 // Export: steps 1-2 of the seal with the partitions laid out destination-major (rank 0's partitions, then rank 1's,
-// ...), so the dense ids come out grouped by destination; then the values of step 3, as one accumulator per key
-// (reduce ops) or each key's values in map order (GROUP).  The per-map ids and the dictionary are freed.  The caller
-// holds c->mu.
+// ...), so the dense ids come out grouped by destination; then the values of step 3, as every accumulator of the
+// spec per key in plain value form (reduce ops and combine_by_key) or each key's values in map order (GROUP).  The
+// per-map ids and the dictionary are freed.  The caller holds c->mu.
 static int export_str_locked(vb_shuf *s, u64 *n_keys, u64 *n_key_bytes, u64 *n_vals)
 {
     vb_ctx *c = s->ctx;
@@ -4998,7 +4992,7 @@ static int export_str_locked(vb_shuf *s, u64 *n_keys, u64 *n_key_bytes, u64 *n_v
             str_diff_u32_kernel<<<str_grid(c, D), 256, 0, c->stream>>>(koff.as<u64>(), D, lens.as<u32>());
             TRY(kl.done("str_diff_u32_kernel"));
         }
-        if (s->multi) {                // combine_by_key: every accumulator of the map spec, in plain value form
+        if (is_reduce_op(s->agg)) {
             DevBuf acc(c);
             TRY(str_fold_multi(s, runs, IN_SOA, dense.as<u32>(), D, acc));
             for (u32 a = 0; a < s->acc_map.n; ++a) {
@@ -5008,11 +5002,6 @@ static int export_str_locked(vb_shuf *s, u64 *n_keys, u64 *n_key_bytes, u64 *n_v
                 tx_inv_kernel<<<(unsigned)((D + 255) / 256), 256, 0, c->stream>>>(acc.as<u64>() + (u64)a * D, D, tx);
                 TRY(kl.done("tx_inv_kernel"));
             }
-            for (u32 d = 0; d < W; ++d) n_vals[d] = n_keys[d];
-            t->x_vals = (u64 *)acc.release();
-        } else if (is_reduce_op(s->agg)) {
-            DevBuf acc(c);
-            TRY(str_fold_values(s, runs, map_opk(s), val_tx(s), dense.as<u32>(), D, acc));
             for (u32 d = 0; d < W; ++d) n_vals[d] = n_keys[d];
             t->x_vals = (u64 *)acc.release();
         } else {
@@ -5052,7 +5041,7 @@ static int str_import_limits(const vb_shuf *s, u64 nk, u64 nv)
 // Seal of an imported string shuffle: the received keys' byte offsets (widened lengths, one scan), a fresh dictionary
 // of them (str_encode_kernel; the received key count bounds the distinct keys), for GROUP each key's entry id over its
 // run of values, then seal_str_runs over the rows as one source-rank-major run: reduce ops merge the accumulators with
-// the merge op (COUNT: ADD_U64), GROUP keeps source-rank order, which is map-id order.
+// the import spec (COUNT as ADD), GROUP keeps source-rank order, which is map-id order.
 static int seal_str_import(vb_shuf *s)
 {
     vb_ctx *c = s->ctx;
@@ -5103,7 +5092,7 @@ static int seal_str_import(vb_shuf *s)
             runs.push_back(StrRun{ids.as<u32>(), t->i_vals, nk});
         }
     }
-    TRY(seal_str_runs(s, runs, merge_opk(s), IN_ACCS));
+    TRY(seal_str_runs(s, runs, IN_ACCS));
     free_str_xchg(s);
     return VB_OK;
 }
@@ -5156,42 +5145,55 @@ extern "C" int32_t vb_shuffle_export_str_buffers(vb_shuf *s, uint32_t **key_lens
     return VB_OK;
 }
 
-extern "C" int32_t vb_shuffle_import_str(vb_shuf *s, const uint32_t *key_lens, const void *key_bytes, const uint32_t *val_counts,
-                                         const uint64_t *vals, const uint64_t *n_keys, const uint64_t *n_key_bytes, const uint64_t *n_vals)
+// The columns a rank received, source-rank major, kept until seal (cnts: GROUP only); the shuffle is then imported.
+static void str_take_import(vb_shuf *s, const u32 *lens, const void *bytes, const u32 *cnts, const u64 *vals, u64 nk, u64 nkb, u64 nv)
 {
-    if (!s || !n_keys || !n_key_bytes || !n_vals) return set_err(VB_ERR_INVALID, "NULL argument");
-    TRY(str_dist_check(s, "vb_shuffle_import_str"));
+    StrState *t = s->str;
+    t->i_lens = lens; t->i_bytes = (const unsigned char *)bytes; t->i_cnts = cnts; t->i_vals = vals;
+    t->i_nk = nk; t->i_nkb = nkb; t->i_nv = nv;
+    std::lock_guard<std::mutex> g(s->mu);
+    s->imported = true;
+}
+
+// vb_shuffle_import_str and vb_shuffle_import_str_cols after their argument checks: the totals nk, nkb and nv (reduce
+// ops: one accumulator row per key) are checked, and the caller's columns are borrowed until seal.
+static int str_import(vb_shuf *s, const char *what, const char *prepare, const uint32_t *key_lens, const void *key_bytes,
+                      const uint32_t *val_counts, const uint64_t *vals, u64 nk, u64 nkb, u64 nv)
+{
     {
         std::lock_guard<std::mutex> g(s->mu);
         if (!s->exported || s->imported || s->sealed || s->sealing || s->freed)
-            return set_err(VB_ERR_STATE, "vb_shuffle_import_str needs vb_shuffle_export_str_prepare first, once, and no seal yet");
+            return set_err(VB_ERR_STATE, "%s needs %s first, once, and no seal yet", what, prepare);
     }
-    u64 nk = 0, nkb = 0, nv = 0;
-    for (u32 r = 0; r < s->world; ++r) { nk += n_keys[r]; nkb += n_key_bytes[r]; nv += n_vals[r]; }
     const bool group = !is_reduce_op(s->agg);
     if ((nk && !key_lens) || (nkb && !key_bytes) || (group && nk && !val_counts) || (nv && !vals))
         return set_err(VB_ERR_INVALID, "NULL column with a non-zero count");
     if (!group && nv != nk) return set_err(VB_ERR_INVALID, "reduce ops import one accumulator per key (%llu keys, %llu values)", (unsigned long long)nk, (unsigned long long)nv);
     TRY(str_import_limits(s, nk, nv));
-    StrState *t = s->str;
-    t->i_lens = key_lens; t->i_bytes = (const unsigned char *)key_bytes; t->i_cnts = group ? val_counts : nullptr; t->i_vals = vals;
-    t->i_nk = nk; t->i_nkb = nkb; t->i_nv = nv;
-    std::lock_guard<std::mutex> g(s->mu);
-    s->imported = true;
+    str_take_import(s, key_lens, key_bytes, group ? val_counts : nullptr, vals, nk, nkb, nv);
     return VB_OK;
 }
 
-// vb_shuffle_exchange of a string shuffle: export, then the exchange of four columns: u32 key lengths and (GROUP)
-// u32 value counts split by the key counts, key bytes by the byte counts, u64 values by the value counts.  The
-// gathered row is the three count vectors (keys, key bytes, values to every destination).  The received columns
-// are owned by the shuffle until seal.
+extern "C" int32_t vb_shuffle_import_str(vb_shuf *s, const uint32_t *key_lens, const void *key_bytes, const uint32_t *val_counts,
+                                         const uint64_t *vals, const uint64_t *n_keys, const uint64_t *n_key_bytes, const uint64_t *n_vals)
+{
+    if (!s || !n_keys || !n_key_bytes || !n_vals) return set_err(VB_ERR_INVALID, "NULL argument");
+    TRY(str_dist_check(s, "vb_shuffle_import_str"));
+    u64 nk = 0, nkb = 0, nv = 0;
+    for (u32 r = 0; r < s->world; ++r) { nk += n_keys[r]; nkb += n_key_bytes[r]; nv += n_vals[r]; }
+    return str_import(s, "vb_shuffle_import_str", "vb_shuffle_export_str_prepare", key_lens, key_bytes, val_counts, vals, nk, nkb, nv);
+}
+
+// vb_shuffle_exchange of a GROUP string shuffle: export, then the exchange of four columns: u32 key lengths and u32
+// value counts split by the key counts, key bytes by the byte counts, u64 values by the value counts.  The gathered
+// row is the three count vectors (keys, key bytes, values to every destination).  The received columns are owned by
+// the shuffle until seal.
 static int exchange_str_locked(vb_shuf *s)
 {
     vb_ctx *c = s->ctx;
     Comm *m = c->comm;
     StrState *t = s->str;
     const u32 W = m->world, me = m->rank;
-    const bool group = !is_reduce_op(s->agg);
     const size_t len = 3 * (size_t)W;            // n_keys[W], n_key_bytes[W], n_vals[W]
     std::vector<u64> row(len, 0);
     auto clk = std::chrono::steady_clock::now();
@@ -5206,18 +5208,16 @@ static int exchange_str_locked(vb_shuf *s)
     DevBuf lens(c), bytes(c), cnts(c), vals(c);
     TRY(lens.alloc(nk * 4));
     TRY(bytes.alloc(nkb));
-    if (group) TRY(cnts.alloc(nk * 4));
+    TRY(cnts.alloc(nk * 4));
     TRY(vals.alloc(nv * 8));
-    std::vector<XCol> cols{{ncclUint32, t->x_lens, lens.p, 0}, {ncclUint8, t->x_bytes, bytes.p, 1}, {ncclUint64, t->x_vals, vals.p, 2}};
-    if (group) cols.push_back({ncclUint32, t->x_cnts, cnts.p, 0});
+    const std::vector<XCol> cols{{ncclUint32, t->x_lens, lens.p, 0}, {ncclUint8, t->x_bytes, bytes.p, 1}, {ncclUint64, t->x_vals, vals.p, 2},
+                                 {ncclUint32, t->x_cnts, cnts.p, 0}};
     TRY(post_group(s, xfers(sp, cols, W)));
     s->xst.post_wall_ms += lap(clk);
     xchg_done(s, VB_XCHG_NCCL, sp[2].soff[W] - sp[2].send[me], nv - sp[2].recv[me]);
-    t->i_lens = lens.as<u32>(); t->i_bytes = bytes.as<unsigned char>(); t->i_cnts = group ? cnts.as<u32>() : nullptr; t->i_vals = vals.as<u64>();
-    t->i_nk = nk; t->i_nkb = nkb; t->i_nv = nv;
-    t->i_own[0] = lens.release(); t->i_own[1] = bytes.release(); t->i_own[2] = cnts.release(); t->i_own[3] = vals.release();
-    std::lock_guard<std::mutex> g(s->mu);
-    s->imported = true;
+    void **own = t->i_own;
+    own[0] = lens.release(); own[1] = bytes.release(); own[2] = cnts.release(); own[3] = vals.release();
+    str_take_import(s, (const u32 *)own[0], own[1], (const u32 *)own[2], (const u64 *)own[3], nk, nkb, nv);
     return VB_OK;
 }
 
@@ -5251,15 +5251,11 @@ static int copy_out_rebased(vb_shuf *s, u64 *dst, const u64 *src, u64 nk, u64 ba
     return copy_out(s, dst, tmp.p, (nk + 1) * 8, dst_loc);
 }
 
-extern "C" int32_t vb_shuffle_reduce_str(vb_shuf *s, uint32_t r, uint64_t *out_key_offsets, void *out_key_bytes, void *out_combined,
-                                         uint64_t *out_offsets, void *out_vals, int32_t dst_loc)
+// vb_shuffle_reduce_str and vb_shuffle_reduce_str_cols after their argument checks: partition r's keys, then its GROUP
+// value lists (out_offsets, out_vals) or its first n_cols result columns (out_cols[o]; a NULL entry is skipped).
+static int str_reduce_out(vb_shuf *s, uint32_t r, uint64_t *out_key_offsets, void *out_key_bytes, void *const *out_cols, u32 n_cols,
+                          uint64_t *out_offsets, void *out_vals, int32_t dst_loc)
 {
-    if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
-    if (!s->str) return set_err(VB_ERR_INVALID, "vb_shuffle_reduce_str needs a shuffle from vb_shuffle_create_str");
-    if (r >= s->n_reduce) return set_err(VB_ERR_INVALID, "reduce_id %u >= n_reduce %u", r, s->n_reduce);
-    if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
-    if (s->multi && (out_combined || out_offsets || out_vals))
-        return set_err(VB_ERR_INVALID, "shuffle %llu has several aggregates per key: read them with vb_shuffle_reduce_str_cols", (unsigned long long)s->id);
     TRY(wait_sealed(s));
     vb_ctx *c = s->ctx;
     std::lock_guard<std::mutex> lk(c->mu);
@@ -5274,10 +5270,24 @@ extern "C" int32_t vb_shuffle_reduce_str(vb_shuf *s, uint32_t r, uint64_t *out_k
         TRY(copy_out_rebased(s, out_offsets, s->res_offs ? s->res_offs + b0 : nullptr, nk, v0, dst_loc));
         TRY(copy_out(s, out_vals, s->res_vals ? s->res_vals + v0 : nullptr, nv * 8, dst_loc));
     } else {
-        TRY(copy_out(s, out_combined, s->res_comb ? s->res_comb + b0 : nullptr, nk * 8, dst_loc));
+        for (u32 o = 0; out_cols && o < n_cols; ++o)
+            TRY(copy_out(s, out_cols[o], s->res_cols ? s->res_cols + (u64)o * s->n_keys + b0 : nullptr, nk * 8, dst_loc));
     }
     CU(cudaStreamSynchronize(c->stream));
     return VB_OK;
+}
+
+extern "C" int32_t vb_shuffle_reduce_str(vb_shuf *s, uint32_t r, uint64_t *out_key_offsets, void *out_key_bytes, void *out_combined,
+                                         uint64_t *out_offsets, void *out_vals, int32_t dst_loc)
+{
+    if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
+    if (!s->str) return set_err(VB_ERR_INVALID, "vb_shuffle_reduce_str needs a shuffle from vb_shuffle_create_str");
+    if (r >= s->n_reduce) return set_err(VB_ERR_INVALID, "reduce_id %u >= n_reduce %u", r, s->n_reduce);
+    if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
+    if (s->multi && (out_combined || out_offsets || out_vals))
+        return set_err(VB_ERR_INVALID, "shuffle %llu has several aggregates per key: read them with vb_shuffle_reduce_str_cols", (unsigned long long)s->id);
+    void *const combined[1] = {out_combined};
+    return str_reduce_out(s, r, out_key_offsets, out_key_bytes, combined, 1, out_offsets, out_vals, dst_loc);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -5294,7 +5304,8 @@ extern "C" int32_t vb_shuffle_create_str_multi(vb_ctx *c, uint64_t shuffle_id, u
     MultiSpec ms;
     TRY(multi_spec(n_val_cols, val_dtypes, n_aggs, aggs, &ms));
     TRY(vb_shuffle_create_str(c, shuffle_id, n_map, n_reduce, VB_U64, VB_AGG_SUM, out));
-    set_multi(*out, ms);
+    set_spec(*out, ms);
+    (*out)->multi = true;
     return VB_OK;
 }
 
@@ -5318,19 +5329,7 @@ extern "C" int32_t vb_shuffle_reduce_str_cols(vb_shuf *s, uint32_t r, uint64_t *
     if (!s->str || !s->multi) return set_err(VB_ERR_INVALID, "vb_shuffle_reduce_str_cols needs a shuffle from vb_shuffle_create_str_multi");
     if (r >= s->n_reduce) return set_err(VB_ERR_INVALID, "reduce_id %u >= n_reduce %u", r, s->n_reduce);
     if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
-    TRY(wait_sealed(s));
-    vb_ctx *c = s->ctx;
-    std::lock_guard<std::mutex> lk(c->mu);
-    CU(cudaSetDevice(c->device));
-    StrState *t = s->str;
-    const u64 b0 = s->bucket_off[r], nk = s->bucket_off[r + 1] - b0;
-    const u64 kb0 = t->kb_off[r], nkb = t->kb_off[r + 1] - kb0;
-    TRY(copy_out_rebased(s, out_key_offsets, t->key_off ? t->key_off + b0 : nullptr, nk, kb0, dst_loc));
-    TRY(copy_out(s, out_key_bytes, t->key_bytes ? t->key_bytes + kb0 : nullptr, nkb, dst_loc));
-    for (u32 o = 0; out_aggs && o < s->outs.n; ++o)
-        TRY(copy_out(s, out_aggs[o], s->res_cols ? s->res_cols + (u64)o * s->n_keys + b0 : nullptr, nk * 8, dst_loc));
-    CU(cudaStreamSynchronize(c->stream));
-    return VB_OK;
+    return str_reduce_out(s, r, out_key_offsets, out_key_bytes, out_aggs, s->outs.n, nullptr, nullptr, dst_loc);
 }
 
 // the checks every string _cols export / import call makes first
@@ -5377,28 +5376,16 @@ extern "C" int32_t vb_shuffle_import_str_cols(vb_shuf *s, const uint32_t *key_le
     if (!s || !n_keys || !n_key_bytes) return set_err(VB_ERR_INVALID, "NULL argument");
     TRY(str_multi_dist_check(s, "vb_shuffle_import_str_cols"));
     if (n_acc != s->acc_map.n) return set_err(VB_ERR_INVALID, "%u accumulator columns imported, the shuffle has %u", n_acc, s->acc_map.n);
-    {
-        std::lock_guard<std::mutex> g(s->mu);
-        if (!s->exported || s->imported || s->sealed || s->sealing || s->freed)
-            return set_err(VB_ERR_STATE, "vb_shuffle_import_str_cols needs vb_shuffle_export_str_cols_prepare first, once, and no seal yet");
-    }
     u64 nk = 0, nkb = 0;
     for (u32 r = 0; r < s->world; ++r) { nk += n_keys[r]; nkb += n_key_bytes[r]; }
-    if ((nk && (!key_lens || !accs)) || (nkb && !key_bytes)) return set_err(VB_ERR_INVALID, "NULL column with a non-zero count");
-    TRY(str_import_limits(s, nk, nk));
-    StrState *t = s->str;
-    t->i_lens = key_lens; t->i_bytes = (const unsigned char *)key_bytes; t->i_cnts = nullptr; t->i_vals = accs;
-    t->i_nk = nk; t->i_nkb = nkb; t->i_nv = nk;
-    std::lock_guard<std::mutex> g(s->mu);
-    s->imported = true;
-    return VB_OK;
+    return str_import(s, "vb_shuffle_import_str_cols", "vb_shuffle_export_str_cols_prepare", key_lens, key_bytes, nullptr, accs, nk, nkb, nk);
 }
 
-// vb_shuffle_exchange of a string-key combine: export, then the exchange of 2 + n_acc columns: u32 key lengths and the
-// n_acc u64 accumulator columns split by the key counts, key bytes by the byte counts.  The gathered row is the key and
-// byte counts to every destination, then exchange_multi_locked's spec fingerprint (no key width: keys are strings),
-// so a rank whose spec differs is refused on every rank before any send.
-static int exchange_str_multi_locked(vb_shuf *s)
+// vb_shuffle_exchange of a string-key reduce op or combine: export, then the exchange of 2 + n_acc columns: u32 key
+// lengths and the n_acc u64 accumulator columns split by the key counts, key bytes by the byte counts.  The gathered
+// row is the key and byte counts to every destination, then exchange_multi_locked's spec fingerprint (no key width:
+// keys are strings), so a rank whose op or spec differs is refused on every rank before any send.
+static int exchange_str_accs_locked(vb_shuf *s)
 {
     vb_ctx *c = s->ctx;
     Comm *m = c->comm;
@@ -5418,7 +5405,7 @@ static int exchange_str_multi_locked(vb_shuf *s)
     for (u32 p = 1; p < W; ++p)
         for (u32 i = 0; i < 3; ++i)
             if (mat[p * len + 2 * W + i] != mat[2 * W + i])
-                return set_err(VB_ERR_INVALID, "rank %u's combine spec differs from rank 0's (accumulators, ops, transforms or n_reduce)", p);
+                return set_err(VB_ERR_INVALID, "rank %u's reduce op or combine spec differs from rank 0's (accumulators, ops, transforms or n_reduce)", p);
     for (u32 d = 0; d < W; ++d) {
         const u64 nd = xsplit(mat, len, W, d, 0).roff[W];
         TRY(str_import_limits(s, nd, nd));
@@ -5434,11 +5421,9 @@ static int exchange_str_multi_locked(vb_shuf *s)
     TRY(post_group(s, xfers(sp, cols, W)));
     s->xst.post_wall_ms += lap(clk);
     xchg_done(s, VB_XCHG_NCCL, n_sent - sp[0].send[me], nk - sp[0].recv[me]);
-    t->i_lens = lens.as<u32>(); t->i_bytes = bytes.as<unsigned char>(); t->i_cnts = nullptr; t->i_vals = accs.as<u64>();
-    t->i_nk = nk; t->i_nkb = nkb; t->i_nv = nk;
-    t->i_own[0] = lens.release(); t->i_own[1] = bytes.release(); t->i_own[3] = accs.release();
-    std::lock_guard<std::mutex> g(s->mu);
-    s->imported = true;
+    void **own = t->i_own;
+    own[0] = lens.release(); own[1] = bytes.release(); own[3] = accs.release();
+    str_take_import(s, (const u32 *)own[0], own[1], nullptr, (const u64 *)own[3], nk, nkb, nk);
     return VB_OK;
 }
 
