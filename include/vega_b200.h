@@ -613,6 +613,29 @@ VB_API int32_t vb_shuffle_export_str_cols_buffers(vb_shuf *s, uint32_t **key_len
 VB_API int32_t vb_shuffle_import_str_cols(vb_shuf *s, const uint32_t *key_lens, const void *key_bytes, const uint64_t *accs,
                                           uint32_t n_acc, const uint64_t *n_keys /*[world]*/,
                                           const uint64_t *n_key_bytes /*[world]*/);
+/* ---- sort_by_key over string keys (PairRdd::sort_by_key / Rdd::sort over `String` keys, one process) ----------------
+ * vb_shuffle_create_str_sort: a sort shuffle of byte-string keys with one payload column of val_dtype (VB_U64 / VB_I64
+ * / VB_F64), or key-only with val_dtype -1 (VB_ERR_INVALID otherwise).  The semantics of the integer sort_by_key, with
+ * keys in `String` order (`<[u8] as Ord>`: bytes compare unsigned, a proper prefix sorts first; the bytes are not
+ * checked for UTF-8):
+ *   order      rows ascending by key; equal keys stay in input order (map-id order, then row order).
+ *   partitions contiguous ranges: with n rows, cut p (0 < p < n_reduce) is the first row at or after floor(p·n/n_reduce)
+ *              where the key changes, so no key is split; partitions may be empty and n_reduce may exceed n.
+ *   payload    moved bit for bit (NaN payloads survive).
+ * Re-submitting a map_id overwrites it (a key only the replaced rows had is gone).  Limits: those of
+ * vb_shuffle_create_str (fewer than 2^32 - 2 rows, fewer than 2^31 distinct keys, keys shorter than 2^32 bytes:
+ * VB_ERR_TOO_LARGE beyond them); bad key offsets are VB_ERR_INVALID as for vb_shuffle_map_str.
+ *   map     vb_shuffle_map_str; vals must be NULL on a key-only shuffle, and non-NULL with rows otherwise (VB_ERR_INVALID).
+ *   read    vb_shuffle_reduce_str_size: n_keys = the partition's rows, n_key_bytes = the bytes of their keys (each row
+ *           carries its own copy), n_vals = 0.  vb_shuffle_reduce_str: out_key_offsets [n_keys + 1] (from 0) into
+ *           out_key_bytes, and out_combined [n_keys] the payload (NULL outputs are skipped); out_offsets / out_vals must
+ *           be NULL, and so must out_combined on a key-only shuffle (VB_ERR_INVALID).  dst_loc: VB_HOST or VB_DEVICE.
+ * set_hint / seal / stats / kernel_time / free work as for any shuffle; kernel_time class 8 is the ordering of the
+ * distinct keys.  On this kind the integer map / reduce / join calls, vb_cogroup_n_str / vb_join_n_str,
+ * vb_shuffle_create_narrow, vb_shuffle_set_key_width and the _str_cols calls return VB_ERR_INVALID; vb_shuffle_set_dist
+ * with world > 1 and the export / import / exchange / blob calls return VB_ERR_UNSUPPORTED (across ranks: not yet). */
+VB_API int32_t vb_shuffle_create_str_sort(vb_ctx *ctx, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce,
+                                          int32_t val_dtype /*VB_U64 / VB_I64 / VB_F64, or -1: key-only*/, vb_shuf **out);
 /* MetroHash64_1(bytes ‖ 0xFF, seed 0): the reference's hash of a `String` / `&str` key */
 VB_API uint64_t vb_hash_str(const void *bytes, uint64_t len);
 VB_API uint32_t vb_get_partition_str(const void *bytes, uint64_t len, uint32_t n_reduce);
@@ -664,7 +687,8 @@ VB_API int32_t vb_gen_pairs(vb_ctx *ctx, void *rows_dev, void *keys_dev, void *v
                             double zipf_s);
 
 /* Device time and launch count per kernel class (profiling on): 0 hash_agg (map-side combine),
- * 1 dict build, 2 merge, 3 rp_hist, 4 rp_scan, 5 rp_scatter, 6 misc, 7 join.                   */
+ * 1 dict build, 2 merge, 3 rp_hist, 4 rp_scan, 5 rp_scatter, 6 misc, 7 join, 8 str_order (the ordering of a
+ * string sort's distinct keys, its radix passes included).                                     */
 VB_API int32_t vb_shuffle_kernel_time(vb_shuf *s, int32_t klass, double *ms, uint64_t *launches);
 
 /* library build info: "vega_b200 <version> sm_90a" */

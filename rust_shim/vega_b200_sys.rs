@@ -150,6 +150,10 @@ extern "C" {
                                               accs: *mut *mut u64, n_acc: *mut u32) -> i32;
     pub fn vb_shuffle_import_str_cols(s: *mut vb_shuf, key_lens: *const u32, key_bytes: *const c_void, accs: *const u64, n_acc: u32,
                                       n_keys: *const u64, n_key_bytes: *const u64) -> i32;
+    // sort_by_key over String keys (one process): map with vb_shuffle_map_str, read with vb_shuffle_reduce_str (rows in
+    // key order, each with its key; the payload in out_combined); val_dtype -1 is key-only
+    pub fn vb_shuffle_create_str_sort(ctx: *mut vb_ctx, shuffle_id: u64, n_map: u32, n_reduce: u32, val_dtype: i32,
+                                      out: *mut *mut vb_shuf) -> i32;
     pub fn vb_hash_str(bytes: *const c_void, len: u64) -> u64;
     pub fn vb_get_partition_str(bytes: *const c_void, len: u64, n_reduce: u32) -> u32;
     pub fn vb_shuffle_free(s: *mut vb_shuf) -> i32;

@@ -62,7 +62,7 @@ extern "C" const char *vb_version(void) { return "vega_b200 0.1 sm_90a"; }
 // ---------------------------------------------------------------------------------------------
 // context
 // ---------------------------------------------------------------------------------------------
-enum { K_HASH_AGG = 0, K_DICT = 1, K_MERGE = 2, K_RP_HIST = 3, K_RP_SCAN = 4, K_RP_SCATTER = 5, K_MISC = 6, K_JOIN = 7, K_N = 8 };
+enum { K_HASH_AGG = 0, K_DICT = 1, K_MERGE = 2, K_RP_HIST = 3, K_RP_SCAN = 4, K_RP_SCATTER = 5, K_MISC = 6, K_JOIN = 7, K_STR_ORDER = 8, K_N = 9 };
 
 struct vb_ctx {
     int device = 0;
@@ -380,6 +380,7 @@ struct vb_shuf {
     // stats
     vb_stats st{};
     std::vector<Timer> timers;
+    int kclass_as = -1;            // >= 0: every kernel launched meanwhile is counted in this class (a string sort's ordering)
     double kms[K_N] = {0};
     u64 klaunch[K_N] = {0};
 };
@@ -423,7 +424,7 @@ struct KLaunch {
     {
         if (a && !pushed) { cudaEventDestroy(a); cudaEventDestroy(b); }
     }
-    KLaunch(vb_shuf *s_, int klass_, u64 rows_ = 0) : s(s_), klass(klass_), rows(rows_)
+    KLaunch(vb_shuf *s_, int klass_, u64 rows_ = 0) : s(s_), klass(s_ && s_->kclass_as >= 0 && klass_ >= 0 ? s_->kclass_as : klass_), rows(rows_)
     {
         if (s && s->ctx->profile) {
             cudaEventCreate(&a);
@@ -4314,6 +4315,13 @@ struct StrState {
     const u64 *i_vals = nullptr;
     u64 i_nk = 0, i_nkb = 0, i_nv = 0;
     void *i_own[4] = {};
+    // sort_by_key (vb_shuffle_create_str_sort): after seal key_off / key_bytes hold the D distinct keys in rank order,
+    // res_vals the payload in row order, and partition r is rows [bucket_off[r], bucket_off[r + 1]), ranks
+    // [rank_cut[r], rank_cut[r + 1]) and key bytes [kb_off[r], kb_off[r + 1])
+    bool sort = false, sort_vals = false;   // a sort shuffle; with a payload column
+    u64 *row_off = nullptr;                 // [D + 1] first row of each rank (the CSR), row_off[D] = rows
+    u64 *row_boff = nullptr;                // [D + 1] first key byte of each rank's rows (each row carries its key)
+    std::vector<u64> rank_cut;              // [n_reduce + 1]
 };
 
 constexpr u32 STR_MAX_LOG_CAP = 33;       // index slots: < 2^31 distinct keys at load <= 0.6
@@ -4380,8 +4388,23 @@ static void free_str(vb_shuf *s)
     dev_free(s->ctx, t->res_hash);
     dev_free(s->ctx, t->ix_fp);
     dev_free(s->ctx, t->ix_id);
+    dev_free(s->ctx, t->row_off);
+    dev_free(s->ctx, t->row_boff);
     delete t;
     s->str = nullptr;
+}
+
+// A fresh string state (empty dictionary, no map output) for a new shuffle
+static StrState *str_attach(vb_shuf *s)
+{
+    StrState *t = new StrState();
+    t->ids.assign(s->n_map, nullptr);
+    t->vals.assign(s->n_map, nullptr);
+    t->cols.assign(s->n_map, StrState::Cols{});
+    t->vals_owned.assign(s->n_map, 0);
+    t->d.fp_mask = str_fp_mask();
+    s->str = t;
+    return t;
 }
 
 extern "C" int32_t vb_shuffle_create_str(vb_ctx *c, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce, int32_t vdt, int32_t agg,
@@ -4399,13 +4422,22 @@ extern "C" int32_t vb_shuffle_create_str(vb_ctx *c, uint64_t shuffle_id, uint32_
         if (rc != VB_OK) { vb_shuffle_free(*out); *out = nullptr; return rc; }
         set_spec(*out, ms);
     }
-    StrState *t = new StrState();
-    t->ids.assign(n_map, nullptr);
-    t->vals.assign(n_map, nullptr);
-    t->cols.assign(n_map, StrState::Cols{});
-    t->vals_owned.assign(n_map, 0);
-    t->d.fp_mask = str_fp_mask();
-    (*out)->str = t;
+    str_attach(*out);
+    return VB_OK;
+}
+
+// sort_by_key over string keys: a VB_AGG_SORT / VB_PART_RANGE shuffle with a string dictionary (val_dtype -1: key-only)
+extern "C" int32_t vb_shuffle_create_str_sort(vb_ctx *c, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce, int32_t val_dtype,
+                                              vb_shuf **out)
+{
+    if (!c || !out) return set_err(VB_ERR_INVALID, "vb_shuffle_create_str_sort: NULL argument");
+    *out = nullptr;
+    if (val_dtype != -1 && (val_dtype < VB_U64 || val_dtype > VB_F64))
+        return set_err(VB_ERR_INVALID, "vb_shuffle_create_str_sort: val_dtype %d (VB_U64, VB_I64, VB_F64, or -1 for key-only)", val_dtype);
+    TRY(vb_shuffle_create(c, shuffle_id, n_map, n_reduce, VB_U64, val_dtype < 0 ? VB_U64 : val_dtype, VB_AGG_SORT, VB_PART_RANGE, out));
+    StrState *t = str_attach(*out);
+    t->sort = true;
+    t->sort_vals = val_dtype >= 0;
     return VB_OK;
 }
 
@@ -4638,10 +4670,13 @@ extern "C" int32_t vb_shuffle_map_str(vb_shuf *s, uint32_t map_id, const uint64_
     if (loc < VB_HOST || loc > VB_DEVICE_BORROWED) return set_err(VB_ERR_INVALID, "bad src_loc %d", loc);
     if (n && !key_offsets) return set_err(VB_ERR_INVALID, "NULL key_offsets with n_rows > 0");
     if (n && n_bytes && !key_bytes) return set_err(VB_ERR_INVALID, "NULL key_bytes with n_bytes > 0");
-    if (n && !vals && s->agg != VB_AGG_COUNT) return set_err(VB_ERR_INVALID, "values required for this aggregator");
+    const bool sort = s->str->sort;
+    if (sort && !s->str->sort_vals && vals) return set_err(VB_ERR_INVALID, "shuffle %llu sorts keys only: vals must be NULL", (unsigned long long)s->id);
+    if (n && !vals && (sort ? s->str->sort_vals : s->agg != VB_AGG_COUNT)) return set_err(VB_ERR_INVALID, "values required for this aggregator");
     if (n >= 0xFFFFFFFEull) return set_err(VB_ERR_TOO_LARGE, "map partition of %llu rows", (unsigned long long)n);
     const u64 *col = (const u64 *)vals;
-    return str_map(s, map_id, key_offsets, key_bytes, n_bytes, &col, s->agg != VB_AGG_COUNT ? 1u : 0u, n, loc);
+    const u32 n_in = sort ? (s->str->sort_vals ? 1u : 0u) : (s->agg != VB_AGG_COUNT ? 1u : 0u);
+    return str_map(s, map_id, key_offsets, key_bytes, n_bytes, &col, n_in, n, loc);
 }
 
 extern "C" int32_t vb_shuffle_map_str_cols(vb_shuf *s, uint32_t map_id, const uint64_t *key_offsets, const void *key_bytes, uint64_t n_bytes,
@@ -4945,8 +4980,303 @@ static int seal_str_runs(vb_shuf *s, const std::vector<StrRun> &runs, int in = I
     return VB_OK;
 }
 
+static int seal_str_sort(vb_shuf *s, const std::vector<StrRun> &runs);
+
 // Seal of a string-key shuffle (world == 1, every map present)
-static int seal_str(vb_shuf *s) { return seal_str_runs(s, str_map_runs(s)); }
+static int seal_str(vb_shuf *s) { return s->str->sort ? seal_str_sort(s, str_map_runs(s)) : seal_str_runs(s, str_map_runs(s)); }
+
+// ---------------------------------------------------------------------------------------------
+// sort_by_key over string keys (vb_shuffle_create_str_sort): the string map side (dictionary encode, per-map entry
+// ids), the distinct keys ordered by their bytes on the device (strkeys.cuh, "sort_by_key over string keys"), and the
+// rows stably sorted by key rank with the id sort of GROUP.  Partitions are sort_cuts_kernel's contiguous ranges.
+// ---------------------------------------------------------------------------------------------
+
+// OR ^ AND of keys[0 .. n): the radix digits on which not every key agrees
+static int str_varying_bits(vb_shuf *s, const u64 *keys, u64 n, u64 *bits_dev, u64 *varying)
+{
+    vb_ctx *c = s->ctx;
+    const unsigned long long init[2] = {0ull, ~0ull};
+    CU(cudaMemcpyAsync(bits_dev, init, 16, cudaMemcpyHostToDevice, c->stream));
+    {
+        KLaunch kl(s, K_MISC);
+        key_bits_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(keys, 1, n, TX_NONE, (unsigned long long *)bits_dev);
+        TRY(kl.done("key_bits_kernel"));
+    }
+    u64 *h = (u64 *)c->h_scratch;
+    CU(cudaMemcpyAsync(h, bits_dev, 16, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    *varying = h[0] ^ h[1];
+    return VB_OK;
+}
+
+// Step 2 of the sort's seal: rank_of[e] for the D live entries live[0 .. D), in byte-wise lexicographic order of their
+// keys.  Round w over the na active entries (all of them at first, each with start 0):
+//   a. each entry's round-w sort key (str_sort_key: 7 key bytes and how the key goes on);
+//   b. LSD radix passes over the digits of the key on which the active entries differ, then (w > 0) over those of their
+//      starts: a stable sort by (start, key), entry ids as values;
+//   c. run heads (same start and key) and group heads (same start); new start = start + (run head − group head);
+//      a run of one is final, the others are compacted stably and go to round w + 1.
+// Rounds: 1 + ceil(longest prefix two distinct keys share / 7); each touches only the keys still tied.
+static int str_sort_order(vb_shuf *s, const u64 *live, u64 D, u32 *rank_of)
+{
+    vb_ctx *c = s->ctx;
+    StrState *t = s->str;
+    const u64 ne = t->n_e;
+    DevBuf ka(c), kb(c), va(c), vb(c), key_of(c), start_of(c), head(c), hx(c), stay(c), spos(c), gpos(c), runpos(c), hist(c), aux(c);
+    TRY(ka.alloc(D * 8)); TRY(kb.alloc(D * 8)); TRY(va.alloc(D * 8)); TRY(vb.alloc(D * 8));
+    TRY(key_of.alloc(ne * 8)); TRY(start_of.alloc(ne * 4));
+    TRY(head.alloc(D * 8)); TRY(hx.alloc(D * 8)); TRY(stay.alloc(D * 8)); TRY(spos.alloc(D * 8));
+    TRY(gpos.alloc(D * 4)); TRY(runpos.alloc(D * 4));
+    TRY(aux.alloc(32));                                   // [0, 2): key bits; [2]: runs; [3]: entries that stay
+    CU(cudaMemsetAsync(start_of.p, 0, ne * 4, c->stream));
+    u64 *bits = aux.as<u64>(), *n_runs = aux.as<u64>() + 2, *n_stay = aux.as<u64>() + 3;
+    auto other_k = [&](const u64 *p) { return p == ka.as<u64>() ? kb.as<u64>() : ka.as<u64>(); };
+    auto other_v = [&](const u64 *p) { return p == va.as<u64>() ? vb.as<u64>() : va.as<u64>(); };
+    const u64 *act = live;
+    u64 na = D;
+    for (u32 w = 0; na; ++w) {
+        if (7ull * w > t->n_a + 7) return set_err(VB_ERR_STATE, "string sort: round %u is past the longest key", w);
+        {
+            KLaunch kl(s, K_MISC, na);
+            str_sort_word_kernel<<<str_grid(c, na), 256, 0, c->stream>>>(act, na, t->d.e_off, t->d.e_len, t->d.arena, w, ka.as<u64>(),
+                                                                           key_of.as<u64>());
+            TRY(kl.done("str_sort_word_kernel"));
+        }
+        const u64 *k = ka.as<u64>(), *v = act;
+        const PassPlan plan = plan_pass<u64, true>(c, na);
+        TRY(hist.alloc(plan.hist_bytes()));
+        auto passes = [&](u64 varying) -> int {
+            for (u32 p = 0; p < 8; ++p) {
+                if (!((varying >> (8 * p)) & 0xFFull)) continue;
+                u64 *dk = other_k(k), *dv = other_v(v);
+                Digit dg{};
+                dg.mode = DG_BITS; dg.shift = 8 * p; dg.mask = 0xFF; dg.tx = TX_NONE;
+                TRY((radix_pass<u64, true>(s, Loader{LD_SOA64, k, v, 0}, dg, na, dk, dv, hist.as<u32>(), plan)));
+                k = dk;
+                v = dv;
+            }
+            return VB_OK;
+        };
+        u64 varying = 0;
+        TRY(str_varying_bits(s, k, na, bits, &varying));
+        TRY(passes(varying));
+        if (w > 0) {                                      // round 0: every start is 0
+            u64 *sk = other_k(k);
+            {
+                KLaunch kl(s, K_MISC, na);
+                str_sort_start_kernel<<<str_grid(c, na), 256, 0, c->stream>>>(v, na, start_of.as<u32>(), sk);
+                TRY(kl.done("str_sort_start_kernel"));
+            }
+            k = sk;
+            TRY(str_varying_bits(s, k, na, bits, &varying));
+            TRY(passes(varying));
+        }
+        {
+            KLaunch kl(s, K_MISC, na);
+            str_sort_heads_kernel<<<str_grid(c, na), 256, 0, c->stream>>>(v, na, key_of.as<u64>(), start_of.as<u32>(), head.as<u64>(),
+                                                                            gpos.as<u32>());
+            TRY(kl.done("str_sort_heads_kernel"));
+        }
+        TRY(exclusive_scan_u64(s, head.as<u64>(), hx.as<u64>(), na, n_runs));
+        {
+            KLaunch kl(s, K_MISC, na);
+            str_sort_runpos_kernel<<<str_grid(c, na), 256, 0, c->stream>>>(head.as<u64>(), hx.as<u64>(), na, runpos.as<u32>());
+            TRY(kl.done("str_sort_runpos_kernel"));
+        }
+        {
+            KLaunch kl(s, K_MISC, na);
+            str_sort_split_kernel<<<str_grid(c, na), 256, 0, c->stream>>>(v, head.as<u64>(), hx.as<u64>(), na, runpos.as<u32>(), n_runs,
+                                                                            gpos.as<u32>(), start_of.as<u32>(), rank_of, stay.as<u64>());
+            TRY(kl.done("str_sort_split_kernel"));
+        }
+        TRY(exclusive_scan_u64(s, stay.as<u64>(), spos.as<u64>(), na, n_stay));
+        u64 next = 0;
+        CU(cudaMemcpyAsync(&next, n_stay, 8, cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaStreamSynchronize(c->stream));
+        if (next) {
+            u64 *dst = other_v(v);
+            KLaunch kl(s, K_MISC, na);
+            str_compact_kernel<<<str_grid(c, na), 256, 0, c->stream>>>(stay.as<u64>(), spos.as<u64>(), v, na, dst);
+            TRY(kl.done("str_compact_kernel"));
+            act = dst;
+        }
+        na = next;
+    }
+    return VB_OK;
+}
+
+// The seal of a string sort over `runs` (map-id order):
+//   1. mark the entries the rows reference, and compact the D live ones stably;
+//   2. order them (str_sort_order): rank_of[entry];
+//   3. the keys once, in rank order: offsets (scan of the lengths) and bytes (str_gather_bytes_kernel);
+//   4. the rows' CSR by rank: with a payload, the rows in run order stably sorted by rank with their values (GROUP's
+//      str_group_values over ranks); key-only, each rank's row count (the COUNT fold of str_reduce_kernel), scanned;
+//   5. partition cuts (first CSR boundary at or after floor(p·n/R)) and per-partition key bytes (scan of count · len).
+// The per-map ids and the dictionary are freed at the end.
+static int seal_str_sort(vb_shuf *s, const std::vector<StrRun> &runs)
+{
+    vb_ctx *c = s->ctx;
+    StrState *t = s->str;
+    const u32 R = s->n_reduce;
+    const u64 ne = t->n_e;
+    s->bucket_off.assign((size_t)R + 1, 0);
+    s->val_off.assign((size_t)R + 1, 0);
+    t->kb_off.assign((size_t)R + 1, 0);
+    t->rank_cut.assign((size_t)R + 1, 0);
+    u64 n = 0;
+    for (const StrRun &r : runs) n += r.n;
+    if (n && ne) {
+        DevBuf live(c), flag(c), pos(c), list(c), tot(c), rank_of(c);
+        TRY(live.alloc(ne * 4));
+        TRY(flag.alloc(ne * 8));
+        TRY(pos.alloc(ne * 8));
+        TRY(tot.alloc(8));
+        CU(cudaMemsetAsync(live.p, 0, ne * 4, c->stream));
+        for (const StrRun &r : runs) {
+            KLaunch kl(s, K_MISC, r.n);
+            str_mark_live_kernel<<<str_grid(c, r.n), 256, 0, c->stream>>>(r.ids, r.n, live.as<u32>());
+            TRY(kl.done("str_mark_live_kernel"));
+        }
+        {
+            KLaunch kl(s, K_MISC, ne);
+            str_widen_u32_kernel<<<str_grid(c, ne), 256, 0, c->stream>>>(live.as<u32>(), ne, flag.as<u64>());
+            TRY(kl.done("str_widen_u32_kernel"));
+        }
+        TRY(exclusive_scan_u64(s, flag.as<u64>(), pos.as<u64>(), ne, tot.as<u64>()));
+        u64 D = 0;
+        CU(cudaMemcpyAsync(&D, tot.p, 8, cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaStreamSynchronize(c->stream));
+        if (D >= (1ull << 31)) return set_err(VB_ERR_TOO_LARGE, "%llu distinct string keys (fewer than 2^31 are supported)", (unsigned long long)D);
+        TRY(list.alloc(D * 8));
+        {
+            KLaunch kl(s, K_MISC, ne);
+            str_compact_kernel<<<str_grid(c, ne), 256, 0, c->stream>>>(flag.as<u64>(), pos.as<u64>(), nullptr, ne, list.as<u64>());
+            TRY(kl.done("str_compact_kernel"));
+        }
+        flag.reset();
+        pos.reset();
+        TRY(rank_of.alloc(ne * 4));
+        s->kclass_as = K_STR_ORDER;
+        const int rc = str_sort_order(s, list.as<u64>(), D, rank_of.as<u32>());
+        s->kclass_as = -1;
+        TRY(rc);
+        // 3. the keys in rank order
+        DevBuf eor(c), klen(c), koff(c), kbytes(c);
+        TRY(eor.alloc(D * 4));
+        TRY(klen.alloc(D * 8));
+        TRY(koff.alloc((D + 1) * 8));
+        {
+            KLaunch kl(s, K_MISC, D);
+            str_sort_rank_kernel<<<str_grid(c, D), 256, 0, c->stream>>>(list.as<u64>(), D, rank_of.as<u32>(), t->d.e_len, eor.as<u32>(),
+                                                                         klen.as<u64>());
+            TRY(kl.done("str_sort_rank_kernel"));
+        }
+        TRY(exclusive_scan_u64(s, klen.as<u64>(), koff.as<u64>(), D, koff.as<u64>() + D));
+        u64 nb = 0;
+        CU(cudaMemcpyAsync(&nb, koff.as<u64>() + D, 8, cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaStreamSynchronize(c->stream));
+        TRY(kbytes.alloc(nb));
+        {
+            KLaunch kl(s, K_MISC, D);
+            str_gather_bytes_kernel<<<(unsigned)((D * 32 + 255) / 256), 256, 0, c->stream>>>(eor.as<u32>(), (u32)D, t->d.e_off, koff.as<u64>(),
+                                                                                            t->d.arena, kbytes.as<unsigned char>());
+            TRY(kl.done("str_gather_bytes_kernel"));
+        }
+        // 4. the rows' CSR by rank, and the payload in row order
+        DevBuf roff(c), vals(c);
+        if (t->sort_vals) {
+            TRY(str_group_values(s, runs, n, rank_of.as<u32>(), D, roff, vals));
+        } else {
+            DevBuf cnt(c);
+            TRY(cnt.alloc(D * 8));
+            CU(cudaMemsetAsync(cnt.p, 0, D * 8, c->stream));
+            for (const StrRun &r : runs) TRY(str_reduce_rows(s, OPK_COUNT, TX_NONE, r.ids, nullptr, r.n, rank_of.as<u32>(), cnt.as<u64>()));
+            TRY(roff.alloc((D + 1) * 8));
+            TRY(exclusive_scan_u64(s, cnt.as<u64>(), roff.as<u64>(), D, roff.as<u64>() + D));
+        }
+        // 5. cuts, and the key bytes of every partition
+        DevBuf rb(c), boff(c), starts(c), rcut(c);
+        TRY(rb.alloc(D * 8));
+        TRY(boff.alloc((D + 1) * 8));
+        TRY(starts.alloc(((u64)R + 1) * 8));
+        TRY(rcut.alloc(((u64)R + 1) * 8));
+        {
+            KLaunch kl(s, K_MISC, D);
+            str_sort_row_bytes_kernel<<<str_grid(c, D), 256, 0, c->stream>>>(roff.as<u64>(), koff.as<u64>(), D, rb.as<u64>());
+            TRY(kl.done("str_sort_row_bytes_kernel"));
+        }
+        TRY(exclusive_scan_u64(s, rb.as<u64>(), boff.as<u64>(), D, boff.as<u64>() + D));
+        {
+            KLaunch kl(s, K_MISC);
+            str_sort_cuts_kernel<<<(R + 1 + 255) / 256, 256, 0, c->stream>>>(roff.as<u64>(), D, n, R, starts.as<u64>(), rcut.as<u64>());
+            TRY(kl.done("str_sort_cuts_kernel"));
+        }
+        CU(cudaMemcpyAsync(s->bucket_off.data(), starts.p, ((size_t)R + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaMemcpyAsync(t->rank_cut.data(), rcut.p, ((size_t)R + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaStreamSynchronize(c->stream));
+        TRY(str_read_at(s, boff.as<u64>(), t->rank_cut, t->kb_off));
+        s->n_keys = D;
+        s->st.rows_out = n;
+        t->key_off = (u64 *)koff.release();
+        t->key_bytes = (unsigned char *)kbytes.release();
+        t->row_off = (u64 *)roff.release();
+        t->row_boff = (u64 *)boff.release();
+        if (t->sort_vals) s->res_vals = (u64 *)vals.release();
+        CU(cudaStreamSynchronize(c->stream));
+    }
+    for (u32 m = 0; m < s->n_map; ++m) free_str_map(s, m);
+    free_str_dict(s);
+    return VB_OK;
+}
+
+static int copy_out_rebased(vb_shuf *s, u64 *dst, const u64 *src, u64 nk, u64 base, int dst_loc);
+
+// vb_shuffle_reduce_str of a string sort: partition r's rows in key order, each with its key (offsets from
+// str_sort_expand_kernel, bytes by str_gather_bytes_kernel over the row ranks), and the payload slice.
+static int str_sort_out(vb_shuf *s, uint32_t r, uint64_t *out_key_offsets, void *out_key_bytes, void *out_vals, int32_t dst_loc)
+{
+    TRY(wait_sealed(s));
+    vb_ctx *c = s->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    StrState *t = s->str;
+    const u64 row0 = s->bucket_off[r], nr = s->bucket_off[r + 1] - row0;
+    const u64 byte0 = t->kb_off[r], nb = t->kb_off[r + 1] - byte0;
+    if (nr == 0) {
+        TRY(copy_out_rebased(s, out_key_offsets, nullptr, 0, 0, dst_loc));
+        CU(cudaStreamSynchronize(c->stream));
+        return VB_OK;
+    }
+    if (out_key_offsets || (out_key_bytes && nb)) {
+        DevBuf off(c), rk(c), kb(c);
+        TRY(off.alloc((nr + 1) * 8));
+        TRY(rk.alloc(nr * 4));
+        {
+            KLaunch kl(s, K_MISC, nr);
+            str_sort_expand_kernel<<<str_grid(c, nr), 256, 0, c->stream>>>(t->row_off, t->row_boff, t->key_off, t->rank_cut[r], t->rank_cut[r + 1],
+                                                                             row0, nr, byte0, off.as<u64>(), rk.as<u32>());
+            TRY(kl.done("str_sort_expand_kernel"));
+        }
+        TRY(copy_out(s, out_key_offsets, off.p, (nr + 1) * 8, dst_loc));
+        if (out_key_bytes && nb) {
+            unsigned char *dst = (unsigned char *)out_key_bytes;
+            if (dst_loc == VB_HOST) {
+                TRY(kb.alloc(nb));
+                dst = kb.as<unsigned char>();
+            }
+            {
+                KLaunch kl(s, K_MISC, nr);
+                str_gather_bytes_kernel<<<(unsigned)((nr * 32 + 255) / 256), 256, 0, c->stream>>>(rk.as<u32>(), (u32)nr, t->key_off, off.as<u64>(),
+                                                                                                 t->key_bytes, dst);
+                TRY(kl.done("str_gather_bytes_kernel"));
+            }
+            if (dst_loc == VB_HOST) TRY(copy_out(s, out_key_bytes, kb.p, nb, dst_loc));
+        }
+    }
+    TRY(copy_out(s, out_vals, s->res_vals ? s->res_vals + row0 : nullptr, nr * 8, dst_loc));
+    CU(cudaStreamSynchronize(c->stream));
+    return VB_OK;
+}
 
 // ---------------------------------------------------------------------------------------------
 // string keys across ranks (vb_shuffle_create_str_dist): the map side of each rank is exported as key columns, packed
@@ -5113,6 +5443,7 @@ extern "C" int32_t vb_shuffle_create_str_dist(vb_ctx *c, uint64_t shuffle_id, ui
 static int str_dist_check(const vb_shuf *s, const char *what)
 {
     if (!s->str || s->multi) return set_err(VB_ERR_INVALID, "%s needs a shuffle from vb_shuffle_create_str_dist", what);
+    if (s->str->sort) return reject_str(s, "sort_by_key across ranks");
     if (s->world < 2) return set_err(VB_ERR_STATE, "%s needs a string shuffle of world > 1 (vb_shuffle_create_str_dist)", what);
     return VB_OK;
 }
@@ -5286,6 +5617,11 @@ extern "C" int32_t vb_shuffle_reduce_str(vb_shuf *s, uint32_t r, uint64_t *out_k
     if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
     if (s->multi && (out_combined || out_offsets || out_vals))
         return set_err(VB_ERR_INVALID, "shuffle %llu has several aggregates per key: read them with vb_shuffle_reduce_str_cols", (unsigned long long)s->id);
+    if (s->str->sort) {
+        if (out_offsets || out_vals) return set_err(VB_ERR_INVALID, "shuffle %llu sorts rows: it has no value lists (out_offsets / out_vals)", (unsigned long long)s->id);
+        if (out_combined && !s->str->sort_vals) return set_err(VB_ERR_INVALID, "key-only sort has no payload");
+        return str_sort_out(s, r, out_key_offsets, out_key_bytes, out_combined, dst_loc);
+    }
     void *const combined[1] = {out_combined};
     return str_reduce_out(s, r, out_key_offsets, out_key_bytes, combined, 1, out_offsets, out_vals, dst_loc);
 }
@@ -5704,7 +6040,7 @@ extern "C" int32_t vb_shuffle_stats(vb_shuf *s, vb_stats *out)
 }
 
 // per-kernel-class device time (profiling on): klass 0 hash_agg, 1 dict, 2 merge, 3 rp_hist,
-// 4 rp_scan, 5 rp_scatter, 6 misc, 7 join
+// 4 rp_scan, 5 rp_scatter, 6 misc, 7 join, 8 str_order
 extern "C" int32_t vb_shuffle_kernel_time(vb_shuf *s, int32_t klass, double *ms, uint64_t *launches)
 {
     if (!s || klass < 0 || klass >= K_N) return set_err(VB_ERR_INVALID, "bad argument");

@@ -527,4 +527,163 @@ __global__ void str_join_keep_kernel(const u64 *__restrict__ pos, u64 nk, u64 to
     idx[o] = o;
 }
 
+// ---- sort_by_key over string keys (engine.cu, "sort_by_key over string keys") -----------------------------------
+// The distinct keys are ordered by rounds over 7-byte big-endian words.  Every active entry carries `start`, the first
+// rank of the group of keys it still ties with; round w stably sorts the active entries by (start, its round-w key)
+// with the LSD radix passes, then gives each run of equal (start, key) the rank start + (run head − group head).  A
+// run of one is final; a longer run can only hold keys that go on past the word, and stays active for round w + 1.
+
+// Round w's sort key of a key of `len` bytes at arena + off: bytes [7w, 7w + 7) big-endian in bits 63..8 (zero past
+// the key's end), and min(len − 7w, 8) in bits 7..0 (0..7: the key ends inside the word; 8: it goes on).  Comparing
+// these u64s compares the keys' bytes from 7w on, a proper prefix first, so one sort key per round carries both.
+VB_D u64 str_sort_key(const unsigned char *arena, u64 off, u32 len, u32 w)
+{
+    const u64 pos = 7ull * w;
+    const u64 rest = len > pos ? len - pos : 0ull;
+    const u64 le = rest ? load_le<false>(arena + off, pos, rest < 7 ? (u32)rest : 7u) : 0ull;   // byte k at bits 8k
+    const u64 be = ((u64)__byte_perm((u32)le, 0u, 0x0123u) << 32) | __byte_perm((u32)(le >> 32), 0u, 0x0123u);
+    return be | (rest < 8 ? rest : 8ull);
+}
+
+// keys[i] = key_of[act[i]] = the round-w sort key of active entry act[i]
+__global__ void str_sort_word_kernel(const u64 *__restrict__ act, u64 na, const u64 *__restrict__ e_off, const u32 *__restrict__ e_len,
+                                     const unsigned char *__restrict__ arena, u32 w, u64 *__restrict__ keys, u64 *__restrict__ key_of)
+{
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < na; i += stride) {
+        const u64 e = act[i];
+        const u64 k = str_sort_key(arena, e_off[e], e_len[e], w);
+        keys[i] = k;
+        key_of[e] = k;
+    }
+}
+
+// keys[i] = start_of[se[i]]: the group starts in the order of the key passes, for the passes over the start
+__global__ void str_sort_start_kernel(const u64 *__restrict__ se, u64 na, const u32 *__restrict__ start_of, u64 *__restrict__ keys)
+{
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < na; i += stride) keys[i] = start_of[se[i]];
+}
+
+// Over the sorted active entries se: head[i] = 1 where a run of equal (start, key) begins; gpos[start] = the position
+// where the group of `start` begins.
+__global__ void str_sort_heads_kernel(const u64 *__restrict__ se, u64 na, const u64 *__restrict__ key_of, const u32 *__restrict__ start_of,
+                                      u64 *__restrict__ head, u32 *__restrict__ gpos)
+{
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < na; i += stride) {
+        const u64 e = se[i];
+        const u32 g = start_of[e];
+        bool gh = true, rh = true;
+        if (i) {
+            const u64 p = se[i - 1];
+            gh = start_of[p] != g;
+            rh = gh || key_of[p] != key_of[e];
+        }
+        head[i] = rh;
+        if (gh) gpos[g] = (u32)i;
+    }
+}
+
+// runpos[hx[i]] = i for every run head (hx: the exclusive scan of head, i.e. the run's index)
+__global__ void str_sort_runpos_kernel(const u64 *__restrict__ head, const u64 *__restrict__ hx, u64 na, u32 *__restrict__ runpos)
+{
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < na; i += stride)
+        if (head[i]) runpos[hx[i]] = (u32)i;
+}
+
+// Each sorted entry's new start: start + (its run head's position − its group head's position).  A run of one entry
+// is final (rank_of = the new start, stay = 0); the entries of a longer run keep the new start and stay active.
+// *n_runs: the number of runs (the total of the head scan).
+__global__ void str_sort_split_kernel(const u64 *__restrict__ se, const u64 *__restrict__ head, const u64 *__restrict__ hx, u64 na,
+                                      const u32 *__restrict__ runpos, const u64 *__restrict__ n_runs, const u32 *__restrict__ gpos,
+                                      u32 *__restrict__ start_of, u32 *__restrict__ rank_of, u64 *__restrict__ stay)
+{
+    const u64 nr = *n_runs;
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < na; i += stride) {
+        const u64 e = se[i];
+        const u64 r = hx[i] + head[i] - 1;
+        const u32 rp = runpos[r];
+        const u64 rend = r + 1 < nr ? runpos[r + 1] : na;
+        const u32 g = start_of[e];
+        const u32 ns = g + (rp - gpos[g]);
+        if (rend - rp == 1) {
+            rank_of[e] = ns;
+            stay[i] = 0;
+        } else {
+            start_of[e] = ns;
+            stay[i] = 1;
+        }
+    }
+}
+
+// out[pos[i]] = src[i] (src NULL: i) where flag[i]; pos is the exclusive scan of flag: a stable compaction
+__global__ void str_compact_kernel(const u64 *__restrict__ flag, const u64 *__restrict__ pos, const u64 *__restrict__ src, u64 n,
+                                   u64 *__restrict__ out)
+{
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
+        if (flag[i]) out[pos[i]] = src ? src[i] : i;
+}
+
+// entry_of_rank and each rank's key length, from the ranks of the D live entries
+__global__ void str_sort_rank_kernel(const u64 *__restrict__ live, u64 D, const u32 *__restrict__ rank_of, const u32 *__restrict__ e_len,
+                                     u32 *__restrict__ entry_of_rank, u64 *__restrict__ klen)
+{
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < D; i += stride) {
+        const u64 e = live[i];
+        const u32 r = rank_of[e];
+        entry_of_rank[r] = (u32)e;
+        klen[r] = e_len[e];
+    }
+}
+
+// out[k] = the bytes the rows of rank k carry: (roff[k + 1] − roff[k]) · (koff[k + 1] − koff[k])
+__global__ void str_sort_row_bytes_kernel(const u64 *__restrict__ roff, const u64 *__restrict__ koff, u64 D, u64 *__restrict__ out)
+{
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 k = (u64)blockIdx.x * blockDim.x + threadIdx.x; k < D; k += stride)
+        out[k] = (roff[k + 1] - roff[k]) * (koff[k + 1] - koff[k]);
+}
+
+// sort_cuts_kernel's rule over the rows' CSR by rank (roff [D + 1], roff[D] = n, every rank with rows): partition p
+// starts at the first rank boundary at or after floor(p·n/R), so no key is split.  starts[p]: its first row;
+// rank_cut[p]: its first rank.
+__global__ void str_sort_cuts_kernel(const u64 *__restrict__ roff, u64 D, u64 n, u32 n_parts, u64 *__restrict__ starts, u64 *__restrict__ rank_cut)
+{
+    const u32 p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p > n_parts) return;
+    const u64 c = ((u64)p * n) / n_parts;
+    u64 lo = 0, hi = D;                                   // the first k with roff[k] >= c (roff[D] = n >= c)
+    while (lo < hi) {
+        const u64 mid = lo + ((hi - lo) >> 1);
+        if (roff[mid] < c) lo = mid + 1; else hi = mid;
+    }
+    starts[p] = roff[lo];
+    rank_cut[p] = lo;
+}
+
+// One partition's rows [row0, row0 + nr), ranks [k0, k1): row j's rank by binary search in the CSR (so a hot key costs
+// what any key costs), its key's byte offset in the partition (the byte scan at its rank, plus its place in the
+// rank's run times the key's length, less byte0), and off[nr] = the partition's bytes.
+__global__ void str_sort_expand_kernel(const u64 *__restrict__ roff, const u64 *__restrict__ boff, const u64 *__restrict__ koff, u64 k0,
+                                       u64 k1, u64 row0, u64 nr, u64 byte0, u64 *__restrict__ off, u32 *__restrict__ rank_of_row)
+{
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 j = (u64)blockIdx.x * blockDim.x + threadIdx.x; j < nr; j += stride) {
+        const u64 g = row0 + j;
+        u64 lo = k0, hi = k1;
+        while (hi - lo > 1) {
+            const u64 mid = (lo + hi) >> 1;
+            if (roff[mid] <= g) lo = mid; else hi = mid;
+        }
+        off[j] = boff[lo] + (g - roff[lo]) * (koff[lo + 1] - koff[lo]) - byte0;
+        rank_of_row[j] = (u32)lo;
+        if (j == 0) off[nr] = boff[k1] - byte0;
+    }
+}
+
 }  // namespace vb

@@ -9,7 +9,7 @@ Differences forced by the boundary (SURVEY.md F4): rows are 64-bit POD (K,V) arr
 ("sum" | "min" | "max") because a closure cannot cross into CUDA.  Keys may also be Rust `String`s: a
 sequence of Python `str` or a `StrKeys` column (offsets + UTF-8 bytes), for reduce_by_key / count_by_key /
 group_by_key / partition_by_key / combine_by_key / count_by_value / distinct; they are placed as the reference places
-`String` keys.
+`String` keys.  sort_by_key / sort over them go through StrSortedRdd, which orders the keys by their bytes on the device.
 
 All compute happens in libvega_b200.so; this module slices the input exactly like
 ParallelCollection::slice, drives map tasks → seal → reduce tasks like the scheduler does
@@ -1220,16 +1220,24 @@ class StrShuffle(Shuffle):
     """One string-key shuffle (vb_shuffle_create_str; vb_shuffle_create_str_dist for rank `rank` of `world` > 1).
     multi: (value column dtype codes, [(vb_agg, column), ...]) for a combine_by_key shuffle (vb_shuffle_create_str_multi /
     _dist; vcode and agg are then ignored), mapped with map_cols and read with reduce_cols, exchanged with export_cols /
-    import_cols.  seal / exchange / stats / free as for Shuffle."""
+    import_cols.  sort=True: a sort_by_key shuffle (vb_shuffle_create_str_sort; agg is ignored) with one payload column
+    of dtype code vcode, or key-only with vcode None; reduce gives each row's key and its payload in key order.
+    seal / exchange / stats / free as for Shuffle."""
 
-    def __init__(self, sc, n_map, n_reduce, vcode, agg, hint=0, rank=0, world=1, multi=None):
+    def __init__(self, sc, n_map, n_reduce, vcode, agg, hint=0, rank=0, world=1, multi=None, sort=False):
         self.sc, self._lib = sc, sc._lib
         self.n_map, self.n_reduce, self.agg, self.vcode, self.kcode = n_map, n_reduce, agg, vcode, None
         self.rank, self.world = rank, world
         self.has_payload = True
         self._keepalive = []
         h = ctypes.c_void_p()
-        if multi is not None:
+        if sort:
+            if world > 1:
+                raise ValueError("sort_by_key over String keys runs on one process")
+            self.agg, self.has_payload = L.VB_AGG_SORT, vcode is not None
+            L.check(self._lib.vb_shuffle_create_str_sort(sc._h, sc.new_shuffle_id(), n_map, n_reduce, -1 if vcode is None else vcode,
+                                                         ctypes.byref(h)))
+        elif multi is not None:
             self.agg, self.vcode = L.VB_AGG_SUM, L.VB_U64
             codes, aggs = multi
             dts = (ctypes.c_int32 * len(codes))(*codes)
@@ -1306,10 +1314,16 @@ class StrShuffle(Shuffle):
         return nk.value, nb.value, nv.value
 
     def reduce_raw(self, r):
-        """Partition r on the host: (key offsets, key bytes, combined) or (key offsets, key bytes, offsets, values)."""
+        """Partition r on the host: (key offsets, key bytes, combined) or (key offsets, key bytes, offsets, values); a sort
+        gives (key offsets, key bytes, payload or None), one key per row."""
         nk, nb, nv = self.reduce_size(r)
         ko, kb = np.empty(nk + 1, dtype=np.uint64), np.empty(nb, dtype=np.uint8)
         p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
+        if self.agg == L.VB_AGG_SORT:
+            vals = np.empty(nk, dtype=_NP_OF[self.vcode]) if self.has_payload else None
+            L.check(self._lib.vb_shuffle_reduce_str(self._h, r, p(ko), p(kb), p(vals) if vals is not None else None, None, None,
+                                                    L.VB_HOST))
+            return ko, kb, vals
         if self.agg == L.VB_AGG_GROUP:
             offs, vals = np.empty(nk + 1, dtype=np.uint64), np.empty(nv, dtype=_NP_OF[self.vcode])
             L.check(self._lib.vb_shuffle_reduce_str(self._h, r, p(ko), p(kb), None, p(offs), p(vals), L.VB_HOST))
@@ -1650,6 +1664,65 @@ class StrCoGroupedRdd(_Base):
 
     def join_collect(self):
         return self.outer_join_collect((1 << len(self.rdds)) - 1)
+
+
+class StrSortedRdd(_Base):
+    """sort_by_key over `String` keys (PairRdd::sort_by_key, and Rdd::sort for a key-only parent) through
+    vb_shuffle_create_str_sort: rows ascending by key in Rust `String` order (bytes compared unsigned, a proper prefix
+    first), equal keys in input order, partitions contiguous key ranges cut as the integer sort cuts them.  parent: a
+    StrPairRdd of one value column (moved bit for bit), or a StrRdd (key-only).
+      compute(r) -> (keys as a numpy object array of str, values), or the keys alone;  collect(): partitions in order
+      compute_raw(r) -> (key offsets, key bytes, values or None), one key per row
+      compute_device(r, out_key_offsets=, out_key_bytes=, out_vals=): into torch CUDA tensors sized from the shuffle's
+      reduce_size (rows, key bytes)."""
+
+    def __init__(self, parent, num_splits):
+        if isinstance(parent, StrPairRdd):
+            if len(parent.cols) != 1:
+                raise TypeError("sort_by_key over String keys takes one value column")
+            vals = parent.cols[0]
+        elif isinstance(parent, StrRdd):
+            vals = None
+        else:
+            raise TypeError("StrSortedRdd takes a String-key PairRdd or Rdd (integer keys: PairRdd.sort_by_key / Rdd.sort)")
+        if num_splits < 1:
+            raise ValueError("num_splits must be >= 1")
+        self.parent, self.vals, self.num_slices, self.sc = parent, vals, num_splits, parent.sc
+        self._sh = None
+
+    def _run(self):
+        if self._sh is not None:
+            return self._sh
+        p = self.parent
+        starts = slice_starts(p.n, p.num_slices)
+        sh = StrShuffle(self.sc, len(starts) - 1, self.num_slices, self.vals.code if self.vals is not None else None, L.VB_AGG_SORT,
+                        sort=True)
+        for m in range(len(starts) - 1):
+            sh.map(m, p.keys, self.vals, int(starts[m]), int(starts[m + 1]))
+        sh.seal()
+        self._sh = sh
+        return sh
+
+    def compute_raw(self, split):
+        return self._run().reduce_raw(split)
+
+    def compute(self, split):
+        ko, kb, vals = self.compute_raw(split)
+        keys = _decode_keys(ko, kb)
+        return keys if self.vals is None else (keys, vals)
+
+    def compute_device(self, split, out_key_offsets=None, out_key_bytes=None, out_vals=None):
+        self._run().reduce_device(split, out_key_offsets=out_key_offsets, out_key_bytes=out_key_bytes, out_comb=out_vals)
+
+    def collect(self):
+        parts = [self.compute_raw(r) for r in range(self.num_slices)]
+        keys = np.concatenate([_decode_keys(ko, kb) for ko, kb, _ in parts])
+        if self.vals is None:
+            return keys
+        return keys, np.concatenate([v for _, _, v in parts])
+
+    def stats(self):
+        return self._run().stats()
 
 
 class StrRdd(Rdd):
