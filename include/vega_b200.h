@@ -633,9 +633,26 @@ VB_API int32_t vb_shuffle_import_str_cols(vb_shuf *s, const uint32_t *key_lens, 
  * set_hint / seal / stats / kernel_time / free work as for any shuffle; kernel_time class 8 is the ordering of the
  * distinct keys.  On this kind the integer map / reduce / join calls, vb_cogroup_n_str / vb_join_n_str,
  * vb_shuffle_create_narrow, vb_shuffle_set_key_width and the _str_cols calls return VB_ERR_INVALID; vb_shuffle_set_dist
- * with world > 1 and the export / import / exchange / blob calls return VB_ERR_UNSUPPORTED (across ranks: not yet). */
+ * with world > 1 and the export / import / exchange / blob calls return VB_ERR_UNSUPPORTED (across ranks:
+ * vb_shuffle_create_str_sort_dist). */
 VB_API int32_t vb_shuffle_create_str_sort(vb_ctx *ctx, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce,
                                           int32_t val_dtype /*VB_U64 / VB_I64 / VB_F64, or -1: key-only*/, vb_shuf **out);
+/* vb_shuffle_create_str_sort_dist: vb_shuffle_create_str_sort for rank `rank` of `world` (1 <= world <= 256; world 1
+ * is the one-process shuffle), with the same limits and argument checks.  Each rank maps its own map tasks (ascending
+ * blocks of map ids, rank order = map-id order); vb_shuffle_exchange(s, VB_XCHG_AUTO or VB_XCHG_NCCL) on a context
+ * with vb_ctx_comm_init then sorts locally, agrees on the exact cut keys with the other ranks word by word (only u64
+ * words and counts cross), and sends every rank's rows of output partition p to rank p % world in one grouped
+ * send/recv; seal re-sorts what arrived.  The partitions a rank owns are then identical, key bytes and payload bits
+ * row for row, to those of the one-process shuffle over the same map tasks; the other partitions are empty.
+ * Errors, the same on every rank: ranks whose val_dtype or n_reduce differ VB_ERR_INVALID; n_reduce > 4096
+ * VB_ERR_UNSUPPORTED; a rank that would receive 2^32 - 2 rows or more, or 2^31 keys or more, VB_ERR_TOO_LARGE.
+ * VB_XCHG_P2P, the _str / _str_cols export and import calls and vb_shuffle_set_dist return VB_ERR_UNSUPPORTED (agreeing
+ * on the cuts takes several collective rounds); seal at world > 1 without the exchange returns VB_ERR_STATE.
+ * vb_shuffle_exchange_stats: prepare_wall_ms the local sort, counts_wall_ms the all-gathers and the cut agreement,
+ * post_wall_ms the send/recv; sent_rows / recv_rows count rows.                                                     */
+VB_API int32_t vb_shuffle_create_str_sort_dist(vb_ctx *ctx, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce,
+                                               int32_t val_dtype /*VB_U64 / VB_I64 / VB_F64, or -1: key-only*/, uint32_t rank,
+                                               uint32_t world, vb_shuf **out);
 /* MetroHash64_1(bytes ‖ 0xFF, seed 0): the reference's hash of a `String` / `&str` key */
 VB_API uint64_t vb_hash_str(const void *bytes, uint64_t len);
 VB_API uint32_t vb_get_partition_str(const void *bytes, uint64_t len, uint32_t n_reduce);

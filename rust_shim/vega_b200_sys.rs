@@ -154,6 +154,10 @@ extern "C" {
     // key order, each with its key; the payload in out_combined); val_dtype -1 is key-only
     pub fn vb_shuffle_create_str_sort(ctx: *mut vb_ctx, shuffle_id: u64, n_map: u32, n_reduce: u32, val_dtype: i32,
                                       out: *mut *mut vb_shuf) -> i32;
+    // the same for rank `rank` of `world`: rows cross ranks through vb_shuffle_exchange (vb_ctx_comm_init), and rank r
+    // holds output partitions p with p % world == r
+    pub fn vb_shuffle_create_str_sort_dist(ctx: *mut vb_ctx, shuffle_id: u64, n_map: u32, n_reduce: u32, val_dtype: i32,
+                                           rank: u32, world: u32, out: *mut *mut vb_shuf) -> i32;
     pub fn vb_hash_str(bytes: *const c_void, len: u64) -> u64;
     pub fn vb_get_partition_str(bytes: *const c_void, len: u64, n_reduce: u32) -> u32;
     pub fn vb_shuffle_free(s: *mut vb_shuf) -> i32;

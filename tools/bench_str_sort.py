@@ -33,13 +33,9 @@ from vega_b200 import _lib as L  # noqa: E402
 from vega_b200.rdd import Shuffle, StrShuffle, _Col, _StrCol  # noqa: E402
 from tests.test_gpu_str_keys import _device_words  # noqa: E402
 
-n = int(float(sys.argv[1])) if len(sys.argv) > 1 else 50_000_000
 M = R = 8
-HOST_ROWS = min(n, 10_000_000)
 PREFIX = b"https://example.com/catalog/item"
 assert len(PREFIX) == 32
-smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
-GPU = {"gpu": torch.cuda.get_device_name(0), "nvidia_smi": smi.stdout.strip(), "rows": n, "map_slices": M, "partitions": R}
 
 
 def timed(f):
@@ -95,31 +91,40 @@ def host_workaround(sc, strs, vals):
     return int_sort(sc, ids, _Col(torch.from_numpy(vals).cuda(), role="value"), len(strs))
 
 
-sc = vb.Context(0)
-prof = vb.Context(0, profile=True)
-for name, mode, D, s in [("uniform 1e4", "uniform", 10_000, 0.0), ("uniform 1e6", "uniform", 1_000_000, 0.0),
-                         ("zipf 1.1 over 1e6", "zipf", 1_000_000, 1.1), ("all distinct", "unique", 0, 0.0),
-                         ("url, 32-byte shared prefix", "uniform", 1_000_000, 0.0)]:
-    ranks = torch.empty(n, dtype=torch.int64, device="cuda")
-    vals = torch.empty(n, dtype=torch.int64, device="cuda")
-    sc.gen_pairs(out_keys=ranks, out_vals=vals, n=n, mode=mode, n_distinct=max(D, 1), seed_k=5, zipf_s=s)
-    ranks &= (1 << 63) - 1 if mode == "unique" else (1 << 28) - 1
-    keys = url_keys(ranks) if name.startswith("url") else _device_words(ranks)
-    torch.cuda.synchronize()
-    K, V = _StrCol(keys), _Col(vals, role="value")
-    case = {"keys": name, **GPU, "key_bytes": int(keys.data.numel()), "distinct": int(torch.unique(ranks).numel())}
-    case["str_sort_ms"] = med3(lambda: str_sort(sc, K, V, n))
-    st = str_sort(prof, K, V, n)
-    case["device_ms"] = {k: round(v["ms"], 2) for k, v in st["kernels"].items() if v["ms"]}
-    case["str_order_launches"] = st["kernels"]["str_order"]["launches"]
-    case["int_rank_sort_ms"] = med3(lambda: int_sort(sc, ranks, V, n))
-    hk = vb.StrKeys(keys.offsets[:HOST_ROWS + 1].cpu().numpy(), keys.data[:int(keys.offsets[HOST_ROWS])].cpu().numpy())
-    strs = hk.to_strs()
-    hv = vals[:HOST_ROWS].cpu().numpy()
-    case["host_workaround_rows"] = HOST_ROWS
-    case["host_workaround_ms"] = round(timed(lambda: host_workaround(sc, strs, hv))[0], 1)
-    print(json.dumps(case), flush=True)
-    del ranks, vals, keys, K, V, hk, strs, hv
-    torch.cuda.empty_cache()
-prof.close()
-sc.close()
+def main():
+    n = int(float(sys.argv[1])) if len(sys.argv) > 1 else 50_000_000
+    host_rows = min(n, 10_000_000)
+    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
+    gpu = {"gpu": torch.cuda.get_device_name(0), "nvidia_smi": smi.stdout.strip(), "rows": n, "map_slices": M, "partitions": R}
+    sc = vb.Context(0)
+    prof = vb.Context(0, profile=True)
+    for name, mode, D, s in [("uniform 1e4", "uniform", 10_000, 0.0), ("uniform 1e6", "uniform", 1_000_000, 0.0),
+                             ("zipf 1.1 over 1e6", "zipf", 1_000_000, 1.1), ("all distinct", "unique", 0, 0.0),
+                             ("url, 32-byte shared prefix", "uniform", 1_000_000, 0.0)]:
+        ranks = torch.empty(n, dtype=torch.int64, device="cuda")
+        vals = torch.empty(n, dtype=torch.int64, device="cuda")
+        sc.gen_pairs(out_keys=ranks, out_vals=vals, n=n, mode=mode, n_distinct=max(D, 1), seed_k=5, zipf_s=s)
+        ranks &= (1 << 63) - 1 if mode == "unique" else (1 << 28) - 1
+        keys = url_keys(ranks) if name.startswith("url") else _device_words(ranks)
+        torch.cuda.synchronize()
+        K, V = _StrCol(keys), _Col(vals, role="value")
+        case = {"keys": name, **gpu, "key_bytes": int(keys.data.numel()), "distinct": int(torch.unique(ranks).numel())}
+        case["str_sort_ms"] = med3(lambda: str_sort(sc, K, V, n))
+        st = str_sort(prof, K, V, n)
+        case["device_ms"] = {k: round(v["ms"], 2) for k, v in st["kernels"].items() if v["ms"]}
+        case["str_order_launches"] = st["kernels"]["str_order"]["launches"]
+        case["int_rank_sort_ms"] = med3(lambda: int_sort(sc, ranks, V, n))
+        hk = vb.StrKeys(keys.offsets[:host_rows + 1].cpu().numpy(), keys.data[:int(keys.offsets[host_rows])].cpu().numpy())
+        strs = hk.to_strs()
+        hv = vals[:host_rows].cpu().numpy()
+        case["host_workaround_rows"] = host_rows
+        case["host_workaround_ms"] = round(timed(lambda: host_workaround(sc, strs, hv))[0], 1)
+        print(json.dumps(case), flush=True)
+        del ranks, vals, keys, K, V, hk, strs, hv
+        torch.cuda.empty_cache()
+    prof.close()
+    sc.close()
+
+
+if __name__ == "__main__":
+    main()

@@ -130,6 +130,7 @@ SYMBOLS = {
     "vb_shuffle_export_str_cols_buffers": (_i32, [_vp, _pvp, _pvp, _pvp, ctypes.POINTER(_u32)]),
     "vb_shuffle_import_str_cols": (_i32, [_vp, _vp, _vp, _vp, _u32, _pu64, _pu64]),
     "vb_shuffle_create_str_sort": (_i32, [_vp, _u64, _u32, _u32, _i32, _pvp]),
+    "vb_shuffle_create_str_sort_dist": (_i32, [_vp, _u64, _u32, _u32, _i32, _u32, _u32, _pvp]),
     "vb_hash_str": (_u64, [_vp, _u64]),
     "vb_get_partition_str": (_u32, [_vp, _u64, _u32]),
     "vb_shuffle_reduce_blob_size": (_i32, [_vp, _u32, _pu64]),

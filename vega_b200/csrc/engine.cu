@@ -391,6 +391,7 @@ static int export_str_locked(vb_shuf *s, u64 *n_keys, u64 *n_key_bytes, u64 *n_v
 static int str_import_limits(const vb_shuf *s, u64 nk, u64 nv);
 static int exchange_str_locked(vb_shuf *s);
 static int exchange_str_accs_locked(vb_shuf *s);
+static int exchange_str_sort_locked(vb_shuf *s);
 static void free_str(vb_shuf *s);
 
 static bool is_reduce_op(int agg) { return agg == VB_AGG_SUM || agg == VB_AGG_MIN || agg == VB_AGG_MAX || agg == VB_AGG_COUNT; }
@@ -2269,7 +2270,7 @@ constexpr u32 COMM_MAX_WORLD = 64;
 constexpr size_t COMM_HOST_OFF = 256 << 10;   // staging region inside vb_ctx::h_scratch
 // u64 per rank of the count all-gather: world + 2 for integer rows (counts, arena bytes and generation), world + 3 for
 // combine_by_key (counts and the spec's fingerprint), 3 * world for String keys, 2 * world + 3 for String-key
-// combine_by_key (key and byte counts, and the spec's fingerprint), 2 for sort
+// combine_by_key (key and byte counts, and the spec's fingerprint), 2 for sort, 3 for String sort
 static size_t comm_row(u32 world) { return std::max<size_t>({(size_t)world + 2, 3 * (size_t)world, 2 * (size_t)world + 3}); }
 
 static void comm_teardown(vb_ctx *c)
@@ -4980,7 +4981,7 @@ static int seal_str_runs(vb_shuf *s, const std::vector<StrRun> &runs, int in = I
     return VB_OK;
 }
 
-static int seal_str_sort(vb_shuf *s, const std::vector<StrRun> &runs);
+static int seal_str_sort(vb_shuf *s, const std::vector<StrRun> &runs, const std::vector<u64> *part_rows = nullptr);
 
 // Seal of a string-key shuffle (world == 1, every map present)
 static int seal_str(vb_shuf *s) { return s->str->sort ? seal_str_sort(s, str_map_runs(s)) : seal_str_runs(s, str_map_runs(s)); }
@@ -5111,9 +5112,11 @@ static int str_sort_order(vb_shuf *s, const u64 *live, u64 D, u32 *rank_of)
 //   3. the keys once, in rank order: offsets (scan of the lengths) and bytes (str_gather_bytes_kernel);
 //   4. the rows' CSR by rank: with a payload, the rows in run order stably sorted by rank with their values (GROUP's
 //      str_group_values over ranks); key-only, each rank's row count (the COUNT fold of str_reduce_kernel), scanned;
-//   5. partition cuts (first CSR boundary at or after floor(p·n/R)) and per-partition key bytes (scan of count · len).
+//   5. partition cuts (first CSR boundary at or after floor(p·n/R), or with part_rows, the owner's seal of a sort
+//      across ranks: the boundaries after each partition's given row count) and per-partition key bytes (scan of
+//      count · len).
 // The per-map ids and the dictionary are freed at the end.
-static int seal_str_sort(vb_shuf *s, const std::vector<StrRun> &runs)
+static int seal_str_sort(vb_shuf *s, const std::vector<StrRun> &runs, const std::vector<u64> *part_rows)
 {
     vb_ctx *c = s->ctx;
     StrState *t = s->str;
@@ -5206,7 +5209,17 @@ static int seal_str_sort(vb_shuf *s, const std::vector<StrRun> &runs)
             TRY(kl.done("str_sort_row_bytes_kernel"));
         }
         TRY(exclusive_scan_u64(s, rb.as<u64>(), boff.as<u64>(), D, boff.as<u64>() + D));
-        {
+        std::vector<u64> target;
+        if (part_rows) {
+            DevBuf tg(c);
+            target.assign((size_t)R + 1, 0);
+            for (u32 p = 0; p < R; ++p) target[p + 1] = target[p] + (*part_rows)[p];
+            TRY(tg.alloc(((u64)R + 1) * 8));
+            CU(cudaMemcpyAsync(tg.p, target.data(), ((size_t)R + 1) * 8, cudaMemcpyHostToDevice, c->stream));
+            KLaunch kl(s, K_MISC);
+            str_sort_cuts_at_kernel<<<(R + 1 + 255) / 256, 256, 0, c->stream>>>(roff.as<u64>(), D, tg.as<u64>(), R, starts.as<u64>(), rcut.as<u64>());
+            TRY(kl.done("str_sort_cuts_at_kernel"));
+        } else {
             KLaunch kl(s, K_MISC);
             str_sort_cuts_kernel<<<(R + 1 + 255) / 256, 256, 0, c->stream>>>(roff.as<u64>(), D, n, R, starts.as<u64>(), rcut.as<u64>());
             TRY(kl.done("str_sort_cuts_kernel"));
@@ -5214,6 +5227,7 @@ static int seal_str_sort(vb_shuf *s, const std::vector<StrRun> &runs)
         CU(cudaMemcpyAsync(s->bucket_off.data(), starts.p, ((size_t)R + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
         CU(cudaMemcpyAsync(t->rank_cut.data(), rcut.p, ((size_t)R + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
         CU(cudaStreamSynchronize(c->stream));
+        if (part_rows && s->bucket_off != target) return set_err(VB_ERR_STATE, "string sort: the received partitions do not end at key boundaries");
         TRY(str_read_at(s, boff.as<u64>(), t->rank_cut, t->kb_off));
         s->n_keys = D;
         s->st.rows_out = n;
@@ -5422,7 +5436,12 @@ static int seal_str_import(vb_shuf *s)
             runs.push_back(StrRun{ids.as<u32>(), t->i_vals, nk});
         }
     }
-    TRY(seal_str_runs(s, runs, IN_ACCS));
+    if (t->sort) {
+        if (s->sort_part_rows.size() != s->n_reduce) return set_err(VB_ERR_STATE, "sort_by_key over string keys across ranks goes through vb_shuffle_exchange");
+        TRY(seal_str_sort(s, runs, &s->sort_part_rows));
+    } else {
+        TRY(seal_str_runs(s, runs, IN_ACCS));
+    }
     free_str_xchg(s);
     return VB_OK;
 }
@@ -5443,7 +5462,7 @@ extern "C" int32_t vb_shuffle_create_str_dist(vb_ctx *c, uint64_t shuffle_id, ui
 static int str_dist_check(const vb_shuf *s, const char *what)
 {
     if (!s->str || s->multi) return set_err(VB_ERR_INVALID, "%s needs a shuffle from vb_shuffle_create_str_dist", what);
-    if (s->str->sort) return reject_str(s, "sort_by_key across ranks");
+    if (s->str->sort) return set_err(VB_ERR_UNSUPPORTED, "%s: sort_by_key over string keys across ranks goes through vb_shuffle_exchange (vb_ctx_comm_init)", what);
     if (s->world < 2) return set_err(VB_ERR_STATE, "%s needs a string shuffle of world > 1 (vb_shuffle_create_str_dist)", what);
     return VB_OK;
 }
@@ -5518,9 +5537,10 @@ extern "C" int32_t vb_shuffle_import_str(vb_shuf *s, const uint32_t *key_lens, c
 // vb_shuffle_exchange of a GROUP string shuffle: export, then the exchange of four columns: u32 key lengths and u32
 // value counts split by the key counts, key bytes by the byte counts, u64 values by the value counts.  The gathered
 // row is the three count vectors (keys, key bytes, values to every destination).  The received columns are owned by
-// the shuffle until seal.
+// the shuffle until seal.  A string sort takes its own path (exchange_str_sort_locked).
 static int exchange_str_locked(vb_shuf *s)
 {
+    if (s->str->sort) return exchange_str_sort_locked(s);
     vb_ctx *c = s->ctx;
     Comm *m = c->comm;
     StrState *t = s->str;
@@ -5549,6 +5569,258 @@ static int exchange_str_locked(vb_shuf *s)
     void **own = t->i_own;
     own[0] = lens.release(); own[1] = bytes.release(); own[2] = cnts.release(); own[3] = vals.release();
     str_take_import(s, (const u32 *)own[0], own[1], (const u32 *)own[2], (const u64 *)own[3], nk, nkb, nv);
+    return VB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// sort_by_key over string keys across ranks (vb_shuffle_create_str_sort_dist + vb_shuffle_exchange).  The integer
+// sort's shape (exchange_sort_locked) with byte-string cut keys:
+//   1. one all-gather of (local rows, val_dtype, n_reduce): a rank that differs is refused on every rank;
+//   2. the local sort (seal_str_sort over this rank's maps): distinct keys in rank order, the rows' CSR by key rank,
+//      the payload in row order;
+//   3. the exact cut keys s_p = the key of global row floor(p·N/R) - 1, agreed word by word for all cuts in lockstep
+//      (str_cut_round_kernel): per word one round gathers every rank's smallest and largest word in the cut's
+//      interval; if they differ, the ranks bisect [min, max] for the smallest word v whose global row count
+//      Σ row_off[upper bound of v] reaches the target, one round per probe.  A word whose tail says the key ends is
+//      final; otherwise the interval narrows to that word and the next one follows.  Only words and counts cross;
+//   4. one all-gather of every rank's (keys, key bytes, rows) per partition; the receive limits are checked for every
+//      rank from it, so all ranks refuse alike;
+//   5. one grouped send/recv of the String GROUP wire columns cut by partition (u32 key lengths, key bytes, u32 row
+//      counts per key, the u64 payload), received partition-major, then source-rank-major;
+//   6. seal_str_import re-encodes them and seal_str_sort re-sorts them as one run (equal keys meet only within a
+//      partition, in source-rank = map-id order), cut at the received partition totals.
+// ---------------------------------------------------------------------------------------------
+extern "C" int32_t vb_shuffle_create_str_sort_dist(vb_ctx *c, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce, int32_t val_dtype,
+                                                   uint32_t rank, uint32_t world, vb_shuf **out)
+{
+    if (!c || !out) return set_err(VB_ERR_INVALID, "vb_shuffle_create_str_sort_dist: NULL argument");
+    *out = nullptr;
+    if (world < 1 || world > 256 || rank >= world) return set_err(VB_ERR_INVALID, "bad rank %u / world %u (1 <= world <= 256)", rank, world);
+    TRY(vb_shuffle_create_str_sort(c, shuffle_id, n_map, n_reduce, val_dtype, out));
+    (*out)->rank = rank;
+    (*out)->world = world;
+    return VB_OK;
+}
+
+// Step 3: kcut[1 .. R) = each cut's local key rank (the local keys at or below s_p), over the D local keys koff /
+// kbytes and their rows' CSR roff.  A cut's word is w; with w > 0 its interval still has to be narrowed to the word
+// agreed at w - 1 (v), which the round's kernel does before it reads word w.  When the intervals of all ranks hold
+// one key between them, that key is s_p: the cut is final without reading the rest of its words.
+static int str_sort_agree_cuts(vb_shuf *s, const u64 *koff, const unsigned char *kbytes, const u64 *roff, u64 D, u64 N,
+                               std::vector<u64> &kcut)
+{
+    vb_ctx *c = s->ctx;
+    Comm *m = c->comm;
+    const u32 W = m->world, R = s->n_reduce, P = R - 1;
+    if (!P || !N) return VB_OK;
+    enum { MINMAX, BISECT, FINAL, DONE };
+    struct Cut { u64 need, lo, hi, v; u32 w; int st; };
+    std::vector<Cut> cut(P);
+    std::vector<u64> ab(2 * (size_t)P), cmd(2 * (size_t)P), all(3 * (size_t)P * W);
+    for (u32 i = 0; i < P; ++i) {
+        const u64 need = (u64)(((unsigned __int128)(i + 1) * N) / R);
+        cut[i] = Cut{need, 0, 0, 0, 0, need ? MINMAX : DONE};
+        ab[2 * i] = 0;
+        ab[2 * i + 1] = D;
+    }
+    DevBuf d_cmd(c), d_ab(c), d_out(c), d_all(c);
+    TRY(d_cmd.alloc((size_t)P * 16)); TRY(d_ab.alloc((size_t)P * 16)); TRY(d_out.alloc((size_t)P * 24)); TRY(d_all.alloc((size_t)P * 24 * W));
+    CU(cudaMemcpyAsync(d_ab.p, ab.data(), (size_t)P * 16, cudaMemcpyHostToDevice, c->stream));
+    // v agreed for cut i at its word: the key ends inside the word (tail < 8) or the search goes on with the next word
+    auto resolve = [](Cut &k, u64 v) {
+        k.v = v;
+        if ((v & 0xFF) < 8) { k.st = FINAL; return; }
+        k.st = MINMAX;
+        ++k.w;
+    };
+    for (;;) {
+        bool any = false, gather = false;
+        for (u32 i = 0; i < P; ++i) {
+            Cut &k = cut[i];
+            u64 op = SCUT_IDLE, w = k.w, v = 0;
+            if (k.st == MINMAX) {
+                op = k.w ? SCUT_NARROW : SCUT_MINMAX;
+                if (k.w) { w = k.w - 1; v = k.v; }
+            } else if (k.st == BISECT) {
+                op = SCUT_COUNT;
+                v = k.lo + ((k.hi - k.lo) >> 1);
+            } else if (k.st == FINAL) {
+                op = SCUT_FINAL;
+                v = k.v;
+                k.st = DONE;
+            }
+            cmd[2 * i] = op | w << 8;
+            cmd[2 * i + 1] = v;
+            any |= op != SCUT_IDLE;
+            gather |= op == SCUT_MINMAX || op == SCUT_NARROW || op == SCUT_COUNT;
+        }
+        if (!any) break;
+        CU(cudaMemcpyAsync(d_cmd.p, cmd.data(), (size_t)P * 16, cudaMemcpyHostToDevice, c->stream));
+        {
+            KLaunch kl(s, K_MISC);
+            str_cut_round_kernel<<<(P + 127) / 128, 128, 0, c->stream>>>(d_cmd.as<u64>(), P, koff, kbytes, roff, d_ab.as<u64>(), d_out.as<u64>());
+            TRY(kl.done("str_cut_round_kernel"));
+        }
+        if (!gather) continue;
+        NC(g_nccl.AllGather(d_out.p, d_all.p, 3 * (size_t)P, ncclUint64, m->comm, c->stream));
+        CU(cudaMemcpyAsync(all.data(), d_all.p, (size_t)P * 24 * W, cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaStreamSynchronize(c->stream));
+        for (u32 i = 0; i < P; ++i) {
+            Cut &k = cut[i];
+            const u64 op = cmd[2 * i] & 0xFF;
+            if (op == SCUT_MINMAX || op == SCUT_NARROW) {
+                u64 lo = ~0ull, hi = 0, keys = 0;
+                for (u32 r = 0; r < W; ++r) {
+                    lo = std::min(lo, all[(size_t)r * 3 * P + 3 * i]);
+                    hi = std::max(hi, all[(size_t)r * 3 * P + 3 * i + 1]);
+                    keys += all[(size_t)r * 3 * P + 3 * i + 2];
+                }
+                if (!keys) return set_err(VB_ERR_STATE, "string sort: cut %u has no key left on any rank", i + 1);
+                if (keys == 1) {                  // FINAL at the key's own word: every rank's cut is its b
+                    k.v = hi;
+                    k.st = FINAL;
+                } else if (lo == hi) {
+                    resolve(k, lo);
+                } else {
+                    k.lo = lo;
+                    k.hi = hi;
+                    k.st = BISECT;
+                }
+            } else if (op == SCUT_COUNT) {
+                u64 tot = 0;
+                for (u32 r = 0; r < W; ++r) tot += all[(size_t)r * 3 * P + 3 * i];
+                const u64 mid = cmd[2 * i + 1];
+                if (tot >= k.need) k.hi = mid; else k.lo = mid + 1;
+                if (k.lo == k.hi) resolve(k, k.lo);
+            }
+        }
+    }
+    CU(cudaMemcpyAsync(ab.data(), d_ab.p, (size_t)P * 16, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    for (u32 i = 0; i < P; ++i) kcut[i + 1] = cut[i].need ? ab[2 * i] : 0;
+    return VB_OK;
+}
+
+static int exchange_str_sort_locked(vb_shuf *s)
+{
+    vb_ctx *c = s->ctx;
+    Comm *m = c->comm;
+    StrState *t = s->str;
+    const u32 W = m->world, me = m->rank, R = s->n_reduce;
+    {
+        std::lock_guard<std::mutex> g(s->mu);
+        if (s->sealed || s->sealing || s->exported || s->freed) return set_err(VB_ERR_STATE, "export after seal/export");
+    }
+    auto clk = std::chrono::steady_clock::now();
+    // 1. rows and fingerprint, before any work: every rank refuses alike
+    const std::vector<StrRun> runs = str_map_runs(s);
+    u64 n_local = 0;
+    for (const StrRun &r : runs) n_local += r.n;
+    const u64 row[3] = {n_local, t->sort_vals ? (u64)s->vdt : ~0ull, R};
+    const u64 *mat = nullptr;
+    TRY(comm_all_gather(c, row, 3, &mat));
+    u64 N = 0;
+    for (u32 r = 0; r < W; ++r) {
+        N += mat[3 * r];
+        if (mat[3 * r + 1] != mat[1] || mat[3 * r + 2] != mat[2])
+            return set_err(VB_ERR_INVALID, "rank %u's string sort differs from rank 0's (val_dtype or n_reduce)", r);
+    }
+    if (R > 4096) return set_err(VB_ERR_UNSUPPORTED, "sort_by_key across ranks supports up to 4096 output partitions");
+    s->xst.counts_wall_ms += lap(clk);
+    // 2. local sort; its one-process partition cuts are not used.  It consumes the map side (ids and dictionary), so
+    // from here the shuffle counts as exported: after any later error a second exchange or a seal is VB_ERR_STATE
+    {
+        std::lock_guard<std::mutex> g(s->mu);
+        s->exported = true;
+    }
+    TRY(seal_str_sort(s, runs));
+    const u64 D = s->n_keys;
+    DevBuf koff(c), kbytes(c), roff(c), pay(c);
+    koff.p = t->key_off; kbytes.p = t->key_bytes; roff.p = t->row_off; pay.p = s->res_vals;
+    dev_free(c, t->row_boff);
+    t->key_off = nullptr; t->key_bytes = nullptr; t->row_off = nullptr; t->row_boff = nullptr;
+    s->res_vals = nullptr;
+    s->n_keys = 0;
+    s->st.rows_out = 0;
+    if (!D) {                                     // no local keys: one zero offset for the searches and reads
+        TRY(koff.alloc(8)); TRY(roff.alloc(8));
+        CU(cudaMemsetAsync(koff.p, 0, 8, c->stream));
+        CU(cudaMemsetAsync(roff.p, 0, 8, c->stream));
+    }
+    s->xst.prepare_wall_ms += lap(clk);
+    // 3. the cut keys
+    std::vector<u64> kcut((size_t)R + 1, 0);
+    kcut[R] = D;
+    TRY(str_sort_agree_cuts(s, koff.as<u64>(), kbytes.as<unsigned char>(), roff.as<u64>(), D, N, kcut));
+    for (u32 p = 1; p <= R; ++p) kcut[p] = std::max(kcut[p], kcut[p - 1]);
+    // 4. the segment table: keys, key bytes and rows of every partition, from every rank
+    std::vector<u64> kb_at, r_at, seg(3 * (size_t)R), segall(3 * (size_t)R * W);
+    TRY(str_read_at(s, koff.as<u64>(), kcut, kb_at));
+    TRY(str_read_at(s, roff.as<u64>(), kcut, r_at));
+    for (u32 p = 0; p < R; ++p) {
+        seg[p] = kcut[p + 1] - kcut[p];
+        seg[R + p] = kb_at[p + 1] - kb_at[p];
+        seg[2 * (size_t)R + p] = r_at[p + 1] - r_at[p];
+    }
+    {
+        DevBuf d_seg(c), d_segall(c);
+        TRY(d_seg.alloc(seg.size() * 8)); TRY(d_segall.alloc(segall.size() * 8));
+        CU(cudaMemcpyAsync(d_seg.p, seg.data(), seg.size() * 8, cudaMemcpyHostToDevice, c->stream));
+        NC(g_nccl.AllGather(d_seg.p, d_segall.p, seg.size(), ncclUint64, m->comm, c->stream));
+        CU(cudaMemcpyAsync(segall.data(), d_segall.p, segall.size() * 8, cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaStreamSynchronize(c->stream));
+    }
+    auto at = [&](u32 r, u32 col, u32 p) { return segall[(size_t)r * 3 * R + (size_t)col * R + p]; };
+    for (u32 d = 0; d < W; ++d) {
+        u64 nk = 0, nv = 0;
+        for (u32 p = d; p < R; p += W)
+            for (u32 r = 0; r < W; ++r) { nk += at(r, 0, p); nv += at(r, 2, p); }
+        TRY(str_import_limits(s, nk, nv));
+    }
+    s->xst.counts_wall_ms += lap(clk);
+    // 5. one grouped send/recv of the wire columns, cut by partition
+    DevBuf lens(c), cnts(c);
+    TRY(lens.alloc(D * 4));
+    TRY(cnts.alloc(D * 4));
+    for (int col = 0; D && col < 2; ++col) {
+        KLaunch kl(s, K_MISC, D);
+        str_diff_u32_kernel<<<str_grid(c, D), 256, 0, c->stream>>>(col ? roff.as<u64>() : koff.as<u64>(), D, col ? cnts.as<u32>() : lens.as<u32>());
+        TRY(kl.done("str_diff_u32_kernel"));
+    }
+    s->sort_part_rows.assign(R, 0);
+    u64 nk = 0, nkb = 0, nv = 0;
+    for (u32 p = me; p < R; p += W)
+        for (u32 r = 0; r < W; ++r) { nk += at(r, 0, p); nkb += at(r, 1, p); nv += at(r, 2, p); s->sort_part_rows[p] += at(r, 2, p); }
+    const bool vals = t->sort_vals;
+    DevBuf rl(c), rb(c), rn(c), rv(c);
+    TRY(rl.alloc(nk * 4)); TRY(rb.alloc(nkb)); TRY(rn.alloc(nk * 4));
+    if (vals) TRY(rv.alloc(nv * 8));
+    std::vector<Xfer> xs;
+    u64 sent = 0, own = 0;
+    for (u32 p = 0; p < R; ++p) {
+        const u32 d = p % W;
+        xs.push_back(Xfer{true, d, lens.as<u32>() + kcut[p], seg[p], ncclUint32});
+        xs.push_back(Xfer{true, d, kbytes.as<unsigned char>() + kb_at[p], seg[R + p], ncclUint8});
+        xs.push_back(Xfer{true, d, cnts.as<u32>() + kcut[p], seg[p], ncclUint32});
+        if (vals) xs.push_back(Xfer{true, d, pay.as<u64>() + r_at[p], seg[2 * (size_t)R + p], ncclUint64});
+        (d == me ? own : sent) += seg[2 * (size_t)R + p];
+    }
+    u64 ok = 0, ob = 0, ov = 0;
+    for (u32 p = me; p < R; p += W)
+        for (u32 r = 0; r < W; ++r) {
+            const u64 k = at(r, 0, p), b = at(r, 1, p), v = at(r, 2, p);
+            xs.push_back(Xfer{false, r, rl.as<u32>() + ok, k, ncclUint32});
+            xs.push_back(Xfer{false, r, rb.as<unsigned char>() + ob, b, ncclUint8});
+            xs.push_back(Xfer{false, r, rn.as<u32>() + ok, k, ncclUint32});
+            if (vals) xs.push_back(Xfer{false, r, rv.as<u64>() + ov, v, ncclUint64});
+            ok += k; ob += b; ov += v;
+        }
+    TRY(post_group(s, xs));
+    s->xst.post_wall_ms += lap(clk);
+    xchg_done(s, VB_XCHG_NCCL, sent, nv - own);
+    void **io = t->i_own;
+    io[0] = rl.release(); io[1] = rb.release(); io[2] = rn.release(); io[3] = vals ? rv.release() : nullptr;
+    str_take_import(s, (const u32 *)io[0], io[1], (const u32 *)io[2], (const u64 *)io[3], nk, nkb, nv);
     return VB_OK;
 }
 
@@ -5671,6 +5943,8 @@ extern "C" int32_t vb_shuffle_reduce_str_cols(vb_shuf *s, uint32_t r, uint64_t *
 // the checks every string _cols export / import call makes first
 static int str_multi_dist_check(const vb_shuf *s, const char *what)
 {
+    if (s->str && s->str->sort && s->world > 1)
+        return set_err(VB_ERR_UNSUPPORTED, "%s: sort_by_key over string keys across ranks goes through vb_shuffle_exchange (vb_ctx_comm_init)", what);
     if (!s->str || !s->multi) return set_err(VB_ERR_INVALID, "%s needs a shuffle from vb_shuffle_create_str_multi_dist", what);
     if (s->world < 2) return set_err(VB_ERR_STATE, "%s needs a string-key combine shuffle of world > 1 (vb_shuffle_create_str_multi_dist)", what);
     return VB_OK;

@@ -686,4 +686,79 @@ __global__ void str_sort_expand_kernel(const u64 *__restrict__ roff, const u64 *
     }
 }
 
+// ---- sort_by_key over string keys across ranks (engine.cu, exchange_str_sort_locked) ---------------------------
+// The ranks agree on each exact cut key word by word (str_sort_key's words).  A cut's state on one rank is ab[2i ..
+// 2i + 2) = [a, b): the local key ranks whose words 0 .. w-1 equal the words agreed so far, so that their word w is
+// non-decreasing over [a, b).  One thread per cut runs the round's command cmd[2i] = op | w << 8, cmd[2i + 1] = v.
+enum { SCUT_IDLE = 0, SCUT_MINMAX = 1, SCUT_COUNT = 2, SCUT_NARROW = 3, SCUT_FINAL = 4 };
+
+// the first key rank in [a, b) whose round-w word is greater than v (b if none), over the keys koff / kbytes
+VB_D u64 str_word_upper(const u64 *__restrict__ koff, const unsigned char *__restrict__ kbytes, u64 a, u64 b, u32 w, u64 v)
+{
+    while (a < b) {
+        const u64 mid = a + ((b - a) >> 1);
+        if (str_sort_key(kbytes, koff[mid], (u32)(koff[mid + 1] - koff[mid]), w) <= v) a = mid + 1; else b = mid;
+    }
+    return a;
+}
+
+// One round of the cut agreement, out[3i .. 3i + 3) per cut:
+//   MINMAX w       (word w of a, word w of b - 1, b - a), or (~0, 0, 0) for an empty interval;
+//   COUNT w, v     (roff[first rank past v at word w], 0, 0): the local rows whose key is at most the probed prefix;
+//   NARROW w, v    [a, b) becomes the ranks whose word w equals v, then MINMAX w + 1;
+//   FINAL w, v     a = b = the first rank past v at word w: the local key cut;
+//   IDLE           (0, 0, 0).
+__global__ void str_cut_round_kernel(const u64 *__restrict__ cmd, u32 n_cuts, const u64 *__restrict__ koff,
+                                     const unsigned char *__restrict__ kbytes, const u64 *__restrict__ roff, u64 *__restrict__ ab,
+                                     u64 *__restrict__ out)
+{
+    const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_cuts) return;
+    const u32 op = (u32)(cmd[2 * i] & 0xFF);
+    u32 w = (u32)(cmd[2 * i] >> 8);
+    const u64 v = cmd[2 * i + 1];
+    u64 a = ab[2 * i], b = ab[2 * i + 1];
+    u64 x = 0, y = 0, z = 0;
+    if (op == SCUT_COUNT) {
+        x = roff[str_word_upper(koff, kbytes, a, b, w, v)];
+    } else if (op == SCUT_FINAL) {
+        a = b = str_word_upper(koff, kbytes, a, b, w, v);
+    } else if (op == SCUT_MINMAX || op == SCUT_NARROW) {
+        if (op == SCUT_NARROW) {
+            const u64 hi = str_word_upper(koff, kbytes, a, b, w, v);
+            a = v ? str_word_upper(koff, kbytes, a, hi, w, v - 1) : a;
+            b = hi;
+            ++w;
+        }
+        x = ~0ull;
+        if (a < b) {
+            x = str_sort_key(kbytes, koff[a], (u32)(koff[a + 1] - koff[a]), w);
+            y = str_sort_key(kbytes, koff[b - 1], (u32)(koff[b] - koff[b - 1]), w);
+        }
+        z = b - a;
+    }
+    ab[2 * i] = a;
+    ab[2 * i + 1] = b;
+    out[3 * i] = x;
+    out[3 * i + 1] = y;
+    out[3 * i + 2] = z;
+}
+
+// str_sort_cuts_kernel with explicit row targets: rank_cut[p] = the first k with roff[k] >= target[p], starts[p] =
+// roff[k].  The owner of a cross-rank sort gets its partitions' first rows from the received totals.
+__global__ void str_sort_cuts_at_kernel(const u64 *__restrict__ roff, u64 D, const u64 *__restrict__ target, u32 n_parts,
+                                        u64 *__restrict__ starts, u64 *__restrict__ rank_cut)
+{
+    const u32 p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p > n_parts) return;
+    const u64 c = target[p];
+    u64 lo = 0, hi = D;
+    while (lo < hi) {
+        const u64 mid = lo + ((hi - lo) >> 1);
+        if (roff[mid] < c) lo = mid + 1; else hi = mid;
+    }
+    starts[p] = roff[lo];
+    rank_cut[p] = lo;
+}
+
 }  // namespace vb

@@ -246,13 +246,15 @@ def run_shuffle(engine, local_maps, n_map, n_reduce, kcode, vcode, agg, rank, wo
 class StrCudaEngine:
     """libvega_b200 on this rank's GPU, for String keys: CudaEngine's calls over vb_shuffle_create_str_dist.
     export gives ((n_keys, n_key_bytes, n_vals) per destination, (key_lens, key_bytes, val_counts, vals)), the wire
-    columns of include/vega_b200.h (val_counts None for reduce ops); import_ takes the same shape, source-rank major."""
+    columns of include/vega_b200.h (val_counts None for reduce ops); import_ takes the same shape, source-rank major.
+    agg VB_AGG_SORT is sort_by_key (vb_shuffle_create_str_sort_dist; vcode None: key-only): reduce then gives
+    (key offsets, key bytes, payload or None), one key per row, and the exchange needs the library's communicator."""
 
     def __init__(self, sc):
         self.sc = sc
 
     def create(self, n_map, n_reduce, vcode, agg, rank, world, hint=0):
-        return StrShuffle(self.sc, n_map, n_reduce, vcode, agg, hint=hint, rank=rank, world=world)
+        return StrShuffle(self.sc, n_map, n_reduce, vcode, agg, hint=hint, rank=rank, world=world, sort=agg == L.VB_AGG_SORT)
 
     def map(self, sh, map_id, keys, vals):
         """keys: a StrKeys column or a sequence of str; vals: a numpy array or torch CUDA tensor (None for count)."""
@@ -270,7 +272,7 @@ class StrCudaEngine:
         sh.seal()
 
     def reduce(self, sh, r):
-        return sh.reduce(r)
+        return sh.reduce_raw(r) if sh.agg == L.VB_AGG_SORT else sh.reduce(r)
 
 
 def _str_export(engine, sh, world):
@@ -287,7 +289,12 @@ def run_str_shuffle(engine, local_maps, n_map, n_reduce, vcode, agg, rank, world
     """run_shuffle for String keys: map side on this rank's partitions → exchange → reduce side for the partitions
     this rank owns.  local_maps: [(map_id, keys, vals_or_None)], ascending map ids from map_block(rank, world, n_map).
     With a communicator on the context the exchange is vb_shuffle_exchange (NCCL inside the library); otherwise
-    all_to_all_v of the four columns (exchange_device: "cpu" for a gloo group on a one-GPU box)."""
+    all_to_all_v of the four columns (exchange_device: "cpu" for a gloo group on a one-GPU box).  agg VB_AGG_SORT
+    (sort_by_key) across ranks has no such fallback: its cut keys are agreed in rounds of the library's collectives."""
+    if agg == L.VB_AGG_SORT and world > 1 and not (isinstance(engine, StrCudaEngine) and getattr(engine.sc, "comm", None)
+                                                   and exchange_device is None):
+        raise ValueError("sort_by_key over String keys across ranks needs the library's communicator (vb_ctx_comm_init, "
+                         "Context.comm_init) and runs its exchange inside the library")
     sh = engine.create(n_map, n_reduce, vcode, agg, rank, world, hint=hint)
     for map_id, keys, vals in local_maps:
         engine.map(sh, map_id, keys, vals)

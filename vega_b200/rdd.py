@@ -1221,7 +1221,9 @@ class StrShuffle(Shuffle):
     multi: (value column dtype codes, [(vb_agg, column), ...]) for a combine_by_key shuffle (vb_shuffle_create_str_multi /
     _dist; vcode and agg are then ignored), mapped with map_cols and read with reduce_cols, exchanged with export_cols /
     import_cols.  sort=True: a sort_by_key shuffle (vb_shuffle_create_str_sort; agg is ignored) with one payload column
-    of dtype code vcode, or key-only with vcode None; reduce gives each row's key and its payload in key order.
+    of dtype code vcode, or key-only with vcode None; reduce gives each row's key and its payload in key order.  With
+    world > 1 (vb_shuffle_create_str_sort_dist) the rows cross ranks through exchange() only, which needs the
+    library's communicator (Context.comm_init); rank r then holds the partitions p with p % world == r.
     seal / exchange / stats / free as for Shuffle."""
 
     def __init__(self, sc, n_map, n_reduce, vcode, agg, hint=0, rank=0, world=1, multi=None, sort=False):
@@ -1232,11 +1234,13 @@ class StrShuffle(Shuffle):
         self._keepalive = []
         h = ctypes.c_void_p()
         if sort:
-            if world > 1:
-                raise ValueError("sort_by_key over String keys runs on one process")
             self.agg, self.has_payload = L.VB_AGG_SORT, vcode is not None
-            L.check(self._lib.vb_shuffle_create_str_sort(sc._h, sc.new_shuffle_id(), n_map, n_reduce, -1 if vcode is None else vcode,
-                                                         ctypes.byref(h)))
+            vdt = -1 if vcode is None else vcode
+            if world > 1:
+                L.check(self._lib.vb_shuffle_create_str_sort_dist(sc._h, sc.new_shuffle_id(), n_map, n_reduce, vdt, rank, world,
+                                                                  ctypes.byref(h)))
+            else:
+                L.check(self._lib.vb_shuffle_create_str_sort(sc._h, sc.new_shuffle_id(), n_map, n_reduce, vdt, ctypes.byref(h)))
         elif multi is not None:
             self.agg, self.vcode = L.VB_AGG_SUM, L.VB_U64
             codes, aggs = multi
