@@ -506,6 +506,26 @@ VB_API int32_t vb_join_n_str(vb_shuf *const *sides, uint32_t n_sides, uint32_t r
                              uint64_t *out_key_offsets /*n_keys+1*/, void *out_key_bytes,
                              uint64_t *out_row_offsets /*n_keys+1*/, void *const *out_vals /*[n_sides] of n_rows*/,
                              uint8_t *const *out_valid /*[n_sides] or NULL; entries may be NULL*/, int32_t dst_loc);
+/* A sealed string reduce-op or combine_by_key shuffle as a cogroup / join parent under the same partitioner, without a
+ * shuffle: vb_shuffle_create_narrow for string keys.  *out is a new sealed string GROUP-kind shuffle: its partition r
+ * holds partition r of `parent` (the keys with vb_hash_str(key) % n_reduce == r), each key once, with the one-element
+ * list [its result].  out_col: the combine_by_key output column (0 for a single-aggregate shuffle).  Blocks until
+ * `parent` is sealed.
+ *   parents   SUM / MIN / MAX / COUNT shuffles of vb_shuffle_create_str(_dist), and any output column of a
+ *             vb_shuffle_create_str_multi(_dist) shuffle (MEAN and COUNT too).  The view's values are the column bit for
+ *             bit, of the column's output dtype: the value dtype for SUM / MIN / MAX, u64 for COUNT, f64 for MEAN.
+ *   refused   VB_ERR_INVALID, the parent staying usable: NULL arguments, integer-key parents (vb_shuffle_create_narrow
+ *             takes those), string GROUP parents (a view is one), string sort parents, out_col out of range.  A string
+ *             reduce shuffle itself stays refused by vb_cogroup_n_str / vb_join_n_str: the view is the side.
+ *   use       an ordinary sealed string GROUP shuffle: vb_shuffle_reduce_str(_size) gives the parent's keys, offsets
+ *             0..n and the column's values, and vb_cogroup_n_str(_size) / vb_join_n_str(_size) take it as any side, next
+ *             to GROUP shuffles and other views.  It has the parent's n_reduce, rank and world: on a rank of a multi-rank
+ *             shuffle it holds the partitions that rank owns, and the others are empty.  Like any side, its key index is
+ *             built by the first cogroup or join that reads it.
+ *   memory    the view owns copies of the key offsets, the key bytes and the column (24 B per key plus the key bytes)
+ *             and its key index, so the parent and the view may be freed in either order; free it with
+ *             vb_shuffle_free.                                                                                        */
+VB_API int32_t vb_shuffle_create_narrow_str(vb_shuf *parent, uint32_t out_col, vb_shuf **out);
 /* String keys across ranks (one process per GPU; ShuffleFetcher::fetch over `String` keys, shuffle_fetcher.rs:16-119).
  * vb_shuffle_create_str_dist is vb_shuffle_create_str for rank `rank` of `world` (1 <= world <= 256, VB_ERR_INVALID
  * otherwise); world == 1 gives the same shuffle as vb_shuffle_create_str.  Placement is unchanged: partition

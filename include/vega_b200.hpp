@@ -6,7 +6,8 @@
 //   PairRdd::group_by_key / reduce_by_key / join   src/rdd/pair_rdd.rs:35-52,54-80,104-121
 //   Rdd::count_by_value / distinct / collect       src/rdd/rdd.rs:450-459,502-522,420-434
 //   Rdd::intersection / subtract                   src/rdd/rdd.rs:838-946
-//   CoGroupedRdd::new over reduce results          src/rdd/co_grouped_rdd.rs:103-112 (OneToOneDependency; reduce_by_key_rdd)
+//   CoGroupedRdd::new over reduce results          src/rdd/co_grouped_rdd.rs:103-112 (OneToOneDependency; reduce_by_key_rdd,
+//                                                  integer and String keys)
 // Rows are Vec<(K,V)> with K in {u64,i64,i32,u32,std::string} and V in {u64,i64,f64}; std::string keys are placed
 // like the reference's String keys and support group_by_key / reduce_by_key / count_by_key / count_by_value /
 // distinct, and cogroup / join / outer joins of any number of parents.  reduce_by_key takes a named Op (the reference's serde_closure cannot cross into CUDA).  Errors throw vega::Error
@@ -86,6 +87,7 @@ public:
 
     // std::string keys (Rust String): group_by_key / reduce_by_key / count_by_key, count_by_value / distinct
     template <typename V> class StrPairRddT;
+    template <typename V> class StrReducedRddT;
     class StrKeyRddT;
     template <typename V>
     StrPairRddT<V> make_rdd(const std::vector<std::pair<std::string, V>> &data, size_t num_slices);
@@ -621,6 +623,67 @@ inline std::vector<std::string> read_str_part(vb_shuf *s, uint32_t r, std::vecto
     for (uint64_t i = 0; i < nk; ++i) keys.emplace_back(kb, ko[i], ko[i + 1] - ko[i]);
     return keys;
 }
+
+// CoGroupedRdd::compute over String keys (vb_cogroup_n_str) of sealed string GROUP sides, partition by partition: every
+// key of any side once, with one value list per side
+template <typename V>
+inline std::vector<std::pair<std::string, std::vector<std::vector<V>>>> read_str_cogroup_n(const std::vector<vb_shuf *> &sides,
+                                                                                           size_t num_splits)
+{
+    const uint32_t n = (uint32_t)sides.size();
+    std::vector<std::pair<std::string, std::vector<std::vector<V>>>> out;
+    for (uint32_t r = 0; r < num_splits; ++r) {
+        uint64_t nk = 0, nb = 0;
+        std::vector<uint64_t> nv(n);
+        check(vb_cogroup_n_str_size(sides.data(), n, r, &nk, &nb, nv.data()));
+        std::vector<uint64_t> ko(nk + 1);
+        std::string kb(nb, '\0');
+        std::vector<std::vector<uint64_t>> offs(n, std::vector<uint64_t>(nk + 1)), vals(n);
+        std::vector<uint64_t *> op(n);
+        std::vector<void *> vp(n);
+        for (uint32_t j = 0; j < n; ++j) { vals[j].resize(nv[j]); op[j] = offs[j].data(); vp[j] = vals[j].data(); }
+        check(vb_cogroup_n_str(sides.data(), n, r, ko.data(), kb.data(), op.data(), vp.data(), VB_HOST));
+        for (uint64_t i = 0; i < nk; ++i) {
+            std::vector<std::vector<V>> lists(n);
+            for (uint32_t j = 0; j < n; ++j)
+                for (uint64_t x = offs[j][i]; x < offs[j][i + 1]; ++x) lists[j].push_back(from_bits<V>(vals[j][x]));
+            out.emplace_back(std::string(kb, ko[i], ko[i + 1] - ko[i]), std::move(lists));
+        }
+    }
+    return out;
+}
+
+// the outer join (vb_join_n_str) of sealed string GROUP sides with `required`, partition by partition:
+// (k, [v_0, ..., v_{n-1}]) per row, std::nullopt where an optional side lacks the key
+template <typename V>
+inline std::vector<std::pair<std::string, std::vector<std::optional<V>>>> read_str_join_n_outer(const std::vector<vb_shuf *> &sides,
+                                                                                                size_t num_splits, uint32_t required)
+{
+    const uint32_t n = (uint32_t)sides.size();
+    std::vector<std::pair<std::string, std::vector<std::optional<V>>>> out;
+    for (uint32_t r = 0; r < num_splits; ++r) {
+        uint64_t rows = 0, nk = 0, nb = 0;
+        check(vb_join_n_str_size(sides.data(), n, r, required, &rows, &nk, &nb));
+        std::vector<uint64_t> ko(nk + 1), ro(nk + 1);
+        std::string kb(nb, '\0');
+        std::vector<std::vector<uint64_t>> vals(n, std::vector<uint64_t>(rows));
+        std::vector<std::vector<uint8_t>> valid(n, std::vector<uint8_t>(rows));
+        std::vector<void *> vp(n);
+        std::vector<uint8_t *> ok(n);
+        for (uint32_t j = 0; j < n; ++j) { vp[j] = vals[j].data(); ok[j] = valid[j].data(); }
+        check(vb_join_n_str(sides.data(), n, r, required, ko.data(), kb.data(), ro.data(), vp.data(), ok.data(), VB_HOST));
+        for (uint64_t i = 0; i < nk; ++i) {
+            const std::string k(kb, ko[i], ko[i + 1] - ko[i]);
+            for (uint64_t x = ro[i]; x < ro[i + 1]; ++x) {
+                std::vector<std::optional<V>> row(n);
+                for (uint32_t j = 0; j < n; ++j)
+                    if (valid[j][x]) row[j] = from_bits<V>(vals[j][x]);
+                out.emplace_back(k, std::move(row));
+            }
+        }
+    }
+    return out;
+}
 }  // namespace detail
 
 template <typename V>
@@ -661,6 +724,14 @@ public:
             for (size_t i = 0; i < k.size(); ++i) out.emplace_back(std::move(k[i]), detail::from_bits<V>(c[i]));
         }
         return out;
+    }
+
+    // reduce_by_key(op, num_splits) kept on the device: a StrReducedRddT to collect, or to join / cogroup with other
+    // results under the same num_splits without a second shuffle
+    StrReducedRddT<V> reduce_by_key_rdd(Op op, size_t num_splits) const
+    {
+        auto s = detail::run_str_shuffle(*sc_, keys_, &vals_, num_slices_, num_splits, detail::dtype<V>::code, (int)op);
+        return StrReducedRddT<V>(std::shared_ptr<vb_shuf>(s.release(), detail::ShufDeleter()), num_splits);
     }
 
     // count_by_key(num_splits).collect()  →  Vec<(String, u64)>
@@ -724,28 +795,7 @@ public:
                                                                                size_t num_splits) const
     {
         auto shs = group_shuffles(others, num_splits);
-        std::vector<vb_shuf *> sides = raw(shs);
-        const uint32_t n = (uint32_t)sides.size();
-        std::vector<std::pair<std::string, std::vector<std::vector<V>>>> out;
-        for (uint32_t r = 0; r < num_splits; ++r) {
-            uint64_t nk = 0, nb = 0;
-            std::vector<uint64_t> nv(n);
-            check(vb_cogroup_n_str_size(sides.data(), n, r, &nk, &nb, nv.data()));
-            std::vector<uint64_t> ko(nk + 1);
-            std::string kb(nb, '\0');
-            std::vector<std::vector<uint64_t>> offs(n, std::vector<uint64_t>(nk + 1)), vals(n);
-            std::vector<uint64_t *> op(n);
-            std::vector<void *> vp(n);
-            for (uint32_t j = 0; j < n; ++j) { vals[j].resize(nv[j]); op[j] = offs[j].data(); vp[j] = vals[j].data(); }
-            check(vb_cogroup_n_str(sides.data(), n, r, ko.data(), kb.data(), op.data(), vp.data(), VB_HOST));
-            for (uint64_t i = 0; i < nk; ++i) {
-                std::vector<std::vector<V>> lists(n);
-                for (uint32_t j = 0; j < n; ++j)
-                    for (uint64_t x = offs[j][i]; x < offs[j][i + 1]; ++x) lists[j].push_back(detail::from_bits<V>(vals[j][x]));
-                out.emplace_back(std::string(kb, ko[i], ko[i + 1] - ko[i]), std::move(lists));
-            }
-        }
-        return out;
+        return detail::read_str_cogroup_n<V>(raw(shs), num_splits);
     }
 
     // outer join of [self, others...] (vb_join_n_str): bit j of `required` marks parent j (this one is 0) required;
@@ -755,31 +805,7 @@ public:
                                                                                     size_t num_splits, uint32_t required) const
     {
         auto shs = group_shuffles(others, num_splits);
-        std::vector<vb_shuf *> sides = raw(shs);
-        const uint32_t n = (uint32_t)sides.size();
-        std::vector<std::pair<std::string, std::vector<std::optional<V>>>> out;
-        for (uint32_t r = 0; r < num_splits; ++r) {
-            uint64_t rows = 0, nk = 0, nb = 0;
-            check(vb_join_n_str_size(sides.data(), n, r, required, &rows, &nk, &nb));
-            std::vector<uint64_t> ko(nk + 1), ro(nk + 1);
-            std::string kb(nb, '\0');
-            std::vector<std::vector<uint64_t>> vals(n, std::vector<uint64_t>(rows));
-            std::vector<std::vector<uint8_t>> valid(n, std::vector<uint8_t>(rows));
-            std::vector<void *> vp(n);
-            std::vector<uint8_t *> ok(n);
-            for (uint32_t j = 0; j < n; ++j) { vp[j] = vals[j].data(); ok[j] = valid[j].data(); }
-            check(vb_join_n_str(sides.data(), n, r, required, ko.data(), kb.data(), ro.data(), vp.data(), ok.data(), VB_HOST));
-            for (uint64_t i = 0; i < nk; ++i) {
-                const std::string k(kb, ko[i], ko[i + 1] - ko[i]);
-                for (uint64_t x = ro[i]; x < ro[i + 1]; ++x) {
-                    std::vector<std::optional<V>> row(n);
-                    for (uint32_t j = 0; j < n; ++j)
-                        if (valid[j][x]) row[j] = detail::from_bits<V>(vals[j][x]);
-                    out.emplace_back(k, std::move(row));
-                }
-            }
-        }
-        return out;
+        return detail::read_str_join_n_outer<V>(raw(shs), num_splits, required);
     }
 
     // inner join of [self, others...]  →  (k, [v_0, ..., v_{n-1}]) per row
@@ -832,6 +858,100 @@ private:
     size_t num_slices_;
     detail::StrCol keys_;
     std::vector<uint64_t> vals_;
+};
+
+// A sealed String reduce_by_key result on the device (StrPairRddT::reduce_by_key_rdd).  Partition r holds the keys with
+// vb_hash_str(key) % num_splits == r, each once, so as a join / cogroup parent under the same num_splits it is read
+// through a view (vb_shuffle_create_narrow_str: CoGroupedRdd::new's OneToOneDependency, co_grouped_rdd.rs:103-112) and
+// not shuffled again; each key's list is [its result].  Parents of a join / cogroup must have the same num_splits
+// (vega::Error otherwise).
+template <typename V>
+class Context::StrReducedRddT {
+public:
+    StrReducedRddT(std::shared_ptr<vb_shuf> s, size_t num_splits) : s_(std::move(s)), num_splits_(num_splits) {}
+    size_t number_of_splits() const { return num_splits_; }
+
+    // collect()  →  Vec<(String, V)>
+    std::vector<std::pair<std::string, V>> collect() const
+    {
+        std::vector<std::pair<std::string, V>> out;
+        for (uint32_t r = 0; r < num_splits_; ++r) {
+            std::vector<uint64_t> c;
+            auto k = detail::read_str_part(s_.get(), r, &c, nullptr, nullptr);
+            for (size_t i = 0; i < k.size(); ++i) out.emplace_back(std::move(k[i]), detail::from_bits<V>(c[i]));
+        }
+        return out;
+    }
+
+    // self.join(other).collect()  →  Vec<(String, (V, W))>: the keys both results have, with both results
+    template <typename W>
+    std::vector<std::pair<std::string, std::pair<V, W>>> join(const StrReducedRddT<W> &other) const
+    {
+        auto a = view(*this), b = view(other);
+        std::vector<std::pair<std::string, std::pair<V, W>>> out;
+        for (auto &kv : detail::read_str_join_n_outer<uint64_t>({a.get(), b.get()}, num_splits_, 0b11))
+            out.emplace_back(std::move(kv.first), std::make_pair(detail::from_bits<V>(*kv.second[0]), detail::from_bits<W>(*kv.second[1])));
+        return out;
+    }
+
+    // self.cogroup(other).collect()  →  Vec<(String, (Vec<V>, Vec<W>))>: every key of either result once, with the list
+    // [result] from a result that has it and [] from the other
+    template <typename W>
+    std::vector<std::pair<std::string, std::pair<std::vector<V>, std::vector<W>>>> cogroup(const StrReducedRddT<W> &other) const
+    {
+        auto a = view(*this), b = view(other);
+        std::vector<std::pair<std::string, std::pair<std::vector<V>, std::vector<W>>>> out;
+        for (auto &kv : detail::read_str_cogroup_n<uint64_t>({a.get(), b.get()}, num_splits_)) {
+            std::vector<V> vs;
+            std::vector<W> ws;
+            for (uint64_t x : kv.second[0]) vs.push_back(detail::from_bits<V>(x));
+            for (uint64_t x : kv.second[1]) ws.push_back(detail::from_bits<W>(x));
+            out.emplace_back(std::move(kv.first), std::make_pair(std::move(vs), std::move(ws)));
+        }
+        return out;
+    }
+
+    // CoGroupedRdd::new([self, others...]).collect()  →  Vec<(String, Vec<Vec<V>>)>: every key of any result once, with
+    // the list [result] from each result that has it and [] from the others
+    std::vector<std::pair<std::string, std::vector<std::vector<V>>>> cogroup_n(const std::vector<StrReducedRddT> &others) const
+    {
+        auto views = views_of(others);
+        return detail::read_str_cogroup_n<V>(raw(views), num_splits_);
+    }
+
+    // outer join of [self, others...] with StrPairRddT::join_n_outer's `required` bitmask and row order
+    std::vector<std::pair<std::string, std::vector<std::optional<V>>>> join_n_outer(const std::vector<StrReducedRddT> &others,
+                                                                                    uint32_t required) const
+    {
+        auto views = views_of(others);
+        return detail::read_str_join_n_outer<V>(raw(views), num_splits_, required);
+    }
+
+    std::shared_ptr<vb_shuf> s_;
+    size_t num_splits_;
+
+private:
+    template <typename W>
+    detail::ShufPtr view(const StrReducedRddT<W> &p) const
+    {
+        if (p.num_splits_ != num_splits_) throw Error(VB_ERR_INVALID, "join / cogroup parents of reduce results need the same num_splits");
+        vb_shuf *v = nullptr;
+        check(vb_shuffle_create_narrow_str(p.s_.get(), 0, &v));
+        return detail::ShufPtr(v);
+    }
+    std::vector<detail::ShufPtr> views_of(const std::vector<StrReducedRddT> &others) const
+    {
+        std::vector<detail::ShufPtr> vs;
+        vs.push_back(view(*this));
+        for (auto &o : others) vs.push_back(view(o));
+        return vs;
+    }
+    static std::vector<vb_shuf *> raw(const std::vector<detail::ShufPtr> &vs)
+    {
+        std::vector<vb_shuf *> r;
+        for (auto &v : vs) r.push_back(v.get());
+        return r;
+    }
 };
 
 class Context::StrKeyRddT {

@@ -104,6 +104,7 @@ extern "C" {
     pub fn vb_shuffle_import_cols(s: *mut vb_shuf, keys: *const c_void, accs: *const c_void, n_acc: u32, counts: *const u64) -> i32;
     // a sealed reduce-op / combine_by_key shuffle as a cogroup or join side under the same partitioner (OneToOneDependency)
     pub fn vb_shuffle_create_narrow(parent: *mut vb_shuf, out_col: u32, out: *mut *mut vb_shuf) -> i32;
+    pub fn vb_shuffle_create_narrow_str(parent: *mut vb_shuf, out_col: u32, out: *mut *mut vb_shuf) -> i32;
     // String keys (Arrow-style offsets + bytes; placed by MetroHash64_1(bytes ‖ 0xFF) like `str::hash`)
     pub fn vb_shuffle_create_str(ctx: *mut vb_ctx, shuffle_id: u64, n_map: u32, n_reduce: u32, val_dtype: i32, agg: i32,
                                  out: *mut *mut vb_shuf) -> i32;

@@ -97,6 +97,7 @@ SYMBOLS = {
     "vb_shuffle_export_cols_buffers": (_i32, [_vp, _pvp, _pvp, ctypes.POINTER(_u32)]),
     "vb_shuffle_import_cols": (_i32, [_vp, _vp, _vp, _u32, _pu64]),
     "vb_shuffle_create_narrow": (_i32, [_vp, _u32, _pvp]),
+    "vb_shuffle_create_narrow_str": (_i32, [_vp, _u32, _pvp]),
     "vb_join_size": (_i32, [_vp, _vp, _u32, _pu64]),
     "vb_join": (_i32, [_vp, _vp, _u32, _vp, _vp, _vp, _i32]),
     "vb_join_outer_size": (_i32, [_vp, _vp, _u32, _i32, _pu64]),

@@ -6075,6 +6075,70 @@ static int str_key_index(vb_shuf *s)
     return VB_OK;
 }
 
+// A string reduce or combine result as a cogroup / join side without a second shuffle (vb_shuffle_create_narrow's string
+// form).  Partition r of the parent holds exactly the keys with vb_hash_str(key) % n_reduce == r, each once, so the view
+// is a sealed string GROUP shuffle over the same placement: copies of the key offsets, the key bytes and one result
+// column, and offsets 0..n (one value per key).  No dictionary is built here: the key index the joins probe comes from
+// str_key_index at the first cogroup or join, as for every GROUP side, and its kernel already inserts distinct keys
+// without comparing their bytes.
+static int narrow_str_build(vb_shuf *v, const vb_shuf *p, const u64 *col)
+{
+    vb_ctx *c = v->ctx;
+    const StrState *pt = p->str;
+    StrState *t = v->str;
+    const u64 n = p->n_keys, nb = pt->kb_off[p->n_reduce];
+    if (n == 0) return VB_OK;                         // an empty side: no arrays (as seal_str_runs leaves it)
+    DevBuf koff(c), kbytes(c), vals(c), offs(c);
+    TRY(koff.alloc((n + 1) * 8)); TRY(kbytes.alloc(nb)); TRY(vals.alloc(n * 8)); TRY(offs.alloc((n + 1) * 8));
+    CU(cudaMemcpyAsync(koff.p, pt->key_off, (n + 1) * 8, cudaMemcpyDeviceToDevice, c->stream));
+    if (nb) CU(cudaMemcpyAsync(kbytes.p, pt->key_bytes, nb, cudaMemcpyDeviceToDevice, c->stream));
+    CU(cudaMemcpyAsync(vals.p, col, n * 8, cudaMemcpyDeviceToDevice, c->stream));
+    {
+        KLaunch kl(v, K_MISC, n + 1);
+        range_kernel<<<str_grid(c, n + 1), 256, 0, c->stream>>>(offs.as<u64>(), 0, 1, n + 1);
+        TRY(kl.done("range_kernel"));
+    }
+    t->key_off = (u64 *)koff.release();
+    t->key_bytes = (unsigned char *)kbytes.release();
+    v->res_vals = (u64 *)vals.release();
+    v->res_offs = (u64 *)offs.release();
+    return VB_OK;
+}
+
+extern "C" int32_t vb_shuffle_create_narrow_str(vb_shuf *p, uint32_t out_col, vb_shuf **out)
+{
+    if (!p || !out) return set_err(VB_ERR_INVALID, "vb_shuffle_create_narrow_str: NULL argument");
+    *out = nullptr;
+    if (!p->str) return set_err(VB_ERR_INVALID, "vb_shuffle_create_narrow_str: shuffle %llu has integer keys (use vb_shuffle_create_narrow)",
+                                (unsigned long long)p->id);
+    if (p->str->sort || !is_reduce_op(p->agg))
+        return set_err(VB_ERR_INVALID, "vb_shuffle_create_narrow_str: shuffle %llu is not a string reduce-op or combine_by_key shuffle",
+                       (unsigned long long)p->id);
+    if (out_col >= p->outs.n) return set_err(VB_ERR_INVALID, "vb_shuffle_create_narrow_str: output column %u of %u", out_col, p->outs.n);
+    TRY(wait_sealed(p));
+    vb_ctx *c = p->ctx;
+    vb_shuf *v = make_internal_like(p);
+    v->agg = VB_AGG_GROUP;
+    v->vdt = p->out_dt[out_col];
+    v->rank = p->rank; v->world = p->world;
+    v->bucket_off = p->bucket_off; v->val_off = p->bucket_off;
+    v->n_keys = v->n_vals = v->st.rows_out = p->n_keys;
+    str_attach(v)->kb_off = p->str->kb_off;
+    int rc;
+    {
+        std::lock_guard<std::mutex> lk(c->mu);
+        rc = [&]() -> int {
+            CU(cudaSetDevice(c->device));
+            TRY(narrow_str_build(v, p, p->res_cols ? p->res_cols + (u64)out_col * p->n_keys : nullptr));
+            CU(cudaStreamSynchronize(c->stream));
+            return VB_OK;
+        }();
+    }
+    if (rc != VB_OK) { vb_shuffle_free(v); return rc; }
+    *out = v;
+    return VB_OK;
+}
+
 // describe the indexed string sides for the kernels
 static int str_n_sides(vb_shuf *const *sides, u32 n, u32 rid, StrNSides *a)
 {

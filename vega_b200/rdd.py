@@ -1262,6 +1262,22 @@ class StrShuffle(Shuffle):
         if hint:
             L.check(self._lib.vb_shuffle_set_hint(h, hint))
 
+    @classmethod
+    def narrow(cls, parent, out_col, vcode):
+        """vb_shuffle_create_narrow_str: the sealed String reduce or combine result `parent` (output column out_col) as a
+        sealed String GROUP side under the same partitioner, each key with the one-element list [its result] (vcode:
+        the column's dtype)."""
+        self = cls.__new__(cls)
+        self.sc, self._lib = parent.sc, parent._lib
+        self.n_map, self.n_reduce, self.agg, self.vcode, self.kcode = 0, parent.n_reduce, L.VB_AGG_GROUP, vcode, None
+        self.rank, self.world = parent.rank, parent.world
+        self.has_payload, self._keepalive = True, []
+        h = ctypes.c_void_p()
+        L.check(self._lib.vb_shuffle_create_narrow_str(parent._h, out_col, ctypes.byref(h)))
+        self._h = h
+        self.sc._shuffles.add(self)
+        return self
+
     def export(self):
         """vb_shuffle_export_str_prepare + buffers (world > 1): ((n_keys, n_key_bytes, n_vals), (key_lens, key_bytes,
         val_counts, vals)).  The counts are lists with one entry per destination rank; the columns are torch views of
@@ -1528,6 +1544,12 @@ class StrCombinedRdd(_Base):
         self._sh = sh
         return sh
 
+    def aggregate(self, name):
+        """The named aggregate as a StrCoGroupedRdd parent: (key, that aggregate's result) rows (StrAggregateRdd)."""
+        if name not in self.names:
+            raise ValueError(f"no aggregate named {name!r} (the aggregates are {self.names})")
+        return StrAggregateRdd(self, name)
+
     def compute_raw(self, split):
         return self._run().reduce_cols(split, self.out_dtypes)
 
@@ -1549,12 +1571,29 @@ class StrCombinedRdd(_Base):
         return self._run().stats()
 
 
+class StrAggregateRdd(_Base):
+    """One named aggregate of a StrCombinedRdd as a StrCoGroupedRdd parent (StrCombinedRdd.aggregate(name)), with the
+    list [its result] per key.  The combine shuffle runs once and is shared by every aggregate taken from it."""
+
+    def __init__(self, combined, name):
+        self.combined, self.name = combined, name
+        self.sc, self.num_slices = combined.sc, combined.num_slices
+
+    def _run(self):
+        return self.combined._run()
+
+    _result_col = AggregateRdd._result_col
+
+
 class StrCoGroupedRdd(_Base):
     """CoGroupedRdd::new(rdds, HashPartitioner::new(num_splits)) over `String` keys (vb_cogroup_n_str / vb_join_n_str):
     the cogroup and the joins of 1 to 16 parents, with keys matched by their bytes.  A parent is a StrPairRdd, shuffled
-    with the Vec-append aggregator, or a string reduce_by_key / count_by_key result, whose partitions are read on the
-    device and shuffled again with the list [its result] per key.  The methods are CoGroupedRdd's, with keys as a
-    numpy object array of str:
+    with the Vec-append aggregator, or a String reduce_by_key / count_by_key result or StrCombinedRdd.aggregate(name),
+    with the list [its result] per key.  Such a result's partition r already holds the keys with
+    vb_hash_str(key) % num_splits == r, each once, so under the same num_splits it joins through a view of the sealed
+    result (vb_shuffle_create_narrow_str: vega's OneToOneDependency, co_grouped_rdd.rs:103-112) with no second shuffle;
+    under another num_splits its partitions are read on the device and shuffled again.  The methods are CoGroupedRdd's,
+    with keys as a numpy object array of str:
       compute(r) -> (keys, [(offsets, values) per parent]);  collect() -> [(k, [vs_0, ..., vs_{n-1}])]
       join_compute(r) / join_collect() -> (k, [v_0, ..., v_{n-1}]), one k per row
       outer_join_compute(r, required) / outer_join_collect(required): optional parents as numpy.ma.MaskedArray
@@ -1572,8 +1611,10 @@ class StrCoGroupedRdd(_Base):
                 if r.agg_name not in _REDUCE_AGGS:
                     raise TypeError(f"parent {j}: a {r.agg_name} result is not a join parent (reduce_by_key and "
                                     "count_by_key results are)")
-            elif not isinstance(r, StrPairRdd):
-                raise TypeError(f"parent {j} is not a String-key PairRdd or reduce result")
+            elif isinstance(r, StrCombinedRdd):
+                raise TypeError(f"parent {j}: a combine_by_key result joins one aggregate at a time (.aggregate(name))")
+            elif not isinstance(r, (StrPairRdd, StrAggregateRdd)):
+                raise TypeError(f"parent {j} is not a String-key PairRdd, reduce result or combine_by_key aggregate")
         if any(r.sc is not rdds[0].sc for r in rdds):
             raise TypeError("the parents live on different contexts")
         self.rdds, self.num_slices, self.sc = rdds, num_splits, rdds[0].sc
@@ -1585,17 +1626,27 @@ class StrCoGroupedRdd(_Base):
         """The sealed string GROUP shuffle over num_splits partitions this parent gives."""
         if isinstance(r, StrPairRdd):
             return StrShuffledRdd(r, "group", self.num_slices)._run()
-        import torch
         sh = r._run()
+        col, n_cols, vcode = r._result_col(sh)
+        if sh.n_reduce == self.num_slices:
+            return StrShuffle.narrow(sh, col, vcode)
+        return self._reshuffled(sh, col, n_cols, vcode)
+
+    def _reshuffled(self, sh, col, n_cols, vcode):
+        """Result column `col` of the sealed shuffle sh shuffled again over num_splits partitions, one map task per result
+        partition read on the device."""
+        import torch
         dev = f"cuda:{sh._lib.vb_ctx_device(self.sc._h)}"
-        vcode = L.VB_U64 if sh.agg == L.VB_AGG_COUNT else sh.vcode
         out = StrShuffle(self.sc, sh.n_reduce, self.num_slices, vcode, L.VB_AGG_GROUP)
         for p in range(sh.n_reduce):
             nk, nb, _ = sh.reduce_size(p)
             ko = torch.empty(nk + 1, dtype=torch.int64, device=dev)
             kb = torch.empty(nb, dtype=torch.uint8, device=dev)
             v = torch.empty(nk, dtype=torch.int64, device=dev)
-            sh.reduce_device(p, out_key_offsets=ko, out_key_bytes=kb, out_comb=v)
+            if n_cols is None:
+                sh.reduce_device(p, out_key_offsets=ko, out_key_bytes=kb, out_comb=v)
+            else:
+                sh.reduce_cols(p, None, L.VB_DEVICE, ko, kb, [v if c == col else None for c in range(n_cols)])
             out.map(p, _StrCol(StrKeys(ko, kb)), _Col(v, role="value"), 0, nk)
         out.seal()
         return out
