@@ -43,8 +43,9 @@
  * (producer stream synchronised) before the call; results are complete when a call returns.
  * There is NO CPU fallback: without a CUDA device every compute entry returns VB_ERR_CUDA.
  *
- * Rows are POD (K,V) with 64-bit K and V; `Aggregator` closures (src/aggregator.rs:8-16) are
- * replaced by named ops (vb_agg).  Arbitrary K/V/closures stay on vega's CPU path.
+ * Rows are POD (K,V) with 64-bit K and V, or byte-string V (VB_BYTES) for the ops that only move values;
+ * `Aggregator` closures (src/aggregator.rs:8-16) are replaced by named ops (vb_agg).  Arbitrary K, values that
+ * are computed on, and closures stay on vega's CPU path.
  */
 #ifndef VEGA_B200_H
 #define VEGA_B200_H
@@ -70,7 +71,8 @@ enum vb_status {
     VB_ERR_TOO_LARGE = -6    /* more than 2^32-2 rows in one device-local shuffle / map partition */
 };
 
-enum vb_dtype { VB_U64 = 0, VB_I64 = 1, VB_F64 = 2 };
+/* VB_BYTES: byte-string values (a value dtype only), see "byte-string values" below. */
+enum vb_dtype { VB_U64 = 0, VB_I64 = 1, VB_F64 = 2, VB_BYTES = 3 };
 
 /* Aggregator (src/aggregator.rs).  GROUP = Default (Vec append, :33-52); SUM/MIN/MAX =
  * reduce_by_key(f) (src/rdd/pair_rdd.rs:65-80) for the named f; COUNT = count_by_value
@@ -673,6 +675,43 @@ VB_API int32_t vb_shuffle_create_str_sort(vb_ctx *ctx, uint64_t shuffle_id, uint
 VB_API int32_t vb_shuffle_create_str_sort_dist(vb_ctx *ctx, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce,
                                                int32_t val_dtype /*VB_U64 / VB_I64 / VB_F64, or -1: key-only*/, uint32_t rank,
                                                uint32_t world, vb_shuf **out);
+/* ---- byte-string values: `String` values as their UTF-8 bytes, any `V: Serialize` as its bincode bytes, for the ops
+ *      that move values without reading them: group_by_key / partition_by_key / cogroup / the joins (CoGroupedRdd::compute,
+ *      src/rdd/co_grouped_rdd.rs:206-249, PairRdd::join, src/rdd/pair_rdd.rs:104-121) and the sort_by_key payload ----
+ * VB_BYTES is accepted as the value dtype of vb_shuffle_create with VB_AGG_GROUP / VB_AGG_COGROUP / VB_AGG_SORT and of
+ * vb_shuffle_create_str with VB_AGG_GROUP; vb_shuffle_create_str_sort_bytes is sort_by_key over string keys with a
+ * byte-string payload (vb_shuffle_create_str_sort's rules; vb_shuffle_create_str_sort keeps refusing val_dtype 3 with
+ * VB_ERR_INVALID, as it always has).  Refused: with a reduce op or COUNT (VB_ERR_UNSUPPORTED); as a key dtype, in
+ * vb_agg_col specs or _multi value columns (VB_ERR_INVALID); vb_shuffle_create_str_dist and
+ * vb_shuffle_create_str_sort_dist with VB_BYTES, vb_shuffle_set_dist with world > 1, the export / import / exchange / P2P
+ * calls and the blob calls (VB_ERR_UNSUPPORTED).
+ *   map     vb_shuffle_map_bytes (integer keys, read as by vb_shuffle_map_soa, VB_DEVICE_BORROWED included) and
+ *           vb_shuffle_map_str_bytes (string keys, read as by vb_shuffle_map_str).  Value i is val_bytes[val_offsets[i] ..
+ *           val_offsets[i + 1]) (Arrow-style: n_rows + 1 offsets that need not start at 0).  The values and their offsets
+ *           are always COPIED, whatever src_loc is (VB_DEVICE_BORROWED applies to the keys only).  Offsets that decrease or
+ *           exceed n_val_bytes are VB_ERR_INVALID and a value of 2^32 bytes or more VB_ERR_TOO_LARGE, for device input
+ *           too.  Re-submitting a map_id replaces its values.  vb_shuffle_map_soa / _aos / _str on a bytes shuffle, and
+ *           the bytes calls on any other shuffle, are VB_ERR_INVALID.
+ *   values  every output call is unchanged and, where it writes values of a bytes shuffle, writes REFERENCES: opaque
+ *           64-bit words (vb_shuffle_reduce(_str) out_vals / out_combined, vb_join*, vb_cogroup*, vb_join_n*_str ...).  A
+ *           side's references are gathered from that side's shuffle.  References stay valid until vb_shuffle_free;
+ *           the reference 0 is never issued, so the 0 of an outer join's None slot gathers as an empty value (its validity
+ *           byte tells None from an empty value).
+ *   gather  vb_shuffle_gather_bytes_size gives the total bytes of n references; vb_shuffle_gather_bytes writes
+ *           out_offsets [n + 1] (from 0) and out_bytes, value i at out_bytes[out_offsets[i] .. [i + 1]).  Both block until
+ *           s is sealed.  refs come from src_loc (VB_HOST or VB_DEVICE); dst_loc is VB_HOST or VB_DEVICE.  A reference s
+ *           did not issue, or a NULL out_bytes with bytes to write, is VB_ERR_INVALID before anything is written, and s
+ *           stays usable.                           */
+VB_API int32_t vb_shuffle_map_bytes(vb_shuf *s, uint32_t map_id, const void *keys, const uint64_t *val_offsets /*n_rows+1*/,
+                                    const void *val_bytes, uint64_t n_val_bytes, uint64_t n_rows, int32_t src_loc);
+VB_API int32_t vb_shuffle_map_str_bytes(vb_shuf *s, uint32_t map_id, const uint64_t *key_offsets /*n_rows+1*/, const void *key_bytes,
+                                        uint64_t n_key_bytes, const uint64_t *val_offsets /*n_rows+1*/, const void *val_bytes,
+                                        uint64_t n_val_bytes, uint64_t n_rows, int32_t src_loc);
+VB_API int32_t vb_shuffle_create_str_sort_bytes(vb_ctx *ctx, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce, vb_shuf **out);
+VB_API int32_t vb_shuffle_gather_bytes_size(vb_shuf *s, const uint64_t *refs, uint64_t n, int32_t src_loc, uint64_t *n_bytes);
+VB_API int32_t vb_shuffle_gather_bytes(vb_shuf *s, const uint64_t *refs, uint64_t n, int32_t src_loc,
+                                       uint64_t *out_offsets /*n+1, from 0*/, void *out_bytes, int32_t dst_loc);
+
 /* MetroHash64_1(bytes ‖ 0xFF, seed 0): the reference's hash of a `String` / `&str` key */
 VB_API uint64_t vb_hash_str(const void *bytes, uint64_t len);
 VB_API uint32_t vb_get_partition_str(const void *bytes, uint64_t len, uint32_t n_reduce);

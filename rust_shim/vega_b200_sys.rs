@@ -12,7 +12,7 @@ use std::os::raw::{c_char, c_void};
 #[repr(C)] pub struct vb_agg_col { pub agg: i32, pub src: i32 }
 
 pub const VB_OK: i32 = 0;
-pub const VB_U64: i32 = 0; pub const VB_I64: i32 = 1; pub const VB_F64: i32 = 2;
+pub const VB_U64: i32 = 0; pub const VB_I64: i32 = 1; pub const VB_F64: i32 = 2; pub const VB_BYTES: i32 = 3;
 pub const VB_AGG_GROUP: i32 = 0; pub const VB_AGG_SUM: i32 = 1; pub const VB_AGG_MIN: i32 = 2;
 pub const VB_AGG_MAX: i32 = 3; pub const VB_AGG_COUNT: i32 = 4; pub const VB_AGG_COGROUP: i32 = 5;
 pub const VB_AGG_MEAN: i32 = 7;   // vb_agg_col only
@@ -151,6 +151,18 @@ extern "C" {
                                               accs: *mut *mut u64, n_acc: *mut u32) -> i32;
     pub fn vb_shuffle_import_str_cols(s: *mut vb_shuf, key_lens: *const u32, key_bytes: *const c_void, accs: *const u64, n_acc: u32,
                                       n_keys: *const u64, n_key_bytes: *const u64) -> i32;
+    // byte-string values (VB_BYTES = 3): a String as its UTF-8 bytes, any V: Serialize as its bincode bytes, for
+    // group / cogroup / join / sort; the output calls return opaque references, gathered back into bytes here
+    pub fn vb_shuffle_map_bytes(s: *mut vb_shuf, map_id: u32, keys: *const c_void, val_offsets: *const u64, val_bytes: *const c_void,
+                                n_val_bytes: u64, n_rows: u64, src_loc: i32) -> i32;
+    pub fn vb_shuffle_map_str_bytes(s: *mut vb_shuf, map_id: u32, key_offsets: *const u64, key_bytes: *const c_void, n_key_bytes: u64,
+                                    val_offsets: *const u64, val_bytes: *const c_void, n_val_bytes: u64, n_rows: u64,
+                                    src_loc: i32) -> i32;
+    pub fn vb_shuffle_create_str_sort_bytes(ctx: *mut vb_ctx, shuffle_id: u64, n_map: u32, n_reduce: u32,
+                                            out: *mut *mut vb_shuf) -> i32;
+    pub fn vb_shuffle_gather_bytes_size(s: *mut vb_shuf, refs: *const u64, n: u64, src_loc: i32, n_bytes: *mut u64) -> i32;
+    pub fn vb_shuffle_gather_bytes(s: *mut vb_shuf, refs: *const u64, n: u64, src_loc: i32, out_offsets: *mut u64,
+                                   out_bytes: *mut c_void, dst_loc: i32) -> i32;
     // sort_by_key over String keys (one process): map with vb_shuffle_map_str, read with vb_shuffle_reduce_str (rows in
     // key order, each with its key; the payload in out_combined); val_dtype -1 is key-only
     pub fn vb_shuffle_create_str_sort(ctx: *mut vb_ctx, shuffle_id: u64, n_map: u32, n_reduce: u32, val_dtype: i32,

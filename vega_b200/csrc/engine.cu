@@ -20,6 +20,7 @@
 #include "sweep.cuh"
 #include "gsweep.cuh"
 #include "strkeys.cuh"
+#include "bytevals.cuh"
 #include <type_traits>
 
 using namespace vb;
@@ -266,6 +267,7 @@ struct MapOut {
     const u64 *vals = nullptr;
     const u64 *cols[MA_MAX_COLS] = {};   // multi-aggregate shuffles: borrowed value columns (shared-table rebuilds)
     bool owned = false;
+    bool vals_owned = false;  // byte-string values: the reference column is the shuffle's even when the keys are borrowed
     bool in_shared = false;   // reduce ops, borrowed device input: combined straight into the shuffle's shared table
 };
 
@@ -375,6 +377,10 @@ struct vb_shuf {
     u64 lz_n = 0;
     std::vector<vb_shuf *> trash;                  // internal shuffles of a failed filtered join
     struct StrState *str = nullptr;                // string-key shuffle (vb_shuffle_create_str): dictionary, rows, results
+    // byte-string values (val dtype VB_BYTES): per map id the store of its values, kept until vb_shuffle_free; the
+    // device copy of the table is made by the first gather.  Internal shuffles of a filtered join have no store.
+    std::vector<ByteSrc> bvals;
+    ByteSrc *bvals_dev = nullptr;
     // by (the right side's uid, join kind): internal (left, right) shuffles over the rows that join kind keeps
     std::map<std::pair<u64, int>, std::pair<vb_shuf *, vb_shuf *>> filtered;
     // stats
@@ -1262,8 +1268,10 @@ extern "C" int32_t vb_shuffle_create(vb_ctx *c, uint64_t shuffle_id, uint32_t n_
     if (!c || !out) return set_err(VB_ERR_INVALID, "vb_shuffle_create: NULL argument");
     *out = nullptr;
     if (n_reduce < 1) return set_err(VB_ERR_INVALID, "vb_shuffle_create: n_reduce must be >= 1");
-    if (kdt < VB_U64 || kdt > VB_F64 || vdt < VB_U64 || vdt > VB_F64) return set_err(VB_ERR_INVALID, "bad dtype");
+    if (kdt < VB_U64 || kdt > VB_F64 || vdt < VB_U64 || vdt > VB_BYTES) return set_err(VB_ERR_INVALID, "bad dtype");
     if (agg < VB_AGG_GROUP || agg > VB_AGG_SORT) return set_err(VB_ERR_INVALID, "bad agg %d", agg);
+    if (vdt == VB_BYTES && !is_group_op(agg) && agg != VB_AGG_SORT)
+        return set_err(VB_ERR_UNSUPPORTED, "byte-string values go with GROUP, COGROUP and SORT only (agg %d computes on values)", agg);
     if (agg != VB_AGG_SORT && kdt == VB_F64) return set_err(VB_ERR_UNSUPPORTED, "f64 keys are not hashable (Rust f64 is not Hash)");
     if ((agg == VB_AGG_SORT) != (part == VB_PART_RANGE)) return set_err(VB_ERR_INVALID, "VB_PART_RANGE goes with VB_AGG_SORT only");
     if (n_reduce > 65536) return set_err(VB_ERR_UNSUPPORTED, "more than 65536 reduce partitions");
@@ -1278,6 +1286,7 @@ extern "C" int32_t vb_shuffle_create(vb_ctx *c, uint64_t shuffle_id, uint32_t n_
     s->agg = agg;
     s->part = part;
     s->maps.resize(n_map);
+    if (vdt == VB_BYTES) s->bvals.assign(n_map, ByteSrc{nullptr, nullptr, 0});
     *out = s;
     return VB_OK;
 }
@@ -1382,6 +1391,11 @@ static int reject_str(const vb_shuf *s, const char *what)
 {
     return set_err(VB_ERR_UNSUPPORTED, "shuffle %llu has string keys: %s is not supported for it yet", (unsigned long long)s->id, what);
 }
+// byte-string values stay on one device for now: every call that moves rows between ranks or serialises them
+static int reject_bytes(const vb_shuf *s, const char *what)
+{
+    return set_err(VB_ERR_UNSUPPORTED, "shuffle %llu has byte-string values: %s is not supported for them yet", (unsigned long long)s->id, what);
+}
 
 extern "C" int32_t vb_shuffle_set_key_width(vb_shuf *s, uint32_t bytes)
 {
@@ -1402,6 +1416,7 @@ extern "C" int32_t vb_shuffle_set_dist(vb_shuf *s, uint32_t rank, uint32_t world
 {
     if (!s || world < 1 || rank >= world || world > 256) return set_err(VB_ERR_INVALID, "bad rank/world");
     if (s->multi && (world > 1 || s->world > 1)) return reject_multi(s, "multi-rank use through vb_shuffle_set_dist (vb_shuffle_create_multi_dist is)");
+    if (s->vdt == VB_BYTES && world > 1) return set_err(VB_ERR_UNSUPPORTED, "shuffle %llu has byte-string values: they do not cross ranks yet", (unsigned long long)s->id);
     if (s->str && (world > 1 || s->world > 1)) return reject_str(s, "multi-rank use through vb_shuffle_set_dist (vb_shuffle_create_str_dist is)");
     s->rank = rank;
     s->world = world;
@@ -1413,14 +1428,16 @@ static void free_map(vb_shuf *s, MapOut &m)
     vb_ctx *c = s->ctx;
     if (m.table) dev_free(c, m.table);
     if (m.owned) { dev_free(c, m.rows); dev_free(c, m.keys); dev_free(c, m.vals); }
+    else if (m.vals_owned) dev_free(c, m.vals);
     m = MapOut();
 }
 
 static const AccSpec *map_spec(const vb_shuf *s) { return s->multi ? &s->acc_map : nullptr; }
 
 // cols: the value columns of a multi-aggregate shuffle (keys + cols, vals unused)
+// own_vals: a device value column the shuffle takes over (byte-string values: the references), read in place of vals
 static int shuffle_map(vb_shuf *s, u32 map_id, const u64 *rows, const u64 *keys, const u64 *vals, u64 n, int loc, bool combined = false,
-                       const u64 *const *cols = nullptr)
+                       const u64 *const *cols = nullptr, DevBuf *own_vals = nullptr)
 {
     if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
     if (s->str) return invalid_str(s, "an integer-key map call");
@@ -1526,6 +1543,7 @@ static int shuffle_map(vb_shuf *s, u32 map_id, const u64 *rows, const u64 *keys,
             else { m.keys = (const u64 *)a.release(); m.vals = vals ? (const u64 *)b.release() : nullptr; }
             m.owned = true;
         }
+        if (own_vals) { m.vals = (const u64 *)own_vals->release(); m.vals_owned = !m.owned; }
     }
     m.present = true;
     s->st.rows_in += n;
@@ -1536,6 +1554,7 @@ static int shuffle_map(vb_shuf *s, u32 map_id, const u64 *rows, const u64 *keys,
 extern "C" int32_t vb_shuffle_map_aos(vb_shuf *s, uint32_t map_id, const void *rows, uint64_t n, int32_t loc)
 {
     if (s && s->multi && !s->str) return reject_multi(s, "AoS rows");
+    if (s && s->vdt == VB_BYTES) return set_err(VB_ERR_INVALID, "shuffle %llu has byte-string values: map it with vb_shuffle_map_bytes", (unsigned long long)s->id);
     // every AoS loader reads a row as one 16-byte vector load; host rows are copied into aligned buffers first
     if (n && loc != VB_HOST && ((uintptr_t)rows & 15u))
         return set_err(VB_ERR_INVALID, "device AoS rows at %p: 16-byte rows must start on a 16-byte boundary", rows);
@@ -1544,6 +1563,7 @@ extern "C" int32_t vb_shuffle_map_aos(vb_shuf *s, uint32_t map_id, const void *r
 extern "C" int32_t vb_shuffle_map_soa(vb_shuf *s, uint32_t map_id, const void *keys, const void *vals, uint64_t n, int32_t loc)
 {
     if (s && s->multi) return set_err(VB_ERR_INVALID, "shuffle %llu has several aggregates per key: map it with vb_shuffle_map_cols", (unsigned long long)s->id);
+    if (s && s->vdt == VB_BYTES) return set_err(VB_ERR_INVALID, "shuffle %llu has byte-string values: map it with vb_shuffle_map_bytes", (unsigned long long)s->id);
     return shuffle_map(s, map_id, nullptr, (const u64 *)keys, (const u64 *)vals, n, loc);
 }
 extern "C" int32_t vb_shuffle_map_cols(vb_shuf *s, uint32_t map_id, const void *keys, const void *const *vals, uint64_t n, int32_t loc)
@@ -1963,6 +1983,7 @@ static int export_prepare_locked(vb_shuf *s, uint64_t *counts)
 
 extern "C" int32_t vb_shuffle_export_prepare(vb_shuf *s, uint64_t *counts)
 {
+    if (s && s->vdt == VB_BYTES) return reject_bytes(s, "vb_shuffle_export_prepare");
     if (!s || !counts) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "multi-rank exchange");
     if (s->str) return reject_str(s, "multi-rank exchange");
@@ -2080,6 +2101,7 @@ static int export_counts_locked(vb_shuf *s, uint64_t *counts)
 
 extern "C" int32_t vb_shuffle_export_counts(vb_shuf *s, uint64_t *counts)
 {
+    if (s && s->vdt == VB_BYTES) return reject_bytes(s, "vb_shuffle_export_counts");
     if (!s || !counts) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "multi-rank exchange");
     if (s->str) return reject_str(s, "multi-rank exchange");
@@ -2146,6 +2168,7 @@ static int export_direct_locked(vb_shuf *s, const uint64_t *dst_row_offset, cons
 
 extern "C" int32_t vb_shuffle_export_direct(vb_shuf *s, const uint64_t *dst_row_offset, const uint64_t *dst_total_rows)
 {
+    if (s && s->vdt == VB_BYTES) return reject_bytes(s, "vb_shuffle_export_direct");
     if (!s || !dst_row_offset || !dst_total_rows) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "multi-rank exchange");
     if (s->str) return reject_str(s, "multi-rank exchange");
@@ -2158,6 +2181,7 @@ extern "C" int32_t vb_shuffle_export_direct(vb_shuf *s, const uint64_t *dst_row_
 // source-rank major): hand them to the reduce side.  counts[world] as in vb_shuffle_import.
 extern "C" int32_t vb_shuffle_import_arena(vb_shuf *s, const uint64_t *counts)
 {
+    if (s && s->vdt == VB_BYTES) return reject_bytes(s, "vb_shuffle_import_arena");
     if (!s || !counts) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "multi-rank exchange");
     if (s->str) return reject_str(s, "multi-rank exchange");
@@ -2175,6 +2199,7 @@ extern "C" int32_t vb_shuffle_import_arena(vb_shuf *s, const uint64_t *counts)
 
 extern "C" int32_t vb_shuffle_export_buffers(vb_shuf *s, void **keys_dev, void **vals_dev)
 {
+    if (s && s->vdt == VB_BYTES) return reject_bytes(s, "vb_shuffle_export_buffers");
     if (!s || !keys_dev || !vals_dev) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "multi-rank exchange");
     if (s->str) return reject_str(s, "multi-rank exchange");
@@ -2186,6 +2211,7 @@ extern "C" int32_t vb_shuffle_export_buffers(vb_shuf *s, void **keys_dev, void *
 
 extern "C" int32_t vb_shuffle_import(vb_shuf *s, const void *keys_dev, const void *vals_dev, const uint64_t *counts)
 {
+    if (s && s->vdt == VB_BYTES) return reject_bytes(s, "vb_shuffle_import");
     if (!s || !counts) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "multi-rank exchange");
     if (s->str) return reject_str(s, "multi-rank exchange");
@@ -2896,6 +2922,7 @@ static int exchange_sort_locked(vb_shuf *s)
 
 extern "C" int32_t vb_shuffle_exchange(vb_shuf *s, int32_t mode)
 {
+    if (s && s->vdt == VB_BYTES) return reject_bytes(s, "vb_shuffle_exchange");
     if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
     if (s->multi && s->world < 2) return reject_multi(s, "an exchange of a one-process shuffle (vb_shuffle_create_multi_dist has world > 1)");
     if (s->multi && mode == VB_XCHG_P2P) return reject_multi(s, "the fused P2P exchange (VB_XCHG_NCCL is supported)");
@@ -3453,6 +3480,7 @@ static u64 blob_bytes(const vb_shuf *s, u32 r)
 
 extern "C" int32_t vb_shuffle_reduce_blob_size(vb_shuf *s, uint32_t r, uint64_t *n_bytes)
 {
+    if (s && s->vdt == VB_BYTES) return reject_bytes(s, "vb_shuffle_reduce_blob_size");
     if (!s || !n_bytes) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "bincode blobs");
     if (s->str) return reject_str(s, "bincode blobs");
@@ -3469,6 +3497,7 @@ extern "C" int32_t vb_shuffle_reduce_blob_size(vb_shuf *s, uint32_t r, uint64_t 
 
 extern "C" int32_t vb_shuffle_reduce_blob(vb_shuf *s, uint32_t r, void *out_blob, int32_t dst_loc)
 {
+    if (s && s->vdt == VB_BYTES) return reject_bytes(s, "vb_shuffle_reduce_blob");
     if (!s || !out_blob) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "bincode blobs");
     if (s->str) return reject_str(s, "bincode blobs");
@@ -3503,6 +3532,7 @@ extern "C" int32_t vb_shuffle_reduce_blob(vb_shuf *s, uint32_t r, void *out_blob
 
 extern "C" int32_t vb_shuffle_map_blob(vb_shuf *s, uint32_t map_id, const void *blob, uint64_t n_bytes, int32_t src_loc)
 {
+    if (s && s->vdt == VB_BYTES) return reject_bytes(s, "vb_shuffle_map_blob");
     if (!s || !blob) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "bincode blobs");
     if (s->str) return reject_str(s, "bincode blobs");
@@ -4442,6 +4472,19 @@ extern "C" int32_t vb_shuffle_create_str_sort(vb_ctx *c, uint64_t shuffle_id, ui
     return VB_OK;
 }
 
+// sort_by_key over string keys with a byte-string payload: the shuffle of vb_shuffle_create_str_sort, mapped with
+// vb_shuffle_map_str_bytes; its payload column holds the references, moved by the sort as any u64 payload
+extern "C" int32_t vb_shuffle_create_str_sort_bytes(vb_ctx *c, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce, vb_shuf **out)
+{
+    if (!c || !out) return set_err(VB_ERR_INVALID, "vb_shuffle_create_str_sort_bytes: NULL argument");
+    *out = nullptr;
+    TRY(vb_shuffle_create(c, shuffle_id, n_map, n_reduce, VB_U64, VB_BYTES, VB_AGG_SORT, VB_PART_RANGE, out));
+    StrState *t = str_attach(*out);
+    t->sort = true;
+    t->sort_vals = true;
+    return VB_OK;
+}
+
 // Reallocate one device array to `cap` elements of `sz` bytes, keeping the first `keep`.
 template <typename T>
 static int str_regrow(vb_ctx *c, T **p, u64 cap, u64 keep)
@@ -4594,7 +4637,7 @@ static int str_encode(vb_shuf *s, const u64 *offs, const unsigned char *bytes, u
 // passes its one column (none for COUNT), a combine_by_key shuffle every column an aggregate reads.  Reduce ops keep
 // them as the spec's value columns (cols), GROUP as its values (vals).
 static int str_map(vb_shuf *s, u32 map_id, const uint64_t *key_offsets, const void *key_bytes, u64 n_bytes, const u64 *const *in, u32 n_in,
-                   u64 n, int loc)
+                   u64 n, int loc, DevBuf *own_vals = nullptr)
 {
     {
         std::lock_guard<std::mutex> g(s->mu);
@@ -4653,6 +4696,10 @@ static int str_map(vb_shuf *s, u32 map_id, const uint64_t *key_offsets, const vo
             else t->vals[map_id] = p;
         }
     }
+    if (n && own_vals) {                           // byte-string values: the references, owned whatever loc is
+        t->vals[map_id] = (const u64 *)own_vals->release();
+        t->vals_owned[map_id] = 1;
+    }
     m.present = true;
     m.n_rows = n;
     s->st.rows_in += n;
@@ -4667,6 +4714,7 @@ extern "C" int32_t vb_shuffle_map_str(vb_shuf *s, uint32_t map_id, const uint64_
     if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
     if (!s->str) return set_err(VB_ERR_INVALID, "vb_shuffle_map_str needs a shuffle from vb_shuffle_create_str");
     if (s->multi) return set_err(VB_ERR_INVALID, "shuffle %llu has several aggregates per key: map it with vb_shuffle_map_str_cols", (unsigned long long)s->id);
+    if (s->vdt == VB_BYTES) return set_err(VB_ERR_INVALID, "shuffle %llu has byte-string values: map it with vb_shuffle_map_str_bytes", (unsigned long long)s->id);
     if (map_id >= s->n_map) return set_err(VB_ERR_INVALID, "map_id %u >= n_map %u", map_id, s->n_map);
     if (loc < VB_HOST || loc > VB_DEVICE_BORROWED) return set_err(VB_ERR_INVALID, "bad src_loc %d", loc);
     if (n && !key_offsets) return set_err(VB_ERR_INVALID, "NULL key_offsets with n_rows > 0");
@@ -4698,6 +4746,211 @@ extern "C" int32_t vb_shuffle_map_str_cols(vb_shuf *s, uint32_t map_id, const ui
         if (n && read[i] && !cols[i]) return set_err(VB_ERR_INVALID, "value column %u is read by an aggregate but NULL", i);
     if (n >= 0xFFFFFFFEull) return set_err(VB_ERR_TOO_LARGE, "map partition of %llu rows", (unsigned long long)n);
     return str_map(s, map_id, key_offsets, key_bytes, n_bytes, cols, s->n_cols, n, loc);
+}
+
+// ---------------------------------------------------------------------------------------------
+// byte-string values (bytevals.cuh): a map call copies its values into a store of the shuffle and maps the rows'
+// references as ordinary u64 values; vb_shuffle_gather_bytes* turn references back into bytes
+// ---------------------------------------------------------------------------------------------
+static int bytes_check_args(vb_shuf *s, u32 map_id, const u64 *val_offsets, const void *val_bytes, u64 n_val_bytes, u64 n, int loc)
+{
+    if (map_id >= s->n_map) return set_err(VB_ERR_INVALID, "map_id %u >= n_map %u", map_id, s->n_map);
+    if (loc < VB_HOST || loc > VB_DEVICE_BORROWED) return set_err(VB_ERR_INVALID, "bad src_loc %d", loc);
+    if (n && !val_offsets) return set_err(VB_ERR_INVALID, "NULL val_offsets with n_rows > 0");
+    if (n && n_val_bytes && !val_bytes) return set_err(VB_ERR_INVALID, "NULL val_bytes with n_val_bytes > 0");
+    if (n >= 0xFFFFFFFEull) return set_err(VB_ERR_TOO_LARGE, "map partition of %llu rows", (unsigned long long)n);
+    std::lock_guard<std::mutex> g(s->mu);
+    if (s->sealed || s->sealing || s->freed) return set_err(VB_ERR_STATE, "shuffle %llu: map after seal", (unsigned long long)s->id);
+    return VB_OK;
+}
+
+// One map task's values: the checked offsets rebased to 0 and the bytes, copied into *st, and the task's references
+// ((map_id + 1) << 32 | row) in refs.  The caller's buffers are free again when it returns.
+static int bytes_store(vb_shuf *s, u32 map_id, const u64 *val_offsets, const void *val_bytes, u64 n_val_bytes, u64 n, int loc,
+                       ByteSrc *st, DevBuf &refs)
+{
+    *st = ByteSrc{nullptr, nullptr, 0};
+    if (n == 0) return VB_OK;
+    vb_ctx *c = s->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    const int in = loc == VB_HOST ? VB_HOST : VB_DEVICE;
+    u64 first = 0, last = 0;
+    const int rc = str_check_offsets(s, val_offsets, n, n_val_bytes, in, &first, &last);
+    if (rc == VB_ERR_INVALID) return set_err(rc, "value offsets decrease or exceed n_val_bytes %llu", (unsigned long long)n_val_bytes);
+    if (rc == VB_ERR_TOO_LARGE) return set_err(rc, "a value of 2^32 bytes or more");
+    TRY(rc);
+    const cudaMemcpyKind kind = in == VB_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
+    DevBuf offs(c), bytes(c), staged(c);
+    TRY(offs.alloc((n + 1) * 8));
+    TRY(bytes.alloc(last - first));
+    TRY(refs.alloc(n * 8));
+    const u64 *src_offs = val_offsets;
+    if (in == VB_HOST) {
+        TRY(staged.alloc((n + 1) * 8));
+        CU(cudaMemcpyAsync(staged.p, val_offsets, (n + 1) * 8, kind, c->stream));
+        s->st.h2d_bytes += (n + 1) * 8 + (last - first);
+        src_offs = staged.as<u64>();
+    }
+    if (last > first) CU(cudaMemcpyAsync(bytes.p, (const unsigned char *)val_bytes + first, last - first, kind, c->stream));
+    {
+        KLaunch kl(s, K_MISC, n);
+        rebase_kernel<<<(unsigned)((n + 256) / 256), 256, 0, c->stream>>>(src_offs, n + 1, first, offs.as<u64>());   // one thread per offset
+        TRY(kl.done("rebase_kernel"));
+    }
+    {
+        KLaunch kl(s, K_MISC, n);
+        const unsigned blocks = (unsigned)std::min<u64>((n + 255) / 256, (u64)c->sm_count * 8);
+        bytes_refs_kernel<<<blocks, 256, 0, c->stream>>>((u64)(map_id + 1) << 32, n, refs.as<u64>());
+        TRY(kl.done("bytes_refs_kernel"));
+    }
+    CU(cudaStreamSynchronize(c->stream));
+    *st = ByteSrc{(const u64 *)offs.release(), (const unsigned char *)bytes.release(), n};
+    return VB_OK;
+}
+
+// After the map call: on success the new store replaces the map id's old one, otherwise it is dropped
+static int bytes_keep(vb_shuf *s, u32 map_id, const ByteSrc &st, int rc)
+{
+    vb_ctx *c = s->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    cudaSetDevice(c->device);
+    const ByteSrc &drop = rc == VB_OK ? s->bvals[map_id] : st;
+    dev_free(c, drop.offs);
+    dev_free(c, drop.bytes);
+    if (rc == VB_OK) s->bvals[map_id] = st;
+    return rc;
+}
+
+extern "C" int32_t vb_shuffle_map_bytes(vb_shuf *s, uint32_t map_id, const void *keys, const uint64_t *val_offsets, const void *val_bytes,
+                                        uint64_t n_val_bytes, uint64_t n, int32_t loc)
+{
+    if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
+    if (s->vdt != VB_BYTES || s->str || s->bvals.size() != s->n_map)
+        return set_err(VB_ERR_INVALID, "vb_shuffle_map_bytes needs an integer-key shuffle of VB_BYTES values");
+    if (n && !keys) return set_err(VB_ERR_INVALID, "NULL keys with n_rows > 0");
+    TRY(bytes_check_args(s, map_id, val_offsets, val_bytes, n_val_bytes, n, loc));
+    ByteSrc st;
+    DevBuf refs(s->ctx);
+    TRY(bytes_store(s, map_id, val_offsets, val_bytes, n_val_bytes, n, loc, &st, refs));
+    return bytes_keep(s, map_id, st, shuffle_map(s, map_id, nullptr, (const u64 *)keys, nullptr, n, loc, false, nullptr, &refs));
+}
+
+extern "C" int32_t vb_shuffle_map_str_bytes(vb_shuf *s, uint32_t map_id, const uint64_t *key_offsets, const void *key_bytes, uint64_t n_key_bytes,
+                                            const uint64_t *val_offsets, const void *val_bytes, uint64_t n_val_bytes, uint64_t n, int32_t loc)
+{
+    if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
+    if (s->vdt != VB_BYTES || !s->str || s->multi || s->bvals.size() != s->n_map)
+        return set_err(VB_ERR_INVALID, "vb_shuffle_map_str_bytes needs a string-key shuffle of VB_BYTES values");
+    if (n && !key_offsets) return set_err(VB_ERR_INVALID, "NULL key_offsets with n_rows > 0");
+    if (n && n_key_bytes && !key_bytes) return set_err(VB_ERR_INVALID, "NULL key_bytes with n_key_bytes > 0");
+    TRY(bytes_check_args(s, map_id, val_offsets, val_bytes, n_val_bytes, n, loc));
+    ByteSrc st;
+    DevBuf refs(s->ctx);
+    TRY(bytes_store(s, map_id, val_offsets, val_bytes, n_val_bytes, n, loc, &st, refs));
+    const u64 *none = nullptr;   // the value column is the references (refs), not a caller column
+    return bytes_keep(s, map_id, st, str_map(s, map_id, key_offsets, key_bytes, n_key_bytes, &none, 1, n, loc, &refs));
+}
+
+// Lengths of n references (copied to the device first when on the host) into lens, and their exclusive scan into
+// offs [n + 1]; VB_ERR_INVALID, with offs untouched, when one of them was not issued by s.  Caller holds c->mu.
+static int bytes_offsets(vb_shuf *s, const u64 *refs_in, u64 n, int src_loc, DevBuf &refs, u64 *offs, u64 *total)
+{
+    vb_ctx *c = s->ctx;
+    *total = 0;
+    if (!s->bvals_dev) {
+        DevBuf t(c);
+        TRY(t.alloc(s->bvals.size() * sizeof(ByteSrc)));
+        CU(cudaMemcpyAsync(t.p, s->bvals.data(), s->bvals.size() * sizeof(ByteSrc), cudaMemcpyHostToDevice, c->stream));
+        CU(cudaStreamSynchronize(c->stream));   // pageable source
+        s->bvals_dev = t.as<ByteSrc>();
+        t.release();
+    }
+    if (n == 0) { CU(cudaMemsetAsync(offs, 0, 8, c->stream)); return VB_OK; }
+    const u64 *r = refs_in;
+    if (src_loc == VB_HOST) {
+        TRY(refs.alloc(n * 8));
+        CU(cudaMemcpyAsync(refs.p, refs_in, n * 8, cudaMemcpyHostToDevice, c->stream));
+        s->st.h2d_bytes += n * 8;
+        r = refs.as<u64>();
+    }
+    DevBuf lens(c), bad(c);
+    TRY(lens.alloc(n * 8));
+    TRY(bad.alloc(4));
+    CU(cudaMemsetAsync(bad.p, 0, 4, c->stream));
+    {
+        KLaunch kl(s, K_MISC, n);
+        const unsigned blocks = (unsigned)std::min<u64>((n + 255) / 256, (u64)c->sm_count * 8);
+        bytes_len_kernel<<<blocks, 256, 0, c->stream>>>(r, n, s->bvals_dev, (u32)s->bvals.size(), lens.as<u64>(), bad.as<u32>());
+        TRY(kl.done("bytes_len_kernel"));
+    }
+    u32 h_bad = 0;
+    TRY(fetch_status_unlocked(c, bad.p, &h_bad, 4));
+    if (h_bad) return set_err(VB_ERR_INVALID, "shuffle %llu: a reference it did not issue", (unsigned long long)s->id);
+    TRY(exclusive_scan_u64(s, lens.as<u64>(), offs, n, offs + n));
+    return fetch_status_unlocked(c, offs + n, total, 8);
+}
+
+static int bytes_gather_check(vb_shuf *s, const void *refs, u64 n, int src_loc)
+{
+    if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
+    if (s->vdt != VB_BYTES || s->bvals.size() != s->n_map) return set_err(VB_ERR_INVALID, "shuffle %llu has no byte-string values", (unsigned long long)s->id);
+    if (n && !refs) return set_err(VB_ERR_INVALID, "NULL refs with n > 0");
+    if (src_loc < VB_HOST || src_loc > VB_DEVICE_BORROWED) return set_err(VB_ERR_INVALID, "bad src_loc %d", src_loc);
+    return wait_sealed(s);
+}
+
+extern "C" int32_t vb_shuffle_gather_bytes_size(vb_shuf *s, const uint64_t *refs, uint64_t n, int32_t src_loc, uint64_t *n_bytes)
+{
+    if (!n_bytes) return set_err(VB_ERR_INVALID, "NULL n_bytes");
+    TRY(bytes_gather_check(s, refs, n, src_loc));
+    vb_ctx *c = s->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    DevBuf r(c), offs(c);
+    TRY(offs.alloc((n + 1) * 8));
+    u64 total = 0;
+    TRY(bytes_offsets(s, refs, n, src_loc, r, offs.as<u64>(), &total));
+    *n_bytes = total;
+    return VB_OK;
+}
+
+extern "C" int32_t vb_shuffle_gather_bytes(vb_shuf *s, const uint64_t *refs, uint64_t n, int32_t src_loc, uint64_t *out_offsets,
+                                           void *out_bytes, int32_t dst_loc)
+{
+    if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
+    if (!out_offsets) return set_err(VB_ERR_INVALID, "NULL out_offsets");
+    TRY(bytes_gather_check(s, refs, n, src_loc));
+    vb_ctx *c = s->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    DevBuf r(c), offs_tmp(c), bytes_tmp(c);
+    // the offsets go straight to a device caller only when nothing can fail after them: with out_bytes NULL the
+    // total decides whether the call is valid, so they are scanned into a buffer of the library first
+    u64 *offs = out_offsets;
+    const bool staged = dst_loc == VB_HOST || !out_bytes;
+    if (staged) { TRY(offs_tmp.alloc((n + 1) * 8)); offs = offs_tmp.as<u64>(); }
+    u64 total = 0;
+    TRY(bytes_offsets(s, refs, n, src_loc, r, offs, &total));
+    if (total && !out_bytes) return set_err(VB_ERR_INVALID, "NULL out_bytes for %llu bytes", (unsigned long long)total);
+    unsigned char *dst = (unsigned char *)out_bytes;
+    if (total && dst_loc == VB_HOST) { TRY(bytes_tmp.alloc(total)); dst = bytes_tmp.as<unsigned char>(); }
+    if (total) {
+        const u64 tiles = (n + total + GB_ITEMS - 1) / GB_ITEMS;
+        const u64 grid = std::min<u64>(tiles, (u64)c->sm_count * occupancy(c, bytes_gather_kernel, GB_THREADS, 0));
+        const u64 *rd = src_loc == VB_HOST ? r.as<u64>() : refs;
+        KLaunch kl(s, K_MISC, n);
+        bytes_gather_kernel<<<(unsigned)grid, GB_THREADS, 0, c->stream>>>(rd, n, offs, total, s->bvals_dev, (u32)s->bvals.size(), dst);
+        TRY(kl.done("bytes_gather_kernel"));
+    }
+    if (staged) {
+        TRY(copy_out(s, out_offsets, offs, (n + 1) * 8, dst_loc));
+    }
+    if (dst_loc == VB_HOST) {
+        TRY(copy_out(s, out_bytes, dst, total, VB_HOST));
+    }
+    CU(cudaStreamSynchronize(c->stream));
+    return VB_OK;
 }
 
 template <int OPK, int TX>
@@ -5451,6 +5704,7 @@ extern "C" int32_t vb_shuffle_create_str_dist(vb_ctx *c, uint64_t shuffle_id, ui
 {
     if (!c || !out) return set_err(VB_ERR_INVALID, "vb_shuffle_create_str_dist: NULL argument");
     *out = nullptr;
+    if (vdt == VB_BYTES) return set_err(VB_ERR_UNSUPPORTED, "vb_shuffle_create_str_dist: byte-string values do not cross ranks yet");
     if (world < 1 || world > 256 || rank >= world) return set_err(VB_ERR_INVALID, "bad rank %u / world %u (1 <= world <= 256)", rank, world);
     TRY(vb_shuffle_create_str(c, shuffle_id, n_map, n_reduce, vdt, agg, out));
     (*out)->rank = rank;
@@ -5469,6 +5723,7 @@ static int str_dist_check(const vb_shuf *s, const char *what)
 
 extern "C" int32_t vb_shuffle_export_str_prepare(vb_shuf *s, uint64_t *n_keys, uint64_t *n_key_bytes, uint64_t *n_vals)
 {
+    if (s && s->vdt == VB_BYTES) return reject_bytes(s, "vb_shuffle_export_str_prepare");
     if (!s || !n_keys || !n_key_bytes || !n_vals) return set_err(VB_ERR_INVALID, "NULL argument");
     TRY(str_dist_check(s, "vb_shuffle_export_str_prepare"));
     vb_ctx *c = s->ctx;
@@ -5481,6 +5736,7 @@ extern "C" int32_t vb_shuffle_export_str_prepare(vb_shuf *s, uint64_t *n_keys, u
 
 extern "C" int32_t vb_shuffle_export_str_buffers(vb_shuf *s, uint32_t **key_lens, void **key_bytes, uint32_t **val_counts, uint64_t **vals)
 {
+    if (s && s->vdt == VB_BYTES) return reject_bytes(s, "vb_shuffle_export_str_buffers");
     if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
     TRY(str_dist_check(s, "vb_shuffle_export_str_buffers"));
     {
@@ -5527,6 +5783,7 @@ static int str_import(vb_shuf *s, const char *what, const char *prepare, const u
 extern "C" int32_t vb_shuffle_import_str(vb_shuf *s, const uint32_t *key_lens, const void *key_bytes, const uint32_t *val_counts,
                                          const uint64_t *vals, const uint64_t *n_keys, const uint64_t *n_key_bytes, const uint64_t *n_vals)
 {
+    if (s && s->vdt == VB_BYTES) return reject_bytes(s, "vb_shuffle_import_str");
     if (!s || !n_keys || !n_key_bytes || !n_vals) return set_err(VB_ERR_INVALID, "NULL argument");
     TRY(str_dist_check(s, "vb_shuffle_import_str"));
     u64 nk = 0, nkb = 0, nv = 0;
@@ -5595,6 +5852,7 @@ extern "C" int32_t vb_shuffle_create_str_sort_dist(vb_ctx *c, uint64_t shuffle_i
 {
     if (!c || !out) return set_err(VB_ERR_INVALID, "vb_shuffle_create_str_sort_dist: NULL argument");
     *out = nullptr;
+    if (val_dtype == VB_BYTES) return set_err(VB_ERR_UNSUPPORTED, "vb_shuffle_create_str_sort_dist: byte-string values do not cross ranks yet");
     if (world < 1 || world > 256 || rank >= world) return set_err(VB_ERR_INVALID, "bad rank %u / world %u (1 <= world <= 256)", rank, world);
     TRY(vb_shuffle_create_str_sort(c, shuffle_id, n_map, n_reduce, val_dtype, out));
     (*out)->rank = rank;
@@ -6359,6 +6617,8 @@ extern "C" int32_t vb_shuffle_free(vb_shuf *s)
         for (auto &kv : s->n_plans) free_cogroup_n_plan(c, kv.second);
         free_lazy_rows(s);
         free_str(s);
+        for (ByteSrc &b : s->bvals) { dev_free(c, b.offs); dev_free(c, b.bytes); }
+        dev_free(c, s->bvals_dev);
         cudaStreamSynchronize(c->stream);
     }
     for (auto &kv : s->filtered) { vb_shuffle_free(kv.second.first); vb_shuffle_free(kv.second.second); }

@@ -235,6 +235,8 @@ def run_shuffle(engine, local_maps, n_map, n_reduce, kcode, vcode, agg, rank, wo
     exchange_device: move the packed buffers there for the collective (tests: "cpu" + gloo on a 1-GPU box).
     p2p: GROUP/COGROUP shuffles use the fused partition+send over peer memory instead of pack + all-to-all-v.
     """
+    if vcode == L.VB_BYTES:
+        raise TypeError("byte-string values do not cross ranks yet")
     sh = engine.create(n_map, n_reduce, kcode, vcode, agg, rank, world, key_width=key_width, hint=hint)
     for map_id, keys, vals in local_maps:
         engine.map(sh, map_id, keys, vals)
@@ -291,6 +293,8 @@ def run_str_shuffle(engine, local_maps, n_map, n_reduce, vcode, agg, rank, world
     With a communicator on the context the exchange is vb_shuffle_exchange (NCCL inside the library); otherwise
     all_to_all_v of the four columns (exchange_device: "cpu" for a gloo group on a one-GPU box).  agg VB_AGG_SORT
     (sort_by_key) across ranks has no such fallback: its cut keys are agreed in rounds of the library's collectives."""
+    if vcode == L.VB_BYTES:
+        raise TypeError("byte-string values do not cross ranks yet")
     if agg == L.VB_AGG_SORT and world > 1 and not (isinstance(engine, StrCudaEngine) and getattr(engine.sc, "comm", None)
                                                    and exchange_device is None):
         raise ValueError("sort_by_key over String keys across ranks needs the library's communicator (vb_ctx_comm_init, "

@@ -10,6 +10,11 @@ Differences forced by the boundary (SURVEY.md F4): rows are 64-bit POD (K,V) arr
 sequence of Python `str` or a `StrKeys` column (offsets + UTF-8 bytes), for reduce_by_key / count_by_key /
 group_by_key / partition_by_key / combine_by_key / count_by_value / distinct; they are placed as the reference places
 `String` keys.  sort_by_key / sort over them go through StrSortedRdd, which orders the keys by their bytes on the device.
+Values may be byte strings (a sequence of str or bytes, or a StrKeys column) for the ops that move values without
+reading them: group_by_key / partition_by_key / join / the outer joins / cogroup / CoGroupedRdd / sort_by_key, and over
+String keys StrPairRdd.group_by_key / partition_by_key, StrCoGroupedRdd and StrSortedRdd.  They travel through the
+shuffle as references and are gathered back into bytes on the device; they come back as numpy object arrays of str (or
+bytes, as given), with None for the missing side of an outer join.
 
 All compute happens in libvega_b200.so; this module slices the input exactly like
 ParallelCollection::slice, drives map tasks → seal → reduce tasks like the scheduler does
@@ -25,7 +30,7 @@ from . import _lib as L
 
 _AGG = {"group": L.VB_AGG_GROUP, "sum": L.VB_AGG_SUM, "min": L.VB_AGG_MIN, "max": L.VB_AGG_MAX,
         "count": L.VB_AGG_COUNT, "cogroup": L.VB_AGG_COGROUP, "sort": L.VB_AGG_SORT}
-_NP_OF = {L.VB_U64: np.uint64, L.VB_I64: np.int64, L.VB_F64: np.float64}
+_NP_OF = {L.VB_U64: np.uint64, L.VB_I64: np.int64, L.VB_F64: np.float64, L.VB_BYTES: np.uint64}   # VB_BYTES: references
 _COMBINE_OPS = {"sum": L.VB_AGG_SUM, "min": L.VB_AGG_MIN, "max": L.VB_AGG_MAX, "count": L.VB_AGG_COUNT, "mean": L.VB_AGG_MEAN}
 
 
@@ -144,9 +149,16 @@ class Context:
 
     def parallelize(self, data, num_slices, values=None):
         """`sc.parallelize(vec, num_slices)`.  data: 1-D keys (→ Rdd), (n,2) rows or
-        (keys, values) (→ PairRdd).  values may also be a tuple of up to 4 value columns (combine_by_key).
+        (keys, values) (→ PairRdd).  values may also be a tuple of up to 4 value columns (combine_by_key), or byte-string
+        values: a sequence or numpy array of str (returned as str), a sequence of bytes (returned as bytes) or a StrKeys
+        column on the host or as CUDA tensors (returned as str).
         String keys (a sequence of str, a numpy str array or a StrKeys column) give a StrRdd / StrPairRdd; a tuple of
         value columns gives a StrPairRdd with value columns, the one kind whose combine_by_key runs."""
+        if _is_bytes_vals(values):
+            vals = _BytesCol(values)
+            if _is_str_keys(data):
+                return StrPairRdd(self, _StrCol(data), vals, num_slices)
+            return PairRdd(self, _Col(data), vals, num_slices)
         if _is_str_keys(data):
             keys = _StrCol(data)
             if values is None:
@@ -341,6 +353,12 @@ class Shuffle:
         n = stop - start
         if keys.loc == L.VB_DEVICE_BORROWED:
             self._keepalive.append((keys.owner, vals.owner if vals is not None else None))
+        if isinstance(vals, _BytesCol):
+            vals.check_loc(keys.loc)
+            self.as_str = vals.as_str
+            L.check(self._lib.vb_shuffle_map_bytes(self._h, map_id, keys.at(start), vals.offs_at(start), vals.data_at(), vals.n_bytes,
+                                                   n, keys.loc))
+            return
         if keys.rows:
             L.check(self._lib.vb_shuffle_map_aos(self._h, map_id, keys.at(start), n, keys.loc))
         else:
@@ -393,6 +411,25 @@ class Shuffle:
         L.check(self._lib.vb_shuffle_reduce_size(self._h, r, ctypes.byref(nk), ctypes.byref(nv)))
         return nk.value, nv.value
 
+    def gather(self, refs, valid=None):
+        """Byte-string values: the references refs (read from this shuffle's output) gathered into an object array of
+        str or bytes, None where valid (one byte per row) is 0."""
+        refs = np.ascontiguousarray(refs, dtype=np.uint64)
+        n, nb = len(refs), ctypes.c_uint64()
+        p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
+        L.check(self._lib.vb_shuffle_gather_bytes_size(self._h, p(refs), n, L.VB_HOST, ctypes.byref(nb)))
+        offs, data = np.empty(n + 1, dtype=np.uint64), np.empty(nb.value, dtype=np.uint8)
+        L.check(self._lib.vb_shuffle_gather_bytes(self._h, p(refs), n, L.VB_HOST, p(offs), p(data), L.VB_HOST))
+        raw, o = data.tobytes(), offs.astype(np.int64).tolist()
+        out = np.empty(n, dtype=object)
+        if getattr(self, "as_str", True):
+            out[:] = [raw[o[i]:o[i + 1]].decode("utf-8", "surrogateescape") for i in range(n)]
+        else:
+            out[:] = [raw[o[i]:o[i + 1]] for i in range(n)]
+        if valid is not None:
+            out[np.asarray(valid) == 0] = None
+        return out
+
     def reduce(self, r):
         """ShuffledRdd::compute(split r) → host arrays."""
         nk, nv = self.reduce_size(r)
@@ -402,14 +439,14 @@ class Shuffle:
             offs = np.empty(nk + 1, dtype=np.uint64)
             vals = np.empty(nv, dtype=_NP_OF[self.vcode])
             L.check(self._lib.vb_shuffle_reduce(self._h, r, p(keys), None, p(offs), p(vals), L.VB_HOST))
-            return keys, offs, vals
+            return keys, offs, _vals_out(self, vals)
         if self.agg == L.VB_AGG_SORT and not self.has_payload:
             L.check(self._lib.vb_shuffle_reduce(self._h, r, p(keys), None, None, None, L.VB_HOST))
             return keys, None
         out_dt = np.uint64 if self.agg == L.VB_AGG_COUNT else _NP_OF[self.vcode]
         comb = np.empty(nk, dtype=out_dt)
         L.check(self._lib.vb_shuffle_reduce(self._h, r, p(keys), p(comb), None, None, L.VB_HOST))
-        return keys, comb
+        return keys, _vals_out(self, comb)
 
     def reduce_device(self, r, out_keys=None, out_comb=None, out_offs=None, out_vals=None):
         """Same, into caller-provided torch CUDA tensors (any may be None)."""
@@ -479,6 +516,21 @@ class _Base:
 
 
 _REDUCE_AGGS = ("sum", "min", "max", "count")
+
+
+def _vals_out(sh, v, valid=None):
+    """One side's values as returned to the caller: numeric values as they are (a numpy.ma.MaskedArray where validity is
+    given), byte-string values gathered from the side's shuffle into an object array (None where validity is 0)."""
+    if sh.vcode == L.VB_BYTES:
+        return sh.gather(v, valid)
+    return v if valid is None else np.ma.MaskedArray(v, mask=valid == 0)
+
+
+def _refuse_bytes(parent, what):
+    """TypeError, before any device work, for an op that computes on byte-string values."""
+    if isinstance(getattr(parent, "vals", None), _BytesCol):
+        raise TypeError(f"{what} computes on values: byte-string values support group_by_key, partition_by_key, the "
+                        "joins, cogroup and sort_by_key")
 _CODE_OF = {np.uint64: L.VB_U64, np.int64: L.VB_I64, np.float64: L.VB_F64}
 
 
@@ -550,6 +602,8 @@ class ShuffledRdd(_AggregatedParent):
             raise ValueError("num_splits must be >= 1")
         if len(getattr(parent, "cols", ())) > 1:
             raise TypeError("a PairRdd with several value columns supports combine_by_key only")
+        if agg_name in _REDUCE_AGGS:
+            _refuse_bytes(parent, "reduce_by_key / count_by_key")
         self.parent, self.agg_name, self.num_slices, self.hint = parent, agg_name, num_splits, hint
         self.sc = parent.sc
         self._sh = None
@@ -662,15 +716,11 @@ class JoinedRdd(_Base):
         w = np.empty(n.value, dtype=_NP_OF[b.vcode])
         if self.kind is None:
             L.check(lib.vb_join(a._h, b._h, split, p(k), p(v), p(w), L.VB_HOST))
-            return k, v, w
+            return k, _vals_out(a, v), _vals_out(b, w)
         vv = np.empty(n.value, dtype=np.uint8) if self.kind != "left" else None     # validity of the side that can be None
         wv = np.empty(n.value, dtype=np.uint8) if self.kind != "right" else None
         L.check(lib.vb_join_outer(a._h, b._h, split, kind, p(k), p(v), p(w), p(vv), p(wv), L.VB_HOST))
-        if vv is not None:
-            v = np.ma.MaskedArray(v, mask=vv == 0)
-        if wv is not None:
-            w = np.ma.MaskedArray(w, mask=wv == 0)
-        return k, v, w
+        return k, _vals_out(a, v, vv), _vals_out(b, w, wv)
 
     def collect(self):
         parts = [self.compute(r) for r in range(self.num_slices)]
@@ -691,7 +741,7 @@ class JoinedRdd(_Base):
         lv, rv = np.empty(nl.value, dtype=_NP_OF[a.vcode]), np.empty(nr.value, dtype=_NP_OF[b.vcode])
         p = lambda x: x.ctypes.data_as(ctypes.c_void_p)
         L.check(lib.vb_cogroup(a._h, b._h, split, p(keys), p(lo), p(lv), p(ro), p(rv), L.VB_HOST))
-        return keys, (lo, lv), (ro, rv)
+        return keys, (lo, _vals_out(a, lv)), (ro, _vals_out(b, rv))
 
     def cogroup_collect(self):
         """cogroup(): per partition, the union of keys with both value lists (co_grouped_rdd.rs:206-249), as a list
@@ -762,7 +812,7 @@ class CoGroupedRdd(_Base):
         vals = [np.empty(nv[j], dtype=_NP_OF[s.vcode]) for j, s in enumerate(shs)]
         ptrs = lambda xs: (ctypes.c_void_p * n)(*[x.ctypes.data for x in xs])
         L.check(lib.vb_cogroup_n(sides, n, split, keys.ctypes.data_as(ctypes.c_void_p), ptrs(offs), ptrs(vals), L.VB_HOST))
-        return keys, list(zip(offs, vals))
+        return keys, list(zip(offs, [_vals_out(s, v) for s, v in zip(shs, vals)]))
 
     def collect(self):
         out = []
@@ -782,7 +832,7 @@ class CoGroupedRdd(_Base):
         vs = [np.empty(nn.value, dtype=_NP_OF[s.vcode]) for s in shs]
         L.check(lib.vb_join_n(sides, n, split, k.ctypes.data_as(ctypes.c_void_p),
                               (ctypes.c_void_p * n)(*[v.ctypes.data for v in vs]), L.VB_HOST))
-        return k, vs
+        return k, [_vals_out(s, v) for s, v in zip(shs, vs)]
 
     def join_collect(self):
         parts = [self.join_compute(r) for r in range(self.num_slices)]
@@ -828,7 +878,7 @@ class CoGroupedRdd(_Base):
         ptrs = lambda xs: (ctypes.c_void_p * n)(*[x.ctypes.data if x is not None else None for x in xs])
         L.check(lib.vb_join_n_outer(sides, n, split, mask, k.ctypes.data_as(ctypes.c_void_p), ptrs(vs), ptrs(valid),
                                     L.VB_HOST))
-        return k, [v if ok is None else np.ma.MaskedArray(v, mask=ok == 0) for v, ok in zip(vs, valid)]
+        return k, [_vals_out(s, v, ok) for s, v, ok in zip(shs, vs, valid)]
 
     def outer_join_collect(self, required):
         mask = self._required_mask(required)
@@ -949,6 +999,7 @@ class PairRdd(_Base):
         {"n": ("count", None), "avg": ("mean", 0), "hi": ("max", 1)}."""
         if not self.cols:
             raise ValueError("combine_by_key needs value columns")
+        _refuse_bytes(self, "combine_by_key")
         if self.keys.rows:
             raise ValueError("combine_by_key takes keys and value columns, not (n,2) rows")
         return CombinedRdd(self, aggs, num_splits, hint)
@@ -1187,6 +1238,66 @@ def _decode_keys(offsets, data):
     return out
 
 
+def _is_bytes_vals(x):
+    """True for byte-string values: a StrKeys column, or a non-empty sequence / numpy array of str or bytes."""
+    if isinstance(x, StrKeys):
+        return True
+    if isinstance(x, np.ndarray):
+        if x.dtype.kind in "US":
+            return x.ndim == 1
+        if x.dtype.kind != "O" or x.size == 0:
+            return False
+        first = x.flat[0]
+    elif isinstance(x, (list, tuple)) and len(x) > 0:
+        first = x[0]
+    else:
+        return False
+    return isinstance(first, (str, bytes, bytearray))
+
+
+class _BytesCol:
+    """A column of byte-string values at the C ABI (vb_shuffle_map_bytes / vb_shuffle_map_str_bytes): Arrow-style
+    offsets + bytes, on the host or as CUDA tensors.  str values (and a StrKeys column) come back as str, bytes as bytes."""
+
+    def __init__(self, x):
+        self.as_str = True
+        if isinstance(x, StrKeys):
+            k = x
+        else:
+            items = x.tolist() if isinstance(x, np.ndarray) else list(x)
+            if all(isinstance(v, str) for v in items):
+                k = StrKeys.from_strs(items)
+            elif all(isinstance(v, (bytes, bytearray)) for v in items):
+                self.as_str = False
+                offsets = np.zeros(len(items) + 1, dtype=np.uint64)
+                np.cumsum(np.fromiter((len(b) for b in items), dtype=np.uint64, count=len(items)), out=offsets[1:])
+                k = StrKeys(offsets, np.frombuffer(b"".join(bytes(b) for b in items), dtype=np.uint8))
+            else:
+                raise TypeError("byte-string values must be all str or all bytes")
+        if _is_torch(k.offsets):
+            import torch
+            torch.cuda.current_stream(k.offsets.device).synchronize()
+            self.loc = L.VB_DEVICE
+            self.offs_ptr, self.data_ptr = k.offsets.data_ptr(), k.data.data_ptr()
+        else:
+            self.loc = L.VB_HOST
+            self.offs_ptr, self.data_ptr = k.offsets.ctypes.data, k.data.ctypes.data
+        self.n_bytes = k.data.shape[0]
+        self.n = len(k)
+        self.owner = k
+        self.code = L.VB_BYTES
+
+    def check_loc(self, key_loc):
+        if (key_loc == L.VB_HOST) != (self.loc == L.VB_HOST):
+            raise ValueError("keys and values must live in the same memory space")
+
+    def offs_at(self, start):
+        return ctypes.c_void_p(self.offs_ptr + 8 * start)
+
+    def data_at(self):
+        return ctypes.c_void_p(self.data_ptr) if self.n_bytes else None
+
+
 class _StrCol:
     """A string key column at the C ABI: offsets / bytes pointers, their location and the row count."""
 
@@ -1236,7 +1347,9 @@ class StrShuffle(Shuffle):
         if sort:
             self.agg, self.has_payload = L.VB_AGG_SORT, vcode is not None
             vdt = -1 if vcode is None else vcode
-            if world > 1:
+            if vcode == L.VB_BYTES and world == 1:        # a byte-string payload
+                L.check(self._lib.vb_shuffle_create_str_sort_bytes(sc._h, sc.new_shuffle_id(), n_map, n_reduce, ctypes.byref(h)))
+            elif world > 1:
                 L.check(self._lib.vb_shuffle_create_str_sort_dist(sc._h, sc.new_shuffle_id(), n_map, n_reduce, vdt, rank, world,
                                                                   ctypes.byref(h)))
             else:
@@ -1319,12 +1432,19 @@ class StrShuffle(Shuffle):
 
     def map(self, map_id, keys, vals, start, stop):
         """Rows [start, stop) of the string key column (and of the values) as map partition map_id."""
-        if vals is not None and vals.loc != keys.loc:
+        if isinstance(vals, _BytesCol):
+            vals.check_loc(keys.loc)
+        elif vals is not None and vals.loc != keys.loc:
             raise ValueError("keys and values must live in the same memory space")
         if keys.loc == L.VB_DEVICE_BORROWED:
             self._keepalive.append((keys.owner, vals.owner if vals is not None else None))
         offs = ctypes.c_void_p(keys.offs_ptr + 8 * start)
         data = ctypes.c_void_p(keys.data_ptr) if keys.n_bytes else None
+        if isinstance(vals, _BytesCol):
+            self.as_str = vals.as_str
+            L.check(self._lib.vb_shuffle_map_str_bytes(self._h, map_id, offs, data, keys.n_bytes, vals.offs_at(start), vals.data_at(),
+                                                       vals.n_bytes, stop - start, keys.loc))
+            return
         L.check(self._lib.vb_shuffle_map_str(self._h, map_id, offs, data, keys.n_bytes,
                                              vals.at(start) if vals is not None else None, stop - start, keys.loc))
 
@@ -1343,11 +1463,11 @@ class StrShuffle(Shuffle):
             vals = np.empty(nk, dtype=_NP_OF[self.vcode]) if self.has_payload else None
             L.check(self._lib.vb_shuffle_reduce_str(self._h, r, p(ko), p(kb), p(vals) if vals is not None else None, None, None,
                                                     L.VB_HOST))
-            return ko, kb, vals
+            return ko, kb, vals if vals is None else _vals_out(self, vals)
         if self.agg == L.VB_AGG_GROUP:
             offs, vals = np.empty(nk + 1, dtype=np.uint64), np.empty(nv, dtype=_NP_OF[self.vcode])
             L.check(self._lib.vb_shuffle_reduce_str(self._h, r, p(ko), p(kb), None, p(offs), p(vals), L.VB_HOST))
-            return ko, kb, offs, vals
+            return ko, kb, offs, _vals_out(self, vals)
         comb = np.empty(nk, dtype=np.uint64 if self.agg == L.VB_AGG_COUNT else _NP_OF[self.vcode])
         L.check(self._lib.vb_shuffle_reduce_str(self._h, r, p(ko), p(kb), p(comb), None, None, L.VB_HOST))
         return ko, kb, comb
@@ -1452,6 +1572,8 @@ class StrShuffledRdd(ShuffledRdd):
             raise ValueError("num_splits must be >= 1")
         if len(getattr(parent, "cols", ())) > 1:
             raise TypeError("a PairRdd with several value columns supports combine_by_key only")
+        if agg_name in _REDUCE_AGGS:
+            _refuse_bytes(parent, "reduce_by_key / count_by_key")
         self.parent, self.agg_name, self.num_slices, self.hint = parent, agg_name, num_splits, hint
         self.sc = parent.sc
         self._sh = None
@@ -1668,7 +1790,7 @@ class StrCoGroupedRdd(_Base):
         ptrs = lambda xs: (ctypes.c_void_p * n)(*[x.ctypes.data for x in xs])
         L.check(lib.vb_cogroup_n_str(sides, n, split, ko.ctypes.data_as(ctypes.c_void_p), kb.ctypes.data_as(ctypes.c_void_p),
                                      ptrs(offs), ptrs(vals), L.VB_HOST))
-        return ko, kb, list(zip(offs, vals))
+        return ko, kb, list(zip(offs, [_vals_out(s, v) for s, v in zip(shs, vals)]))
 
     def compute(self, split):
         ko, kb, lists = self.compute_raw(split)
@@ -1697,6 +1819,7 @@ class StrCoGroupedRdd(_Base):
         ptrs = lambda xs: (ctypes.c_void_p * n)(*[x.ctypes.data if x is not None else None for x in xs])
         p = lambda x: x.ctypes.data_as(ctypes.c_void_p)
         L.check(lib.vb_join_n_str(sides, n, split, mask, p(ko), p(kb), p(ro), ptrs(vs), ptrs(valid), L.VB_HOST))
+        vs = [v if s.vcode != L.VB_BYTES else s.gather(v, ok) for s, v, ok in zip(shs, vs, valid)]   # bytes: None where invalid
         return ko, kb, ro, vs, valid
 
     def outer_join_compute(self, split, required):
@@ -1705,7 +1828,7 @@ class StrCoGroupedRdd(_Base):
         ko, kb, ro, vs, valid = self.join_raw(split, required)
         keys = _decode_keys(ko, kb)
         k = np.repeat(keys, np.diff(ro.astype(np.int64))) if len(keys) else np.empty(0, dtype=object)
-        return k, [v if ok is None else np.ma.MaskedArray(v, mask=ok == 0) for v, ok in zip(vs, valid)]
+        return k, [v if ok is None or v.dtype == object else np.ma.MaskedArray(v, mask=ok == 0) for v, ok in zip(vs, valid)]
 
     def outer_join_collect(self, required):
         mask = self._required_mask(required)
@@ -1725,7 +1848,8 @@ class StrSortedRdd(_Base):
     """sort_by_key over `String` keys (PairRdd::sort_by_key, and Rdd::sort for a key-only parent) through
     vb_shuffle_create_str_sort: rows ascending by key in Rust `String` order (bytes compared unsigned, a proper prefix
     first), equal keys in input order, partitions contiguous key ranges cut as the integer sort cuts them.  parent: a
-    StrPairRdd of one value column (moved bit for bit), or a StrRdd (key-only).
+    StrPairRdd of one value column (moved bit for bit; byte-string values come back as str or bytes), or a StrRdd
+    (key-only).
       compute(r) -> (keys as a numpy object array of str, values), or the keys alone;  collect(): partitions in order
       compute_raw(r) -> (key offsets, key bytes, values or None), one key per row
       compute_device(r, out_key_offsets=, out_key_bytes=, out_vals=): into torch CUDA tensors sized from the shuffle's
