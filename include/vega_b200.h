@@ -684,7 +684,7 @@ VB_API int32_t vb_shuffle_create_str_sort_dist(vb_ctx *ctx, uint64_t shuffle_id,
  * VB_ERR_INVALID, as it always has).  Refused: with a reduce op or COUNT (VB_ERR_UNSUPPORTED); as a key dtype, in
  * vb_agg_col specs or _multi value columns (VB_ERR_INVALID); vb_shuffle_create_str_dist and
  * vb_shuffle_create_str_sort_dist with VB_BYTES, vb_shuffle_set_dist with world > 1, the export / import / exchange / P2P
- * calls and the blob calls (VB_ERR_UNSUPPORTED).
+ * calls and the blob calls (VB_ERR_UNSUPPORTED).  Across ranks: the _bytes_dist creates below.
  *   map     vb_shuffle_map_bytes (integer keys, read as by vb_shuffle_map_soa, VB_DEVICE_BORROWED included) and
  *           vb_shuffle_map_str_bytes (string keys, read as by vb_shuffle_map_str).  Value i is val_bytes[val_offsets[i] ..
  *           val_offsets[i + 1]) (Arrow-style: n_rows + 1 offsets that need not start at 0).  The values and their offsets
@@ -711,6 +711,68 @@ VB_API int32_t vb_shuffle_create_str_sort_bytes(vb_ctx *ctx, uint64_t shuffle_id
 VB_API int32_t vb_shuffle_gather_bytes_size(vb_shuf *s, const uint64_t *refs, uint64_t n, int32_t src_loc, uint64_t *n_bytes);
 VB_API int32_t vb_shuffle_gather_bytes(vb_shuf *s, const uint64_t *refs, uint64_t n, int32_t src_loc,
                                        uint64_t *out_offsets /*n+1, from 0*/, void *out_bytes, int32_t dst_loc);
+/* ---- byte-string values across ranks: each value's bytes are sent once, never its reference --------------------------
+ * vb_shuffle_create_bytes_dist        vb_shuffle_create(key_dtype, VB_BYTES, agg, part) for rank `rank` of `world`:
+ *                                     agg VB_AGG_GROUP / VB_AGG_COGROUP / VB_AGG_SORT (a reduce op or COUNT is
+ *                                     VB_ERR_UNSUPPORTED); vb_shuffle_set_key_width applies.
+ * vb_shuffle_create_str_bytes_dist    vb_shuffle_create_str(VB_BYTES, VB_AGG_GROUP) for rank `rank` of `world`; String
+ *                                     cogroup and the joins (vb_cogroup_n_str, vb_join_n_str) read such shuffles.
+ * vb_shuffle_create_str_sort_bytes_dist  vb_shuffle_create_str_sort_bytes for rank `rank` of `world`.
+ * 1 <= world <= 256 (VB_ERR_INVALID otherwise); world 1 is the one-process create.  Map with vb_shuffle_map_bytes /
+ * vb_shuffle_map_str_bytes, map ids in contiguous blocks by rank as for every multi-rank shuffle; rank r owns the
+ * partitions p with p % world == r.  The exchange, for GROUP and COGROUP, is the export / import pair below (any
+ * all-to-all-v moves the columns) or vb_shuffle_exchange; the sorts cross ranks through vb_shuffle_exchange only.
+ * vb_shuffle_exchange(VB_XCHG_AUTO or VB_XCHG_NCCL) runs the whole exchange with NCCL on the library's stream; it counts
+ * rows in stats as integer rows do (String GROUP: values).  VB_XCHG_P2P, vb_shuffle_set_dist with world > 1, the plain,
+ * _str and _cols export / import calls, vb_shuffle_export_counts / export_direct / import_arena and the blob calls return
+ * VB_ERR_UNSUPPORTED.
+ * Wire format: the kind's columns without the value references, plus two columns for the values:
+ *   val_lens   u32 [values]   each value's length in bytes, split by the kind's value counts (integer rows: counts)
+ *   val_bytes  u8  [bytes]    the values' bytes, concatenated in row order, split by n_val_bytes
+ * integer GROUP / COGROUP  keys (i64) [rows] by counts, then val_lens and val_bytes; the gathered count row is counts[W]
+ *                          and n_val_bytes[W].
+ * String GROUP             key_lens, key_bytes and val_counts as for vb_shuffle_export_str_*, then val_lens (by n_vals)
+ *                          and val_bytes; the gathered count row is n_keys, n_key_bytes, n_vals and n_val_bytes [W] each.
+ * sorts                    per output partition as their numeric forms, val_lens and val_bytes in place of the payload,
+ *                          with each partition's value bytes added to the gathered segment table.
+ * Receive side: the received bytes become one more value store of the shuffle, and the received rows get fresh
+ * references into it in receive order, so everything downstream (seal, cogroup, joins, gather) runs as on one process.
+ * The map stores are freed once the export has packed them: a reference read before the exchange is refused by the
+ * gather from then on (VB_ERR_INVALID).  Memory: during the exchange a rank holds its map stores, the packed copy of
+ * its values and what it receives, about three times its share of value bytes; afterwards only what it received.
+ *   vb_shuffle_export_bytes_prepare  finishes the local map side and packs it by destination rank; counts / n_val_bytes
+ *                                    [world] get the rows and value bytes that go to each rank.
+ *   vb_shuffle_export_bytes_buffers  the packed columns (library-owned device buffers, destination-major, valid until
+ *                                    seal).
+ *   vb_shuffle_import_bytes          the received columns, source-rank major, with what every source sent.  keys are
+ *                                    borrowed until seal; val_lens and val_bytes are read (and the bytes copied) during
+ *                                    the call.
+ *   vb_shuffle_export_str_bytes_prepare / _buffers / vb_shuffle_import_str_bytes: the same for String GROUP; the key
+ *                                    columns and val_counts are borrowed until seal.
+ * Errors: the export / import calls on a bytes shuffle of world 1: VB_ERR_STATE (VB_ERR_INVALID on a shuffle the matching
+ * create did not make, VB_ERR_UNSUPPORTED on a sort); import before export, twice, or after seal, map after export, and
+ * seal without import: VB_ERR_STATE; a NULL column with a non-zero count: VB_ERR_INVALID; value lengths that do not add
+ * up to the byte counts: VB_ERR_INVALID, the import keeps nothing and the shuffle can still be imported; a rank that
+ * would receive 2^32 - 2 rows or more: VB_ERR_TOO_LARGE, decided from the counts so that, in vb_shuffle_exchange, every
+ * rank returns it alike. */
+VB_API int32_t vb_shuffle_create_bytes_dist(vb_ctx *ctx, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce, int32_t key_dtype,
+                                            int32_t agg, int32_t part, uint32_t rank, uint32_t world, vb_shuf **out);
+VB_API int32_t vb_shuffle_create_str_bytes_dist(vb_ctx *ctx, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce, uint32_t rank,
+                                                uint32_t world, vb_shuf **out);
+VB_API int32_t vb_shuffle_create_str_sort_bytes_dist(vb_ctx *ctx, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce, uint32_t rank,
+                                                     uint32_t world, vb_shuf **out);
+VB_API int32_t vb_shuffle_export_bytes_prepare(vb_shuf *s, uint64_t *counts /*[world]*/, uint64_t *n_val_bytes /*[world]*/);
+VB_API int32_t vb_shuffle_export_bytes_buffers(vb_shuf *s, void **keys, uint32_t **val_lens, void **val_bytes);
+VB_API int32_t vb_shuffle_import_bytes(vb_shuf *s, const void *keys, const uint32_t *val_lens, const void *val_bytes,
+                                       const uint64_t *counts /*[world]*/, const uint64_t *n_val_bytes /*[world]*/);
+VB_API int32_t vb_shuffle_export_str_bytes_prepare(vb_shuf *s, uint64_t *n_keys /*[world]*/, uint64_t *n_key_bytes /*[world]*/,
+                                                   uint64_t *n_vals /*[world]*/, uint64_t *n_val_bytes /*[world]*/);
+VB_API int32_t vb_shuffle_export_str_bytes_buffers(vb_shuf *s, uint32_t **key_lens, void **key_bytes, uint32_t **val_counts,
+                                                   uint32_t **val_lens, void **val_bytes);
+VB_API int32_t vb_shuffle_import_str_bytes(vb_shuf *s, const uint32_t *key_lens, const void *key_bytes, const uint32_t *val_counts,
+                                           const uint32_t *val_lens, const void *val_bytes, const uint64_t *n_keys /*[world]*/,
+                                           const uint64_t *n_key_bytes /*[world]*/, const uint64_t *n_vals /*[world]*/,
+                                           const uint64_t *n_val_bytes /*[world]*/);
 
 /* MetroHash64_1(bytes ‖ 0xFF, seed 0): the reference's hash of a `String` / `&str` key */
 VB_API uint64_t vb_hash_str(const void *bytes, uint64_t len);

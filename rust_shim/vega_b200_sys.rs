@@ -163,6 +163,25 @@ extern "C" {
     pub fn vb_shuffle_gather_bytes_size(s: *mut vb_shuf, refs: *const u64, n: u64, src_loc: i32, n_bytes: *mut u64) -> i32;
     pub fn vb_shuffle_gather_bytes(s: *mut vb_shuf, refs: *const u64, n: u64, src_loc: i32, out_offsets: *mut u64,
                                    out_bytes: *mut c_void, dst_loc: i32) -> i32;
+    // byte-string values across ranks: the rows' bytes travel as u32 lengths + bytes, never their references
+    pub fn vb_shuffle_create_bytes_dist(ctx: *mut vb_ctx, shuffle_id: u64, n_map: u32, n_reduce: u32, key_dtype: i32, agg: i32,
+                                        part: i32, rank: u32, world: u32, out: *mut *mut vb_shuf) -> i32;
+    pub fn vb_shuffle_create_str_bytes_dist(ctx: *mut vb_ctx, shuffle_id: u64, n_map: u32, n_reduce: u32, rank: u32, world: u32,
+                                            out: *mut *mut vb_shuf) -> i32;
+    pub fn vb_shuffle_create_str_sort_bytes_dist(ctx: *mut vb_ctx, shuffle_id: u64, n_map: u32, n_reduce: u32, rank: u32,
+                                                 world: u32, out: *mut *mut vb_shuf) -> i32;
+    pub fn vb_shuffle_export_bytes_prepare(s: *mut vb_shuf, counts: *mut u64, n_val_bytes: *mut u64) -> i32;
+    pub fn vb_shuffle_export_bytes_buffers(s: *mut vb_shuf, keys: *mut *mut c_void, val_lens: *mut *mut u32,
+                                           val_bytes: *mut *mut c_void) -> i32;
+    pub fn vb_shuffle_import_bytes(s: *mut vb_shuf, keys: *const c_void, val_lens: *const u32, val_bytes: *const c_void,
+                                   counts: *const u64, n_val_bytes: *const u64) -> i32;
+    pub fn vb_shuffle_export_str_bytes_prepare(s: *mut vb_shuf, n_keys: *mut u64, n_key_bytes: *mut u64, n_vals: *mut u64,
+                                               n_val_bytes: *mut u64) -> i32;
+    pub fn vb_shuffle_export_str_bytes_buffers(s: *mut vb_shuf, key_lens: *mut *mut u32, key_bytes: *mut *mut c_void,
+                                               val_counts: *mut *mut u32, val_lens: *mut *mut u32, val_bytes: *mut *mut c_void) -> i32;
+    pub fn vb_shuffle_import_str_bytes(s: *mut vb_shuf, key_lens: *const u32, key_bytes: *const c_void, val_counts: *const u32,
+                                       val_lens: *const u32, val_bytes: *const c_void, n_keys: *const u64, n_key_bytes: *const u64,
+                                       n_vals: *const u64, n_val_bytes: *const u64) -> i32;
     // sort_by_key over String keys (one process): map with vb_shuffle_map_str, read with vb_shuffle_reduce_str (rows in
     // key order, each with its key; the payload in out_combined); val_dtype -1 is key-only
     pub fn vb_shuffle_create_str_sort(ctx: *mut vb_ctx, shuffle_id: u64, n_map: u32, n_reduce: u32, val_dtype: i32,

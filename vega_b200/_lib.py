@@ -137,6 +137,15 @@ SYMBOLS = {
     "vb_shuffle_create_str_sort_bytes": (_i32, [_vp, _u64, _u32, _u32, _pvp]),
     "vb_shuffle_gather_bytes_size": (_i32, [_vp, _vp, _u64, _i32, _pu64]),
     "vb_shuffle_gather_bytes": (_i32, [_vp, _vp, _u64, _i32, _vp, _vp, _i32]),
+    "vb_shuffle_create_bytes_dist": (_i32, [_vp, _u64, _u32, _u32, _i32, _i32, _i32, _u32, _u32, _pvp]),
+    "vb_shuffle_create_str_bytes_dist": (_i32, [_vp, _u64, _u32, _u32, _u32, _u32, _pvp]),
+    "vb_shuffle_create_str_sort_bytes_dist": (_i32, [_vp, _u64, _u32, _u32, _u32, _u32, _pvp]),
+    "vb_shuffle_export_bytes_prepare": (_i32, [_vp, _pu64, _pu64]),
+    "vb_shuffle_export_bytes_buffers": (_i32, [_vp, _pvp, _pvp, _pvp]),
+    "vb_shuffle_import_bytes": (_i32, [_vp, _vp, _vp, _vp, _pu64, _pu64]),
+    "vb_shuffle_export_str_bytes_prepare": (_i32, [_vp, _pu64, _pu64, _pu64, _pu64]),
+    "vb_shuffle_export_str_bytes_buffers": (_i32, [_vp, _pvp, _pvp, _pvp, _pvp, _pvp]),
+    "vb_shuffle_import_str_bytes": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _pu64, _pu64, _pu64, _pu64]),
     "vb_hash_str": (_u64, [_vp, _u64]),
     "vb_get_partition_str": (_u32, [_vp, _u64, _u32]),
     "vb_shuffle_reduce_blob_size": (_i32, [_vp, _u32, _pu64]),

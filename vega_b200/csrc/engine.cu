@@ -381,6 +381,11 @@ struct vb_shuf {
     // device copy of the table is made by the first gather.  Internal shuffles of a filtered join have no store.
     std::vector<ByteSrc> bvals;
     ByteSrc *bvals_dev = nullptr;
+    // ... across ranks (vb_shuffle_create_*bytes_dist): the packed values of the export (u32 lengths and the bytes, in
+    // the exported rows' order), owned until seal; what a rank receives is one more store, bvals[n_map]
+    bool bdist = false;
+    u32 *bx_lens = nullptr;
+    unsigned char *bx_bytes = nullptr;
     // by (the right side's uid, join kind): internal (left, right) shuffles over the rows that join kind keeps
     std::map<std::pair<u64, int>, std::pair<vb_shuf *, vb_shuf *>> filtered;
     // stats
@@ -393,7 +398,9 @@ struct vb_shuf {
 
 static int seal_str(vb_shuf *s);
 static int seal_str_import(vb_shuf *s);
-static int export_str_locked(vb_shuf *s, u64 *n_keys, u64 *n_key_bytes, u64 *n_vals);
+static int export_str_locked(vb_shuf *s, u64 *n_keys, u64 *n_key_bytes, u64 *n_vals, u64 *n_val_bytes = nullptr);
+static int bytes_pack(vb_shuf *s, const u64 *refs, u64 n, const std::vector<u64> &cut, std::vector<u64> &at);
+static int bytes_adopt(vb_shuf *s, const u32 *lens, u64 n, DevBuf &bytes, u64 n_bytes, DevBuf &refs);
 static int str_import_limits(const vb_shuf *s, u64 nk, u64 nv);
 static int exchange_str_locked(vb_shuf *s);
 static int exchange_str_accs_locked(vb_shuf *s);
@@ -1935,6 +1942,10 @@ static void release_inputs(vb_shuf *s)
     dev_free(s->ctx, s->imp_own_k);
     dev_free(s->ctx, s->imp_own_v);
     s->imp_own_k = s->imp_own_v = nullptr;
+    dev_free(s->ctx, s->bx_lens);
+    dev_free(s->ctx, s->bx_bytes);
+    s->bx_lens = nullptr;
+    s->bx_bytes = nullptr;
 }
 
 // Finish the local map side and pack rows by destination rank (caller holds c->mu).
@@ -1995,6 +2006,19 @@ extern "C" int32_t vb_shuffle_export_prepare(vb_shuf *s, uint64_t *counts)
     CU(cudaSetDevice(c->device));
     TRY(export_prepare_locked(s, counts));
     CU(cudaStreamSynchronize(c->stream));
+    return VB_OK;
+}
+
+// export_prepare_locked of a byte-string-value shuffle across ranks: the rows packed by destination, then their values'
+// bytes packed in that order (bytes_pack); n_val_bytes[d] = the value bytes that go to rank d.  Caller holds c->mu.
+static int export_bytes_locked(vb_shuf *s, u64 *counts, u64 *n_val_bytes)
+{
+    const u32 W = s->world;
+    TRY(export_prepare_locked(s, counts));
+    std::vector<u64> cut((size_t)W + 1, 0), at;
+    for (u32 d = 0; d < W; ++d) cut[d + 1] = cut[d] + counts[d];
+    TRY(bytes_pack(s, s->exp_vals, cut[W], cut, at));
+    for (u32 d = 0; d < W; ++d) n_val_bytes[d] = at[d + 1] - at[d];
     return VB_OK;
 }
 
@@ -2293,11 +2317,15 @@ struct Comm {
     bool handles_valid = false;
 };
 constexpr u32 COMM_MAX_WORLD = 64;
-constexpr size_t COMM_HOST_OFF = 256 << 10;   // staging region inside vb_ctx::h_scratch
+constexpr size_t COMM_HOST_OFF = 256 << 10;   // staging region inside vb_ctx::h_scratch: the count matrix, then the IPC handles
+constexpr size_t COMM_MAT_BYTES = 192 << 10;  // the count matrix and this rank's row: (world + 1) * comm_row(world) u64
+static_assert(COMM_HOST_OFF + COMM_MAT_BYTES + 128 + 80 * 64 <= (1 << 20) - 4096, "staging inside h_scratch, before its status cells");
 // u64 per rank of the count all-gather: world + 2 for integer rows (counts, arena bytes and generation), world + 3 for
 // combine_by_key (counts and the spec's fingerprint), 3 * world for String keys, 2 * world + 3 for String-key
-// combine_by_key (key and byte counts, and the spec's fingerprint), 2 for sort, 3 for String sort
-static size_t comm_row(u32 world) { return std::max<size_t>({(size_t)world + 2, 3 * (size_t)world, 2 * (size_t)world + 3}); }
+// combine_by_key (key and byte counts, and the spec's fingerprint), 2 * world for integer rows with byte-string values
+// (counts and value bytes), 4 * world for String keys with them, 2 for sort, 3 for String sort
+static size_t comm_row(u32 world) { return std::max<size_t>({(size_t)world + 2, 4 * (size_t)world, 2 * (size_t)world + 3}); }
+static_assert((COMM_MAX_WORLD + 1) * 4 * COMM_MAX_WORLD * 8 <= COMM_MAT_BYTES, "the widest count matrix fits its staging");
 
 static void comm_teardown(vb_ctx *c)
 {
@@ -2498,13 +2526,17 @@ static int exchange_nccl_locked(vb_shuf *s)
     vb_ctx *c = s->ctx;
     Comm *m = c->comm;
     const u32 W = m->world, me = m->rank;
-    const size_t len = (size_t)W + 2;            // counts[W], arena bytes, arena generation
+    // byte-string values: counts[W] and value bytes[W], and u32 value lengths plus the bytes in place of the values
+    const bool bx = s->bdist;
+    const size_t len = bx ? 2 * (size_t)W : (size_t)W + 2;   // counts[W], arena bytes, arena generation
     std::vector<u64> row(len, 0);
     auto clk = std::chrono::steady_clock::now();
-    TRY(export_prepare_locked(s, row.data()));
+    TRY(bx ? export_bytes_locked(s, row.data(), row.data() + W) : export_prepare_locked(s, row.data()));
     s->xst.prepare_wall_ms += lap(clk);
-    row[W] = c->arena_bytes;
-    row[W + 1] = c->arena_gen;
+    if (!bx) {
+        row[W] = c->arena_bytes;
+        row[W + 1] = c->arena_gen;
+    }
     const u64 *mat = nullptr;
     TRY(comm_all_gather(c, row.data(), len, &mat));
     s->xst.counts_wall_ms += lap(clk);
@@ -2512,12 +2544,20 @@ static int exchange_nccl_locked(vb_shuf *s)
         const u64 nd = xsplit(mat, len, W, d, 0).roff[W];
         if (nd >= 0xFFFFFFFEull) return set_err(VB_ERR_TOO_LARGE, "rank %u would receive %llu rows", d, (unsigned long long)nd);
     }
-    const std::vector<XSplit> sp{xsplit(mat, len, W, me, 0)};
+    std::vector<XSplit> sp{xsplit(mat, len, W, me, 0)};
+    if (bx) sp.push_back(xsplit(mat, len, W, me, 1));
     const u64 n_recv = sp[0].roff[W];
-    DevBuf rk(c), rv(c);
+    DevBuf rk(c), rv(c), rl(c), rb(c);
     TRY(rk.alloc(std::max<u64>(n_recv, 1) * 8));
-    TRY(rv.alloc(std::max<u64>(n_recv, 1) * 8));
-    TRY(post_group(s, xfers(sp, {{ncclUint64, s->exp_keys, rk.p, 0}, {ncclUint64, s->exp_vals, rv.p, 0}}, W)));
+    if (bx) {
+        TRY(rl.alloc(n_recv * 4));
+        TRY(rb.alloc(sp[1].roff[W]));
+        TRY(post_group(s, xfers(sp, {{ncclUint64, s->exp_keys, rk.p, 0}, {ncclUint32, s->bx_lens, rl.p, 0}, {ncclUint8, s->bx_bytes, rb.p, 1}}, W)));
+        TRY(bytes_adopt(s, rl.as<u32>(), n_recv, rb, sp[1].roff[W], rv));
+    } else {
+        TRY(rv.alloc(std::max<u64>(n_recv, 1) * 8));
+        TRY(post_group(s, xfers(sp, {{ncclUint64, s->exp_keys, rk.p, 0}, {ncclUint64, s->exp_vals, rv.p, 0}}, W)));
+    }
     s->xst.post_wall_ms += lap(clk);
     xchg_done(s, VB_XCHG_NCCL, sp[0].soff[W] - sp[0].send[me], n_recv - sp[0].recv[me]);
     s->imp_own_k = (u64 *)rk.release();
@@ -2565,7 +2605,7 @@ static int exchange_p2p_locked(vb_shuf *s)
     if (any_regrow) {
         memcpy(hbuf + 64, &gen, 8);
         memset(hbuf + 72, 0, 8);
-        unsigned char *hh = (unsigned char *)c->h_scratch + COMM_HOST_OFF + 128 * 1024;
+        unsigned char *hh = (unsigned char *)c->h_scratch + COMM_HOST_OFF + COMM_MAT_BYTES;
         memcpy(hh, hbuf, 80);
         CU(cudaMemcpyAsync(m->d_hs, hh, 80, cudaMemcpyHostToDevice, c->stream));
         NC(g_nccl.AllGather(m->d_hs, m->d_hr, 80, ncclUint8, m->comm, c->stream));
@@ -2820,7 +2860,7 @@ static int exchange_sort_locked(vb_shuf *s)
     const u64 *mat = nullptr;
     TRY(comm_all_gather(c, c0, 2, &mat));
     s->xst.counts_wall_ms += lap(clk);
-    u64 N = 0; bool any_val = false;
+    u64 N = 0; bool any_val = s->bdist;          // byte-string values: lengths and bytes always travel
     for (u32 r = 0; r < W; ++r) { N += mat[2 * r]; if (mat[2 * r] && mat[2 * r + 1]) any_val = true; }
     // 2. exact cut keys: s_p = the key of global rank c_p - 1, c_p = floor(p N / R); rows with key <= s_p go to partitions < p
     const u32 P = R - 1;
@@ -2866,49 +2906,70 @@ static int exchange_sort_locked(vb_shuf *s)
     }
     cut[0] = 0; cut[R] = n_local;
     for (u32 p = 1; p <= R; ++p) cut[p] = std::max(cut[p], cut[p - 1]);
-    // 3. segment sizes of every rank for every partition
-    std::vector<u64> seg(R);
+    // 3. segment sizes of every rank for every partition (byte-string values: then each segment's value bytes, from the
+    // pack of the sorted payload)
+    const bool bx = s->bdist;
+    const u32 SR = bx ? 2 * R : R;
+    std::vector<u64> seg(SR), bat;
     for (u32 p = 0; p < R; ++p) seg[p] = cut[p + 1] - cut[p];
+    if (bx) {
+        TRY(bytes_pack(s, lv, n_local, cut, bat));
+        for (u32 p = 0; p < R; ++p) seg[R + p] = bat[p + 1] - bat[p];
+    }
     DevBuf d_seg(c), d_segall(c);
-    TRY(d_seg.alloc((size_t)R * 8)); TRY(d_segall.alloc((size_t)W * R * 8));
-    std::vector<u64> segall((size_t)W * R);
-    CU(cudaMemcpyAsync(d_seg.p, seg.data(), (size_t)R * 8, cudaMemcpyHostToDevice, c->stream));
-    NC(g_nccl.AllGather(d_seg.p, d_segall.p, R, ncclUint64, m->comm, c->stream));
-    CU(cudaMemcpyAsync(segall.data(), d_segall.p, (size_t)W * R * 8, cudaMemcpyDeviceToHost, c->stream));
+    TRY(d_seg.alloc((size_t)SR * 8)); TRY(d_segall.alloc((size_t)W * SR * 8));
+    std::vector<u64> segall((size_t)W * SR);
+    CU(cudaMemcpyAsync(d_seg.p, seg.data(), (size_t)SR * 8, cudaMemcpyHostToDevice, c->stream));
+    NC(g_nccl.AllGather(d_seg.p, d_segall.p, SR, ncclUint64, m->comm, c->stream));
+    CU(cudaMemcpyAsync(segall.data(), d_segall.p, (size_t)W * SR * 8, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
     // every rank's receive total, so that all ranks refuse alike
     for (u32 d = 0; d < W; ++d) {
         u64 nd = 0;
         for (u32 p = d; p < R; p += W)
-            for (u32 r = 0; r < W; ++r) nd += segall[(size_t)r * R + p];
+            for (u32 r = 0; r < W; ++r) nd += segall[(size_t)r * SR + p];
         if (nd >= 0xFFFFFFFEull) return set_err(VB_ERR_TOO_LARGE, "rank %u would receive %llu rows", d, (unsigned long long)nd);
     }
     s->sort_part_rows.assign(R, 0);
-    u64 n_recv = 0;
+    u64 n_recv = 0, nb_recv = 0;
     for (u32 p = me; p < R; p += W)
-        for (u32 r = 0; r < W; ++r) { s->sort_part_rows[p] += segall[(size_t)r * R + p]; n_recv += segall[(size_t)r * R + p]; }
+        for (u32 r = 0; r < W; ++r) {
+            s->sort_part_rows[p] += segall[(size_t)r * SR + p];
+            n_recv += segall[(size_t)r * SR + p];
+            if (bx) nb_recv += segall[(size_t)r * SR + R + p];
+        }
     // 4. one grouped send/recv: partition-major, source-rank-major at the receiver
-    DevBuf rk(c), rv(c);
+    DevBuf rk(c), rv(c), rl(c), rb(c);
     TRY(rk.alloc(std::max<u64>(n_recv, 1) * 8));
-    if (any_val) TRY(rv.alloc(std::max<u64>(n_recv, 1) * 8));
+    if (bx) { TRY(rl.alloc(n_recv * 4)); TRY(rb.alloc(nb_recv)); }
+    else if (any_val) TRY(rv.alloc(std::max<u64>(n_recv, 1) * 8));
     DevBuf zero_v(c);
-    if (any_val && !lv && n_local) { TRY(zero_v.alloc(n_local * 8)); CU(cudaMemsetAsync(zero_v.p, 0, n_local * 8, c->stream)); lv = zero_v.as<u64>(); }
+    if (any_val && !bx && !lv && n_local) { TRY(zero_v.alloc(n_local * 8)); CU(cudaMemsetAsync(zero_v.p, 0, n_local * 8, c->stream)); lv = zero_v.as<u64>(); }
     std::vector<Xfer> xs;
     u64 sent = 0, own = 0;
     for (u32 p = 0; p < R; ++p) {
         xs.push_back(Xfer{true, p % W, lk + cut[p], seg[p], ncclUint64});
-        if (any_val) xs.push_back(Xfer{true, p % W, lv + cut[p], seg[p], ncclUint64});
+        if (bx) {
+            xs.push_back(Xfer{true, p % W, s->bx_lens + cut[p], seg[p], ncclUint32});
+            xs.push_back(Xfer{true, p % W, s->bx_bytes + bat[p], seg[R + p], ncclUint8});
+        } else if (any_val) xs.push_back(Xfer{true, p % W, lv + cut[p], seg[p], ncclUint64});
         (p % W == me ? own : sent) += seg[p];
     }
-    u64 off = 0;
+    u64 off = 0, boff = 0;
     for (u32 p = me; p < R; p += W)
         for (u32 r = 0; r < W; ++r) {
-            const u64 cnt = segall[(size_t)r * R + p];
+            const u64 cnt = segall[(size_t)r * SR + p];
             xs.push_back(Xfer{false, r, rk.as<u64>() + off, cnt, ncclUint64});
-            if (any_val) xs.push_back(Xfer{false, r, rv.as<u64>() + off, cnt, ncclUint64});
+            if (bx) {
+                const u64 nb = segall[(size_t)r * SR + R + p];
+                xs.push_back(Xfer{false, r, rl.as<u32>() + off, cnt, ncclUint32});
+                xs.push_back(Xfer{false, r, rb.as<unsigned char>() + boff, nb, ncclUint8});
+                boff += nb;
+            } else if (any_val) xs.push_back(Xfer{false, r, rv.as<u64>() + off, cnt, ncclUint64});
             off += cnt;
         }
     TRY(post_group(s, xs));
+    if (bx) TRY(bytes_adopt(s, rl.as<u32>(), n_recv, rb, nb_recv, rv));
     s->xst.post_wall_ms += lap(clk);
     xchg_done(s, VB_XCHG_NCCL, sent, n_recv - own);
     s->imp_own_k = (u64 *)rk.release();
@@ -2922,7 +2983,8 @@ static int exchange_sort_locked(vb_shuf *s)
 
 extern "C" int32_t vb_shuffle_exchange(vb_shuf *s, int32_t mode)
 {
-    if (s && s->vdt == VB_BYTES) return reject_bytes(s, "vb_shuffle_exchange");
+    if (s && s->vdt == VB_BYTES && !s->bdist) return reject_bytes(s, "vb_shuffle_exchange (the _bytes_dist creates make shuffles that cross ranks)");
+    if (s && s->bdist && mode == VB_XCHG_P2P) return reject_bytes(s, "the fused P2P exchange (VB_XCHG_NCCL is supported)");
     if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
     if (s->multi && s->world < 2) return reject_multi(s, "an exchange of a one-process shuffle (vb_shuffle_create_multi_dist has world > 1)");
     if (s->multi && mode == VB_XCHG_P2P) return reject_multi(s, "the fused P2P exchange (VB_XCHG_NCCL is supported)");
@@ -2938,7 +3000,7 @@ extern "C" int32_t vb_shuffle_exchange(vb_shuf *s, int32_t mode)
         CU(cudaSetDevice(c->device));
         return s->str ? (is_reduce_op(s->agg) ? exchange_str_accs_locked(s) : exchange_str_locked(s)) : exchange_multi_locked(s);
     }
-    if (mode == VB_XCHG_AUTO) mode = is_group_op(s->agg) ? VB_XCHG_P2P : VB_XCHG_NCCL;
+    if (mode == VB_XCHG_AUTO) mode = is_group_op(s->agg) && !s->bdist ? VB_XCHG_P2P : VB_XCHG_NCCL;
     if (mode == VB_XCHG_P2P && !is_group_op(s->agg)) return set_err(VB_ERR_UNSUPPORTED, "the fused P2P exchange is for GROUP/COGROUP shuffles");
     std::lock_guard<std::mutex> lk(c->mu);
     CU(cudaSetDevice(c->device));
@@ -4761,6 +4823,7 @@ static int bytes_check_args(vb_shuf *s, u32 map_id, const u64 *val_offsets, cons
     if (n >= 0xFFFFFFFEull) return set_err(VB_ERR_TOO_LARGE, "map partition of %llu rows", (unsigned long long)n);
     std::lock_guard<std::mutex> g(s->mu);
     if (s->sealed || s->sealing || s->freed) return set_err(VB_ERR_STATE, "shuffle %llu: map after seal", (unsigned long long)s->id);
+    if (s->exported) return set_err(VB_ERR_STATE, "shuffle %llu: map after export", (unsigned long long)s->id);
     return VB_OK;
 }
 
@@ -4826,7 +4889,7 @@ extern "C" int32_t vb_shuffle_map_bytes(vb_shuf *s, uint32_t map_id, const void 
                                         uint64_t n_val_bytes, uint64_t n, int32_t loc)
 {
     if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
-    if (s->vdt != VB_BYTES || s->str || s->bvals.size() != s->n_map)
+    if (s->vdt != VB_BYTES || s->str || s->bvals.size() < s->n_map)
         return set_err(VB_ERR_INVALID, "vb_shuffle_map_bytes needs an integer-key shuffle of VB_BYTES values");
     if (n && !keys) return set_err(VB_ERR_INVALID, "NULL keys with n_rows > 0");
     TRY(bytes_check_args(s, map_id, val_offsets, val_bytes, n_val_bytes, n, loc));
@@ -4840,7 +4903,7 @@ extern "C" int32_t vb_shuffle_map_str_bytes(vb_shuf *s, uint32_t map_id, const u
                                             const uint64_t *val_offsets, const void *val_bytes, uint64_t n_val_bytes, uint64_t n, int32_t loc)
 {
     if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
-    if (s->vdt != VB_BYTES || !s->str || s->multi || s->bvals.size() != s->n_map)
+    if (s->vdt != VB_BYTES || !s->str || s->multi || s->bvals.size() < s->n_map)
         return set_err(VB_ERR_INVALID, "vb_shuffle_map_str_bytes needs a string-key shuffle of VB_BYTES values");
     if (n && !key_offsets) return set_err(VB_ERR_INVALID, "NULL key_offsets with n_rows > 0");
     if (n && n_key_bytes && !key_bytes) return set_err(VB_ERR_INVALID, "NULL key_bytes with n_key_bytes > 0");
@@ -4891,10 +4954,21 @@ static int bytes_offsets(vb_shuf *s, const u64 *refs_in, u64 n, int src_loc, Dev
     return fetch_status_unlocked(c, offs + n, total, 8);
 }
 
+// out [total] = the values of the n device references refs at the offsets offs (bytes_offsets)
+static int bytes_gather_launch(vb_shuf *s, const u64 *refs, u64 n, const u64 *offs, u64 total, unsigned char *out)
+{
+    vb_ctx *c = s->ctx;
+    const u64 tiles = (n + total + GB_ITEMS - 1) / GB_ITEMS;
+    const u64 grid = std::min<u64>(tiles, (u64)c->sm_count * occupancy(c, bytes_gather_kernel, GB_THREADS, 0));
+    KLaunch kl(s, K_MISC, n);
+    bytes_gather_kernel<<<(unsigned)grid, GB_THREADS, 0, c->stream>>>(refs, n, offs, total, s->bvals_dev, (u32)s->bvals.size(), out);
+    return kl.done("bytes_gather_kernel");
+}
+
 static int bytes_gather_check(vb_shuf *s, const void *refs, u64 n, int src_loc)
 {
     if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
-    if (s->vdt != VB_BYTES || s->bvals.size() != s->n_map) return set_err(VB_ERR_INVALID, "shuffle %llu has no byte-string values", (unsigned long long)s->id);
+    if (s->vdt != VB_BYTES || s->bvals.size() < s->n_map) return set_err(VB_ERR_INVALID, "shuffle %llu has no byte-string values", (unsigned long long)s->id);
     if (n && !refs) return set_err(VB_ERR_INVALID, "NULL refs with n > 0");
     if (src_loc < VB_HOST || src_loc > VB_DEVICE_BORROWED) return set_err(VB_ERR_INVALID, "bad src_loc %d", src_loc);
     return wait_sealed(s);
@@ -4935,14 +5009,7 @@ extern "C" int32_t vb_shuffle_gather_bytes(vb_shuf *s, const uint64_t *refs, uin
     if (total && !out_bytes) return set_err(VB_ERR_INVALID, "NULL out_bytes for %llu bytes", (unsigned long long)total);
     unsigned char *dst = (unsigned char *)out_bytes;
     if (total && dst_loc == VB_HOST) { TRY(bytes_tmp.alloc(total)); dst = bytes_tmp.as<unsigned char>(); }
-    if (total) {
-        const u64 tiles = (n + total + GB_ITEMS - 1) / GB_ITEMS;
-        const u64 grid = std::min<u64>(tiles, (u64)c->sm_count * occupancy(c, bytes_gather_kernel, GB_THREADS, 0));
-        const u64 *rd = src_loc == VB_HOST ? r.as<u64>() : refs;
-        KLaunch kl(s, K_MISC, n);
-        bytes_gather_kernel<<<(unsigned)grid, GB_THREADS, 0, c->stream>>>(rd, n, offs, total, s->bvals_dev, (u32)s->bvals.size(), dst);
-        TRY(kl.done("bytes_gather_kernel"));
-    }
+    if (total) TRY(bytes_gather_launch(s, src_loc == VB_HOST ? r.as<u64>() : refs, n, offs, total, dst));
     if (staged) {
         TRY(copy_out(s, out_offsets, offs, (n + 1) * 8, dst_loc));
     }
@@ -5553,7 +5620,7 @@ static int str_sort_out(vb_shuf *s, uint32_t r, uint64_t *out_key_offsets, void 
 // ...), so the dense ids come out grouped by destination; then the values of step 3, as every accumulator of the
 // spec per key in plain value form (reduce ops and combine_by_key) or each key's values in map order (GROUP).  The
 // per-map ids and the dictionary are freed.  The caller holds c->mu.
-static int export_str_locked(vb_shuf *s, u64 *n_keys, u64 *n_key_bytes, u64 *n_vals)
+static int export_str_locked(vb_shuf *s, u64 *n_keys, u64 *n_key_bytes, u64 *n_vals, u64 *n_val_bytes)
 {
     vb_ctx *c = s->ctx;
     StrState *t = s->str;
@@ -5563,6 +5630,7 @@ static int export_str_locked(vb_shuf *s, u64 *n_keys, u64 *n_key_bytes, u64 *n_v
     }
     const u32 W = s->world, R = s->n_reduce;
     for (u32 d = 0; d < W; ++d) n_keys[d] = n_key_bytes[d] = n_vals[d] = 0;
+    if (n_val_bytes) std::fill(n_val_bytes, n_val_bytes + W, 0);
     const std::vector<StrRun> runs = str_map_runs(s);
     u64 n = 0;
     for (const StrRun &r : runs) n += r.n;
@@ -5612,6 +5680,11 @@ static int export_str_locked(vb_shuf *s, u64 *n_keys, u64 *n_key_bytes, u64 *n_v
             }
             TRY(str_read_at(s, offs.as<u64>(), cut, at));
             for (u32 d = 0; d < W; ++d) n_vals[d] = at[d + 1] - at[d];
+            if (s->bdist) {                     // byte-string values: their bytes travel in the values' order
+                std::vector<u64> bat;
+                TRY(bytes_pack(s, vals.as<u64>(), n, at, bat));
+                for (u32 d = 0; d < W; ++d) n_val_bytes[d] = bat[d + 1] - bat[d];
+            }
             t->x_cnts = (u32 *)cnts.release();
             t->x_vals = (u64 *)vals.release();
         }
@@ -5802,25 +5875,31 @@ static int exchange_str_locked(vb_shuf *s)
     Comm *m = c->comm;
     StrState *t = s->str;
     const u32 W = m->world, me = m->rank;
-    const size_t len = 3 * (size_t)W;            // n_keys[W], n_key_bytes[W], n_vals[W]
+    // byte-string values: a fourth count vector (value bytes), and u32 value lengths plus the bytes in place of the values
+    const bool bx = s->bdist;
+    const size_t len = (bx ? 4 : 3) * (size_t)W;   // n_keys[W], n_key_bytes[W], n_vals[W] (, n_val_bytes[W])
     std::vector<u64> row(len, 0);
     auto clk = std::chrono::steady_clock::now();
-    TRY(export_str_locked(s, row.data(), row.data() + W, row.data() + 2 * (size_t)W));
+    TRY(export_str_locked(s, row.data(), row.data() + W, row.data() + 2 * (size_t)W, bx ? row.data() + 3 * (size_t)W : nullptr));
     s->xst.prepare_wall_ms += lap(clk);
     const u64 *mat = nullptr;
     TRY(comm_all_gather(c, row.data(), len, &mat));
     s->xst.counts_wall_ms += lap(clk);
     for (u32 d = 0; d < W; ++d) TRY(str_import_limits(s, xsplit(mat, len, W, d, 0).roff[W], xsplit(mat, len, W, d, 2).roff[W]));
-    const std::vector<XSplit> sp{xsplit(mat, len, W, me, 0), xsplit(mat, len, W, me, 1), xsplit(mat, len, W, me, 2)};
-    const u64 nk = sp[0].roff[W], nkb = sp[1].roff[W], nv = sp[2].roff[W];
-    DevBuf lens(c), bytes(c), cnts(c), vals(c);
+    std::vector<XSplit> sp{xsplit(mat, len, W, me, 0), xsplit(mat, len, W, me, 1), xsplit(mat, len, W, me, 2)};
+    if (bx) sp.push_back(xsplit(mat, len, W, me, 3));
+    const u64 nk = sp[0].roff[W], nkb = sp[1].roff[W], nv = sp[2].roff[W], nvb = bx ? sp[3].roff[W] : 0;
+    DevBuf lens(c), bytes(c), cnts(c), vals(c), vlens(c), vbytes(c);
     TRY(lens.alloc(nk * 4));
     TRY(bytes.alloc(nkb));
     TRY(cnts.alloc(nk * 4));
-    TRY(vals.alloc(nv * 8));
-    const std::vector<XCol> cols{{ncclUint32, t->x_lens, lens.p, 0}, {ncclUint8, t->x_bytes, bytes.p, 1}, {ncclUint64, t->x_vals, vals.p, 2},
-                                 {ncclUint32, t->x_cnts, cnts.p, 0}};
+    if (bx) { TRY(vlens.alloc(nv * 4)); TRY(vbytes.alloc(nvb)); }
+    else TRY(vals.alloc(nv * 8));
+    std::vector<XCol> cols{{ncclUint32, t->x_lens, lens.p, 0}, {ncclUint8, t->x_bytes, bytes.p, 1}, {ncclUint32, t->x_cnts, cnts.p, 0}};
+    if (bx) { cols.push_back({ncclUint32, s->bx_lens, vlens.p, 2}); cols.push_back({ncclUint8, s->bx_bytes, vbytes.p, 3}); }
+    else cols.push_back({ncclUint64, t->x_vals, vals.p, 2});
     TRY(post_group(s, xfers(sp, cols, W)));
+    if (bx) TRY(bytes_adopt(s, vlens.as<u32>(), nv, vbytes, nvb, vals));
     s->xst.post_wall_ms += lap(clk);
     xchg_done(s, VB_XCHG_NCCL, sp[2].soff[W] - sp[2].send[me], nv - sp[2].recv[me]);
     void **own = t->i_own;
@@ -6011,14 +6090,19 @@ static int exchange_str_sort_locked(vb_shuf *s)
     kcut[R] = D;
     TRY(str_sort_agree_cuts(s, koff.as<u64>(), kbytes.as<unsigned char>(), roff.as<u64>(), D, N, kcut));
     for (u32 p = 1; p <= R; ++p) kcut[p] = std::max(kcut[p], kcut[p - 1]);
-    // 4. the segment table: keys, key bytes and rows of every partition, from every rank
-    std::vector<u64> kb_at, r_at, seg(3 * (size_t)R), segall(3 * (size_t)R * W);
+    // 4. the segment table: keys, key bytes and rows of every partition, from every rank (byte-string values: then
+    // each partition's value bytes, from the pack of the payload in row order)
+    const bool bx = s->bdist;
+    const u32 ncol = bx ? 4 : 3;
+    std::vector<u64> kb_at, r_at, b_at, seg(ncol * (size_t)R), segall(ncol * (size_t)R * W);
     TRY(str_read_at(s, koff.as<u64>(), kcut, kb_at));
     TRY(str_read_at(s, roff.as<u64>(), kcut, r_at));
+    if (bx) TRY(bytes_pack(s, pay.as<u64>(), n_local, r_at, b_at));
     for (u32 p = 0; p < R; ++p) {
         seg[p] = kcut[p + 1] - kcut[p];
         seg[R + p] = kb_at[p + 1] - kb_at[p];
         seg[2 * (size_t)R + p] = r_at[p + 1] - r_at[p];
+        if (bx) seg[3 * (size_t)R + p] = b_at[p + 1] - b_at[p];
     }
     {
         DevBuf d_seg(c), d_segall(c);
@@ -6028,7 +6112,7 @@ static int exchange_str_sort_locked(vb_shuf *s)
         CU(cudaMemcpyAsync(segall.data(), d_segall.p, segall.size() * 8, cudaMemcpyDeviceToHost, c->stream));
         CU(cudaStreamSynchronize(c->stream));
     }
-    auto at = [&](u32 r, u32 col, u32 p) { return segall[(size_t)r * 3 * R + (size_t)col * R + p]; };
+    auto at = [&](u32 r, u32 col, u32 p) { return segall[(size_t)r * ncol * R + (size_t)col * R + p]; };
     for (u32 d = 0; d < W; ++d) {
         u64 nk = 0, nv = 0;
         for (u32 p = d; p < R; p += W)
@@ -6046,13 +6130,17 @@ static int exchange_str_sort_locked(vb_shuf *s)
         TRY(kl.done("str_diff_u32_kernel"));
     }
     s->sort_part_rows.assign(R, 0);
-    u64 nk = 0, nkb = 0, nv = 0;
+    u64 nk = 0, nkb = 0, nv = 0, nvb = 0;
     for (u32 p = me; p < R; p += W)
-        for (u32 r = 0; r < W; ++r) { nk += at(r, 0, p); nkb += at(r, 1, p); nv += at(r, 2, p); s->sort_part_rows[p] += at(r, 2, p); }
+        for (u32 r = 0; r < W; ++r) {
+            nk += at(r, 0, p); nkb += at(r, 1, p); nv += at(r, 2, p); s->sort_part_rows[p] += at(r, 2, p);
+            if (bx) nvb += at(r, 3, p);
+        }
     const bool vals = t->sort_vals;
-    DevBuf rl(c), rb(c), rn(c), rv(c);
+    DevBuf rl(c), rb(c), rn(c), rv(c), rvl(c), rvb(c);
     TRY(rl.alloc(nk * 4)); TRY(rb.alloc(nkb)); TRY(rn.alloc(nk * 4));
-    if (vals) TRY(rv.alloc(nv * 8));
+    if (bx) { TRY(rvl.alloc(nv * 4)); TRY(rvb.alloc(nvb)); }
+    else if (vals) TRY(rv.alloc(nv * 8));
     std::vector<Xfer> xs;
     u64 sent = 0, own = 0;
     for (u32 p = 0; p < R; ++p) {
@@ -6060,25 +6148,280 @@ static int exchange_str_sort_locked(vb_shuf *s)
         xs.push_back(Xfer{true, d, lens.as<u32>() + kcut[p], seg[p], ncclUint32});
         xs.push_back(Xfer{true, d, kbytes.as<unsigned char>() + kb_at[p], seg[R + p], ncclUint8});
         xs.push_back(Xfer{true, d, cnts.as<u32>() + kcut[p], seg[p], ncclUint32});
-        if (vals) xs.push_back(Xfer{true, d, pay.as<u64>() + r_at[p], seg[2 * (size_t)R + p], ncclUint64});
+        if (bx) {
+            xs.push_back(Xfer{true, d, s->bx_lens + r_at[p], seg[2 * (size_t)R + p], ncclUint32});
+            xs.push_back(Xfer{true, d, s->bx_bytes + b_at[p], seg[3 * (size_t)R + p], ncclUint8});
+        } else if (vals) xs.push_back(Xfer{true, d, pay.as<u64>() + r_at[p], seg[2 * (size_t)R + p], ncclUint64});
         (d == me ? own : sent) += seg[2 * (size_t)R + p];
     }
-    u64 ok = 0, ob = 0, ov = 0;
+    u64 ok = 0, ob = 0, ov = 0, obv = 0;
     for (u32 p = me; p < R; p += W)
         for (u32 r = 0; r < W; ++r) {
             const u64 k = at(r, 0, p), b = at(r, 1, p), v = at(r, 2, p);
             xs.push_back(Xfer{false, r, rl.as<u32>() + ok, k, ncclUint32});
             xs.push_back(Xfer{false, r, rb.as<unsigned char>() + ob, b, ncclUint8});
             xs.push_back(Xfer{false, r, rn.as<u32>() + ok, k, ncclUint32});
-            if (vals) xs.push_back(Xfer{false, r, rv.as<u64>() + ov, v, ncclUint64});
+            if (bx) {
+                const u64 vb = at(r, 3, p);
+                xs.push_back(Xfer{false, r, rvl.as<u32>() + ov, v, ncclUint32});
+                xs.push_back(Xfer{false, r, rvb.as<unsigned char>() + obv, vb, ncclUint8});
+                obv += vb;
+            } else if (vals) xs.push_back(Xfer{false, r, rv.as<u64>() + ov, v, ncclUint64});
             ok += k; ob += b; ov += v;
         }
     TRY(post_group(s, xs));
+    if (bx) TRY(bytes_adopt(s, rvl.as<u32>(), nv, rvb, nvb, rv));
     s->xst.post_wall_ms += lap(clk);
     xchg_done(s, VB_XCHG_NCCL, sent, nv - own);
     void **io = t->i_own;
     io[0] = rl.release(); io[1] = rb.release(); io[2] = rn.release(); io[3] = vals ? rv.release() : nullptr;
     str_take_import(s, (const u32 *)io[0], io[1], (const u32 *)io[2], (const u64 *)io[3], nk, nkb, nv);
+    return VB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// byte-string values across ranks (vb_shuffle_create_*bytes_dist).  References never leave their rank: the export packs
+// the values' bytes in the exported rows' order (the gather of bytevals.cuh over the exported references), the wire
+// carries u32 value lengths and the bytes, and the receiver makes what it received one more store, bvals[n_map], with
+// fresh references into it in receive order.  Seal, cogroup, joins and the gather then run as on one process.
+// ---------------------------------------------------------------------------------------------
+// The pack: the values of the n device references refs, in their order, into s->bx_lens (u32) and s->bx_bytes, and
+// at[i] = the byte offset of row cut[i].  The map stores are freed after it, in stream order: a reference issued at map
+// time decodes to an empty store from here on and is refused by the gather.  Caller holds c->mu.
+static int bytes_pack(vb_shuf *s, const u64 *refs, u64 n, const std::vector<u64> &cut, std::vector<u64> &at)
+{
+    vb_ctx *c = s->ctx;
+    DevBuf none(c), offs(c), lens(c), bytes(c);
+    TRY(offs.alloc((n + 1) * 8));
+    u64 total = 0;
+    TRY(bytes_offsets(s, refs, n, VB_DEVICE, none, offs.as<u64>(), &total));
+    TRY(lens.alloc(n * 4));
+    TRY(bytes.alloc(total));
+    if (total) TRY(bytes_gather_launch(s, refs, n, offs.as<u64>(), total, bytes.as<unsigned char>()));
+    if (n) {
+        KLaunch kl(s, K_MISC, n);
+        str_diff_u32_kernel<<<str_grid(c, n), 256, 0, c->stream>>>(offs.as<u64>(), n, lens.as<u32>());
+        TRY(kl.done("str_diff_u32_kernel"));
+    }
+    TRY(str_read_at(s, offs.as<u64>(), cut, at));
+    for (u32 m = 0; m < s->n_map; ++m) {
+        dev_free(c, s->bvals[m].offs);
+        dev_free(c, s->bvals[m].bytes);
+        s->bvals[m] = ByteSrc{nullptr, nullptr, 0};
+    }
+    dev_free(c, s->bvals_dev);
+    s->bvals_dev = nullptr;
+    s->bx_lens = (u32 *)lens.release();
+    s->bx_bytes = (unsigned char *)bytes.release();
+    return VB_OK;
+}
+
+// The receive side: n received value lengths (device) and the received bytes, which the shuffle takes over as its store
+// n_map (offsets: the scan of the lengths); refs [n] = ((n_map + 1) << 32) | i in receive order.  Lengths that do not
+// add up to n_bytes are VB_ERR_INVALID, and then nothing is kept.  Caller holds c->mu.
+static int bytes_adopt(vb_shuf *s, const u32 *lens, u64 n, DevBuf &bytes, u64 n_bytes, DevBuf &refs)
+{
+    vb_ctx *c = s->ctx;
+    DevBuf wide(c), offs(c), r(c);
+    TRY(offs.alloc((n + 1) * 8));
+    TRY(r.alloc(n * 8));
+    if (n) {
+        TRY(wide.alloc(n * 8));
+        {
+            KLaunch kl(s, K_MISC, n);
+            str_widen_u32_kernel<<<str_grid(c, n), 256, 0, c->stream>>>(lens, n, wide.as<u64>());
+            TRY(kl.done("str_widen_u32_kernel"));
+        }
+        TRY(exclusive_scan_u64(s, wide.as<u64>(), offs.as<u64>(), n, offs.as<u64>() + n));
+        KLaunch kl(s, K_MISC, n);
+        bytes_refs_kernel<<<str_grid(c, n), 256, 0, c->stream>>>(((u64)s->n_map + 1) << 32, n, r.as<u64>());
+        TRY(kl.done("bytes_refs_kernel"));
+    } else {
+        CU(cudaMemsetAsync(offs.p, 0, 8, c->stream));
+    }
+    u64 total = 0;
+    TRY(fetch_status_unlocked(c, offs.as<u64>() + n, &total, 8));
+    if (total != n_bytes)
+        return set_err(VB_ERR_INVALID, "received value lengths add up to %llu bytes, %llu announced", (unsigned long long)total, (unsigned long long)n_bytes);
+    s->bvals.resize((size_t)s->n_map + 1, ByteSrc{nullptr, nullptr, 0});
+    s->bvals[s->n_map] = ByteSrc{(const u64 *)offs.release(), (const unsigned char *)bytes.release(), n};
+    dev_free(c, s->bvals_dev);            // the gather builds the device table again, with the new store
+    s->bvals_dev = nullptr;
+    refs.reset();
+    refs.p = r.release();
+    return VB_OK;
+}
+
+static int bytes_dist_args(vb_ctx *c, vb_shuf **out, uint32_t rank, uint32_t world, const char *what)
+{
+    if (!c || !out) return set_err(VB_ERR_INVALID, "%s: NULL argument", what);
+    *out = nullptr;
+    if (world < 1 || world > 256 || rank >= world) return set_err(VB_ERR_INVALID, "%s: bad rank %u / world %u (1 <= world <= 256)", what, rank, world);
+    return VB_OK;
+}
+
+static int bytes_dist_set(vb_shuf *s, uint32_t rank, uint32_t world)
+{
+    s->rank = rank;
+    s->world = world;
+    s->bdist = true;
+    return VB_OK;
+}
+
+extern "C" int32_t vb_shuffle_create_bytes_dist(vb_ctx *c, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce, int32_t kdt, int32_t agg,
+                                                int32_t part, uint32_t rank, uint32_t world, vb_shuf **out)
+{
+    TRY(bytes_dist_args(c, out, rank, world, "vb_shuffle_create_bytes_dist"));
+    TRY(vb_shuffle_create(c, shuffle_id, n_map, n_reduce, kdt, VB_BYTES, agg, part, out));
+    return bytes_dist_set(*out, rank, world);
+}
+
+extern "C" int32_t vb_shuffle_create_str_bytes_dist(vb_ctx *c, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce, uint32_t rank,
+                                                    uint32_t world, vb_shuf **out)
+{
+    TRY(bytes_dist_args(c, out, rank, world, "vb_shuffle_create_str_bytes_dist"));
+    TRY(vb_shuffle_create_str(c, shuffle_id, n_map, n_reduce, VB_BYTES, VB_AGG_GROUP, out));
+    return bytes_dist_set(*out, rank, world);
+}
+
+extern "C" int32_t vb_shuffle_create_str_sort_bytes_dist(vb_ctx *c, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce, uint32_t rank,
+                                                         uint32_t world, vb_shuf **out)
+{
+    TRY(bytes_dist_args(c, out, rank, world, "vb_shuffle_create_str_sort_bytes_dist"));
+    TRY(vb_shuffle_create_str_sort_bytes(c, shuffle_id, n_map, n_reduce, out));
+    return bytes_dist_set(*out, rank, world);
+}
+
+// the checks every bytes export / import call makes first: the matching create (str: String keys), GROUP or COGROUP,
+// world > 1
+static int bytes_dist_check(const vb_shuf *s, bool str, const char *what)
+{
+    if (!s->bdist || (s->str != nullptr) != str)
+        return set_err(VB_ERR_INVALID, "%s needs a shuffle from vb_shuffle_create_%sbytes_dist", what, str ? "str_" : "");
+    if (s->agg == VB_AGG_SORT) return set_err(VB_ERR_UNSUPPORTED, "%s: sort_by_key across ranks goes through vb_shuffle_exchange", what);
+    if (s->world < 2) return set_err(VB_ERR_STATE, "%s needs a shuffle of world > 1", what);
+    return VB_OK;
+}
+
+// the state an import needs: exported, not imported yet, not sealed
+static int bytes_import_state(vb_shuf *s, const char *what)
+{
+    std::lock_guard<std::mutex> g(s->mu);
+    if (!s->exported || s->imported || s->sealed || s->sealing || s->freed)
+        return set_err(VB_ERR_STATE, "%s needs the export first, once, and no seal yet", what);
+    return VB_OK;
+}
+
+// The received bytes copied into a buffer of the library, then bytes_adopt.  Caller holds c->mu.
+static int bytes_import_values(vb_shuf *s, const u32 *lens, u64 n, const void *val_bytes, u64 n_bytes, DevBuf &refs)
+{
+    vb_ctx *c = s->ctx;
+    DevBuf b(c);
+    TRY(b.alloc(n_bytes));
+    if (n_bytes) CU(cudaMemcpyAsync(b.p, val_bytes, n_bytes, cudaMemcpyDeviceToDevice, c->stream));
+    return bytes_adopt(s, lens, n, b, n_bytes, refs);
+}
+
+extern "C" int32_t vb_shuffle_export_bytes_prepare(vb_shuf *s, uint64_t *counts, uint64_t *n_val_bytes)
+{
+    if (!s || !counts || !n_val_bytes) return set_err(VB_ERR_INVALID, "NULL argument");
+    TRY(bytes_dist_check(s, false, "vb_shuffle_export_bytes_prepare"));
+    vb_ctx *c = s->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    TRY(export_bytes_locked(s, counts, n_val_bytes));
+    CU(cudaStreamSynchronize(c->stream));
+    return VB_OK;
+}
+
+extern "C" int32_t vb_shuffle_export_bytes_buffers(vb_shuf *s, void **keys, uint32_t **val_lens, void **val_bytes)
+{
+    if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
+    TRY(bytes_dist_check(s, false, "vb_shuffle_export_bytes_buffers"));
+    {
+        std::lock_guard<std::mutex> g(s->mu);
+        if (!s->exported || s->sealed || s->freed) return set_err(VB_ERR_STATE, "vb_shuffle_export_bytes_buffers needs vb_shuffle_export_bytes_prepare first and no seal yet");
+    }
+    if (keys) *keys = s->exp_keys;
+    if (val_lens) *val_lens = s->bx_lens;
+    if (val_bytes) *val_bytes = s->bx_bytes;
+    return VB_OK;
+}
+
+extern "C" int32_t vb_shuffle_import_bytes(vb_shuf *s, const void *keys, const uint32_t *val_lens, const void *val_bytes,
+                                           const uint64_t *counts, const uint64_t *n_val_bytes)
+{
+    if (!s || !counts || !n_val_bytes) return set_err(VB_ERR_INVALID, "NULL argument");
+    TRY(bytes_dist_check(s, false, "vb_shuffle_import_bytes"));
+    TRY(bytes_import_state(s, "vb_shuffle_import_bytes"));
+    u64 n = 0, nb = 0;
+    for (u32 r = 0; r < s->world; ++r) { n += counts[r]; nb += n_val_bytes[r]; }
+    if (n >= 0xFFFFFFFEull) return set_err(VB_ERR_TOO_LARGE, "import of %llu rows (fewer than 2^32 - 2 are supported)", (unsigned long long)n);
+    if ((n && (!keys || !val_lens)) || (nb && !val_bytes)) return set_err(VB_ERR_INVALID, "NULL column with a non-zero count");
+    vb_ctx *c = s->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    DevBuf refs(c);
+    TRY(bytes_import_values(s, val_lens, n, val_bytes, nb, refs));
+    std::lock_guard<std::mutex> g(s->mu);
+    s->imp_own_v = (u64 *)refs.release();
+    s->imp_keys = (const u64 *)keys;
+    s->imp_vals = s->imp_own_v;
+    s->imp_n = n;
+    s->imported = true;
+    return VB_OK;
+}
+
+extern "C" int32_t vb_shuffle_export_str_bytes_prepare(vb_shuf *s, uint64_t *n_keys, uint64_t *n_key_bytes, uint64_t *n_vals, uint64_t *n_val_bytes)
+{
+    if (!s || !n_keys || !n_key_bytes || !n_vals || !n_val_bytes) return set_err(VB_ERR_INVALID, "NULL argument");
+    TRY(bytes_dist_check(s, true, "vb_shuffle_export_str_bytes_prepare"));
+    vb_ctx *c = s->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    TRY(export_str_locked(s, n_keys, n_key_bytes, n_vals, n_val_bytes));
+    CU(cudaStreamSynchronize(c->stream));
+    return VB_OK;
+}
+
+extern "C" int32_t vb_shuffle_export_str_bytes_buffers(vb_shuf *s, uint32_t **key_lens, void **key_bytes, uint32_t **val_counts,
+                                                       uint32_t **val_lens, void **val_bytes)
+{
+    if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
+    TRY(bytes_dist_check(s, true, "vb_shuffle_export_str_bytes_buffers"));
+    {
+        std::lock_guard<std::mutex> g(s->mu);
+        if (!s->exported || s->sealed || s->freed) return set_err(VB_ERR_STATE, "vb_shuffle_export_str_bytes_buffers needs vb_shuffle_export_str_bytes_prepare first and no seal yet");
+    }
+    const StrState *t = s->str;
+    if (key_lens) *key_lens = t->x_lens;
+    if (key_bytes) *key_bytes = t->x_bytes;
+    if (val_counts) *val_counts = t->x_cnts;
+    if (val_lens) *val_lens = s->bx_lens;
+    if (val_bytes) *val_bytes = s->bx_bytes;
+    return VB_OK;
+}
+
+extern "C" int32_t vb_shuffle_import_str_bytes(vb_shuf *s, const uint32_t *key_lens, const void *key_bytes, const uint32_t *val_counts,
+                                               const uint32_t *val_lens, const void *val_bytes, const uint64_t *n_keys,
+                                               const uint64_t *n_key_bytes, const uint64_t *n_vals, const uint64_t *n_val_bytes)
+{
+    if (!s || !n_keys || !n_key_bytes || !n_vals || !n_val_bytes) return set_err(VB_ERR_INVALID, "NULL argument");
+    TRY(bytes_dist_check(s, true, "vb_shuffle_import_str_bytes"));
+    TRY(bytes_import_state(s, "vb_shuffle_import_str_bytes"));
+    u64 nk = 0, nkb = 0, nv = 0, nvb = 0;
+    for (u32 r = 0; r < s->world; ++r) { nk += n_keys[r]; nkb += n_key_bytes[r]; nv += n_vals[r]; nvb += n_val_bytes[r]; }
+    if ((nk && (!key_lens || !val_counts)) || (nkb && !key_bytes) || (nv && !val_lens) || (nvb && !val_bytes))
+        return set_err(VB_ERR_INVALID, "NULL column with a non-zero count");
+    TRY(str_import_limits(s, nk, nv));
+    vb_ctx *c = s->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    DevBuf refs(c);
+    TRY(bytes_import_values(s, val_lens, nv, val_bytes, nvb, refs));
+    StrState *t = s->str;
+    t->i_own[3] = refs.release();
+    str_take_import(s, key_lens, key_bytes, val_counts, (const u64 *)t->i_own[3], nk, nkb, nv);
     return VB_OK;
 }
 

@@ -20,6 +20,11 @@ driver, _exchange):
   as one [rows][1 + n_acc] column.
 - combine_by_key over String keys (StrCombineCudaEngine): u32 key lengths split by the key counts, key bytes by the
   byte counts, and the partials of every accumulator packed as one [keys][n_acc] column split by the key counts.
+- byte-string values (BytesCudaEngine, StrBytesCudaEngine): the columns of integer rows or of String keys without the
+  values, plus u32 value lengths split by the row (or value) counts and the values' bytes split by the byte counts.
+  A value's reference never leaves its rank: the receiver stores the bytes it got and issues fresh references, so the
+  results of a rank are gathered through that rank's shuffle (Shuffle.gather).  sort_by_key with byte-string values
+  crosses ranks inside the library only (vb_shuffle_exchange).
 
 The exchange itself lives in libvega_b200.so (vb_ctx_comm_init + vb_shuffle_exchange: NCCL grouped
 send/recv, or the fused peer-memory scatter, on the library's stream).  The run_*shuffle functions call it
@@ -32,7 +37,7 @@ import ctypes
 import numpy as np
 
 from . import _lib as L
-from .rdd import Shuffle, StrShuffle, _Col, _StrCol
+from .rdd import Shuffle, StrKeys, StrShuffle, _BytesCol, _Col, _is_str_keys, _StrCol
 
 
 def map_block(rank, world, n_map):
@@ -235,12 +240,18 @@ def run_shuffle(engine, local_maps, n_map, n_reduce, kcode, vcode, agg, rank, wo
     exchange_device: move the packed buffers there for the collective (tests: "cpu" + gloo on a 1-GPU box).
     p2p: GROUP/COGROUP shuffles use the fused partition+send over peer memory instead of pack + all-to-all-v.
     """
-    if vcode == L.VB_BYTES:
-        raise TypeError("byte-string values do not cross ranks yet")
+    if (vcode == L.VB_BYTES) != isinstance(engine, BytesCudaEngine):
+        raise TypeError("byte-string values cross ranks with dist.BytesCudaEngine, and it takes byte-string values only")
+    if isinstance(engine, BytesCudaEngine):
+        _bytes_checks(engine, local_maps, n_map, agg, (L.VB_AGG_GROUP, L.VB_AGG_COGROUP, L.VB_AGG_SORT), rank, world,
+                      exchange_device)
     sh = engine.create(n_map, n_reduce, kcode, vcode, agg, rank, world, key_width=key_width, hint=hint)
     for map_id, keys, vals in local_maps:
         engine.map(sh, map_id, keys, vals)
     p2p = p2p and agg in (L.VB_AGG_GROUP, L.VB_AGG_COGROUP)
+    if isinstance(engine, BytesCudaEngine):       # VB_XCHG_AUTO: NCCL, the one exchange of byte-string values
+        return _exchange(engine, sh, (BytesCudaEngine, _bytes_export, _bytes_import, 0), rank, world, group, stats,
+                         exchange_device, L.VB_XCHG_AUTO)
     return _exchange(engine, sh, (CudaEngine, _rows_export, _rows_import, 0), rank, world, group, stats, exchange_device,
                      L.VB_XCHG_P2P if p2p else L.VB_XCHG_NCCL, p2p and isinstance(engine, CudaEngine))
 
@@ -293,8 +304,15 @@ def run_str_shuffle(engine, local_maps, n_map, n_reduce, vcode, agg, rank, world
     With a communicator on the context the exchange is vb_shuffle_exchange (NCCL inside the library); otherwise
     all_to_all_v of the four columns (exchange_device: "cpu" for a gloo group on a one-GPU box).  agg VB_AGG_SORT
     (sort_by_key) across ranks has no such fallback: its cut keys are agreed in rounds of the library's collectives."""
-    if vcode == L.VB_BYTES:
-        raise TypeError("byte-string values do not cross ranks yet")
+    if (vcode == L.VB_BYTES) != isinstance(engine, StrBytesCudaEngine):
+        raise TypeError("byte-string values cross ranks with dist.StrBytesCudaEngine, and it takes byte-string values only")
+    if isinstance(engine, StrBytesCudaEngine):
+        _bytes_checks(engine, local_maps, n_map, agg, (L.VB_AGG_GROUP, L.VB_AGG_SORT), rank, world, exchange_device)
+        sh = engine.create(n_map, n_reduce, vcode, agg, rank, world, hint=hint)
+        for map_id, keys, vals in local_maps:
+            engine.map(sh, map_id, keys, vals)
+        return _exchange(engine, sh, (StrBytesCudaEngine, _str_bytes_export, _str_bytes_import, 3), rank, world, group, stats,
+                         exchange_device, L.VB_XCHG_AUTO)
     if agg == L.VB_AGG_SORT and world > 1 and not (isinstance(engine, StrCudaEngine) and getattr(engine.sc, "comm", None)
                                                    and exchange_device is None):
         raise ValueError("sort_by_key over String keys across ranks needs the library's communicator (vb_ctx_comm_init, "
@@ -434,6 +452,110 @@ def run_str_combine_shuffle(engine, local_maps, n_map, n_reduce, multi, rank, wo
         engine.map(sh, map_id, keys, cols)
     return _exchange(engine, sh, (StrCombineCudaEngine, _str_combine_export, _str_combine_import, 0), rank, world, group,
                      stats, exchange_device)
+
+
+class BytesCudaEngine:
+    """libvega_b200 on this rank's GPU, for byte-string values with integer keys: CudaEngine's calls over
+    Shuffle.bytes_dist (vb_shuffle_create_bytes_dist; GROUP, COGROUP or SORT).  map takes the values as a sequence of str
+    or bytes, or a StrKeys column.  export gives ((counts, n_val_bytes) per destination, (keys, val_lens, val_bytes)),
+    the wire columns of include/vega_b200.h; import_ takes the same shape, source-rank major.  reduce gives references;
+    gather them with sh.gather."""
+
+    def __init__(self, sc):
+        self.sc = sc
+
+    def create(self, n_map, n_reduce, kcode, vcode, agg, rank, world, key_width=8, hint=0):
+        return Shuffle.bytes_dist(self.sc, n_map, n_reduce, kcode, agg, rank, world, key_width=key_width, hint=hint)
+
+    def map(self, sh, map_id, keys, vals):
+        k = keys if isinstance(keys, _Col) else _Col(keys)
+        v = vals if isinstance(vals, _BytesCol) else _BytesCol(vals)
+        if v.n != k.n:
+            raise ValueError(f"map task {map_id}: {k.n} keys and {v.n} values")
+        sh.map(map_id, k, v, 0, k.n)
+
+    def export(self, sh, world):
+        return sh.export_bytes()
+
+    def import_(self, sh, cols, counts):
+        sh.import_bytes(*cols, *counts)
+
+    def seal(self, sh):
+        sh.seal()
+
+    def reduce(self, sh, r):
+        return sh.reduce(r)
+
+
+class StrBytesCudaEngine:
+    """libvega_b200 on this rank's GPU, for byte-string values with String keys: StrCudaEngine's calls over
+    StrShuffle.bytes_dist (GROUP, or SORT: sort_by_key with a byte-string payload).  map takes str keys (or a StrKeys
+    column) and the values as BytesCudaEngine does.  export gives ((n_keys, n_key_bytes, n_vals, n_val_bytes) per
+    destination, (key_lens, key_bytes, val_counts, val_lens, val_bytes)); import_ takes the same shape, source-rank major.
+    reduce gives references (raw: key offsets and bytes); gather them with sh.gather."""
+
+    def __init__(self, sc):
+        self.sc = sc
+
+    def create(self, n_map, n_reduce, vcode, agg, rank, world, hint=0):
+        return StrShuffle.bytes_dist(self.sc, n_map, n_reduce, rank, world, sort=agg == L.VB_AGG_SORT, hint=hint)
+
+    def map(self, sh, map_id, keys, vals):
+        if not isinstance(keys, (_StrCol, StrKeys)) and len(keys) and not _is_str_keys(keys):
+            raise TypeError("String keys: a sequence of str or a StrKeys column")
+        k = keys if isinstance(keys, _StrCol) else _StrCol(keys)
+        v = vals if isinstance(vals, _BytesCol) else _BytesCol(vals)
+        if v.n != k.n:
+            raise ValueError(f"map task {map_id}: {k.n} keys and {v.n} values")
+        sh.map(map_id, k, v, 0, k.n)
+
+    def export(self, sh, world):
+        return sh.export_bytes()
+
+    def import_(self, sh, cols, counts):
+        sh.import_bytes(*cols, *counts)
+
+    def seal(self, sh):
+        sh.seal()
+
+    def reduce(self, sh, r):
+        return sh.reduce_raw(r)
+
+
+def _bytes_checks(engine, local_maps, n_map, agg, aggs, rank, world, exchange_device):
+    """The bytes engines' refusals, before any device work: an op that computes on values (TypeError), a rank outside
+    the world, map ids outside the rank's block, or a sort without the library's communicator (ValueError)."""
+    if agg not in aggs:
+        raise TypeError(f"agg {agg} computes on values: byte-string values cross ranks for group_by_key, cogroup, the joins "
+                        "and sort_by_key")
+    if not 0 <= rank < world <= 256:
+        raise ValueError(f"rank {rank} of world {world}: 0 <= rank < world <= 256")
+    lo, hi = map_block(rank, world, n_map)
+    ids = [m for m, _, _ in local_maps]
+    if any(not lo <= m < hi for m in ids) or ids != sorted(set(ids)):
+        raise ValueError(f"rank {rank} runs map tasks {ids}: ascending ids in its block [{lo}, {hi}) expected")
+    if agg == L.VB_AGG_SORT and world > 1 and not (getattr(engine.sc, "comm", None) and exchange_device is None):
+        raise ValueError("sort_by_key with byte-string values across ranks needs the library's communicator "
+                         "(Context.comm_init) and runs its exchange inside the library")
+
+
+def _bytes_export(engine, sh, world):
+    (counts, n_val_bytes), cols = engine.export(sh, world)
+    return list(cols), [counts, counts, n_val_bytes]         # keys, value lengths, value bytes
+
+
+def _bytes_import(engine, sh, cols, splits):
+    engine.import_(sh, tuple(cols), (splits[0], splits[2]))
+
+
+def _str_bytes_export(engine, sh, world):
+    (n_keys, n_key_bytes, n_vals, n_val_bytes), cols = engine.export(sh, world)
+    # key lengths, key bytes, value counts, value lengths, value bytes
+    return list(cols), [n_keys, n_key_bytes, n_keys, n_vals, n_val_bytes]
+
+
+def _str_bytes_import(engine, sh, cols, splits):
+    engine.import_(sh, tuple(cols), (splits[0], splits[1], splits[3], splits[4]))
 
 
 def owned_partitions(rank, world, n_reduce):

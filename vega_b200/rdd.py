@@ -335,6 +335,50 @@ class Shuffle:
         L.check(self._lib.vb_shuffle_import_cols(self._h, p(keys), p(accs), accs.shape[0], (ctypes.c_uint64 * len(counts))(*counts)))
 
     @classmethod
+    def bytes_dist(cls, sc, n_map, n_reduce, kcode, agg, rank, world, key_width=8, hint=0):
+        """vb_shuffle_create_bytes_dist: a GROUP / COGROUP / SORT shuffle of byte-string values on rank `rank` of `world`.
+        Map it with byte-string values (a _BytesCol); exchange it with export_bytes / import_bytes (GROUP and COGROUP), or
+        with exchange() when the context has a communicator.  Its results are references, gathered with gather()."""
+        self = cls.__new__(cls)
+        self.sc, self._lib = sc, sc._lib
+        self.n_map, self.n_reduce, self.agg, self.vcode, self.kcode = n_map, n_reduce, agg, L.VB_BYTES, kcode
+        self.rank, self.world = rank, world
+        self.has_payload, self._keepalive = True, []
+        part = L.VB_PART_RANGE if agg == L.VB_AGG_SORT else L.VB_PART_HASH_METRO64
+        h = ctypes.c_void_p()
+        L.check(self._lib.vb_shuffle_create_bytes_dist(sc._h, sc.new_shuffle_id(), n_map, n_reduce, kcode, agg, part, rank, world,
+                                                       ctypes.byref(h)))
+        self._h = h
+        sc._shuffles.add(self)
+        if key_width != 8:
+            L.check(self._lib.vb_shuffle_set_key_width(h, key_width))
+        if hint:
+            L.check(self._lib.vb_shuffle_set_hint(h, hint))
+        return self
+
+    def export_bytes(self):
+        """vb_shuffle_export_bytes_prepare + buffers (bytes_dist, world > 1): ((counts, n_val_bytes), (keys, val_lens,
+        val_bytes)).  The counts are lists with one entry per destination rank; the columns are torch views of the
+        library's device buffers (int64 keys, int32 value lengths, uint8 value bytes), destination-major, valid until seal."""
+        W = self.world
+        cnt, nvb = (ctypes.c_uint64 * W)(), (ctypes.c_uint64 * W)()
+        L.check(self._lib.vb_shuffle_export_bytes_prepare(self._h, cnt, nvb))
+        counts = ([int(x) for x in cnt], [int(x) for x in nvb])
+        ptrs = [ctypes.c_void_p() for _ in range(3)]
+        L.check(self._lib.vb_shuffle_export_bytes_buffers(self._h, *[ctypes.byref(p) for p in ptrs]))
+        n, b = sum(counts[0]), sum(counts[1])
+        return counts, (_dev_view(self, ptrs[0], n, "<i8"), _dev_view(self, ptrs[1], n, "<i4"), _dev_view(self, ptrs[2], b, "|u1"))
+
+    def import_bytes(self, keys, val_lens, val_bytes, counts, n_val_bytes):
+        """vb_shuffle_import_bytes: the received columns (torch CUDA tensors, source-rank major) and what every source rank
+        sent.  The keys are kept alive until seal; the values are copied by the call."""
+        _sync_torch(keys, val_lens, val_bytes)
+        self._keepalive.append(keys)
+        p = lambda t: ctypes.c_void_p(t.data_ptr()) if t.numel() else None
+        arr = lambda c: (ctypes.c_uint64 * len(c))(*c)
+        L.check(self._lib.vb_shuffle_import_bytes(self._h, p(keys), p(val_lens), p(val_bytes), arr(counts), arr(n_val_bytes)))
+
+    @classmethod
     def narrow(cls, parent, out_col, vcode):
         """vb_shuffle_create_narrow: the sealed reduce result `parent` (output column out_col) as a sealed COGROUP side
         under the same partitioner, each key with the one-element list [its result] (vcode: the result's dtype)."""
@@ -1327,6 +1371,18 @@ class _DevView:
         self.__cuda_array_interface__ = {"shape": (n,), "typestr": typestr, "data": (ptr, False), "version": 2}
 
 
+_TORCH_OF = {"<i8": "int64", "<i4": "int32", "|u1": "uint8"}
+
+
+def _dev_view(sh, p, n, typestr):
+    """A torch view of n elements of a device buffer of sh's library (an empty tensor for n = 0 or a NULL pointer)."""
+    import torch
+    dev = f"cuda:{sh._lib.vb_ctx_device(sh.sc._h)}"
+    if n == 0 or not p.value:
+        return torch.empty(0, dtype=getattr(torch, _TORCH_OF[typestr]), device=dev)
+    return torch.as_tensor(_DevView(p.value, n, typestr), device=dev)
+
+
 class StrShuffle(Shuffle):
     """One string-key shuffle (vb_shuffle_create_str; vb_shuffle_create_str_dist for rank `rank` of `world` > 1).
     multi: (value column dtype codes, [(vb_agg, column), ...]) for a combine_by_key shuffle (vb_shuffle_create_str_multi /
@@ -1374,6 +1430,52 @@ class StrShuffle(Shuffle):
         sc._shuffles.add(self)
         if hint:
             L.check(self._lib.vb_shuffle_set_hint(h, hint))
+
+    @classmethod
+    def bytes_dist(cls, sc, n_map, n_reduce, rank, world, sort=False, hint=0):
+        """vb_shuffle_create_str_bytes_dist (GROUP; cogroup and the joins read it), or with sort=True
+        vb_shuffle_create_str_sort_bytes_dist (sort_by_key with a byte-string payload), on rank `rank` of `world`.  Map it
+        with byte-string values; exchange a GROUP one with export_bytes / import_bytes or exchange(), a sort with
+        exchange() only.  Its results are references, gathered with gather()."""
+        self = cls.__new__(cls)
+        self.sc, self._lib = sc, sc._lib
+        self.n_map, self.n_reduce, self.vcode, self.kcode = n_map, n_reduce, L.VB_BYTES, None
+        self.agg = L.VB_AGG_SORT if sort else L.VB_AGG_GROUP
+        self.rank, self.world = rank, world
+        self.has_payload, self._keepalive = True, []
+        h = ctypes.c_void_p()
+        create = self._lib.vb_shuffle_create_str_sort_bytes_dist if sort else self._lib.vb_shuffle_create_str_bytes_dist
+        L.check(create(sc._h, sc.new_shuffle_id(), n_map, n_reduce, rank, world, ctypes.byref(h)))
+        self._h = h
+        sc._shuffles.add(self)
+        if hint:
+            L.check(self._lib.vb_shuffle_set_hint(h, hint))
+        return self
+
+    def export_bytes(self):
+        """vb_shuffle_export_str_bytes_prepare + buffers (bytes_dist GROUP, world > 1): ((n_keys, n_key_bytes, n_vals,
+        n_val_bytes), (key_lens, key_bytes, val_counts, val_lens, val_bytes)).  The counts are lists with one entry per
+        destination rank; the columns are torch views of the library's device buffers (int32 lengths and counts, uint8
+        bytes), destination-major, valid until seal."""
+        W = self.world
+        cs = [(ctypes.c_uint64 * W)() for _ in range(4)]
+        L.check(self._lib.vb_shuffle_export_str_bytes_prepare(self._h, *cs))
+        counts = tuple([int(x) for x in c] for c in cs)
+        ptrs = [ctypes.c_void_p() for _ in range(5)]
+        L.check(self._lib.vb_shuffle_export_str_bytes_buffers(self._h, *[ctypes.byref(p) for p in ptrs]))
+        K, B, V, VB = (sum(c) for c in counts)
+        return counts, (_dev_view(self, ptrs[0], K, "<i4"), _dev_view(self, ptrs[1], B, "|u1"), _dev_view(self, ptrs[2], K, "<i4"),
+                        _dev_view(self, ptrs[3], V, "<i4"), _dev_view(self, ptrs[4], VB, "|u1"))
+
+    def import_bytes(self, key_lens, key_bytes, val_counts, val_lens, val_bytes, n_keys, n_key_bytes, n_vals, n_val_bytes):
+        """vb_shuffle_import_str_bytes: the received columns (torch CUDA tensors, source-rank major) and what every source
+        rank sent.  The key columns are kept alive until seal; the values are copied by the call."""
+        _sync_torch(key_lens, key_bytes, val_counts, val_lens, val_bytes)
+        self._keepalive.append((key_lens, key_bytes, val_counts))
+        p = lambda t: ctypes.c_void_p(t.data_ptr()) if t.numel() else None
+        arr = lambda c: (ctypes.c_uint64 * len(c))(*c)
+        L.check(self._lib.vb_shuffle_import_str_bytes(self._h, p(key_lens), p(key_bytes), p(val_counts), p(val_lens), p(val_bytes),
+                                                      arr(n_keys), arr(n_key_bytes), arr(n_vals), arr(n_val_bytes)))
 
     @classmethod
     def narrow(cls, parent, out_col, vcode):
