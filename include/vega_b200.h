@@ -453,8 +453,9 @@ VB_API int32_t vb_join_n_outer(vb_shuf *const *sides, uint32_t n_sides, uint32_t
  * Limits: fewer than 2^32 - 2 rows per map partition and per shuffle, fewer than 2^31 distinct keys, every key shorter
  * than 2^32 bytes (VB_ERR_TOO_LARGE beyond them).  Key offsets that decrease or exceed n_bytes are VB_ERR_INVALID,
  * for device input too (checked on the device).  Several ranks: vb_shuffle_create_str_dist and the string export /
- * import calls below (vb_shuffle_set_dist with world > 1, the integer export / import / P2P calls and the blob calls
- * return VB_ERR_UNSUPPORTED on a string shuffle); vb_shuffle_set_key_width, the integer map and
+ * import calls below (vb_shuffle_set_dist with world > 1, the integer export / import / P2P calls, the blob calls on a
+ * GROUP shuffle and vb_shuffle_map_blob with world > 1 return VB_ERR_UNSUPPORTED on a string shuffle; the blob calls
+ * of the reduce ops are described with them below); vb_shuffle_set_key_width, the integer map and
  * reduce calls and the join / cogroup calls return VB_ERR_INVALID on a string shuffle (vb_cogroup_n_str / vb_join_n_str
  * below join and cogroup string GROUP shuffles), and the string calls return
  * VB_ERR_INVALID on any other shuffle.  seal / is_sealed / stats / kernel_time / set_hint / free work as for any
@@ -785,10 +786,21 @@ VB_API uint32_t vb_get_partition_str(const void *bytes, uint64_t len, uint32_t n
  * served to, and CPU-produced buckets consumed from, unmodified vega executors:
  *   Vec<(u64,u64)>      = u64 n | n x (u64 k, u64 c)                       (reduce ops, sort)
  *   Vec<(u64,Vec<u64>)> = u64 n | n x (u64 k, u64 len, len x u64)          (group ops)
+ *   Vec<(String,u64)>   = u64 n | n x (u64 len, len key bytes, u64 c)      (string-key SUM / MIN / MAX / COUNT)
  * vb_shuffle_reduce_blob encodes one sealed reduce partition; vb_shuffle_map_blob submits one
  * map-side-COMBINED bucket as the output of map task `map_id` (combiners are merged with
  * merge_combiners, so partial counts are summed).  A blob whose length field disagrees with its
- * size is rejected with VB_ERR_INVALID (the reference's DeserializationError).                   */
+ * size is rejected with VB_ERR_INVALID (the reference's DeserializationError).
+ * String keys (vb_shuffle_create_str / _str_dist with a reduce op): records are unaligned, so a blob
+ * is 8 + 16 n + key bytes long; c is the op's combiner (the value's bits, a u64 count for COUNT).
+ * vb_shuffle_reduce_blob gives the rows of vb_shuffle_reduce_str in the same key order (a partition
+ * this rank does not own: 8 zero bytes); its device destination must be 16-byte aligned
+ * (VB_ERR_INVALID otherwise).  vb_shuffle_map_blob (world == 1 only, VB_ERR_UNSUPPORTED otherwise)
+ * takes any src_loc; a map id may be submitted as rows or as a blob, the last submission wins.
+ * Rejected before any allocation or device work: fewer than 8 bytes, more records than the bytes
+ * can hold, a record whose key or value runs past the end, trailing bytes (VB_ERR_INVALID); a key
+ * of 2^32 bytes or more (VB_ERR_TOO_LARGE).  Key bytes are not UTF-8-validated.  String GROUP,
+ * sort and combine_by_key shuffles and byte-string values return VB_ERR_UNSUPPORTED.            */
 VB_API int32_t vb_shuffle_reduce_blob_size(vb_shuf *s, uint32_t reduce_id, uint64_t *n_bytes);
 VB_API int32_t vb_shuffle_reduce_blob(vb_shuf *s, uint32_t reduce_id, void *out_blob, int32_t dst_loc);
 VB_API int32_t vb_shuffle_map_blob(vb_shuf *s, uint32_t map_id, const void *blob, uint64_t n_bytes, int32_t src_loc);

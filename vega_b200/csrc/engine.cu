@@ -3533,8 +3533,14 @@ extern "C" int32_t vb_shuffle_create_narrow(vb_shuf *p, uint32_t out_col, vb_shu
 // ---------------------------------------------------------------------------------------------
 // bincode blobs (N1)
 // ---------------------------------------------------------------------------------------------
+static u64 str_blob_bytes(const vb_shuf *s, u32 r);
+static int str_reduce_blob_locked(vb_shuf *s, u32 r, unsigned char *dst);
+static int str_map_blob(vb_shuf *s, u32 map_id, const void *blob, u64 n_bytes, int src_loc);
+static int str_blob_check(const vb_shuf *s);
+
 static u64 blob_bytes(const vb_shuf *s, u32 r)
 {
+    if (s->str) return str_blob_bytes(s, r);
     const u64 nk = s->bucket_off[r + 1] - s->bucket_off[r];
     if (is_group_op(s->agg)) return 8 + 16 * nk + 8 * (s->val_off[r + 1] - s->val_off[r]);
     return 8 + 16 * nk;
@@ -3545,7 +3551,7 @@ extern "C" int32_t vb_shuffle_reduce_blob_size(vb_shuf *s, uint32_t r, uint64_t 
     if (s && s->vdt == VB_BYTES) return reject_bytes(s, "vb_shuffle_reduce_blob_size");
     if (!s || !n_bytes) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "bincode blobs");
-    if (s->str) return reject_str(s, "bincode blobs");
+    if (s->str) TRY(str_blob_check(s));
     if (r >= s->n_reduce) return set_err(VB_ERR_INVALID, "reduce_id %u >= n_reduce %u", r, s->n_reduce);
     TRY(wait_sealed(s));
     if (s->lazy) {
@@ -3562,9 +3568,11 @@ extern "C" int32_t vb_shuffle_reduce_blob(vb_shuf *s, uint32_t r, void *out_blob
     if (s && s->vdt == VB_BYTES) return reject_bytes(s, "vb_shuffle_reduce_blob");
     if (!s || !out_blob) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "bincode blobs");
-    if (s->str) return reject_str(s, "bincode blobs");
+    if (s->str) TRY(str_blob_check(s));
     if (r >= s->n_reduce) return set_err(VB_ERR_INVALID, "reduce_id %u >= n_reduce %u", r, s->n_reduce);
     if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
+    if (s->str && dst_loc == VB_DEVICE && ((uintptr_t)out_blob & 15))
+        return set_err(VB_ERR_INVALID, "a string-key blob's device destination must be 16-byte aligned");
     TRY(wait_sealed(s));
     vb_ctx *c = s->ctx;
     std::lock_guard<std::mutex> lk(c->mu);
@@ -3576,7 +3584,9 @@ extern "C" int32_t vb_shuffle_reduce_blob(vb_shuf *s, uint32_t r, void *out_blob
     u64 *dst = (u64 *)out_blob;
     if (dst_loc == VB_HOST) { TRY(tmp.alloc(bytes)); dst = tmp.as<u64>(); }
     const unsigned grid = (unsigned)std::min<u64>(std::max<u64>(1, (std::max(nk, s->val_off[r + 1] - s->val_off[r]) + 255) / 256), (u64)c->sm_count * 8);
-    {
+    if (s->str) {
+        TRY(str_reduce_blob_locked(s, r, (unsigned char *)dst));
+    } else {
         KLaunch kl(s, K_MISC);
         if (is_group_op(s->agg)) {
             if (nk) blob_group_kernel<<<grid, 256, 0, c->stream>>>(s->res_keys + b0, s->res_offs + b0, nk, s->res_vals, dst);
@@ -3597,7 +3607,12 @@ extern "C" int32_t vb_shuffle_map_blob(vb_shuf *s, uint32_t map_id, const void *
     if (s && s->vdt == VB_BYTES) return reject_bytes(s, "vb_shuffle_map_blob");
     if (!s || !blob) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "bincode blobs");
-    if (s->str) return reject_str(s, "bincode blobs");
+    if (s->str) {
+        TRY(str_blob_check(s));
+        if (s->world > 1) return reject_str(s, "vb_shuffle_map_blob across ranks (map tasks cross ranks through the exchange)");
+        if (src_loc < VB_HOST || src_loc > VB_DEVICE_BORROWED) return set_err(VB_ERR_INVALID, "bad src_loc");
+        return str_map_blob(s, map_id, blob, n_bytes, src_loc);
+    }
     if (src_loc < VB_HOST || src_loc > VB_DEVICE_BORROWED) return set_err(VB_ERR_INVALID, "bad src_loc");
     if (s->agg == VB_AGG_SORT) return set_err(VB_ERR_UNSUPPORTED, "sort_by_key takes rows, not combined buckets");
     if (n_bytes < 8 || (n_bytes & 7)) return set_err(VB_ERR_INVALID, "corrupted blob: %llu bytes", (unsigned long long)n_bytes);
@@ -4389,6 +4404,7 @@ struct StrState {
     struct Cols { const u64 *c[MA_MAX_COLS]; };
     std::vector<Cols> cols;               // reduce ops and combine_by_key, per map id: the value columns of the spec
     std::vector<char> vals_owned;         // per map id: vals / cols are copies (else borrowed, VB_DEVICE_BORROWED)
+    std::vector<char> blob;               // per map id: a bincode blob's partials in vals (vb_shuffle_map_blob), not rows
     u64 *key_off = nullptr;               // [n_keys + 1] byte offset of every result key (partition-major, from 0)
     unsigned char *key_bytes = nullptr;   // the result keys' bytes
     std::vector<u64> kb_off;              // [n_reduce + 1] first key byte of each partition
@@ -4443,6 +4459,7 @@ static void free_str_map(vb_shuf *s, u32 m)
     t->vals[m] = nullptr;
     t->cols[m] = StrState::Cols{};
     t->vals_owned[m] = 0;
+    t->blob[m] = 0;
 }
 
 static void free_str_dict(vb_shuf *s)
@@ -4495,6 +4512,7 @@ static StrState *str_attach(vb_shuf *s)
     t->vals.assign(s->n_map, nullptr);
     t->cols.assign(s->n_map, StrState::Cols{});
     t->vals_owned.assign(s->n_map, 0);
+    t->blob.assign(s->n_map, 0);
     t->d.fp_mask = str_fp_mask();
     s->str = t;
     return t;
@@ -4698,17 +4716,18 @@ static int str_encode(vb_shuf *s, const u64 *offs, const unsigned char *bytes, u
 // (a NULL column is neither read nor copied), copied, or borrowed for VB_DEVICE_BORROWED.  A single-column shuffle
 // passes its one column (none for COUNT), a combine_by_key shuffle every column an aggregate reads.  Reduce ops keep
 // them as the spec's value columns (cols), GROUP as its values (vals).
-static int str_map(vb_shuf *s, u32 map_id, const uint64_t *key_offsets, const void *key_bytes, u64 n_bytes, const u64 *const *in, u32 n_in,
-                   u64 n, int loc, DevBuf *own_vals = nullptr)
+static int str_map_state(vb_shuf *s)
 {
-    {
-        std::lock_guard<std::mutex> g(s->mu);
-        if (s->sealed || s->sealing || s->freed) return set_err(VB_ERR_STATE, "shuffle %llu: map after seal", (unsigned long long)s->id);
-        if (s->exported) return set_err(VB_ERR_STATE, "shuffle %llu: map after export", (unsigned long long)s->id);
-    }
+    std::lock_guard<std::mutex> g(s->mu);
+    if (s->sealed || s->sealing || s->freed) return set_err(VB_ERR_STATE, "shuffle %llu: map after seal", (unsigned long long)s->id);
+    if (s->exported) return set_err(VB_ERR_STATE, "shuffle %llu: map after export", (unsigned long long)s->id);
+    return VB_OK;
+}
+
+static int str_map_locked(vb_shuf *s, u32 map_id, const uint64_t *key_offsets, const void *key_bytes, u64 n_bytes, const u64 *const *in,
+                          u32 n_in, u64 n, int loc, DevBuf *own_vals)
+{
     vb_ctx *c = s->ctx;
-    std::lock_guard<std::mutex> lk(c->mu);
-    CU(cudaSetDevice(c->device));
     KLaunch call(s, -1);
     StrState *t = s->str;
     u64 others = 0;
@@ -4767,6 +4786,120 @@ static int str_map(vb_shuf *s, u32 map_id, const uint64_t *key_offsets, const vo
     s->st.rows_in += n;
     CU(cudaStreamSynchronize(c->stream));          // the caller's key column is free again when the call returns
     TRY(call.done("map"));
+    return VB_OK;
+}
+
+static int str_map(vb_shuf *s, u32 map_id, const uint64_t *key_offsets, const void *key_bytes, u64 n_bytes, const u64 *const *in, u32 n_in,
+                   u64 n, int loc, DevBuf *own_vals = nullptr)
+{
+    TRY(str_map_state(s));
+    vb_ctx *c = s->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    return str_map_locked(s, map_id, key_offsets, key_bytes, n_bytes, in, n_in, n, loc, own_vals);
+}
+
+// ---- bincode blobs of string reduce ops (Vec<(String, C)>; strkeys.cuh, str_blob_encode_kernel) -------------------
+static unsigned str_grid(const vb_ctx *c, u64 x);
+
+// String GROUP and sort shuffles have no blob format yet: a GROUP's Vec<(String, Vec<V>)> would need its own encoder,
+// and a sort takes rows, not combined buckets
+static int str_blob_check(const vb_shuf *s)
+{
+    if (s->str->sort || !is_reduce_op(s->agg)) return reject_str(s, "bincode blobs of a GROUP or sort shuffle");
+    return VB_OK;
+}
+
+static u64 str_blob_bytes(const vb_shuf *s, u32 r)
+{
+    return 8 + 16 * (s->bucket_off[r + 1] - s->bucket_off[r]) + (s->str->kb_off[r + 1] - s->str->kb_off[r]);
+}
+
+// Partition r's blob into dst (device, 16-byte aligned): one output-driven kernel; an empty partition is 8 zero bytes.
+// The caller holds c->mu.
+static int str_reduce_blob_locked(vb_shuf *s, u32 r, unsigned char *dst)
+{
+    vb_ctx *c = s->ctx;
+    const StrState *t = s->str;
+    const u64 b0 = s->bucket_off[r], nk = s->bucket_off[r + 1] - b0, bytes = str_blob_bytes(s, r);
+    KLaunch kl(s, K_MISC, nk);
+    if (nk) str_blob_encode_kernel<<<str_grid(c, (bytes + 15) / 16), 256, 0, c->stream>>>(t->key_off + b0, t->key_bytes, s->res_cols + b0, nk, bytes, dst);
+    else CU(cudaMemsetAsync(dst, 0, 8, c->stream));
+    return kl.done("str_blob_encode_kernel");
+}
+
+// One map task's combined bucket Vec<(String, C)> of a string reduce op (world == 1).  The host walks the length
+// fields (each record's position depends on the lengths before it) and rejects a malformed blob before allocating or
+// launching anything; then the blob and its u32 key lengths go to the device, a scan gives the key offsets, and
+// str_blob_decode_kernel writes the key bytes and the partials column.  The keys are encoded as a map call's are, and
+// the partials kept as the map task's (blob[m]: the seal merges them with the import spec, as it does received
+// partials).  A blob replaces an earlier submission of the map id, rows or blob, and rows replace a blob.
+static int str_map_blob(vb_shuf *s, u32 map_id, const void *blob, u64 n_bytes, int src_loc)
+{
+    if (map_id >= s->n_map) return set_err(VB_ERR_INVALID, "map_id %u >= n_map %u", map_id, s->n_map);
+    if (n_bytes < 8) return set_err(VB_ERR_INVALID, "corrupted blob: %llu bytes", (unsigned long long)n_bytes);
+    vb_ctx *c = s->ctx;
+    std::vector<unsigned char> host;
+    const unsigned char *b = (const unsigned char *)blob;
+    if (src_loc != VB_HOST) {
+        host.resize(n_bytes);
+        std::lock_guard<std::mutex> lk(c->mu);
+        CU(cudaSetDevice(c->device));
+        CU(cudaMemcpyAsync(host.data(), blob, n_bytes, cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaStreamSynchronize(c->stream));
+        b = host.data();
+    }
+    u64 n = 0;
+    memcpy(&n, b, 8);
+    if (n > (n_bytes - 8) / 16) return set_err(VB_ERR_INVALID, "corrupted blob: %llu records in %llu bytes", (unsigned long long)n, (unsigned long long)n_bytes);
+    std::vector<u32> lens(n);
+    u64 pos = 8;
+    for (u64 i = 0; i < n; ++i) {
+        if (n_bytes - pos < 16) return set_err(VB_ERR_INVALID, "corrupted blob: record %llu runs past the end", (unsigned long long)i);
+        u64 len = 0;
+        memcpy(&len, b + pos, 8);
+        if (len > n_bytes - pos - 16) return set_err(VB_ERR_INVALID, "corrupted blob: record %llu has a key of %llu bytes", (unsigned long long)i, (unsigned long long)len);
+        if (len >= (1ull << 32)) return set_err(VB_ERR_TOO_LARGE, "a key of 2^32 bytes or more");
+        lens[i] = (u32)len;
+        pos += 16 + len;
+    }
+    if (pos != n_bytes) return set_err(VB_ERR_INVALID, "corrupted blob: %llu trailing bytes", (unsigned long long)(n_bytes - pos));
+    if (n >= 0xFFFFFFFEull) return set_err(VB_ERR_TOO_LARGE, "map partition of %llu rows", (unsigned long long)n);
+    TRY(str_map_state(s));
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    const u64 nkb = n_bytes - 8 - 16 * n;
+    DevBuf d_blob(c), d_lens(c), wide(c), koff(c), kbytes(c), vals(c);
+    if (n) {
+        const unsigned char *db = (const unsigned char *)blob;
+        if (src_loc == VB_HOST) {
+            TRY(d_blob.alloc(n_bytes));
+            CU(cudaMemcpyAsync(d_blob.p, blob, n_bytes, cudaMemcpyHostToDevice, c->stream));
+            s->st.h2d_bytes += n_bytes;
+            db = d_blob.as<unsigned char>();
+        }
+        TRY(d_lens.alloc(n * 4));
+        CU(cudaMemcpyAsync(d_lens.p, lens.data(), n * 4, cudaMemcpyHostToDevice, c->stream));
+        s->st.h2d_bytes += n * 4;
+        TRY(wide.alloc(n * 8));
+        TRY(koff.alloc((n + 1) * 8));
+        {
+            KLaunch kl(s, K_MISC, n);
+            str_widen_u32_kernel<<<str_grid(c, n), 256, 0, c->stream>>>(d_lens.as<u32>(), n, wide.as<u64>());
+            TRY(kl.done("str_widen_u32_kernel"));
+        }
+        TRY(exclusive_scan_u64(s, wide.as<u64>(), koff.as<u64>(), n, koff.as<u64>() + n));
+        TRY(kbytes.alloc((nkb + 15) & ~15ull));
+        TRY(vals.alloc(n * 8));
+        {
+            KLaunch kl(s, K_MISC, n);
+            str_blob_decode_kernel<<<str_grid(c, std::max<u64>(n, (nkb + 15) / 16)), 256, 0, c->stream>>>(db, koff.as<u64>(), n, kbytes.as<unsigned char>(),
+                                                                                                      vals.as<u64>());
+            TRY(kl.done("str_blob_decode_kernel"));
+        }
+    }
+    TRY(str_map_locked(s, map_id, koff.as<u64>(), kbytes.p, nkb, nullptr, 0, n, VB_DEVICE, &vals));
+    s->str->blob[map_id] = 1;
     return VB_OK;
 }
 
@@ -5051,19 +5184,22 @@ static int str_reduce_rows(vb_shuf *s, int opk, int tx, const u32 *ids, const u6
 }
 
 // Rows as dictionary entry ids and their values: one map task's, or the rows a rank imported.  Reduce ops and
-// combine_by_key: a map task's value columns in cols, or the imported accumulators [n_acc][n] in vals.
+// combine_by_key: a map task's value columns in cols (in = IN_SOA), or partials [n_acc][n] in vals (IN_ACCS): the
+// accumulators a rank imported, or a map task's bincode blob.
 struct StrRun {
     const u32 *ids;
     const u64 *vals;
     u64 n;
     StrState::Cols cols{};
+    int in = IN_SOA;
 };
 
 static std::vector<StrRun> str_map_runs(const vb_shuf *s)
 {
     std::vector<StrRun> runs;
     for (u32 m = 0; m < s->n_map; ++m)
-        if (s->maps[m].n_rows) runs.push_back(StrRun{s->str->ids[m], s->str->vals[m], s->maps[m].n_rows, s->str->cols[m]});
+        if (s->maps[m].n_rows)
+            runs.push_back(StrRun{s->str->ids[m], s->str->vals[m], s->maps[m].n_rows, s->str->cols[m], s->str->blob[m] ? IN_ACCS : IN_SOA});
     return runs;
 }
 
@@ -5158,23 +5294,25 @@ static int str_dense_keys(vb_shuf *s, const std::vector<StrRun> &runs, const std
 }
 
 // Reduce ops and combine_by_key: acc [n_acc][D] = every accumulator of the spec folded over the rows of `runs`, by
-// dense id, in the spec's order transform (IN_SOA: the map rows and the map spec; IN_ACCS: imported partials and the
-// merge spec).  A spec of one accumulator (every reduce op, and a combine of one aggregate) folds with
+// dense id, in the spec's order transform, each run with the spec of its input kind (IN_SOA: the map rows and the map
+// spec; IN_ACCS: partials and the import spec, whose merge ops have the map ops' identities).  A spec of one accumulator (every reduce op, and a combine of one aggregate) folds with
 // str_reduce_kernel, whose 26-28 registers keep about twice the warps of str_reduce_multi_kernel resident (DESIGN
 // §3.5, §5.2).
 __global__ void range_kernel(u64 *__restrict__ out, u64 start, u64 step, u64 n);
 
-static int str_fold_multi(vb_shuf *s, const std::vector<StrRun> &runs, int in, const u32 *dense, u64 D, DevBuf &acc)
+static int str_fold_multi(vb_shuf *s, const std::vector<StrRun> &runs, const u32 *dense, u64 D, DevBuf &acc)
 {
     vb_ctx *c = s->ctx;
-    const AccSpec &sp = in == IN_ACCS ? s->acc_imp : s->acc_map;
-    TRY(acc.alloc(D * 8 * sp.n));
-    for (u32 a = 0; a < sp.n; ++a) {
+    const AccSpec &ms = s->acc_map;
+    TRY(acc.alloc(D * 8 * ms.n));
+    for (u32 a = 0; a < ms.n; ++a) {
         KLaunch kl(s, K_MISC);
-        str_fill_kernel<<<str_grid(c, D), 256, 0, c->stream>>>(acc.as<u64>() + (u64)a * D, D, op_identity(spec_at(sp.op, a)));
+        str_fill_kernel<<<str_grid(c, D), 256, 0, c->stream>>>(acc.as<u64>() + (u64)a * D, D, op_identity(spec_at(ms.op, a)));
         TRY(kl.done("str_fill_kernel"));
     }
     for (const StrRun &r : runs) {
+        const int in = r.in;
+        const AccSpec &sp = in == IN_ACCS ? s->acc_imp : s->acc_map;
         if (sp.n == 1) {               // a COUNT reads no column (its c[0] may be NULL)
             const u64 *vals = in == IN_ACCS ? r.vals : r.cols.c[spec_at(sp.src, 0)];
             TRY(str_reduce_rows(s, spec_at(sp.op, 0), spec_at(sp.tx, 0), r.ids, vals, r.n, dense, acc.as<u64>()));
@@ -5254,11 +5392,11 @@ static int str_group_values(vb_shuf *s, const std::vector<StrRun> &runs, u64 n, 
 //   1. mark the entries the rows reference;
 //   2. split the live entries by h % n_reduce into partition-major dense ids, and lay their bytes out in that order;
 //   3. reduce ops and combine_by_key: one RED per (warp, distinct id) into acc[accumulator][dense id] for every
-//      accumulator of the spec (`in`: map rows or imported partials), then the output columns;  GROUP: the rows in
+//      accumulator of the spec (each run's `in`: map rows, or imported or blob partials), then the output columns;  GROUP: the rows in
 //      run order (map-id order, or source-rank major), stably sorted by dense id, then the CSR (seal_group's steps
 //      4-7).
 // The per-map ids and the dictionary are freed at the end.
-static int seal_str_runs(vb_shuf *s, const std::vector<StrRun> &runs, int in = IN_SOA)
+static int seal_str_runs(vb_shuf *s, const std::vector<StrRun> &runs)
 {
     vb_ctx *c = s->ctx;
     StrState *t = s->str;
@@ -5278,7 +5416,7 @@ static int seal_str_runs(vb_shuf *s, const std::vector<StrRun> &runs, int in = I
         TRY(str_read_at(s, koff.as<u64>(), s->bucket_off, t->kb_off));
         if (is_reduce_op(s->agg)) {    // fold every accumulator, then the output columns
             DevBuf acc(c), out(c);
-            TRY(str_fold_multi(s, runs, in, dense.as<u32>(), D, acc));
+            TRY(str_fold_multi(s, runs, dense.as<u32>(), D, acc));
             TRY(str_finalize_multi(s, acc.as<u64>(), D, out));
             s->res_cols = (u64 *)out.release();
             s->st.rows_out = D;
@@ -5659,7 +5797,7 @@ static int export_str_locked(vb_shuf *s, u64 *n_keys, u64 *n_key_bytes, u64 *n_v
         }
         if (is_reduce_op(s->agg)) {
             DevBuf acc(c);
-            TRY(str_fold_multi(s, runs, IN_SOA, dense.as<u32>(), D, acc));
+            TRY(str_fold_multi(s, runs, dense.as<u32>(), D, acc));
             for (u32 a = 0; a < s->acc_map.n; ++a) {
                 const int tx = spec_at(s->acc_map.tx, a);
                 if (tx == TX_NONE) continue;
@@ -5759,14 +5897,14 @@ static int seal_str_import(vb_shuf *s)
                 runs.push_back(StrRun{row_ids.as<u32>(), t->i_vals, nv});
             }
         } else {
-            runs.push_back(StrRun{ids.as<u32>(), t->i_vals, nk});
+            runs.push_back(StrRun{ids.as<u32>(), t->i_vals, nk, {}, IN_ACCS});
         }
     }
     if (t->sort) {
         if (s->sort_part_rows.size() != s->n_reduce) return set_err(VB_ERR_STATE, "sort_by_key over string keys across ranks goes through vb_shuffle_exchange");
         TRY(seal_str_sort(s, runs, &s->sort_part_rows));
     } else {
-        TRY(seal_str_runs(s, runs, IN_ACCS));
+        TRY(seal_str_runs(s, runs));
     }
     free_str_xchg(s);
     return VB_OK;

@@ -761,4 +761,97 @@ __global__ void str_sort_cuts_at_kernel(const u64 *__restrict__ roff, u64 D, con
     rank_cut[p] = lo;
 }
 
+// ---- bincode blobs of string reduce ops (engine.cu, vb_shuffle_reduce_blob / vb_shuffle_map_blob) ----------------
+// Vec<(String, u64)>: u64 n, then per record u64 len | len key bytes | u64 value, unaligned.  Record i starts at
+// 8 + 16 i + (key_off[i] - key_off[0]), so the key offsets place every record without a scan.  Both kernels are
+// output-driven: a thread assembles one aligned 16-byte chunk of its destination from shifted aligned loads (load_le)
+// and stores it once.
+
+// x with its byte 0 at byte d of a word: the part of x that lands in the word (none when |d| >= 8)
+VB_D u64 place_le(u64 x, i64 d)
+{
+    if (d <= -8 || d >= 8) return 0;
+    return d >= 0 ? x << (8 * d) : x >> (-8 * d);
+}
+
+// Bytes [p, p + 8) of a blob from the record that starts at st, whose key is the len bytes at kb + ksrc and whose value
+// is v (zero where the record has no byte)
+VB_D u64 blob_record_word(u64 p, u64 st, u64 len, const unsigned char *kb, u64 ksrc, u64 v)
+{
+    const u64 k0 = st + 8, k1 = k0 + len;
+    u64 w = place_le(len, (i64)(st - p)) | place_le(v, (i64)(k1 - p));
+    const u64 a = p > k0 ? p : k0, b = p + 8 < k1 ? p + 8 : k1;
+    if (a < b) w |= load_le<false>(kb, ksrc + (a - k0), (u32)(b - a)) << (8 * (a - p));
+    return w;
+}
+
+// One partition's blob (n_bytes = 8 + 16 nk + key bytes, nk >= 1) into out (16-byte aligned).  key_off [nk + 1]: the
+// partition's offsets into key_bytes (key_off[0] need not be 0); vals [nk]: its values.  The first record that reaches
+// chunk p is the last one starting at or before p (a binary search over the closed-form starts; record i starts at or
+// after 8 + 16 i, so i < p / 16).  Records are at least 16 bytes long, so only it and the next reach the chunk.  The
+// last chunk is stored in pieces when the blob does not end on a 16-byte boundary.
+__global__ void str_blob_encode_kernel(const u64 *__restrict__ key_off, const unsigned char *__restrict__ key_bytes,
+                                       const u64 *__restrict__ vals, u64 nk, u64 n_bytes, unsigned char *__restrict__ out)
+{
+    const u64 kb0 = key_off[0], n_chunks = (n_bytes + 15) / 16;
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 q = (u64)blockIdx.x * blockDim.x + threadIdx.x; q < n_chunks; q += stride) {
+        const u64 p = 16 * q;
+        u64 lo = 0, hi = p / 16 < nk ? p / 16 : nk;
+        while (hi - lo > 1) {
+            const u64 mid = (lo + hi) >> 1;
+            if (8 + 16 * mid + (key_off[mid] - kb0) <= p) lo = mid; else hi = mid;
+        }
+        u64 w0 = p == 0 ? nk : 0, w1 = 0;
+        for (u64 i = lo; i < lo + 2 && i < nk; ++i) {
+            const u64 ko = key_off[i], len = key_off[i + 1] - ko, st = 8 + 16 * i + (ko - kb0);
+            if (st >= p + 16) break;
+            const u64 v = vals[i];
+            w0 |= blob_record_word(p, st, len, key_bytes, ko, v);
+            w1 |= blob_record_word(p + 8, st, len, key_bytes, ko, v);
+        }
+        if (p + 16 <= n_bytes) {
+            *(ulonglong2 *)(out + p) = make_ulonglong2(w0, w1);
+            continue;
+        }
+        u64 at = p, rest = n_bytes - p, w = w0;    // 1..15 bytes: 8, 4, 2, 1 in turn keep every store aligned
+        if (rest >= 8) { *(u64 *)(out + at) = w0; at += 8; rest -= 8; w = w1; }
+        if (rest & 4) { *(u32 *)(out + at) = (u32)w; at += 4; w >>= 32; }
+        if (rest & 2) { *(unsigned short *)(out + at) = (unsigned short)w; at += 2; w >>= 16; }
+        if (rest & 1) out[at] = (unsigned char)w;
+    }
+}
+
+// The inverse, over a blob of n >= 1 records whose key lengths the host walk checked: koff [n + 1] (the scanned
+// lengths) → the key bytes, contiguous (out_bytes padded to whole 16-byte chunks), and the values.  Key byte j of record
+// i sits at blob offset 16 + 16 i + j and its value at 16 + 16 i + koff[i + 1].  A chunk starts in the last record with
+// koff[i] <= j0 (which skips empty keys) and walks forward through the records that end inside it.
+__global__ void str_blob_decode_kernel(const unsigned char *__restrict__ blob, const u64 *__restrict__ koff, u64 n,
+                                       unsigned char *__restrict__ out_bytes, u64 *__restrict__ out_vals)
+{
+    const u64 nkb = koff[n], n_chunks = (nkb + 15) / 16, total = n_chunks > n ? n_chunks : n;
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 t = (u64)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += stride) {
+        if (t < n) out_vals[t] = load_le<false>(blob, 16 + 16 * t + koff[t + 1], 8);
+        if (t >= n_chunks) continue;
+        const u64 j0 = 16 * t, j1 = j0 + 16 < nkb ? j0 + 16 : nkb;
+        u64 lo = 0, hi = n;
+        while (hi - lo > 1) {
+            const u64 mid = (lo + hi) >> 1;
+            if (koff[mid] <= j0) lo = mid; else hi = mid;
+        }
+        u64 w[2] = {0, 0};
+        for (u64 i = lo, j = j0; j < j1; ++i) {                  // [j, e): the part of record i's key in the chunk
+            const u64 e = koff[i + 1] < j1 ? koff[i + 1] : j1;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const u64 lo_h = j0 + 8 * h, a = j > lo_h ? j : lo_h, b = e < lo_h + 8 ? e : lo_h + 8;
+                if (a < b) w[h] |= load_le<false>(blob, 16 + 16 * i + a, (u32)(b - a)) << (8 * (a - lo_h));
+            }
+            j = e;
+        }
+        *(ulonglong2 *)(out_bytes + j0) = make_ulonglong2(w[0], w[1]);
+    }
+}
+
 }  // namespace vb

@@ -506,6 +506,17 @@ class Shuffle:
         L.check(self._lib.vb_shuffle_reduce_blob(self._h, r, buf.ctypes.data_as(ctypes.c_void_p), L.VB_HOST))
         return buf.tobytes()
 
+    def reduce_blob_device(self, r, out):
+        """Same, into a caller-provided torch CUDA uint8 tensor of reduce_blob_size(r) bytes (16-byte aligned for a
+        string-key shuffle)."""
+        _sync_torch(out)
+        L.check(self._lib.vb_shuffle_reduce_blob(self._h, r, ctypes.c_void_p(out.data_ptr()), L.VB_DEVICE))
+
+    def reduce_blob_size(self, r):
+        n = ctypes.c_uint64()
+        L.check(self._lib.vb_shuffle_reduce_blob_size(self._h, r, ctypes.byref(n)))
+        return n.value
+
     def map_blob(self, map_id, blob):
         """Submit one map-side-combined bucket (bincode blob, bytes) as the output of map task `map_id`."""
         buf = np.frombuffer(blob, dtype=np.uint8)
