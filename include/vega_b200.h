@@ -712,6 +712,51 @@ VB_API int32_t vb_shuffle_create_str_sort_bytes(vb_ctx *ctx, uint64_t shuffle_id
 VB_API int32_t vb_shuffle_gather_bytes_size(vb_shuf *s, const uint64_t *refs, uint64_t n, int32_t src_loc, uint64_t *n_bytes);
 VB_API int32_t vb_shuffle_gather_bytes(vb_shuf *s, const uint64_t *refs, uint64_t n, int32_t src_loc,
                                        uint64_t *out_offsets /*n+1, from 0*/, void *out_bytes, int32_t dst_loc);
+/* ---- repartition(n) = coalesce(n, shuffle = true) (Rdd::coalesce, src/rdd/rdd.rs:386-418): any item, spread evenly ----
+ * The map task of parent partition m gives its items the positions start_m + 1 + i (i = 0, 1, ...; u64 arithmetic mod
+ * 2^64), and item i goes to reduce partition vb_get_partition(position, 8, n_reduce), as vega's HashPartitioner::<usize>
+ * places it.  start_m is vega's own draw (rdd.rs:393-398), made by the caller; the library draws nothing.  The library
+ * fixes the order that vega leaves to a HashMap: partition r holds its items in map-id order, then input order (a stable
+ * split), which is one of the orders vega can produce.
+ * Items are only moved, never read: n_cols (0 to 2) 64-bit columns, plus one byte-string column if has_bytes (a String
+ * as its UTF-8 bytes, any T: Serialize as its bincode bytes); at least one column in all, else VB_ERR_INVALID.
+ *   create  vb_shuffle_create_repartition: one process.  n_reduce 1 .. 65536 (VB_ERR_INVALID for 0, VB_ERR_UNSUPPORTED
+ *           above).  has_bytes is 0 or 1.  vb_shuffle_create_repartition_dist is the same for rank `rank` of `world`
+ *           (1 <= world <= 256, rank < world, VB_ERR_INVALID otherwise; world 1 is the one-process create).  Rank r owns
+ *           the partitions p with p % world == r; map ids are assigned in contiguous blocks by rank, and each rank maps its
+ *           own block (the maps it never submits are empty).
+ *   exchange  world > 1: vb_shuffle_exchange with VB_XCHG_AUTO or VB_XCHG_NCCL (needs vb_ctx_comm_init) between the map
+ *           calls and the seal: each partition's items go to their owner, which keeps them in source-rank order, i.e.
+ *           map-id order.  VB_XCHG_P2P is VB_ERR_UNSUPPORTED, an exchange of a world-1 shuffle VB_ERR_STATE.  Ranks that
+ *           disagree on n_cols or has_bytes, or a rank that would receive 2^32 - 2 items or more, make every rank return
+ *           the same code (VB_ERR_INVALID / VB_ERR_TOO_LARGE) before any send; each shuffle can still be freed.  A seal
+ *           before the exchange, or a map call after it, is VB_ERR_STATE.
+ *   map     vb_shuffle_map_repartition: map task map_id, its items' positions from first_position + 1.  The 64-bit
+ *           columns cols[n_cols] follow vb_shuffle_map_soa's rules, VB_DEVICE_BORROWED included (read until seal); the
+ *           bytes follow vb_shuffle_map_bytes's rules (Arrow-style offsets, always copied, the same offset checks and
+ *           2^32-byte limit; ignored without has_bytes).  Re-submitting a map_id replaces it.  A map task of 2^32 - 2
+ *           items or more, or a shuffle of as many, is VB_ERR_TOO_LARGE.
+ *   seal    vb_shuffle_seal, once every map id was submitted (VB_ERR_STATE otherwise).
+ *   reduce  vb_shuffle_reduce_repartition_size gives partition r's items and, with has_bytes, their total bytes;
+ *           vb_shuffle_reduce_repartition writes out_cols[k] (n_rows words each), out_offsets [n_rows + 1] (from 0) and
+ *           out_bytes, item i's bytes at out_bytes[out_offsets[i] .. [i + 1]), to dst_loc (VB_HOST or VB_DEVICE; a device
+ *           out_bytes may have any alignment).  Any output may be NULL to skip it, except out_bytes when the partition has
+ *           bytes and the offsets or bytes are asked for (VB_ERR_INVALID, nothing written).  Both block until s is sealed.
+ *   refused VB_ERR_INVALID before any device work, the shuffle staying usable: the repartition calls on any other
+ *           shuffle; on a repartition shuffle every other map call (vb_shuffle_map_soa / _aos / _cols / _bytes / _str* /
+ *           _blob), reduce call (vb_shuffle_reduce* / _blob*), join, cogroup, narrow, gather and export / import call,
+ *           vb_shuffle_set_key_width and vb_shuffle_set_dist.  Seal, stats, kernel_time and free work as for
+ *           any shuffle.  A partition a rank does not own has 0 items.                                                    */
+VB_API int32_t vb_shuffle_create_repartition(vb_ctx *ctx, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce, uint32_t n_cols,
+                                             int32_t has_bytes, vb_shuf **out);
+VB_API int32_t vb_shuffle_create_repartition_dist(vb_ctx *ctx, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce, uint32_t n_cols,
+                                                  int32_t has_bytes, uint32_t rank, uint32_t world, vb_shuf **out);
+VB_API int32_t vb_shuffle_map_repartition(vb_shuf *s, uint32_t map_id, uint64_t first_position, const void *const *cols /*n_cols*/,
+                                          const uint64_t *val_offsets /*n_rows+1*/, const void *val_bytes, uint64_t n_val_bytes,
+                                          uint64_t n_rows, int32_t src_loc);
+VB_API int32_t vb_shuffle_reduce_repartition_size(vb_shuf *s, uint32_t r, uint64_t *n_rows, uint64_t *n_bytes);
+VB_API int32_t vb_shuffle_reduce_repartition(vb_shuf *s, uint32_t r, void *const *out_cols /*n_cols*/,
+                                             uint64_t *out_offsets /*n_rows+1, from 0*/, void *out_bytes, int32_t dst_loc);
 /* ---- byte-string values across ranks: each value's bytes are sent once, never its reference --------------------------
  * vb_shuffle_create_bytes_dist        vb_shuffle_create(key_dtype, VB_BYTES, agg, part) for rank `rank` of `world`:
  *                                     agg VB_AGG_GROUP / VB_AGG_COGROUP / VB_AGG_SORT (a reduce op or COUNT is

@@ -163,6 +163,17 @@ extern "C" {
     pub fn vb_shuffle_gather_bytes_size(s: *mut vb_shuf, refs: *const u64, n: u64, src_loc: i32, n_bytes: *mut u64) -> i32;
     pub fn vb_shuffle_gather_bytes(s: *mut vb_shuf, refs: *const u64, n: u64, src_loc: i32, out_offsets: *mut u64,
                                    out_bytes: *mut c_void, dst_loc: i32) -> i32;
+    // repartition(n) = coalesce(n, shuffle = true): items of 0-2 u64 columns plus optional bytes, placed by position
+    pub fn vb_shuffle_create_repartition(ctx: *mut vb_ctx, shuffle_id: u64, n_map: u32, n_reduce: u32, n_cols: u32, has_bytes: i32,
+                                         out: *mut *mut vb_shuf) -> i32;
+    pub fn vb_shuffle_create_repartition_dist(ctx: *mut vb_ctx, shuffle_id: u64, n_map: u32, n_reduce: u32, n_cols: u32, has_bytes: i32,
+                                              rank: u32, world: u32, out: *mut *mut vb_shuf) -> i32;
+    pub fn vb_shuffle_map_repartition(s: *mut vb_shuf, map_id: u32, first_position: u64, cols: *const *const c_void,
+                                      val_offsets: *const u64, val_bytes: *const c_void, n_val_bytes: u64, n_rows: u64,
+                                      src_loc: i32) -> i32;
+    pub fn vb_shuffle_reduce_repartition_size(s: *mut vb_shuf, r: u32, n_rows: *mut u64, n_bytes: *mut u64) -> i32;
+    pub fn vb_shuffle_reduce_repartition(s: *mut vb_shuf, r: u32, out_cols: *const *mut c_void, out_offsets: *mut u64,
+                                         out_bytes: *mut c_void, dst_loc: i32) -> i32;
     // byte-string values across ranks: the rows' bytes travel as u32 lengths + bytes, never their references
     pub fn vb_shuffle_create_bytes_dist(ctx: *mut vb_ctx, shuffle_id: u64, n_map: u32, n_reduce: u32, key_dtype: i32, agg: i32,
                                         part: i32, rank: u32, world: u32, out: *mut *mut vb_shuf) -> i32;

@@ -137,6 +137,11 @@ SYMBOLS = {
     "vb_shuffle_create_str_sort_bytes": (_i32, [_vp, _u64, _u32, _u32, _pvp]),
     "vb_shuffle_gather_bytes_size": (_i32, [_vp, _vp, _u64, _i32, _pu64]),
     "vb_shuffle_gather_bytes": (_i32, [_vp, _vp, _u64, _i32, _vp, _vp, _i32]),
+    "vb_shuffle_create_repartition": (_i32, [_vp, _u64, _u32, _u32, _u32, _i32, _pvp]),
+    "vb_shuffle_create_repartition_dist": (_i32, [_vp, _u64, _u32, _u32, _u32, _i32, _u32, _u32, _pvp]),
+    "vb_shuffle_map_repartition": (_i32, [_vp, _u32, _u64, _vp, _vp, _vp, _u64, _u64, _i32]),
+    "vb_shuffle_reduce_repartition_size": (_i32, [_vp, _u32, _pu64, _pu64]),
+    "vb_shuffle_reduce_repartition": (_i32, [_vp, _u32, _vp, _vp, _vp, _i32]),
     "vb_shuffle_create_bytes_dist": (_i32, [_vp, _u64, _u32, _u32, _i32, _i32, _i32, _u32, _u32, _pvp]),
     "vb_shuffle_create_str_bytes_dist": (_i32, [_vp, _u64, _u32, _u32, _u32, _u32, _pvp]),
     "vb_shuffle_create_str_sort_bytes_dist": (_i32, [_vp, _u64, _u32, _u32, _u32, _u32, _pvp]),

@@ -377,6 +377,7 @@ struct vb_shuf {
     u64 lz_n = 0;
     std::vector<vb_shuf *> trash;                  // internal shuffles of a failed filtered join
     struct StrState *str = nullptr;                // string-key shuffle (vb_shuffle_create_str): dictionary, rows, results
+    struct RepState *rep = nullptr;                // repartition shuffle (vb_shuffle_create_repartition): items and results
     // byte-string values (val dtype VB_BYTES): per map id the store of its values, kept until vb_shuffle_free; the
     // device copy of the table is made by the first gather.  Internal shuffles of a filtered join have no store.
     std::vector<ByteSrc> bvals;
@@ -406,6 +407,10 @@ static int exchange_str_locked(vb_shuf *s);
 static int exchange_str_accs_locked(vb_shuf *s);
 static int exchange_str_sort_locked(vb_shuf *s);
 static void free_str(vb_shuf *s);
+static void free_rep(vb_shuf *s);
+static int seal_rep(vb_shuf *s);
+static int exchange_rep(vb_shuf *s, int mode);
+static int reject_rep(const vb_shuf *s, const char *what);
 
 static bool is_reduce_op(int agg) { return agg == VB_AGG_SUM || agg == VB_AGG_MIN || agg == VB_AGG_MAX || agg == VB_AGG_COUNT; }
 static bool is_group_op(int agg) { return agg == VB_AGG_GROUP || agg == VB_AGG_COGROUP; }
@@ -894,12 +899,12 @@ struct PassPlan {
 };
 
 // (LDM, DGM) combinations the engine passes per row type; anything else is a programming error.
-//   (u64, u64): seal_sort, the multisplits and the partition-first hash aggregate;
+//   (u64, u64): seal_sort, the multisplits (a repartition's with the position loader) and the partition-first hash aggregate;
 //   u64 key only: seal_sort;  (u32 id, u64): sort_id_pairs.
 #define RP_COMBOS_U64V(X)                                                                            \
     X(LD_SOA64, DG_BITS) X(LD_AOS64, DG_BITS) X(LD_SOA64, DG_BUCKET) X(LD_TABLE_KV, DG_BUCKET)         \
     X(LD_TABLE_KI, DG_BUCKET) X(LD_SOA64, DG_DEST) X(LD_AOS64, DG_DEST) X(LD_SOA64, DG_HASHTOP)        \
-    X(LD_AOS64, DG_HASHTOP)
+    X(LD_AOS64, DG_HASHTOP) X(LD_POS, DG_BUCKET)
 #define RP_COMBOS_U64K(X) X(LD_SOA64, DG_BITS)
 #define RP_COMBOS_U32V(X) X(LD_KEY32_VAL_SOA, DG_BITS) X(LD_KEY32_VAL_AOS, DG_BITS)
 
@@ -1407,6 +1412,7 @@ static int reject_bytes(const vb_shuf *s, const char *what)
 extern "C" int32_t vb_shuffle_set_key_width(vb_shuf *s, uint32_t bytes)
 {
     if (!s || (bytes != 4 && bytes != 8)) return set_err(VB_ERR_INVALID, "key width must be 4 or 8");
+    if (s->rep) return reject_rep(s, "vb_shuffle_set_key_width (positions hash as 8 bytes)");
     if (s->str) return invalid_str(s, "vb_shuffle_set_key_width");
     s->key_width = bytes;
     return VB_OK;
@@ -1422,6 +1428,7 @@ extern "C" int32_t vb_shuffle_set_hint(vb_shuf *s, uint64_t d)
 extern "C" int32_t vb_shuffle_set_dist(vb_shuf *s, uint32_t rank, uint32_t world)
 {
     if (!s || world < 1 || rank >= world || world > 256) return set_err(VB_ERR_INVALID, "bad rank/world");
+    if (s->rep) return reject_rep(s, "vb_shuffle_set_dist");
     if (s->multi && (world > 1 || s->world > 1)) return reject_multi(s, "multi-rank use through vb_shuffle_set_dist (vb_shuffle_create_multi_dist is)");
     if (s->vdt == VB_BYTES && world > 1) return set_err(VB_ERR_UNSUPPORTED, "shuffle %llu has byte-string values: they do not cross ranks yet", (unsigned long long)s->id);
     if (s->str && (world > 1 || s->world > 1)) return reject_str(s, "multi-rank use through vb_shuffle_set_dist (vb_shuffle_create_str_dist is)");
@@ -1447,6 +1454,7 @@ static int shuffle_map(vb_shuf *s, u32 map_id, const u64 *rows, const u64 *keys,
                        const u64 *const *cols = nullptr, DevBuf *own_vals = nullptr)
 {
     if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
+    if (s->rep) return reject_rep(s, "vb_shuffle_map_aos / vb_shuffle_map_soa");
     if (s->str) return invalid_str(s, "an integer-key map call");
     if (map_id >= s->n_map) return set_err(VB_ERR_INVALID, "map_id %u >= n_map %u", map_id, s->n_map);
     if (loc < VB_HOST || loc > VB_DEVICE_BORROWED) return set_err(VB_ERR_INVALID, "bad src_loc %d", loc);
@@ -1994,6 +2002,7 @@ static int export_prepare_locked(vb_shuf *s, uint64_t *counts)
 
 extern "C" int32_t vb_shuffle_export_prepare(vb_shuf *s, uint64_t *counts)
 {
+    if (s && s->rep) return reject_rep(s, "vb_shuffle_export_prepare");
     if (s && s->vdt == VB_BYTES) return reject_bytes(s, "vb_shuffle_export_prepare");
     if (!s || !counts) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "multi-rank exchange");
@@ -2125,6 +2134,7 @@ static int export_counts_locked(vb_shuf *s, uint64_t *counts)
 
 extern "C" int32_t vb_shuffle_export_counts(vb_shuf *s, uint64_t *counts)
 {
+    if (s && s->rep) return reject_rep(s, "vb_shuffle_export_counts");
     if (s && s->vdt == VB_BYTES) return reject_bytes(s, "vb_shuffle_export_counts");
     if (!s || !counts) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "multi-rank exchange");
@@ -2192,6 +2202,7 @@ static int export_direct_locked(vb_shuf *s, const uint64_t *dst_row_offset, cons
 
 extern "C" int32_t vb_shuffle_export_direct(vb_shuf *s, const uint64_t *dst_row_offset, const uint64_t *dst_total_rows)
 {
+    if (s && s->rep) return reject_rep(s, "vb_shuffle_export_direct");
     if (s && s->vdt == VB_BYTES) return reject_bytes(s, "vb_shuffle_export_direct");
     if (!s || !dst_row_offset || !dst_total_rows) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "multi-rank exchange");
@@ -2205,6 +2216,7 @@ extern "C" int32_t vb_shuffle_export_direct(vb_shuf *s, const uint64_t *dst_row_
 // source-rank major): hand them to the reduce side.  counts[world] as in vb_shuffle_import.
 extern "C" int32_t vb_shuffle_import_arena(vb_shuf *s, const uint64_t *counts)
 {
+    if (s && s->rep) return reject_rep(s, "vb_shuffle_import_arena");
     if (s && s->vdt == VB_BYTES) return reject_bytes(s, "vb_shuffle_import_arena");
     if (!s || !counts) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "multi-rank exchange");
@@ -2223,6 +2235,7 @@ extern "C" int32_t vb_shuffle_import_arena(vb_shuf *s, const uint64_t *counts)
 
 extern "C" int32_t vb_shuffle_export_buffers(vb_shuf *s, void **keys_dev, void **vals_dev)
 {
+    if (s && s->rep) return reject_rep(s, "vb_shuffle_export_buffers");
     if (s && s->vdt == VB_BYTES) return reject_bytes(s, "vb_shuffle_export_buffers");
     if (!s || !keys_dev || !vals_dev) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "multi-rank exchange");
@@ -2235,6 +2248,7 @@ extern "C" int32_t vb_shuffle_export_buffers(vb_shuf *s, void **keys_dev, void *
 
 extern "C" int32_t vb_shuffle_import(vb_shuf *s, const void *keys_dev, const void *vals_dev, const uint64_t *counts)
 {
+    if (s && s->rep) return reject_rep(s, "vb_shuffle_import");
     if (s && s->vdt == VB_BYTES) return reject_bytes(s, "vb_shuffle_import");
     if (!s || !counts) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "multi-rank exchange");
@@ -2983,6 +2997,7 @@ static int exchange_sort_locked(vb_shuf *s)
 
 extern "C" int32_t vb_shuffle_exchange(vb_shuf *s, int32_t mode)
 {
+    if (s && s->rep) return exchange_rep(s, mode);
     if (s && s->vdt == VB_BYTES && !s->bdist) return reject_bytes(s, "vb_shuffle_exchange (the _bytes_dist creates make shuffles that cross ranks)");
     if (s && s->bdist && mode == VB_XCHG_P2P) return reject_bytes(s, "the fused P2P exchange (VB_XCHG_NCCL is supported)");
     if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
@@ -3285,7 +3300,10 @@ extern "C" int32_t vb_shuffle_seal(vb_shuf *s)
         cudaSetDevice(c->device);
         KLaunch call(s, -2);
         auto body = [&]() -> int {
-            if (s->world == 1) {
+            if (s->rep) {
+                if (s->world == 1) TRY(seal_rep(s));
+                else if (!s->exported) return set_err(VB_ERR_STATE, "shuffle %llu: a multi-rank repartition is sealed after vb_shuffle_exchange", (unsigned long long)s->id);
+            } else if (s->world == 1) {
                 for (u32 m = 0; m < s->n_map; ++m)
                     if (!s->maps[m].present) return set_err(VB_ERR_STATE, "shuffle %llu sealed but map %u was never submitted", (unsigned long long)s->id, m);
                 if (s->str) {
@@ -3346,8 +3364,9 @@ extern "C" int32_t vb_shuffle_seal(vb_shuf *s)
 
 extern "C" int32_t vb_shuffle_is_sealed(vb_shuf *s) { return s && s->sealed ? 1 : 0; }
 
-static int wait_sealed(vb_shuf *s)
+static int wait_sealed(vb_shuf *s, bool rep_call = false)
 {
+    if (s->rep && !rep_call) return reject_rep(s, "an integer-key reduce, join, cogroup or blob call");
     std::unique_lock<std::mutex> g(s->mu);
     ++s->waiters;
     s->cv.wait(g, [&] { return s->sealed || s->failed || s->freed; });
@@ -3604,6 +3623,7 @@ extern "C" int32_t vb_shuffle_reduce_blob(vb_shuf *s, uint32_t r, void *out_blob
 
 extern "C" int32_t vb_shuffle_map_blob(vb_shuf *s, uint32_t map_id, const void *blob, uint64_t n_bytes, int32_t src_loc)
 {
+    if (s && s->rep) return reject_rep(s, "vb_shuffle_map_blob");
     if (s && s->vdt == VB_BYTES) return reject_bytes(s, "vb_shuffle_map_blob");
     if (!s || !blob) return set_err(VB_ERR_INVALID, "NULL argument");
     if (s->multi) return reject_multi(s, "bincode blobs");
@@ -5148,6 +5168,412 @@ extern "C" int32_t vb_shuffle_gather_bytes(vb_shuf *s, const uint64_t *refs, uin
     }
     if (dst_loc == VB_HOST) {
         TRY(copy_out(s, out_bytes, dst, total, VB_HOST));
+    }
+    CU(cudaStreamSynchronize(c->stream));
+    return VB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// repartition (Rdd::repartition = coalesce(n, shuffle = true), rdd.rs:386-418): row i of map m is placed by
+// HashPartitioner::<usize> at position start_m + 1 + i.  The seal is one stable multisplit whose loader computes each
+// row's position from its index (LD_POS): no key column exists, and each partition holds its rows in map-id, then
+// input order.
+// ---------------------------------------------------------------------------------------------
+struct RepMapIn {
+    bool present = false;
+    bool owned = false;          // the columns are copies owned by the shuffle (not VB_DEVICE_BORROWED)
+    u64 n_rows = 0;
+    u64 start = 0;               // first_position
+    const u64 *cols[2] = {};
+};
+
+struct RepState {
+    u32 n_cols = 0;
+    bool bytes = false;
+    std::vector<RepMapIn> maps;
+    u64 n = 0;                   // sealed rows
+    u64 *cols = nullptr;         // [n_cols][n] item columns, partition r at rows [bucket_off[r], bucket_off[r + 1])
+    u64 *refs = nullptr;         // bytes: [n] row references in the same order, gathered by the byte-string copy path
+};
+
+static int reject_rep(const vb_shuf *s, const char *what)
+{
+    return set_err(VB_ERR_INVALID, "shuffle %llu is a repartition shuffle: %s does not apply to it", (unsigned long long)s->id, what);
+}
+
+static void free_rep_map(vb_ctx *c, RepMapIn &m)
+{
+    if (m.owned) { dev_free(c, m.cols[0]); dev_free(c, m.cols[1]); }
+    m = RepMapIn();
+}
+
+static void free_rep(vb_shuf *s)
+{
+    if (!s->rep) return;
+    for (RepMapIn &m : s->rep->maps) free_rep_map(s->ctx, m);
+    dev_free(s->ctx, s->rep->cols);
+    dev_free(s->ctx, s->rep->refs);
+    delete s->rep;
+    s->rep = nullptr;
+}
+
+extern "C" int32_t vb_shuffle_create_repartition_dist(vb_ctx *c, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce, uint32_t n_cols,
+                                                      int32_t has_bytes, uint32_t rank, uint32_t world, vb_shuf **out)
+{
+    if (!c || !out) return set_err(VB_ERR_INVALID, "vb_shuffle_create_repartition: NULL argument");
+    *out = nullptr;
+    if (world < 1 || world > 256 || rank >= world) return set_err(VB_ERR_INVALID, "vb_shuffle_create_repartition_dist: bad rank %u / world %u", rank, world);
+    if (n_reduce < 1) return set_err(VB_ERR_INVALID, "vb_shuffle_create_repartition: n_reduce must be >= 1");
+    if (has_bytes != 0 && has_bytes != 1) return set_err(VB_ERR_INVALID, "vb_shuffle_create_repartition: has_bytes must be 0 or 1");
+    if (n_cols > 2 || (n_cols == 0 && !has_bytes))
+        return set_err(VB_ERR_INVALID, "vb_shuffle_create_repartition: items are 0 to 2 64-bit columns plus an optional byte-string column, at least one column in all");
+    if (n_reduce > 65536) return set_err(VB_ERR_UNSUPPORTED, "more than 65536 reduce partitions");
+    vb_shuf *s = new vb_shuf();
+    s->uid = next_uid.fetch_add(1);
+    s->ctx = c;
+    s->id = shuffle_id;
+    s->n_map = n_map;
+    s->n_reduce = n_reduce;
+    s->kdt = VB_U64;
+    s->vdt = VB_U64;
+    s->agg = -1;                  // no aggregator: every GROUP / reduce / sort path refuses the shuffle
+    s->part = VB_PART_HASH_METRO64;
+    s->rep = new RepState();
+    s->rep->n_cols = n_cols;
+    s->rep->bytes = has_bytes == 1;
+    s->rep->maps.resize(n_map);
+    if (has_bytes) s->bvals.assign(n_map, ByteSrc{nullptr, nullptr, 0});
+    s->rank = rank;
+    s->world = world;
+    *out = s;
+    return VB_OK;
+}
+
+extern "C" int32_t vb_shuffle_create_repartition(vb_ctx *c, uint64_t shuffle_id, uint32_t n_map, uint32_t n_reduce, uint32_t n_cols,
+                                                 int32_t has_bytes, vb_shuf **out)
+{
+    return vb_shuffle_create_repartition_dist(c, shuffle_id, n_map, n_reduce, n_cols, has_bytes, 0, 1, out);
+}
+
+extern "C" int32_t vb_shuffle_map_repartition(vb_shuf *s, uint32_t map_id, uint64_t first_position, const void *const *cols,
+                                              const uint64_t *val_offsets, const void *val_bytes, uint64_t n_val_bytes, uint64_t n,
+                                              int32_t loc)
+{
+    if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
+    if (!s->rep) return set_err(VB_ERR_INVALID, "vb_shuffle_map_repartition needs a shuffle from vb_shuffle_create_repartition");
+    RepState *rs = s->rep;
+    if (map_id >= s->n_map) return set_err(VB_ERR_INVALID, "map_id %u >= n_map %u", map_id, s->n_map);
+    if (loc < VB_HOST || loc > VB_DEVICE_BORROWED) return set_err(VB_ERR_INVALID, "bad src_loc %d", loc);
+    {
+        std::lock_guard<std::mutex> g(s->mu);
+        if (s->exported) return set_err(VB_ERR_STATE, "shuffle %llu: map after exchange", (unsigned long long)s->id);
+    }
+    for (u32 k = 0; k < rs->n_cols; ++k)
+        if (n && (!cols || !cols[k])) return set_err(VB_ERR_INVALID, "NULL item column %u with n_rows > 0", k);
+    if (rs->bytes && n && !val_offsets) return set_err(VB_ERR_INVALID, "NULL val_offsets with n_rows > 0");
+    if (rs->bytes && n && n_val_bytes && !val_bytes) return set_err(VB_ERR_INVALID, "NULL val_bytes with n_val_bytes > 0");
+    if (n >= 0xFFFFFFFEull) return set_err(VB_ERR_TOO_LARGE, "map partition of %llu rows", (unsigned long long)n);
+    {
+        std::lock_guard<std::mutex> g(s->mu);
+        if (s->sealed || s->sealing || s->freed) return set_err(VB_ERR_STATE, "shuffle %llu: map after seal", (unsigned long long)s->id);
+    }
+    vb_ctx *c = s->ctx;
+    ByteSrc st{nullptr, nullptr, 0};
+    if (rs->bytes) {
+        DevBuf refs(c);   // bytes_store's references are not kept: a repartition computes them from the row index
+        TRY(bytes_store(s, map_id, val_offsets, val_bytes, n_val_bytes, n, loc, &st, refs));
+    }
+    auto columns = [&]() -> int {
+        std::lock_guard<std::mutex> lk(c->mu);
+        CU(cudaSetDevice(c->device));
+        RepMapIn in;
+        in.present = true;
+        in.n_rows = n;
+        in.start = first_position;
+        if (n && loc == VB_DEVICE_BORROWED) {
+            for (u32 k = 0; k < rs->n_cols; ++k) in.cols[k] = (const u64 *)cols[k];
+        } else if (n && rs->n_cols) {
+            const cudaMemcpyKind kind = loc == VB_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
+            DevBuf b0(c), b1(c);
+            DevBuf *b[2] = {&b0, &b1};
+            for (u32 k = 0; k < rs->n_cols; ++k) {
+                TRY(b[k]->alloc(n * 8));
+                CU(cudaMemcpyAsync(b[k]->p, cols[k], n * 8, kind, c->stream));
+                if (loc == VB_HOST) s->st.h2d_bytes += n * 8;
+            }
+            CU(cudaStreamSynchronize(c->stream));      // the caller may reuse its buffers on return
+            for (u32 k = 0; k < rs->n_cols; ++k) in.cols[k] = (const u64 *)b[k]->release();
+            in.owned = true;
+        }
+        RepMapIn &m = rs->maps[map_id];
+        if (m.present) s->st.rows_in -= m.n_rows;     // resubmission: the last submission wins
+        free_rep_map(c, m);
+        m = in;
+        s->st.rows_in += n;
+        return VB_OK;
+    };
+    const int rc = columns();
+    return rs->bytes ? bytes_keep(s, map_id, st, rc) : rc;
+}
+
+// out[k * n + i] = item column k of the row with reference refs[i]; src[k * n_map + m] is map m's column k
+__global__ void rep_gather_kernel(const u64 *__restrict__ refs, u64 n, const u64 *const *__restrict__ src, u32 n_map, u32 n_cols,
+                                  u64 *__restrict__ out)
+{
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+        const u64 ref = refs[i];
+        const u32 m = (u32)(ref >> 32) - 1;
+        const u64 r = ref & 0xFFFFFFFFull;
+        for (u32 k = 0; k < n_cols; ++k) out[(u64)k * n + i] = src[(u64)k * n_map + m][r];
+    }
+}
+
+// One stable multisplit of every row by the partition of its position (multisplit: one pass for <= 256 partitions,
+// two LSD passes over the 16-bit partition id above).  An item of one 64-bit column moves as the pass's value; any
+// other item moves as its row reference, and a gather then reads its columns.
+static int seal_rep(vb_shuf *s)
+{
+    vb_ctx *c = s->ctx;
+    RepState *rs = s->rep;
+    const u32 M = s->n_map, R = s->n_reduce;
+    const bool direct = rs->n_cols == 1 && !rs->bytes;
+    std::vector<RepMap> h((size_t)M + 1);
+    u64 n = 0;
+    for (u32 m = 0; m < M; ++m) {
+        const RepMapIn &mi = rs->maps[m];
+        if (!mi.present && s->world == 1) return set_err(VB_ERR_STATE, "shuffle %llu sealed but map %u was never submitted", (unsigned long long)s->id, m);
+        h[m] = RepMap{n, mi.start, direct ? mi.cols[0] : nullptr};
+        n += mi.n_rows;
+    }
+    h[M] = RepMap{n, 0, nullptr};
+    if (n >= 0xFFFFFFFEull) return set_err(VB_ERR_TOO_LARGE, "shuffle of %llu rows on one device", (unsigned long long)n);
+    s->bucket_off.assign((size_t)R + 1, 0);
+    rs->n = n;
+    if (n == 0) return VB_OK;
+    DevBuf tab(c), pos(c), vals(c);
+    TRY(tab.alloc(h.size() * sizeof(RepMap)));
+    CU(cudaMemcpyAsync(tab.p, h.data(), h.size() * sizeof(RepMap), cudaMemcpyHostToDevice, c->stream));
+    TRY(pos.alloc(n * 8));
+    TRY(vals.alloc(n * 8));
+    TRY(multisplit(s, Loader{LD_POS, tab.p, nullptr, M}, n, DG_BUCKET, R, n, pos.as<u64>(), vals.as<u64>(), s->bucket_off));
+    if (direct) {
+        rs->cols = vals.as<u64>();
+        vals.release();
+    } else {
+        if (rs->n_cols) {
+            std::vector<const u64 *> hs((size_t)rs->n_cols * M);
+            for (u32 k = 0; k < rs->n_cols; ++k)
+                for (u32 m = 0; m < M; ++m) hs[(size_t)k * M + m] = rs->maps[m].cols[k];
+            DevBuf src(c), out(c);
+            TRY(src.alloc(hs.size() * sizeof(u64 *)));
+            TRY(out.alloc((u64)rs->n_cols * n * 8));
+            CU(cudaMemcpyAsync(src.p, hs.data(), hs.size() * sizeof(u64 *), cudaMemcpyHostToDevice, c->stream));
+            {
+                KLaunch kl(s, K_MISC, n);
+                const unsigned blocks = (unsigned)std::min<u64>((n + 255) / 256, (u64)c->sm_count * 8);
+                rep_gather_kernel<<<blocks, 256, 0, c->stream>>>(vals.as<u64>(), n, (const u64 *const *)src.p, M, rs->n_cols, out.as<u64>());
+                TRY(kl.done("rep_gather_kernel"));
+            }
+            CU(cudaStreamSynchronize(c->stream));      // pageable sources of the two tables
+            rs->cols = out.as<u64>();
+            out.release();
+        }
+        if (rs->bytes) { rs->refs = vals.as<u64>(); vals.release(); }
+    }
+    CU(cudaStreamSynchronize(c->stream));
+    for (RepMapIn &m : rs->maps) {             // the items now live in the result (the byte stores stay for the gather)
+        if (m.owned) { dev_free(c, m.cols[0]); dev_free(c, m.cols[1]); }
+        m.cols[0] = m.cols[1] = nullptr;
+        m.owned = false;
+    }
+    s->st.rows_out = n;
+    return VB_OK;
+}
+
+// Across ranks (vb_shuffle_exchange): the rank's own map tasks are split by output partition with the one-process seal,
+// every partition's run goes to its owner (p % world) in one grouped send/recv, as the sort exchange sends them, and the
+// owner appends the runs in source-rank order, which is map-id order because map ids are assigned in contiguous blocks
+// by rank.  The count all-gather carries each rank's rows, n_cols and has_bytes; a second all-gather carries the rows
+// (and bytes) of every partition.  Every limit and the agreement of n_cols and has_bytes are checked on every rank from
+// the gathered counts, so all ranks return the same code before any send.
+static int exchange_rep_locked(vb_shuf *s)
+{
+    vb_ctx *c = s->ctx;
+    Comm *m = c->comm;
+    RepState *rs = s->rep;
+    const u32 W = m->world, me = m->rank, R = s->n_reduce, K = rs->n_cols;
+    auto clk = std::chrono::steady_clock::now();
+    u64 n_local = 0;
+    for (const RepMapIn &mi : rs->maps) n_local += mi.present ? mi.n_rows : 0;
+    const u64 row[3] = {n_local, K, rs->bytes ? 1ull : 0ull};
+    const u64 *mat = nullptr;
+    TRY(comm_all_gather(c, row, 3, &mat));
+    s->xst.counts_wall_ms += lap(clk);
+    for (u32 r = 0; r < W; ++r) {
+        if (mat[3 * r + 1] != K || mat[3 * r + 2] != row[2])
+            return set_err(VB_ERR_INVALID, "repartition across ranks: rank %u has %llu columns and has_bytes %llu, rank %u %u and %llu", r,
+                           (unsigned long long)mat[3 * r + 1], (unsigned long long)mat[3 * r + 2], me, K, (unsigned long long)row[2]);
+        if (mat[3 * r] >= 0xFFFFFFFEull) return set_err(VB_ERR_TOO_LARGE, "rank %u maps %llu rows", r, (unsigned long long)mat[3 * r]);
+    }
+    // 1. the local split: partition p's rows at [bucket_off[p], bucket_off[p + 1]) of rs->cols / rs->refs
+    TRY(seal_rep(s));
+    const u64 nl = rs->n;
+    const std::vector<u64> cut = s->bucket_off;
+    std::vector<u64> bat;
+    if (rs->bytes) TRY(bytes_pack(s, rs->refs, nl, cut, bat));
+    s->xst.prepare_wall_ms += lap(clk);
+    // 2. rows (and bytes) of every partition on every rank
+    const u32 SR = rs->bytes ? 2 * R : R;
+    std::vector<u64> seg(SR), segall((size_t)W * SR);
+    for (u32 p = 0; p < R; ++p) {
+        seg[p] = cut[p + 1] - cut[p];
+        if (rs->bytes) seg[R + p] = bat[p + 1] - bat[p];
+    }
+    DevBuf d_seg(c), d_segall(c);
+    TRY(d_seg.alloc((size_t)SR * 8));
+    TRY(d_segall.alloc((size_t)W * SR * 8));
+    CU(cudaMemcpyAsync(d_seg.p, seg.data(), (size_t)SR * 8, cudaMemcpyHostToDevice, c->stream));
+    NC(g_nccl.AllGather(d_seg.p, d_segall.p, SR, ncclUint64, m->comm, c->stream));
+    CU(cudaMemcpyAsync(segall.data(), d_segall.p, (size_t)W * SR * 8, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    for (u32 d = 0; d < W; ++d) {                 // every rank's receive total, so that all ranks refuse alike
+        u64 nd = 0;
+        for (u32 p = d; p < R; p += W)
+            for (u32 r = 0; r < W; ++r) nd += segall[(size_t)r * SR + p];
+        if (nd >= 0xFFFFFFFEull) return set_err(VB_ERR_TOO_LARGE, "rank %u would receive %llu rows", d, (unsigned long long)nd);
+    }
+    std::vector<u64> off((size_t)R + 1, 0);
+    u64 nb_recv = 0;
+    for (u32 p = 0; p < R; ++p) {
+        u64 np = 0;
+        if (p % W == me)
+            for (u32 r = 0; r < W; ++r) {
+                np += segall[(size_t)r * SR + p];
+                if (rs->bytes) nb_recv += segall[(size_t)r * SR + R + p];
+            }
+        off[p + 1] = off[p] + np;
+    }
+    const u64 n_recv = off[R];
+    // 3. one grouped send/recv: partition-major, source-rank-major at the owner
+    DevBuf rc(c), rl(c), rb(c), refs(c);
+    TRY(rc.alloc((u64)K * n_recv * 8));
+    if (rs->bytes) { TRY(rl.alloc(n_recv * 4)); TRY(rb.alloc(nb_recv)); }
+    std::vector<Xfer> xs;
+    u64 sent = 0, own = 0;
+    for (u32 p = 0; p < R; ++p) {
+        for (u32 k = 0; k < K; ++k) xs.push_back(Xfer{true, p % W, rs->cols + (u64)k * nl + cut[p], seg[p], ncclUint64});
+        if (rs->bytes) {
+            xs.push_back(Xfer{true, p % W, s->bx_lens + cut[p], seg[p], ncclUint32});
+            xs.push_back(Xfer{true, p % W, s->bx_bytes + bat[p], seg[R + p], ncclUint8});
+        }
+        (p % W == me ? own : sent) += seg[p];
+    }
+    u64 boff = 0;
+    for (u32 p = me; p < R; p += W) {
+        u64 o = off[p];
+        for (u32 r = 0; r < W; ++r) {
+            const u64 cnt = segall[(size_t)r * SR + p];
+            for (u32 k = 0; k < K; ++k) xs.push_back(Xfer{false, r, rc.as<u64>() + (u64)k * n_recv + o, cnt, ncclUint64});
+            if (rs->bytes) {
+                const u64 nb = segall[(size_t)r * SR + R + p];
+                xs.push_back(Xfer{false, r, rl.as<u32>() + o, cnt, ncclUint32});
+                xs.push_back(Xfer{false, r, rb.as<unsigned char>() + boff, nb, ncclUint8});
+                boff += nb;
+            }
+            o += cnt;
+        }
+    }
+    TRY(post_group(s, xs));
+    if (rs->bytes) TRY(bytes_adopt(s, rl.as<u32>(), n_recv, rb, nb_recv, refs));   // synchronises the stream
+    CU(cudaStreamSynchronize(c->stream));
+    s->xst.post_wall_ms += lap(clk);
+    xchg_done(s, VB_XCHG_NCCL, sent, n_recv - own);
+    dev_free(c, rs->cols);
+    dev_free(c, rs->refs);
+    dev_free(c, s->bx_lens);
+    dev_free(c, s->bx_bytes);
+    s->bx_lens = nullptr;
+    s->bx_bytes = nullptr;
+    rs->cols = K ? rc.as<u64>() : nullptr;
+    if (K) rc.release();
+    rs->refs = rs->bytes ? refs.as<u64>() : nullptr;
+    if (rs->bytes) refs.release();
+    rs->n = n_recv;
+    s->bucket_off = off;
+    s->st.rows_out = n_recv;
+    std::lock_guard<std::mutex> g(s->mu);
+    s->exported = s->imported = true;
+    return VB_OK;
+}
+
+static int exchange_rep(vb_shuf *s, int mode)
+{
+    vb_ctx *c = s->ctx;
+    if (mode < VB_XCHG_AUTO || mode > VB_XCHG_P2P) return set_err(VB_ERR_INVALID, "bad exchange mode");
+    if (mode == VB_XCHG_P2P) return set_err(VB_ERR_UNSUPPORTED, "repartition: the fused P2P exchange (VB_XCHG_NCCL is supported)");
+    if (s->world < 2) return set_err(VB_ERR_STATE, "vb_shuffle_exchange of a one-process repartition (vb_shuffle_create_repartition_dist has world > 1)");
+    if (!c->comm) return set_err(VB_ERR_STATE, "vb_shuffle_exchange needs vb_ctx_comm_init");
+    if (c->comm->world != s->world || c->comm->rank != s->rank) return set_err(VB_ERR_INVALID, "shuffle rank/world differ from the communicator's");
+    {
+        std::lock_guard<std::mutex> g(s->mu);
+        if (s->sealed || s->sealing || s->exported || s->freed) return set_err(VB_ERR_STATE, "shuffle %llu: exchange after seal/exchange", (unsigned long long)s->id);
+    }
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    return exchange_rep_locked(s);
+}
+
+static int rep_reduce_check(vb_shuf *s, u32 r, const char *what)
+{
+    if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
+    if (!s->rep) return set_err(VB_ERR_INVALID, "%s needs a shuffle from vb_shuffle_create_repartition", what);
+    if (r >= s->n_reduce) return set_err(VB_ERR_INVALID, "reduce_id %u >= n_reduce %u", r, s->n_reduce);
+    return wait_sealed(s, true);
+}
+
+extern "C" int32_t vb_shuffle_reduce_repartition_size(vb_shuf *s, uint32_t r, uint64_t *n_rows, uint64_t *n_bytes)
+{
+    TRY(rep_reduce_check(s, r, "vb_shuffle_reduce_repartition_size"));
+    const u64 b0 = s->bucket_off[r], nk = s->bucket_off[r + 1] - b0;
+    if (n_rows) *n_rows = nk;
+    if (!n_bytes) return VB_OK;
+    *n_bytes = 0;
+    if (!s->rep->bytes || nk == 0) return VB_OK;
+    vb_ctx *c = s->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    DevBuf rr(c), offs(c);
+    TRY(offs.alloc((nk + 1) * 8));
+    return bytes_offsets(s, s->rep->refs + b0, nk, VB_DEVICE, rr, offs.as<u64>(), n_bytes);
+}
+
+extern "C" int32_t vb_shuffle_reduce_repartition(vb_shuf *s, uint32_t r, void *const *out_cols, uint64_t *out_offsets, void *out_bytes,
+                                                 int32_t dst_loc)
+{
+    if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
+    TRY(rep_reduce_check(s, r, "vb_shuffle_reduce_repartition"));
+    vb_ctx *c = s->ctx;
+    RepState *rs = s->rep;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    const u64 b0 = s->bucket_off[r], nk = s->bucket_off[r + 1] - b0;
+    DevBuf rr(c), offs(c), tmp(c);
+    u64 total = 0;
+    const bool want_bytes = rs->bytes && (out_offsets || out_bytes);
+    if (want_bytes) {                           // the offsets first: a NULL out_bytes for a partition with bytes writes nothing
+        TRY(offs.alloc((nk + 1) * 8));
+        TRY(bytes_offsets(s, rs->refs ? rs->refs + b0 : nullptr, nk, VB_DEVICE, rr, offs.as<u64>(), &total));
+        if (total && !out_bytes) return set_err(VB_ERR_INVALID, "NULL out_bytes for %llu bytes", (unsigned long long)total);
+    }
+    for (u32 k = 0; out_cols && k < rs->n_cols; ++k)
+        if (nk) TRY(copy_out(s, out_cols[k], rs->cols + (u64)k * rs->n + b0, nk * 8, dst_loc));
+    if (want_bytes) {
+        unsigned char *dst = (unsigned char *)out_bytes;
+        if (total && dst_loc == VB_HOST) { TRY(tmp.alloc(total)); dst = tmp.as<unsigned char>(); }
+        if (total) TRY(bytes_gather_launch(s, rs->refs + b0, nk, offs.as<u64>(), total, dst));
+        TRY(copy_out(s, out_offsets, offs.p, (nk + 1) * 8, dst_loc));
+        if (dst_loc == VB_HOST) TRY(copy_out(s, out_bytes, dst, total, VB_HOST));
     }
     CU(cudaStreamSynchronize(c->stream));
     return VB_OK;
@@ -7098,6 +7524,7 @@ extern "C" int32_t vb_shuffle_free(vb_shuf *s)
         for (auto &kv : s->n_plans) free_cogroup_n_plan(c, kv.second);
         free_lazy_rows(s);
         free_str(s);
+        free_rep(s);
         for (ByteSrc &b : s->bvals) { dev_free(c, b.offs); dev_free(c, b.bytes); }
         dev_free(c, s->bvals_dev);
         cudaStreamSynchronize(c->stream);

@@ -942,7 +942,7 @@ constexpr int RPS_ITEMS = RP_TILE / RPS_THREADS; // (256 x 16 needed 128 registe
 // Every pass, the LSD sort passes included, uses 8-bit digits: a 10-bit variant of the sort was slower per pass
 // (per-tile scan over 1025 bins + 4-row write runs).
 
-enum : int { LD_SOA64 = 0, LD_AOS64 = 1, LD_KEY32_VAL_SOA = 2, LD_KEY32_VAL_AOS = 3, LD_TABLE_KV = 4, LD_TABLE_KI = 5 };
+enum : int { LD_SOA64 = 0, LD_AOS64 = 1, LD_KEY32_VAL_SOA = 2, LD_KEY32_VAL_AOS = 3, LD_TABLE_KV = 4, LD_TABLE_KI = 5, LD_POS = 6 };
 
 // Where a pass reads its rows from.  One struct, run-time mode (CTA-uniform branch).
 struct Loader {
@@ -951,6 +951,28 @@ struct Loader {
     const void *vals;   // u64* (table modes: the accs array) or AoS rows for LD_KEY32_VAL_AOS
     u64 cap;            // table modes: number of regular slots (row `cap` is the special slot)
 };
+
+// LD_POS rows (repartition, vb_shuffle_map_repartition): the maps' rows in map-id order, row i of map m at position
+// start + 1 + i (mod 2^64).  The loader's key is that position, computed from the row index: no key column exists.
+// Loader.keys = RepMap[cap + 1] over the cap maps; entry cap holds the total row count.
+struct RepMap {
+    u64 row_off;        // the map's first row in the concatenation of the maps
+    u64 start;          // first_position of the map
+    const u64 *col;     // the one item column, moved as the value; NULL: the value is the row reference ((m + 1) << 32 | i)
+};
+
+// the map holding row i (the last m with row_off <= i; empty maps share their successor's offset) and the row in it
+VB_D u64 rep_locate(const RepMap *__restrict__ t, u32 n_map, u64 i, u32 &m)
+{
+    u32 lo = 0, hi = n_map;
+    while (hi - lo > 1) {
+        const u32 mid = (lo + hi) >> 1;
+        if (__ldg(&t[mid].row_off) <= i) lo = mid;
+        else hi = mid;
+    }
+    m = lo;
+    return i - __ldg(&t[lo].row_off);
+}
 
 // Loader / digit modes are compile-time (LDM, DGM): a run-time switch per item left ptxas with a
 // branch per load and no memory-level parallelism.
@@ -973,6 +995,14 @@ VB_D bool rp_load(const Loader &ld, u64 i, KeyT &key, u64 &val, u64 pol)
         key = (KeyT)ld_stream_u32((const u32 *)ld.keys + i, pol);
         val = ld_stream_u64((const u64 *)ld.vals + 2 * i + 1, pol);
         return true;
+    } else if constexpr (LDM == LD_POS) {
+        const RepMap *t = (const RepMap *)ld.keys;
+        u32 m;
+        const u64 r = rep_locate(t, (u32)ld.cap, i, m);
+        key = (KeyT)(__ldg(&t[m].start) + 1 + r);
+        const u64 *col = (const u64 *)__ldg((const unsigned long long *)&t[m].col);
+        val = col ? ld_stream_u64(col + r, pol) : ((u64)(m + 1) << 32 | r);
+        return true;
     } else {
         const u64 k = ld_stream_u64((const u64 *)ld.keys + i, pol);
         val = (LDM == LD_TABLE_KI) ? i : ld_stream_u64((const u64 *)ld.vals + i, pol);
@@ -989,6 +1019,13 @@ VB_D bool rp_load_key(const Loader &ld, u64 i, KeyT &key, u64 pol)
     if constexpr (LDM == LD_SOA64) { key = (KeyT)ld_stream_u64((const u64 *)ld.keys + i, pol); return true; }
     else if constexpr (LDM == LD_AOS64) { key = (KeyT)ld_stream_u64((const u64 *)ld.keys + 2 * i, pol); return true; }
     else if constexpr (LDM == LD_KEY32_VAL_SOA || LDM == LD_KEY32_VAL_AOS) { key = (KeyT)ld_stream_u32((const u32 *)ld.keys + i, pol); return true; }
+    else if constexpr (LDM == LD_POS) {
+        const RepMap *t = (const RepMap *)ld.keys;
+        u32 m;
+        const u64 r = rep_locate(t, (u32)ld.cap, i, m);
+        key = (KeyT)(__ldg(&t[m].start) + 1 + r);
+        return true;
+    }
     else {
         const u64 k = ld_stream_u64((const u64 *)ld.keys + i, pol);
         if (i == ld.cap) { key = (KeyT)EMPTY_KEY; return k == 1ull; }
@@ -1086,7 +1123,7 @@ rp_hist_kernel(Loader ld, Digit dg, u64 n, u64 rows_per_part, u32 *__restrict__ 
     };
     constexpr int HB = 8;   // items per batch: keeps the u64 instantiation at <= 64 registers
     u32 tiles_since_fold = 0;
-    constexpr bool STREAM = (LDM == LD_SOA64 || LDM == LD_AOS64 || LDM == LD_KEY32_VAL_SOA || LDM == LD_KEY32_VAL_AOS);   // every row valid
+    constexpr bool STREAM = (LDM == LD_SOA64 || LDM == LD_AOS64 || LDM == LD_KEY32_VAL_SOA || LDM == LD_KEY32_VAL_AOS || LDM == LD_POS);   // every row valid
     for (u64 t0 = begin + (u64)sub * RP_TILE; t0 < end; t0 += (u64)split * RP_TILE) {
         if (STREAM && t0 + RP_TILE <= end) {      // whole tile in range: no bounds checks, no branch around the counter update
 #pragma unroll 1

@@ -1033,6 +1033,150 @@ class AggregateRdd(_AggregatedParent):
         return i, len(self.combined.names), _CODE_OF[self.combined.out_dtypes[i]]
 
 
+class RepShuffle(Shuffle):
+    """vb_shuffle_create_repartition: repartition(n) = coalesce(n, shuffle=true) of items of n_cols 64-bit columns plus,
+    with has_bytes, one byte-string column.  Partition r holds its items in map-id, then input order."""
+
+    def __init__(self, sc, n_map, n_reduce, codes, has_bytes, as_str=True, rank=0, world=1):
+        """codes: the dtype code of each 64-bit column (the dtype its items come back as).  world > 1: rank `rank`'s
+        shuffle (vb_shuffle_create_repartition_dist); map this rank's block of map ids, then exchange() and seal()."""
+        self.sc, self._lib = sc, sc._lib
+        self.n_map, self.n_reduce, self.codes, self.has_bytes, self.as_str = n_map, n_reduce, tuple(codes), bool(has_bytes), as_str
+        self.agg = self.vcode = self.kcode = None
+        self.has_payload, self._keepalive = True, []
+        h = ctypes.c_void_p()
+        self.rank, self.world = rank, world
+        L.check(self._lib.vb_shuffle_create_repartition_dist(sc._h, sc.new_shuffle_id(), n_map, n_reduce, len(self.codes),
+                                                              int(self.has_bytes), rank, world, ctypes.byref(h)))
+        self._h = h
+        sc._shuffles.add(self)
+
+    def map_items(self, map_id, first_position, cols, bcol, start, stop):
+        """Map task map_id: items [start, stop) of the columns cols and of the byte-string column bcol (or None), at the
+        positions first_position + 1, first_position + 2, ..."""
+        host = [c.loc == L.VB_HOST for c in cols] + ([bcol.loc == L.VB_HOST] if bcol is not None else [])
+        if len(set(host)) > 1:
+            raise ValueError("the item columns must live in the same memory space")
+        loc = cols[0].loc if cols else bcol.loc
+        if loc == L.VB_DEVICE_BORROWED:
+            self._keepalive.append(tuple(c.owner for c in cols))
+        ptrs = (ctypes.c_void_p * len(cols))(*[c.at(start) for c in cols]) if cols else None
+        offs, data, nb = (bcol.offs_at(start), bcol.data_at(), bcol.n_bytes) if bcol is not None else (None, None, 0)
+        L.check(self._lib.vb_shuffle_map_repartition(self._h, map_id, int(first_position), ptrs, offs, data, nb, stop - start, loc))
+
+    def reduce_size(self, r):
+        """(items, their total bytes) of partition r."""
+        n, nb = ctypes.c_uint64(), ctypes.c_uint64()
+        L.check(self._lib.vb_shuffle_reduce_repartition_size(self._h, r, ctypes.byref(n), ctypes.byref(nb)))
+        return n.value, nb.value
+
+    def reduce(self, r):
+        """Partition r on the host: ([one array per 64-bit column], object array of str / bytes, or None)."""
+        n, nb = self.reduce_size(r)
+        cols = [np.empty(n, dtype=_NP_OF[c]) for c in self.codes]
+        ptrs = (ctypes.c_void_p * len(cols))(*[c.ctypes.data for c in cols]) if cols else None
+        offs = np.empty(n + 1, dtype=np.uint64) if self.has_bytes else None
+        data = np.empty(nb, dtype=np.uint8) if self.has_bytes else None
+        p = lambda a: a.ctypes.data_as(ctypes.c_void_p) if a is not None else None
+        L.check(self._lib.vb_shuffle_reduce_repartition(self._h, r, ptrs, p(offs), p(data), L.VB_HOST))
+        if not self.has_bytes:
+            return cols, None
+        raw, o = data.tobytes(), offs.astype(np.int64).tolist()
+        items = np.empty(n, dtype=object)
+        if self.as_str:
+            items[:] = [raw[o[i]:o[i + 1]].decode("utf-8", "surrogateescape") for i in range(n)]
+        else:
+            items[:] = [raw[o[i]:o[i + 1]] for i in range(n)]
+        return cols, items
+
+    def reduce_device(self, r, out_cols=None, out_offsets=None, out_bytes=None):
+        """Partition r into caller-provided torch CUDA tensors (any may be None; sizes from reduce_size)."""
+        out_cols = list(out_cols or [None] * len(self.codes))
+        _sync_torch(out_offsets, out_bytes, *out_cols)
+        p = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None
+        ptrs = (ctypes.c_void_p * len(out_cols))(*[p(t) for t in out_cols]) if out_cols else None
+        L.check(self._lib.vb_shuffle_reduce_repartition(self._h, r, ptrs, p(out_offsets), p(out_bytes), L.VB_DEVICE))
+
+
+def _rep_starts(parent, starts):
+    """One u64 start per map partition of parent (vega's start_m, drawn by the caller); 0 for every one by default."""
+    n_map = len(slice_starts(parent.n, parent.num_slices)) - 1
+    if starts is None:
+        return [0] * n_map
+    starts = [int(x) for x in (starts.tolist() if hasattr(starts, "tolist") else starts)]
+    if len(starts) != n_map:
+        raise ValueError(f"starts: one per map partition expected ({n_map}), got {len(starts)}")
+    if any(not 0 <= x < 1 << 64 for x in starts):
+        raise ValueError("starts must be u64 values")
+    return starts
+
+
+def _repartition(parent, num_partitions, shuffle, starts, cols, bcol=None, bytes_first=False):
+    if not shuffle:
+        raise NotImplementedError("coalesce(shuffle=False) (vega's narrow CoalescedRdd) is not served by the library")
+    if isinstance(num_partitions, bool) or not isinstance(num_partitions, (int, np.integer)) or num_partitions < 1:
+        raise ValueError("Number of partitions should be greater than or equal to 1")
+    return RepartitionedRdd(parent, int(num_partitions), _rep_starts(parent, starts), cols, bcol, bytes_first)
+
+
+def _split_rows(col):
+    """(n,2) AoS rows as two 64-bit columns."""
+    x = col.owner
+    a, b = (x[:, 0].contiguous(), x[:, 1].contiguous()) if _is_torch(x) else (np.ascontiguousarray(x[:, 0]), np.ascontiguousarray(x[:, 1]))
+    ka, kb = _Col(a, role="value"), _Col(b, role="value")
+    ka.code = kb.code = col.code
+    return ka, kb
+
+
+class RepartitionedRdd(_Base):
+    """`rdd.repartition(n)` = `rdd.coalesce(n, shuffle=true)` (rdd.rs:386-418): map partition m gives its items the positions
+    starts[m] + 1 + i, and HashPartitioner::<usize> places each item by its position.  glom() lists the items per partition
+    (in map-id, then input order), collect() concatenates them.  An item of one column comes back as an array; pairs come
+    back as a tuple of two arrays, byte strings as an object array of str or bytes.
+    With a communicator (Context.comm_init) every rank maps its contiguous block of map partitions, the library's NCCL
+    exchange moves each partition to its owner (partition p on rank p % world), and a rank's glom() holds its own
+    partitions (the others empty)."""
+
+    def __init__(self, parent, num_partitions, starts, cols, bcol, bytes_first):
+        self.sc, self.parent, self.num_slices, self.starts = parent.sc, parent, num_partitions, starts
+        self.cols, self.bcol, self.bytes_first = tuple(cols), bcol, bytes_first
+        self._sh = None
+
+    def _run(self):
+        if self._sh is not None:
+            return self._sh
+        bounds = slice_starts(self.parent.n, self.parent.num_slices)
+        n_map = len(bounds) - 1
+        rank, world = self.sc.comm or (0, 1)
+        sh = RepShuffle(self.sc, n_map, self.num_slices, [c.code for c in self.cols], self.bcol is not None,
+                        as_str=getattr(self.bcol, "as_str", True), rank=rank, world=world)
+        for m in range((rank * n_map) // world, ((rank + 1) * n_map) // world):
+            sh.map_items(m, self.starts[m], self.cols, self.bcol, int(bounds[m]), int(bounds[m + 1]))
+        if world > 1:
+            sh.exchange(L.VB_XCHG_NCCL)
+        sh.seal()
+        self._sh = sh
+        return sh
+
+    def _item(self, cols, items):
+        parts = list(cols)
+        if items is not None:
+            parts.insert(0 if self.bytes_first else len(parts), items)
+        return parts[0] if len(parts) == 1 else tuple(parts)
+
+    def compute(self, split):
+        return self._item(*self._run().reduce(split))
+
+    def glom(self):
+        return [self.compute(r) for r in range(self.num_slices)]
+
+    def collect(self):
+        parts = self.glom()
+        if isinstance(parts[0], tuple):
+            return tuple(np.concatenate([p[j] for p in parts]) for j in range(len(parts[0])))
+        return np.concatenate(parts)
+
+
 class PairRdd(_Base):
     """PairRdd<K,V> source (ParallelCollection of (K,V)); methods per src/rdd/pair_rdd.rs."""
 
@@ -1096,6 +1240,20 @@ class PairRdd(_Base):
         flatten the values; `glom()` = values per partition."""
         return _Repartitioned(ShuffledRdd(self, "group", num_splits))
 
+    def repartition(self, num_partitions, starts=None):
+        """coalesce(num_partitions, shuffle=true) of the (k, v) items: see RepartitionedRdd."""
+        return self.coalesce(num_partitions, True, starts)
+
+    def coalesce(self, num_partitions, shuffle=False, starts=None):
+        """rdd.rs:386-418 over (k, v) items: two 64-bit columns, or a key column and byte-string values.  starts: vega's
+        start_m of each map partition (default 0)."""
+        if isinstance(self.vals, _BytesCol):
+            return _repartition(self, num_partitions, shuffle, starts, (self.keys,), self.vals)
+        if len(self.cols) > 1:
+            raise NotImplementedError("repartition of items with several value columns")
+        keys = _split_rows(self.keys) if self.keys.rows else (self.keys,)
+        return _repartition(self, num_partitions, shuffle, starts, keys + tuple(self.cols))
+
 
 class _Repartitioned:
     def __init__(self, sh):
@@ -1157,6 +1315,15 @@ class Rdd(_Base):
         return PairRdd(self.sc, _Col(k), _Col(owner, role="value"), self.num_slices).group_by_key(num_splits or self.number_of_splits_exact())
 
     group_by_with_num_partitions = group_by
+
+    def repartition(self, num_partitions, starts=None):
+        """rdd.rs:386-390 `repartition(n)` = coalesce(n, shuffle=true): see RepartitionedRdd."""
+        return self.coalesce(num_partitions, True, starts)
+
+    def coalesce(self, num_partitions, shuffle=False, starts=None):
+        """rdd.rs:392-418.  shuffle=True spreads the items evenly over num_partitions partitions; starts are vega's start_m
+        of each map partition (one u64 each, default 0).  shuffle=False (the narrow CoalescedRdd) is not served."""
+        return _repartition(self, num_partitions, shuffle, starts, (self.keys,))
 
     def number_of_splits_exact(self):
         return len(slice_starts(self.n, self.num_slices)) - 1
@@ -1748,6 +1915,12 @@ class StrPairRdd(PairRdd):
     def partition_by_key(self, num_splits):
         return _Repartitioned(StrShuffledRdd(self, "group", num_splits))
 
+    def coalesce(self, num_partitions, shuffle=False, starts=None):
+        """rdd.rs:386-418 over (String, v) items with one 64-bit value column; returns (str keys, values) per partition."""
+        if isinstance(self.vals, _BytesCol) or len(self.cols) != 1:
+            raise NotImplementedError("repartition of String-key items with byte-string or several value columns")
+        return _repartition(self, num_partitions, shuffle, starts, self.cols, _BytesCol(self.keys.owner), bytes_first=True)
+
     join = _no_str("join")
     left_outer_join = _no_str("left_outer_join")
     right_outer_join = _no_str("right_outer_join")
@@ -2029,6 +2202,11 @@ class StrRdd(Rdd):
         return _Distinct(StrShuffledRdd(_StrKeysOnly(self), "count", n_splits))
 
     distinct_with_num_partitions = distinct
+
+    def coalesce(self, num_partitions, shuffle=False, starts=None):
+        """rdd.rs:386-418 over String items; partitions come back as object arrays of str."""
+        return _repartition(self, num_partitions, shuffle, starts, (), _BytesCol(self.keys.owner))
+
     sort = _no_str("sort")
     intersection = _no_str("intersection")
     intersection_with_num_partitions = intersection
