@@ -83,6 +83,16 @@ enum vb_dtype { VB_U64 = 0, VB_I64 = 1, VB_F64 = 2, VB_BYTES = 3 };
  * f64 MIN/MAX fold Rust's f64::min / f64::max over a key's values: a NaN value is ignored,
  * the result is NaN only when every value of the key is NaN (payload unspecified), and
  * -0.0 < +0.0, so the result does not depend on the order of the rows.
+ * f64 SUM adds a key's values in an unspecified order (any tree of IEEE round-to-nearest
+ * additions), from the additive identity -0.0.  The result is NaN if a value is NaN or both
+ * +inf and -inf occur; else +inf (-inf) if +inf (-inf) occurs, or NaN when the finite values
+ * of the other sign can overflow in some order.  A zero sum is -0.0 exactly when every value
+ * is -0.0 (vega folds from the first value: -0.0 + -0.0 = -0.0), else +0.0.  Otherwise, when
+ * every partial sum is representable (all values multiples of 2^q, sum |x| <= 2^(53+q)), it
+ * is the exact sum bit for bit in every order; else it is within gamma(m-1) * sum |x| of
+ * the exact sum (m values, gamma(k) = k*2^-53 / (1 - k*2^-53)), and may also be +-inf (or
+ * NaN, when both signs can) when the positive (negative) values' sum times 1 + gamma(m-1)
+ * reaches the overflow threshold 2^1024 - 2^970.
  * SORT over f64 keys orders them by f64::total_cmp (-NaN < -inf < ... < -0.0 < +0.0 < ...
  * < +inf < +NaN); "equal keys", which a range cut never separates, are bit-equal keys.     */
 enum vb_agg {
@@ -256,7 +266,8 @@ VB_API int32_t vb_shuffle_reduce(vb_shuf *s, uint32_t reduce_id, void *out_keys,
  *         compares, f64 MIN/MAX as f64::min / f64::max with NaN ignored); output dtype = the column's dtype.
  *   COUNT rows of the key (src ignored); output u64.
  *   MEAN  f64: for u64 / i64 columns (double)S / (double)n, S = the 64-bit wrapping sum read with the column's
- *         signedness, so it is exact only while the key's sum does not wrap; for f64 columns the f64 SUM / n.
+ *         signedness, so it is exact only while the key's sum does not wrap; for f64 columns the f64 SUM (the
+ *         vb_agg rules: NaN, +-inf and a zero's sign included) / (double)n, so an all -0.0 key averages to -0.0.
  * A MEAN keeps a SUM accumulator and shares one COUNT accumulator (the spec's own COUNT if it has one, else an
  * internal one); that internal COUNT counts against VB_MAX_AGGS.  Keys are placed by MetroHash64_1(k) % n_reduce,
  * the same partition as any single-column shuffle of the same keys; vb_shuffle_set_key_width / set_hint apply.

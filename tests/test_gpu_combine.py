@@ -3,10 +3,9 @@ single-column references.
 
 Every output column is checked on its own: integer SUM/MIN/MAX, COUNT and f64 MIN/MAX bit for bit against the CPU
 oracle's single-column shuffle, f64 SUM with tests/util.py:assert_f64_sums, integer MEAN as (double)oracle_sum /
-oracle_count with the sum read with the column's signedness, and f64 MEAN within the f64 SUM bound divided by the
-count.  Each path asserts the statistic that proves it ran."""
+oracle_count with the sum read with the column's signedness, and f64 MEAN as the f64 SUM outcome of
+tests/f64_sum_ref.py divided by the count.  Each path asserts the statistic that proves it ran."""
 import ctypes
-import math
 from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
@@ -15,6 +14,7 @@ import pytest
 import vega_b200 as vb
 from oracle import oracle as O
 from tests.test_gpu_reduce_paths import _col, _dev
+from tests import f64_sum_ref as F
 from tests.util import assert_f64_sums, assert_parts_equal, bits_dict, oracle_reduce_bits, rand_pairs
 from vega_b200 import _lib as L
 from vega_b200.rdd import Shuffle, _Col
@@ -45,6 +45,11 @@ def sc():
     c.close()
 
 
+def spec_of(spec):
+    """(value dtypes with modes, aggregates) of a SPECS name, or such a pair itself."""
+    return SPECS[spec] if isinstance(spec, str) else spec
+
+
 def make_data(seed, spec, n, n_keys, hot=0.0):
     """Keys and the value columns of a spec.  The keys come with the first f64 column (cancelling pairs share a key);
     the other columns are drawn independently over the same rows."""
@@ -57,14 +62,14 @@ def make_data(seed, spec, n, n_keys, hot=0.0):
 
 
 def out_dtype(spec, a):
-    op, c = SPECS[spec][1][a]
-    return np.uint64 if op == "count" else np.float64 if op == "mean" else NP[SPECS[spec][0][c][0]]
+    op, c = spec_of(spec)[1][a]
+    return np.uint64 if op == "count" else np.float64 if op == "mean" else NP[spec_of(spec)[0][c][0]]
 
 
 def run_combine(sc, spec, kcol, vcols, n, M, R, hint=0, key_width=8, dst=L.VB_HOST):
     """One multi-aggregate shuffle: M map tasks over rows [0, n) as ParallelCollection slices them, seal, every
     reduce partition as (keys, [column per aggregate])."""
-    dts, aggs = SPECS[spec]
+    dts, aggs = spec_of(spec)
     starts = vb.slice_starts(n, M)
     sh = Shuffle(sc, len(starts) - 1, R, L.VB_U64, L.VB_U64, L.VB_AGG_SUM, key_width=key_width, hint=hint,
                  multi=([CODE[d] for d, _ in dts], [(AGG[op], c) for op, c in aggs]))
@@ -90,34 +95,18 @@ def run_combine(sc, spec, kcol, vcols, n, M, R, hint=0, key_width=8, dst=L.VB_HO
     return parts, st
 
 
-def check_f64_means(got_parts, keys, vals):
-    """Per key: |mean - fsum/m| <= (gamma(m-1) * sum|x| + ulp(fsum)) / m + ulp(mean), finite inputs only."""
-    keys = np.ascontiguousarray(keys).view(np.uint64)
-    order = np.argsort(keys, kind="stable")
-    ks, vs = keys[order], np.asarray(vals, dtype=np.float64)[order]
-    starts = np.flatnonzero(np.r_[True, ks[1:] != ks[:-1]])
-    ends = np.r_[starts[1:], len(ks)]
+def check_f64_means(got_parts, keys, vals, exact=False, lenient=None):
+    """Per key: a mean tests/f64_sum_ref.py admits, the SUM outcome over the count: fl(sum / m) bit for bit where the
+    sum is exact, NaN and infinities as the sum's, within the SUM bound over m (plus the division's rounding) otherwise."""
     got = {}
     for d in got_parts:
         got.update(d)
-    assert set(got) == set(ks[starts].tolist())
-    u = 2.0 ** -53
-    vl = vs.tolist()
-    bad = []
-    for s, e in zip(starts.tolist(), ends.tolist()):
-        k, m = int(ks[s]), e - s
-        g = got[k]
-        x = vl[s:e]
-        want = math.fsum(x)
-        gamma = (m - 1) * u / (1 - (m - 1) * u)
-        bound = (gamma * sum(abs(v) for v in x) * (1 + 2 * m * u) + math.ulp(want)) / m + math.ulp(g)
-        if not abs(g - want / m) <= bound:
-            bad.append((hex(k), m, g, want / m))
-    assert not bad, f"{len(bad)} f64 means wrong (key, rows, got, want): {bad[:5]}"
+    F.assert_outcomes(got, F.key_outcomes(keys, vals, mean=True), "f64 means", exact=exact, lenient=lenient)
 
 
-def check_combine(parts, spec, keys, cols, R, key_width=8):
-    dts, aggs = SPECS[spec]
+def check_combine(parts, spec, keys, cols, R, key_width=8, lenient=None):
+    """lenient: the keys whose f64 SUM / MEAN may take more than one outcome class (tests/f64_sum_ref.py)."""
+    dts, aggs = spec_of(spec)
     kw = key_width
     oracle = {}
 
@@ -132,10 +121,10 @@ def check_combine(parts, spec, keys, cols, R, key_width=8):
         d, mode = dts[c]
         if op == "sum" and d == "f64":
             got = [dict(zip(k.view(np.uint64).tolist(), o[a].tolist())) for k, o in parts]
-            assert_f64_sums(got, keys, cols[c], R, key_width=kw, exact=mode in ("exact", "subnormal"))
+            assert_f64_sums(got, keys, cols[c], R, key_width=kw, exact=mode in ("exact", "subnormal"), lenient=lenient)
         elif op == "mean" and d == "f64":
             got = [dict(zip(k.view(np.uint64).tolist(), o[a].tolist())) for k, o in parts]
-            check_f64_means(got, keys, cols[c])
+            check_f64_means(got, keys, cols[c], exact=mode in ("exact", "subnormal"), lenient=lenient)
         elif op == "mean":
             sums = ref("sum", c)
             want = []
@@ -166,7 +155,7 @@ PATHS = {
 
 
 def _cols(keys, cols, spec, device, misalign=False):
-    dts = SPECS[spec][0]
+    dts = spec_of(spec)[0]
     if not device:
         return _Col(keys), tuple(_Col(c, role="value") for c in cols)
     return _col(_dev(keys, misalign), L.VB_U64), tuple(_col(_dev(c, misalign), CODE[d]) for c, (d, _) in zip(cols, dts))

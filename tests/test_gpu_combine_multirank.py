@@ -16,7 +16,7 @@ import vega_b200 as vb
 from tests import cogroup_n_ref as CN
 from tests import multirank as MR
 from tests.test_gpu_cogroup_n import abi_parts_n, join_parts_n
-from tests.test_gpu_combine import AGG, CODE, SPECS, check_combine, make_data, out_dtype, run_combine
+from tests.test_gpu_combine import AGG, CODE, SPECS, check_combine, make_data, out_dtype, run_combine, spec_of
 from tests.util import EMPTY_KEY, assert_parts_equal, bits_dict, rand_pairs
 from vega_b200 import _lib as L
 from vega_b200.dist import CudaEngine
@@ -32,7 +32,7 @@ def sc():
 
 
 def multi_of(spec):
-    dts, aggs = SPECS[spec]
+    dts, aggs = spec_of(spec)
     return [CODE[d] for d, _ in dts], [(AGG[o], c) for o, c in aggs]
 
 
@@ -94,7 +94,7 @@ def run_ranks(sc, W, spec, keys, cols, M, R, loc="host", hint=0, key_width=8, re
         for sh in shs:
             sh.seal()
         exports = kept
-    outs = [out_dtype(spec, a) for a in range(len(SPECS[spec][1]))]
+    outs = [out_dtype(spec, a) for a in range(len(spec_of(spec)[1]))]
     parts = [None] * R
     for d, sh in enumerate(shs):
         for r in range(R):

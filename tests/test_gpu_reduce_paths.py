@@ -2,8 +2,9 @@
 
 Each path asserts the statistic that proves it ran, so a change in kernel selection fails here instead of silently
 testing another path.  Integer ops, COUNT and f64 MIN/MAX are compared bit for bit with the CPU oracle (NaN results
-as one bit pattern); f64 SUM is compared with math.fsum per key by tests/util.py:assert_f64_sums, bit-exact on values
-whose partial sums are all representable and within the order-independent error bound otherwise."""
+as one bit pattern); f64 SUM is checked per key by tests/util.py:assert_f64_sums against the exact reference of
+tests/f64_sum_ref.py, bit-exact on values whose partial sums are all representable and within the order-independent
+error bound otherwise."""
 import numpy as np
 import pytest
 

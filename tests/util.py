@@ -4,6 +4,7 @@ import math
 import numpy as np
 
 from oracle import oracle as O
+from tests import f64_sum_ref as F
 
 MASK64 = (1 << 64) - 1
 EMPTY_KEY = MASK64                       # the device table's empty marker: a real key with this value takes the special slot
@@ -156,19 +157,19 @@ def assert_parts_equal(got, want):
                      f"first wrong (key, got, want)): {bad[:4]}")
 
 
-def assert_f64_sums(got_parts, keys, vals, R, key_width=8, exact=False):
-    """Check an f64 SUM result against the exact per-key sum, for every key.
+def assert_f64_sums(got_parts, keys, vals, R, key_width=8, exact=False, lenient=None):
+    """Check an f64 SUM result against tests/f64_sum_ref.py, the results some summation order can give, for every key.
 
     got_parts: one {key: sum} dict per reduce partition.  For each key of the input:
       * it is in partition hash(key) % R, and only there;
-      * a key with a NaN, or with both +inf and -inf, sums to NaN; otherwise a key with an inf sums to that inf;
-      * otherwise, with s = math.fsum of its m values, |got - s| <= gamma(m-1) * sum|x| (+ the rounding of s),
-        gamma(k) = k*u / (1 - k*u), u = 2^-53.  Every summation order meets this bound (atomics in any order, hot-key
-        partial sums, per-map partial sums merged at seal), and it holds under cancellation;
-      * exact=True (values whose partial sums are all representable): got == s, bit for bit up to the sign of zero.
+      * its sum is one the reference admits: NaN for a NaN or both infinities, the infinity present otherwise, the
+        exact sum bit for bit (the sign of a zero included) when every partial sum is representable, and within
+        gamma(m-1) * sum|x| of the exact sum otherwise.  Every summation order meets these (atomics in any order,
+        hot-key partial sums, per-map partial sums merged at seal, other ranks' partial sums);
+      * exact=True: the reference must pin every key to one value (the case's values have representable partial sums);
+      * lenient: the keys allowed more than one outcome class (those whose partial sums can overflow); None: any key.
     """
     keys = np.ascontiguousarray(keys).view(np.uint64)
-    vals = np.ascontiguousarray(vals, dtype=np.float64)
     assert len(got_parts) == R
     got = {}
     for r, d in enumerate(got_parts):
@@ -177,37 +178,4 @@ def assert_f64_sums(got_parts, keys, vals, R, key_width=8, exact=False):
             assert k not in got, f"key {k:#x} in two partitions"
             assert O.get_partition(k, R, key_width) == r, f"key {k:#x} in partition {r}"
             got[k] = float(v)
-    if len(keys) == 0:
-        assert not got
-        return
-    order = np.argsort(keys, kind="stable")
-    ks, vs = keys[order], vals[order]
-    starts = np.flatnonzero(np.r_[True, ks[1:] != ks[:-1]])
-    ends = np.r_[starts[1:], len(ks)]
-    uniq = ks[starts].tolist()
-    missing = set(uniq) - set(got)
-    extra = set(got) - set(uniq)
-    assert not missing and not extra, f"{len(missing)} keys missing, {len(extra)} keys not in the input"
-    m = (ends - starts).astype(np.float64)
-    u = 2.0 ** -53
-    gamma = (m - 1) * u / (1 - (m - 1) * u)
-    finite = np.isfinite(vs)
-    abs_sum = np.add.reduceat(np.where(finite, np.abs(vs), 0.0), starts) * (1 + 2 * m * u)   # covers its own rounding
-    has_nan = np.logical_or.reduceat(np.isnan(vs), starts)
-    has_pinf = np.logical_or.reduceat(vs == math.inf, starts)
-    has_ninf = np.logical_or.reduceat(vs == -math.inf, starts)
-    vl = vs.tolist()
-    bad = []
-    for i, k in enumerate(uniq):
-        g = got[k]
-        if has_nan[i] or (has_pinf[i] and has_ninf[i]):
-            ok, want = math.isnan(g), math.nan
-        elif has_pinf[i] or has_ninf[i]:
-            want = math.inf if has_pinf[i] else -math.inf
-            ok = g == want
-        else:
-            want = math.fsum(vl[starts[i]:ends[i]])
-            ok = g == want if exact else abs(g - want) <= gamma[i] * abs_sum[i] + math.ulp(want)
-        if not ok:
-            bad.append((hex(k), int(m[i]), g, want))
-    assert not bad, f"{len(bad)} of {len(uniq)} f64 sums wrong (key, rows, got, exact): {bad[:5]}"
+    F.assert_outcomes(got, F.key_outcomes(keys, vals), exact=exact, lenient=lenient)

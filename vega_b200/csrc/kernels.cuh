@@ -49,7 +49,9 @@ struct TableCtl {
 enum : int { IN_AOS = 0, IN_SOA = 1, IN_TABLE = 2, IN_ACCS = 3 };   // IN_ACCS: received partials (hash_agg_multi_kernel)
 enum : int { OPK_ADD_U64 = 0, OPK_ADD_F64 = 1, OPK_MIN_U64 = 2, OPK_MAX_U64 = 3, OPK_COUNT = 4, OPK_DICT = 5 };
 
-VB_HD u64 op_identity(int opk) { return opk == OPK_MIN_U64 ? ~0ull : 0ull; }
+// f64 ADD starts from -0.0, the IEEE additive identity (-0.0 + x == x for every x, +0.0 included): a key whose values
+// are all -0.0 sums to -0.0, as vega's fold from the first value does, and any other zero sum to +0.0, in every order.
+VB_HD u64 op_identity(int opk) { return opk == OPK_MIN_U64 ? ~0ull : opk == OPK_ADD_F64 ? 0x8000000000000000ull : 0ull; }
 
 template <int OPK>
 VB_D void op_red(u64 *acc, u64 v)
