@@ -485,6 +485,24 @@ VB_API int32_t vb_shuffle_reduce_str_size(vb_shuf *s, uint32_t reduce_id, uint64
 VB_API int32_t vb_shuffle_reduce_str(vb_shuf *s, uint32_t reduce_id, uint64_t *out_key_offsets /*n_keys+1*/,
                                      void *out_key_bytes, void *out_combined, uint64_t *out_offsets /*n_keys+1*/,
                                      void *out_vals, int32_t dst_loc);
+/* Byte-slice keys: the string-key shuffle placing keys as Rust hashes `Vec<u8>` (HashPartitioner::get_partition,
+ * src/partitioner.rs:29-60, over `Vec<u8>`, `&[u8]`, `Box<[u8]>` or `[u8; N]` keys).  `<[u8] as Hash>` writes the
+ * length as a usize and then the bytes, so
+ *   placement  VB_STRKEY_BYTES: MetroHash64_1(le64(len) ‖ bytes, seed 0) % n_reduce (vb_hash_bytes /
+ *              vb_get_partition_bytes); VB_STRKEY_STR, the default: the `String` placement above.
+ * Nothing else depends on the kind: keys are equal when their bytes are, sort in `<[u8] as Ord>` order (the `String`
+ * order), and bincode writes `Vec<u8>`, `&[u8]` and `Box<[u8]>` as u64 len | bytes, as it writes a `String`, so the
+ * reduce-op blobs below are the same bytes for both kinds (a `[u8; N]` is written with no length: not a blob of these).
+ * vb_shuffle_set_str_key sets the kind of a shuffle of any vb_shuffle_create_str* call (plain, _dist, _multi(_dist),
+ * _sort(_dist), _sort_bytes(_dist), _bytes_dist) before its first map, blob or import call (VB_ERR_STATE after one, or
+ * after seal); VB_ERR_INVALID for any other shuffle or kind.  Checked: vb_cogroup_n_str / vb_join_n_str (and _size)
+ * refuse sides of different kinds (VB_ERR_INVALID, every side staying usable); vb_shuffle_create_narrow_str gives the
+ * view its parent's kind; vb_shuffle_exchange of a reduce-op or combine_by_key shuffle refuses, on every rank and before
+ * any send, a rank whose kind differs (VB_ERR_INVALID).  Not checked: the GROUP exchanges and the export / import calls
+ * carry no kind, so every rank of a shuffle must set the same one.  A sort places rows by cut keys, not by hash: the
+ * kind changes none of its output.                                                                                   */
+enum vb_str_key { VB_STRKEY_STR = 0, VB_STRKEY_BYTES = 1 };
+VB_API int32_t vb_shuffle_set_str_key(vb_shuf *s, int32_t kind /*vb_str_key*/);
 /* Cogroup and join of string-key shuffles, for one partition: vb_cogroup_n and vb_join_n_outer with keys compared as
  * byte strings (CoGroupedRdd::compute over `String` keys, co_grouped_rdd.rs:75-135, 206-249).  Each side is a sealed
  * GROUP shuffle of vb_shuffle_create_str (the calls block until every side is sealed); 1 <= n_sides <=
@@ -834,6 +852,9 @@ VB_API int32_t vb_shuffle_import_str_bytes(vb_shuf *s, const uint32_t *key_lens,
 /* MetroHash64_1(bytes ‖ 0xFF, seed 0): the reference's hash of a `String` / `&str` key */
 VB_API uint64_t vb_hash_str(const void *bytes, uint64_t len);
 VB_API uint32_t vb_get_partition_str(const void *bytes, uint64_t len, uint32_t n_reduce);
+/* MetroHash64_1(le64(len) ‖ bytes, seed 0): the reference's hash of a `Vec<u8>` / `&[u8]` / `[u8; N]` key */
+VB_API uint64_t vb_hash_bytes(const void *bytes, uint64_t len);
+VB_API uint32_t vb_get_partition_bytes(const void *bytes, uint64_t len, uint32_t n_reduce);
 
 /* ---- SURVEY §8(f) N1: bincode blobs — the payload format of SHUFFLE_CACHE ------------------------
  * The reference serialises every (map, reduce) bucket with bincode 1.2.1 defaults (src/dependency.rs:213-214:

@@ -94,6 +94,13 @@ public:
     template <typename V>
     StrPairRddT<V> parallelize(const std::vector<std::pair<std::string, V>> &data, size_t num_slices) { return make_rdd(data, num_slices); }
     StrKeyRddT parallelize(const std::vector<std::string> &data, size_t num_slices);
+    // byte-slice keys (Rust Vec<u8> / &[u8] / [u8; N]): the String-key RDDs with the keys placed as a Vec<u8> hashes
+    // (vb_shuffle_set_str_key(VB_STRKEY_BYTES)); results carry each key's bytes in a std::string
+    template <typename V>
+    StrPairRddT<V> make_rdd(const std::vector<std::pair<std::vector<uint8_t>, V>> &data, size_t num_slices);
+    template <typename V>
+    StrPairRddT<V> parallelize(const std::vector<std::pair<std::vector<uint8_t>, V>> &data, size_t num_slices) { return make_rdd(data, num_slices); }
+    StrKeyRddT parallelize(const std::vector<std::vector<uint8_t>> &data, size_t num_slices);
 
 private:
     Context() = default;
@@ -583,7 +590,9 @@ namespace detail {
 struct StrCol {
     std::vector<uint64_t> offs{0};
     std::string bytes;
+    int32_t kind = VB_STRKEY_STR;         // how the shuffles of this column place its keys (vb_shuffle_set_str_key)
     void push(const std::string &k) { bytes += k; offs.push_back(bytes.size()); }
+    void push(const std::vector<uint8_t> &k) { bytes.append(k.begin(), k.end()); offs.push_back(bytes.size()); }
     uint64_t size() const { return offs.size() - 1; }
 };
 
@@ -597,6 +606,7 @@ inline ShufPtr run_str_shuffle(Context &sc, const StrCol &keys, const std::vecto
     vb_shuf *raw = nullptr;
     check(vb_shuffle_create_str(sc.raw(), sc.new_shuffle_id(), (uint32_t)n_map, (uint32_t)num_splits, vcode, agg, &raw));
     ShufPtr s(raw);
+    if (keys.kind != VB_STRKEY_STR) check(vb_shuffle_set_str_key(raw, keys.kind));
     for (uint64_t m = 0; m < n_map; ++m) {
         const uint64_t lo = starts[m], cnt = starts[m + 1] - lo;
         check(vb_shuffle_map_str(raw, (uint32_t)m, keys.offs.data() + lo, keys.bytes.data(), keys.bytes.size(),
@@ -694,6 +704,12 @@ public:
     {
         for (auto &kv : data) { keys_.push(kv.first); vals_.push_back(detail::to_bits<V>(kv.second)); }
     }
+    StrPairRddT(std::shared_ptr<Context> sc, const std::vector<std::pair<std::vector<uint8_t>, V>> &data, size_t num_slices)
+        : sc_(std::move(sc)), num_slices_(num_slices)
+    {
+        keys_.kind = VB_STRKEY_BYTES;
+        for (auto &kv : data) { keys_.push(kv.first); vals_.push_back(detail::to_bits<V>(kv.second)); }
+    }
     size_t number_of_splits() const { return num_slices_; }
 
     // group_by_key(num_splits).collect()  →  Vec<(String, Vec<V>)>, values in input order
@@ -763,6 +779,7 @@ public:
         check(vb_shuffle_create_str_multi(sc_->raw(), sc_->new_shuffle_id(), (uint32_t)n_map, (uint32_t)num_splits, 1, &vcode,
                                           (uint32_t)spec.size(), spec.data(), &raw));
         detail::ShufPtr s(raw);
+        if (keys_.kind != VB_STRKEY_STR) check(vb_shuffle_set_str_key(raw, keys_.kind));
         for (uint64_t m = 0; m < n_map; ++m) {
             const uint64_t lo = starts[m], cnt = starts[m + 1] - lo;
             const void *col = cnt ? vals_.data() + lo : nullptr;
@@ -960,6 +977,12 @@ public:
     {
         for (auto &k : data) keys_.push(k);
     }
+    StrKeyRddT(std::shared_ptr<Context> sc, const std::vector<std::vector<uint8_t>> &data, size_t num_slices)
+        : sc_(std::move(sc)), num_slices_(num_slices)
+    {
+        keys_.kind = VB_STRKEY_BYTES;
+        for (auto &k : data) keys_.push(k);
+    }
     // count_by_value().collect() → Vec<(String, u64)>   (src/rdd/rdd.rs:450-459)
     std::vector<std::pair<std::string, uint64_t>> count_by_value() const
     {
@@ -994,6 +1017,15 @@ Context::StrPairRddT<V> Context::make_rdd(const std::vector<std::pair<std::strin
     return StrPairRddT<V>(shared_from_this(), data, num_slices);
 }
 inline Context::StrKeyRddT Context::parallelize(const std::vector<std::string> &data, size_t num_slices)
+{
+    return StrKeyRddT(shared_from_this(), data, num_slices);
+}
+template <typename V>
+Context::StrPairRddT<V> Context::make_rdd(const std::vector<std::pair<std::vector<uint8_t>, V>> &data, size_t num_slices)
+{
+    return StrPairRddT<V>(shared_from_this(), data, num_slices);
+}
+inline Context::StrKeyRddT Context::parallelize(const std::vector<std::vector<uint8_t>> &data, size_t num_slices)
 {
     return StrKeyRddT(shared_from_this(), data, num_slices);
 }

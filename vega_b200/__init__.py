@@ -8,7 +8,7 @@ Importing works without a GPU (so the C ABI can be inspected); computing does no
 from ._lib import (LIB_PATH, SYMBOLS, VegaB200Error, lib)  # noqa: F401
 from .rdd import (AggregateRdd, CoGroupedRdd, CombinedRdd, Context, Grouped, JoinedRdd, PairRdd, Rdd, RepartitionedRdd, RepShuffle,  # noqa: F401
                   Shuffle, ShuffledRdd,
-                  StrAggregateRdd, StrCoGroupedRdd, StrCombinedRdd, StrKeys, StrPairRdd, StrRdd, StrShuffle, StrShuffledRdd, StrSortedRdd, slice_starts)
+                  BytesKeys, StrAggregateRdd, StrCoGroupedRdd, StrCombinedRdd, StrKeys, StrPairRdd, StrRdd, StrShuffle, StrShuffledRdd, StrSortedRdd, slice_starts)
 
 __all__ = ["Context", "PairRdd", "CoGroupedRdd", "CombinedRdd", "AggregateRdd", "Rdd", "RepartitionedRdd", "RepShuffle", "Shuffle", "ShuffledRdd", "JoinedRdd", "Grouped", "slice_starts",
-           "StrAggregateRdd", "StrCoGroupedRdd", "StrCombinedRdd", "StrKeys", "StrPairRdd", "StrRdd", "StrShuffle", "StrShuffledRdd", "StrSortedRdd", "VegaB200Error", "lib", "LIB_PATH", "SYMBOLS"]
+           "BytesKeys", "StrAggregateRdd", "StrCoGroupedRdd", "StrCombinedRdd", "StrKeys", "StrPairRdd", "StrRdd", "StrShuffle", "StrShuffledRdd", "StrSortedRdd", "VegaB200Error", "lib", "LIB_PATH", "SYMBOLS"]

@@ -4414,6 +4414,7 @@ extern "C" int32_t vb_join(vb_shuf *l, vb_shuf *r, uint32_t rid, void *out_k, vo
 // One shuffle's dictionary of distinct keys (strkeys.cuh: entries + arena + index), the map calls' rows as entry ids,
 // and after seal the partition-major key column (Arrow-style offsets + bytes) beside the usual res_* arrays.
 struct StrState {
+    int kind = STRKEY_STR;                // how the keys hash (vb_shuffle_set_str_key): placement only
     StrDict d{};                          // device arrays; d.fp / d.id have 1 << d.log_cap slots
     u64 cap_e = 0, cap_a = 0;             // entries / arena bytes reserved
     u32 n_e = 0;                          // entries in use (ctl->n_entries after the last call)
@@ -4585,6 +4586,22 @@ extern "C" int32_t vb_shuffle_create_str_sort_bytes(vb_ctx *c, uint64_t shuffle_
     return VB_OK;
 }
 
+// How the keys of a string shuffle hash: as `String` (the default) or as a byte slice (`Vec<u8>`).  Only the placement
+// changes, so the kind may be chosen until the first map, blob or import call, and not after.
+extern "C" int32_t vb_shuffle_set_str_key(vb_shuf *s, int32_t kind)
+{
+    if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
+    if (!s->str) return set_err(VB_ERR_INVALID, "vb_shuffle_set_str_key: shuffle %llu has no string keys (vb_shuffle_create_str*)", (unsigned long long)s->id);
+    if (kind != VB_STRKEY_STR && kind != VB_STRKEY_BYTES)
+        return set_err(VB_ERR_INVALID, "vb_shuffle_set_str_key: kind %d (VB_STRKEY_STR or VB_STRKEY_BYTES)", kind);
+    std::lock_guard<std::mutex> g(s->mu);
+    bool started = s->exported || s->imported || s->sealed || s->sealing || s->freed;
+    for (const MapOut &m : s->maps) started = started || m.present;
+    if (started) return set_err(VB_ERR_STATE, "vb_shuffle_set_str_key: shuffle %llu already has map output", (unsigned long long)s->id);
+    s->str->kind = kind == VB_STRKEY_BYTES ? STRKEY_BYTES : STRKEY_STR;
+    return VB_OK;
+}
+
 // Reallocate one device array to `cap` elements of `sz` bytes, keeping the first `keep`.
 template <typename T>
 static int str_regrow(vb_ctx *c, T **p, u64 cap, u64 keep)
@@ -4719,7 +4736,10 @@ static int str_encode(vb_shuf *s, const u64 *offs, const unsigned char *bytes, u
         {
             KLaunch kl(s, K_DICT, n);
             const u64 blocks = std::min<u64>((n + 255) / 256, (u64)c->sm_count * 8);
-            str_encode_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(offs, bytes, first, n, t->d, t->ctl, max_entries, ids);
+            if (t->kind == STRKEY_BYTES)
+                str_encode_kernel<STRKEY_BYTES><<<(unsigned)blocks, 256, 0, c->stream>>>(offs, bytes, first, n, t->d, t->ctl, max_entries, ids);
+            else
+                str_encode_kernel<STRKEY_STR><<<(unsigned)blocks, 256, 0, c->stream>>>(offs, bytes, first, n, t->d, t->ctl, max_entries, ids);
             TRY(kl.done("str_encode_kernel"));
         }
         StrCtl h;
@@ -7159,7 +7179,8 @@ extern "C" int32_t vb_shuffle_import_str_cols(vb_shuf *s, const uint32_t *key_le
 // vb_shuffle_exchange of a string-key reduce op or combine: export, then the exchange of 2 + n_acc columns: u32 key
 // lengths and the n_acc u64 accumulator columns split by the key counts, key bytes by the byte counts.  The gathered
 // row is the key and byte counts to every destination, then exchange_multi_locked's spec fingerprint (no key width:
-// keys are strings), so a rank whose op or spec differs is refused on every rank before any send.
+// keys are strings; the key kind of vb_shuffle_set_str_key in its place), so a rank whose op, spec or key kind differs
+// is refused on every rank before any send.
 static int exchange_str_accs_locked(vb_shuf *s)
 {
     vb_ctx *c = s->ctx;
@@ -7173,14 +7194,14 @@ static int exchange_str_accs_locked(vb_shuf *s)
     s->xst.prepare_wall_ms += lap(clk);
     row[2 * W] = s->acc_map.op;
     row[2 * W + 1] = s->acc_map.tx;
-    row[2 * W + 2] = (u64)NA | (u64)s->n_reduce << 32;
+    row[2 * W + 2] = (u64)NA | (u64)t->kind << 8 | (u64)s->n_reduce << 32;
     const u64 *mat = nullptr;
     TRY(comm_all_gather(c, row.data(), len, &mat));
     s->xst.counts_wall_ms += lap(clk);
     for (u32 p = 1; p < W; ++p)
         for (u32 i = 0; i < 3; ++i)
             if (mat[p * len + 2 * W + i] != mat[2 * W + i])
-                return set_err(VB_ERR_INVALID, "rank %u's reduce op or combine spec differs from rank 0's (accumulators, ops, transforms or n_reduce)", p);
+                return set_err(VB_ERR_INVALID, "rank %u's reduce op or combine spec differs from rank 0's (accumulators, ops, transforms, key kind or n_reduce)", p);
     for (u32 d = 0; d < W; ++d) {
         const u64 nd = xsplit(mat, len, W, d, 0).roff[W];
         TRY(str_import_limits(s, nd, nd));
@@ -7228,8 +7249,12 @@ static int str_key_index(vb_shuf *s)
     {
         KLaunch kl(s, K_DICT, D);
         const u64 blocks = std::min<u64>((D + 255) / 256, (u64)c->sm_count * 8);
-        str_key_index_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(t->key_off, t->key_bytes, (u32)D, fp.as<u64>(), id.as<u32>(),
-                                                                      log_cap, str_fp_mask(), h.as<u64>());
+        if (t->kind == STRKEY_BYTES)
+            str_key_index_kernel<STRKEY_BYTES><<<(unsigned)blocks, 256, 0, c->stream>>>(t->key_off, t->key_bytes, (u32)D, fp.as<u64>(), id.as<u32>(),
+                                                                                        log_cap, str_fp_mask(), h.as<u64>());
+        else
+            str_key_index_kernel<STRKEY_STR><<<(unsigned)blocks, 256, 0, c->stream>>>(t->key_off, t->key_bytes, (u32)D, fp.as<u64>(), id.as<u32>(),
+                                                                                      log_cap, str_fp_mask(), h.as<u64>());
         TRY(kl.done("str_key_index_kernel"));
     }
     CU(cudaStreamSynchronize(c->stream));
@@ -7288,7 +7313,9 @@ extern "C" int32_t vb_shuffle_create_narrow_str(vb_shuf *p, uint32_t out_col, vb
     v->rank = p->rank; v->world = p->world;
     v->bucket_off = p->bucket_off; v->val_off = p->bucket_off;
     v->n_keys = v->n_vals = v->st.rows_out = p->n_keys;
-    str_attach(v)->kb_off = p->str->kb_off;
+    StrState *vt = str_attach(v);
+    vt->kb_off = p->str->kb_off;
+    vt->kind = p->str->kind;
     int rc;
     {
         std::lock_guard<std::mutex> lk(c->mu);
@@ -7411,6 +7438,9 @@ static int cogroup_n_str_check(vb_shuf *const *sides, u32 n, u32 rid)
         if (!s->str) return set_err(VB_ERR_INVALID, "side %u is not a string-key shuffle (use vb_cogroup_n / vb_join_n_outer)", j);
         if (s->agg != VB_AGG_GROUP) return set_err(VB_ERR_INVALID, "side %u is not a GROUP shuffle", j);
         if (s->n_reduce != sides[0]->n_reduce) return set_err(VB_ERR_INVALID, "side %u uses a different partitioner than side 0", j);
+        if (s->str->kind != sides[0]->str->kind)     // equal bytes sit in different partitions under the two hashes
+            return set_err(VB_ERR_INVALID, "side %u hashes its keys as %s, side 0 as %s", j, s->str->kind == STRKEY_BYTES ? "bytes" : "String",
+                           sides[0]->str->kind == STRKEY_BYTES ? "bytes" : "String");
         if (s->ctx != sides[0]->ctx) return set_err(VB_ERR_INVALID, "side %u lives on a different context than side 0", j);
     }
     if (rid >= sides[0]->n_reduce) return set_err(VB_ERR_INVALID, "reduce_id %u >= n_reduce %u", rid, sides[0]->n_reduce);
@@ -7497,6 +7527,14 @@ extern "C" uint32_t vb_get_partition_str(const void *bytes, uint64_t len, uint32
 {
     if (n_reduce == 0) return 0;
     return (uint32_t)(metro64_1_str((const unsigned char *)bytes, len) % (uint64_t)n_reduce);
+}
+
+extern "C" uint64_t vb_hash_bytes(const void *bytes, uint64_t len) { return metro64_1_bytes((const unsigned char *)bytes, len); }
+
+extern "C" uint32_t vb_get_partition_bytes(const void *bytes, uint64_t len, uint32_t n_reduce)
+{
+    if (n_reduce == 0) return 0;
+    return (uint32_t)(metro64_1_bytes((const unsigned char *)bytes, len) % (uint64_t)n_reduce);
 }
 
 // ---------------------------------------------------------------------------------------------

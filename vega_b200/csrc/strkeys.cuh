@@ -5,6 +5,8 @@
 // A key is a byte run of a caller column (Arrow-style offsets + bytes).  `impl Hash for str` writes the bytes and then
 // one 0xFF byte; the buffering MetroHasher hashes that stream with MetroHash64_1 (seed 0) at finish.  The suffix is
 // never materialised: every word of the stream is assembled from aligned 8-byte loads of the key and the 0xFF byte.
+// A shuffle of byte-slice keys (`Vec<u8>` and kin) hashes `le64(len) ‖ key` instead, built the same way; everything
+// else (equality, order, the dictionary) is the same for both kinds.
 //
 // Dictionary: dense entries (hash, arena offset, length) indexed by a u32 entry id, an arena holding each distinct
 // key's bytes once, and an open-addressing index of 4-slot buckets (fingerprint, entry id).  Entries are the source of
@@ -42,20 +44,41 @@ VB_HD u64 str_word(const unsigned char *p, u64 len, u64 pos, u32 n)
     return v;
 }
 
-// MetroHash64_1(key ‖ 0xFF, seed 0): `str::hash` fed to the reference's MetroHasher (fasthash 0.4.0).
-VB_HD u64 metro64_1_str(const unsigned char *p, u64 len)
+// How a shuffle's keys hash (vb_shuffle_set_str_key): as a Rust `String` / `&str`, or as a byte slice (`Vec<u8>`,
+// `&[u8]`, `Box<[u8]>`, `[u8; N]`), whose `Hash` writes the length as a usize and then the bytes.
+enum { STRKEY_STR = 0, STRKEY_BYTES = 1 };
+
+// Bytes [pos, pos + n) of the hashed stream `le64(len) ‖ key[0..len)` (pos + n <= len + 8).  The stream is at least 8
+// bytes long, so MetroHash64_1 reads its first word whole: pos 0 is always the length word, and every later read lies
+// in the key at pos - 8.
+VB_HD u64 bytes_word(const unsigned char *p, u64 len, u64 pos, u32 n)
+{
+    return pos == 0 ? len : load_le<false>(p, pos - 8, n);
+}
+
+template <int KIND>
+VB_HD u64 key_word(const unsigned char *p, u64 len, u64 pos, u32 n)
+{
+    static_assert(KIND == STRKEY_STR || KIND == STRKEY_BYTES, "String or byte-slice keys");
+    return KIND == STRKEY_STR ? str_word(p, len, pos, n) : bytes_word(p, len, pos, n);
+}
+
+// MetroHash64_1(stream, seed 0) as the reference's MetroHasher (fasthash 0.4.0) computes it at finish.  KIND STRKEY_STR:
+// the stream `str::hash` writes, key ‖ 0xFF; STRKEY_BYTES: the one `<[u8]>::hash` writes, le64(len) ‖ key.
+template <int KIND>
+VB_HD u64 metro64_1_key(const unsigned char *p, u64 len)
 {
     const u64 k0 = 0xC83A91E1ull, k1 = 0x8648DBDBull, k2 = 0x7BDEC03Bull, k3 = 0x2F5870A5ull;
-    const u64 n = len + 1;
+    const u64 n = len + (KIND == STRKEY_STR ? 1 : 8);
     u64 h = (k2 * k0) + n;
     u64 pos = 0;
     if (n >= 32) {
         u64 v0 = h, v1 = h, v2 = h, v3 = h;
         do {
-            v0 += str_word(p, len, pos, 8) * k0;      v0 = rotr64(v0, 29) + v2;
-            v1 += str_word(p, len, pos + 8, 8) * k1;  v1 = rotr64(v1, 29) + v3;
-            v2 += str_word(p, len, pos + 16, 8) * k2; v2 = rotr64(v2, 29) + v0;
-            v3 += str_word(p, len, pos + 24, 8) * k3; v3 = rotr64(v3, 29) + v1;
+            v0 += key_word<KIND>(p, len, pos, 8) * k0;      v0 = rotr64(v0, 29) + v2;
+            v1 += key_word<KIND>(p, len, pos + 8, 8) * k1;  v1 = rotr64(v1, 29) + v3;
+            v2 += key_word<KIND>(p, len, pos + 16, 8) * k2; v2 = rotr64(v2, 29) + v0;
+            v3 += key_word<KIND>(p, len, pos + 24, 8) * k3; v3 = rotr64(v3, 29) + v1;
             pos += 32;
         } while (pos + 32 <= n);
         v2 ^= rotr64(((v0 + v3) * k0) + v1, 33) * k1;
@@ -65,22 +88,27 @@ VB_HD u64 metro64_1_str(const unsigned char *p, u64 len)
         h += v0 ^ v1;
     }
     if (n - pos >= 16) {
-        u64 a = h + str_word(p, len, pos, 8) * k0;     a = rotr64(a, 33) * k1;
-        u64 b = h + str_word(p, len, pos + 8, 8) * k1; b = rotr64(b, 33) * k2;
+        u64 a = h + key_word<KIND>(p, len, pos, 8) * k0;     a = rotr64(a, 33) * k1;
+        u64 b = h + key_word<KIND>(p, len, pos + 8, 8) * k1; b = rotr64(b, 33) * k2;
         a ^= rotr64(a * k0, 35) + b;
         b ^= rotr64(b * k3, 35) + a;
         h += b;
         pos += 16;
     }
-    if (n - pos >= 8) { h += str_word(p, len, pos, 8) * k3; h ^= rotr64(h, 33) * k1; pos += 8; }
-    if (n - pos >= 4) { h += str_word(p, len, pos, 4) * k3; h ^= rotr64(h, 15) * k1; pos += 4; }
-    if (n - pos >= 2) { h += str_word(p, len, pos, 2) * k3; h ^= rotr64(h, 13) * k1; pos += 2; }
-    if (n - pos >= 1) { h += str_word(p, len, pos, 1) * k3; h ^= rotr64(h, 25) * k1; }
+    if (n - pos >= 8) { h += key_word<KIND>(p, len, pos, 8) * k3; h ^= rotr64(h, 33) * k1; pos += 8; }
+    if (n - pos >= 4) { h += key_word<KIND>(p, len, pos, 4) * k3; h ^= rotr64(h, 15) * k1; pos += 4; }
+    if (n - pos >= 2) { h += key_word<KIND>(p, len, pos, 2) * k3; h ^= rotr64(h, 13) * k1; pos += 2; }
+    if (n - pos >= 1) { h += key_word<KIND>(p, len, pos, 1) * k3; h ^= rotr64(h, 25) * k1; }
     h ^= rotr64(h, 33);
     h *= k0;
     h ^= rotr64(h, 33);
     return h;
 }
+
+// MetroHash64_1(key ‖ 0xFF, seed 0): `str::hash` fed to the reference's MetroHasher.
+VB_HD u64 metro64_1_str(const unsigned char *p, u64 len) { return metro64_1_key<STRKEY_STR>(p, len); }
+// MetroHash64_1(le64(len) ‖ key, seed 0): `<[u8]>::hash` fed to the same hasher.
+VB_HD u64 metro64_1_bytes(const unsigned char *p, u64 len) { return metro64_1_key<STRKEY_BYTES>(p, len); }
 
 constexpr u32 STR_UNPUBLISHED = 0xFFFFFFFFu;   // index slot claimed, entry id not written yet (or slot empty)
 constexpr u32 STR_MAX_PROBE = 64;              // buckets probed before a call gives up and the index grows
@@ -131,8 +159,11 @@ VB_D bool str_equal(const unsigned char *key, const unsigned char *stored, u64 l
 // bytes[offs[i] - base .. offs[i + 1] - base).  Entries and arena are reserved by the host for the worst case of the
 // call, so only the index can overflow; that is decided BEFORE a slot is claimed (load or probe length), so a claimed
 // slot is always published and no thread waits on one forever.  An aborted call is rerun whole after the index grows:
-// rows already encoded find the same entries again.
-__global__ void __launch_bounds__(256) str_encode_kernel(const u64 *__restrict__ offs, const unsigned char *__restrict__ bytes, u64 base,
+// rows already encoded find the same entries again.  KIND: the shuffle's key hash (STRKEY_*).  The byte-slice hash
+// asks ptxas for 4 blocks per SM: left to its default it holds 40 registers and spills the row index (8 bytes); the
+// String instantiation keeps the bare bound (0: none), and with it the code it always had.
+template <int KIND>
+__global__ void __launch_bounds__(256, KIND == STRKEY_BYTES ? 4 : 0) str_encode_kernel(const u64 *__restrict__ offs, const unsigned char *__restrict__ bytes, u64 base,
                                                          u64 n, StrDict d, StrCtl *ctl, u32 max_entries, u32 *__restrict__ ids_out)
 {
     const u64 nb = 1ull << (d.log_cap - 2);
@@ -142,7 +173,7 @@ __global__ void __launch_bounds__(256) str_encode_kernel(const u64 *__restrict__
         if (ld_volatile_u32(&ctl->abort)) return;
         const u64 o0 = offs[i], len = offs[i + 1] - o0;
         const unsigned char *p = bytes + (o0 - base);
-        const u64 h = metro64_1_str(p, len);
+        const u64 h = metro64_1_key<KIND>(p, len);
         const u64 f = str_fp(h, d.fp_mask);
         u64 b = str_bucket(h, d.log_cap);
         u32 found = STR_UNPUBLISHED;
@@ -426,7 +457,8 @@ struct StrNSides {
 };
 
 // One thread per dense key: hash its bytes, then claim a slot.  The keys are distinct, so nothing is compared; the
-// index is sized for load <= 0.6, so every key finds a free slot.
+// index is sized for load <= 0.6, so every key finds a free slot.  KIND: the shuffle's key hash, as str_encode_kernel's.
+template <int KIND>
 __global__ void str_key_index_kernel(const u64 *__restrict__ key_off, const unsigned char *__restrict__ bytes, u32 n, u64 *fp,
                                      u32 *__restrict__ id, u32 log_cap, u64 fp_mask, u64 *__restrict__ hash)
 {
@@ -434,7 +466,7 @@ __global__ void str_key_index_kernel(const u64 *__restrict__ key_off, const unsi
     const u64 stride = (u64)gridDim.x * blockDim.x;
     for (u64 e = (u64)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += stride) {
         const u64 o = key_off[e];
-        const u64 h = metro64_1_str(bytes + o, key_off[e + 1] - o), f = str_fp(h, fp_mask);
+        const u64 h = metro64_1_key<KIND>(bytes + o, key_off[e + 1] - o), f = str_fp(h, fp_mask);
         hash[e] = h;
         u64 b = str_bucket(h, log_cap);
         bool placed = false;

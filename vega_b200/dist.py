@@ -261,13 +261,16 @@ class StrCudaEngine:
     export gives ((n_keys, n_key_bytes, n_vals) per destination, (key_lens, key_bytes, val_counts, vals)), the wire
     columns of include/vega_b200.h (val_counts None for reduce ops); import_ takes the same shape, source-rank major.
     agg VB_AGG_SORT is sort_by_key (vb_shuffle_create_str_sort_dist; vcode None: key-only): reduce then gives
-    (key offsets, key bytes, payload or None), one key per row, and the exchange needs the library's communicator."""
+    (key offsets, key bytes, payload or None), one key per row, and the exchange needs the library's communicator.
+    key_kind VB_STRKEY_BYTES places keys as Rust hashes a Vec<u8> (vb_shuffle_set_str_key); every rank must pass the
+    same kind (a reduce op's exchange inside the library refuses a rank that differs; a GROUP exchange cannot tell)."""
 
-    def __init__(self, sc):
-        self.sc = sc
+    def __init__(self, sc, key_kind=L.VB_STRKEY_STR):
+        self.sc, self.key_kind = sc, key_kind
 
     def create(self, n_map, n_reduce, vcode, agg, rank, world, hint=0):
-        return StrShuffle(self.sc, n_map, n_reduce, vcode, agg, hint=hint, rank=rank, world=world, sort=agg == L.VB_AGG_SORT)
+        return StrShuffle(self.sc, n_map, n_reduce, vcode, agg, hint=hint, rank=rank, world=world, sort=agg == L.VB_AGG_SORT,
+                          key_kind=self.key_kind)
 
     def map(self, sh, map_id, keys, vals):
         """keys: a StrKeys column or a sequence of str; vals: a numpy array or torch CUDA tensor (None for count)."""
@@ -396,13 +399,14 @@ class StrCombineCudaEngine:
     """libvega_b200 on this rank's GPU, for combine_by_key over String keys: CudaEngine's calls over
     vb_shuffle_create_str_multi_dist.  multi is StrShuffle's (value column dtype codes, [(vb_agg, column), ...]).  export
     gives ((n_keys, n_key_bytes) per destination, (key_lens, key_bytes, accs)), accs an (n_acc, keys) view, the wire
-    columns of include/vega_b200.h; import_ takes the same shape, source-rank major."""
+    columns of include/vega_b200.h; import_ takes the same shape, source-rank major.  key_kind: as StrCudaEngine's."""
 
-    def __init__(self, sc):
-        self.sc = sc
+    def __init__(self, sc, key_kind=L.VB_STRKEY_STR):
+        self.sc, self.key_kind = sc, key_kind
 
     def create(self, n_map, n_reduce, multi, rank, world, hint=0):
-        return StrShuffle(self.sc, n_map, n_reduce, L.VB_U64, L.VB_AGG_SUM, hint=hint, rank=rank, world=world, multi=multi)
+        return StrShuffle(self.sc, n_map, n_reduce, L.VB_U64, L.VB_AGG_SUM, hint=hint, rank=rank, world=world, multi=multi,
+                          key_kind=self.key_kind)
 
     def map(self, sh, map_id, keys, cols):
         """keys: a StrKeys column or a sequence of str; cols: the value columns (numpy arrays or torch CUDA tensors of
@@ -492,13 +496,14 @@ class StrBytesCudaEngine:
     StrShuffle.bytes_dist (GROUP, or SORT: sort_by_key with a byte-string payload).  map takes str keys (or a StrKeys
     column) and the values as BytesCudaEngine does.  export gives ((n_keys, n_key_bytes, n_vals, n_val_bytes) per
     destination, (key_lens, key_bytes, val_counts, val_lens, val_bytes)); import_ takes the same shape, source-rank major.
-    reduce gives references (raw: key offsets and bytes); gather them with sh.gather."""
+    reduce gives references (raw: key offsets and bytes); gather them with sh.gather.  key_kind: as StrCudaEngine's."""
 
-    def __init__(self, sc):
-        self.sc = sc
+    def __init__(self, sc, key_kind=L.VB_STRKEY_STR):
+        self.sc, self.key_kind = sc, key_kind
 
     def create(self, n_map, n_reduce, vcode, agg, rank, world, hint=0):
-        return StrShuffle.bytes_dist(self.sc, n_map, n_reduce, rank, world, sort=agg == L.VB_AGG_SORT, hint=hint)
+        return StrShuffle.bytes_dist(self.sc, n_map, n_reduce, rank, world, sort=agg == L.VB_AGG_SORT, hint=hint,
+                                     key_kind=self.key_kind)
 
     def map(self, sh, map_id, keys, vals):
         if not isinstance(keys, (_StrCol, StrKeys)) and len(keys) and not _is_str_keys(keys):

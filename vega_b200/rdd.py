@@ -1425,14 +1425,45 @@ class StrKeys:
                             self.data.cpu().numpy() if _is_torch(self.data) else self.data)
 
 
+class BytesKeys(StrKeys):
+    """A column of byte-slice keys (Rust `Vec<u8>`, `&[u8]`, `Box<[u8]>`, `[u8; N]`), laid out as StrKeys.  Equality and
+    order are the String ones; only the placement differs: `<[u8]>::hash` writes the length before the bytes, so key k
+    goes to partition vb_get_partition_bytes(k) (MetroHash64_1(le64(len) ‖ k) % R).  Context.parallelize over it gives
+    a StrPairRdd / StrRdd whose shuffles place keys so (VB_STRKEY_BYTES); their keys come back as bytes."""
+
+    @staticmethod
+    def from_bytes(items):
+        """Concatenate Python bytes / bytearray keys into (offsets, bytes) on the host."""
+        items = [bytes(b) for b in items]
+        if not all(isinstance(b, bytes) for b in items):
+            raise TypeError("BytesKeys.from_bytes takes bytes keys")
+        offsets = np.zeros(len(items) + 1, dtype=np.uint64)
+        np.cumsum(np.fromiter((len(b) for b in items), dtype=np.uint64, count=len(items)), out=offsets[1:])
+        return BytesKeys(offsets, np.frombuffer(b"".join(items), dtype=np.uint8))
+
+    def to_bytes(self):
+        """The keys as Python bytes."""
+        return _decode_keys(np.asarray(self.offsets.cpu() if _is_torch(self.offsets) else self.offsets, dtype=np.uint64),
+                            self.data.cpu().numpy() if _is_torch(self.data) else self.data, L.VB_STRKEY_BYTES)
+
+
+_BYTES_KEYS_MSG = ("bytes keys: a Rust Vec<u8> hashes with a length prefix, unlike a String; pass str keys, or "
+                   "vb.BytesKeys.from_bytes(keys) for Vec<u8> placement")
+
+
+def _key_kind(x):
+    """VB_STRKEY_BYTES for a BytesKeys column (or a _StrCol / an RDD over one), else VB_STRKEY_STR."""
+    return getattr(x, "key_kind", L.VB_STRKEY_BYTES if isinstance(x, BytesKeys) else L.VB_STRKEY_STR)
+
+
 def _is_str_keys(x):
-    """True for a StrKeys column or a non-empty sequence / numpy array of str; a sequence of bytes is refused: Rust
-    hashes a Vec<u8> with a length prefix, not like a String."""
+    """True for a StrKeys (or BytesKeys) column or a non-empty sequence / numpy array of str; a sequence of bytes is
+    refused: Rust hashes a Vec<u8> with a length prefix, not like a String (BytesKeys places keys that way)."""
     if isinstance(x, StrKeys):
         return True
     if isinstance(x, np.ndarray):
         if x.dtype.kind == "S":
-            raise TypeError("bytes keys: a Rust Vec<u8> hashes with a length prefix, unlike a String; pass str keys")
+            raise TypeError(_BYTES_KEYS_MSG)
         if x.dtype.kind == "U":
             return True
         if x.dtype.kind != "O" or x.size == 0:
@@ -1443,7 +1474,7 @@ def _is_str_keys(x):
     else:
         return False
     if isinstance(first, (bytes, bytearray)):
-        raise TypeError("bytes keys: a Rust Vec<u8> hashes with a length prefix, unlike a String; pass str keys")
+        raise TypeError(_BYTES_KEYS_MSG)
     if not isinstance(first, str):
         return False
     if not all(isinstance(k, str) for k in (x.flat if isinstance(x, np.ndarray) else x)):
@@ -1451,12 +1482,16 @@ def _is_str_keys(x):
     return True
 
 
-def _decode_keys(offsets, data):
-    """Key bytes → numpy object array of Python str (NUL bytes survive, unlike in a numpy 'U' array)."""
+def _decode_keys(offsets, data, kind=L.VB_STRKEY_STR):
+    """Key bytes → numpy object array of Python str (NUL bytes survive, unlike in a numpy 'U' array), or of bytes for
+    kind VB_STRKEY_BYTES (never decoded)."""
     raw = data.tobytes()
     o = offsets.astype(np.int64).tolist()
     out = np.empty(len(o) - 1, dtype=object)
-    out[:] = [raw[o[i]:o[i + 1]].decode("utf-8", "surrogateescape") for i in range(len(o) - 1)]
+    if kind == L.VB_STRKEY_BYTES:
+        out[:] = [raw[o[i]:o[i + 1]] for i in range(len(o) - 1)]
+    else:
+        out[:] = [raw[o[i]:o[i + 1]].decode("utf-8", "surrogateescape") for i in range(len(o) - 1)]
     return out
 
 
@@ -1485,6 +1520,7 @@ class _BytesCol:
         self.as_str = True
         if isinstance(x, StrKeys):
             k = x
+            self.as_str = not isinstance(x, BytesKeys)
         else:
             items = x.tolist() if isinstance(x, np.ndarray) else list(x)
             if all(isinstance(v, str) for v in items):
@@ -1540,6 +1576,7 @@ class _StrCol:
         self.rows = False
         self.key_width = 8
         self.code = None
+        self.key_kind = _key_kind(k)
 
 
 class _DevView:
@@ -1569,10 +1606,14 @@ class StrShuffle(Shuffle):
     of dtype code vcode, or key-only with vcode None; reduce gives each row's key and its payload in key order.  With
     world > 1 (vb_shuffle_create_str_sort_dist) the rows cross ranks through exchange() only, which needs the
     library's communicator (Context.comm_init); rank r then holds the partitions p with p % world == r.
-    seal / exchange / stats / free as for Shuffle."""
+    seal / exchange / stats / free as for Shuffle.  key_kind: VB_STRKEY_STR (Rust String placement) or VB_STRKEY_BYTES
+    (Vec<u8> placement, vb_shuffle_set_str_key); keys come back as str or bytes accordingly."""
 
-    def __init__(self, sc, n_map, n_reduce, vcode, agg, hint=0, rank=0, world=1, multi=None, sort=False):
+    key_kind = L.VB_STRKEY_STR
+
+    def __init__(self, sc, n_map, n_reduce, vcode, agg, hint=0, rank=0, world=1, multi=None, sort=False, key_kind=L.VB_STRKEY_STR):
         self.sc, self._lib = sc, sc._lib
+        self.key_kind = key_kind
         self.n_map, self.n_reduce, self.agg, self.vcode, self.kcode = n_map, n_reduce, agg, vcode, None
         self.rank, self.world = rank, world
         self.has_payload = True
@@ -1606,11 +1647,13 @@ class StrShuffle(Shuffle):
             L.check(self._lib.vb_shuffle_create_str(sc._h, sc.new_shuffle_id(), n_map, n_reduce, vcode, agg, ctypes.byref(h)))
         self._h = h
         sc._shuffles.add(self)
+        if key_kind != L.VB_STRKEY_STR:
+            L.check(self._lib.vb_shuffle_set_str_key(h, key_kind))
         if hint:
             L.check(self._lib.vb_shuffle_set_hint(h, hint))
 
     @classmethod
-    def bytes_dist(cls, sc, n_map, n_reduce, rank, world, sort=False, hint=0):
+    def bytes_dist(cls, sc, n_map, n_reduce, rank, world, sort=False, hint=0, key_kind=L.VB_STRKEY_STR):
         """vb_shuffle_create_str_bytes_dist (GROUP; cogroup and the joins read it), or with sort=True
         vb_shuffle_create_str_sort_bytes_dist (sort_by_key with a byte-string payload), on rank `rank` of `world`.  Map it
         with byte-string values; exchange a GROUP one with export_bytes / import_bytes or exchange(), a sort with
@@ -1626,6 +1669,9 @@ class StrShuffle(Shuffle):
         L.check(create(sc._h, sc.new_shuffle_id(), n_map, n_reduce, rank, world, ctypes.byref(h)))
         self._h = h
         sc._shuffles.add(self)
+        self.key_kind = key_kind
+        if key_kind != L.VB_STRKEY_STR:
+            L.check(self._lib.vb_shuffle_set_str_key(h, key_kind))
         if hint:
             L.check(self._lib.vb_shuffle_set_hint(h, hint))
         return self
@@ -1665,6 +1711,7 @@ class StrShuffle(Shuffle):
         self.n_map, self.n_reduce, self.agg, self.vcode, self.kcode = 0, parent.n_reduce, L.VB_AGG_GROUP, vcode, None
         self.rank, self.world = parent.rank, parent.world
         self.has_payload, self._keepalive = True, []
+        self.key_kind = parent.key_kind                   # the library gives the view its parent's kind too
         h = ctypes.c_void_p()
         L.check(self._lib.vb_shuffle_create_narrow_str(parent._h, out_col, ctypes.byref(h)))
         self._h = h
@@ -1756,7 +1803,7 @@ class StrShuffle(Shuffle):
         """ShuffledRdd::compute(split r): keys as a numpy object array of str, then the combined values, or the CSR
         offsets and values for GROUP."""
         out = self.reduce_raw(r)
-        return (_decode_keys(out[0], out[1]),) + out[2:]
+        return (_decode_keys(out[0], out[1], self.key_kind),) + out[2:]
 
     def reduce_device(self, r, out_key_offsets=None, out_key_bytes=None, out_comb=None, out_offs=None, out_vals=None):
         """Partition r into caller-provided torch CUDA tensors (any may be None; sizes from reduce_size)."""
@@ -1864,7 +1911,8 @@ class StrShuffledRdd(ShuffledRdd):
         p = self.parent
         starts = slice_starts(p.n, p.num_slices)
         vcode = p.vals.code if p.vals is not None else L.VB_U64
-        sh = StrShuffle(self.sc, len(starts) - 1, self.num_slices, vcode, _AGG[self.agg_name], hint=self.hint)
+        sh = StrShuffle(self.sc, len(starts) - 1, self.num_slices, vcode, _AGG[self.agg_name], hint=self.hint,
+                        key_kind=_key_kind(p.keys))
         for m in range(len(starts) - 1):
             sh.map(m, p.keys, p.vals, int(starts[m]), int(starts[m + 1]))
         sh.seal()
@@ -1945,7 +1993,7 @@ class StrCombinedRdd(_Base):
         p = self.parent
         starts = slice_starts(p.n, p.num_slices)
         sh = StrShuffle(self.sc, len(starts) - 1, self.num_slices, L.VB_U64, L.VB_AGG_SUM, hint=self.hint,
-                        multi=([c.code for c in p.cols], self.spec))
+                        multi=([c.code for c in p.cols], self.spec), key_kind=_key_kind(p.keys))
         for m in range(len(starts) - 1):
             sh.map_cols(m, p.keys, p.cols, int(starts[m]), int(starts[m + 1]))
         sh.seal()
@@ -1963,7 +2011,7 @@ class StrCombinedRdd(_Base):
 
     def compute(self, split):
         ko, kb, outs = self.compute_raw(split)
-        return _decode_keys(ko, kb), dict(zip(self.names, outs))
+        return _decode_keys(ko, kb, self._run().key_kind), dict(zip(self.names, outs))
 
     def compute_device(self, split, out_key_offsets=None, out_key_bytes=None, out_aggs=None):
         """compute(split) into caller-provided torch CUDA tensors (any may be None; sizes from the shuffle's
@@ -1993,6 +2041,13 @@ class StrAggregateRdd(_Base):
     _result_col = AggregateRdd._result_col
 
 
+def _parent_key_kind(r):
+    """The key kind of a StrCoGroupedRdd parent: of its keys, or of the keys of the shuffle that made it."""
+    if isinstance(r, StrAggregateRdd):
+        r = r.combined
+    return _key_kind(r.parent.keys if isinstance(r, (StrShuffledRdd, StrCombinedRdd)) else r.keys)
+
+
 class StrCoGroupedRdd(_Base):
     """CoGroupedRdd::new(rdds, HashPartitioner::new(num_splits)) over `String` keys (vb_cogroup_n_str / vb_join_n_str):
     the cogroup and the joins of 1 to 16 parents, with keys matched by their bytes.  A parent is a StrPairRdd, shuffled
@@ -2007,6 +2062,8 @@ class StrCoGroupedRdd(_Base):
       outer_join_compute(r, required) / outer_join_collect(required): optional parents as numpy.ma.MaskedArray
     join_raw(r, required) returns the device's keyed form without decoding: (key offsets, key bytes, row offsets,
     [values], [validity or None]), each key once with its rows [row_offsets[i], row_offsets[i + 1])."""
+
+    key_kind = L.VB_STRKEY_STR           # the parents' key kind (all alike: __init__ refuses a mix)
 
     def __init__(self, rdds, num_splits):
         rdds = list(rdds)
@@ -2025,6 +2082,10 @@ class StrCoGroupedRdd(_Base):
                 raise TypeError(f"parent {j} is not a String-key PairRdd, reduce result or combine_by_key aggregate")
         if any(r.sc is not rdds[0].sc for r in rdds):
             raise TypeError("the parents live on different contexts")
+        kinds = [_parent_key_kind(r) for r in rdds]
+        if any(k != kinds[0] for k in kinds):      # equal bytes sit in different partitions under the two hashes
+            raise TypeError("the parents mix String keys and BytesKeys (Vec<u8>) keys: they are placed by different hashes")
+        self.key_kind = kinds[0]
         self.rdds, self.num_slices, self.sc = rdds, num_splits, rdds[0].sc
         self._shs = None
 
@@ -2045,7 +2106,7 @@ class StrCoGroupedRdd(_Base):
         partition read on the device."""
         import torch
         dev = f"cuda:{sh._lib.vb_ctx_device(self.sc._h)}"
-        out = StrShuffle(self.sc, sh.n_reduce, self.num_slices, vcode, L.VB_AGG_GROUP)
+        out = StrShuffle(self.sc, sh.n_reduce, self.num_slices, vcode, L.VB_AGG_GROUP, key_kind=self.key_kind)
         for p in range(sh.n_reduce):
             nk, nb, _ = sh.reduce_size(p)
             ko = torch.empty(nk + 1, dtype=torch.int64, device=dev)
@@ -2055,7 +2116,7 @@ class StrCoGroupedRdd(_Base):
                 sh.reduce_device(p, out_key_offsets=ko, out_key_bytes=kb, out_comb=v)
             else:
                 sh.reduce_cols(p, None, L.VB_DEVICE, ko, kb, [v if c == col else None for c in range(n_cols)])
-            out.map(p, _StrCol(StrKeys(ko, kb)), _Col(v, role="value"), 0, nk)
+            out.map(p, _StrCol((BytesKeys if self.key_kind == L.VB_STRKEY_BYTES else StrKeys)(ko, kb)), _Col(v, role="value"), 0, nk)
         out.seal()
         return out
 
@@ -2080,7 +2141,7 @@ class StrCoGroupedRdd(_Base):
 
     def compute(self, split):
         ko, kb, lists = self.compute_raw(split)
-        return _decode_keys(ko, kb), lists
+        return _decode_keys(ko, kb, self.key_kind), lists
 
     def collect(self):
         out = []
@@ -2112,7 +2173,7 @@ class StrCoGroupedRdd(_Base):
         """Partition `split` of the outer join of all parents: (k, [v_0, ..., v_{n-1}]) with one key per row; see
         CoGroupedRdd.outer_join_compute."""
         ko, kb, ro, vs, valid = self.join_raw(split, required)
-        keys = _decode_keys(ko, kb)
+        keys = _decode_keys(ko, kb, self.key_kind)
         k = np.repeat(keys, np.diff(ro.astype(np.int64))) if len(keys) else np.empty(0, dtype=object)
         return k, [v if ok is None or v.dtype == object else np.ma.MaskedArray(v, mask=ok == 0) for v, ok in zip(vs, valid)]
 
@@ -2161,7 +2222,7 @@ class StrSortedRdd(_Base):
         p = self.parent
         starts = slice_starts(p.n, p.num_slices)
         sh = StrShuffle(self.sc, len(starts) - 1, self.num_slices, self.vals.code if self.vals is not None else None, L.VB_AGG_SORT,
-                        sort=True)
+                        sort=True, key_kind=_key_kind(p.keys))
         for m in range(len(starts) - 1):
             sh.map(m, p.keys, self.vals, int(starts[m]), int(starts[m + 1]))
         sh.seal()
@@ -2173,7 +2234,7 @@ class StrSortedRdd(_Base):
 
     def compute(self, split):
         ko, kb, vals = self.compute_raw(split)
-        keys = _decode_keys(ko, kb)
+        keys = _decode_keys(ko, kb, _key_kind(self.parent.keys))
         return keys if self.vals is None else (keys, vals)
 
     def compute_device(self, split, out_key_offsets=None, out_key_bytes=None, out_vals=None):
@@ -2181,7 +2242,7 @@ class StrSortedRdd(_Base):
 
     def collect(self):
         parts = [self.compute_raw(r) for r in range(self.num_slices)]
-        keys = np.concatenate([_decode_keys(ko, kb) for ko, kb, _ in parts])
+        keys = np.concatenate([_decode_keys(ko, kb, _key_kind(self.parent.keys)) for ko, kb, _ in parts])
         if self.vals is None:
             return keys
         return keys, np.concatenate([v for _, _, v in parts])
