@@ -158,6 +158,21 @@ VB_API int32_t vb_shuffle_set_hint(vb_shuf *s, uint64_t expected_distinct);
 /* One-process-per-GPU mode: this process is `rank` of `world`; reduce partition r is owned by
  * rank r % world.  Must precede the first map call.  world == 1 is the default.              */
 VB_API int32_t vb_shuffle_set_dist(vb_shuf *s, uint32_t rank, uint32_t world);
+/* Order of the values inside each key's list of a GROUP or COGROUP shuffle.  VB_VALORDER_INPUT, the default: map-id
+ * order (source-rank major across ranks).  VB_VALORDER_ASC: ascending in the value dtype's order, sorted on the device
+ * right after the reduce side's CSR is built — u64 unsigned, i64 signed, f64 as f64::total_cmp (-NaN < -inf < ... <
+ * -0.0 < +0.0 < ... < +inf < +NaN, NaNs by payload), so two values tie only when their bits are equal.  Keys, bucket
+ * and value offsets are those of the same shuffle in input order; only the order inside each list changes, and with
+ * it everything that reads the lists: vb_shuffle_reduce(_str), the blobs, vb_cogroup(_n)(_str) and every join's
+ * nested-loop order (the internal sides of a join inherit the setting of the shuffle they are cut from).
+ * Accepted by integer VB_AGG_GROUP / VB_AGG_COGROUP shuffles (vb_shuffle_create, the _dist creates) with u64, i64 or
+ * f64 values and by GROUP shuffles of vb_shuffle_create_str(_dist) of either key kind, before the first map, blob or
+ * import call (VB_ERR_STATE after one, or after seal).  VB_ERR_UNSUPPORTED for VB_BYTES values; VB_ERR_INVALID for an
+ * unknown order and for any other shuffle (reduce ops, combine_by_key, sort, repartition, narrow views), checked
+ * before the state.  Across ranks the setting applies where a partition is sealed, on the rank that owns it; the
+ * export side does not sort.  Every rank of a shuffle is expected to set the same order: it is not checked.        */
+enum vb_value_order { VB_VALORDER_INPUT = 0, VB_VALORDER_ASC = 1 };
+VB_API int32_t vb_shuffle_set_value_order(vb_shuf *s, int32_t order /*vb_value_order*/);
 
 /* do_shuffle_task for one map partition.  AoS = the reference's native Vec<(K,V)> layout
  * (16-byte rows); SoA = separate key/value arrays (vals may be NULL for VB_AGG_COUNT and

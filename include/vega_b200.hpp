@@ -109,10 +109,11 @@ private:
 };
 
 namespace detail {
-// Run one shuffle: slice like ParallelCollection::slice, one map task per slice, seal.
+// Run one shuffle: slice like ParallelCollection::slice, one map task per slice, seal.  sorted_values: each key's list of
+// a GROUP / COGROUP shuffle ascending in the value dtype's order (vb_shuffle_set_value_order).
 template <typename K>
 inline ShufPtr run_shuffle(Context &sc, const std::vector<uint64_t> &keys, const std::vector<uint64_t> *vals, size_t num_slices,
-                           size_t num_splits, int vcode, int agg)
+                           size_t num_splits, int vcode, int agg, bool sorted_values = false)
 {
     if (num_slices < 1) throw Error(VB_ERR_INVALID, "Number of slices should be greater than or equal to 1");
     const uint64_t n = keys.size();
@@ -123,6 +124,7 @@ inline ShufPtr run_shuffle(Context &sc, const std::vector<uint64_t> &keys, const
                             VB_PART_HASH_METRO64, &raw));
     ShufPtr s(raw);
     if (dtype<K>::width == 4) check(vb_shuffle_set_key_width(raw, 4));
+    if (sorted_values) check(vb_shuffle_set_value_order(raw, VB_VALORDER_ASC));
     for (uint64_t m = 0; m < n_map; ++m) {
         const uint64_t lo = starts[m], cnt = starts[m + 1] - lo;
         check(vb_shuffle_map_soa(raw, (uint32_t)m, cnt ? keys.data() + lo : nullptr, (vals && cnt) ? vals->data() + lo : nullptr, cnt, VB_HOST));
@@ -197,10 +199,11 @@ public:
     }
     size_t number_of_splits() const { return num_slices_; }
 
-    // group_by_key(num_splits).collect()  →  Vec<(K, Vec<V>)>, values in input order
-    std::vector<std::pair<K, std::vector<V>>> group_by_key(size_t num_splits) const
+    // group_by_key(num_splits).collect()  →  Vec<(K, Vec<V>)>, values in input order, or ascending with sorted_values
+    // (u64 unsigned, i64 signed, f64 as f64::total_cmp), sorted on the device
+    std::vector<std::pair<K, std::vector<V>>> group_by_key(size_t num_splits, bool sorted_values = false) const
     {
-        auto s = detail::run_shuffle<K>(*sc_, keys_, &vals_, num_slices_, num_splits, detail::dtype<V>::code, VB_AGG_GROUP);
+        auto s = detail::run_shuffle<K>(*sc_, keys_, &vals_, num_slices_, num_splits, detail::dtype<V>::code, VB_AGG_GROUP, sorted_values);
         std::vector<std::pair<K, std::vector<V>>> out;
         for (uint32_t r = 0; r < num_splits; ++r) {
             uint64_t nk = 0, nv = 0;
@@ -280,12 +283,14 @@ public:
         return out;
     }
 
-    // self.join(other, num_splits).collect()  →  Vec<(K, (V, W))>, inner join
+    // self.join(other, num_splits).collect()  →  Vec<(K, (V, W))>, inner join.  sorted_values (here and in the cogroups
+    // and joins below): every side's lists ascending, so a key's rows come in ascending (v, w) order.
     template <typename W>
-    std::vector<std::pair<K, std::pair<V, W>>> join(const PairRddT<K, W> &other, size_t num_splits) const
+    std::vector<std::pair<K, std::pair<V, W>>> join(const PairRddT<K, W> &other, size_t num_splits, bool sorted_values = false) const
     {
-        auto a = detail::run_shuffle<K>(*sc_, keys_, &vals_, num_slices_, num_splits, detail::dtype<V>::code, VB_AGG_COGROUP);
-        auto b = detail::run_shuffle<K>(*sc_, other.keys_, &other.vals_, other.num_slices_, num_splits, detail::dtype<W>::code, VB_AGG_COGROUP);
+        auto a = detail::run_shuffle<K>(*sc_, keys_, &vals_, num_slices_, num_splits, detail::dtype<V>::code, VB_AGG_COGROUP, sorted_values);
+        auto b = detail::run_shuffle<K>(*sc_, other.keys_, &other.vals_, other.num_slices_, num_splits, detail::dtype<W>::code, VB_AGG_COGROUP,
+                                        sorted_values);
         std::vector<std::pair<K, std::pair<V, W>>> out;
         for (uint32_t r = 0; r < num_splits; ++r) {
             uint64_t n = 0;
@@ -301,10 +306,12 @@ public:
     // self.cogroup(other, num_splits).collect()  →  Vec<(K, (Vec<V>, Vec<W>))> (src/rdd/pair_rdd.rs:123-155): every key
     // of either side once, with both value lists in cogroup order; a side that lacks the key has an empty list.
     template <typename W>
-    std::vector<std::pair<K, std::pair<std::vector<V>, std::vector<W>>>> cogroup(const PairRddT<K, W> &other, size_t num_splits) const
+    std::vector<std::pair<K, std::pair<std::vector<V>, std::vector<W>>>> cogroup(const PairRddT<K, W> &other, size_t num_splits,
+                                                                                 bool sorted_values = false) const
     {
-        auto a = detail::run_shuffle<K>(*sc_, keys_, &vals_, num_slices_, num_splits, detail::dtype<V>::code, VB_AGG_COGROUP);
-        auto b = detail::run_shuffle<K>(*sc_, other.keys_, &other.vals_, other.num_slices_, num_splits, detail::dtype<W>::code, VB_AGG_COGROUP);
+        auto a = detail::run_shuffle<K>(*sc_, keys_, &vals_, num_slices_, num_splits, detail::dtype<V>::code, VB_AGG_COGROUP, sorted_values);
+        auto b = detail::run_shuffle<K>(*sc_, other.keys_, &other.vals_, other.num_slices_, num_splits, detail::dtype<W>::code, VB_AGG_COGROUP,
+                                        sorted_values);
         std::vector<std::pair<K, std::pair<std::vector<V>, std::vector<W>>>> out;
         for (uint32_t r = 0; r < num_splits; ++r) {
             uint64_t nk = 0, nv = 0, nw = 0;
@@ -325,33 +332,37 @@ public:
     // Outer joins (Spark's leftOuterJoin / rightOuterJoin / fullOuterJoin; vega has none): a key missing on the other
     // side still gives rows, with std::nullopt on that side.  A key's rows are contiguous.
     template <typename W>
-    std::vector<std::pair<K, std::pair<V, std::optional<W>>>> left_outer_join(const PairRddT<K, W> &other, size_t num_splits) const
+    std::vector<std::pair<K, std::pair<V, std::optional<W>>>> left_outer_join(const PairRddT<K, W> &other, size_t num_splits,
+                                                       bool sorted_values = false) const
     {
         std::vector<std::pair<K, std::pair<V, std::optional<W>>>> out;
-        outer_join_rows(other, num_splits, VB_JOIN_LEFT, [&](K k, std::optional<V> v, std::optional<W> w) { out.emplace_back(k, std::make_pair(*v, w)); });
+        outer_join_rows(other, num_splits, VB_JOIN_LEFT, sorted_values, [&](K k, std::optional<V> v, std::optional<W> w) { out.emplace_back(k, std::make_pair(*v, w)); });
         return out;
     }
     template <typename W>
-    std::vector<std::pair<K, std::pair<std::optional<V>, W>>> right_outer_join(const PairRddT<K, W> &other, size_t num_splits) const
+    std::vector<std::pair<K, std::pair<std::optional<V>, W>>> right_outer_join(const PairRddT<K, W> &other, size_t num_splits,
+                                                       bool sorted_values = false) const
     {
         std::vector<std::pair<K, std::pair<std::optional<V>, W>>> out;
-        outer_join_rows(other, num_splits, VB_JOIN_RIGHT, [&](K k, std::optional<V> v, std::optional<W> w) { out.emplace_back(k, std::make_pair(v, *w)); });
+        outer_join_rows(other, num_splits, VB_JOIN_RIGHT, sorted_values, [&](K k, std::optional<V> v, std::optional<W> w) { out.emplace_back(k, std::make_pair(v, *w)); });
         return out;
     }
     template <typename W>
-    std::vector<std::pair<K, std::pair<std::optional<V>, std::optional<W>>>> full_outer_join(const PairRddT<K, W> &other, size_t num_splits) const
+    std::vector<std::pair<K, std::pair<std::optional<V>, std::optional<W>>>> full_outer_join(const PairRddT<K, W> &other, size_t num_splits,
+                                                       bool sorted_values = false) const
     {
         std::vector<std::pair<K, std::pair<std::optional<V>, std::optional<W>>>> out;
-        outer_join_rows(other, num_splits, VB_JOIN_FULL, [&](K k, std::optional<V> v, std::optional<W> w) { out.emplace_back(k, std::make_pair(v, w)); });
+        outer_join_rows(other, num_splits, VB_JOIN_FULL, sorted_values, [&](K k, std::optional<V> v, std::optional<W> w) { out.emplace_back(k, std::make_pair(v, w)); });
         return out;
     }
 
     // CoGroupedRdd::new([self, others...], HashPartitioner::new(num_splits)).collect()  →  Vec<(K, Vec<Vec<V>>)>
     // (src/rdd/co_grouped_rdd.rs:75-135, 206-249): every key of any parent once, with one value list per parent in
     // parent order (this one first); a parent that lacks the key has an empty list.
-    std::vector<std::pair<K, std::vector<std::vector<V>>>> cogroup_n(const std::vector<PairRddT> &others, size_t num_splits) const
+    std::vector<std::pair<K, std::vector<std::vector<V>>>> cogroup_n(const std::vector<PairRddT> &others, size_t num_splits,
+                                                                     bool sorted_values = false) const
     {
-        auto shs = cogroup_shuffles(others, num_splits);
+        auto shs = cogroup_shuffles(others, num_splits, sorted_values);
         std::vector<vb_shuf *> sides;
         for (auto &s : shs) sides.push_back(s.get());
         return detail::read_cogroup_n<K, V>(sides, num_splits);
@@ -359,9 +370,9 @@ public:
 
     // inner join of [self, others...]  →  (k, [v_0, ..., v_{n-1}]) per row: for a key on every parent,
     // for v0 in vs_0 { for v1 in vs_1 { ... } }
-    std::vector<std::pair<K, std::vector<V>>> join_n(const std::vector<PairRddT> &others, size_t num_splits) const
+    std::vector<std::pair<K, std::vector<V>>> join_n(const std::vector<PairRddT> &others, size_t num_splits, bool sorted_values = false) const
     {
-        auto shs = cogroup_shuffles(others, num_splits);
+        auto shs = cogroup_shuffles(others, num_splits, sorted_values);
         std::vector<vb_shuf *> sides;
         for (auto &s : shs) sides.push_back(s.get());
         const uint32_t n = (uint32_t)sides.size();
@@ -387,9 +398,9 @@ public:
     // key on every required parent gives, for v0 in L0 { for v1 in L1 { ... } }, (k, [v_0, ..., v_{n-1}]) where L_j is
     // parent j's list, or [std::nullopt] for an optional parent that lacks the key.  A key's rows are contiguous.
     std::vector<std::pair<K, std::vector<std::optional<V>>>> join_n_outer(const std::vector<PairRddT> &others, size_t num_splits,
-                                                                          uint32_t required) const
+                                                                          uint32_t required, bool sorted_values = false) const
     {
-        auto shs = cogroup_shuffles(others, num_splits);
+        auto shs = cogroup_shuffles(others, num_splits, sorted_values);
         std::vector<vb_shuf *> sides;
         for (auto &s : shs) sides.push_back(s.get());
         return detail::read_join_n_outer<K, V>(sides, num_splits, required);
@@ -401,21 +412,23 @@ public:
 
 private:
     // one COGROUP shuffle per parent: this one, then others in order
-    std::vector<detail::ShufPtr> cogroup_shuffles(const std::vector<PairRddT> &others, size_t num_splits) const
+    std::vector<detail::ShufPtr> cogroup_shuffles(const std::vector<PairRddT> &others, size_t num_splits, bool sorted_values) const
     {
         std::vector<detail::ShufPtr> shs;
-        shs.push_back(detail::run_shuffle<K>(*sc_, keys_, &vals_, num_slices_, num_splits, detail::dtype<V>::code, VB_AGG_COGROUP));
+        shs.push_back(detail::run_shuffle<K>(*sc_, keys_, &vals_, num_slices_, num_splits, detail::dtype<V>::code, VB_AGG_COGROUP, sorted_values));
         for (auto &o : others)
-            shs.push_back(detail::run_shuffle<K>(*sc_, o.keys_, &o.vals_, o.num_slices_, num_splits, detail::dtype<V>::code, VB_AGG_COGROUP));
+            shs.push_back(detail::run_shuffle<K>(*sc_, o.keys_, &o.vals_, o.num_slices_, num_splits, detail::dtype<V>::code, VB_AGG_COGROUP,
+                                                 sorted_values));
         return shs;
     }
 
     // every row of vb_join_outer, partition by partition, as emit(k, v or nullopt, w or nullopt)
     template <typename W, typename Emit>
-    void outer_join_rows(const PairRddT<K, W> &other, size_t num_splits, int32_t kind, Emit emit) const
+    void outer_join_rows(const PairRddT<K, W> &other, size_t num_splits, int32_t kind, bool sorted_values, Emit emit) const
     {
-        auto a = detail::run_shuffle<K>(*sc_, keys_, &vals_, num_slices_, num_splits, detail::dtype<V>::code, VB_AGG_COGROUP);
-        auto b = detail::run_shuffle<K>(*sc_, other.keys_, &other.vals_, other.num_slices_, num_splits, detail::dtype<W>::code, VB_AGG_COGROUP);
+        auto a = detail::run_shuffle<K>(*sc_, keys_, &vals_, num_slices_, num_splits, detail::dtype<V>::code, VB_AGG_COGROUP, sorted_values);
+        auto b = detail::run_shuffle<K>(*sc_, other.keys_, &other.vals_, other.num_slices_, num_splits, detail::dtype<W>::code, VB_AGG_COGROUP,
+                                        sorted_values);
         for (uint32_t r = 0; r < num_splits; ++r) {
             uint64_t n = 0;
             check(vb_join_outer_size(a.get(), b.get(), r, kind, &n));
@@ -597,7 +610,7 @@ struct StrCol {
 };
 
 inline ShufPtr run_str_shuffle(Context &sc, const StrCol &keys, const std::vector<uint64_t> *vals, size_t num_slices, size_t num_splits,
-                               int vcode, int agg)
+                               int vcode, int agg, bool sorted_values = false)
 {
     if (num_slices < 1) throw Error(VB_ERR_INVALID, "Number of slices should be greater than or equal to 1");
     const uint64_t n = keys.size();
@@ -607,6 +620,7 @@ inline ShufPtr run_str_shuffle(Context &sc, const StrCol &keys, const std::vecto
     check(vb_shuffle_create_str(sc.raw(), sc.new_shuffle_id(), (uint32_t)n_map, (uint32_t)num_splits, vcode, agg, &raw));
     ShufPtr s(raw);
     if (keys.kind != VB_STRKEY_STR) check(vb_shuffle_set_str_key(raw, keys.kind));
+    if (sorted_values) check(vb_shuffle_set_value_order(raw, VB_VALORDER_ASC));
     for (uint64_t m = 0; m < n_map; ++m) {
         const uint64_t lo = starts[m], cnt = starts[m + 1] - lo;
         check(vb_shuffle_map_str(raw, (uint32_t)m, keys.offs.data() + lo, keys.bytes.data(), keys.bytes.size(),
@@ -712,10 +726,10 @@ public:
     }
     size_t number_of_splits() const { return num_slices_; }
 
-    // group_by_key(num_splits).collect()  →  Vec<(String, Vec<V>)>, values in input order
-    std::vector<std::pair<std::string, std::vector<V>>> group_by_key(size_t num_splits) const
+    // group_by_key(num_splits).collect()  →  Vec<(String, Vec<V>)>, values in input order, or ascending with sorted_values
+    std::vector<std::pair<std::string, std::vector<V>>> group_by_key(size_t num_splits, bool sorted_values = false) const
     {
-        auto s = detail::run_str_shuffle(*sc_, keys_, &vals_, num_slices_, num_splits, detail::dtype<V>::code, VB_AGG_GROUP);
+        auto s = detail::run_str_shuffle(*sc_, keys_, &vals_, num_slices_, num_splits, detail::dtype<V>::code, VB_AGG_GROUP, sorted_values);
         std::vector<std::pair<std::string, std::vector<V>>> out;
         for (uint32_t r = 0; r < num_splits; ++r) {
             std::vector<uint64_t> o, v;
@@ -809,9 +823,9 @@ public:
     // CoGroupedRdd::new([self, others...], HashPartitioner::new(num_splits)).collect() over String keys
     // (vb_cogroup_n_str): every key of any parent once, with one value list per parent (this one first)
     std::vector<std::pair<std::string, std::vector<std::vector<V>>>> cogroup_n(const std::vector<StrPairRddT> &others,
-                                                                               size_t num_splits) const
+                                                                               size_t num_splits, bool sorted_values = false) const
     {
-        auto shs = group_shuffles(others, num_splits);
+        auto shs = group_shuffles(others, num_splits, sorted_values);
         return detail::read_str_cogroup_n<V>(raw(shs), num_splits);
     }
 
@@ -819,17 +833,19 @@ public:
     // an optional parent that lacks the key gives std::nullopt.  (k, [v_0, ..., v_{n-1}]) per row, a key's rows
     // contiguous, for v0 in L0 { for v1 in L1 { ... } }
     std::vector<std::pair<std::string, std::vector<std::optional<V>>>> join_n_outer(const std::vector<StrPairRddT> &others,
-                                                                                    size_t num_splits, uint32_t required) const
+                                                                                    size_t num_splits, uint32_t required,
+                                                                                    bool sorted_values = false) const
     {
-        auto shs = group_shuffles(others, num_splits);
+        auto shs = group_shuffles(others, num_splits, sorted_values);
         return detail::read_str_join_n_outer<V>(raw(shs), num_splits, required);
     }
 
     // inner join of [self, others...]  →  (k, [v_0, ..., v_{n-1}]) per row
-    std::vector<std::pair<std::string, std::vector<V>>> join_n(const std::vector<StrPairRddT> &others, size_t num_splits) const
+    std::vector<std::pair<std::string, std::vector<V>>> join_n(const std::vector<StrPairRddT> &others, size_t num_splits,
+                                                               bool sorted_values = false) const
     {
         std::vector<std::pair<std::string, std::vector<V>>> out;
-        for (auto &kv : join_n_outer(others, num_splits, (uint32_t)((1ull << (others.size() + 1)) - 1))) {
+        for (auto &kv : join_n_outer(others, num_splits, (uint32_t)((1ull << (others.size() + 1)) - 1), sorted_values)) {
             std::vector<V> row;
             for (auto &v : kv.second) row.push_back(*v);
             out.emplace_back(std::move(kv.first), std::move(row));
@@ -838,30 +854,32 @@ public:
     }
 
     // PairRdd::join (src/rdd/pair_rdd.rs:104-121)  →  Vec<(String, (V, V))>
-    std::vector<std::pair<std::string, std::pair<V, V>>> join(const StrPairRddT &other, size_t num_splits) const
+    std::vector<std::pair<std::string, std::pair<V, V>>> join(const StrPairRddT &other, size_t num_splits, bool sorted_values = false) const
     {
         std::vector<std::pair<std::string, std::pair<V, V>>> out;
-        for (auto &kv : join_n({other}, num_splits)) out.emplace_back(std::move(kv.first), std::make_pair(kv.second[0], kv.second[1]));
+        for (auto &kv : join_n({other}, num_splits, sorted_values)) out.emplace_back(std::move(kv.first), std::make_pair(kv.second[0], kv.second[1]));
         return out;
     }
 
     // PairRdd::cogroup (src/rdd/pair_rdd.rs:123-155)  →  Vec<(String, (Vec<V>, Vec<V>))>
-    std::vector<std::pair<std::string, std::pair<std::vector<V>, std::vector<V>>>> cogroup(const StrPairRddT &other, size_t num_splits) const
+    std::vector<std::pair<std::string, std::pair<std::vector<V>, std::vector<V>>>> cogroup(const StrPairRddT &other, size_t num_splits,
+                                                                                           bool sorted_values = false) const
     {
         std::vector<std::pair<std::string, std::pair<std::vector<V>, std::vector<V>>>> out;
-        for (auto &kv : cogroup_n({other}, num_splits))
+        for (auto &kv : cogroup_n({other}, num_splits, sorted_values))
             out.emplace_back(std::move(kv.first), std::make_pair(std::move(kv.second[0]), std::move(kv.second[1])));
         return out;
     }
 
 private:
     // this parent and the others, each shuffled into a string GROUP shuffle over num_splits
-    std::vector<detail::ShufPtr> group_shuffles(const std::vector<StrPairRddT> &others, size_t num_splits) const
+    std::vector<detail::ShufPtr> group_shuffles(const std::vector<StrPairRddT> &others, size_t num_splits, bool sorted_values) const
     {
         std::vector<detail::ShufPtr> shs;
-        shs.push_back(detail::run_str_shuffle(*sc_, keys_, &vals_, num_slices_, num_splits, detail::dtype<V>::code, VB_AGG_GROUP));
+        shs.push_back(detail::run_str_shuffle(*sc_, keys_, &vals_, num_slices_, num_splits, detail::dtype<V>::code, VB_AGG_GROUP, sorted_values));
         for (auto &o : others)
-            shs.push_back(detail::run_str_shuffle(*o.sc_, o.keys_, &o.vals_, o.num_slices_, num_splits, detail::dtype<V>::code, VB_AGG_GROUP));
+            shs.push_back(detail::run_str_shuffle(*o.sc_, o.keys_, &o.vals_, o.num_slices_, num_splits, detail::dtype<V>::code, VB_AGG_GROUP,
+                                                  sorted_values));
         return shs;
     }
     static std::vector<vb_shuf *> raw(const std::vector<detail::ShufPtr> &shs)

@@ -14,6 +14,7 @@ use std::os::raw::{c_char, c_void};
 pub const VB_OK: i32 = 0;
 pub const VB_U64: i32 = 0; pub const VB_I64: i32 = 1; pub const VB_F64: i32 = 2; pub const VB_BYTES: i32 = 3;
 pub const VB_STRKEY_STR: i32 = 0; pub const VB_STRKEY_BYTES: i32 = 1;   // vb_shuffle_set_str_key
+pub const VB_VALORDER_INPUT: i32 = 0; pub const VB_VALORDER_ASC: i32 = 1;   // vb_shuffle_set_value_order
 pub const VB_AGG_GROUP: i32 = 0; pub const VB_AGG_SUM: i32 = 1; pub const VB_AGG_MIN: i32 = 2;
 pub const VB_AGG_MAX: i32 = 3; pub const VB_AGG_COUNT: i32 = 4; pub const VB_AGG_COGROUP: i32 = 5;
 pub const VB_AGG_MEAN: i32 = 7;   // vb_agg_col only
@@ -208,6 +209,8 @@ extern "C" {
     pub fn vb_hash_bytes(bytes: *const c_void, len: u64) -> u64;
     pub fn vb_get_partition_bytes(bytes: *const c_void, len: u64, n_reduce: u32) -> u32;
     pub fn vb_shuffle_set_str_key(s: *mut vb_shuf, kind: i32) -> i32;
+    // each key's list of a GROUP / COGROUP shuffle in map order, or ascending (sorted on the device); before the first map call
+    pub fn vb_shuffle_set_value_order(s: *mut vb_shuf, order: i32) -> i32;
     pub fn vb_shuffle_free(s: *mut vb_shuf) -> i32;
     pub fn vb_last_error() -> *const c_char;
     pub fn vb_get_partition(key: u64, key_width: u32, n_reduce: u32) -> u32;

@@ -13,6 +13,7 @@ LIB_PATH = os.environ.get("VEGA_B200_LIB") or os.path.join(_PKG, "libvega_b200.s
 VB_OK, VB_ERR_INVALID, VB_ERR_CUDA, VB_ERR_OOM, VB_ERR_STATE, VB_ERR_UNSUPPORTED, VB_ERR_TOO_LARGE = 0, -1, -2, -3, -4, -5, -6
 VB_U64, VB_I64, VB_F64, VB_BYTES = 0, 1, 2, 3
 VB_STRKEY_STR, VB_STRKEY_BYTES = 0, 1        # vb_shuffle_set_str_key: keys hash as a Rust String, or as a Vec<u8>
+VB_VALORDER_INPUT, VB_VALORDER_ASC = 0, 1    # vb_shuffle_set_value_order: each key's values in map order, or ascending
 VB_AGG_GROUP, VB_AGG_SUM, VB_AGG_MIN, VB_AGG_MAX, VB_AGG_COUNT, VB_AGG_COGROUP, VB_AGG_SORT, VB_AGG_MEAN = range(8)
 VB_MAX_VAL_COLS, VB_MAX_AGGS = 4, 8
 VB_PART_HASH_METRO64, VB_PART_RANGE = 0, 1
@@ -67,6 +68,7 @@ SYMBOLS = {
     "vb_shuffle_set_key_width": (_i32, [_vp, _u32]),
     "vb_shuffle_set_hint": (_i32, [_vp, _u64]),
     "vb_shuffle_set_dist": (_i32, [_vp, _u32, _u32]),
+    "vb_shuffle_set_value_order": (_i32, [_vp, _i32]),
     "vb_shuffle_map_aos": (_i32, [_vp, _u32, _vp, _u64, _i32]),
     "vb_shuffle_map_soa": (_i32, [_vp, _u32, _vp, _vp, _u64, _i32]),
     "vb_shuffle_export_prepare": (_i32, [_vp, _pu64]),

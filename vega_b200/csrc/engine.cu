@@ -21,6 +21,7 @@
 #include "gsweep.cuh"
 #include "strkeys.cuh"
 #include "bytevals.cuh"
+#include "segsort.cuh"
 #include <type_traits>
 
 using namespace vb;
@@ -372,6 +373,8 @@ struct vb_shuf {
     // (cogroup materialisation), or — if a join comes first — only for the rows the join kind needs: the keys on BOTH
     // sides (inner), every row of the preserved side plus the matching rows of the other (LEFT / RIGHT), or all (FULL).
     u64 uid = 0;                                   // process-unique id (cache key that survives pointer reuse)
+    int vorder = VB_VALORDER_INPUT;                // vb_shuffle_set_value_order: each list of a GROUP CSR in map order or ascending
+    bool internal = false;                         // made by make_internal_like: a narrow view or a filtered join's side
     bool lazy = false;                             // sealed, rows in lz_*, not grouped yet
     u64 *lz_keys = nullptr, *lz_vals = nullptr;
     u64 lz_n = 0;
@@ -1662,6 +1665,8 @@ __global__ void rebase_kernel(const u64 *__restrict__ src, u64 n, u64 base, u64 
     if (i < n) out[i] = src[i] - base;
 }
 
+static int sort_segments(vb_shuf *s, const u64 *offs, u64 D, u64 *vals, u64 n);
+
 // group_by_key / cogroup reduce side over n rows (AoS `rows`, or SoA keys/vals).
 static int seal_group(vb_shuf *s, const Gathered &g)
 {
@@ -1720,7 +1725,12 @@ static int seal_group(vb_shuf *s, const Gathered &g)
         csr_bounds_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(sorted_ids, n, offs.as<u64>(), D);
         TRY(kl.done("csr_bounds_kernel"));
     }
-    // 7. value offsets at the partition boundaries
+    DevBuf sv_guard(c);
+    sv_guard.p = sorted_vals;
+    // 7. each list ascending where the shuffle asks for it (vb_shuffle_set_value_order)
+    TRY(sort_segments(s, offs.as<u64>(), D, sorted_vals, n));
+    sv_guard.release();
+    // 8. value offsets at the partition boundaries
     {
         DevBuf idx(c), out(c);
         TRY(idx.alloc(((size_t)R + 1) * 8));
@@ -1864,17 +1874,14 @@ static int finalize_reduce(vb_shuf *s, void *tab, u32 log_cap, u64 n_ins)
     return VB_OK;
 }
 
-static int seal_sort(vb_shuf *s, const Gathered &g)
+// Stable LSD sort of n (u64 key, u64 value) rows by tx_fwd(key); the first pass reads them through `first`, whose keys
+// are also at kscan, kstride words apart.  The rows end in *out_k / *out_v, which lie in ka or kb and va or vbuf (the
+// passes alternate between them, starting with ka / va).
+static int lsd_sort_u64(vb_shuf *s, const Loader &first, const u64 *kscan, u32 kstride, u64 n, int tx, bool has_val, DevBuf &ka, DevBuf &kb,
+                        DevBuf &va, DevBuf &vbuf, u64 **out_k, u64 **out_v)
 {
     vb_ctx *c = s->ctx;
-    const u32 R = s->n_reduce;
-    s->bucket_off.assign((size_t)R + 1, 0);
-    s->val_off.assign((size_t)R + 1, 0);
-    const u64 n = g.n;
-    if (n == 0) return VB_OK;
-    const bool has_val = g.rows != nullptr || g.vals != nullptr;
-    const int tx = s->kdt == VB_I64 ? TX_I64 : s->kdt == VB_F64 ? TX_F64 : TX_NONE;
-    DevBuf ka(c), kb(c), va(c), vbuf(c), hist(c);
+    DevBuf hist(c);
     TRY(ka.alloc(n * 8));
     TRY(kb.alloc(n * 8));
     if (has_val) { TRY(va.alloc(n * 8)); TRY(vbuf.alloc(n * 8)); }
@@ -1889,24 +1896,22 @@ static int seal_sort(vb_shuf *s, const Gathered &g)
         const unsigned long long init[2] = {0ull, ~0ull};
         CU(cudaMemcpyAsync(bits.p, init, 16, cudaMemcpyHostToDevice, c->stream));
         KLaunch kl(s, K_MISC);
-        key_bits_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(g.rows ? g.rows : g.keys, g.rows ? 2 : 1, n, tx, (unsigned long long *)bits.p);
+        key_bits_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(kscan, kstride, n, tx, (unsigned long long *)bits.p);
         TRY(kl.done("key_bits_kernel"));
         u64 *h = (u64 *)c->h_scratch;
         CU(cudaMemcpyAsync(h, bits.p, 16, cudaMemcpyDeviceToHost, c->stream));
         CU(cudaStreamSynchronize(c->stream));
         varying = h[0] ^ h[1];
     }
-    bool first = true;
+    bool at_first = true;
     u32 done = 0;
     for (u32 p = 0; p < 8; ++p) {
         const u64 dmask = 0xFFull << (8 * p);
         const bool last_chance = p == 7 && done == 0;      // at least one pass: it also copies the rows out
         if (!(varying & dmask) && !last_chance) continue;
         ++done;
-        Loader ld;
-        if (first) ld = g.rows ? Loader{LD_AOS64, g.rows, nullptr, 0} : Loader{LD_SOA64, g.keys, g.vals, 0};
-        else ld = Loader{LD_SOA64, src_k, has_val ? src_v : nullptr, 0};
-        first = false;
+        const Loader ld = at_first ? first : Loader{LD_SOA64, src_k, has_val ? src_v : nullptr, 0};
+        at_first = false;
         Digit dg{};
         dg.mode = DG_BITS; dg.shift = 8 * p; dg.mask = 0xFF; dg.tx = tx;
         if (has_val) TRY((radix_pass<u64, true>(s, ld, dg, n, dst_k, dst_v, hist.as<u32>(), plan)));
@@ -1915,7 +1920,25 @@ static int seal_sort(vb_shuf *s, const Gathered &g)
         u64 *nv = (src_v == nullptr) ? vbuf.as<u64>() : src_v;
         src_k = dst_k; src_v = dst_v; dst_k = nk; dst_v = nv;
     }
-    // results are in the buffer written by the last pass (ka, kb alternate starting with ka)
+    *out_k = src_k;
+    *out_v = has_val ? src_v : nullptr;
+    return VB_OK;
+}
+
+static int seal_sort(vb_shuf *s, const Gathered &g)
+{
+    vb_ctx *c = s->ctx;
+    const u32 R = s->n_reduce;
+    s->bucket_off.assign((size_t)R + 1, 0);
+    s->val_off.assign((size_t)R + 1, 0);
+    const u64 n = g.n;
+    if (n == 0) return VB_OK;
+    const bool has_val = g.rows != nullptr || g.vals != nullptr;
+    const int tx = s->kdt == VB_I64 ? TX_I64 : s->kdt == VB_F64 ? TX_F64 : TX_NONE;
+    DevBuf ka(c), kb(c), va(c), vbuf(c);
+    u64 *src_k = nullptr, *src_v = nullptr;
+    const Loader first = g.rows ? Loader{LD_AOS64, g.rows, nullptr, 0} : Loader{LD_SOA64, g.keys, g.vals, 0};
+    TRY(lsd_sort_u64(s, first, g.rows ? g.rows : g.keys, g.rows ? 2 : 1, n, tx, has_val, ka, kb, va, vbuf, &src_k, &src_v));
     DevBuf starts(c);
     TRY(starts.alloc(((size_t)R + 1) * 8));
     {
@@ -1932,6 +1955,98 @@ static int seal_sort(vb_shuf *s, const Gathered &g)
     if (has_val) { if (src_v == va.as<u64>()) va.release(); else vbuf.release(); }
     s->st.rows_out = n;
     return VB_OK;
+}
+
+// Each CSR run vals[offs[i] .. offs[i+1]) of the D keys sorted ascending in the value dtype's order, in place, when the
+// shuffle asks for it (vb_shuffle_set_value_order; segsort.cuh).  Runs of 2 to SS_T values are sorted in shared memory,
+// one launch per size class; the longer ones are gathered into one buffer of their values and run ranks, sorted stably
+// by value and then by rank with the radix passes, and scattered back (temporary memory ~ 60 B per value of those runs).
+static int sort_segments(vb_shuf *s, const u64 *offs, u64 D, u64 *vals, u64 n)
+{
+    if (s->vorder != VB_VALORDER_ASC || n <= D) return VB_OK;     // n == D: every list holds one value
+    vb_ctx *c = s->ctx;
+    const int tx = s->vdt == VB_I64 ? TX_I64 : s->vdt == VB_F64 ? TX_F64 : TX_NONE;
+    DevBuf ctr(c), list(c);
+    TRY(ctr.alloc(SS_NCLS * 4));
+    CU(cudaMemsetAsync(ctr.p, 0, SS_NCLS * 4, c->stream));
+    const unsigned grid = (unsigned)std::min<u64>((D + 255) / 256, (u64)c->sm_count * 8);
+    {
+        KLaunch kl(s, K_MISC, D);
+        seg_classify_kernel<<<grid, 256, 0, c->stream>>>(offs, D, ctr.as<u32>(), nullptr, 0);
+        TRY(kl.done("seg_classify_kernel"));
+    }
+    u32 *h = (u32 *)c->h_scratch;
+    CU(cudaMemcpyAsync(h, ctr.p, SS_NCLS * 4, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    std::vector<u32> cnt(h, h + SS_NCLS), start(SS_NCLS + 1, 0);
+    for (int k = 0; k < SS_NCLS; ++k) start[k + 1] = start[k] + cnt[k];
+    if (start[SS_NCLS] == 0) return VB_OK;
+    TRY(list.alloc((u64)start[SS_NCLS] * 4));
+    CU(cudaMemcpyAsync(ctr.p, start.data(), SS_NCLS * 4, cudaMemcpyHostToDevice, c->stream));   // pageable: copied before the call returns
+    {
+        KLaunch kl(s, K_MISC, D);
+        seg_classify_kernel<<<grid, 256, 0, c->stream>>>(offs, D, ctr.as<u32>(), list.as<u32>(), 1);
+        TRY(kl.done("seg_classify_kernel"));
+    }
+    const size_t smem = (size_t)SS_T * 8;
+    CU(cudaFuncSetAttribute((const void *)seg_sort_cta_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    for (u32 k = 0; k < (u32)SS_LOG_T; ++k) {
+        if (!cnt[k]) continue;
+        const u32 log_c = k + 1, per_cta = (u32)SS_T >> log_c;
+        KLaunch kl(s, K_MISC, cnt[k]);
+        seg_sort_cta_kernel<<<(cnt[k] + per_cta - 1) / per_cta, SS_THREADS, smem, c->stream>>>(vals, offs, list.as<u32>() + start[k], cnt[k],
+                                                                                               log_c, tx);
+        TRY(kl.done("seg_sort_cta_kernel"));
+    }
+    const u32 nl = cnt[SS_LOG_T];
+    if (!nl) return VB_OK;
+    // the large runs: bounds, and their values' buffer positions in list order
+    DevBuf starts(c), lens(c), pref(c);
+    TRY(starts.alloc((u64)nl * 8));
+    TRY(lens.alloc((u64)nl * 8));
+    TRY(pref.alloc(((u64)nl + 1) * 8));
+    {
+        KLaunch kl(s, K_MISC, nl);
+        seg_bounds_kernel<<<(nl + 255) / 256, 256, 0, c->stream>>>(offs, list.as<u32>() + start[SS_LOG_T], nl, starts.as<u64>(), lens.as<u64>());
+        TRY(kl.done("seg_bounds_kernel"));
+    }
+    std::vector<u64> hp((size_t)nl + 1, 0);
+    CU(cudaMemcpyAsync(hp.data() + 1, lens.p, (u64)nl * 8, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    for (u32 r = 0; r < nl; ++r) hp[r + 1] += hp[r];
+    const u64 NL = hp[nl];
+    CU(cudaMemcpyAsync(pref.p, hp.data(), ((u64)nl + 1) * 8, cudaMemcpyHostToDevice, c->stream));
+    lens.reset();
+    const unsigned mgrid = (unsigned)std::min<u64>((NL + 255) / 256, (u64)c->sm_count * 8);
+    DevBuf buf(c), rank(c);
+    TRY(buf.alloc(NL * 8));
+    TRY(rank.alloc(NL * 8));
+    {
+        KLaunch kl(s, K_MISC, NL);
+        seg_move_kernel<<<mgrid, 256, 0, c->stream>>>(vals, starts.as<u64>(), pref.as<u64>(), nl, NL, buf.as<u64>(), rank.as<u64>(), 1);
+        TRY(kl.done("seg_move_kernel"));
+    }
+    // stable by value (rank carried along), then stable by rank: each run's values together, ascending
+    DevBuf ka(c), kb(c), va(c), vbuf(c), ids(c);
+    u64 *sk = nullptr, *sr = nullptr;
+    TRY(lsd_sort_u64(s, Loader{LD_SOA64, buf.as<u64>(), rank.as<u64>(), 0}, buf.as<u64>(), 1, NL, tx, true, ka, kb, va, vbuf, &sk, &sr));
+    buf.reset();
+    rank.reset();
+    TRY(ids.alloc(NL * 4));
+    {
+        KLaunch kl(s, K_MISC, NL);
+        narrow_u32_kernel<<<mgrid, 256, 0, c->stream>>>(sr, NL, ids.as<u32>());
+        TRY(kl.done("narrow_u32_kernel"));
+    }
+    u32 *sorted_ids = nullptr;
+    u64 *sorted_vals = nullptr;
+    TRY(sort_id_pairs(s, ids.as<u32>(), Loader{LD_KEY32_VAL_SOA, nullptr, sk, 0}, NL, ceil_log2_u64(std::max<u64>(nl, 2)), &sorted_ids, &sorted_vals));
+    DevBuf sid_guard(c), sv_guard(c);
+    if (sorted_ids != ids.as<u32>()) sid_guard.p = sorted_ids;
+    sv_guard.p = sorted_vals;
+    KLaunch kl(s, K_MISC, NL);
+    seg_move_kernel<<<mgrid, 256, 0, c->stream>>>(vals, starts.as<u64>(), pref.as<u64>(), nl, NL, sorted_vals, nullptr, 0);
+    return kl.done("seg_move_kernel");
 }
 
 static void release_inputs(vb_shuf *s)
@@ -3193,6 +3308,8 @@ static vb_shuf *make_internal_like(const vb_shuf *s)
     t->uid = next_uid.fetch_add(1);                 // N-way plans are cached by the sides' uids
     t->ctx = s->ctx; t->id = s->id; t->n_map = 0; t->n_reduce = s->n_reduce;
     t->kdt = s->kdt; t->vdt = s->vdt; t->agg = s->agg; t->part = s->part; t->key_width = s->key_width;
+    t->vorder = s->vorder;                          // a filtered join's sides read their lists in the user shuffle's order
+    t->internal = true;
     t->rank = 0; t->world = 1;                      // internal shuffles are device-local
     t->sealed = true;
     return t;
@@ -4602,6 +4719,23 @@ extern "C" int32_t vb_shuffle_set_str_key(vb_shuf *s, int32_t kind)
     return VB_OK;
 }
 
+extern "C" int32_t vb_shuffle_set_value_order(vb_shuf *s, int32_t order)
+{
+    if (!s) return set_err(VB_ERR_INVALID, "NULL shuffle");
+    const bool group = s->str ? s->agg == VB_AGG_GROUP && !s->str->sort : is_group_op(s->agg);
+    if (!group || s->internal || s->rep)
+        return set_err(VB_ERR_INVALID, "vb_shuffle_set_value_order: shuffle %llu is not a GROUP or COGROUP shuffle", (unsigned long long)s->id);
+    if (order != VB_VALORDER_INPUT && order != VB_VALORDER_ASC)
+        return set_err(VB_ERR_INVALID, "vb_shuffle_set_value_order: order %d (VB_VALORDER_INPUT or VB_VALORDER_ASC)", order);
+    if (s->vdt == VB_BYTES) return set_err(VB_ERR_UNSUPPORTED, "vb_shuffle_set_value_order: byte-string values have no value order");
+    std::lock_guard<std::mutex> g(s->mu);
+    bool started = s->exported || s->imported || s->sealed || s->sealing || s->freed;
+    for (const MapOut &m : s->maps) started = started || m.present;
+    if (started) return set_err(VB_ERR_STATE, "vb_shuffle_set_value_order: shuffle %llu already has map output", (unsigned long long)s->id);
+    s->vorder = order;
+    return VB_OK;
+}
+
 // Reallocate one device array to `cap` elements of `sz` bytes, keeping the first `keep`.
 template <typename T>
 static int str_regrow(vb_ctx *c, T **p, u64 cap, u64 keep)
@@ -5869,6 +6003,7 @@ static int seal_str_runs(vb_shuf *s, const std::vector<StrRun> &runs)
         } else {
             DevBuf offs(c), vals(c);
             TRY(str_group_values(s, runs, n, dense.as<u32>(), D, offs, vals));
+            TRY(sort_segments(s, offs.as<u64>(), D, vals.as<u64>(), n));
             TRY(str_read_at(s, offs.as<u64>(), s->bucket_off, s->val_off));
             s->n_vals = n;
             s->res_offs = (u64 *)offs.release();

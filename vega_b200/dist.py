@@ -231,14 +231,22 @@ def _rows_import(engine, sh, cols, splits):
     engine.import_(sh, cols[0], cols[1], splits[0])
 
 
+def _set_value_order(sh, value_order):
+    """vb_shuffle_set_value_order on this rank's handle, before its first map call.  Every rank of a shuffle is expected
+    to pass the same order; the library does not check it."""
+    if value_order != L.VB_VALORDER_INPUT:
+        L.check(sh._lib.vb_shuffle_set_value_order(sh._h, value_order))
+
+
 def run_shuffle(engine, local_maps, n_map, n_reduce, kcode, vcode, agg, rank, world, group=None, key_width=8, hint=0,
-                stats=None, exchange_device=None, p2p=False):
+                stats=None, exchange_device=None, p2p=False, value_order=L.VB_VALORDER_INPUT):
     """Map side on this rank's partitions → exchange → reduce side for the partitions this rank owns.
 
     local_maps: [(map_id, keys, vals_or_None)], ascending map ids from map_block(rank, world, n_map).
     Returns the sealed engine handle; engine.reduce(h, r) is non-empty only for r % world == rank.
     exchange_device: move the packed buffers there for the collective (tests: "cpu" + gloo on a 1-GPU box).
     p2p: GROUP/COGROUP shuffles use the fused partition+send over peer memory instead of pack + all-to-all-v.
+    value_order: VB_VALORDER_ASC sorts each key's list of a GROUP/COGROUP shuffle on the rank that owns it.
     """
     if (vcode == L.VB_BYTES) != isinstance(engine, BytesCudaEngine):
         raise TypeError("byte-string values cross ranks with dist.BytesCudaEngine, and it takes byte-string values only")
@@ -246,6 +254,7 @@ def run_shuffle(engine, local_maps, n_map, n_reduce, kcode, vcode, agg, rank, wo
         _bytes_checks(engine, local_maps, n_map, agg, (L.VB_AGG_GROUP, L.VB_AGG_COGROUP, L.VB_AGG_SORT), rank, world,
                       exchange_device)
     sh = engine.create(n_map, n_reduce, kcode, vcode, agg, rank, world, key_width=key_width, hint=hint)
+    _set_value_order(sh, value_order)
     for map_id, keys, vals in local_maps:
         engine.map(sh, map_id, keys, vals)
     p2p = p2p and agg in (L.VB_AGG_GROUP, L.VB_AGG_COGROUP)
@@ -301,17 +310,19 @@ def _str_import(engine, sh, cols, splits):
 
 
 def run_str_shuffle(engine, local_maps, n_map, n_reduce, vcode, agg, rank, world, group=None, hint=0, stats=None,
-                    exchange_device=None):
+                    exchange_device=None, value_order=L.VB_VALORDER_INPUT):
     """run_shuffle for String keys: map side on this rank's partitions → exchange → reduce side for the partitions
     this rank owns.  local_maps: [(map_id, keys, vals_or_None)], ascending map ids from map_block(rank, world, n_map).
     With a communicator on the context the exchange is vb_shuffle_exchange (NCCL inside the library); otherwise
     all_to_all_v of the four columns (exchange_device: "cpu" for a gloo group on a one-GPU box).  agg VB_AGG_SORT
-    (sort_by_key) across ranks has no such fallback: its cut keys are agreed in rounds of the library's collectives."""
+    (sort_by_key) across ranks has no such fallback: its cut keys are agreed in rounds of the library's collectives.
+    value_order as for run_shuffle (GROUP only)."""
     if (vcode == L.VB_BYTES) != isinstance(engine, StrBytesCudaEngine):
         raise TypeError("byte-string values cross ranks with dist.StrBytesCudaEngine, and it takes byte-string values only")
     if isinstance(engine, StrBytesCudaEngine):
         _bytes_checks(engine, local_maps, n_map, agg, (L.VB_AGG_GROUP, L.VB_AGG_SORT), rank, world, exchange_device)
         sh = engine.create(n_map, n_reduce, vcode, agg, rank, world, hint=hint)
+        _set_value_order(sh, value_order)
         for map_id, keys, vals in local_maps:
             engine.map(sh, map_id, keys, vals)
         return _exchange(engine, sh, (StrBytesCudaEngine, _str_bytes_export, _str_bytes_import, 3), rank, world, group, stats,
@@ -321,6 +332,7 @@ def run_str_shuffle(engine, local_maps, n_map, n_reduce, vcode, agg, rank, world
         raise ValueError("sort_by_key over String keys across ranks needs the library's communicator (vb_ctx_comm_init, "
                          "Context.comm_init) and runs its exchange inside the library")
     sh = engine.create(n_map, n_reduce, vcode, agg, rank, world, hint=hint)
+    _set_value_order(sh, value_order)
     for map_id, keys, vals in local_maps:
         engine.map(sh, map_id, keys, vals)
     return _exchange(engine, sh, (StrCudaEngine, _str_export, _str_import, 3), rank, world, group, stats, exchange_device)

@@ -254,8 +254,11 @@ class Context:
 class Shuffle:
     """Thin RAII wrapper of one vb_shuf (== one ShuffleDependency / shuffle_id)."""
 
-    def __init__(self, sc, n_map, n_reduce, kcode, vcode, agg, key_width=8, hint=0, rank=0, world=1, multi=None):
-        """multi: (value column dtype codes, [(vb_agg, column), ...]) for a vb_shuffle_create_multi shuffle."""
+    def __init__(self, sc, n_map, n_reduce, kcode, vcode, agg, key_width=8, hint=0, rank=0, world=1, multi=None,
+                 value_order=L.VB_VALORDER_INPUT):
+        """multi: (value column dtype codes, [(vb_agg, column), ...]) for a vb_shuffle_create_multi shuffle.
+        value_order: VB_VALORDER_ASC sorts each key's list of a GROUP / COGROUP shuffle ascending on the device
+        (vb_shuffle_set_value_order)."""
         self.sc, self._lib = sc, sc._lib
         self.n_map, self.n_reduce, self.agg, self.vcode, self.kcode = n_map, n_reduce, agg, vcode, kcode
         self.has_payload = True
@@ -278,6 +281,8 @@ class Shuffle:
             L.check(self._lib.vb_shuffle_set_hint(h, hint))
         if world > 1:
             L.check(self._lib.vb_shuffle_set_dist(h, rank, world))
+        if value_order != L.VB_VALORDER_INPUT:
+            L.check(self._lib.vb_shuffle_set_value_order(h, value_order))
 
     @classmethod
     def combine_dist(cls, sc, n_map, n_reduce, kcode, multi, rank, world, key_width=8, hint=0):
@@ -581,6 +586,19 @@ def _vals_out(sh, v, valid=None):
     return v if valid is None else np.ma.MaskedArray(v, mask=valid == 0)
 
 
+def _value_order(sort_values, parents):
+    """The vb_value_order of sort_values=... for shuffles of `parents` (TypeError, before any device work, for a
+    non-bool or for byte-string values, which have no value order)."""
+    if not isinstance(sort_values, (bool, np.bool_)):
+        raise TypeError(f"sort_values must be a bool, got {sort_values!r}")
+    if not sort_values:
+        return L.VB_VALORDER_INPUT
+    for r in parents:
+        if isinstance(getattr(r, "vals", None), _BytesCol):
+            raise TypeError("sort_values: byte-string values have no value order")
+    return L.VB_VALORDER_ASC
+
+
 def _refuse_bytes(parent, what):
     """TypeError, before any device work, for an op that computes on byte-string values."""
     if isinstance(getattr(parent, "vals", None), _BytesCol):
@@ -652,13 +670,14 @@ class ShuffledRdd(_AggregatedParent):
     """ShuffledRdd<K,V,C> (src/rdd/shuffled_rdd.rs): lazy; `collect()` runs the job.  A sum / min / max / count result
     is also a join and cogroup parent (see _AggregatedParent)."""
 
-    def __init__(self, parent, agg_name, num_splits, hint=0):
+    def __init__(self, parent, agg_name, num_splits, hint=0, sort_values=False):
         if num_splits < 1:
             raise ValueError("num_splits must be >= 1")
         if len(getattr(parent, "cols", ())) > 1:
             raise TypeError("a PairRdd with several value columns supports combine_by_key only")
         if agg_name in _REDUCE_AGGS:
             _refuse_bytes(parent, "reduce_by_key / count_by_key")
+        self.value_order = _value_order(sort_values, [parent])
         self.parent, self.agg_name, self.num_slices, self.hint = parent, agg_name, num_splits, hint
         self.sc = parent.sc
         self._sh = None
@@ -682,7 +701,7 @@ class ShuffledRdd(_AggregatedParent):
         starts = slice_starts(p.n, p.num_slices)
         vcode = p.vals.code if p.vals is not None else (p.keys.code if p.keys.rows else L.VB_U64)
         sh = Shuffle(self.sc, len(starts) - 1, self.num_slices, p.keys.code, vcode, _AGG[self.agg_name],
-                     key_width=p.keys.key_width, hint=self.hint)
+                     key_width=p.keys.key_width, hint=self.hint, value_order=self.value_order)
         sh.has_payload = p.vals is not None or p.keys.rows
         for m in range(len(starts) - 1):                    # map stage
             sh.map(m, p.keys, p.vals, int(starts[m]), int(starts[m + 1]))
@@ -722,9 +741,11 @@ class JoinedRdd(_Base):
     kind "left" / "right" / "full": the outer joins (Spark's leftOuterJoin / rightOuterJoin / fullOuterJoin, which
     vega lacks).  A key missing on the other side still gives rows, with None on that side.  compute(r) / collect()
     return (k, v, w); a side that can be None is a numpy.ma.MaskedArray (masked = None, data 0), the other side a
-    plain array."""
+    plain array.  sort_values=True: each PairRdd side's lists ascending in its value dtype's order (so the rows of a
+    key come in that order too); a reduce-result side has one value per key."""
 
-    def __init__(self, left, right, num_splits, kind=None):
+    def __init__(self, left, right, num_splits, kind=None, sort_values=False):
+        self.value_order = _value_order(sort_values, (left, right))
         if kind is not None:
             if kind not in _JOIN_KINDS:
                 raise ValueError(f"join kind {kind!r} is not one of {sorted(_JOIN_KINDS)}")
@@ -749,7 +770,8 @@ class JoinedRdd(_Base):
 
     def _run(self):
         if self._shs is None:
-            a, b = (r if isinstance(r, _AggregatedParent) else ShuffledRdd(r, "cogroup", self.num_slices)
+            a, b = (r if isinstance(r, _AggregatedParent) else
+                    ShuffledRdd(r, "cogroup", self.num_slices, sort_values=self.value_order == L.VB_VALORDER_ASC)
                     for r in (self.left, self.right))
             if self.left.keys.key_width != self.right.keys.key_width:
                 raise TypeError("join sides have different key types")
@@ -820,9 +842,10 @@ class CoGroupedRdd(_Base):
     reference's Vec<(K, Vec<Vec<V>>)> as a list of (k, [vs_0, ..., vs_{n-1}]).  join_compute(r) / join_collect() give
     the inner join of all parents as (k, [v_0, ..., v_{n-1}]) arrays: per key, for v0 in vs_0 { for v1 in vs_1 { ... } }.
     outer_join_compute(r, required) / outer_join_collect(required) give the outer join in which only the required
-    parents must have the key.  Each parent's values keep that parent's dtype."""
+    parents must have the key.  Each parent's values keep that parent's dtype.  sort_values=True: every shuffled
+    parent's lists ascending in its value dtype's order (vb_shuffle_set_value_order)."""
 
-    def __init__(self, rdds, num_splits):
+    def __init__(self, rdds, num_splits, sort_values=False):
         rdds = list(rdds)
         if not 1 <= len(rdds) <= L.VB_MAX_COGROUP_SIDES:
             raise ValueError(f"a cogroup takes 1 to {L.VB_MAX_COGROUP_SIDES} parents, got {len(rdds)}")
@@ -843,12 +866,14 @@ class CoGroupedRdd(_Base):
         k0 = rdds[0].keys
         if any(r.keys.key_width != k0.key_width or r.keys.code != k0.code for r in rdds):
             raise TypeError("the parents have different key types")
+        self.value_order = _value_order(sort_values, rdds)
         self.rdds, self.num_slices, self.sc = rdds, num_splits, rdds[0].sc
         self._shs = None
 
     def _run(self):
         if self._shs is None:
-            self._shs = [(r if isinstance(r, _AggregatedParent) else ShuffledRdd(r, "cogroup", self.num_slices))
+            asc = self.value_order == L.VB_VALORDER_ASC
+            self._shs = [(r if isinstance(r, _AggregatedParent) else ShuffledRdd(r, "cogroup", self.num_slices, sort_values=asc))
                          ._cogroup_side(self.num_slices) for r in self.rdds]
         return self._shs
 
@@ -1203,8 +1228,10 @@ class PairRdd(_Base):
             raise ValueError("combine_by_key takes keys and value columns, not (n,2) rows")
         return CombinedRdd(self, aggs, num_splits, hint)
 
-    def group_by_key(self, num_splits):
-        return ShuffledRdd(self, "group", num_splits)
+    def group_by_key(self, num_splits, sort_values=False):
+        """sort_values=True: each key's values ascending in the value dtype's order (u64 unsigned, i64 signed, f64 as
+        f64::total_cmp), sorted on the device; otherwise in map order."""
+        return ShuffledRdd(self, "group", num_splits, sort_values=sort_values)
 
     def reduce_by_key(self, op, num_splits, hint=0):
         if op not in ("sum", "min", "max"):
@@ -1214,23 +1241,24 @@ class PairRdd(_Base):
     def count_by_key(self, num_splits=None, hint=0):
         return ShuffledRdd(self, "count", num_splits or self.num_slices, hint)
 
-    def join(self, other, num_splits):
-        return JoinedRdd(self, other, num_splits)
+    def join(self, other, num_splits, sort_values=False):
+        """sort_values=True: each key's rows in ascending order of both sides' values (see JoinedRdd)."""
+        return JoinedRdd(self, other, num_splits, sort_values=sort_values)
 
-    def left_outer_join(self, other, num_splits):
+    def left_outer_join(self, other, num_splits, sort_values=False):
         """(k, v, w) for every left row; w is None (masked) for a key the other side lacks."""
-        return JoinedRdd(self, other, num_splits, "left")
+        return JoinedRdd(self, other, num_splits, "left", sort_values=sort_values)
 
-    def right_outer_join(self, other, num_splits):
+    def right_outer_join(self, other, num_splits, sort_values=False):
         """(k, v, w) for every right row; v is None (masked) for a key this side lacks."""
-        return JoinedRdd(self, other, num_splits, "right")
+        return JoinedRdd(self, other, num_splits, "right", sort_values=sort_values)
 
-    def full_outer_join(self, other, num_splits):
+    def full_outer_join(self, other, num_splits, sort_values=False):
         """Rows of both sides; v or w is None (masked) for a key only the other side has."""
-        return JoinedRdd(self, other, num_splits, "full")
+        return JoinedRdd(self, other, num_splits, "full", sort_values=sort_values)
 
-    def cogroup(self, other, num_splits):
-        return JoinedRdd(self, other, num_splits)
+    def cogroup(self, other, num_splits, sort_values=False):
+        return JoinedRdd(self, other, num_splits, sort_values=sort_values)
 
     def sort_by_key(self, num_splits):
         return ShuffledRdd(self, "sort", num_splits)
@@ -1607,11 +1635,13 @@ class StrShuffle(Shuffle):
     world > 1 (vb_shuffle_create_str_sort_dist) the rows cross ranks through exchange() only, which needs the
     library's communicator (Context.comm_init); rank r then holds the partitions p with p % world == r.
     seal / exchange / stats / free as for Shuffle.  key_kind: VB_STRKEY_STR (Rust String placement) or VB_STRKEY_BYTES
-    (Vec<u8> placement, vb_shuffle_set_str_key); keys come back as str or bytes accordingly."""
+    (Vec<u8> placement, vb_shuffle_set_str_key); keys come back as str or bytes accordingly.  value_order as for Shuffle
+    (GROUP shuffles only)."""
 
     key_kind = L.VB_STRKEY_STR
 
-    def __init__(self, sc, n_map, n_reduce, vcode, agg, hint=0, rank=0, world=1, multi=None, sort=False, key_kind=L.VB_STRKEY_STR):
+    def __init__(self, sc, n_map, n_reduce, vcode, agg, hint=0, rank=0, world=1, multi=None, sort=False, key_kind=L.VB_STRKEY_STR,
+                 value_order=L.VB_VALORDER_INPUT):
         self.sc, self._lib = sc, sc._lib
         self.key_kind = key_kind
         self.n_map, self.n_reduce, self.agg, self.vcode, self.kcode = n_map, n_reduce, agg, vcode, None
@@ -1651,6 +1681,8 @@ class StrShuffle(Shuffle):
             L.check(self._lib.vb_shuffle_set_str_key(h, key_kind))
         if hint:
             L.check(self._lib.vb_shuffle_set_hint(h, hint))
+        if value_order != L.VB_VALORDER_INPUT:
+            L.check(self._lib.vb_shuffle_set_value_order(h, value_order))
 
     @classmethod
     def bytes_dist(cls, sc, n_map, n_reduce, rank, world, sort=False, hint=0, key_kind=L.VB_STRKEY_STR):
@@ -1894,13 +1926,14 @@ def _no_str(what):
 class StrShuffledRdd(ShuffledRdd):
     """ShuffledRdd over string keys: collect() gives (keys, combined) or a Grouped whose keys are Python strs."""
 
-    def __init__(self, parent, agg_name, num_splits, hint=0):
+    def __init__(self, parent, agg_name, num_splits, hint=0, sort_values=False):
         if num_splits < 1:
             raise ValueError("num_splits must be >= 1")
         if len(getattr(parent, "cols", ())) > 1:
             raise TypeError("a PairRdd with several value columns supports combine_by_key only")
         if agg_name in _REDUCE_AGGS:
             _refuse_bytes(parent, "reduce_by_key / count_by_key")
+        self.value_order = _value_order(sort_values, [parent])
         self.parent, self.agg_name, self.num_slices, self.hint = parent, agg_name, num_splits, hint
         self.sc = parent.sc
         self._sh = None
@@ -1912,7 +1945,7 @@ class StrShuffledRdd(ShuffledRdd):
         starts = slice_starts(p.n, p.num_slices)
         vcode = p.vals.code if p.vals is not None else L.VB_U64
         sh = StrShuffle(self.sc, len(starts) - 1, self.num_slices, vcode, _AGG[self.agg_name], hint=self.hint,
-                        key_kind=_key_kind(p.keys))
+                        key_kind=_key_kind(p.keys), value_order=self.value_order)
         for m in range(len(starts) - 1):
             sh.map(m, p.keys, p.vals, int(starts[m]), int(starts[m + 1]))
         sh.seal()
@@ -1949,8 +1982,9 @@ class StrPairRdd(PairRdd):
                             "Context.parallelize(keys, num_slices, values=(c0, ...))")
         return StrCombinedRdd(self, aggs, num_splits, hint)
 
-    def group_by_key(self, num_splits):
-        return StrShuffledRdd(self, "group", num_splits)
+    def group_by_key(self, num_splits, sort_values=False):
+        """sort_values=True: each key's values ascending in the value dtype's order, as PairRdd.group_by_key."""
+        return StrShuffledRdd(self, "group", num_splits, sort_values=sort_values)
 
     def reduce_by_key(self, op, num_splits, hint=0):
         if op not in ("sum", "min", "max"):
@@ -2061,11 +2095,12 @@ class StrCoGroupedRdd(_Base):
       join_compute(r) / join_collect() -> (k, [v_0, ..., v_{n-1}]), one k per row
       outer_join_compute(r, required) / outer_join_collect(required): optional parents as numpy.ma.MaskedArray
     join_raw(r, required) returns the device's keyed form without decoding: (key offsets, key bytes, row offsets,
-    [values], [validity or None]), each key once with its rows [row_offsets[i], row_offsets[i + 1])."""
+    [values], [validity or None]), each key once with its rows [row_offsets[i], row_offsets[i + 1]).
+    sort_values=True: every StrPairRdd parent's lists ascending in its value dtype's order."""
 
     key_kind = L.VB_STRKEY_STR           # the parents' key kind (all alike: __init__ refuses a mix)
 
-    def __init__(self, rdds, num_splits):
+    def __init__(self, rdds, num_splits, sort_values=False):
         rdds = list(rdds)
         if not 1 <= len(rdds) <= L.VB_MAX_COGROUP_SIDES:
             raise ValueError(f"a cogroup takes 1 to {L.VB_MAX_COGROUP_SIDES} parents, got {len(rdds)}")
@@ -2086,6 +2121,7 @@ class StrCoGroupedRdd(_Base):
         if any(k != kinds[0] for k in kinds):      # equal bytes sit in different partitions under the two hashes
             raise TypeError("the parents mix String keys and BytesKeys (Vec<u8>) keys: they are placed by different hashes")
         self.key_kind = kinds[0]
+        self.value_order = _value_order(sort_values, rdds)
         self.rdds, self.num_slices, self.sc = rdds, num_splits, rdds[0].sc
         self._shs = None
 
@@ -2094,7 +2130,7 @@ class StrCoGroupedRdd(_Base):
     def _side(self, r):
         """The sealed string GROUP shuffle over num_splits partitions this parent gives."""
         if isinstance(r, StrPairRdd):
-            return StrShuffledRdd(r, "group", self.num_slices)._run()
+            return StrShuffledRdd(r, "group", self.num_slices, sort_values=self.value_order == L.VB_VALORDER_ASC)._run()
         sh = r._run()
         col, n_cols, vcode = r._result_col(sh)
         if sh.n_reduce == self.num_slices:
