@@ -133,6 +133,19 @@ VB_D u64 policy_evict_first()
     return p;
 }
 
+VB_D u64 policy_evict_normal()
+{
+    u64 p;
+    asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+VB_D u64 policy_evict_last()
+{
+    u64 p;
+    asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+
 // 128-bit streaming load: read-only path, no L1 allocation, L2 evict-first (the input is read
 // exactly once and must not push the hash table out of the 50 MB L2).
 VB_D ulonglong2 ld_stream_u64x2(const void *p, u64 pol)

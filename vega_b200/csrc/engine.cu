@@ -520,6 +520,8 @@ static int launch_hash_agg_t(vb_shuf *s, int klass, const u64 *a, const u64 *b, 
                              TableCtl *ctl, u64 max_inserts, u32 *slot_out)
 {
     vb_ctx *c = s->ctx;
+    Table t = table_at(tab, log_cap);
+    t.keep_l2 = table_bytes(log_cap) <= c->l2_bytes / 3 * 2;     // choose_log_cap's L2 budget
     if constexpr (IN != IN_TABLE) {
         // bulk-staged (copy engine) variant: 16-byte aligned inputs of at least a few tiles per CTA
         const bool aligned = (((uintptr_t)a | (uintptr_t)(b ? b : a)) & 15u) == 0;
@@ -533,7 +535,7 @@ static int launch_hash_agg_t(vb_shuf *s, int klass, const u64 *a, const u64 *b, 
             u64 grid = std::min<u64>(n / HB_TILE, (u64)c->sm_count * occ);
             KLaunch kl(s, klass, n);
             if (klass == K_HASH_AGG) s->st.hot_kernel_variant = 1;
-            kb<<<(unsigned)grid, HB_THREADS, smem, c->stream>>>(a, b, n, table_at(tab, log_cap), ctl, max_inserts, slot_out);
+            kb<<<(unsigned)grid, HB_THREADS, smem, c->stream>>>(a, b, n, t, ctl, max_inserts, slot_out);
             return kl.done("hash_agg_bulk_kernel");
         }
     }
@@ -543,7 +545,7 @@ static int launch_hash_agg_t(vb_shuf *s, int klass, const u64 *a, const u64 *b, 
     u64 grid = std::min<u64>(tiles, (u64)c->sm_count * occ);
     if (grid == 0) return VB_OK;
     KLaunch kl(s, klass, n);
-    kern<<<(unsigned)grid, HA_THREADS, 0, c->stream>>>(a, b, n, table_at(tab, log_cap), ctl, max_inserts, slot_out);
+    kern<<<(unsigned)grid, HA_THREADS, 0, c->stream>>>(a, b, n, t, ctl, max_inserts, slot_out);
     return kl.done("hash_agg_kernel");
 }
 

@@ -27,6 +27,7 @@ struct Table {
     u64 *keys;    // [cap + 4]: keys[cap] is the marker of the special slot (1 = EMPTY_KEY present)
     u64 *accs;    // [cap + 4]: combiner per slot (reduce ops); unused by the dictionary
     u32 log_cap;  // cap = 1 << log_cap slots = cap / 4 buckets; log_cap >= 2
+    u32 keep_l2;  // 1: bucket probes ask L2 to evict the table last (set by the host when the table fits L2)
 };
 constexpr u64 EMPTY_KEY = ~0ull;
 constexpr u32 BUCKET = 4;
@@ -37,6 +38,7 @@ VB_HD Table table_at(void *base, u32 log_cap)
     t.keys = (u64 *)base;
     t.accs = (u64 *)base + (((size_t)1 << log_cap) + BUCKET);
     t.log_cap = log_cap;
+    t.keep_l2 = 0;
     return t;
 }
 
@@ -78,14 +80,18 @@ struct Bucket4 { u64 k0, k1, k2, k3; };
 
 // one 32-byte sector: 4 candidate keys.  sm_90 loads at most 128 bits per thread, so the sector is read
 // by two independent 128-bit loads issued back to back (both in flight together: one L2 latency, not two).
-VB_D Bucket4 ld_bucket(const u64 *p)
+// t.keep_l2: the loads carry an L2 evict_last policy (else evict_normal, the default), so that the streamed input (evict_first) never pushes a table
+// that fits L2 out of it (H100: 11 % off the headline step, DESIGN §5).  Not for larger tables, where it made
+// the kernel slower.
+VB_D Bucket4 ld_bucket(const Table &t, u64 b)
 {
-    Bucket4 b;
-    asm volatile("ld.global.L1::no_allocate.v2.u64 {%0, %1}, [%4];\n\t"
-                 "ld.global.L1::no_allocate.v2.u64 {%2, %3}, [%4+16];"
-                 : "=l"(b.k0), "=l"(b.k1), "=l"(b.k2), "=l"(b.k3)
-                 : "l"(p));
-    return b;
+    const u64 *p = &t.keys[4 * b];
+    Bucket4 r;
+    asm volatile("ld.global.L1::no_allocate.L2::cache_hint.v2.u64 {%0, %1}, [%4], %5;\n\t"
+                 "ld.global.L1::no_allocate.L2::cache_hint.v2.u64 {%2, %3}, [%4+16], %5;"
+                 : "=l"(r.k0), "=l"(r.k1), "=l"(r.k2), "=l"(r.k3)
+                 : "l"(p), "l"(t.keep_l2 ? policy_evict_last() : policy_evict_normal()));
+    return r;
 }
 VB_D int bucket_find(const Bucket4 &b, u64 key)
 {
@@ -124,7 +130,7 @@ VB_D bool table_resolve_with(const Table &t, u64 b, Bucket4 bk, u64 key, u32 &in
             on_hit(4 * b + (u64)hit);
             return true;
         }
-        bk = ld_bucket(&t.keys[4 * b]);
+        bk = ld_bucket(t, b);
     }
     return false;
 }
@@ -237,7 +243,7 @@ VB_D void ha_probe_rows(const Table &t, TableCtl *ctl, const u64 (&k)[ROWS], boo
 #pragma unroll
     for (int j = 0; j < ROWS; ++j) {
         bidx[j] = h[j] >> hshift;
-        if (ok[j]) bk[j] = ld_bucket(&t.keys[4 * bidx[j]]);
+        if (ok[j]) bk[j] = ld_bucket(t, bidx[j]);
     }
     bool pending = true;
 #pragma unroll 1
@@ -268,7 +274,7 @@ VB_D void ha_probe_rows(const Table &t, TableCtl *ctl, const u64 (&k)[ROWS], boo
         if (pending) {
 #pragma unroll
             for (int j = 0; j < ROWS; ++j)
-                if (ok[j]) bk[j] = ld_bucket(&t.keys[4 * bidx[j]]);
+                if (ok[j]) bk[j] = ld_bucket(t, bidx[j]);
         }
     }
     if (pending) atomicExch(&ctl->abort, 1u);   // probe chain longer than HA_MAX_PROBE buckets
@@ -353,7 +359,7 @@ hash_agg_kernel(const u64 *__restrict__ a, const u64 *__restrict__ b, u64 n, Tab
             if (key == EMPTY_KEY) continue;
             const u64 hb = home_bucket(key, t.log_cap);
             u32 slot = 0;
-            if (!table_resolve<OPK_FLUSH>(t, hb, ld_bucket(&t.keys[4 * hb]), key, hc_acc[i], slot, my_inserts)) atomicExch(&ctl->abort, 1u);
+            if (!table_resolve<OPK_FLUSH>(t, hb, ld_bucket(t, hb), key, hc_acc[i], slot, my_inserts)) atomicExch(&ctl->abort, 1u);
         }
     }
     u32 w = __reduce_add_sync(0xffffffffu, my_inserts);
@@ -515,7 +521,7 @@ hash_agg_bulk_kernel(const u64 *__restrict__ a, const u64 *__restrict__ b, u64 n
                 if (key == EMPTY_KEY) continue;
                 const u64 hb = home_bucket(key, t.log_cap);
                 u32 slot = 0;
-                if (!table_resolve<OPK_FLUSH>(t, hb, ld_bucket(&t.keys[4 * hb]), key, hc_acc[i], slot, my_inserts)) atomicExch(&ctl->abort, 1u);
+                if (!table_resolve<OPK_FLUSH>(t, hb, ld_bucket(t, hb), key, hc_acc[i], slot, my_inserts)) atomicExch(&ctl->abort, 1u);
             }
     }
     u32 w = __reduce_add_sync(0xffffffffu, my_inserts);
@@ -662,7 +668,7 @@ VB_D void ma_cache_flush(const Table &t, TableCtl *ctl, const AccSpec &sp, const
         const u64 key = hc_keys[i];
         if (key == EMPTY_KEY) continue;
         const u64 hb = home_bucket(key, t.log_cap);
-        if (!table_resolve_with(t, hb, ld_bucket(&t.keys[4 * hb]), key, my_inserts, [&](u64 s) {
+        if (!table_resolve_with(t, hb, ld_bucket(t, hb), key, my_inserts, [&](u64 s) {
                 for (int a = 0; a < (int)sp.n; ++a) op_red_rt(t.accs + (u64)a * stride + s, merge_op(spec_at(sp.op, a)), hc_acc[a * MA_HC_SLOTS + i]);
             }))
             atomicExch(&ctl->abort, 1u);
@@ -915,7 +921,7 @@ VB_D u32 table_find(const Table &t, u64 key)
     if (key == EMPTY_KEY) return t.keys[cap] == 1ull ? (u32)cap : 0xFFFFFFFFu;
     u64 b = home_bucket(key, t.log_cap);
     for (u32 probe = 0; probe <= HA_MAX_PROBE; ++probe) {
-        const Bucket4 bk = ld_bucket(&t.keys[4 * b]);
+        const Bucket4 bk = ld_bucket(t, b);
         const int hit = bucket_find(bk, key);
         if (hit >= 0) return (u32)(4 * b + hit);
         if (bucket_find(bk, EMPTY_KEY) >= 0) return 0xFFFFFFFFu;
@@ -1611,7 +1617,7 @@ __global__ void narrow_dict_kernel(const u64 *__restrict__ keys, u64 n, Table t,
     }
     const u64 b = home_bucket(key, t.log_cap);
     u32 inserted = 0;
-    if (!table_resolve_with(t, b, ld_bucket(&t.keys[4 * b]), key, inserted, [&](u64 slot) { dense_of_slot[slot] = (u32)i; }))
+    if (!table_resolve_with(t, b, ld_bucket(t, b), key, inserted, [&](u64 slot) { dense_of_slot[slot] = (u32)i; }))
         atomicExch(&ctl->abort, 1u);
 }
 
