@@ -522,6 +522,7 @@ static int launch_hash_agg_t(vb_shuf *s, int klass, const u64 *a, const u64 *b, 
     vb_ctx *c = s->ctx;
     Table t = table_at(tab, log_cap);
     t.keep_l2 = table_bytes(log_cap) <= c->l2_bytes / 3 * 2;     // choose_log_cap's L2 budget
+    t.max_probe = chain_limit(max_inserts != ~0ull);              // no insert limit: the table is at its final size
     if constexpr (IN != IN_TABLE) {
         // bulk-staged (copy engine) variant: 16-byte aligned inputs of at least a few tiles per CTA
         const bool aligned = (((uintptr_t)a | (uintptr_t)(b ? b : a)) & 15u) == 0;
@@ -589,7 +590,8 @@ static int launch_hash_agg_multi_t(vb_shuf *s, int klass, const AccSpec &sp, con
                                    u32 log_cap, TableCtl *ctl, u64 max_inserts)
 {
     vb_ctx *c = s->ctx;
-    const Table t = table_at(tab, log_cap);
+    Table t = table_at(tab, log_cap);
+    t.max_probe = chain_limit(max_inserts != ~0ull);              // no insert limit: the table is at its final size
     if constexpr (IN == IN_SOA) {
         uintptr_t addr = (uintptr_t)keys;
         for (int i = 0; i < NV; ++i) addr |= (uintptr_t)cols.c[i];
@@ -800,7 +802,10 @@ static int build_table(vb_shuf *s, int klass, const std::vector<AggInput> &input
     }
     if (slot_out && any_host) return set_err(VB_ERR_INVALID, "build_table: dictionary inputs must be on the device");
     // capacity never needs to exceed 2x the items; slot indices are 32-bit, so 2^31 slots is the ceiling — an input
-    // with more than ~1.3e9 distinct keys fails with "overflow at maximum capacity", fewer distinct keys fit whatever the row count
+    // with more than ~1.3e9 distinct keys fails with "overflow at maximum capacity", fewer distinct keys fit whatever the row
+    // count and wherever they hash: a table of max_log slots holds at most half as many keys, so it runs without an insert
+    // limit and no probe-round limit (chain_limit).  Only above 2^30 items, where the 2^31-slot ceiling can be over half
+    // full, does the table keep the 0.6 insert limit and the HA_MAX_PROBE round limit.
     const u32 max_log = std::min<u32>(MAX_LOG_CAP, std::max<u32>(4, ceil_log2_u64(2 * std::max<u64>(total, 1))));
     bool estimated = false;
     if (!hint_distinct && total > (1ull << 20)) { TRY(estimate_distinct(s, inputs, total, &hint_distinct)); estimated = true; }
@@ -827,7 +832,7 @@ static int build_table(vb_shuf *s, int klass, const std::vector<AggInput> &input
         TRY(tab.alloc(ms ? table_bytes_multi(log_cap, ms->n) : table_bytes(log_cap)));
         TRY(init_table(s, tab.p, log_cap, opk, ms));
         CU(cudaMemsetAsync(ctl.p, 0, sizeof(TableCtl), c->stream));
-        const u64 max_inserts = (log_cap == max_log) ? ~0ull : (cap / 10) * 6;
+        const u64 max_inserts = (log_cap == max_log && cap >= 2 * total) ? ~0ull : (cap / 10) * 6;
         u64 row_base = 0;
         for (auto &in : inputs) {
             if (in.n == 0) continue;
@@ -1499,7 +1504,9 @@ static int shuffle_map(vb_shuf *s, u32 map_id, const u64 *rows, const u64 *keys,
             TRY(ctl.alloc(sizeof(TableCtl)));
             CU(cudaMemsetAsync(ctl.p, 0, sizeof(TableCtl), c->stream));
             TRY(init_table(s, tab.p, s->sh_log_cap, map_opk(s), ms));
-            s->sh_max_inserts = (s->sh_log_cap >= max_log) ? ~0ull : ((1ull << s->sh_log_cap) / 10) * 6;
+            // the total is a guess from the first map task, so even a table at max_log keeps the insert limit (and the
+            // HA_MAX_PROBE chain limit): a wrong guess or a long chain rebuilds it at seal through build_table
+            s->sh_max_inserts = ((1ull << s->sh_log_cap) / 10) * 6;
             s->sh_tab = tab.release();
             s->sh_ctl = (TableCtl *)ctl.release();
             s->st.table_slots = std::max<u64>(s->st.table_slots, 1ull << s->sh_log_cap);
@@ -3598,7 +3605,8 @@ static int narrow_build(vb_shuf *v, const u64 *keys, const u64 *col, u64 n)
     TRY(k.alloc(n * 8)); TRY(vals.alloc(n * 8)); TRY(offs.alloc((n + 1) * 8)); TRY(ctl.alloc(sizeof(TableCtl)));
     CU(cudaMemcpyAsync(k.p, keys, n * 8, cudaMemcpyDeviceToDevice, c->stream));
     CU(cudaMemcpyAsync(vals.p, col, n * 8, cudaMemcpyDeviceToDevice, c->stream));
-    // load <= 0.5 by construction, so only a probe chain longer than HA_MAX_PROBE buckets makes the kernel give up
+    // load <= 0.5 by construction; a probe chain longer than HA_MAX_PROBE buckets restarts the table larger, and at max_log,
+    // where it cannot grow, inserts have no probe-round limit (chain_limit), so every insert succeeds
     const u32 max_log = std::min<u32>(MAX_LOG_CAP, std::max<u32>(4, ceil_log2_u64(2 * n)));
     u32 log_cap = choose_log_cap(n, n, false, max_log, c->l2_bytes);
     for (;;) {
@@ -3611,8 +3619,10 @@ static int narrow_build(vb_shuf *v, const u64 *keys, const u64 *col, u64 n)
         CU(cudaMemsetAsync(ctl.p, 0, sizeof(TableCtl), c->stream));
         {
             KLaunch kl(v, K_DICT, n);
-            narrow_dict_kernel<<<(unsigned)((n + 1 + 255) / 256), 256, 0, c->stream>>>(k.as<u64>(), n, table_at(tab.p, log_cap),
-                                                                                      dense.as<u32>(), offs.as<u64>(), ctl.as<TableCtl>());
+            Table t = table_at(tab.p, log_cap);
+            t.max_probe = chain_limit(log_cap < max_log || cap < 2 * n);
+            narrow_dict_kernel<<<(unsigned)((n + 1 + 255) / 256), 256, 0, c->stream>>>(k.as<u64>(), n, t, dense.as<u32>(), offs.as<u64>(),
+                                                                                      ctl.as<TableCtl>());
             TRY(kl.done("narrow_dict_kernel"));
         }
         TableCtl h;

@@ -24,13 +24,24 @@ namespace vb {
 // the REDs that follow from invalidating L1 lines.
 // ---------------------------------------------------------------------------------------------
 struct Table {
-    u64 *keys;    // [cap + 4]: keys[cap] is the marker of the special slot (1 = EMPTY_KEY present)
-    u64 *accs;    // [cap + 4]: combiner per slot (reduce ops); unused by the dictionary
-    u32 log_cap;  // cap = 1 << log_cap slots = cap / 4 buckets; log_cap >= 2
-    u32 keep_l2;  // 1: bucket probes ask L2 to evict the table last (set by the host when the table fits L2)
+    u64 *keys;      // [cap + 4]: keys[cap] is the marker of the special slot (1 = EMPTY_KEY present)
+    u64 *accs;      // [cap + 4]: combiner per slot (reduce ops); unused by the dictionary
+    u32 log_cap;    // cap = 1 << log_cap slots = cap / 4 buckets; log_cap >= 2
+    u32 keep_l2;    // 1: bucket probes ask L2 to evict the table last (set by the host when the table fits L2)
+    u32 max_probe;  // probe rounds an insert may take before it raises the abort flag (chain_limit, set by the host)
 };
 constexpr u64 EMPTY_KEY = ~0ull;
 constexpr u32 BUCKET = 4;
+constexpr u32 HA_MAX_PROBE = 256;   // buckets
+
+// Probe-round limit of the inserts into a table.  A round either moves on to the next bucket or, after a CAS lost to a
+// concurrent insert, re-reads the same bucket.  A table that can grow gives up after HA_MAX_PROBE rounds, and the host
+// rebuilds it larger.  A table that cannot grow is one the host sized to at least twice the keys that can enter it, and
+// its inserts have no round limit: at load <= 0.5 fewer than nb / 2 buckets are full, so a walk passes fewer than nb / 2
+// full buckets, and every lost CAS is a slot another key took, of which there are fewer than 2 nb.  So every insert ends
+// within 2.5 nb < 2^32 rounds, however many keys share a home bucket and however the inserts interleave (crafted keys
+// cost time in the chain length, never a failure).
+VB_HD u32 chain_limit(bool can_grow) { return can_grow ? HA_MAX_PROBE : ~0u; }
 VB_HD size_t table_bytes(u32 log_cap) { return (((size_t)1 << log_cap) + BUCKET) * 16; }
 VB_HD Table table_at(void *base, u32 log_cap)
 {
@@ -39,6 +50,7 @@ VB_HD Table table_at(void *base, u32 log_cap)
     t.accs = (u64 *)base + (((size_t)1 << log_cap) + BUCKET);
     t.log_cap = log_cap;
     t.keep_l2 = 0;
+    t.max_probe = HA_MAX_PROBE;
     return t;
 }
 
@@ -101,7 +113,6 @@ VB_D int bucket_find(const Bucket4 &b, u64 key)
 constexpr int HA_THREADS = 256;
 constexpr int HA_ROWS = 4;
 constexpr int HA_TILE = HA_THREADS * HA_ROWS;
-constexpr u32 HA_MAX_PROBE = 256;   // buckets
 
 VB_D u64 home_bucket(u64 key, u32 log_cap) { return slot_hash(key) >> (64 - (log_cap - 2)); }
 
@@ -114,7 +125,7 @@ VB_D bool table_resolve_with(const Table &t, u64 b, Bucket4 bk, u64 key, u32 &in
 {
     const u64 nb_mask = (1ull << (t.log_cap - 2)) - 1;
 #pragma unroll 1
-    for (u32 probe = 0; probe < HA_MAX_PROBE; ++probe) {
+    for (u32 probe = 0; probe < t.max_probe; ++probe) {
         int hit = bucket_find(bk, key);
         if (hit < 0) {
             const int e = bucket_find(bk, EMPTY_KEY);
@@ -228,7 +239,7 @@ VB_D void ha_process_rows(const Table &t, TableCtl *ctl, u64 (&k)[ROWS], u64 (&v
 }
 
 // Lockstep probe/insert of the pending rows (ok[j]) of one thread, with hashes h[j]; on_hit(slot, j) once per
-// resolved row.  A probe chain longer than HA_MAX_PROBE buckets raises the table's abort flag.
+// resolved row.  A row still pending after t.max_probe probe rounds raises the table's abort flag.
 template <int ROWS, class OnHit>
 VB_D void ha_probe_rows(const Table &t, TableCtl *ctl, const u64 (&k)[ROWS], bool (&ok)[ROWS], const u64 (&h)[ROWS], u32 &my_inserts,
                         OnHit &&on_hit)
@@ -247,7 +258,7 @@ VB_D void ha_probe_rows(const Table &t, TableCtl *ctl, const u64 (&k)[ROWS], boo
     }
     bool pending = true;
 #pragma unroll 1
-    for (u32 probe = 0; pending && probe < HA_MAX_PROBE; ++probe) {
+    for (u32 probe = 0; pending && probe < t.max_probe; ++probe) {
         pending = false;
 #pragma unroll
         for (int j = 0; j < ROWS; ++j) {
@@ -277,7 +288,7 @@ VB_D void ha_probe_rows(const Table &t, TableCtl *ctl, const u64 (&k)[ROWS], boo
                 if (ok[j]) bk[j] = ld_bucket(t, bidx[j]);
         }
     }
-    if (pending) atomicExch(&ctl->abort, 1u);   // probe chain longer than HA_MAX_PROBE buckets
+    if (pending) atomicExch(&ctl->abort, 1u);   // a row took more than t.max_probe probe rounds
 }
 
 // One pass over n rows.  IN_AOS: a = rows (16 B each).  IN_SOA: a = keys, b = vals (b may be
@@ -914,13 +925,14 @@ __global__ void sample_keys_kernel(const u64 *__restrict__ a, u64 n, u64 stride,
     out[j] = (IN == IN_AOS) ? a[2 * i] : a[i];
 }
 
-// Read-only lookup used by the join: slot index of `key`, or 0xFFFFFFFF.
+// Read-only lookup used by the join: slot index of `key`, or 0xFFFFFFFF.  Slots never go back to EMPTY_KEY, so the
+// first bucket with an empty slot ends the key's chain; a chain can run up to half the table (chain_limit).
 VB_D u32 table_find(const Table &t, u64 key)
 {
     const u64 cap = 1ull << t.log_cap, nb_mask = (cap >> 2) - 1;
     if (key == EMPTY_KEY) return t.keys[cap] == 1ull ? (u32)cap : 0xFFFFFFFFu;
     u64 b = home_bucket(key, t.log_cap);
-    for (u32 probe = 0; probe <= HA_MAX_PROBE; ++probe) {
+    for (u64 probe = 0; probe <= nb_mask; ++probe) {
         const Bucket4 bk = ld_bucket(t, b);
         const int hit = bucket_find(bk, key);
         if (hit >= 0) return (u32)(4 * b + hit);
@@ -1600,7 +1612,7 @@ __global__ void translate_ids_kernel(u32 *__restrict__ ids, u64 n, const u32 *__
 // Key dictionary of n keys known to be distinct (a reduce result taken as a cogroup side), one thread per key: insert key i
 // into the table (keys[] pre-set to EMPTY_KEY, keys[cap..cap+4) to 0), dense_of_slot[its slot] = i, and offs[i] = i (one
 // value per key), offs[n] = n.  A key equal to EMPTY_KEY takes the special slot cap.  A probe chain longer than
-// HA_MAX_PROBE buckets raises ctl->abort and the host rebuilds the table larger.
+// t.max_probe probe rounds raises ctl->abort and the host rebuilds the table larger.
 __global__ void narrow_dict_kernel(const u64 *__restrict__ keys, u64 n, Table t, u32 *__restrict__ dense_of_slot,
                                    u64 *__restrict__ offs, TableCtl *ctl)
 {
