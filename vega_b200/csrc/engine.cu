@@ -4862,6 +4862,16 @@ static int str_check_offsets(vb_shuf *s, const u64 *offs, u64 n, u64 n_bytes, in
 // Entry ids of n keys (key i is bytes[offs[i] - first .. offs[i + 1] - first), n_bytes in all) in the shuffle's
 // dictionary, creating the entries of new keys.  A missing index is first sized from (guess, hint); when it fills,
 // it grows and the whole call reruns.
+//
+// Growth rule.  Load: an index holds at most 0.6 of its slots (max_entries), and a call that would pass that grows it
+// at least 4x.  Chains: a probe gives up after STR_MAX_PROBE buckets.  Keys that share their full hash share their home
+// bucket at every index size, so growth cannot shorten their chain, and keys can be crafted so (MetroHash64_1 is not
+// seeded: placement must equal the reference's HashPartitioner).  So a chain abort grows the index at most once per
+// call, and only while it holds fewer than twice the call's worst-case key count (entries before the call plus its
+// rows); then the call reruns with the probe limit lifted to the bucket count, for the rest of the call.  The load
+// bound leaves an empty slot, so every lifted probe ends within the bucket count; equal-hash keys cost their chain's
+// length in byte compares, never a failure.  Random keys practically never chain past STR_MAX_PROBE buckets at load
+// <= 0.6, so their index sizes are those of the load rule alone.
 static int str_encode(vb_shuf *s, const u64 *offs, const unsigned char *bytes, u64 first, u64 n, u64 n_bytes, u64 guess, u64 hint,
                       u32 *ids)
 {
@@ -4875,17 +4885,22 @@ static int str_encode(vb_shuf *s, const u64 *offs, const unsigned char *bytes, u
         t->ctl = (StrCtl *)ctl.release();
     }
     if (!t->d.fp) TRY(str_index_build(s, choose_log_cap(guess, hint, false, STR_MAX_LOG_CAP, c->l2_bytes, 12)));
+    const u64 worst = (u64)t->n_e + n;         // keys the dictionary can hold after this call
+    bool lifted = (1ull << t->d.log_cap) >= 2 * worst;
     for (;;) {
-        const u64 cap = 1ull << t->d.log_cap;
+        const u64 cap = 1ull << t->d.log_cap, nb = cap / BUCKET;
         const u32 max_entries = (u32)std::min<u64>((cap / 10) * 6, 0xFFFFFFFFull);
+        const u32 max_probe = (u32)(lifted || nb < STR_MAX_PROBE ? nb : STR_MAX_PROBE);
         CU(cudaMemsetAsync(&t->ctl->abort, 0, 4, c->stream));
         {
             KLaunch kl(s, K_DICT, n);
             const u64 blocks = std::min<u64>((n + 255) / 256, (u64)c->sm_count * 8);
             if (t->kind == STRKEY_BYTES)
-                str_encode_kernel<STRKEY_BYTES><<<(unsigned)blocks, 256, 0, c->stream>>>(offs, bytes, first, n, t->d, t->ctl, max_entries, ids);
+                str_encode_kernel<STRKEY_BYTES><<<(unsigned)blocks, 256, 0, c->stream>>>(offs, bytes, first, n, t->d, t->ctl, max_entries,
+                                                                                         max_probe, ids);
             else
-                str_encode_kernel<STRKEY_STR><<<(unsigned)blocks, 256, 0, c->stream>>>(offs, bytes, first, n, t->d, t->ctl, max_entries, ids);
+                str_encode_kernel<STRKEY_STR><<<(unsigned)blocks, 256, 0, c->stream>>>(offs, bytes, first, n, t->d, t->ctl, max_entries,
+                                                                                       max_probe, ids);
             TRY(kl.done("str_encode_kernel"));
         }
         StrCtl h;
@@ -4893,8 +4908,12 @@ static int str_encode(vb_shuf *s, const u64 *offs, const unsigned char *bytes, u
         t->n_e = h.n_entries;
         t->n_a = h.n_arena;
         if (!h.abort) return VB_OK;
-        s->st.table_restarts++;                // grow the index (at least 4x) and rerun the whole call
-        TRY(str_index_build(s, std::max<u32>(t->d.log_cap + 2, ceil_log2_u64(3 * (u64)t->n_e))));
+        s->st.table_restarts++;                // rerun the whole call, in a larger index or with the limit lifted
+        // Below max_entries the abort was a chain of max_probe full buckets; a walk of every bucket fails only when the
+        // index is full, which the count then shows.
+        const bool chain = h.n_entries < max_entries;
+        if (chain) lifted = true;
+        if (!chain || cap < 2 * worst) TRY(str_index_build(s, std::max<u32>(t->d.log_cap + 2, ceil_log2_u64(3 * (u64)t->n_e))));
     }
 }
 

@@ -111,7 +111,7 @@ VB_HD u64 metro64_1_str(const unsigned char *p, u64 len) { return metro64_1_key<
 VB_HD u64 metro64_1_bytes(const unsigned char *p, u64 len) { return metro64_1_key<STRKEY_BYTES>(p, len); }
 
 constexpr u32 STR_UNPUBLISHED = 0xFFFFFFFFu;   // index slot claimed, entry id not written yet (or slot empty)
-constexpr u32 STR_MAX_PROBE = 64;              // buckets probed before a call gives up and the index grows
+constexpr u32 STR_MAX_PROBE = 64;              // buckets probed before a call gives up (str_encode: grow or lift)
 
 struct StrDict {
     u64 *fp;                  // [cap] index fingerprints: 0 = empty slot
@@ -125,7 +125,7 @@ struct StrDict {
 };
 
 struct StrCtl {
-    u32 abort;                     // the index is too full or a probe ran too long: the host grows it and reruns the call
+    u32 abort;                     // the index is too full or a probe ran too long: the host grows it or lifts the probe limit, and reruns the call
     u32 n_entries;                 // entries in use (persistent across calls)
     unsigned long long n_arena;    // arena bytes in use (persistent across calls)
 };
@@ -158,16 +158,19 @@ VB_D bool str_equal(const unsigned char *key, const unsigned char *stored, u64 l
 // One thread per row: hash the key, find or create its dictionary entry, write the entry id.  Key i is
 // bytes[offs[i] - base .. offs[i + 1] - base).  Entries and arena are reserved by the host for the worst case of the
 // call, so only the index can overflow; that is decided BEFORE a slot is claimed (load or probe length), so a claimed
-// slot is always published and no thread waits on one forever.  An aborted call is rerun whole after the index grows:
-// rows already encoded find the same entries again.  KIND: the shuffle's key hash (STRKEY_*).  The byte-slice hash
-// asks ptxas for 4 blocks per SM: left to its default it holds 40 registers and spills the row index (8 bytes); the
-// String instantiation keeps the bare bound (0: none), and with it the code it always had.
+// slot is always published and no thread waits on one forever.  An aborted call is rerun whole after the index grows
+// or the probe limit is lifted: rows already encoded find the same entries again.  max_probe (<= the bucket count, set
+// by str_encode): buckets a probe walks before it gives up.  A walk of every bucket that finds neither the key nor an
+// empty slot means the index is full, so the host, which sees n_entries >= max_entries, grows it for load.  KIND: the
+// shuffle's key hash (STRKEY_*).  The byte-slice hash asks ptxas for 4 blocks per SM: left to its default it holds 40
+// registers and spills the row index (8 bytes); the String instantiation keeps the bare bound (0: none), and with it
+// the code it always had.
 template <int KIND>
 __global__ void __launch_bounds__(256, KIND == STRKEY_BYTES ? 4 : 0) str_encode_kernel(const u64 *__restrict__ offs, const unsigned char *__restrict__ bytes, u64 base,
-                                                         u64 n, StrDict d, StrCtl *ctl, u32 max_entries, u32 *__restrict__ ids_out)
+                                                         u64 n, StrDict d, StrCtl *ctl, u32 max_entries, u32 max_probe,
+                                                         u32 *__restrict__ ids_out)
 {
     const u64 nb = 1ull << (d.log_cap - 2);
-    const u32 max_probe = nb < STR_MAX_PROBE ? (u32)nb : STR_MAX_PROBE;
     const u64 stride = (u64)gridDim.x * blockDim.x;
     for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
         if (ld_volatile_u32(&ctl->abort)) return;
