@@ -24,6 +24,8 @@
  *   vb_join_n_outer*       <- nothing: vega has no outer joins (N-way, over the same cogroup, new)
  *   vb_cogroup_n_str* / vb_join_n_str*
  *                          <- the same two over `String` keys (keys matched by their bytes; join keys once per key)
+ *   vb_semi_join_n*        <- nothing: vega has no semi or anti join (subtractByKey, left semi join; the rule is
+ *                             restated over CoGroupedRdd::compute, src/rdd/co_grouped_rdd.rs:206-249, new)
  *   vb_shuffle_free        <- (the reference never evicts SHUFFLE_CACHE, src/env.rs:27)
  *   vb_slice               <- ParallelCollection::slice           src/rdd/parallel_collection_rdd.rs:116-145
  *   vb_shuffle_export_* / vb_shuffle_import
@@ -464,6 +466,27 @@ VB_API int32_t vb_join_n_outer(vb_shuf *const *sides, uint32_t n_sides, uint32_t
                                void *out_k, void *const *out_vals /*[n_sides]*/,
                                uint8_t *const *out_valid /*[n_sides] or NULL; entries may be NULL*/, int32_t dst_loc);
 
+/* Semi and anti join of side 0 by the other sides, for one partition.  vega has no such op (Spark's subtractByKey and
+ * left semi join); the rule is restated over CoGroupedRdd::compute, src/rdd/co_grouped_rdd.rs:206-249, so there is no
+ * reference output to compare against.  `required` and `excluded` are masks over sides 1 .. n_sides-1.  A key of the
+ * partition, with cogroup lists l_0 .. l_{n-1}, is kept when l_0 is non-empty, every side of `required` has it and no
+ * side of `excluded` has it; a kept key gives the rows (k, v) for v in l_0, contiguous and in l_0's order (map-id order,
+ * or ascending under vb_shuffle_set_value_order).  The order of keys within the partition is unspecified.
+ *   subtract_by_key(a, b) = {a, b} with excluded = 0b10;  semi_join(a, b) = {a, b} with required = 0b10;
+ *   both masks 0 gives side 0's rows as vb_shuffle_reduce gives them.
+ * Only side 0's values are read or moved: the other sides' value dtypes are free.  out_v has side 0's value dtype
+ * (VB_BYTES: references that vb_shuffle_gather_bytes of side 0 resolves).  Sides: those vb_cogroup_n takes.  A lazy
+ * COGROUP filter side gives its rows' keys and is not grouped; a lazy side 0 has only its kept rows grouped.  The
+ * filter (one presence dictionary of the filter sides' keys) is built once per (sides, masks) and kept on sides[0].
+ * Argument rules: vb_cogroup_n's; and VB_ERR_INVALID, before any device work and with every side staying usable, for a
+ * mask bit at n_sides or above, bit 0 in either mask, a side in both masks, or (once the partition has rows) a NULL
+ * out_k or out_v.  The size call keeps the partition's plan on sides[0] for the write call, as vb_join_n_size does.  On
+ * a rank of a multi-rank shuffle only the partitions that rank owns have rows.                                      */
+VB_API int32_t vb_semi_join_n_size(vb_shuf *const *sides, uint32_t n_sides, uint32_t reduce_id, uint32_t required,
+                                   uint32_t excluded, uint64_t *n_rows);
+VB_API int32_t vb_semi_join_n(vb_shuf *const *sides, uint32_t n_sides, uint32_t reduce_id, uint32_t required,
+                              uint32_t excluded, void *out_k, void *out_v, int32_t dst_loc);
+
 /* ---- string keys: byte-string keys that hash like Rust `String` (reduce_by_key / count_by_key / count_by_value /
  *      distinct / group_by_key / partition_by_key over `String` keys, examples/group_by.rs, tests/test_pair_rdd.rs:8-37)
  * Key i of a map partition is key_bytes[key_offsets[i] .. key_offsets[i+1]) (Arrow-style: key_offsets has n_rows + 1
@@ -553,6 +576,18 @@ VB_API int32_t vb_join_n_str(vb_shuf *const *sides, uint32_t n_sides, uint32_t r
                              uint64_t *out_key_offsets /*n_keys+1*/, void *out_key_bytes,
                              uint64_t *out_row_offsets /*n_keys+1*/, void *const *out_vals /*[n_sides] of n_rows*/,
                              uint8_t *const *out_valid /*[n_sides] or NULL; entries may be NULL*/, int32_t dst_loc);
+/* vb_semi_join_n over string GROUP shuffles and vb_shuffle_create_narrow_str views, all of one key kind (the same rule,
+ * restated over CoGroupedRdd::compute, src/rdd/co_grouped_rdd.rs:206-249; vega has no such op).  Side 0's keys of the
+ * partition are looked up in each filter side's key index by their hash, then their bytes, so keys that share a hash
+ * stay apart.  The output is vb_join_n_str's with one value column: each kept key once (out_key_offsets [n_keys + 1],
+ * out_key_bytes), out_row_offsets [n_keys + 1] its rows, out_vals [n_rows] side 0's values.  Argument rules:
+ * vb_join_n_str's and vb_semi_join_n's masks; once the partition has rows out_key_offsets, out_row_offsets, out_vals
+ * and (with key bytes) out_key_bytes must be non-NULL.                                                               */
+VB_API int32_t vb_semi_join_n_str_size(vb_shuf *const *sides, uint32_t n_sides, uint32_t reduce_id, uint32_t required,
+                                       uint32_t excluded, uint64_t *n_rows, uint64_t *n_keys, uint64_t *n_key_bytes);
+VB_API int32_t vb_semi_join_n_str(vb_shuf *const *sides, uint32_t n_sides, uint32_t reduce_id, uint32_t required,
+                                  uint32_t excluded, uint64_t *out_key_offsets /*n_keys+1*/, void *out_key_bytes,
+                                  uint64_t *out_row_offsets /*n_keys+1*/, void *out_vals /*n_rows*/, int32_t dst_loc);
 /* A sealed string reduce-op or combine_by_key shuffle as a cogroup / join parent under the same partitioner, without a
  * shuffle: vb_shuffle_create_narrow for string keys.  *out is a new sealed string GROUP-kind shuffle: its partition r
  * holds partition r of `parent` (the keys with vb_hash_str(key) % n_reduce == r), each key once, with the one-element

@@ -185,6 +185,23 @@ inline std::vector<std::pair<K, std::vector<std::optional<V>>>> read_join_n_oute
     }
     return out;
 }
+
+// partitions [0, num_splits) of vb_semi_join_n over sealed sides  →  side 0's (k, v) rows of the kept keys
+template <typename K, typename V>
+inline std::vector<std::pair<K, V>> read_semi_join_n(std::vector<vb_shuf *> sides, size_t num_splits, uint32_t required,
+                                                    uint32_t excluded)
+{
+    const uint32_t n = (uint32_t)sides.size();
+    std::vector<std::pair<K, V>> out;
+    for (uint32_t r = 0; r < num_splits; ++r) {
+        uint64_t rows = 0;
+        check(vb_semi_join_n_size(sides.data(), n, r, required, excluded, &rows));
+        std::vector<uint64_t> k(rows), v(rows);
+        check(vb_semi_join_n(sides.data(), n, r, required, excluded, k.data(), v.data(), VB_HOST));
+        for (uint64_t i = 0; i < rows; ++i) out.emplace_back(detail::from_bits<K>(k[i]), detail::from_bits<V>(v[i]));
+    }
+    return out;
+}
 }  // namespace detail
 
 template <typename K, typename V>
@@ -404,6 +421,28 @@ public:
         std::vector<vb_shuf *> sides;
         for (auto &s : shs) sides.push_back(s.get());
         return detail::read_join_n_outer<K, V>(sides, num_splits, required);
+    }
+
+    // semi / anti join of this parent by [others...] (vega has none): bit j of `required` / `excluded` marks parent j
+    // (1 .. n-1; this one is 0) as a parent that must / must not have the key.  A kept key gives its (k, v) rows of this
+    // parent, contiguous and in list order.  The other parents' values are never read and their lazy rows never grouped.
+    std::vector<std::pair<K, V>> semi_join_n(const std::vector<PairRddT> &others, size_t num_splits, uint32_t required,
+                                             uint32_t excluded, bool sorted_values = false) const
+    {
+        auto shs = cogroup_shuffles(others, num_splits, sorted_values);
+        std::vector<vb_shuf *> sides;
+        for (auto &s : shs) sides.push_back(s.get());
+        return detail::read_semi_join_n<K, V>(sides, num_splits, required, excluded);
+    }
+    // Spark's subtractByKey: this parent's rows whose key `other` lacks
+    std::vector<std::pair<K, V>> subtract_by_key(const PairRddT &other, size_t num_splits, bool sorted_values = false) const
+    {
+        return semi_join_n({other}, num_splits, 0, 0b10, sorted_values);
+    }
+    // left semi join: this parent's rows whose key `other` has, each once
+    std::vector<std::pair<K, V>> semi_join(const PairRddT &other, size_t num_splits, bool sorted_values = false) const
+    {
+        return semi_join_n({other}, num_splits, 0b10, 0, sorted_values);
     }
 
     std::shared_ptr<Context> sc_;
@@ -708,6 +747,27 @@ inline std::vector<std::pair<std::string, std::vector<std::optional<V>>>> read_s
     }
     return out;
 }
+
+// vb_semi_join_n_str over sealed string GROUP sides, partition by partition: side 0's (k, v) rows of the kept keys
+template <typename V>
+inline std::vector<std::pair<std::string, V>> read_str_semi_join_n(const std::vector<vb_shuf *> &sides, size_t num_splits,
+                                                                   uint32_t required, uint32_t excluded)
+{
+    const uint32_t n = (uint32_t)sides.size();
+    std::vector<std::pair<std::string, V>> out;
+    for (uint32_t r = 0; r < num_splits; ++r) {
+        uint64_t rows = 0, nk = 0, nb = 0;
+        check(vb_semi_join_n_str_size(sides.data(), n, r, required, excluded, &rows, &nk, &nb));
+        std::vector<uint64_t> ko(nk + 1), ro(nk + 1), v(rows);
+        std::string kb(nb, '\0');
+        check(vb_semi_join_n_str(sides.data(), n, r, required, excluded, ko.data(), kb.data(), ro.data(), v.data(), VB_HOST));
+        for (uint64_t i = 0; i < nk; ++i) {
+            const std::string k(kb, ko[i], ko[i + 1] - ko[i]);
+            for (uint64_t x = ro[i]; x < ro[i + 1]; ++x) out.emplace_back(k, from_bits<V>(v[x]));
+        }
+    }
+    return out;
+}
 }  // namespace detail
 
 template <typename V>
@@ -838,6 +898,22 @@ public:
     {
         auto shs = group_shuffles(others, num_splits, sorted_values);
         return detail::read_str_join_n_outer<V>(raw(shs), num_splits, required);
+    }
+
+    // PairRddT::semi_join_n over String keys (vb_semi_join_n_str), keys matched by their bytes
+    std::vector<std::pair<std::string, V>> semi_join_n(const std::vector<StrPairRddT> &others, size_t num_splits, uint32_t required,
+                                                       uint32_t excluded, bool sorted_values = false) const
+    {
+        auto shs = group_shuffles(others, num_splits, sorted_values);
+        return detail::read_str_semi_join_n<V>(raw(shs), num_splits, required, excluded);
+    }
+    std::vector<std::pair<std::string, V>> subtract_by_key(const StrPairRddT &other, size_t num_splits, bool sorted_values = false) const
+    {
+        return semi_join_n({other}, num_splits, 0, 0b10, sorted_values);
+    }
+    std::vector<std::pair<std::string, V>> semi_join(const StrPairRddT &other, size_t num_splits, bool sorted_values = false) const
+    {
+        return semi_join_n({other}, num_splits, 0b10, 0, sorted_values);
     }
 
     // inner join of [self, others...]  →  (k, [v_0, ..., v_{n-1}]) per row

@@ -67,6 +67,12 @@ extern "C" {
                                 n_out: *mut u64) -> i32;
     pub fn vb_join_n_outer(sides: *const *mut vb_shuf, n_sides: u32, reduce_id: u32, required: u32, out_k: *mut c_void,
                            out_vals: *const *mut c_void, out_valid: *const *mut u8, dst_loc: i32) -> i32;
+    // semi / anti join of side 0 (subtractByKey, left semi join; vega has none): a side-0 key is kept when every side of
+    // `required` has it and no side of `excluded` does (masks over sides 1..n-1), and gives its side-0 rows
+    pub fn vb_semi_join_n_size(sides: *const *mut vb_shuf, n_sides: u32, reduce_id: u32, required: u32, excluded: u32,
+                               n_rows: *mut u64) -> i32;
+    pub fn vb_semi_join_n(sides: *const *mut vb_shuf, n_sides: u32, reduce_id: u32, required: u32, excluded: u32,
+                          out_k: *mut c_void, out_v: *mut c_void, dst_loc: i32) -> i32;
     // N1: bincode blobs (the payload format of SHUFFLE_CACHE)
     pub fn vb_shuffle_reduce_blob_size(s: *mut vb_shuf, reduce_id: u32, n_bytes: *mut u64) -> i32;
     pub fn vb_shuffle_reduce_blob(s: *mut vb_shuf, reduce_id: u32, out_blob: *mut c_void, dst_loc: i32) -> i32;
@@ -128,6 +134,11 @@ extern "C" {
     pub fn vb_join_n_str(sides: *const *mut vb_shuf, n_sides: u32, reduce_id: u32, required: u32, out_key_offsets: *mut u64,
                          out_key_bytes: *mut c_void, out_row_offsets: *mut u64, out_vals: *const *mut c_void,
                          out_valid: *const *mut u8, dst_loc: i32) -> i32;
+    pub fn vb_semi_join_n_str_size(sides: *const *mut vb_shuf, n_sides: u32, reduce_id: u32, required: u32, excluded: u32,
+                                   n_rows: *mut u64, n_keys: *mut u64, n_key_bytes: *mut u64) -> i32;
+    pub fn vb_semi_join_n_str(sides: *const *mut vb_shuf, n_sides: u32, reduce_id: u32, required: u32, excluded: u32,
+                              out_key_offsets: *mut u64, out_key_bytes: *mut c_void, out_row_offsets: *mut u64,
+                              out_vals: *mut c_void, dst_loc: i32) -> i32;
     // String keys across ranks: export packs by destination rank as four columns (u32 key lengths, key bytes, u32 value
     // counts for GROUP, u64 values), import takes them source-rank major (borrowed until seal)
     pub fn vb_shuffle_create_str_dist(ctx: *mut vb_ctx, shuffle_id: u64, n_map: u32, n_reduce: u32, val_dtype: i32, agg: i32,

@@ -6,9 +6,9 @@ interface for the path (rdd.py) plus the one-process-per-GPU exchange (dist.py).
 Importing works without a GPU (so the C ABI can be inspected); computing does not.
 """
 from ._lib import (LIB_PATH, SYMBOLS, VegaB200Error, lib)  # noqa: F401
-from .rdd import (AggregateRdd, CoGroupedRdd, CombinedRdd, Context, Grouped, JoinedRdd, PairRdd, Rdd, RepartitionedRdd, RepShuffle,  # noqa: F401
+from .rdd import (AggregateRdd, CoGroupedRdd, CombinedRdd, Context, Grouped, JoinedRdd, PairRdd, Rdd, RepartitionedRdd, RepShuffle, SemiJoinedRdd,  # noqa: F401
                   Shuffle, ShuffledRdd,
                   BytesKeys, StrAggregateRdd, StrCoGroupedRdd, StrCombinedRdd, StrKeys, StrPairRdd, StrRdd, StrShuffle, StrShuffledRdd, StrSortedRdd, slice_starts)
 
-__all__ = ["Context", "PairRdd", "CoGroupedRdd", "CombinedRdd", "AggregateRdd", "Rdd", "RepartitionedRdd", "RepShuffle", "Shuffle", "ShuffledRdd", "JoinedRdd", "Grouped", "slice_starts",
+__all__ = ["Context", "PairRdd", "CoGroupedRdd", "CombinedRdd", "AggregateRdd", "Rdd", "RepartitionedRdd", "RepShuffle", "SemiJoinedRdd", "Shuffle", "ShuffledRdd", "JoinedRdd", "Grouped", "slice_starts",
            "BytesKeys", "StrAggregateRdd", "StrCoGroupedRdd", "StrCombinedRdd", "StrKeys", "StrPairRdd", "StrRdd", "StrShuffle", "StrShuffledRdd", "StrSortedRdd", "VegaB200Error", "lib", "LIB_PATH", "SYMBOLS"]

@@ -113,6 +113,8 @@ SYMBOLS = {
     "vb_join_n": (_i32, [_pvp, _u32, _u32, _vp, _pvp, _i32]),
     "vb_join_n_outer_size": (_i32, [_pvp, _u32, _u32, _u32, _pu64]),
     "vb_join_n_outer": (_i32, [_pvp, _u32, _u32, _u32, _vp, _pvp, _pvp, _i32]),
+    "vb_semi_join_n_size": (_i32, [_pvp, _u32, _u32, _u32, _u32, _pu64]),
+    "vb_semi_join_n": (_i32, [_pvp, _u32, _u32, _u32, _u32, _vp, _vp, _i32]),
     "vb_shuffle_create_str": (_i32, [_vp, _u64, _u32, _u32, _i32, _i32, _pvp]),
     "vb_shuffle_map_str": (_i32, [_vp, _u32, _vp, _vp, _u64, _vp, _u64, _i32]),
     "vb_shuffle_reduce_str_size": (_i32, [_vp, _u32, _pu64, _pu64, _pu64]),
@@ -121,6 +123,8 @@ SYMBOLS = {
     "vb_cogroup_n_str": (_i32, [_pvp, _u32, _u32, _vp, _vp, _pvp, _pvp, _i32]),
     "vb_join_n_str_size": (_i32, [_pvp, _u32, _u32, _u32, _pu64, _pu64, _pu64]),
     "vb_join_n_str": (_i32, [_pvp, _u32, _u32, _u32, _vp, _vp, _vp, _pvp, _pvp, _i32]),
+    "vb_semi_join_n_str_size": (_i32, [_pvp, _u32, _u32, _u32, _u32, _pu64, _pu64, _pu64]),
+    "vb_semi_join_n_str": (_i32, [_pvp, _u32, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _i32]),
     "vb_shuffle_create_str_dist": (_i32, [_vp, _u64, _u32, _u32, _i32, _i32, _u32, _u32, _pvp]),
     "vb_shuffle_export_str_prepare": (_i32, [_vp, _pu64, _pu64, _pu64]),
     "vb_shuffle_export_str_buffers": (_i32, [_vp, _pvp, _pvp, _pvp, _pvp]),

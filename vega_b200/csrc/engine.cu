@@ -22,6 +22,7 @@
 #include "strkeys.cuh"
 #include "bytevals.cuh"
 #include "segsort.cuh"
+#include "semijoin.cuh"
 #include <type_traits>
 
 using namespace vb;
@@ -304,8 +305,18 @@ struct CogroupNPlan {
     u64 *str_koff = nullptr;       // [str_nk + 1] key byte offsets from 0
     u64 *str_roff = nullptr;       // join: [str_nk + 1] each key's first row, then the total
 };
-// n_plans kinds: the cogroup, the inner join, or (>= 0) an outer join by its mask of required sides
-constexpr i64 NP_COGROUP = -2, NP_INNER = -1;
+// n_plans kinds: the cogroup, the inner join, (>= 0) an outer join by its mask of required sides, or (<= NP_SEMI) a
+// semi join by its two masks (semi_kind)
+constexpr i64 NP_COGROUP = -2, NP_INNER = -1, NP_SEMI = -3;
+
+// vb_semi_join_n's filter for one (sides, required, excluded), built by the first call and kept on side 0 until
+// vb_shuffle_free: the presence dictionary of the filter sides' keys, or, when side 0 was lazy, its kept rows grouped
+struct SemiFilter {
+    void *tab = nullptr;           // presence dictionary (NULL: the filter sides have no keys)
+    u32 log_cap = 0;
+    u32 *mask = nullptr;           // [slots] bit j: side j has the slot's key
+    struct vb_shuf *kept = nullptr;   // side 0 lazy: an internal GROUP-like shuffle of its kept rows (tab, mask freed)
+};
 
 struct vb_shuf {
     vb_ctx *ctx = nullptr;
@@ -369,6 +380,8 @@ struct vb_shuf {
     std::map<std::tuple<u64, u32, int>, JoinPlan> join_plans;   // by (right side's uid, partition, outer kind)
     // on side 0 of a cogroup or a join, of two sides or N: by (every side's uid, partition, NP_* kind or outer mask)
     std::map<std::tuple<std::vector<u64>, u32, i64>, CogroupNPlan> n_plans;
+    // on side 0 of a semi join: by (every side's uid, required, excluded)
+    std::map<std::tuple<std::vector<u64>, u32, u32>, SemiFilter> semi;
     // COGROUP shuffles are grouped lazily: seal keeps the (owned) rows; the CSR is built by the first reduce call
     // (cogroup materialisation), or — if a join comes first — only for the rows the join kind needs: the keys on BOTH
     // sides (inner), every row of the preserved side plus the matching rows of the other (LEFT / RIGHT), or all (FULL).
@@ -4485,6 +4498,253 @@ extern "C" int32_t vb_join_n_outer(vb_shuf *const *sides, uint32_t n_sides, uint
     return join_n_outer_write(sides, n_sides, rid, required, out_k, out_vals, out_valid, dst_loc);
 }
 
+// ---------------------------------------------------------------------------------------------
+// semi and anti joins of n sides.  vega has no such op; this restates it over CoGroupedRdd::compute
+// (co_grouped_rdd.rs:206-249): a key of side 0's partition r is kept when its side-0 list is non-empty, every side of
+// `required` has it and no side of `excluded` does, and then gives the rows (k, v) for v in its side-0 list.  Only side
+// 0's values are read.  The keys of the filter sides (required | excluded, a shuffle listed twice counted once) go into
+// one presence dictionary with a side mask per slot; a lazy filter side gives its rows' keys and is never grouped.  A
+// lazy side 0 is filtered row by row and only its kept rows are grouped; a grouped side 0 (GROUP, grouped COGROUP,
+// narrow view) is probed once per key of the partition.  Either way the partition is a one-side join plan over a
+// grouped source, written by join_n_expand_kernel.  Cost: linear in side 0's rows (or keys) and the filter sides' keys.
+// ---------------------------------------------------------------------------------------------
+static i64 semi_kind(u32 required, u32 excluded) { return NP_SEMI - (i64)(((u64)excluded << 16) | required); }
+
+// the mask rules of vb_semi_join_n*, after the cogroup rules (so n_sides <= 16)
+static int semi_masks_check(u32 n, u32 required, u32 excluded)
+{
+    if ((required | excluded) >> n)
+        return set_err(VB_ERR_INVALID, "mask %#x names a side >= n_sides %u", (required | excluded), n);
+    if ((required | excluded) & 1u) return set_err(VB_ERR_INVALID, "side 0 cannot be required or excluded: it is the side filtered");
+    if (required & excluded) return set_err(VB_ERR_INVALID, "sides %#x are both required and excluded", required & excluded);
+    return VB_OK;
+}
+
+static void semi_count_launches(vb_shuf *s0, const vb_shuf *t)
+{
+    for (int k = 0; k < K_N; ++k) s0->klaunch[k] += t->klaunch[k];
+    s0->st.kernel_launches += t->st.kernel_launches;
+    s0->st.table_slots = std::max(s0->st.table_slots, t->st.table_slots);
+}
+
+// The filter of (sides, required, excluded), built once and kept on side 0; the context is locked
+static int semi_filter(vb_shuf *const *sides, u32 n, u32 required, u32 excluded, SemiFilter **out)
+{
+    vb_shuf *s0 = sides[0];
+    vb_ctx *c = s0->ctx;
+    std::vector<u64> uids(n);
+    for (u32 j = 0; j < n; ++j) uids[j] = sides[j]->uid;
+    const auto key = std::make_tuple(uids, required, excluded);
+    auto it = s0->semi.find(key);
+    if (it != s0->semi.end()) { *out = &it->second; return VB_OK; }
+    const u32 filter = required | excluded;
+    SemiFilter f;
+    if (!filter) {                                     // no filter side: side 0's rows as its reduce gives them
+        TRY(ensure_grouped(s0));
+        *out = &s0->semi.emplace(key, f).first->second;
+        return VB_OK;
+    }
+    // 1. every filter shuffle once, with the bits of the sides it is; its keys (a lazy side's rows' keys)
+    std::vector<vb_shuf *> fs;
+    std::vector<u32> bits;
+    for (u32 j = 1; j < n; ++j) {
+        if (!(filter >> j & 1u)) continue;
+        const size_t i = std::find(fs.begin(), fs.end(), sides[j]) - fs.begin();
+        if (i == fs.size()) { fs.push_back(sides[j]); bits.push_back(0); }
+        bits[i] |= 1u << j;
+    }
+    std::vector<AggInput> in;
+    std::vector<u32> in_bits;
+    u64 total = 0;
+    for (size_t i = 0; i < fs.size(); ++i) {
+        const vb_shuf *s = fs[i];
+        const u64 m = s->lazy ? s->lz_n : s->n_keys;
+        if (!m) continue;
+        in.push_back(AggInput{IN_SOA, s->lazy ? s->lz_keys : s->res_keys, nullptr, m, VB_DEVICE});
+        in_bits.push_back(bits[i]);
+        total += m;
+    }
+    // 2. the presence dictionary: one table over all of them, then each input's bits ORed into its rows' slots
+    DevBuf tab(c), mask(c);
+    if (total) {
+        DevBuf ids(c);
+        TRY(ids.alloc(total * 4));
+        u64 n_ins = 0;
+        TRY(build_table(s0, K_DICT, in, OPK_DICT, TX_NONE, 0, &tab.p, &f.log_cap, &n_ins, ids.as<u32>()));
+        const u64 slots = (1ull << f.log_cap) + 1 + 16;
+        TRY(mask.alloc(slots * 4));
+        CU(cudaMemsetAsync(mask.p, 0, slots * 4, c->stream));
+        u64 at = 0;
+        for (size_t i = 0; i < in.size(); ++i) {
+            KLaunch kl(s0, K_JOIN, in[i].n);
+            const unsigned g = (unsigned)std::min<u64>((in[i].n + 255) / 256, (u64)c->sm_count * 16);
+            presence_mark_kernel<<<g, 256, 0, c->stream>>>(ids.as<u32>() + at, in[i].n, in_bits[i], mask.as<u32>());
+            TRY(kl.done("presence_mark_kernel"));
+            at += in[i].n;
+        }
+        s0->st.table_slots = std::max<u64>(s0->st.table_slots, 1ull << f.log_cap);
+    }
+    const Table t = table_at(tab.p, f.log_cap);
+    if (s0->lazy) {
+        // 3. a lazy side 0: keep its rows by the rule (stable), then group only those, in side 0's value order
+        Gathered g;
+        DevBuf keep(c), gk(c), gv(c);
+        if (s0->lz_n) {
+            TRY(keep.alloc(s0->lz_n));
+            {
+                KLaunch kl(s0, K_JOIN, s0->lz_n);
+                const unsigned gr = (unsigned)std::min<u64>((s0->lz_n + 255) / 256, (u64)c->sm_count * 16);
+                presence_probe_kernel<<<gr, 256, 0, c->stream>>>(s0->lz_keys, s0->lz_n, t, mask.as<u32>(), required, excluded,
+                                                                 keep.as<unsigned char>());
+                TRY(kl.done("presence_probe_kernel"));
+            }
+            TRY(compact_rows(s0, s0->lz_keys, s0->lz_vals, s0->lz_n, keep.as<unsigned char>(), gk, gv, &g.n));
+            g.keys = gk.as<u64>(); g.vals = gv.as<u64>();
+        }
+        vb_shuf *k = make_internal_like(s0);
+        k->bucket_off.assign((size_t)s0->n_reduce + 1, 0);
+        k->val_off = k->bucket_off;
+        if (g.n) {
+            const int rc = seal_group(k, g);
+            if (rc) { s0->trash.push_back(k); return rc; }   // freed with s0 (vb_shuffle_free would re-lock the context)
+        }
+        CU(cudaStreamSynchronize(c->stream));
+        semi_count_launches(s0, k);
+        f.kept = k;
+    } else {
+        CU(cudaStreamSynchronize(c->stream));
+        f.tab = tab.release();
+        f.mask = (u32 *)mask.release();
+    }
+    *out = &s0->semi.emplace(key, f).first->second;
+    return VB_OK;
+}
+
+// The plan of partition rid: the kept keys' side-0 list lengths scanned (pos, total) over a one-side match (each key's
+// own index), cached in side 0's n_plans.  *src: the grouped shuffle the plan indexes (side 0, or its kept rows).
+static int semi_plan(vb_shuf *const *sides, u32 n, u32 rid, u32 required, u32 excluded, CogroupNPlan **out, vb_shuf **src)
+{
+    vb_shuf *s0 = sides[0];
+    vb_ctx *c = s0->ctx;
+    const bool str = s0->str != nullptr;
+    SemiFilter *f = nullptr;
+    if (!str) TRY(semi_filter(sides, n, required, excluded, &f));
+    vb_shuf *g = f && f->kept ? f->kept : s0;
+    *src = g;
+    std::vector<u64> uids(n);
+    for (u32 j = 0; j < n; ++j) uids[j] = sides[j]->uid;
+    const auto key = std::make_tuple(uids, rid, semi_kind(required, excluded));
+    auto it = s0->n_plans.find(key);
+    if (it != s0->n_plans.end()) { *out = &it->second; return VB_OK; }
+    const u64 nk = g->bucket_off[rid + 1] - g->bucket_off[rid];
+    if (nk >= 0xFFFFFFFFull) return set_err(VB_ERR_TOO_LARGE, "%llu keys in one semi-join partition", (unsigned long long)nk);
+    CogroupNPlan p;
+    p.n_keys = nk;
+    if (nk) {
+        DevBuf match(c), cnt(c), pos(c);
+        TRY(match.alloc(nk * 4)); TRY(cnt.alloc(nk * 8)); TRY(pos.alloc((nk + 1) * 8));
+        const u32 kb = (u32)g->bucket_off[rid];
+        {
+            KLaunch kl(s0, K_JOIN, nk);
+            const unsigned gr = (unsigned)((nk + 255) / 256);
+            if (str) {
+                StrNSides sa;
+                TRY(str_n_sides(sides, n, rid, &sa));
+                semi_str_count_kernel<<<gr, 256, 0, c->stream>>>(sa, g->res_offs, (u32)nk, required, excluded, cnt.as<u64>(), match.as<u32>());
+                TRY(kl.done("semi_str_count_kernel"));
+            } else {
+                // the kept rows were filtered already: every key of theirs is kept
+                const bool all = f->kept != nullptr;
+                presence_count_kernel<<<gr, 256, 0, c->stream>>>(g->res_keys, g->res_offs, kb, (u32)nk, table_at(f->tab, f->log_cap),
+                                                                 f->mask, all ? 0 : required, all ? 0 : excluded, cnt.as<u64>(),
+                                                                 match.as<u32>());
+                TRY(kl.done("presence_count_kernel"));
+            }
+        }
+        TRY(exclusive_scan_u64(s0, cnt.as<u64>(), pos.as<u64>(), nk, pos.as<u64>() + nk));
+        CU(cudaMemcpyAsync(c->h_scratch, pos.as<u64>() + nk, 8, cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaStreamSynchronize(c->stream));
+        p.total = *(u64 *)c->h_scratch;
+        p.match = (u32 *)match.release();
+        p.pos = (u64 *)pos.release();
+    }
+    *out = &s0->n_plans.emplace(key, p).first->second;
+    return VB_OK;
+}
+
+// one side of the plan's grouped source, for join_n_expand_kernel / cogroup_n_gather_kernel
+static CogroupNSides semi_side(const vb_shuf *g, u32 rid)
+{
+    CogroupNSides a{};
+    a.n = 1;
+    a.keys[0] = g->res_keys; a.offs[0] = g->res_offs; a.vals[0] = g->res_vals;
+    a.kb[0] = (u32)g->bucket_off[rid];
+    return a;
+}
+
+static int semi_write(vb_shuf *const *sides, u32 n, u32 rid, u32 required, u32 excluded, void *out_k, void *out_v, int dst_loc)
+{
+    vb_shuf *s0 = sides[0];
+    vb_ctx *c = s0->ctx;
+    CogroupNPlan *p = nullptr;
+    vb_shuf *g = nullptr;
+    TRY(semi_plan(sides, n, rid, required, excluded, &p, &g));
+    const u64 total = p->total;
+    int rc = [&]() -> int {
+        if (!total) return VB_OK;
+        if (!out_k || !out_v) return set_err(VB_ERR_INVALID, "NULL output with %llu rows to write", (unsigned long long)total);
+        JoinNOut o{};
+        o.k = (u64 *)out_k; o.v[0] = (u64 *)out_v;
+        DevBuf bk(c), bv(c);
+        if (dst_loc == VB_HOST) {
+            TRY(bk.alloc(total * 8)); TRY(bv.alloc(total * 8));
+            o.k = bk.as<u64>(); o.v[0] = bv.as<u64>();
+        }
+        {
+            KLaunch kl(s0, K_JOIN, total);
+            const u64 blocks = std::min<u64>((total + 255) / 256, (u64)c->sm_count * 8);
+            join_n_expand_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(semi_side(g, rid), p->pos, (u32)p->n_keys, total, p->match, o);
+            TRY(kl.done("join_n_expand_kernel"));
+        }
+        if (dst_loc == VB_HOST) {
+            TRY(copy_out(s0, out_k, o.k, total * 8, VB_HOST));
+            TRY(copy_out(s0, out_v, o.v[0], total * 8, VB_HOST));
+        }
+        return VB_OK;
+    }();
+    cudaStreamSynchronize(c->stream);
+    drop_cogroup_n_plan(sides, n, rid, semi_kind(required, excluded));
+    return rc;
+}
+
+extern "C" int32_t vb_semi_join_n_size(vb_shuf *const *sides, uint32_t n_sides, uint32_t rid, uint32_t required,
+                                       uint32_t excluded, uint64_t *n_rows)
+{
+    TRY(cogroup_n_check(sides, n_sides, rid));
+    TRY(semi_masks_check(n_sides, required, excluded));
+    if (!n_rows) return set_err(VB_ERR_INVALID, "n_rows is NULL");
+    vb_ctx *c = sides[0]->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    CogroupNPlan *p = nullptr;
+    vb_shuf *g = nullptr;
+    TRY(semi_plan(sides, n_sides, rid, required, excluded, &p, &g));
+    *n_rows = p->total;
+    return VB_OK;
+}
+
+extern "C" int32_t vb_semi_join_n(vb_shuf *const *sides, uint32_t n_sides, uint32_t rid, uint32_t required, uint32_t excluded,
+                                  void *out_k, void *out_v, int32_t dst_loc)
+{
+    TRY(cogroup_n_check(sides, n_sides, rid));
+    TRY(semi_masks_check(n_sides, required, excluded));
+    if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
+    vb_ctx *c = sides[0]->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    return semi_write(sides, n_sides, rid, required, excluded, out_k, out_v, dst_loc);
+}
+
 extern "C" int32_t vb_cogroup_size(vb_shuf *l, vb_shuf *r, uint32_t rid, uint64_t *n_keys, uint64_t *n_left_vals,
                                    uint64_t *n_right_vals)
 {
@@ -7687,6 +7947,69 @@ extern "C" int32_t vb_join_n_str(vb_shuf *const *sides, uint32_t n_sides, uint32
                               out_row_offsets);
 }
 
+// vb_semi_join_n over string sides: side 0's keys of the partition probed against each filter side's key index (by the
+// full hash, then the bytes); the kept keys written once, from side 0, with their row offsets, and side 0's lists as rows
+extern "C" int32_t vb_semi_join_n_str_size(vb_shuf *const *sides, uint32_t n_sides, uint32_t rid, uint32_t required,
+                                           uint32_t excluded, uint64_t *n_rows, uint64_t *n_keys, uint64_t *n_key_bytes)
+{
+    TRY(cogroup_n_str_check(sides, n_sides, rid));
+    TRY(semi_masks_check(n_sides, required, excluded));
+    vb_ctx *c = sides[0]->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    for (u32 j = 0; j < n_sides; ++j) TRY(str_key_index(sides[j]));
+    CogroupNPlan *p = nullptr;
+    vb_shuf *g = nullptr;
+    TRY(semi_plan(sides, n_sides, rid, required, excluded, &p, &g));
+    TRY(str_plan_keys(sides, 1, rid, semi_kind(required, excluded), p));
+    if (n_rows) *n_rows = p->total;
+    if (n_keys) *n_keys = p->str_nk;
+    if (n_key_bytes) *n_key_bytes = p->str_nkb;
+    return VB_OK;
+}
+
+extern "C" int32_t vb_semi_join_n_str(vb_shuf *const *sides, uint32_t n_sides, uint32_t rid, uint32_t required, uint32_t excluded,
+                                      uint64_t *out_key_offsets, void *out_key_bytes, uint64_t *out_row_offsets, void *out_vals,
+                                      int32_t dst_loc)
+{
+    TRY(cogroup_n_str_check(sides, n_sides, rid));
+    TRY(semi_masks_check(n_sides, required, excluded));
+    if (dst_loc != VB_HOST && dst_loc != VB_DEVICE) return set_err(VB_ERR_INVALID, "bad dst_loc");
+    vb_shuf *s0 = sides[0];
+    vb_ctx *c = s0->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    for (u32 j = 0; j < n_sides; ++j) TRY(str_key_index(sides[j]));
+    const i64 kind = semi_kind(required, excluded);
+    CogroupNPlan *p = nullptr;
+    vb_shuf *g = nullptr;
+    TRY(semi_plan(sides, n_sides, rid, required, excluded, &p, &g));
+    int rc = [&]() -> int {
+        TRY(str_plan_keys(sides, 1, rid, kind, p));      // one-side plan: every key's bytes come from side 0
+        const u64 total = p->total;
+        if (total && (!out_vals || !out_key_offsets || !out_row_offsets || (p->str_nkb && !out_key_bytes)))
+            return set_err(VB_ERR_INVALID, "NULL output with %llu rows to write", (unsigned long long)total);
+        if (total) {
+            DevBuf tmp(c);
+            u64 *d = (u64 *)out_vals;
+            if (dst_loc == VB_HOST) { TRY(tmp.alloc(total * 8)); d = tmp.as<u64>(); }
+            {
+                KLaunch kl(s0, K_JOIN, total);
+                const u64 blocks = std::min<u64>((total + 255) / 256, (u64)c->sm_count * 8);
+                cogroup_n_gather_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(p->pos, (u32)p->n_keys, p->match, 1, 0, g->res_offs,
+                                                                                g->res_vals, d);
+                TRY(kl.done("cogroup_n_gather_kernel"));
+            }
+            if (dst_loc == VB_HOST) TRY(copy_out(s0, out_vals, d, total * 8, VB_HOST));
+        }
+        TRY(str_write_keys(sides, 1, rid, kind, p, out_key_offsets, out_key_bytes, dst_loc));
+        return copy_out(s0, out_row_offsets, p->str_roff, (p->str_nk + 1) * 8, dst_loc);
+    }();
+    cudaStreamSynchronize(c->stream);
+    drop_cogroup_n_plan(sides, n_sides, rid, kind);
+    return rc;
+}
+
 extern "C" uint64_t vb_hash_str(const void *bytes, uint64_t len) { return metro64_1_str((const unsigned char *)bytes, len); }
 
 extern "C" uint32_t vb_get_partition_str(const void *bytes, uint64_t len, uint32_t n_reduce)
@@ -7726,6 +8049,7 @@ extern "C" int32_t vb_shuffle_free(vb_shuf *s)
         dev_free(c, s->dict); dev_free(c, s->dense_of_slot);
         for (auto &kv : s->join_plans) { dev_free(c, kv.second.pos); dev_free(c, kv.second.match); }
         for (auto &kv : s->n_plans) free_cogroup_n_plan(c, kv.second);
+        for (auto &kv : s->semi) { dev_free(c, kv.second.tab); dev_free(c, kv.second.mask); }
         free_lazy_rows(s);
         free_str(s);
         free_rep(s);
@@ -7735,6 +8059,7 @@ extern "C" int32_t vb_shuffle_free(vb_shuf *s)
     }
     for (auto &kv : s->filtered) { vb_shuffle_free(kv.second.first); vb_shuffle_free(kv.second.second); }
     for (vb_shuf *t : s->trash) vb_shuffle_free(t);
+    for (auto &kv : s->semi) vb_shuffle_free(kv.second.kept);
     delete s;
     return VB_OK;
 }

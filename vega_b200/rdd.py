@@ -630,6 +630,17 @@ class _AggregatedParent(_Base):
     def cogroup(self, other, num_splits):
         return JoinedRdd(self, other, num_splits)
 
+    def subtract_by_key(self, other, num_splits, sort_values=False):
+        """PairRdd.subtract_by_key with this result as the filtered side: under the same num_splits it is read through
+        a view, without a second shuffle."""
+        cls = StrCoGroupedRdd if isinstance(self, StrShuffledRdd) else CoGroupedRdd
+        return SemiJoinedRdd(cls([self, other], num_splits, sort_values=sort_values), 0, 0b10)
+
+    def semi_join(self, other, num_splits, sort_values=False):
+        """PairRdd.semi_join with this result as the filtered side (see subtract_by_key)."""
+        cls = StrCoGroupedRdd if isinstance(self, StrShuffledRdd) else CoGroupedRdd
+        return SemiJoinedRdd(cls([self, other], num_splits, sort_values=sort_values), 0b10, 0)
+
     def _cogroup_side(self, num_splits):
         """The sealed COGROUP-kind shuffle a cogroup over num_splits partitions reads for this parent."""
         sh = self._run()
@@ -941,6 +952,38 @@ class CoGroupedRdd(_Base):
             mask |= 1 << int(j)
         return mask
 
+    def _semi_masks(self, required, excluded):
+        """(required, excluded) of a semi join as bitmasks over parents 1..n-1 (ValueError for parent 0 or a parent in
+        both)."""
+        req, exc = self._required_mask(required), self._required_mask(excluded)
+        if (req | exc) & 1:
+            raise ValueError("parent 0 is the parent filtered: it can be neither required nor excluded")
+        if req & exc:
+            raise ValueError(f"parents {req & exc:#x} are both required and excluded")
+        return req, exc
+
+    def semi_join_compute(self, split, required, excluded=0):
+        """Partition `split` of the semi / anti join of parent 0 (vb_semi_join_n): (keys, values), one key per row.  A
+        key of parent 0 is kept when every parent of `required` has it and no parent of `excluded` does, and gives its
+        parent-0 rows in that parent's list order.  Both masks are bitmasks or iterables of parent indices, over parents
+        1..n-1; the other parents' values are never read.  vega has no such op (Spark's subtractByKey: excluded = [1];
+        left semi join: required = [1])."""
+        req, exc = self._semi_masks(required, excluded)
+        shs, sides = self._sides()
+        n, lib = len(shs), self.sc._lib
+        nn = ctypes.c_uint64()
+        L.check(lib.vb_semi_join_n_size(sides, n, split, req, exc, ctypes.byref(nn)))
+        k = np.empty(nn.value, dtype=_NP_OF[shs[0].kcode])
+        v = np.empty(nn.value, dtype=_NP_OF[shs[0].vcode])
+        L.check(lib.vb_semi_join_n(sides, n, split, req, exc, k.ctypes.data_as(ctypes.c_void_p), v.ctypes.data_as(ctypes.c_void_p),
+                                   L.VB_HOST))
+        return k, _vals_out(shs[0], v)
+
+    def semi_join_collect(self, required, excluded=0):
+        req, exc = self._semi_masks(required, excluded)
+        parts = [self.semi_join_compute(r, req, exc) for r in range(self.num_slices)]
+        return np.concatenate([p[0] for p in parts]), np.concatenate([p[1] for p in parts])
+
     def outer_join_compute(self, split, required):
         """Partition `split` of the outer join of all parents (vb_join_n_outer): (k, [v_0, ..., v_{n-1}]).  A key is
         kept if every required parent has it; an optional parent that lacks it gives one None slot, so the key gives
@@ -965,6 +1008,25 @@ class CoGroupedRdd(_Base):
         parts = [self.outer_join_compute(r, mask) for r in range(self.num_slices)]
         cat = lambda xs: np.ma.concatenate(xs) if isinstance(xs[0], np.ma.MaskedArray) else np.concatenate(xs)
         return np.concatenate([p[0] for p in parts]), [cat([p[1][j] for p in parts]) for j in range(len(self.rdds))]
+
+
+class SemiJoinedRdd(_Base):
+    """subtract_by_key / semi_join (Spark's subtractByKey and left semi join; vega has neither): the (k, v) rows of the
+    first parent whose key the other parent lacks, or has.  Computed on the device by vb_semi_join_n(_str) over the
+    cogroup of the two parents, with no cross product and without grouping the other parent; only the first parent's
+    values are read.  compute(r) -> (keys, values), one key per row, a key's rows in its list order (ascending with
+    sort_values=True); collect() -> the same over every partition in order.  String keys come back as str or bytes."""
+
+    def __init__(self, cogrouped, required, excluded):
+        self.cogrouped = cogrouped
+        self.required, self.excluded = cogrouped._semi_masks(required, excluded)
+        self.sc, self.num_slices = cogrouped.sc, cogrouped.num_slices
+
+    def compute(self, split):
+        return self.cogrouped.semi_join_compute(split, self.required, self.excluded)
+
+    def collect(self):
+        return self.cogrouped.semi_join_collect(self.required, self.excluded)
 
 
 def _combine_spec(aggs, cols, num_splits):
@@ -1259,6 +1321,16 @@ class PairRdd(_Base):
 
     def cogroup(self, other, num_splits, sort_values=False):
         return JoinedRdd(self, other, num_splits, sort_values=sort_values)
+
+    def subtract_by_key(self, other, num_splits, sort_values=False):
+        """Spark's subtractByKey (vega has none): this PairRdd's (k, v) rows whose key `other` lacks.  other: a PairRdd
+        or a reduce result of the same key type; its values are never read (SemiJoinedRdd)."""
+        return SemiJoinedRdd(CoGroupedRdd([self, other], num_splits, sort_values=sort_values), 0, 0b10)
+
+    def semi_join(self, other, num_splits, sort_values=False):
+        """Left semi join (vega has none): this PairRdd's (k, v) rows whose key `other` has, each row once however many
+        values `other` has for the key (SemiJoinedRdd)."""
+        return SemiJoinedRdd(CoGroupedRdd([self, other], num_splits, sort_values=sort_values), 0b10, 0)
 
     def sort_by_key(self, num_splits):
         return ShuffledRdd(self, "sort", num_splits)
@@ -2003,6 +2075,15 @@ class StrPairRdd(PairRdd):
             raise NotImplementedError("repartition of String-key items with byte-string or several value columns")
         return _repartition(self, num_partitions, shuffle, starts, self.cols, _BytesCol(self.keys.owner), bytes_first=True)
 
+    def subtract_by_key(self, other, num_splits, sort_values=False):
+        """PairRdd.subtract_by_key over `String` keys, matched by their bytes: other is a StrPairRdd, a String reduce
+        result or a StrCombinedRdd aggregate of the same key kind."""
+        return SemiJoinedRdd(StrCoGroupedRdd([self, other], num_splits, sort_values=sort_values), 0, 0b10)
+
+    def semi_join(self, other, num_splits, sort_values=False):
+        """PairRdd.semi_join over `String` keys (see subtract_by_key)."""
+        return SemiJoinedRdd(StrCoGroupedRdd([self, other], num_splits, sort_values=sort_values), 0b10, 0)
+
     join = _no_str("join")
     left_outer_join = _no_str("left_outer_join")
     right_outer_join = _no_str("right_outer_join")
@@ -2218,6 +2299,34 @@ class StrCoGroupedRdd(_Base):
         parts = [self.outer_join_compute(r, mask) for r in range(self.num_slices)]
         cat = lambda xs: np.ma.concatenate(xs) if isinstance(xs[0], np.ma.MaskedArray) else np.concatenate(xs)
         return np.concatenate([p[0] for p in parts]), [cat([p[1][j] for p in parts]) for j in range(len(self.rdds))]
+
+    _semi_masks = CoGroupedRdd._semi_masks
+
+    def semi_join_raw(self, split, required, excluded=0):
+        """Partition `split` of the semi / anti join of parent 0 (vb_semi_join_n_str) in the keyed form: (key offsets,
+        key bytes, row offsets, values), each kept key once with its rows [row_offsets[i], row_offsets[i + 1])."""
+        req, exc = self._semi_masks(required, excluded)
+        shs, sides = self._sides()
+        n, lib = len(shs), self.sc._lib
+        nr, nk, nb = ctypes.c_uint64(), ctypes.c_uint64(), ctypes.c_uint64()
+        L.check(lib.vb_semi_join_n_str_size(sides, n, split, req, exc, ctypes.byref(nr), ctypes.byref(nk), ctypes.byref(nb)))
+        ko, kb = np.empty(nk.value + 1, dtype=np.uint64), np.empty(nb.value, dtype=np.uint8)
+        ro = np.empty(nk.value + 1, dtype=np.uint64)
+        v = np.empty(nr.value, dtype=_NP_OF[shs[0].vcode])
+        p = lambda x: x.ctypes.data_as(ctypes.c_void_p)
+        L.check(lib.vb_semi_join_n_str(sides, n, split, req, exc, p(ko), p(kb), p(ro), p(v), L.VB_HOST))
+        return ko, kb, ro, _vals_out(shs[0], v)
+
+    def semi_join_compute(self, split, required, excluded=0):
+        """CoGroupedRdd.semi_join_compute over `String` keys: (keys, values), one key per row."""
+        ko, kb, ro, v = self.semi_join_raw(split, required, excluded)
+        keys = _decode_keys(ko, kb, self.key_kind)
+        return (np.repeat(keys, np.diff(ro.astype(np.int64))) if len(keys) else np.empty(0, dtype=object)), v
+
+    def semi_join_collect(self, required, excluded=0):
+        req, exc = self._semi_masks(required, excluded)
+        parts = [self.semi_join_compute(r, req, exc) for r in range(self.num_slices)]
+        return np.concatenate([p[0] for p in parts]), np.concatenate([p[1] for p in parts])
 
     def join_compute(self, split):
         """Partition `split` of the inner join of all parents: (k, [v_0, ..., v_{n-1}])."""
